@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- headline benchmark of the PermutoSDF hot path on B200 (contract: see DESIGN.md "Measurement").
+"""bench.py -- headline benchmark of the PermutoSDF hot path on an H100 (contract: see DESIGN.md "Measurement").
 
   python bench.py --gpus N --steps K --warmup W            our arm (CUDA kernels through the C ABI)
   python bench.py --impl reference --gpus N --steps K ...  reference arm: the CPU (PyTorch-only) restatement of the
@@ -12,6 +12,9 @@ Lipschitz RGB MLP, 256^3 occupancy grid of the analytic sphere SDF |x|-0.3. A st
 importance resampling, forward, losses, backward through the double backward, dense AdamW.
   python bench.py --rays 8192 ...                          same step with more rays per GPU (BASELINE config 4 = 8192 rays/GPU x 8 GPUs)
   python bench.py --workload sphere_trace [--gpus N]       sphere-traced render of one 1920x1080 frame (BASELINE config 5): px/s
+  python bench.py ... --dump-outputs DIR                   after the timed steps, write what the last timed step computed as DIR/*.npy
+                                                           (train: its loss and the updated parameters, large tables as a fixed seeded
+                                                           sample; sphere_trace: the frame), so that two builds can be compared
 
 Metric: rays/s (whole job). `value`: inputs resident on the device. `e2e`: per step the ray indices come from pinned
 host memory and the loss is read back. Multi-GPU: rays sharded by rank (weak scaling), one NCCL all-reduce of the
@@ -42,7 +45,7 @@ def peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return d["hbm_gbs"], "measured (MEASURED_PEAKS.json)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (HBM3), not measured"
 
 
 class ClockSampler:
@@ -174,8 +177,10 @@ def run_ours(args):
     hp.nr_samples_imp_sampling = 16
     NR_RAYS = int(args.rays)
     hp.nr_rays = NR_RAYS
+    # deterministic mode: the timed steps compute the same bits in every run with the same arguments (--dump-outputs can be compared)
     tr = Trainer(hp, nr_levels=16, capacity=2 ** 18, sdf_hidden=64, nr_images=8, occupancy_resolution=256, seed=0,
-                 fused_inference=not args.modular, fused_training=not args.modular, optimizer="adamw" if args.modular else "fused")
+                 fused_inference=not args.modular, fused_training=not args.modular, optimizer="adamw" if args.modular else "fused",
+                 deterministic=True)
     tr.set_analytic_scene()
     tr.iter_nr = 20000          # past coarse-to-fine: all 16 levels active, cos-anneal half way
     graphed = not (args.modular or args.eager)
@@ -201,6 +206,8 @@ def run_ours(args):
         # captured in the optimizer graph; nccl_overlap: bucketed all-reduce overlapped with the SDF backward / AdamW
         tr.enable_data_parallel(world, overlap=(dp_mode == "nccl_overlap"), mode="peer" if dp_mode == "peer" else "nccl")
 
+    last = {}
+
     def one_step(i, e2e):
         # e2e: the step's inputs start in pinned host memory; otherwise they are device resident
         pix, img = (pix_host[i], img_host[i]) if e2e else (pix_dev[i], img_dev[i])
@@ -216,7 +223,8 @@ def run_ours(args):
             dist.all_reduce(tr.optimizer.flat_grad if flat is None else flat.flat, op=dist.ReduceOp.SUM)
             tr.optimizer_step(grad_scale=1.0 / world)
         if e2e:
-            return float(loss)          # device -> host read of the step's result
+            loss = float(loss)          # device -> host read of the step's result
+        last["loss"] = loss
         return loss
 
     if graphed:
@@ -257,6 +265,15 @@ def run_ours(args):
         return float(t.item()), launches, times, cs.summary(), nsamples / steps
 
     ms_dev, launches, ktimes, clocks, avg_samples = timed(e2e=False, with_events=not graphed)
+    if args.dump_outputs and rank == 0:
+        # the last step of the timed region behind `value`: its loss and the parameters it left (what the caller of the training step
+        # holds afterwards; deterministic mode, so two runs with the same arguments write the same bits)
+        torch.cuda.synchronize()
+        arrays = {"loss": torch.tensor([float(last["loss"])])}
+        for prefix, model in (("sdf", tr.model_sdf), ("rgb", tr.model_rgb), ("colorcal", tr.model_colorcal)):
+            if model is not None:
+                arrays.update({"%s.%s" % (prefix, k): v for k, v in model.named_parameters()})
+        dump_outputs(args.dump_outputs, arrays)
     ms_e2e, _, _, clocks2, _ = timed(e2e=True, with_events=False)
     ms_per_step = ms_dev / args.steps
     prof_steps = 0
@@ -292,8 +309,6 @@ def run_ours(args):
         "psdf_rgb_fused_backward_acc": 12 + 2 * L * 4 * 8 + 12 + 12 + 128 + 12 + 12 + 128,
     }
     units = dict(_lib.LAST_UNITS)
-    # dram__bytes_read.sum + dram__bytes_write.sum per launch from the tracked `ncu --set full` capture of this workload
-    ncu_traffic = ncu_traffic_from_profiles()
     roof = None
     if ktimes:
         top = sorted(((v[1], k) for k, v in ktimes.items()), reverse=True)
@@ -304,7 +319,7 @@ def run_ours(args):
         nsamp = units.get(name, 0) * (args.steps / prof_steps if prof_steps else 1.0)
         ach = (alg_bytes[name] * nsamp / (tot_ms / 1e3) / 1e9) if name in alg_bytes and nsamp else None
         roof = {"kernel": name, "bound": "hbm", "achieved": ach, "peak": hbm, "unit": "GB/s", "frac": (ach / hbm) if ach else None,
-                "traffic": ncu_traffic.get(name), "launches": n, "avg_us": per_launch_s * 1e6, "samples_per_launch": nsamp / n if n else None,
+                "launches": n, "avg_us": per_launch_s * 1e6, "samples_per_launch": nsamp / n if n else None,
                 "peak_source": peak_src,
                 "share_of_step": tot_ms / ms_dev,
                 "top5_ms_per_step": {k: round(v / args.steps, 4) for v, k in top[:5]},
@@ -319,8 +334,9 @@ def run_ours(args):
             "data": "synthetic", "impl": "ours",
             "config": {"workload": WORKLOAD if NR_RAYS == 512 else WORKLOAD.replace("512 rays", "%d rays" % NR_RAYS).replace("C2:", "C2 shape at %d rays/GPU (BASELINE config 4 when 8192 x 8 GPUs):" % NR_RAYS),
                        "rays_per_gpu": NR_RAYS, "avg_samples_per_step": avg_samples, "parallelism": "dp%d" % world, "gradient_exchange": (dp_mode if world > 1 else None),
-                       "l2": "per-step working set (2 lattice tables + grads + Adam moments ~0.4 GB) exceeds the 126 MB L2; no explicit flush",
+                       "l2": "per-step working set (2 lattice tables + grads + Adam moments ~0.4 GB) exceeds the 50 MB L2; no explicit flush",
                        "timed_region": "sum of per-step CUDA-event intervals",
+                       "reductions": "deterministic (fixed-point gradient sums, Trainer(deterministic=True))",
                        "execution": "eager" if (args.modular or args.eager) else "CUDA graphs (forward+backward graph, optimizer graph), static-capacity containers"},
             "e2e": {"value": e2e_value, "unit": "rays/s", "ms_per_step": ms_e2e / args.steps, "h2d_bytes_per_step": NR_RAYS * 4 * 2 * world,
                     "d2h_bytes_per_step": 4 * world},
@@ -354,7 +370,8 @@ def run_sphere_trace(args):
     assert load_library().psdf_device_ok() == 1
     W, H = args.width, args.height
     hp = HyperParams()
-    tr = Trainer(hp, nr_levels=16, capacity=2 ** 18, sdf_hidden=64, nr_images=8, occupancy_resolution=256, seed=0, optimizer="fused")
+    tr = Trainer(hp, nr_levels=16, capacity=2 ** 18, sdf_hidden=64, nr_images=8, occupancy_resolution=256, seed=0, optimizer="fused",
+                 deterministic=True)
     tr.set_analytic_scene()
     m = tr.model_sdf
     # fit the SDF to the analytic sphere of the scene (the reference's sphere initialisation, train_permuto_sdf.py:262-291): rays then
@@ -396,6 +413,7 @@ def run_sphere_trace(args):
             img = rgb
         if e2e:
             img_host.view(-1, 3).copy_(img, non_blocking=True)
+        last["img"] = img
         return img
 
     def timed(e2e, with_events):
@@ -425,7 +443,11 @@ def run_sphere_trace(args):
             dist.all_reduce(t, op=dist.ReduceOp.MAX)
         return float(t.item()), launches, times, cs.summary()
 
+    last = {}
     ms_dev, launches, _, clocks = timed(False, False)
+    if args.dump_outputs and rank == 0:
+        torch.cuda.synchronize()
+        dump_outputs(args.dump_outputs, {"image": last["img"].reshape(H, W, 3)})       # the frame of the last step behind `value`
     ms_e2e, _, _, _ = timed(True, False)
     _, _, ktimes, _ = timed(False, True)               # per-kernel CUDA-event times (serialising events: outside the reported time)
     hbm, peak_src = peaks()
@@ -437,7 +459,7 @@ def run_sphere_trace(args):
         alg = 12 + 16 * 4 * 8                      # per network evaluation: position + 16 levels x 4 vertices x 8 B (SURVEY.md 8d, fused: no feature write)
         ach = alg * evals_per_launch * n / (tot_ms / 1e3) / 1e9
         top = sorted(((v[1], k) for k, v in ktimes.items()), reverse=True)
-        roof = {"kernel": name, "bound": "hbm", "achieved": ach, "peak": hbm, "unit": "GB/s", "frac": ach / hbm, "traffic": ncu_traffic_from_profiles().get(name),
+        roof = {"kernel": name, "bound": "hbm", "achieved": ach, "peak": hbm, "unit": "GB/s", "frac": ach / hbm,
                 "launches": n, "avg_us": tot_ms / n * 1e3, "network_evaluations_per_launch": evals_per_launch, "peak_source": peak_src,
                 "share_of_step": tot_ms / n / (ms_dev / args.steps), "top5_ms_per_step": {k: round(v / args.steps, 4) for v, k in top[:5]}}
     if rank == 0:
@@ -448,7 +470,7 @@ def run_sphere_trace(args):
                "data": "synthetic", "impl": "ours",
                "config": {"workload": "C5: sphere-trace inference %dx%d, %d max steps, OccupancyGrid 256^3 on, 16-level lattice 2^18x2, 3x64 SDF MLP fitted "
                                       "to the analytic sphere, RGB Lipschitz MLP; image tiled by rows over the ranks + one all_gather" % (W, H, args.trace_iters),
-                          "parallelism": "tiles%d" % world, "l2": "lattice table 33.5 MB + 16.8 MB occupancy are L2 resident by design; no flush",
+                          "parallelism": "tiles%d" % world, "l2": "lattice table 33.5 MB + 16.8 MB occupancy, about the 50 MB L2; no flush",
                           "timed_region": "sum of per-frame CUDA-event intervals"},
                "e2e": {"value": px / (ms_e2e / 1e3), "unit": "px/s", "ms_per_step": ms_e2e / args.steps, "h2d_bytes_per_step": 24 * world,
                        "d2h_bytes_per_step": W * H * 3 * 4},
@@ -461,32 +483,20 @@ def run_sphere_trace(args):
         dist.destroy_process_group()
 
 
-NCU_KERNEL_OF = {"psdf_sdf_fused_forward": "k_sdf_fused_dual", "psdf_sdf_fused_backward": "k_sdf_fused_backward",
-                 "psdf_sdf_fused_forward_multi": "k_sdf_fused_dual", "psdf_sdf_fused_backward_multi": "k_sdf_fused_backward",
-                 "psdf_rgb_fused_forward": "k_rgb_fused", "psdf_rgb_fused_backward": "k_rgb_fused_backward",
-                 "psdf_rgb_fused_backward_acc": "k_rgb_fused_backward",
-                 "psdf_sdf_sphere_trace": "k_sdf_sphere_trace"}
+DUMP_SAMPLE = 1 << 18        # entries kept of a larger parameter tensor by --dump-outputs (fixed seeded sample)
 
 
-def ncu_traffic_from_profiles():
-    """entry point -> DRAM bytes (read + write) per launch, read from the newest tracked profiles/r*_ncu_kernels.csv (65 536-sample
-    launches of the bench workload). None for kernels the capture does not hold."""
-    import csv
-    import glob
-    files = sorted(glob.glob(os.path.join(ROOT, "profiles", "r*_ncu_kernels.csv")))
-    out = {}
-    if not files:
-        return out
-    rows = list(csv.DictReader(open(files[-1])))
-    for entry, kern in NCU_KERNEL_OF.items():
-        for r in rows:
-            if r.get("kernel", "").startswith(kern):
-                try:
-                    out[entry] = (float(r["dram__bytes_read.sum [Mbyte]"]) + float(r["dram__bytes_write.sum [Mbyte]"])) * 1e6
-                except (KeyError, ValueError):
-                    pass
-                break
-    return out
+def dump_outputs(out_dir, arrays):
+    """name -> tensor: DIR/<name>.npy as float32. Tensors above DUMP_SAMPLE entries are reduced to the same seeded sample of flat indices
+    on every run (the sample's indices are written beside it)."""
+    os.makedirs(out_dir, exist_ok=True)
+    for name, t in arrays.items():
+        a = t.detach().float().reshape(-1).cpu().numpy() if isinstance(t, torch.Tensor) else np.asarray(t, dtype=np.float32).reshape(-1)
+        if a.size > DUMP_SAMPLE:
+            idx = np.sort(np.random.default_rng(0).choice(a.size, DUMP_SAMPLE, replace=False))
+            np.save(os.path.join(out_dir, name + ".sample_index.npy"), idx.astype(np.float64))
+            a = a[idx]
+        np.save(os.path.join(out_dir, name + ".npy"), a.astype(np.float32))
 
 
 def cpu_baseline(sample_rays, steps, warmup, threads=None):
@@ -525,12 +535,14 @@ def main():
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--eager", action="store_true", help="launch every kernel from Python (no CUDA-graph replay)")
-    ap.add_argument("--modular", action="store_true", help="drop-in API path only (encoding kernels + torch MLP), no fused tcgen05 kernels")
+    ap.add_argument("--modular", action="store_true", help="drop-in API path only (encoding kernels + torch MLP), no fused MLP kernels")
     ap.add_argument("--rays", type=int, default=512, help="rays per GPU and step (512 = BASELINE config 2, 8192 = config 4 per GPU)")
     ap.add_argument("--workload", default="train", choices=["train", "sphere_trace"])
     ap.add_argument("--width", type=int, default=1920)
     ap.add_argument("--height", type=int, default=1080)
     ap.add_argument("--trace_iters", type=int, default=256)
+    ap.add_argument("--dump-outputs", dest="dump_outputs", default=None, metavar="DIR",
+                    help="write the outputs of the last timed step to DIR/<name>.npy (float32, at most 64 MB)")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3) if args.impl == "ours" else args.warmup
     if args.impl == "reference":

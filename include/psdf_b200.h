@@ -1,5 +1,5 @@
 /*
- * psdf_b200.h -- C ABI of libpsdf_b200.so, the sm_100a (B200) implementation of PermutoSDF's per-ray
+ * psdf_b200.h -- C ABI of libpsdf_b200.so, the sm_90a (H100) implementation of PermutoSDF's per-ray
  * training / sphere-tracing hot path.
  *
  * Boundary: the reference exposes this path to Python as a pybind11 module `permuto_sdf`
@@ -35,8 +35,17 @@ extern "C" {
 #define PSDF_ERR_UNSUPPORTED_ -3
 
 int psdf_abi_version(void);
-/* 1 when the library was built for sm_100a and a CUDA device is present, else 0 (never a CPU fallback) */
+/* 1 when a compute-capability 9.x (H100, the library's sm_90a target) device is present, else 0 (never a CPU fallback) */
 int psdf_device_ok(void);
+/* Deterministic mode of the current device. Off (the default): gradient reductions use float atomics, so a training step's
+ * gradients differ from run to run in their last bits. On: the training path's reductions (fused SDF / colour backward, compositing
+ * backward, Lipschitz backward, loss terms) accumulate in 64-bit fixed point (2^-34 grid, |values| < 5.3e8) and a random occupancy
+ * update lets the last sample of a repeated voxel win, so runs with the same inputs give the same bits. lattice_entries = the
+ * largest L * T * F of a backward call, voxels = the largest occupancy grid (larger calls return PSDF_ERR_UNSUPPORTED). Allocates or
+ * frees device memory: call outside CUDA-graph capture with no launch of this library in flight.
+ * Launches of one fused kernel must not run concurrently on a device: each fused kernel keeps its accumulators in one per-device
+ * area (and, in deterministic mode, shares the fixed-point accumulators). */
+int psdf_set_deterministic(int on, long long lattice_entries, long long voxels);
 
 /* ---------------------------------------------------------------- Sphere (include/permuto_sdf/Sphere.cuh:12-24) */
 /* Sphere::ray_intersection, src/Sphere.cu:42-79 */
@@ -218,7 +227,7 @@ int psdf_enc_double_backward(int N, int D, int L, int F, int T, const float* pos
                              const float* shift, const float* window, int concat_points, float points_scaling,
                              const float* gg_pos, const float* grad_out, float* grad_lattice, float* grad_grad_out, void* stream);
 
-/* ---------------------------------------------------------------- fused encoding + SDF MLP (tcgen05)
+/* ---------------------------------------------------------------- fused encoding + SDF MLP (wgmma)
  * Replaces SDF.forward / SDF.get_sdf_and_gradient of permuto_sdf_py/models/models.py:176-259 for evaluations that
  * need no parameter gradients: importance sampling (sdf_utils.py:388,401), occupancy refresh
  * (train_permuto_sdf.py:388-391), sphere tracing (sdf_utils.py:166,199-204).
@@ -272,8 +281,8 @@ int psdf_rgb_fused_forward(int N, int L, int T, const float* pos, const float* d
  * weight gradients gW_l [N_l,K_l] (+=, wrt the normalised matrices) and bias gradients gb_l (+=). workspace:
  * psdf_rgb_fused_backward_workspace_bytes(N) bytes of scratch. */
 /* psdf_sdf_fused_backward over up to three independent sample sets in ONE launch (N_i = 0: unused set); every set has its own
- * positions and upstream gradients, the accumulated parameter gradients are shared. One launch of 1024 tiles loses 1 % to the last
- * partial wave on 148 SMs where two launches of 512 tiles lose 13 % each. */
+ * positions and upstream gradients, the accumulated parameter gradients are shared. The sets share one last partial wave instead
+ * of paying one each. */
 long long psdf_sdf_fused_backward_multi_workspace_bytes(int N0, int N1, int N2);
 int psdf_sdf_fused_backward_multi(int L, int T, const float* lattice, const float* scale_factor, const float* shift, const float* window,
                                   float points_scaling, int hidden, int out_dim, const uint8_t* blob, int N0, const float* pos0,

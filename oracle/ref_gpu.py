@@ -1,7 +1,7 @@
 """TEST INFRASTRUCTURE -- NOT PRODUCT CODE.
 
 Python front-end of oracle/_ref/libpsdf_ref_gpu.so: the UNMODIFIED reference CUDA kernels
-(/root/reference/kernels/permuto_sdf/*GPU.cuh, compiled for sm_100a by oracle/ref_shim/Makefile) launched
+(the original project's kernels/permuto_sdf/*GPU.cuh, compiled for sm_90a by oracle/ref_shim/Makefile) launched
 the way the reference host code does (src/*.cu): grid ceil(n/256) x 256 threads, same output initial
 values. Needs a GPU; used by the `-m gpu` parity tests, by tests/golden/make_ref_golden.py to produce
 reference-made fixtures, and by bench.py to time the reference kernels next to ours.

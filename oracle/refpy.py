@@ -1,7 +1,7 @@
 """TEST INFRASTRUCTURE -- NOT PRODUCT CODE.
 
 Runs the reference's own, UNMODIFIED Python (permuto_sdf_py/models/models.py, volume_rendering/*.py, utils/sdf_utils.py, ...) on the
-CPU, in this container, where /root/reference exists: `install()` puts CPU stand-ins for the two compiled modules the reference
+CPU, where a checkout of the original project is present (PERMUTO_SDF_REFERENCE, else /root/reference): `install()` puts CPU stand-ins for the two compiled modules the reference
 imports into sys.modules --
 
   permuto_sdf            (src/PyBridge.cxx)   -> classes over the C restatement oracle/rayops_oracle.c (pinned on reference-kernel goldens)
@@ -23,7 +23,7 @@ import torch
 from . import encoding_oracle as eo
 from . import rayops as ro
 
-REF_ROOT = "/root/reference"
+REF_ROOT = os.environ.get("PERMUTO_SDF_REFERENCE") or "/root/reference"
 
 
 # ================================================================================================ permutohedral_encoding (CPU)
@@ -244,7 +244,7 @@ class _Stub:
 def install(ref_root=REF_ROOT):
     """-> the imported reference module permuto_sdf_py.models.models"""
     if not os.path.isdir(ref_root):
-        raise RuntimeError("%s not present: the reference's Python only runs in the build container" % ref_root)
+        raise RuntimeError("%r is not a checkout of the original project: set PERMUTO_SDF_REFERENCE" % ref_root)
     if "permuto_sdf_py.models.models" in sys.modules:
         return sys.modules["permuto_sdf_py.models.models"]
     for name in ("easypbr", "dataloaders", "skimage", "skimage.measure", "matplotlib", "matplotlib.cm"):

@@ -1,11 +1,11 @@
-"""permuto_sdf_b200 -- B200-native (sm_100a) implementation of PermutoSDF's per-ray training and
+"""permuto_sdf_b200 -- H100-native (sm_90a) implementation of PermutoSDF's per-ray training and
 sphere-tracing hot path behind the reference's own Python operator API.
 
     permuto_sdf_b200.permuto_sdf              mirror of the pybind module `permuto_sdf` (src/PyBridge.cxx)
     permuto_sdf_b200.permutohedral_encoding   mirror of the external `permutohedral_encoding` package
     compat/                                   top-level `permuto_sdf` / `permutohedral_encoding` shims so the
                                               reference's permuto_sdf_py runs unchanged (see INTEGRATION.md)
-    permuto_sdf_b200.patch_reference_models   routes the reference's own SDF / RGB classes through the fused tcgen05 kernels
+    permuto_sdf_b200.patch_reference_models   routes the reference's own SDF / RGB classes through the fused tensor-core kernels
 
 All device work goes through the C ABI in include/psdf_b200.h (libpsdf_b200.so, hand-written CUDA).
 There is no CPU or PyTorch fallback: importing is cheap, but any op raises if the library is missing

@@ -70,7 +70,7 @@ def load_library(path=LIB_PATH):
         return _lib
     if not os.path.exists(path):
         raise RuntimeError(
-            "permuto_sdf_b200: %s not found. Build it with `python __graft_entry__.py` (nvcc, sm_100a). "
+            "permuto_sdf_b200: %s not found. Build it with `python __graft_entry__.py` (nvcc, sm_90a). "
             "There is no CPU or PyTorch fallback for this path." % path)
     lib = ctypes.CDLL(path)
     for name, (ret, args) in PROTOS.items():

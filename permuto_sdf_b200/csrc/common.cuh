@@ -1,6 +1,6 @@
-// Shared device helpers for the PermutoSDF B200 hot path.
+// Shared device helpers for the PermutoSDF H100 hot path.
 //
-// Everything in this header is written from scratch for sm_100a. Where a helper mirrors a
+// Everything in this header is written from scratch for sm_90a. Where a helper mirrors a
 // piece of reference arithmetic the reference location is cited so that parity can be audited:
 //   Morton code / voxel <-> position : kernels/permuto_sdf/OccupancyGridGPU.cuh:37-71,112-193
 //   DDA step                          : kernels/permuto_sdf/OccupancyGridGPU.cuh:95-109
@@ -8,7 +8,7 @@
 //
 // Floating point policy for the ray-path translation units (compiled with -fmad=false):
 // every fused multiply-add is written explicitly with __fmaf_rn at exactly the places where
-// nvcc 12.9 contracts the reference source for sm_100a (checked in the SASS of the reference
+// nvcc 12.9 contracts the reference source (checked in the SASS of the reference
 // kernels, see DESIGN.md "FMA map"), so integer decisions taken from floats (voxel index,
 // sample counts) are bit-identical to the reference CUDA path.
 #pragma once
@@ -280,12 +280,86 @@ __device__ __forceinline__ int occ_advance_resumable(const GridGeom& g, const ui
     }
     return ((double)steps < max_steps) ? 0 : 1;
 }
-// one-time (per device and kernel) opt-in to more than 48 KB of dynamic shared memory; `slot` is a static array owned by the call site
+// one AdamW element update (math: optim.cu). The roundings are explicit so that every kernel applying it (optim.cu k_adamw / k_adamw_dp,
+// iter_glue.cu k_adamw_multi) produces the same bits whatever the compiler would contract.
+__device__ __forceinline__ void adamw_update(float& p, float& m, float& v, float g, float grad_scale, float decay, float step_size, float beta1,
+                                             float beta2, float bias_c2_sqrt, float eps) {
+    const float gr = __fmul_rn(g, grad_scale);
+    const float pk = __fmul_rn(p, decay);
+    m = __fmaf_rn(beta1, m, __fmul_rn(1.0f - beta1, gr));
+    v = __fmaf_rn(beta2, v, __fmul_rn(__fmul_rn(1.0f - beta2, gr), gr));
+    const float denom = __fadd_rn(__fdiv_rn(sqrtf(v), bias_c2_sqrt), eps);
+    p = __fmaf_rn(-step_size, __fdiv_rn(m, denom), pk);
+}
+// ---------------------------------------------------------------- deterministic mode (opt-in)
+// Float atomics add in arrival order, so by default a gradient reduced over many threads differs from run to run in its last bits
+// (and a training step amplifies that: Adam with eps 1e-15 makes a whole learning-rate step of a near-zero gradient, sampling
+// decisions flip). psdf_set_deterministic(1, ...) switches the training path's reductions to 64-bit fixed point instead: every
+// contribution is rounded to the grid 2^-34 (resolution 5.8e-11; contributions and totals up to +-5.3e8) and the integers are added,
+// which is associative (and modular, so partial sums may wrap), so the totals are the same in every run; k_fx_flush then adds them to
+// the float gradients (+=) and clears the accumulators. The accumulators are allocated when the mode is switched on.
+constexpr double kFxScale = 17179869184.0;
+__device__ __forceinline__ unsigned long long fx_of(float v) { return (unsigned long long)__double2ll_rn((double)v * kFxScale); }
+__device__ __forceinline__ void fx_add(unsigned long long* acc, float v) { atomicAdd(acc, fx_of(v)); }
+constexpr int kDetImages = 1 << 16;                 // calibration images with fixed-point gradients (later images: float atomics)
+constexpr int kDetSdfW = 64 * 64, kDetRgbW = 128 * 128;
+struct DetBufs {
+    unsigned long long* sdf_lattice;   // [lattice_len]
+    unsigned long long* sdf_mlp;       // [4 x kDetSdfW weights | 4 x 64 biases]
+    unsigned long long* rgb_lattice;   // [lattice_len]
+    unsigned long long* rgb_mlp;       // [4 x kDetRgbW weights | 4 x 128 biases]
+    unsigned long long* neus;          // [3 kDetImages weight delta | 3 kDetImages bias | inv_s]
+    unsigned long long* lip;           // [4]
+    unsigned long long* loss;          // [5]
+    int* winner;                       // [voxels]: occupancy-update arbitration (rayops.cu)
+    long long lattice_len, voxels;
+};
+const DetBufs* det_buffers();        // of the current device; nullptr when the mode is off (optim.cu)
+constexpr int kFxMaxSegs = 12;
+struct FxSegs {
+    int n = 0;
+    unsigned long long* src[kFxMaxSegs];
+    float* dst[kFxMaxSegs];
+    long long len[kFxMaxSegs];
+    // accumulators src[0, len) -> destination dst[0, len); a destination entry is only touched where its accumulator is non-zero
+    void add(unsigned long long* s, float* d, long long l) {
+        if (d && l > 0 && n < kFxMaxSegs) { src[n] = s; dst[n] = d; len[n] = l; n++; }
+    }
+};
+static __global__ void __launch_bounds__(256) k_fx_flush(FxSegs S) {
+    const long long stride = (long long)gridDim.x * blockDim.x;
+    for (int s = 0; s < S.n; s++) {
+        unsigned long long* __restrict__ src = S.src[s];
+        float* __restrict__ dst = S.dst[s];
+        for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < S.len[s]; i += stride) {
+            const unsigned long long v = src[i];
+            if (v) { dst[i] += (float)((double)(long long)v / kFxScale); src[i] = 0ull; }
+        }
+    }
+}
+inline int fx_flush(const FxSegs& S, cudaStream_t stream) {
+    long long m = 0;
+    for (int s = 0; s < S.n; s++) m = S.len[s] > m ? S.len[s] : m;
+    if (m == 0) return 0;
+    int dev = 0, sms = 132;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+    const long long blocks = (m + 255) / 256, cap = 8LL * sms;
+    k_fx_flush<<<(unsigned)(blocks < cap ? blocks : cap), 256, 0, stream>>>(S);
+    return cudaGetLastError() == cudaSuccess ? 0 : -2;
+}
+// one-time (per device and kernel) opt-in to more than 48 KB of dynamic shared memory; `slot` is a static array owned by the call site.
+// The request is capped at what the device allows next to the kernel's static shared memory.
 template <typename K>
 inline void psdf_optin_smem(K kernel, int bytes, bool (&slot)[64]) {
     int dev = 0;
     cudaGetDevice(&dev);
     if (dev < 0 || dev >= 64 || !slot[dev]) {
+        int optin = bytes;
+        cudaFuncAttributes fa;
+        if (cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev) == cudaSuccess &&
+            cudaFuncGetAttributes(&fa, kernel) == cudaSuccess)
+            bytes = min(bytes, optin - (int)fa.sharedSizeBytes);
         cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
         if (dev >= 0 && dev < 64) slot[dev] = true;
     }

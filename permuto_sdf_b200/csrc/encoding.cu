@@ -1,4 +1,4 @@
-// Multi-resolution permutohedral-lattice hash encoding for sm_100a: forward (barycentric gather),
+// Multi-resolution permutohedral-lattice hash encoding for sm_90a: forward (barycentric gather),
 // backward to the lattice (warp-aggregated vector atomics), backward to positions, and the double
 // backward needed by the eikonal / curvature losses.
 //
@@ -9,10 +9,10 @@
 // residuals, barycentric weights by rank, hash the D-int key of each of the D+1 simplex vertices
 // (h = (h + key_i) * 2531011 over i, mod capacity), blend F features, multiply by the level window.
 //
-// B200 mapping. One thread per sample, all levels in that thread; a warp is 32 consecutive samples,
+// Mapping. One thread per sample, all levels in that thread; a warp is 32 consecutive samples,
 // i.e. neighbours on a ray, so on coarse levels the 32 lanes hit the same few 8-byte table rows (L1
 // broadcast) and on fine levels each lane has 4*UNROLL independent gathers in flight against the
-// L2-resident table (L*T*F*4 B = 33.5 MB at L=16 << 126 MB L2). Outputs are staged in shared memory
+// L2-resident table (L*T*F*4 B = 33.5 MB at L=16 < 50 MB L2). Outputs are staged in shared memory
 // and written as one contiguous [32, C] block per warp. The backward reduces duplicates inside the warp
 // (match_any + segmented shuffle tree) before issuing one red.global.add.v2.f32 per distinct vertex.
 // Position gradients need no atomics because a thread owns all levels of its sample.
@@ -538,7 +538,7 @@ int psdf_device_ok(void) {
     if (cudaGetDeviceCount(&n) != cudaSuccess || n <= 0) { cudaGetLastError(); return 0; }
     cudaDeviceProp prop;
     if (cudaGetDeviceProperties(&prop, 0) != cudaSuccess) return 0;
-    return prop.major == 10 ? 1 : 0;
+    return prop.major == 9 ? 1 : 0;
 }
 
 }  // extern "C"

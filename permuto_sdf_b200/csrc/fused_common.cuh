@@ -1,6 +1,6 @@
 // Shared pieces of the fused encoding + MLP kernels (fused_sdf.cu: forward / inference, fused_sdf_bwd.cu: training
 // backward): MLP operand-blob geometry, permutohedral simplex helpers for D = 3, GELU and its derivatives, operand
-// tile stores (bf16 hi/lo split in the UMMA core-matrix layout) and the split-product GEMM issue.
+// tile stores (bf16 hi/lo split in the core-matrix operand layout) and the split-product GEMM issue.
 #pragma once
 #include "common.cuh"
 #include "umma.cuh"
@@ -13,6 +13,9 @@ constexpr int kNL = 4;                 // linear layers of the SDF MLP
 constexpr int kATileBytes = 128 * 64 * 2;   // one bf16 operand tile [128 x 64]
 constexpr int kLBO = 128;
 constexpr int kSBO_A = 1024;           // 8 core matrices (K = 64) per 8-row group
+// Accumulator areas (umma.cuh) are sized for one persistent CTA per SM of an H100 SXM (132 SMs), or two for the kernels that run
+// two per SM; launches clamp their persistent grids to these counts.
+constexpr int kAccCtas = 132;
 
 struct MlpGeom {
     int K[kNL], N[kNL];        // true dims
@@ -49,7 +52,7 @@ inline MlpGeom make_geom(int in_dim, int hidden, int out_dim) {
     return make_geom_dims(dims);
 }
 
-// weights [N][K] fp32 (torch.nn.Linear layout) -> hi/lo bf16 in the UMMA K-major core-matrix layout + fp32 bias;
+// weights [N][K] fp32 (torch.nn.Linear layout) -> hi/lo bf16 in the K-major core-matrix operand layout + fp32 bias;
 // second half of the blob: the same weights transposed (rows = input features, K = output features) for the
 // backward GEMMs dA = dZ * W
 static __global__ void k_pack_mlp(MlpGeom g, const float* W0, const float* b0, const float* W1, const float* b1, const float* W2,
@@ -203,39 +206,25 @@ __device__ __forceinline__ void store8(uint8_t* a_hi, uint8_t* a_lo, int row, in
 }
 
 
-// issue the three split products of one [128 x Kp] x [Np x Kp]^T GEMM into TMEM (single thread).
-// Descriptor convention validated on B200 by tests/test_fused_gpu.py::test_umma_gemm_self_test: the first offset field
-// (LBO) is the stride between core matrices adjacent along K, the second (SBO) between 8-row groups.
-__device__ __forceinline__ void issue_gemm_rebuild(uint32_t tmem_d, const uint8_t* a_hi, const uint8_t* a_lo, const uint8_t* w_hi,
-                                           const uint8_t* w_lo, int Kp, int Np) {
-    const uint32_t idesc = umma::make_idesc(128, Np, umma::kFmtBF16);
-    const uint32_t sbo_w = (Kp / 8) * kLBO;
-    const uint32_t ah = umma::smem_u32(a_hi), al = umma::smem_u32(a_lo), wh = umma::smem_u32(w_hi), wl = umma::smem_u32(w_lo);
-    for (int kk = 0; kk < Kp / 16; kk++) {
-        uint32_t ko = kk * 2 * kLBO;      // 16 bf16 = 2 core matrices along K
-        uint64_t dah = umma::make_desc(ah + ko, kLBO, kSBO_A), dal = umma::make_desc(al + ko, kLBO, kSBO_A);
-        uint64_t dwh = umma::make_desc(wh + ko, kLBO, sbo_w), dwl = umma::make_desc(wl + ko, kLBO, sbo_w);
-        umma::mma_bf16(tmem_d, dah, dwh, idesc, kk > 0 ? 1u : 0u);
-        umma::mma_bf16(tmem_d, dah, dwl, idesc, 1u);
-        umma::mma_bf16(tmem_d, dal, dwh, idesc, 1u);
-    }
+// column halves of an N-column product in units of 16 columns (MMA N % 16 == 0); the second half may be empty
+__device__ __forceinline__ void split_n(int N, int half, int& n0, int& nn) {
+    const int na = ((N / 16 + 1) / 2) * 16;
+    n0 = half ? na : 0;
+    nn = half ? N - na : na;
 }
 
-
-// same products with the four descriptors built once and only their start-address field advanced per K step (fewer
-// instructions on the single issuing thread); this is the variant the kernels use, issue_gemm_rebuild stays as its cross-check
-__device__ __forceinline__ void issue_gemm(uint32_t tmem_d, const uint8_t* a_hi, const uint8_t* a_lo, const uint8_t* w_hi,
-                                                   const uint8_t* w_lo, int Kp, int Np) {
-    const uint32_t idesc = umma::make_idesc(128, Np, umma::kFmtBF16);
+// rows [64 mh, 64 mh + 64) of one stream of D[128 x Np] = A[128 x Kp] W^T as the three split products (one warpgroup, see
+// umma::wg_gemm). A tiles have the 8-row-group stride a_sbo; the weight tile is [Np rows][Kp] K-major. Descriptor convention
+// checked by tests/test_fused_gpu.py::test_umma_gemm_self_test: the first offset field (LBO) is the stride between core
+// matrices adjacent along K, the second (SBO) between 8-row groups.
+__device__ __forceinline__ void issue_gemm(uint32_t tmem_d, int mh, const uint8_t* a_hi, const uint8_t* a_lo, const uint8_t* w_hi,
+                                           const uint8_t* w_lo, int Kp, int Np, int a_sbo = kSBO_A) {
     const uint32_t sbo_w = (Kp / 8) * kLBO;
-    const uint64_t dah0 = umma::make_desc(umma::smem_u32(a_hi), kLBO, kSBO_A), dal0 = umma::make_desc(umma::smem_u32(a_lo), kLBO, kSBO_A);
-    const uint64_t dwh0 = umma::make_desc(umma::smem_u32(w_hi), kLBO, sbo_w), dwl0 = umma::make_desc(umma::smem_u32(w_lo), kLBO, sbo_w);
-    for (int kk = 0; kk < Kp / 16; kk++) {
-        const uint64_t off = (uint64_t)(kk * ((2 * kLBO) >> 4));
-        umma::mma_bf16(tmem_d, dah0 + off, dwh0 + off, idesc, kk > 0 ? 1u : 0u);
-        umma::mma_bf16(tmem_d, dah0 + off, dwl0 + off, idesc, 1u);
-        umma::mma_bf16(tmem_d, dal0 + off, dwh0 + off, idesc, 1u);
-    }
+    const uint32_t ao = (uint32_t)(mh * 8 * a_sbo);
+    const uint64_t dah = umma::make_desc(umma::smem_u32(a_hi) + ao, kLBO, a_sbo), dal = umma::make_desc(umma::smem_u32(a_lo) + ao, kLBO, a_sbo);
+    const uint64_t dwh = umma::make_desc(umma::smem_u32(w_hi), kLBO, sbo_w), dwl = umma::make_desc(umma::smem_u32(w_lo), kLBO, sbo_w);
+    umma::wg_gemm<0, 0>(tmem_d + ((uint32_t)(64 * mh) << 16), false, dah, dal, dwh, dwl, (2 * kLBO) >> 4, (2 * kLBO) >> 4, (8 * sbo_w) >> 4,
+                        Kp / 16, Np, false);
 }
 
 // ---------------------------------------------------------------------------------------------- backward helpers
@@ -270,6 +259,11 @@ __device__ __forceinline__ void red_v2(float* addr, float2 v) {
 }
 __device__ __forceinline__ void red_v4(float* addr, float a, float b, float c, float d) {     // 16-byte aligned address
     asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(addr), "f"(a), "f"(b), "f"(c), "f"(d) : "memory");
+}
+// one lattice-gradient contribution: float atomics, or fixed point (deterministic mode, ftab != NULL)
+__device__ __forceinline__ void scatter2(float* gtab, unsigned long long* ftab, unsigned idx, float2 cv) {
+    if (ftab) { fx_add(ftab + (size_t)idx * 2, cv.x); fx_add(ftab + (size_t)idx * 2 + 1, cv.y); }
+    else red_v2(gtab + (size_t)idx * 2, cv);
 }
 // column sums of 16 per-lane values over the 32 lanes of a warp with 16 shuffles (halving butterfly): afterwards both
 // lanes of the pair {2p, 2p+1} hold the sum of column `col` = bit-reversal-free index built from lane bits 4..1.

@@ -1,11 +1,11 @@
-// Fused colour network for sm_100a: positions, view directions, sdf gradients and geometric features in -> linear RGB out
+// Fused colour network for sm_90a: positions, view directions, sdf gradients and geometric features in -> linear RGB out
 // (before colour calibration / sigmoid), i.e. RGB.forward of the reference (permuto_sdf_py/models/models.py:309-420):
 //     feat = permutohedral_encoding(points) (+ concat points)        2L + 4 columns
 //     x    = [feat | SH_5(view dir) (25) | normalize(sdf gradient) (3) | geom feature (32)]
 //     y    = LipshitzMLP(x): K0 -> 128 -> 128 -> 64 -> 3, GELU between layers (weights already row-normalised by the caller)
 // One CTA = one 128-sample tile = MMA M. Input columns are built in registers and written as bf16 hi/lo operand tiles
 // ([128 x <=128] K-major core-matrix layout, 8-row-group stride 2048 B); every layer is three split products of
-// tcgen05.mma (M128 x N{128,128,64,16} x K16) accumulating in TMEM; the epilogue (bias + GELU) writes the next layer's tiles
+// wgmma (M64 x N<=64 x K16, the four warpgroups take one row half x column half each); the epilogue (bias + GELU) writes the next layer's tiles
 // in place. Weights do not fit in shared memory next to the tiles, so each layer's hi/lo block streams in by one TMA bulk
 // copy into a single buffer; the copy of layer l+1 is issued the moment layer l's MMAs retire and hides behind the epilogue.
 // The backward pass (fused_rgb_bwd.cu) recomputes this forward, so nothing is saved for it.
@@ -17,6 +17,7 @@ using namespace psdf_fused;
 using namespace psdf_rgb;
 
 namespace {
+__device__ float g_acc_rgb[(size_t)kAccCtas * kTile * 128];     // accumulator areas (umma.cuh)
 
 __global__ void __launch_bounds__(kRgbThreads, 1)
 k_rgb_fused(RgbParams P, const float* __restrict__ pos, const float* __restrict__ dirs, const float* __restrict__ sdf_grad,
@@ -27,24 +28,23 @@ k_rgb_fused(RgbParams P, const float* __restrict__ pos, const float* __restrict_
     uint8_t* s_w = s_a + 2 * kWTileBytes;                  // weights of the current layer [hi | lo]
     LevelC* lc = reinterpret_cast<LevelC*>(s_w + 2 * kWTileBytes);
     float* s_bias = reinterpret_cast<float*>(lc + 1);      // 4 x 128
-    uint64_t* bars = reinterpret_cast<uint64_t*>(s_bias + kNL * 128);      // [0] weights, [1] mma
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2);
+    uint64_t* bars = reinterpret_cast<uint64_t*>(s_bias + kNL * 128);      // [0] weights
 
     const int tid = threadIdx.x, warp = tid >> 5;
     const int row = tid & 127, grp = tid >> 7;
-    if (tid == 0) { umma::mbar_init(&bars[0], 1); umma::mbar_init(&bars[1], 1); umma::mbar_fence_init(); }
+    if (tid == 0) {
+        umma::mbar_init(&bars[0], 1);
+        umma::mbar_fence_init();
+        umma::acc_attach(g_acc_rgb + (size_t)blockIdx.x * kTile * 128, 128);
+    }
     load_level_consts(lc, P.L, scale, shift, window, tid, kRgbThreads);
     for (int i = tid; i < kNL * 128; i += kRgbThreads) {
         int l = i >> 7, c = i & 127;
         s_bias[i] = (c < P.g.Np[l]) ? reinterpret_cast<const float*>(blob + P.g.bias[l])[c] : 0.0f;
     }
     __syncthreads();
-    if (warp == 0) umma::tmem_alloc(tmem_slot, 128);
-    umma::fence_before_sync();
-    __syncthreads();
-    umma::fence_after_sync();
-    const uint32_t tmem_base = *tmem_slot;
-    uint32_t w_phase = 0, mma_phase = 0;
+    const uint32_t tmem_base = 0;
+    uint32_t w_phase = 0;
 
     const int ntiles = (P.N + kTile - 1) / kTile;
     // weights of layer 0 for the first tile
@@ -58,16 +58,9 @@ k_rgb_fused(RgbParams P, const float* __restrict__ pos, const float* __restrict_
             umma::mbar_wait(&bars[0], w_phase);
             w_phase ^= 1;
             umma::fence_async_smem();
-            umma::fence_before_sync();
             __syncthreads();
-            if (tid == 0) {
-                umma::fence_after_sync();
-                issue_gemm_w(tmem_base, s_a, s_a + kWTileBytes, s_w, s_w + P.g.Np[l] * P.g.Kp[l] * 2, P.g.Kp[l], P.g.Np[l]);
-                umma::commit(&bars[1]);
-            }
-            umma::mbar_wait(&bars[1], mma_phase);
-            mma_phase ^= 1;
-            umma::fence_after_sync();
+            issue_gemm_w(tmem_base, warp >> 2, s_a, s_a + kWTileBytes, s_w, s_w + P.g.Np[l] * P.g.Kp[l] * 2, P.g.Kp[l], P.g.Np[l]);
+            __syncthreads();
             // the weight buffer is free again: stream the next layer (or layer 0 of this CTA's next tile) behind the epilogue
             if (tid == 0) {
                 if (l + 1 < kNL) load_layer_weights(s_w, blob, P.g, l + 1, false, &bars[0]);
@@ -78,7 +71,6 @@ k_rgb_fused(RgbParams P, const float* __restrict__ pos, const float* __restrict_
                 for (int c = grp; c < P.g.Np[l] / 16; c += kRgbGroups) {
                     float z[16];
                     umma::tmem_ld16(trow + c * 16, z);
-                    umma::tmem_ld_wait();
 #pragma unroll
                     for (int i = 0; i < 16; i++) { const float zz = z[i] + s_bias[l * 128 + c * 16 + i]; z[i] = zz * gelu_eval(zz).cdf; }
                     store8w(s_a, s_a + kWTileBytes, row, 2 * c, z);
@@ -87,18 +79,14 @@ k_rgb_fused(RgbParams P, const float* __restrict__ pos, const float* __restrict_
             } else if (grp == 0) {
                 float z[16];
                 umma::tmem_ld16(trow, z);
-                umma::tmem_ld_wait();
                 if (valid) {
 #pragma unroll
                     for (int i = 0; i < 3; i++) out[(size_t)n * 3 + i] = z[i] + s_bias[l * 128 + i];
                 }
             }
-            umma::fence_before_sync();
         }
-        __syncthreads();      // all TMEM reads / tile writes of this tile done before the next tile's encoder overwrites s_a
+        __syncthreads();      // all accumulator reads / tile writes of this tile done before the next tile's encoder overwrites s_a
     }
-    __syncthreads();
-    if (warp == 0) umma::tmem_dealloc(tmem_base, 128);
 }
 
 #define ST ((cudaStream_t)stream)
@@ -130,13 +118,13 @@ int psdf_rgb_fused_forward(int N, int L, int T, const float* pos, const float* d
     int rc = make_rgb_params(P, N, L, T, geom_dim, points_scaling, h1, h2, h3);
     if (rc != PSDF_OK) return rc;
     if (N == 0) return PSDF_OK;
-    int dev = 0, sms = 148;
+    int dev = 0, sms = 132;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     const size_t smem = (size_t)4 * kWTileBytes + sizeof(LevelC) + kNL * 128 * sizeof(float) + 64;
     { static bool optin_[64]; psdf::psdf_optin_smem(k_rgb_fused, 227 * 1024, optin_); }
     const int ntiles = div_up(N, kTile);
-    k_rgb_fused<<<min(ntiles, sms), kRgbThreads, smem, ST>>>(P, pos, dirs, sdf_grad, geom, reinterpret_cast<const float2*>(lattice),
+    k_rgb_fused<<<min(min(ntiles, sms), kAccCtas), kRgbThreads, smem, ST>>>(P, pos, dirs, sdf_grad, geom, reinterpret_cast<const float2*>(lattice),
                                                              scale_factor, shift, window, blob, out);
     PSDF_CHECK_LAUNCH();
     return PSDF_OK;

@@ -70,19 +70,20 @@ __device__ __forceinline__ void store8w(uint8_t* a_hi, uint8_t* a_lo, int row, i
     *reinterpret_cast<uint4*>(a_lo + off) = make_uint4(l[0], l[1], l[2], l[3]);
 }
 
-// three split products of [128 x Kp] x [Np x Kp]^T into TMEM (single thread); A tiles use the 2048-byte row-group stride
-__device__ __forceinline__ void issue_gemm_w(uint32_t tmem_d, const uint8_t* a_hi, const uint8_t* a_lo, const uint8_t* w_hi, const uint8_t* w_lo,
-                                             int Kp, int Np) {
-    const uint32_t idesc = umma::make_idesc(128, Np, umma::kFmtBF16);
+// quarter `part` (row half part & 1, column half part >> 1) of the three split products of [128 x Kp] x [Np x Kp]^T into the
+// accumulator columns of tmem_d (one warpgroup); A tiles use the 2048-byte row-group stride
+__device__ __forceinline__ void issue_gemm_w(uint32_t tmem_d, int part, const uint8_t* a_hi, const uint8_t* a_lo, const uint8_t* w_hi,
+                                             const uint8_t* w_lo, int Kp, int Np) {
+    int n0, nn;
+    split_n(Np, part >> 1, n0, nn);
+    if (nn <= 0) return;
+    const int mh = part & 1;
     const uint32_t sbo_w = (Kp / 8) * kLBO;
-    const uint64_t dah0 = umma::make_desc(umma::smem_u32(a_hi), kLBO, kWSBO), dal0 = umma::make_desc(umma::smem_u32(a_lo), kLBO, kWSBO);
-    const uint64_t dwh0 = umma::make_desc(umma::smem_u32(w_hi), kLBO, sbo_w), dwl0 = umma::make_desc(umma::smem_u32(w_lo), kLBO, sbo_w);
-    for (int kk = 0; kk < Kp / 16; kk++) {
-        const uint64_t off = (uint64_t)(kk * ((2 * kLBO) >> 4));      // start-address field, 16-byte units
-        umma::mma_bf16(tmem_d, dah0 + off, dwh0 + off, idesc, kk > 0 ? 1u : 0u);
-        umma::mma_bf16(tmem_d, dah0 + off, dwl0 + off, idesc, 1u);
-        umma::mma_bf16(tmem_d, dal0 + off, dwh0 + off, idesc, 1u);
-    }
+    const uint32_t ao = (uint32_t)(mh * 8 * kWSBO), wo = (uint32_t)(n0 / 8) * sbo_w;
+    const uint64_t dah = umma::make_desc(umma::smem_u32(a_hi) + ao, kLBO, kWSBO), dal = umma::make_desc(umma::smem_u32(a_lo) + ao, kLBO, kWSBO);
+    const uint64_t dwh = umma::make_desc(umma::smem_u32(w_hi) + wo, kLBO, sbo_w), dwl = umma::make_desc(umma::smem_u32(w_lo) + wo, kLBO, sbo_w);
+    umma::wg_gemm<0, 0>(tmem_d + (uint32_t)n0 + ((uint32_t)(64 * mh) << 16), false, dah, dal, dwh, dwl, (2 * kLBO) >> 4, (2 * kLBO) >> 4,
+                        (8 * sbo_w) >> 4, Kp / 16, nn, false);
 }
 
 // Layer-0 operand tile of one sample row. Thread (row, grp) builds the 8-column cores grp, grp+4, ... of the lattice part and

@@ -1,13 +1,13 @@
-// Fused permutohedral encoding + SDF MLP for sm_100a: positions in, {sdf, d sdf/d x, geometric feature} out;
+// Fused permutohedral encoding + SDF MLP for sm_90a: positions in, {sdf, d sdf/d x, geometric feature} out;
 // the 36..52 encoded features and every hidden activation stay on chip (registers -> shared memory operand
-// tiles -> tcgen05 tensor cores -> TMEM accumulators -> registers). Replaces the reference's chain
+// tiles -> wgmma tensor cores -> accumulators -> registers). Replaces the reference's chain
 //   permutohedral_encoding.forward -> 4x cuBLAS SGEMM + 3x GELU kernels (+ autograd.grad for the normal)
 // of SDF.forward / SDF.get_sdf_and_gradient (permuto_sdf_py/models/models.py:176-259).
 //
 // Numerics. The reference runs the MLP in fp32 (TF32 explicitly off, train_permuto_sdf.py:65) and the parity
 // bar is 1e-3 relative, so single-pass bf16/tf32 operands are not good enough for d sdf/d x. Every operand is
-// split as x = hi + lo (two bf16, |x-hi-lo| <= 2^-17 |x|) and each product uses three tcgen05.mma
-// (hi*hi + hi*lo + lo*hi, fp32 accumulation in TMEM): ~1e-5 relative error at 3x the (tiny) MMA cost.
+// split as x = hi + lo (two bf16, |x-hi-lo| <= 2^-17 |x|) and each product uses three wgmma
+// (hi*hi + hi*lo + lo*hi, fp32 accumulation): ~1e-5 relative error at 3x the (tiny) MMA cost.
 //
 // The gradient is computed in forward mode: three tangent streams d/dx_j ride along the value stream through
 // the same weights ( tz_l = W_l ta_{l-1}, ta_l = gelu'(z_l) * tz_l ), their level-0 input being d feat / d x_j,
@@ -16,10 +16,12 @@
 // Work mapping: one CTA = one 128-sample tile = the M of the MMA, 512 threads = 4 groups x 128 rows.
 //   encoder : thread (row, g) computes the 16-byte operand cores g, g+4, ... (4 lattice levels = 8 features each)
 //             of its sample for all streams -> 16 gathers per thread in flight at L = 16, 16 warps per SM;
-//   MMA     : thread 0 issues S streams x (K/16) x 3 tcgen05.mma, one tcgen05.commit -> mbarrier;
-//   epilogue: thread (row, g) owns accumulator columns [16g, 16g+16) of row `row` (TMEM lane row) of every stream:
-//             tcgen05.ld, bias, GELU / GELU', bf16 hi/lo split, 16-byte core stores for the next layer.
-// Weights (hi+lo, pre-packed in the UMMA core-matrix layout by k_pack_mlp) are fetched once per CTA with one
+//   MMA     : warpgroup s issues stream s, (K/16) x 3 wgmma per 64 rows, into the CTA's accumulator area;
+//   epilogue: thread (row, g) owns accumulator columns [16g, 16g+16) of row `row` (accumulator lane row) of every stream:
+//             bias, GELU / GELU', bf16 hi/lo split, 16-byte core stores for the next layer.
+// The value-only kernels (256 threads) and the two-group value + tangent kernel keep their products in registers instead (see
+// value_rows and k_sdf_fused_dual).
+// Weights (hi+lo, pre-packed in the core-matrix operand layout by k_pack_mlp) are fetched once per CTA with one
 // cp.async.bulk (TMA) and stay resident; CTAs are persistent over tiles (one CTA per SM).
 #include <cstdlib>
 #include "fused_common.cuh"
@@ -44,6 +46,61 @@ struct FwdSegs {
     float* geom[2];
 };
 template <bool TAN> struct FwdCfg { static constexpr int kThreads = TAN ? kFusedThreads : kValueThreads; static constexpr int kCtasPerSm = TAN ? 1 : 2; };
+// accumulator areas (umma.cuh) of the kernels of this file
+__device__ float g_acc_tan[(size_t)kAccCtas * kTile * 256];
+
+// bf16 hi / lo pair of two adjacent columns of one row -> the two operand tiles (4-byte stores; a warp covers whole 128-byte cores)
+__device__ __forceinline__ void store_pair(uint8_t* t_hi, uint8_t* t_lo, int row, int col, float x0, float x1) {
+    uint32_t h, l;
+    umma::split2_bf16(x0, x1, h, l);
+    const int off = (row >> 3) * kSBO_A + (col >> 3) * kLBO + (row & 7) * 16 + (col & 7) * 2;
+    *reinterpret_cast<uint32_t*>(t_hi + off) = h;
+    *reinterpret_cast<uint32_t*>(t_lo + off) = l;
+}
+
+// ---------------------------------------------------------------------------------------------- value-only layers in registers
+// Layer l of a value-only 128-row tile (inference forward, sphere tracer): warpgroup mh forms rows 64 mh .. 64 mh + 63 of D = A W^T in
+// its registers (umma::wg_mma_regs fragments) and consumes them itself -- bias + GELU into the next layer's operand cores, or the
+// output values. No other warp reads or writes those rows of the operand tiles in between, so no CTA barrier separates the two.
+template <int N>
+__device__ __forceinline__ void rows_product(float* acc, int mh, const uint8_t* s_a, const uint8_t* w_hi, const uint8_t* w_lo, int Kp) {
+    const uint32_t sbo_w = (Kp / 8) * kLBO, ao = (uint32_t)(mh * 8 * kSBO_A);
+    const uint64_t dah = umma::make_desc(umma::smem_u32(s_a) + ao, kLBO, kSBO_A), dal = umma::make_desc(umma::smem_u32(s_a + kATileBytes) + ao, kLBO, kSBO_A);
+    const uint64_t dwh = umma::make_desc(umma::smem_u32(w_hi), kLBO, sbo_w), dwl = umma::make_desc(umma::smem_u32(w_lo), kLBO, sbo_w);
+    umma::wgmma_fence();
+    umma::wg_mma_regs<N, 0, 0>(acc, dah, dal, dwh, dwl, (2 * kLBO) >> 4, (2 * kLBO) >> 4, Kp / 16, false);
+    umma::wgmma_commit();
+    umma::wgmma_wait0();
+}
+// the fragment (32 floats, the first Np / 2 used) of rows 64 mh .. 64 mh + 63 of layer l
+__device__ __forceinline__ void value_rows(float* acc, const MlpGeom& g, int l, int mh, const uint8_t* s_a, const uint8_t* s_blob) {
+#pragma unroll
+    for (int i = 0; i < 32; i++) acc[i] = 0.f;
+    const uint8_t *wh = s_blob + g.w_hi[l], *wl = s_blob + g.w_lo[l];
+    switch (g.Np[l] / 16) {
+        case 1: rows_product<16>(acc, mh, s_a, wh, wl, g.Kp[l]); break;
+        case 2: rows_product<32>(acc, mh, s_a, wh, wl, g.Kp[l]); break;
+        case 3: rows_product<48>(acc, mh, s_a, wh, wl, g.Kp[l]); break;
+        default: rows_product<64>(acc, mh, s_a, wh, wl, g.Kp[l]); break;
+    }
+}
+// fragment row / column of accumulator entry 4 j + 2 h + b (warp w of the warpgroup, lane t)
+__device__ __forceinline__ int frag_row(int mh, int h) { return 64 * mh + 16 * ((threadIdx.x >> 5) & 3) + (threadIdx.x & 31) / 4 + 8 * h; }
+__device__ __forceinline__ int frag_col(int j) { return 8 * j + 2 * (threadIdx.x & 3); }
+// bias + GELU of a hidden layer's fragment -> the next layer's operand cores
+__device__ __forceinline__ void gelu_to_tiles(const float* acc, const float* bias, int Np, int mh, uint8_t* s_a) {
+#pragma unroll
+    for (int j = 0; j < 8; j++) {
+        if (8 * j < Np) {
+#pragma unroll
+            for (int h = 0; h < 2; h++) {
+                const int c = frag_col(j);
+                const float z0 = acc[4 * j + 2 * h] + bias[c], z1 = acc[4 * j + 2 * h + 1] + bias[c + 1];
+                store_pair(s_a, s_a + kATileBytes, frag_row(mh, h), c, z0 * gelu_eval(z0).cdf, z1 * gelu_eval(z1).cdf);
+            }
+        }
+    }
+}
 
 template <bool TAN>
 __global__ void __launch_bounds__(FwdCfg<TAN>::kThreads, FwdCfg<TAN>::kCtasPerSm)
@@ -55,15 +112,14 @@ k_sdf_fused(FusedParams P, FwdSegs G, const float2* __restrict__ lattice, const 
     uint8_t* s_blob = smem;
     uint8_t* s_a = smem + P.g.total;                       // S streams x {hi, lo} x 16 KB
     LevelC* lc = reinterpret_cast<LevelC*>(s_a + S * 2 * kATileBytes);
-    uint64_t* bars = reinterpret_cast<uint64_t*>(lc + 1);  // [0] weights, [1] mma
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2);
+    uint64_t* bars = reinterpret_cast<uint64_t*>(lc + 1);  // [0] weights
     const int tid = threadIdx.x, warp = tid >> 5;
     const int row = tid & (kTile - 1), grp = tid >> 7;
 
     if (tid == 0) {
         umma::mbar_init(&bars[0], 1);
-        umma::mbar_init(&bars[1], S);          // one tcgen05.commit per issuing thread (one per stream)
         umma::mbar_fence_init();
+        if (TAN) umma::acc_attach(g_acc_tan + (size_t)blockIdx.x * kTile * (S * 64), S * 64);
     }
     for (int i = tid; i < P.L * 3; i += kThreads) {
         lc->scale[(i / 3) * 4 + (i % 3)] = scale[i];
@@ -71,17 +127,12 @@ k_sdf_fused(FusedParams P, FwdSegs G, const float2* __restrict__ lattice, const 
     }
     for (int i = tid; i < P.L; i += kThreads) lc->window[i] = window ? window[i] : 1.0f;
     __syncthreads();
-    if (warp == 0) umma::tmem_alloc(tmem_slot, S * 64);
     if (tid == 0) {
         umma::mbar_expect_tx(&bars[0], (uint32_t)P.g.total);
         umma::bulk_g2s(s_blob, blob, (uint32_t)P.g.total, &bars[0]);
     }
-    umma::fence_before_sync();
-    __syncthreads();
-    umma::fence_after_sync();
-    const uint32_t tmem_base = *tmem_slot;
+    const uint32_t tmem_base = 0;
     umma::mbar_wait(&bars[0], 0);
-    uint32_t mma_phase = 0;
     const int level_cores = P.L / 4;                        // 4 levels x 2 features = one 16-byte core row
     const int all_cores = P.g.Kp[0] / 8;
 
@@ -171,28 +222,48 @@ k_sdf_fused(FusedParams P, FwdSegs G, const float2* __restrict__ lattice, const 
 #pragma unroll 1
         for (int l = 0; l < kNL; l++) {
             if (!(P.knockout & 128)) umma::fence_async_smem();
-            umma::fence_before_sync();
             __syncthreads();
-            if ((tid & 31) == 0 && warp < S) {
-                // stream s is issued by lane 0 of warp s: the four single-thread issue sequences run on four different SM
-                // sub-partitions side by side; the mbarrier completes when all S commits have arrived
-                const int s = warp;
-                umma::fence_after_sync();
-                if (!(P.knockout & 2))
-                    issue_gemm(tmem_base + s * 64, s_a + s * 2 * kATileBytes, s_a + s * 2 * kATileBytes + kATileBytes, s_blob + P.g.w_hi[l],
-                               s_blob + P.g.w_lo[l], P.g.Kp[l], P.g.Np[l]);
-                if (P.knockout & 64) umma::mbar_arrive(&bars[1]);      // diagnostics: plain arrive instead of tcgen05.commit
-                else umma::commit(&bars[1]);
+            if constexpr (!TAN) {
+                // value only: warpgroup mh owns rows 64 mh .. 64 mh + 63 from the product to the outputs (see value_rows)
+                const int mh = warp >> 2;
+                float acc[32];
+                value_rows(acc, P.g, l, mh, s_a, s_blob);
+                const float* bias = reinterpret_cast<const float*>(s_blob + P.g.bias[l]);
+                if (l < kNL - 1) {
+                    gelu_to_tiles(acc, bias, P.g.Np[l], mh, s_a);
+                } else {
+                    const int nout = P.g.N[l], n0 = n - row, cnt = seg1 ? G.n[1] : G.n[0];
+#pragma unroll
+                    for (int j = 0; j < 8; j++) {
+#pragma unroll
+                        for (int h = 0; h < 2; h++) {
+#pragma unroll
+                            for (int b = 0; b < 2; b++) {
+                                const int c = frag_col(j) + b, nr = n0 + frag_row(mh, h);
+                                if (c >= nout || nr >= cnt) continue;
+                                const float v = acc[4 * j + 2 * h + b] + bias[c];
+                                if (c == 0) sdf_out[nr] = v;
+                                else if (geom_out) geom_out[(size_t)nr * (nout - 1) + c - 1] = v;
+                            }
+                        }
+                    }
+                }
+                continue;
             }
-            umma::mbar_wait(&bars[1], mma_phase);
-            mma_phase ^= 1;
-            umma::fence_after_sync();
+            // value + tangents: warpgroup s issues stream s (both row halves)
+            if (!(P.knockout & 2)) {
+                const int wgi = warp >> 2;
+                for (int mh = 0; mh < 2; mh++)
+                    issue_gemm(tmem_base + wgi * 64, mh, s_a + wgi * 2 * kATileBytes, s_a + wgi * 2 * kATileBytes + kATileBytes,
+                               s_blob + P.g.w_hi[l], s_blob + P.g.w_lo[l], P.g.Kp[l], P.g.Np[l]);
+            }
+            __syncthreads();
             const float* bias = reinterpret_cast<const float*>(s_blob + P.g.bias[l]);
             const uint32_t trow = tmem_base + ((uint32_t)((warp & 3) * 32) << 16);
             const bool last = (l == kNL - 1);
             for (int c = grp; c < P.g.Np[l] / 16; c += kGroups) {     // this thread's 16-column chunks
                 float z[16], tz[3][16];
-                if (P.knockout & 16) {                 // diagnostics: no TMEM reads
+                if (P.knockout & 16) {                 // diagnostics: no accumulator reads
 #pragma unroll
                     for (int i = 0; i < 16; i++) { z[i] = 0.f; tz[0][i] = 0.f; tz[1][i] = 0.f; tz[2][i] = 0.f; }
                 } else {
@@ -201,7 +272,6 @@ k_sdf_fused(FusedParams P, FwdSegs G, const float2* __restrict__ lattice, const 
 #pragma unroll
                         for (int j = 0; j < 3; j++) umma::tmem_ld16(trow + (1 + j) * 64 + c * 16, tz[j]);
                     }
-                    umma::tmem_ld_wait();
                 }
 #pragma unroll
                 for (int i = 0; i < 16; i++) z[i] += bias[c * 16 + i];
@@ -251,47 +321,39 @@ k_sdf_fused(FusedParams P, FwdSegs G, const float2* __restrict__ lattice, const 
                 }
             }
         }
-        umma::fence_before_sync();
-        __syncthreads();   // all TMEM reads of this tile done before the next tile's MMAs overwrite the accumulators
+        __syncthreads();   // all accumulator reads of this tile done before the next tile's MMAs overwrite them
     }
-    __syncthreads();
-    if (warp == 0) umma::tmem_dealloc(tmem_base, S * 64);
 }
 
 // ---------------------------------------------------------------------------------------------- value + tangents, two groups per CTA
 // The kernel above runs its phases in lock step: all 16 warps gather, then all wait for the tensor core, then all run the epilogue
-// (ncu, profiles/README.md: a warp issues 10 % of the time; 28 % long-scoreboard on the MMA mbarrier / gathers, 10 % CTA barrier).
 // Two CTAs per SM would let one CTA's waits be filled by the other's work, but the operand tiles of four streams (128 KB) + the weight
 // blob (57 KB) allow one. Here ONE CTA holds TWO independent groups of 256 threads, each working on its own 64-sample sub-tile
-// (M = 64 MMAs, 64 KB of operand tiles, its own mbarrier, named barrier and 256 TMEM columns) and sharing the resident weights: the
+// (M = 64 MMAs, 64 KB of operand tiles, its own named barrier and 256 accumulator columns) and sharing the resident weights: the
 // groups drift apart and each one's MMA / barrier / gather waits overlap the other's encoder and epilogue work.
-// M = 64 accumulators keep rows 16 q .. 16 q + 15 in TMEM lanes 32 q .. 32 q + 15; they are read with tcgen05.ld.16x256b (m16n8
-// fragment layout, every thread holds useful values) and the next layer's operand cores are written as 4-byte bf16 pairs.
+// Warpgroup hc of a group forms columns 32 hc .. 32 hc + 31 of all four streams (M = 64, N = 32) and keeps them in registers: the
+// m16n8 fragments are exactly what its epilogue consumes (every thread holds useful values), so these products never leave the SM;
+// the next layer's operand cores are written as 4-byte bf16 pairs.
 constexpr int kSub = 64;                        // samples per sub-tile
 constexpr int kSubTileBytes = kSub * 64 * 2;    // one bf16 operand tile [64 x 64]
 constexpr int kGroupThreads = 256;
 constexpr int kStg = 69;                         // row stride (floats) of the output staging tile: 64 value columns max + 3 gradient columns
 
-__device__ __forceinline__ void issue_gemm_m64(uint32_t tmem_d, const uint8_t* a_hi, const uint8_t* a_lo, const uint8_t* w_hi,
-                                               const uint8_t* w_lo, int Kp, int Np) {
-    const uint32_t idesc = umma::make_idesc(64, Np, umma::kFmtBF16);
-    const uint32_t sbo_w = (Kp / 8) * kLBO;
-    const uint64_t dah0 = umma::make_desc(umma::smem_u32(a_hi), kLBO, kSBO_A), dal0 = umma::make_desc(umma::smem_u32(a_lo), kLBO, kSBO_A);
-    const uint64_t dwh0 = umma::make_desc(umma::smem_u32(w_hi), kLBO, sbo_w), dwl0 = umma::make_desc(umma::smem_u32(w_lo), kLBO, sbo_w);
-    for (int kk = 0; kk < Kp / 16; kk++) {
-        const uint64_t off = (uint64_t)(kk * ((2 * kLBO) >> 4));
-        umma::mma_bf16(tmem_d, dah0 + off, dwh0 + off, idesc, kk > 0 ? 1u : 0u);
-        umma::mma_bf16(tmem_d, dah0 + off, dwl0 + off, idesc, 1u);
-        umma::mma_bf16(tmem_d, dal0 + off, dwh0 + off, idesc, 1u);
+// columns [n0, n0 + N) of the four streams' D[64 x Np] = A[64 x Kp] W^T into registers (one warpgroup; fragment layout of
+// umma::wg_mma_regs). Stream s's A tiles are s_a + s * 2 * kSubTileBytes (hi, lo).
+template <int N>
+__device__ __forceinline__ void issue_streams_regs(float (*acc)[16], const uint8_t* s_a, const uint8_t* w_hi, const uint8_t* w_lo, int Kp, int n0) {
+    const uint32_t sbo_w = (Kp / 8) * kLBO, wo = (uint32_t)(n0 / 8) * sbo_w;
+    const uint64_t dwh = umma::make_desc(umma::smem_u32(w_hi) + wo, kLBO, sbo_w), dwl = umma::make_desc(umma::smem_u32(w_lo) + wo, kLBO, sbo_w);
+    umma::wgmma_fence();
+#pragma unroll
+    for (int s = 0; s < 4; s++) {
+        const uint8_t* a = s_a + s * 2 * kSubTileBytes;
+        const uint64_t dah = umma::make_desc(umma::smem_u32(a), kLBO, kSBO_A), dal = umma::make_desc(umma::smem_u32(a + kSubTileBytes), kLBO, kSBO_A);
+        umma::wg_mma_regs<N, 0, 0>(acc[s], dah, dal, dwh, dwl, (2 * kLBO) >> 4, (2 * kLBO) >> 4, Kp / 16, false);
     }
-}
-// bf16 hi / lo pair of two adjacent columns of one row -> the two operand tiles (4-byte stores; a warp covers whole 128-byte cores)
-__device__ __forceinline__ void store_pair(uint8_t* t_hi, uint8_t* t_lo, int row, int col, float x0, float x1) {
-    uint32_t h, l;
-    umma::split2_bf16(x0, x1, h, l);
-    const int off = (row >> 3) * kSBO_A + (col >> 3) * kLBO + (row & 7) * 16 + (col & 7) * 2;
-    *reinterpret_cast<uint32_t*>(t_hi + off) = h;
-    *reinterpret_cast<uint32_t*>(t_lo + off) = l;
+    umma::wgmma_commit();
+    umma::wgmma_wait0();
 }
 
 __global__ void __launch_bounds__(2 * kGroupThreads, 1)
@@ -303,17 +365,14 @@ k_sdf_fused_dual(FusedParams P, FwdSegs G, const float2* __restrict__ lattice, c
     const int tid = threadIdx.x, grp2 = tid >> 8, t = tid & 255;            // group of the CTA, thread inside the group
     uint8_t* s_a = smem + P.g.total + grp2 * (S * 2 * kSubTileBytes);       // this group's S streams x {hi, lo} x 8 KB
     LevelC* lc = reinterpret_cast<LevelC*>(smem + P.g.total + 2 * S * 2 * kSubTileBytes);
-    uint64_t* bars = reinterpret_cast<uint64_t*>(lc + 1);                    // [0] weights, [1 + g] MMAs of group g, [3] start skew
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 4);
-    const int warp = tid >> 5, lane = tid & 31;
+    uint64_t* bars = reinterpret_cast<uint64_t*>(lc + 1);                    // [0] weights, [3] start skew
+    const int lane = tid & 31;
     const int wg = t >> 5;                                                   // warp inside the group, 0..7
     const int row = t & (kSub - 1), eg = t >> 6;                             // encoder: 4 threads per sample row
     constexpr int kEnc = kGroupThreads / kSub;
 
     if (tid == 0) {
         umma::mbar_init(&bars[0], 1);
-        umma::mbar_init(&bars[1], S);
-        umma::mbar_init(&bars[2], S);
         umma::mbar_init(&bars[3], 1);
         umma::mbar_fence_init();
     }
@@ -323,29 +382,21 @@ k_sdf_fused_dual(FusedParams P, FwdSegs G, const float2* __restrict__ lattice, c
     }
     for (int i = tid; i < P.L; i += 2 * kGroupThreads) lc->window[i] = window ? window[i] : 1.0f;
     __syncthreads();
-    if (warp == 0) umma::tmem_alloc(tmem_slot, 2 * S * 64);
     if (tid == 0) {
         umma::mbar_expect_tx(&bars[0], (uint32_t)P.g.total);
         umma::bulk_g2s(s_blob, blob, (uint32_t)P.g.total, &bars[0]);
     }
-    umma::fence_before_sync();
-    __syncthreads();
-    umma::fence_after_sync();
-    const uint32_t tmem_base = *tmem_slot + (uint32_t)(grp2 * S * 64);       // this group's 256 columns
     umma::mbar_wait(&bars[0], 0);
-    uint64_t* mbar = &bars[1 + grp2];
-    uint32_t mma_phase = 0;
     const int level_cores = P.L / 4, all_cores = P.g.Kp[0] / 8;
-    // epilogue mapping: warp quadrant q = rows 16 q .. 16 q + 15 (TMEM lanes 32 q ..), column half hc = columns 32 hc .. 32 hc + 31
+    // epilogue mapping: warp quadrant q = rows 16 q .. 16 q + 15, column half hc = columns 32 hc .. 32 hc + 31 (the warpgroup's products)
     const int q = wg & 3, hc = wg >> 2;
-    const uint32_t tq = tmem_base + ((uint32_t)(q * 32) << 16);
     const int er0 = q * 16 + (lane >> 2);                                     // rows er0 and er0 + 8 of the sub-tile
     const int ec0 = hc * 32 + 2 * (lane & 3);                                 // columns ec0 + 8 j + {0, 1}
 
     const int nsub = G.tile0[2];                                             // in units of 64-sample sub-tiles (see launch_forward)
     // Two identical groups that start together stay in lock step (every unit is shared fairly), waiting for the tensor core at the same
     // time. Group 1 therefore starts half a sub-tile late: it waits until group 0 has finished the second layer of its first sub-tile;
-    // from then on one group's MMA / TMEM-read phases meet the other's encoder / GELU / store phases.
+    // from then on one group's MMA / accumulator-read phases meet the other's encoder / GELU / store phases.
     bool skew_pending = P.skew != 0;
     if (skew_pending && grp2 == 1 && blockIdx.x * 2 < nsub) { umma::mbar_wait(&bars[3], 0); skew_pending = false; }
     for (int sub = blockIdx.x * 2 + grp2; sub < nsub; sub += 2 * gridDim.x) {
@@ -422,26 +473,22 @@ k_sdf_fused_dual(FusedParams P, FwdSegs G, const float2* __restrict__ lattice, c
 #pragma unroll 1
         for (int l = 0; l < kNL; l++) {
             umma::fence_async_smem();
-            umma::fence_before_sync();
             umma::bar_sync(1 + grp2, kGroupThreads);
-            if (lane == 0 && wg < S) {
-                const int s = wg;
-                umma::fence_after_sync();
-                issue_gemm_m64(tmem_base + s * 64, s_a + s * 2 * kSubTileBytes, s_a + s * 2 * kSubTileBytes + kSubTileBytes, s_blob + P.g.w_hi[l],
-                               s_blob + P.g.w_lo[l], P.g.Kp[l], P.g.Np[l]);
-                umma::commit(mbar);
-            }
-            umma::mbar_wait(mbar, mma_phase);
-            mma_phase ^= 1;
-            umma::fence_after_sync();
+            // acc[0] = z, acc[1 + j] = tz_j: this warpgroup's 32 (or, in a narrower output layer, 16) columns of the four streams
+            float acc[S][16];
+#pragma unroll
+            for (int s = 0; s < S; s++)
+#pragma unroll
+                for (int i = 0; i < 16; i++) acc[s][i] = 0.f;
+            const int ncols = min(32, P.g.Np[l] - hc * 32);
+            if (ncols == 32) issue_streams_regs<32>(acc, s_a, s_blob + P.g.w_hi[l], s_blob + P.g.w_lo[l], P.g.Kp[l], hc * 32);
+            else if (ncols == 16) issue_streams_regs<16>(acc, s_a, s_blob + P.g.w_hi[l], s_blob + P.g.w_lo[l], P.g.Kp[l], hc * 32);
+            umma::bar_sync(1 + grp2, kGroupThreads);     // every product of the group has read this layer's operand tiles
             const float* bias = reinterpret_cast<const float*>(s_blob + P.g.bias[l]);
             const bool last = (l == kNL - 1);
-            if (hc * 32 < P.g.Np[l]) {                    // this warp's 32 columns exist in this layer (the output layer may be narrower)
-                float z[16], tz[3][16];
-                umma::tmem_ld16x32(tq + hc * 32, z);
-#pragma unroll
-                for (int j = 0; j < 3; j++) umma::tmem_ld16x32(tq + (1 + j) * 64 + hc * 32, tz[j]);
-                umma::tmem_ld_wait();
+            if (ncols > 0) {                              // this warp's columns exist in this layer (the output layer may be narrower)
+                float* z = acc[0];
+                float (*tz)[16] = acc + 1;
 #pragma unroll
                 for (int j = 0; j < 4; j++) {
 #pragma unroll
@@ -475,7 +522,7 @@ k_sdf_fused_dual(FusedParams P, FwdSegs G, const float2* __restrict__ lattice, c
                     if (skew_pending && grp2 == 0 && l == 1) { if (t == 0) umma::mbar_arrive(&bars[3]); skew_pending = false; }
                 } else {
                     // outputs are staged in shared memory (the operand tiles are dead: the last MMAs completed) and leave as whole rows:
-                    // a fragment thread holds 2 columns of 2 rows, which would be 4-byte stores 128 bytes apart (measured: 8 us of 92)
+                    // a fragment thread holds 2 columns of 2 rows, which would be 4-byte stores 128 bytes apart
                     const int nout = P.g.N[l];
                     float* stg = reinterpret_cast<float*>(s_a);            // [64][kStg]: sdf | geom (nout - 1) | grad (3)
 #pragma unroll
@@ -495,8 +542,7 @@ k_sdf_fused_dual(FusedParams P, FwdSegs G, const float2* __restrict__ lattice, c
             }
         }
         // ---------------- coalesced copy-out of the sub-tile's rows
-        umma::fence_before_sync();
-        umma::bar_sync(1 + grp2, kGroupThreads);     // staging complete; TMEM reads of this sub-tile done before its next MMAs
+        umma::bar_sync(1 + grp2, kGroupThreads);     // staging complete
         {
             const float* stg = reinterpret_cast<const float*>(s_a);
             const int nout = P.g.N[kNL - 1];
@@ -511,9 +557,6 @@ k_sdf_fused_dual(FusedParams P, FwdSegs G, const float2* __restrict__ lattice, c
         }
         umma::bar_sync(1 + grp2, kGroupThreads);     // the staging area is the next sub-tile's operand tile
     }
-    umma::fence_before_sync();
-    __syncthreads();
-    if (warp == 0) umma::tmem_dealloc(*tmem_slot, 2 * S * 64);
 }
 
 // ---------------------------------------------------------------------------------------------- fused sphere tracing
@@ -550,20 +593,23 @@ k_sdf_sphere_trace(FusedParams P, TraceParams Q, const float* __restrict__ pos_i
     int* s_ms = s_it + kTile;                              // [128] DDA steps of a march in progress, -1: not marching
     float* s_mt = reinterpret_cast<float*>(s_ms + kTile);  // [128] march parameter t of a march in progress
     int* s_new = reinterpret_cast<int*>(s_mt + kTile);     // [128] |sdf| < threshold at the evaluation that started the march
-    int* s_flag = s_new + kTile;                           // [0]: queue drained
+    float* s_sdf = reinterpret_cast<float*>(s_new + kTile);   // [128] network output of the slot in this round
+    int* s_flag = reinterpret_cast<int*>(s_sdf + kTile);   // [0]: queue drained
     uint64_t* bars = reinterpret_cast<uint64_t*>(s_flag + 2);
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2);
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int row = tid & (kTile - 1), grp = tid >> 7;
     constexpr int kGroups = kValueThreads / kTile;
-    if (tid == 0) { umma::mbar_init(&bars[0], 1); umma::mbar_init(&bars[1], 1); umma::mbar_fence_init(); s_flag[0] = 0; }
+    if (tid == 0) {
+        umma::mbar_init(&bars[0], 1);
+        umma::mbar_fence_init();
+        s_flag[0] = 0;
+    }
     for (int i = tid; i < P.L * 3; i += kValueThreads) {
         lc->scale[(i / 3) * 4 + (i % 3)] = scale[i];
         lc->shift[(i / 3) * 4 + (i % 3)] = shift ? shift[i] : 0.0f;
     }
     for (int i = tid; i < P.L; i += kValueThreads) lc->window[i] = window ? window[i] : 1.0f;
     __syncthreads();
-    if (warp == 0) umma::tmem_alloc(tmem_slot, 64);
     if (tid == 0) {
         umma::mbar_expect_tx(&bars[0], (uint32_t)P.g.total);
         umma::bulk_g2s(s_blob, blob, (uint32_t)P.g.total, &bars[0]);
@@ -581,12 +627,8 @@ k_sdf_sphere_trace(FusedParams P, TraceParams Q, const float* __restrict__ pos_i
         s_it[row] = 0;
         s_ms[row] = -1;
     }
-    umma::fence_before_sync();
     __syncthreads();
-    umma::fence_after_sync();
-    const uint32_t tmem_base = *tmem_slot;
     umma::mbar_wait(&bars[0], 0);
-    uint32_t mma_phase = 0;
     const int level_cores = P.L / 4, all_cores = P.g.Kp[0] / 8;
     const float* bias3 = reinterpret_cast<const float*>(s_blob + P.g.bias[kNL - 1]);
     const int first_queued = gridDim.x * kTile;
@@ -649,36 +691,19 @@ k_sdf_sphere_trace(FusedParams P, TraceParams Q, const float* __restrict__ pos_i
 #pragma unroll 1
             for (int l = 0; l < kNL; l++) {
                 umma::fence_async_smem();
-                umma::fence_before_sync();
                 __syncthreads();
-                if (tid == 0) {
-                    umma::fence_after_sync();
-                    issue_gemm(tmem_base, s_a, s_a + kATileBytes, s_blob + P.g.w_hi[l], s_blob + P.g.w_lo[l], P.g.Kp[l], P.g.Np[l]);
-                    umma::commit(&bars[1]);
-                }
-                umma::mbar_wait(&bars[1], mma_phase);
-                mma_phase ^= 1;
-                umma::fence_after_sync();
-                const float* bias = reinterpret_cast<const float*>(s_blob + P.g.bias[l]);
-                const uint32_t trow = tmem_base + ((uint32_t)((warp & 3) * 32) << 16);
+                const int mh = warp >> 2;             // warpgroup mh owns rows 64 mh .. 64 mh + 63 (see value_rows)
+                float acc[32];
+                value_rows(acc, P.g, l, mh, s_a, s_blob);
                 if (l < kNL - 1) {
-                    for (int c = grp; c < P.g.Np[l] / 16; c += kGroups) {
-                        float z[16];
-                        umma::tmem_ld16(trow + c * 16, z);
-                        umma::tmem_ld_wait();
-#pragma unroll
-                        for (int i = 0; i < 16; i++) { const float zz = z[i] + bias[c * 16 + i]; z[i] = zz * gelu_eval(zz).cdf; }
-                        store8(s_a, s_a + kATileBytes, row, 2 * c, z);
-                        store8(s_a, s_a + kATileBytes, row, 2 * c + 1, z + 8);
-                    }
-                } else if (grp == 0) {
-                    float z[16];
-                    umma::tmem_ld16(trow, z);
-                    umma::tmem_ld_wait();
-                    sdf = z[0] + bias3[0];
+                    gelu_to_tiles(acc, reinterpret_cast<const float*>(s_blob + P.g.bias[l]), P.g.Np[l], mh, s_a);
+                } else if ((lane & 3) == 0) {         // column 0 of rows frag_row(mh, 0 / 1)
+                    s_sdf[frag_row(mh, 0)] = acc[0] + bias3[0];
+                    s_sdf[frag_row(mh, 1)] = acc[2] + bias3[0];
                 }
-                umma::fence_before_sync();
             }
+            __syncthreads();
+            sdf = s_sdf[row];
         }
         // ---- step / march / refill: one thread per slot
         if (grp == 0) {
@@ -748,7 +773,7 @@ k_sdf_sphere_trace(FusedParams P, TraceParams Q, const float* __restrict__ pos_i
                 }
             }
         }
-        __syncthreads();      // slots of this round visible, TMEM reads done
+        __syncthreads();      // slots of this round visible, accumulator reads done
     }
     __syncthreads();
     if (tid == 0 && evaluations) {      // statistics of the launch: network evaluations, rounds, rounds that ran the network, longest CTA
@@ -757,7 +782,6 @@ k_sdf_sphere_trace(FusedParams P, TraceParams Q, const float* __restrict__ pos_i
         atomicAdd(queue + 3, net_rounds);
         atomicMax(queue + 4, rounds);
     }
-    if (warp == 0) umma::tmem_dealloc(tmem_base, 64);
 }
 
 #define ST ((cudaStream_t)stream)
@@ -787,13 +811,13 @@ int psdf_sdf_sphere_trace(int N, int L, int T, const float* pos, const float* di
     const float zero3[3] = {0.f, 0.f, 0.f};
     Q.grid = psdf::make_grid_geom(occupancy ? V : 1, occupancy ? extent : 1.0f, occupancy ? trans : zero3);
     Q.sph_radius = sphere_radius; Q.sph_cx = sphere_center[0]; Q.sph_cy = sphere_center[1]; Q.sph_cz = sphere_center[2];
-    int dev = 0, sms = 148;
+    int dev = 0, sms = 132;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    const size_t smem = (size_t)P.g.total + 2 * kATileBytes + sizeof(LevelC) + kTile * 11 * sizeof(float) + 96;
+    const size_t smem = (size_t)P.g.total + 2 * kATileBytes + sizeof(LevelC) + kTile * 12 * sizeof(float) + 80;
     { static bool optin_[64]; psdf::psdf_optin_smem(k_sdf_sphere_trace, 227 * 1024, optin_); }
     const int ntiles = div_up(N, kTile);
-    k_sdf_sphere_trace<<<min(ntiles, 2 * sms), kValueThreads, smem, ST>>>(P, Q, pos, dirs, reinterpret_cast<const float2*>(lattice), scale_factor,
+    k_sdf_sphere_trace<<<min(min(ntiles, 2 * sms), 2 * kAccCtas), kValueThreads, smem, ST>>>(P, Q, pos, dirs, reinterpret_cast<const float2*>(lattice), scale_factor,
                                                                      shift, window, blob, occupancy, pos_out, converged, queue_counter);
     PSDF_CHECK_LAUNCH();
     return PSDF_OK;
@@ -870,7 +894,7 @@ static int launch_forward(int L, int T, const float* lattice, const float* scale
     G.tile0[2] = tiles;
     P.N = total;
     if (tiles == 0) return PSDF_OK;
-    int dev = 0, sms = 148;
+    int dev = 0, sms = 132;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     const float2* lat = reinterpret_cast<const float2*>(lattice);
@@ -885,15 +909,15 @@ static int launch_forward(int L, int T, const float* lattice, const float* scale
         H.tile0[2] = subs;
         size_t smem = (size_t)P.g.total + 2 * 4 * 2 * kSubTileBytes + sizeof(LevelC) + 64;
         { static bool optin_[64]; psdf::psdf_optin_smem(k_sdf_fused_dual, 227 * 1024, optin_); }
-        k_sdf_fused_dual<<<min(div_up(subs, 2), sms), 2 * kGroupThreads, smem, ST>>>(P, H, lat, scale_factor, shift, window, blob);
+        k_sdf_fused_dual<<<min(min(div_up(subs, 2), sms), kAccCtas), 2 * kGroupThreads, smem, ST>>>(P, H, lat, scale_factor, shift, window, blob);
     } else if (tangents) {
         size_t smem = (size_t)P.g.total + 4 * 2 * kATileBytes + sizeof(LevelC) + 64;
         { static bool optin_[64]; psdf::psdf_optin_smem(k_sdf_fused<true>, 227 * 1024, optin_); }
-        k_sdf_fused<true><<<min(tiles, sms), kFusedThreads, smem, ST>>>(P, G, lat, scale_factor, shift, window, blob);
+        k_sdf_fused<true><<<min(min(tiles, sms), kAccCtas), kFusedThreads, smem, ST>>>(P, G, lat, scale_factor, shift, window, blob);
     } else {
         size_t smem = (size_t)P.g.total + 2 * kATileBytes + sizeof(LevelC) + 64;
         { static bool optin_[64]; psdf::psdf_optin_smem(k_sdf_fused<false>, 113 * 1024, optin_); }
-        k_sdf_fused<false><<<min(tiles, 2 * sms), kValueThreads, smem, ST>>>(P, G, lat, scale_factor, shift, window, blob);
+        k_sdf_fused<false><<<min(min(tiles, 2 * sms), 2 * kAccCtas), kValueThreads, smem, ST>>>(P, G, lat, scale_factor, shift, window, blob);
     }
     PSDF_CHECK_LAUNCH();
     return PSDF_OK;

@@ -1,7 +1,7 @@
-// Training backward of the fused encoding + SDF MLP (sm_100a, tcgen05): given d loss / d {sdf, d sdf/dx, geom}
+// Training backward of the fused encoding + SDF MLP (sm_90a, wgmma): given d loss / d {sdf, d sdf/dx, geom}
 // per sample it produces the lattice gradient (scatter-add fused in the kernel), the bias gradients and the weight
 // gradients -- ONE kernel, the weight-gradient products are formed on the tensor cores from the operand tiles while they
-// are still in shared memory and accumulate in TMEM over all tiles of the CTA.
+// are still in shared memory and accumulate in the CTA's accumulator area (umma.cuh) over all tiles of the CTA.
 //
 // What it replaces in the reference: `loss.backward()` through SDF.get_sdf_and_gradient
 // (permuto_sdf_py/models/models.py:199-259, create_graph=True) -- i.e. the double backward of the
@@ -22,17 +22,19 @@
 // Per 128-sample tile (512 threads: row = tid & 127, group g = tid >> 7 owns operand cores g, g+4, .. in the encoder phases
 // and the 16-column chunk g in the epilogues). Two 64 KB operand-tile buffers X, Y ([value hi | value lo | tangent hi | tangent lo]):
 //   1. encoder: a_0, ta_0 -> X; X leaves by ONE TMA store (64 KB / tile, re-read from L2 in step 4: the only spill left)
-//   2. forward recompute, layers 0..2: z_1, z_2 (value + tangent) STAY in TMEM (4 x 64 columns); a_1 -> Y, a_2 -> X, a_3 -> Y;
+//   2. forward recompute, layers 0..2: z_1, z_2 (value + tangent) STAY in the accumulator area (4 x 64 columns); a_1 -> Y, a_2 -> X, a_3 -> Y;
 //      gelu'(z_3), gelu''(z_3) tz_3 stay in registers (layer 3 is reversed right away)
 //   3. seed zbar_4 -> X
 //   4. reverse sweep l = 3..0:  abar_l = zbar_{l+1} W_l uses the FORWARD weight tile as an MN-major B operand (no transposed
-//      copy, weights resident for the CTA's lifetime); while it runs, a_l / ta_l are rebuilt into Y from the TMEM-resident z_l
+//      copy, weights resident for the CTA's lifetime); while it runs, a_l / ta_l are rebuilt into Y from the stored z_l
 //      (l = 2, 1) or come back by TMA (l = 0); then dW_l += zbar_{l+1}^T a_l: the sample axis is the MMA K dimension and a
 //      K-major operand tile IS an MN-major operand for that product, so X and Y are multiplied as they sit. The four dW
-//      accumulators (M = 64) share 2 x 64 TMEM columns: an M = 64 instruction only writes lanes (m / 16) * 32 + m % 16, so a
-//      second accumulator lives at lane offset 16 of the same columns (validated on B200: tests/test_umma_probe_gpu.py).
+//      accumulators (M = 64) share 2 x 64 columns: an M = 64 product is stored to lanes (m / 16) * 32 + m % 16, so a second
+//      accumulator lives at lane offset 16 of the same columns (tests/test_umma_probe_gpu.py).
 //   5. encoder backward: warp-aggregated red.global.add.v2.f32 into the lattice gradient.
-// TMEM map (512 columns): [0,256) z_1 | tz_1 | z_2 | tz_2, [256,384) work (value | tangent), [384,512) dW_0/dW_1, dW_2/dW_3.
+// Deterministic mode (common.cuh): every gradient (lattice, weights, biases) is summed in fixed point instead and added to the float
+// gradients by the flush that follows the launch.
+// Accumulator map (512 columns): [0,256) z_1 | tz_1 | z_2 | tz_2, [256,384) work (value | tangent), [384,512) dW_0/dW_1, dW_2/dW_3.
 #include <cstdio>
 #include <cstdlib>
 #include "fused_common.cuh"
@@ -45,16 +47,20 @@ constexpr int kBwdThreads = 512;
 constexpr int kGroups = kBwdThreads / kTile;
 constexpr int kSetBytes = 4 * kATileBytes;         // one operand tile set [value hi | value lo | tangent hi | tangent lo]
 constexpr uint32_t kColWork = 256, kColDw = 384;
+__device__ float g_acc_bwd[(size_t)kAccCtas * kTile * 512];     // accumulator areas (umma.cuh)
+constexpr int kFxW = kDetSdfW, kFxB = 4 * kDetSdfW;    // weight / bias offsets in DetBufs::sdf_mlp
 
 struct BwdOut {
     uint8_t* a0_spill;  // [ntiles][64 KB] encoder operand tiles, written and re-read by the same CTA
     float* gW[kNL];     // [N_l, K_l] (+=)
     float* gbias[kNL];  // [N_l]      (+=)
+    unsigned long long* fx_lattice;   // deterministic mode: fixed-point accumulators (DetBufs::sdf_lattice, ::sdf_mlp), else NULL
+    unsigned long long* fx_mlp;
     unsigned long long* phase_cycles;   // [16] += clock64 deltas of thread 0 per phase (PSDF_PHASE_TIMING=1, diagnostics), else NULL
 };
 // Up to kMaxSeg independent sample sets (the main samples, the curvature pass' shifted samples, the off-surface points of one training
-// iteration) are processed by ONE launch: every set starts on a tile boundary; 1024 tiles on 148 SMs lose 1 % to the last partial wave
-// where two launches of 512 tiles lose 13 % each (3.46 -> 4 tile times per CTA).
+// iteration) are processed by ONE launch: every set starts on a tile boundary, so the sets share one last partial wave instead of
+// one each.
 constexpr int kMaxSeg = 3;
 struct Segments {
     int n[kMaxSeg];          // samples of the set
@@ -96,67 +102,36 @@ __device__ __forceinline__ void store_set16(uint8_t* set, int row, int c, const 
     store8(set + 2 * kATileBytes, set + 3 * kATileBytes, row, 2 * c + 1, ta + 8);
 }
 
-// The tcgen05.mma sequences of a phase are issued by several threads: lane 0 of warps 0 / 1 issues the value / tangent stream of the
-// forward and reverse GEMMs, lane 0 of warps 4 / 5 one half of the weight-gradient columns each. Every issuer owns its accumulator
-// columns, the single-thread issue sequences run side by side on different SM sub-partitions, and each issuer commits to the phase's
-// mbarrier (initialised with the issuer count). Streams are NOT split along N: a shared-memory-operand MMA re-reads its whole A tile
-// (128 x 16 bf16 = 4 KB) whatever N is, so narrower MMAs only multiply the A traffic (measured: the colour network, split four ways
-// along N, got 30 % slower).
-__device__ __forceinline__ void split_n(int N, int half, int& n0, int& nn) {      // halves in units of 16 columns (MMA N % 16 == 0)
-    const int na = ((N / 16 + 1) / 2) * 16;
-    n0 = half ? na : 0;
-    nn = half ? N - na : na;
-}
-// columns [n0, n0 + nn) of one stream of  D[128 x Np] = A[128 x Kp] W^T  (A, W K-major)
-__device__ __forceinline__ void issue_forward_part(uint32_t tmem_d, const uint8_t* a_hi, const uint8_t* a_lo, const uint8_t* w_hi,
-                                                   const uint8_t* w_lo, int Kp, int n0, int nn) {
-    if (nn <= 0) return;
-    const uint32_t idesc = umma::make_idesc(128, nn, umma::kFmtBF16);
+// The wgmma sequences of a phase are issued by several warpgroups: warpgroups 0 / 1 issue the value / tangent stream of the forward
+// and reverse GEMMs, warpgroups 2 / 3 one half of the weight-gradient columns each. Every issuer owns its accumulator columns and
+// all its threads arrive on the phase's mbarrier (initialised with the issuers' thread count) once the results are stored.
+// one stream of  abar[128 x Kp] = zbar[128 x Np] W : A = zbar tiles K-major, B = the FORWARD weight tile [Np rows][Kp] read as an
+// MN-major operand (reduction over the rows: 8-row groups are sbo_w apart, the k cores kLBO); both row halves, one warpgroup
+__device__ __forceinline__ void issue_reverse(uint32_t tmem_d, const uint8_t* z_hi, const uint8_t* z_lo, const uint8_t* w_hi,
+                                              const uint8_t* w_lo, int Kp, int Np) {
     const uint32_t sbo_w = (Kp / 8) * kLBO;
-    const uint32_t woff = (n0 / 8) * sbo_w;
-    const uint64_t dah0 = umma::make_desc(umma::smem_u32(a_hi), kLBO, kSBO_A), dal0 = umma::make_desc(umma::smem_u32(a_lo), kLBO, kSBO_A);
-    const uint64_t dwh0 = umma::make_desc(umma::smem_u32(w_hi) + woff, kLBO, sbo_w), dwl0 = umma::make_desc(umma::smem_u32(w_lo) + woff, kLBO, sbo_w);
-    for (int kk = 0; kk < Kp / 16; kk++) {
-        const uint64_t off = (uint64_t)(kk * ((2 * kLBO) >> 4));
-        umma::mma_bf16(tmem_d + n0, dah0 + off, dwh0 + off, idesc, kk > 0 ? 1u : 0u);
-        umma::mma_bf16(tmem_d + n0, dah0 + off, dwl0 + off, idesc, 1u);
-        umma::mma_bf16(tmem_d + n0, dal0 + off, dwh0 + off, idesc, 1u);
-    }
-}
-// columns [n0, n0 + nn) of one stream of  abar[128 x Kp] = zbar[128 x Np] W : A = zbar tiles K-major, B = the FORWARD weight tile
-// [Np rows][Kp] read as an MN-major operand (reduction over the rows: 8-row groups are sbo_w apart, the k cores kLBO)
-__device__ __forceinline__ void issue_reverse_part(uint32_t tmem_d, const uint8_t* z_hi, const uint8_t* z_lo, const uint8_t* w_hi,
-                                                   const uint8_t* w_lo, int Kp, int Np, int n0, int nn) {
-    if (nn <= 0) return;
-    const uint32_t idesc = umma::make_idesc(128, nn, umma::kFmtBF16) | (1u << 16);
-    const uint32_t sbo_w = (Kp / 8) * kLBO;
-    const uint32_t woff = (n0 / 8) * kLBO;
-    const uint64_t dwh0 = umma::make_desc(umma::smem_u32(w_hi) + woff, sbo_w, kLBO), dwl0 = umma::make_desc(umma::smem_u32(w_lo) + woff, sbo_w, kLBO);
-    const uint64_t dzh0 = umma::make_desc(umma::smem_u32(z_hi), kLBO, kSBO_A), dzl0 = umma::make_desc(umma::smem_u32(z_lo), kLBO, kSBO_A);
-    for (int kk = 0; kk < Np / 16; kk++) {
-        const uint64_t oa = (uint64_t)(kk * ((2 * kLBO) >> 4)), ow = (uint64_t)(kk * ((2 * sbo_w) >> 4));
-        umma::mma_bf16(tmem_d + n0, dzh0 + oa, dwh0 + ow, idesc, kk > 0 ? 1u : 0u);
-        umma::mma_bf16(tmem_d + n0, dzh0 + oa, dwl0 + ow, idesc, 1u);
-        umma::mma_bf16(tmem_d + n0, dzl0 + oa, dwh0 + ow, idesc, 1u);
+    const uint64_t dwh = umma::make_desc(umma::smem_u32(w_hi), sbo_w, kLBO), dwl = umma::make_desc(umma::smem_u32(w_lo), sbo_w, kLBO);
+    for (int mh = 0; mh < 2; mh++) {
+        const uint32_t ao = (uint32_t)(mh * 8 * kSBO_A);
+        const uint64_t dzh = umma::make_desc(umma::smem_u32(z_hi) + ao, kLBO, kSBO_A), dzl = umma::make_desc(umma::smem_u32(z_lo) + ao, kLBO, kSBO_A);
+        umma::wg_gemm<0, 1>(tmem_d + ((uint32_t)(64 * mh) << 16), false, dzh, dzl, dwh, dwl, (2 * kLBO) >> 4, (2 * sbo_w) >> 4, (8 * kLBO) >> 4,
+                            Np / 16, Kp, false);
     }
 }
 // columns [n0, n0 + nn) of  dW (+)= zbar^T a + tzbar^T ta : both tile sets consumed as MN-major operands, K = the 128 samples, M = 64
+// (one warpgroup)
 __device__ __forceinline__ void issue_dw_part(uint32_t tmem_d, const uint8_t* zset, const uint8_t* aset, int n0, int nn, bool clear) {
     if (nn <= 0) return;
-    const uint32_t idesc = umma::make_idesc_mn(64, nn, umma::kFmtBF16);
     const uint32_t aoff = (n0 / 8) * kLBO;
 #pragma unroll 1
     for (int s = 0; s < 2; s++) {
-        const uint64_t dzh0 = umma::make_desc(umma::smem_u32(zset + s * 2 * kATileBytes), kSBO_A, kLBO);
-        const uint64_t dzl0 = umma::make_desc(umma::smem_u32(zset + s * 2 * kATileBytes + kATileBytes), kSBO_A, kLBO);
-        const uint64_t dah0 = umma::make_desc(umma::smem_u32(aset + s * 2 * kATileBytes) + aoff, kSBO_A, kLBO);
-        const uint64_t dal0 = umma::make_desc(umma::smem_u32(aset + s * 2 * kATileBytes + kATileBytes) + aoff, kSBO_A, kLBO);
-        for (int kk = 0; kk < kTile / 16; kk++) {
-            const uint64_t o = (uint64_t)(kk * ((2 * kSBO_A) >> 4));          // 16 samples = two 8-sample groups
-            umma::mma_bf16(tmem_d + n0, dzh0 + o, dah0 + o, idesc, (clear && s == 0 && kk == 0) ? 0u : 1u);
-            umma::mma_bf16(tmem_d + n0, dzh0 + o, dal0 + o, idesc, 1u);
-            umma::mma_bf16(tmem_d + n0, dzl0 + o, dah0 + o, idesc, 1u);
-        }
+        const uint64_t dzh = umma::make_desc(umma::smem_u32(zset + s * 2 * kATileBytes), kSBO_A, kLBO);
+        const uint64_t dzl = umma::make_desc(umma::smem_u32(zset + s * 2 * kATileBytes + kATileBytes), kSBO_A, kLBO);
+        const uint64_t dah = umma::make_desc(umma::smem_u32(aset + s * 2 * kATileBytes) + aoff, kSBO_A, kLBO);
+        const uint64_t dal = umma::make_desc(umma::smem_u32(aset + s * 2 * kATileBytes + kATileBytes) + aoff, kSBO_A, kLBO);
+        // 16 samples = two 8-sample groups per K step
+        umma::wg_gemm<1, 1>(tmem_d + n0, true, dzh, dzl, dah, dal, (2 * kSBO_A) >> 4, (2 * kSBO_A) >> 4, (8 * kLBO) >> 4, kTile / 16, nn,
+                            !(clear && s == 0));
     }
 }
 
@@ -169,37 +144,43 @@ k_sdf_fused_backward(FusedParams P, Segments S, const float2* __restrict__ latti
     uint8_t* s_X = smem + P.g.total;
     uint8_t* s_Y = s_X + kSetBytes;
     LevelC* lc = reinterpret_cast<LevelC*>(s_Y + kSetBytes);
-    float* s_gb = reinterpret_cast<float*>(lc + 1);        // 4 x 64 bias-gradient accumulators of this CTA
+    // 4 x 64 bias-gradient accumulators of this CTA: float (s_gbf), or fixed point (s_gb) in deterministic mode
+    unsigned long long* s_gb = reinterpret_cast<unsigned long long*>(lc + 1);
+    float* s_gbf = reinterpret_cast<float*>(s_gb);
+    const bool det = out.fx_mlp != nullptr;
     uint64_t* bars = reinterpret_cast<uint64_t*>(s_gb + kNL * 64);   // [0] TMA loads, [1] mma, [2] dW mma
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 3);
-    float* s_seed = reinterpret_cast<float*>(tmem_slot + 4);   // [128][(out_dim - 1) | 1] upstream d loss / d geom of the tile (coalesced copy)
+    float* s_seed = reinterpret_cast<float*>(bars + 5);   // [128][(out_dim - 1) | 1] upstream d loss / d geom of the tile (coalesced copy)
     float* s_x = reinterpret_cast<float*>(s_X);            // exchange tile abar_0 | tabar_0 : [128][2*Kp0+1] fp32 (aliases X, Y)
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int row = tid & 127, grp = tid >> 7;
     const int level_cores = P.L / 4;
     const int K0 = P.g.Kp[0];
-    const bool gemm_issuer = lane == 0 && warp < 2;        // stream = warp
-    const bool dw_issuer = lane == 0 && (warp == 4 || warp == 5);   // column half = warp - 4
+    const int wgi = warp >> 2;
+    const bool gemm_issuer = wgi < 2;                      // stream = warpgroup
+    const bool dw_issuer = wgi >= 2;                       // column half = warpgroup - 2
 
-    if (tid == 0) { umma::mbar_init(&bars[0], 1); umma::mbar_init(&bars[1], 2); umma::mbar_init(&bars[2], 2); umma::mbar_fence_init(); }
+    if (tid == 0) {
+        umma::mbar_init(&bars[0], 1);
+        umma::mbar_init(&bars[1], 2 * 128);
+        umma::mbar_init(&bars[2], 2 * 128);
+        umma::mbar_fence_init();
+        umma::acc_attach(g_acc_bwd + (size_t)blockIdx.x * kTile * 512, 512);
+    }
     for (int i = tid; i < P.L * 3; i += kBwdThreads) {
         lc->scale[(i / 3) * 4 + (i % 3)] = scale[i];
         lc->shift[(i / 3) * 4 + (i % 3)] = shift ? shift[i] : 0.0f;
     }
     for (int i = tid; i < P.L; i += kBwdThreads) lc->window[i] = window ? window[i] : 1.0f;
-    for (int i = tid; i < kNL * 64; i += kBwdThreads) s_gb[i] = 0.0f;
+    for (int i = tid; i < kNL * 64; i += kBwdThreads) s_gb[i] = 0ull;     // also clears s_gbf
     __syncthreads();
-    if (warp == 0) umma::tmem_alloc(tmem_slot, 512);
     if (tid == 0) {
         umma::mbar_expect_tx(&bars[0], (uint32_t)P.g.total);
         umma::bulk_g2s(s_w, blob, (uint32_t)P.g.total, &bars[0]);
     }
-    umma::fence_before_sync();
     __syncthreads();
-    umma::fence_after_sync();
-    const uint32_t tmem_base = *tmem_slot;
-    const uint32_t tlane = tmem_base + ((uint32_t)((warp & 3) * 32) << 16);     // this warp's 32 TMEM lanes
+    const uint32_t tmem_base = 0;
+    const uint32_t tlane = tmem_base + ((uint32_t)((warp & 3) * 32) << 16);     // this warp's 32 accumulator lanes
     umma::mbar_wait(&bars[0], 0);
     uint32_t ld_phase = 1, mma_phase = 0, dw_phase = 0;
 
@@ -280,28 +261,27 @@ k_sdf_fused_backward(FusedParams P, Segments S, const float2* __restrict__ latti
         }
 
         PSDF_PHASE(kPhEncoder);
-        // ---------------- 2. forward recompute, layers 0..2. z_{l+1} | tz_{l+1} -> TMEM columns l * 128 (l = 0, 1) or the work columns (l = 2)
+        // ---------------- 2. forward recompute, layers 0..2. z_{l+1} | tz_{l+1} -> accumulator columns l * 128 (l = 0, 1) or the work columns (l = 2)
         float g1[16], g2t[16];                 // gelu'(z_3), gelu''(z_3) tz_3 of this thread's chunk: consumed by the first reverse step
         float seed[2][8];                      // upstream gradient columns of this thread (prefetched behind the layer-2 MMAs)
 #pragma unroll 1
         for (int l = 0; l < 3; l++) {
             umma::fence_async_smem();
-            umma::fence_before_sync();
             __syncthreads();
             const uint8_t* at = (l == 1) ? s_Y : s_X;
             uint8_t* dst = (l == 1) ? s_X : s_Y;
             const uint32_t col = (l == 2) ? kColWork : (uint32_t)(l * 128);
             if (gemm_issuer) {
-                umma::fence_after_sync();
                 if (l == 0 && tid == 0) {      // a_0 | ta_0 leave as they are (needed again for dW_0 at the end of the reverse sweep)
                     umma::bulk_s2g(out.a0_spill + (size_t)tile * kSetBytes, s_X, kSetBytes);
                     umma::bulk_commit();
                 }
-                const int s = warp;
-                issue_forward_part(tmem_base + col + s * 64, at + s * 2 * kATileBytes, at + s * 2 * kATileBytes + kATileBytes, s_w + P.g.w_hi[l],
-                                   s_w + P.g.w_lo[l], P.g.Kp[l], 0, P.g.Np[l]);
+                const int s = wgi;
+                for (int mh = 0; mh < 2; mh++)
+                    issue_gemm(tmem_base + col + s * 64, mh, at + s * 2 * kATileBytes, at + s * 2 * kATileBytes + kATileBytes, s_w + P.g.w_hi[l],
+                               s_w + P.g.w_lo[l], P.g.Kp[l], P.g.Np[l]);
                 if (l == 1 && tid == 0) umma::bulk_wait_read0();   // X is overwritten by this layer's epilogue: the store must have read it
-                umma::commit(&bars[1]);
+                umma::mbar_arrive(&bars[1]);
             }
             if (l == 2) {                      // zbar_4 = [g_sdf, g_geom...] columns of this thread, loaded while the MMAs run
                 const int Np = P.g.Np[3], nout = P.g.N[3];
@@ -322,13 +302,11 @@ k_sdf_fused_backward(FusedParams P, Segments S, const float2* __restrict__ latti
             }
             umma::mbar_wait(&bars[1], mma_phase);
             mma_phase ^= 1;
-            umma::fence_after_sync();
             const int c = grp;
             if (c < P.g.Np[l] / 16) {
                 float z[16], tz[16];
                 umma::tmem_ld16(tlane + col + c * 16, z);
                 umma::tmem_ld16(tlane + col + 64 + c * 16, tz);
-                umma::tmem_ld_wait();
                 activations16(z, tz, reinterpret_cast<const float*>(s_w + P.g.bias[l]) + c * 16, g1, g2t);
                 store_set16(dst, row, c, z, tz);
             }
@@ -351,7 +329,10 @@ k_sdf_fused_backward(FusedParams P, Segments S, const float2* __restrict__ latti
                     for (int i = 0; i < 8; i++) { z16[i] = seed[j][i]; z16[i + 8] = 0.f; }
                     int colb;
                     const float cs = colsum16(z16, lane, colb);                       // bias gradient of the output layer
-                    if (!(lane & 1) && colb < 8) atomicAdd(&s_gb[3 * 64 + c * 8 + colb], cs);
+                    if (!(lane & 1) && colb < 8) {
+                        if (det) fx_add(&s_gb[3 * 64 + c * 8 + colb], cs);
+                        else atomicAdd(&s_gbf[3 * 64 + c * 8 + colb], cs);
+                    }
                 }
             }
         }
@@ -361,58 +342,50 @@ k_sdf_fused_backward(FusedParams P, Segments S, const float2* __restrict__ latti
         for (int l = 3; l >= 0; l--) {
             const uint32_t dw_col = tmem_base + kColDw + (uint32_t)(l >> 1) * 64 + ((l & 1) ? (16u << 16) : 0u);
             umma::fence_async_smem();
-            umma::fence_before_sync();
             __syncthreads();
             if (gemm_issuer) {
-                umma::fence_after_sync();
-                const int s = warp;
-                issue_reverse_part(tmem_base + kColWork + s * 64, s_X + s * 2 * kATileBytes, s_X + s * 2 * kATileBytes + kATileBytes,
-                                   s_w + P.g.w_hi[l], s_w + P.g.w_lo[l], P.g.Kp[l], P.g.Np[l], 0, P.g.Kp[l]);
-                umma::commit(&bars[1]);
+                const int s = wgi;
+                issue_reverse(tmem_base + kColWork + s * 64, s_X + s * 2 * kATileBytes, s_X + s * 2 * kATileBytes + kATileBytes,
+                              s_w + P.g.w_hi[l], s_w + P.g.w_lo[l], P.g.Kp[l], P.g.Np[l]);
+                umma::mbar_arrive(&bars[1]);
             }
             if (dw_issuer && (l == 3 || l == 0)) {
                 // l = 3: a_3 | ta_3 are in Y since the forward epilogue; l = 0: a_0 | ta_0 come back by TMA (requested after the
                 // previous step released Y)
-                umma::fence_after_sync();
-                if (l == 0) { umma::mbar_wait(&bars[0], ld_phase); umma::fence_after_sync(); }
+                if (l == 0) umma::mbar_wait(&bars[0], ld_phase);
                 int n0, nn;
-                split_n(P.g.Kp[l], warp - 4, n0, nn);
+                split_n(P.g.Kp[l], wgi - 2, n0, nn);
                 issue_dw_part(dw_col, s_X, s_Y, n0, nn, first_tile);
-                umma::commit(&bars[2]);
+                umma::mbar_arrive(&bars[2]);
             }
             if (l == 1 || l == 2) {
-                // while the reverse MMAs run: rebuild a_l | ta_l -> Y and the GELU' / GELU'' factors from the TMEM-resident z_l, tz_l
+                // beside the reverse MMAs: rebuild a_l | ta_l -> Y and the GELU' / GELU'' factors from the stored z_l, tz_l
                 const int c = grp;
                 if (c < P.g.Kp[l] / 16) {
                     float z[16], tz[16];
                     const uint32_t col = (uint32_t)((l - 1) * 128);
                     umma::tmem_ld16(tlane + col + c * 16, z);
                     umma::tmem_ld16(tlane + col + 64 + c * 16, tz);
-                    umma::tmem_ld_wait();
                     activations16(z, tz, reinterpret_cast<const float*>(s_w + P.g.bias[l - 1]) + c * 16, g1, g2t);
                     store_set16(s_Y, row, c, z, tz);
                 }
                 umma::fence_async_smem();
-                umma::fence_before_sync();
                 __syncthreads();
                 if (dw_issuer) {
-                    umma::fence_after_sync();
                     int n0, nn;
-                    split_n(P.g.Kp[l], warp - 4, n0, nn);
+                    split_n(P.g.Kp[l], wgi - 2, n0, nn);
                     issue_dw_part(dw_col, s_X, s_Y, n0, nn, first_tile);
-                    umma::commit(&bars[2]);
+                    umma::mbar_arrive(&bars[2]);
                 }
             }
             umma::mbar_wait(&bars[1], mma_phase);
             mma_phase ^= 1;
-            umma::fence_after_sync();
             const int c = grp;
             const bool have = c < P.g.Kp[l] / 16;
             float ab[16], tab_[16];
             if (have) {
                 umma::tmem_ld16(tlane + kColWork + c * 16, ab);
                 umma::tmem_ld16(tlane + kColWork + 64 + c * 16, tab_);
-                umma::tmem_ld_wait();
                 if (l > 0) {
 #pragma unroll
                     for (int i = 0; i < 16; i++) {
@@ -425,7 +398,6 @@ k_sdf_fused_backward(FusedParams P, Segments S, const float2* __restrict__ latti
             // X and Y are still operands of the weight-gradient MMAs
             umma::mbar_wait(&bars[2], dw_phase);
             dw_phase ^= 1;
-            umma::fence_after_sync();
             if (l == 1 && tid == 0) {          // Y is free: bring a_0 | ta_0 back for the last step (the store completed long ago)
                 umma::bulk_wait0();
                 umma::mbar_expect_tx(&bars[0], (uint32_t)kSetBytes);
@@ -440,7 +412,10 @@ k_sdf_fused_backward(FusedParams P, Segments S, const float2* __restrict__ latti
                     }
                     int colb;
                     const float cs = colsum16(ab, lane, colb);       // bias gradient: column sums over the warp's 32 rows
-                    if (!(lane & 1)) atomicAdd(&s_gb[(l - 1) * 64 + c * 16 + colb], cs);
+                    if (!(lane & 1)) {
+                        if (det) fx_add(&s_gb[(l - 1) * 64 + c * 16 + colb], cs);
+                        else atomicAdd(&s_gbf[(l - 1) * 64 + c * 16 + colb], cs);
+                    }
                 }
             } else {
                 // abar_0 | tabar_0 for the encoder backward (fp32 exchange tile over X and Y, which no MMA reads any more)
@@ -455,7 +430,6 @@ k_sdf_fused_backward(FusedParams P, Segments S, const float2* __restrict__ latti
             PSDF_PHASE(kPhReverse3 + (3 - l));
         }
         ld_phase ^= 1;
-        umma::fence_before_sync();
         __syncthreads();
 
         // ---------------- 5. encoder backward: lattice[l][idx_r] += window_l (B_r abar_0[l] + dB_r tabar_0[l])
@@ -476,6 +450,7 @@ k_sdf_fused_backward(FusedParams P, Segments S, const float2* __restrict__ latti
                 const float w = lc->window[l];
                 const float a0 = xr[2 * l], a1 = xr[2 * l + 1], t0 = xr[K0 + 2 * l], t1 = xr[K0 + 2 * l + 1];
                 float* gtab = grad_lattice + (size_t)l * P.T * 2;
+                unsigned long long* ftab = det ? out.fx_lattice + (size_t)l * P.T * 2 : nullptr;
                 const bool aggregate = lc->scale[l * 4] < kAggregateBelowScale && !(P.knockout & 2);       // warp-uniform (l is)
                 const bool do_red = !(P.knockout & 1);            // diagnostics (PSDF_EXPERIMENT_KNOCKOUT): bit 0 no atomics, bit 1 no aggregation
 #pragma unroll
@@ -487,30 +462,32 @@ k_sdf_fused_backward(FusedParams P, Segments S, const float2* __restrict__ latti
                         unsigned key = valid ? idx : 0xffffffffu;
                         unsigned peers = __match_any_sync(kFull, key);
                         cv = add_peers2(peers, cv, lane);
-                        if (valid && lane == __ffs(peers) - 1 && do_red) red_v2(gtab + (size_t)idx * 2, cv);
+                        if (valid && lane == __ffs(peers) - 1 && do_red) scatter2(gtab, ftab, idx, cv);
                     } else if (valid && (do_red || cv.x == 123.456f)) {
-                        red_v2(gtab + (size_t)idx * 2, cv);
+                        scatter2(gtab, ftab, idx, cv);
                     }
                 }
             }
         }
-        umma::fence_before_sync();
-        __syncthreads();     // exchange tile / TMEM free for the next tile
+        __syncthreads();     // exchange tile / accumulators free for the next tile
         PSDF_PHASE(kPhEncoderBwd);
         if (out.phase_cycles && tid == 0) atomicAdd(out.phase_cycles + kPhTiles, 1ull);
     }
-    // ---------------- weight gradients of this CTA: TMEM -> global (+=). Warp w reads lanes 32 (w & 3) .. +31 of column chunk w >> 2:
+    // ---------------- weight gradients of this CTA: accumulators -> global (+=). Warp w reads lanes 32 (w & 3) .. +31 of column chunk w >> 2:
     // lanes 0..15 hold rows 16 (w & 3) + lane of the even layer of the pair, lanes 16..31 the same rows of the odd layer
-    umma::fence_after_sync();
     if (!first_tile) {
         const int q = warp & 3, c = warp >> 2;
 #pragma unroll 1
         for (int p = 0; p < 2; p++) {
             float acc[16];
             umma::tmem_ld16(tlane + kColDw + p * 64 + c * 16, acc);
-            umma::tmem_ld_wait();
             const int l = 2 * p + (lane >> 4), m = q * 16 + (lane & 15);
-            if (m < P.g.N[l]) {
+            if (m < P.g.N[l] && det) {
+                const int K = P.g.K[l];
+                unsigned long long* dst = out.fx_mlp + l * kFxW + m * K;
+#pragma unroll
+                for (int i = 0; i < 16; i++) if (c * 16 + i < K) fx_add(dst + c * 16 + i, acc[i]);
+            } else if (m < P.g.N[l]) {
                 const int K = P.g.K[l];
                 float* dst = out.gW[l] + (size_t)m * K + c * 16;
                 const bool vec = (K & 3) == 0 && ((uintptr_t)out.gW[l] & 15) == 0;      // rows stay 16-byte aligned
@@ -528,13 +505,11 @@ k_sdf_fused_backward(FusedParams P, Segments S, const float2* __restrict__ latti
     }
     for (int i = tid; i < kNL * 64; i += kBwdThreads) {
         int l = i >> 6, c = i & 63;
-        if (c < P.g.N[l] && s_gb[i] != 0.0f) atomicAdd(out.gbias[l] + c, s_gb[i]);
+        if (det) { if (c < P.g.N[l] && s_gb[i] != 0ull) atomicAdd(out.fx_mlp + kFxB + l * 64 + c, s_gb[i]); }
+        else if (c < P.g.N[l] && s_gbf[i] != 0.0f) atomicAdd(out.gbias[l] + c, s_gbf[i]);
     }
     PSDF_PHASE(kPhFlush);
     if (tid == 0) umma::bulk_wait0();      // spill stores complete before the CTA retires
-    umma::fence_before_sync();
-    __syncthreads();
-    if (warp == 0) umma::tmem_dealloc(tmem_base, 512);
 }
 
 #define ST ((cudaStream_t)stream)
@@ -577,8 +552,12 @@ static int launch_backward(int nseg, const int* Ns, const float* const* pos, con
     S.tile0[kMaxSeg] = tiles;
     P.N = total;
     if (tiles == 0) return PSDF_OK;
+    const DetBufs* dbuf = det_buffers();
+    if (dbuf && (long long)L * T * 2 > dbuf->lattice_len) return PSDF_ERR_UNSUPPORTED;   // reserve more with psdf_set_deterministic
     BwdOut out;
     for (int l = 0; l < kNL; l++) { out.gW[l] = gW[l]; out.gbias[l] = gb[l]; }
+    out.fx_lattice = dbuf ? dbuf->sdf_lattice : nullptr;
+    out.fx_mlp = dbuf ? dbuf->sdf_mlp : nullptr;
     out.a0_spill = workspace;
     // diagnostics: PSDF_PHASE_TIMING=1 prints thread 0's clock64 breakdown per phase (average cycles per tile) after every launch
     static const bool timing = getenv("PSDF_PHASE_TIMING") && atoi(getenv("PSDF_PHASE_TIMING")) != 0;
@@ -589,15 +568,24 @@ static int launch_backward(int nseg, const int* Ns, const float* const* pos, con
         cudaMemsetAsync(d_cycles, 0, 16 * sizeof(unsigned long long), ST);
         out.phase_cycles = d_cycles;
     }
-    int dev = 0, sms = 148;
+    int dev = 0, sms = 132;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    const size_t smem = (size_t)P.g.total + 2 * kSetBytes + sizeof(LevelC) + kNL * 64 * sizeof(float) + 64 + (size_t)kTile * (size_t)((out_dim - 1) | 1) * sizeof(float);
+    const size_t smem = (size_t)P.g.total + 2 * kSetBytes + sizeof(LevelC) + kNL * 64 * sizeof(unsigned long long) + 64 + (size_t)kTile * (size_t)((out_dim - 1) | 1) * sizeof(float);
     if ((size_t)128 * (2 * P.g.Kp[0] + 1) * 4 > (size_t)2 * kSetBytes || smem > 227 * 1024) return PSDF_ERR_UNSUPPORTED;
     { static bool optin_[64]; psdf::psdf_optin_smem(k_sdf_fused_backward, 227 * 1024, optin_); }
-    k_sdf_fused_backward<<<min(tiles, sms), kBwdThreads, smem, ST>>>(P, S, reinterpret_cast<const float2*>(lattice), scale_factor, shift, window,
+    k_sdf_fused_backward<<<min(min(tiles, sms), kAccCtas), kBwdThreads, smem, ST>>>(P, S, reinterpret_cast<const float2*>(lattice), scale_factor, shift, window,
                                                                     blob, grad_lattice, out);
     PSDF_CHECK_LAUNCH();
+    if (dbuf) {      // deterministic mode: fixed-point totals -> the float gradients (+=)
+        FxSegs F;
+        F.add(dbuf->sdf_lattice, grad_lattice, (long long)L * T * 2);
+        for (int l = 0; l < kNL; l++) {
+            F.add(dbuf->sdf_mlp + l * kFxW, gW[l], (long long)P.g.N[l] * P.g.K[l]);
+            F.add(dbuf->sdf_mlp + kFxB + l * 64, gb[l], P.g.N[l]);
+        }
+        if (fx_flush(F, ST) != 0) return PSDF_ERR_LAUNCH;
+    }
     if (timing) {
         unsigned long long h[16];
         cudaMemcpyAsync(h, d_cycles, sizeof(h), cudaMemcpyDeviceToHost, ST);

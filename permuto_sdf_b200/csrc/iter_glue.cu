@@ -1,4 +1,4 @@
-// Glue of the direct (autograd-free) training iteration (train.py Trainer._iteration_direct), sm_100a. Each kernel replaces a chain of
+// Glue of the direct (autograd-free) training iteration (train.py Trainer._iteration_direct), sm_90a. Each kernel replaces a chain of
 // one-block PyTorch launches that the autograd formulation of train_permuto_sdf.py:311-422 spends between the big kernels:
 //   k_iter_scalars      schedule ramps evaluated from the device-resident iteration number (map_range_val, common_utils.py:156-160) and
 //                       inv_s = exp(10 * forced_variance) (SingleVarianceNetwork, volume_rendering_modules.py:94-114)             1 launch for ~12
@@ -82,6 +82,7 @@ k_lipschitz_pack(MlpGeom g, Lip4 A, uint8_t* __restrict__ blob) {
 }
 
 struct Lip4Bwd {
+    unsigned long long* fx;          // deterministic mode: DetBufs::lip (d loss / d c_l in fixed point), else NULL
     const float* W[kNL];
     const float* c[kNL];
     float* G[kNL];        // d loss / d W_eff (read, then reset to zero for the next iteration)
@@ -101,7 +102,8 @@ k_lipschitz_bwd4(Lip4Bwd A) {
     if (r == 0 && lane == 0 && A.lip_weight != 0.0f) {
         float prod = A.lip_weight;
         for (int q = 0; q < kNL; q++) if (q != l) prod *= softplus_f(A.c[q][0]);
-        atomicAdd(A.gc[l], prod * sigmoid_sp(A.c[l][0]));
+        if (A.fx) fx_add(A.fx + l, prod * sigmoid_sp(A.c[l][0]));
+        else atomicAdd(A.gc[l], prod * sigmoid_sp(A.c[l][0]));
     }
     if (r >= rows) return;
     const float* W = A.W[l] + (size_t)r * cols;
@@ -126,11 +128,15 @@ k_lipschitz_bwd4(Lip4Bwd A) {
         gW[j] += G[j] * s - k * sg;
         G[j] = 0.0f;
     }
-    if (lane == 0 && active) atomicAdd(A.gc[l], d / a * sigmoid_sp(cv));
+    if (lane == 0 && active) {
+        if (A.fx) fx_add(A.fx + l, d / a * sigmoid_sp(cv));
+        else atomicAdd(A.gc[l], d / a * sigmoid_sp(cv));
+    }
 }
 
 // ---------------------------------------------------------------------------------------------- loss terms
 struct LossArgs {
+    unsigned long long* fx;          // deterministic mode: DetBufs::loss (the sums in fixed point), else NULL
     int N;                           // rows of the sample buffers
     const int* nr_valid_dev;         // [1] valid rows (static-capacity containers) or NULL (all N)
     const int* nr_mean_dev;          // [1] divisor of the per-sample means (data-parallel: mean per-rank count) or NULL (= valid rows)
@@ -185,7 +191,10 @@ k_loss_terms(LossArgs A) {
     if (threadIdx.x < 5) {
         float s = 0.f;
         for (int w = 0; w < kThreads / 32; w++) s += red[threadIdx.x][w];
-        if (s != 0.0f) atomicAdd(A.acc + threadIdx.x, s);
+        if (s != 0.0f) {
+            if (A.fx) fx_add(A.fx + threadIdx.x, s);
+            else atomicAdd(A.acc + threadIdx.x, s);
+        }
     }
     __threadfence();
     __syncthreads();
@@ -196,8 +205,15 @@ k_loss_terms(LossArgs A) {
     __syncthreads();
     if (!last || threadIdx.x != 0) return;
     __threadfence();
-    volatile float* acc = A.acc;
-    const float l1 = acc[0], bce = acc[1], eik = acc[2], curv = acc[3], off = acc[4];
+    float sums[5];
+    if (A.fx) {
+        volatile unsigned long long* fx = A.fx;
+        for (int q = 0; q < 5; q++) { sums[q] = (float)((double)(long long)fx[q] / kFxScale); fx[q] = 0ull; }
+    } else {
+        volatile float* acc = A.acc;
+        for (int q = 0; q < 5; q++) sums[q] = acc[q];
+    }
+    const float l1 = sums[0], bce = sums[1], eik = sums[2], curv = sums[3], off = sums[4];
     const int cnt = max(A.nr_mean_dev ? A.nr_mean_dev[0] : nv, 1);
     const float curv_mean = curv / (float)cnt;
     const float off_mean = A.sdf_off ? off / (float)A.n_off : 0.0f;
@@ -278,14 +294,7 @@ k_adamw_multi(AdamGroups A, float beta1, float beta2, float eps, const int* __re
             const float step_size = lr / bias_c1;
             float* pp = &P[q].x; float* gg = &G[q].x; float* mm = &M[q].x; float* vv = &V[q].x;
 #pragma unroll
-            for (int k = 0; k < 4; k++) {
-                float gr = gg[k] * grad_scale;
-                float pk = pp[k] * decay;
-                mm[k] = beta1 * mm[k] + (1.0f - beta1) * gr;
-                vv[k] = beta2 * vv[k] + (1.0f - beta2) * gr * gr;
-                float denom = sqrtf(vv[k]) / bias_c2_sqrt + eps;
-                pp[k] = pk - step_size * (mm[k] / denom);
-            }
+            for (int k = 0; k < 4; k++) adamw_update(pp[k], mm[k], vv[k], gg[k], grad_scale, decay, step_size, beta1, beta2, bias_c2_sqrt, eps);
             reinterpret_cast<float4*>(A.p[gi[q]])[j[q]] = P[q];
             reinterpret_cast<float4*>(A.m[gi[q]])[j[q]] = M[q];
             reinterpret_cast<float4*>(A.v[gi[q]])[j[q]] = V[q];
@@ -342,6 +351,8 @@ int psdf_lipschitz_backward4(int in_dim, int h1, int h2, int h3, int out_dim, co
                              float* gW2, float* gc2, const float* W3, const float* c3, float* G3, float* gW3, float* gc3, float lip_weight,
                              void* stream) {
     Lip4Bwd A;
+    const DetBufs* dbuf = det_buffers();
+    A.fx = dbuf ? dbuf->lip : nullptr;
     const int dims[kNL + 1] = {in_dim, h1, h2, h3, out_dim};
     A.W[0] = W0; A.W[1] = W1; A.W[2] = W2; A.W[3] = W3;
     A.c[0] = c0; A.c[1] = c1; A.c[2] = c2; A.c[3] = c3;
@@ -354,6 +365,11 @@ int psdf_lipschitz_backward4(int in_dim, int h1, int h2, int h3, int out_dim, co
     dim3 grid(div_up(max_rows * 32, kThreads), kNL);
     k_lipschitz_bwd4<<<grid, kThreads, 0, ST>>>(A);
     PSDF_CHECK_LAUNCH();
+    if (dbuf) {      // deterministic mode: fixed-point totals -> the float gradients (+=)
+        FxSegs F;
+        for (int l = 0; l < kNL; l++) F.add(dbuf->lip + l, A.gc[l], 1);
+        if (fx_flush(F, ST) != 0) return PSDF_ERR_LAUNCH;
+    }
     return PSDF_OK;
 }
 
@@ -370,6 +386,8 @@ int psdf_loss_terms(int N, const int* nr_valid_dev, const int* nr_mean_dev, cons
                     const float* lip_c3, float* acc, float* loss, float* terms, void* stream) {
     if (N < 0 || R < 0 || n_off < 0 || !acc || !loss || !terms || (sdf_off && !g_off)) return PSDF_ERR_ARG;
     LossArgs A;
+    const DetBufs* dbuf = det_buffers();
+    A.fx = dbuf ? dbuf->loss : nullptr;
     A.N = N; A.nr_valid_dev = nr_valid_dev; A.nr_mean_dev = nr_mean_dev; A.g = grad; A.gs = grad_shifted; A.R = R; A.ray_loss = ray_loss;
     A.n_off = sdf_off ? n_off : 0; A.sdf_off = sdf_off; A.g_off = g_off;
     A.c_rgb = c_rgb; A.c_mask = c_mask; A.w_eik = w_eik; A.w_curv = w_curv; A.w_off = w_off; A.w_lip = w_lip; A.w_curv_dev = w_curv_dev;
@@ -408,14 +426,14 @@ int psdf_adamw_multi_step(int n_groups, const long long* n, const uint64_t* para
     }
     A.off4[n_groups] = off;
     if (off == 0) return PSDF_OK;
-    int dev = 0, sms = 148;
+    int dev = 0, sms = 132;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    // Persistent grid-stride blocks. leave_room = 0: 8 blocks of 256 threads per SM, 2 float4 quadruples in flight per thread (104 us for
-    // the 16.9 M parameters of the bench, 72 % of the measured copy peak). leave_room != 0: 2 blocks per SM with 4 quadruples in flight
-    // (136 us alone) -- most of the register file stays free, so that the next iteration's ray generation / occupancy sampling kernels,
-    // replayed on another stream while this sweep runs (Trainer._step_graphed), are co-resident instead of waiting for the sweep to drain:
-    // measured 1.215 vs 1.24-1.26 ms per iteration (profiles/README.md; 3 or 4 blocks per SM and a high-priority stream are worse).
+    // Persistent grid-stride blocks. leave_room = 0: 8 blocks of 256 threads per SM, 2 float4 quadruples in flight per thread (the
+    // fastest sweep on its own). leave_room != 0: 2 blocks per SM with 4 quadruples in flight -- most of the register file stays free, so
+    // that the next iteration's ray generation / occupancy sampling kernels, replayed on another stream while this sweep runs
+    // (Trainer._step_graphed), are co-resident instead of waiting for the sweep to drain. PSDF_ADAMW_BLOCKS_PER_SM / PSDF_ADAMW_UNROLL
+    // override both for measurements.
     static const int per_sm_env = getenv("PSDF_ADAMW_BLOCKS_PER_SM") ? atoi(getenv("PSDF_ADAMW_BLOCKS_PER_SM")) : 0;
     static const int unroll_env = getenv("PSDF_ADAMW_UNROLL") ? atoi(getenv("PSDF_ADAMW_UNROLL")) : 0;
     const int per_sm = per_sm_env > 0 ? per_sm_env : (leave_room ? 2 : 8);

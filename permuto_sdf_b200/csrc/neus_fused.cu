@@ -1,4 +1,4 @@
-// Fused NeuS compositing + per-ray losses for training (sm_100a), forward and backward, one warp per ray.
+// Fused NeuS compositing + per-ray losses for training (sm_90a), forward and backward, one warp per ray.
 //
 // Replaces, in one kernel each way, what the reference runs as ~60 PyTorch element-wise launches plus 8 of its own
 // kernels per iteration (volume_rendering_modules.py:129-176 `VolumeRenderingNeus.compute_weights` + `integrate`,
@@ -31,6 +31,7 @@ __device__ __forceinline__ float sigmoidf_(float x) { return 1.0f / (1.0f + __ex
 //  * tail: rows [nr_samples_dev[0], n_rows) of the gradient buffers are zero-filled by extra blocks (static-capacity containers),
 //    so that the caller needs no memset.
 struct NeusExt {
+    unsigned long long* fx;         // deterministic mode: DetBufs::neus (calibration and inv_s gradients in fixed point), else NULL
     int head;                       // 1: rgb is the raw network output
     const int* img_idx;             // [R] or NULL
     const float* weight_delta;      // [nr_imgs,3]
@@ -297,13 +298,17 @@ k_neus_backward(int nr_rays, int max_nr_samples, const int* __restrict__ start_e
             float sw = hgw[c], sb = hgb[c];
 #pragma unroll
             for (int o = 16; o > 0; o >>= 1) { sw += __shfl_xor_sync(kFull, sw, o); sb += __shfl_xor_sync(kFull, sb, o); }
-            if (lane == 0) { atomicAdd(ext.g_weight_delta + 3 * him + c, sw); atomicAdd(ext.g_bias + 3 * him + c, sb); }
+            if (lane == 0 && ext.fx && him < kDetImages) { fx_add(ext.fx + 3 * him + c, sw); fx_add(ext.fx + 3 * kDetImages + 3 * him + c, sb); }
+            else if (lane == 0) { atomicAdd(ext.g_weight_delta + 3 * him + c, sw); atomicAdd(ext.g_bias + 3 * him + c, sb); }
         }
     }
     if (g_inv_s) {
 #pragma unroll
         for (int o = 16; o > 0; o >>= 1) gs_acc += __shfl_xor_sync(kFull, gs_acc, o);
-        if (lane == 0 && s_active && gs_acc != 0.0f) atomicAdd(g_inv_s, gs_acc);
+        if (lane == 0 && s_active && gs_acc != 0.0f) {
+            if (ext.fx) fx_add(ext.fx + 6 * kDetImages, gs_acc);
+            else atomicAdd(g_inv_s, gs_acc);
+        }
     }
 }
 #define ST ((cudaStream_t)stream)
@@ -333,16 +338,30 @@ static int neus_backward_impl(int nr_rays, int max_nr_samples, const int* ray_st
     if (nr_rays <= 0) return nr_rays == 0 ? PSDF_OK : PSDF_ERR_ARG;
     const int rb = ray_blocks(nr_rays);
     ext.ray_blocks = rb;
-    const int tail_blocks = ext.n_rows > 0 ? min(div_up(ext.n_rows, kThreads), 148) : 0;
+    const DetBufs* dbuf = det_buffers();
+    ext.fx = dbuf ? dbuf->neus : nullptr;
+    const int tail_blocks = ext.n_rows > 0 ? min(div_up(ext.n_rows, kThreads), 132) : 0;
     k_neus_backward<<<rb + tail_blocks, kThreads, 0, ST>>>(nr_rays, max_nr_samples, ray_start_end, equal != 0, fixed_n, sdf, grad, rgb, dirs, dt,
                                                           inv_s_dev, cos_anneal_ratio, cos_anneal_dev, gt_rgb, gt_mask, hit, bg_rgb, alpha,
                                                           transmittance, pred_rgb, weights_sum, bg_transmittance, g_total_dev, scale_rgb,
                                                           scale_mask, scale_eik, nr_samples_dev, g_sdf, g_grad, g_rgb, g_bg_rgb, g_inv_s, ext);
     PSDF_CHECK_LAUNCH();
+    if (dbuf) {
+        // deterministic mode: fixed-point totals -> the float gradients (+=); entries of images the buffers do not have stay zero and
+        // are never written
+        FxSegs F;
+        if (ext.head) {
+            F.add(dbuf->neus, ext.g_weight_delta, 3 * kDetImages);
+            F.add(dbuf->neus + 3 * kDetImages, ext.g_bias, 3 * kDetImages);
+        }
+        F.add(dbuf->neus + 6 * kDetImages, g_inv_s, 1);
+        if (fx_flush(F, ST) != 0) return PSDF_ERR_LAUNCH;
+    }
     return PSDF_OK;
 }
 static NeusExt no_ext() {
     NeusExt e;
+    e.fx = nullptr;
     e.head = 0; e.img_idx = nullptr; e.weight_delta = nullptr; e.bias = nullptr; e.fixed_img = -1; e.g_weight_delta = nullptr; e.g_bias = nullptr;
     e.gs = nullptr; e.ggs = nullptr; e.curv_scale = 0.f; e.curv_scale_dev = nullptr; e.n_rows = 0; e.ray_blocks = 0; e.nr_valid_dev = nullptr;
     return e;

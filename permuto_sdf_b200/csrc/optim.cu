@@ -1,4 +1,4 @@
-// Dense fused AdamW sweep for the hash tables and MLP parameters (sm_100a).
+// Dense fused AdamW sweep for the hash tables and MLP parameters (sm_90a).
 // One pass over {param, grad, exp_avg, exp_avg_sq}: 28 B/parameter (read 16, write 12), optional gradient
 // zeroing folded in (+4 B) so that no separate zero_grad memset is needed. Math = torch.optim.AdamW /
 // apex FusedAdam as used by the reference (train_permuto_sdf.py:293-304: betas (0.9, 0.99), eps 1e-15,
@@ -42,14 +42,7 @@ k_adamw(long long n, float* __restrict__ p, float* __restrict__ g, float* __rest
             if (q == 1 && !two) break;
             float* pp = &P[q].x; float* gg = &G[q].x; float* mm = &M[q].x; float* vv = &V[q].x;
 #pragma unroll
-            for (int k = 0; k < 4; k++) {
-                float gr = gg[k] * grad_scale;
-                float pk = pp[k] * decay;
-                mm[k] = beta1 * mm[k] + (1.0f - beta1) * gr;
-                vv[k] = beta2 * vv[k] + (1.0f - beta2) * gr * gr;
-                float denom = sqrtf(vv[k]) / bias_c2_sqrt + eps;
-                pp[k] = pk - step_size * (mm[k] / denom);
-            }
+            for (int k = 0; k < 4; k++) adamw_update(pp[k], mm[k], vv[k], gg[k], grad_scale, decay, step_size, beta1, beta2, bias_c2_sqrt, eps);
             const long long i = q ? i1 : i0;
             reinterpret_cast<float4*>(p)[i] = P[q];
             reinterpret_cast<float4*>(m)[i] = M[q];
@@ -60,12 +53,9 @@ k_adamw(long long n, float* __restrict__ p, float* __restrict__ g, float* __rest
     // tail
     if (blockIdx.x == 0 && threadIdx.x < (n & 3)) {
         long long i = (n4 << 2) + threadIdx.x;
-        float gr = g[i] * grad_scale;
-        float pk = p[i] * decay;
-        float mk = beta1 * m[i] + (1.0f - beta1) * gr;
-        float vk = beta2 * v[i] + (1.0f - beta2) * gr * gr;
-        m[i] = mk; v[i] = vk;
-        p[i] = pk - step_size * (mk / (sqrtf(vk) / bias_c2_sqrt + eps));
+        float pk = p[i], mk = m[i], vk = v[i];
+        adamw_update(pk, mk, vk, g[i], grad_scale, decay, step_size, beta1, beta2, bias_c2_sqrt, eps);
+        p[i] = pk; m[i] = mk; v[i] = vk;
         if (zero_grad) g[i] = 0.f;
     }
 }
@@ -136,13 +126,7 @@ k_adamw_dp(long long n, int rank, PeerPtrs grads, PeerPtrs params, float* __rest
             const long long i = i0 + u * stride;
             float* pp = &P[u].x; float* gg = &G[u].x; float* mm = &M[u].x; float* vv = &V[u].x;
 #pragma unroll
-            for (int k = 0; k < 4; k++) {
-                const float gr = gg[k] * grad_scale;
-                const float pk = pp[k] * decay;
-                mm[k] = beta1 * mm[k] + (1.0f - beta1) * gr;
-                vv[k] = beta2 * vv[k] + (1.0f - beta2) * gr * gr;
-                pp[k] = pk - step_size * (mm[k] / (sqrtf(vv[k]) / bias_c2_sqrt + eps));
-            }
+            for (int k = 0; k < 4; k++) adamw_update(pp[k], mm[k], vv[k], gg[k], grad_scale, decay, step_size, beta1, beta2, bias_c2_sqrt, eps);
             reinterpret_cast<float4*>(m)[i] = M[u];
             reinterpret_cast<float4*>(v)[i] = V[u];
             if (MC) mc_st(mc_param + 4 * i, P[u]);
@@ -156,7 +140,50 @@ k_adamw_dp(long long n, int rank, PeerPtrs grads, PeerPtrs params, float* __rest
 #define ST ((cudaStream_t)stream)
 }  // namespace
 
+// ---------------------------------------------------------------------------------------------- deterministic mode (common.cuh)
+static psdf::DetBufs g_det[64];
+static bool g_det_on[64];
+namespace psdf {
+const DetBufs* det_buffers() {
+    int dev = 0;
+    cudaGetDevice(&dev);
+    return (dev >= 0 && dev < 64 && g_det_on[dev]) ? &g_det[dev] : nullptr;
+}
+}  // namespace psdf
+
 extern "C" {
+// Switch the training path's gradient reductions (and random occupancy updates) of the current device between float atomics (on = 0,
+// the default) and the order-independent fixed-point sums of common.cuh (on = 1), whose results are the same in every run.
+// lattice_entries = the largest L * T * F of a backward call, voxels = the largest occupancy grid. Allocates / frees device memory:
+// call it outside CUDA-graph capture, with no launch of this library in flight.
+int psdf_set_deterministic(int on, long long lattice_entries, long long voxels) {
+    int dev = 0;
+    cudaGetDevice(&dev);
+    if (dev < 0 || dev >= 64 || lattice_entries < 0 || voxels < 0) return PSDF_ERR_ARG;
+    DetBufs& d = g_det[dev];
+    if (g_det_on[dev]) {
+        cudaFree(d.sdf_lattice); cudaFree(d.sdf_mlp); cudaFree(d.rgb_lattice); cudaFree(d.rgb_mlp); cudaFree(d.neus); cudaFree(d.lip);
+        cudaFree(d.loss); cudaFree(d.winner);
+        g_det_on[dev] = false;
+    }
+    if (!on) return PSDF_OK;
+    typedef unsigned long long U;
+    const long long n_sdf = 4LL * kDetSdfW + 4 * 64, n_rgb = 4LL * kDetRgbW + 4 * 128, n_neus = 6LL * kDetImages + 1;
+    const long long lat = lattice_entries > 0 ? lattice_entries : 1, vox = voxels > 0 ? voxels : 1;
+    bool ok = cudaMalloc(&d.sdf_lattice, lat * sizeof(U)) == cudaSuccess && cudaMalloc(&d.rgb_lattice, lat * sizeof(U)) == cudaSuccess &&
+              cudaMalloc(&d.sdf_mlp, n_sdf * sizeof(U)) == cudaSuccess && cudaMalloc(&d.rgb_mlp, n_rgb * sizeof(U)) == cudaSuccess &&
+              cudaMalloc(&d.neus, n_neus * sizeof(U)) == cudaSuccess && cudaMalloc(&d.lip, 4 * sizeof(U)) == cudaSuccess &&
+              cudaMalloc(&d.loss, 5 * sizeof(U)) == cudaSuccess && cudaMalloc(&d.winner, vox * sizeof(int)) == cudaSuccess;
+    ok = ok && cudaMemset(d.sdf_lattice, 0, lat * sizeof(U)) == cudaSuccess && cudaMemset(d.rgb_lattice, 0, lat * sizeof(U)) == cudaSuccess &&
+         cudaMemset(d.sdf_mlp, 0, n_sdf * sizeof(U)) == cudaSuccess && cudaMemset(d.rgb_mlp, 0, n_rgb * sizeof(U)) == cudaSuccess &&
+         cudaMemset(d.neus, 0, n_neus * sizeof(U)) == cudaSuccess && cudaMemset(d.lip, 0, 4 * sizeof(U)) == cudaSuccess &&
+         cudaMemset(d.loss, 0, 5 * sizeof(U)) == cudaSuccess && cudaMemset(d.winner, 0, vox * sizeof(int)) == cudaSuccess &&
+         cudaDeviceSynchronize() == cudaSuccess;
+    if (!ok) { cudaGetLastError(); return PSDF_ERR_LAUNCH; }
+    d.lattice_len = lattice_entries; d.voxels = voxels;
+    g_det_on[dev] = true;
+    return PSDF_OK;
+}
 // step >= 1 is the (already incremented) step count, read from step_dev[0] instead when that is not NULL; pointers 16-byte aligned
 int psdf_adamw_step(long long n, float* param, float* grad, float* exp_avg, float* exp_avg_sq, float lr, float beta1, float beta2,
                     float eps, float weight_decay, int step, const int* step_dev, const float* hyper_dev, float grad_scale, int zero_grad,
@@ -167,7 +194,7 @@ int psdf_adamw_step(long long n, float* param, float* grad, float* exp_avg, floa
     if ((((uintptr_t)param | (uintptr_t)grad | (uintptr_t)exp_avg | (uintptr_t)exp_avg_sq) & 15) != 0) return PSDF_ERR_ARG;
     double c1 = 1.0 - pow((double)beta1, (double)step);
     double c2 = 1.0 - pow((double)beta2, (double)step);
-    int dev = 0, sms = 148;
+    int dev = 0, sms = 132;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     long long n4 = n >> 2;
@@ -202,7 +229,7 @@ int psdf_adamw_dp_step(long long n, long long shard_lo, int world, int rank, con
     float* mcg = mc ? reinterpret_cast<float*>((uintptr_t)mc_grad_ptr) + shard_lo : nullptr;
     float* mcp = mc ? reinterpret_cast<float*>((uintptr_t)mc_param_ptr) + shard_lo : nullptr;
     const double c1 = 1.0 - pow((double)beta1, (double)step), c2 = 1.0 - pow((double)beta2, (double)step);
-    int dev = 0, sms = 148;
+    int dev = 0, sms = 132;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     const long long n4 = n >> 2;

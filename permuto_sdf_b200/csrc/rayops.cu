@@ -1,9 +1,9 @@
-// Ray-path kernels for sm_100a: bounding sphere, occupancy grid (Morton DDA), packed sample
+// Ray-path kernels for sm_90a: bounding sphere, occupancy grid (Morton DDA), packed sample
 // containers, fg/bg ray samplers, spherical harmonics and ray generation.
 // Compiled with -fmad=false: every FMA below is explicit and placed where the reference's nvcc build
 // contracts (see common.cuh). Reference semantics cited per kernel.
 //
-// Work mapping (B200): the voxel walk is a serial float recurrence (t += step + eps) that must be reproduced
+// Work mapping: the voxel walk is a serial float recurrence (t += step + eps) that must be reproduced
 // bit-for-bit, but the occupancy bytes do not feed it. The sampler used in training runs one WARP per ray with
 // speculative 32-step windows (see k_occ_samples_in_occupied); the first-sample / advance marchers of sphere tracing
 // are one thread per ray with an 8-step look-ahead of the recurrence over the loads (common.cuh). Copy/packing
@@ -97,13 +97,28 @@ __global__ void __launch_bounds__(kThreads) k_occ_grid_points(int n, GridGeom g,
     }
     out[3 * i] = p.x; out[3 * i + 1] = p.y; out[3 * i + 2] = p.z;
 }
+// A random update sample may hold a voxel more than once, and then whichever thread stores last wins, as in the reference. In
+// deterministic mode (common.cuh) the LAST sample of a voxel in sample order wins instead, what a sequential loop over the sample
+// does: k_occ_claim records 1 + the highest sample index per voxel in `winner`, and only that sample writes (and clears the record).
+__global__ void __launch_bounds__(kThreads) k_occ_claim(int n, const int* __restrict__ idx, int* __restrict__ winner, long long voxels) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n && idx[i] < voxels) atomicMax(&winner[idx[i]], i + 1);
+}
+__device__ __forceinline__ bool occ_wins(int* winner, long long voxels, int i, int v) {
+    if (!winner || v >= voxels) return true;       // no arbitration (default, or a voxel beyond the reserved grid)
+    if (winner[v] != i + 1) return false;
+    winner[v] = 0;
+    return true;
+}
 // OccupancyGridGPU.cuh:303-378
 __global__ void __launch_bounds__(kThreads) k_occ_update_density(int n, const float* __restrict__ density,
                                                                  const int* __restrict__ idx, float decay, float thresh,
-                                                                 float* __restrict__ values, uint8_t* __restrict__ occ) {
+                                                                 float* __restrict__ values, uint8_t* __restrict__ occ, int* __restrict__ winner,
+                                                             long long voxels) {
     int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     int v = idx ? idx[i] : i;
+    if (!occ_wins(winner, voxels, i, v)) return;
     float upd = fmaxf(density[i], __fmul_rn(values[v], decay));
     values[v] = upd;
     occ[v] = upd > thresh;
@@ -112,10 +127,12 @@ __global__ void __launch_bounds__(kThreads) k_occ_update_density(int n, const fl
 __global__ void __launch_bounds__(kThreads) k_occ_update_sdf(int n, const float* __restrict__ sdf, const int* __restrict__ idx,
                                                              float range, float inv_s_scalar,
                                                              const float* __restrict__ inv_s_dev, float thresh,
-                                                             float* __restrict__ values, uint8_t* __restrict__ occ) {
+                                                             float* __restrict__ values, uint8_t* __restrict__ occ, int* __restrict__ winner,
+                                                             long long voxels) {
     int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     int v = idx ? idx[i] : i;
+    if (!occ_wins(winner, voxels, i, v)) return;
     float s = sdf[i];
     values[v] = s;
     float inv_s = inv_s_dev ? inv_s_dev[0] : inv_s_scalar;
@@ -720,19 +737,27 @@ int psdf_occ_compute_grid_points(int n, int V, float extent, const float trans[3
 int psdf_occ_update_with_density(int n, const float* density, const int* idx, float decay, float thresh, float* values,
                                  uint8_t* occ, void* stream) {
     if (n <= 0) return n == 0 ? PSDF_OK : PSDF_ERR_ARG;
-    k_occ_update_density<<<div_up(n, kThreads), kThreads, 0, ST>>>(n, density, idx, decay, thresh, values, occ);
+    // deterministic mode: arbitration of repeated voxels (indices must stay below the grid size reserved by psdf_set_deterministic)
+    const DetBufs* dbuf = det_buffers();
+    int* winner = (dbuf && idx) ? dbuf->winner : nullptr;
+    if (winner) k_occ_claim<<<div_up(n, kThreads), kThreads, 0, ST>>>(n, idx, winner, dbuf->voxels);
+    k_occ_update_density<<<div_up(n, kThreads), kThreads, 0, ST>>>(n, density, idx, decay, thresh, values, occ, winner, winner ? dbuf->voxels : 0);
     PSDF_CHECK_LAUNCH();
     return PSDF_OK;
 }
 int psdf_occ_update_with_sdf(int n, const float* sdf, const int* idx, float extent, int V, float inv_s, const float* inv_s_dev,
                              float thresh, int random_sample_variant, float* values, uint8_t* occ, void* stream) {
     if (n <= 0) return n == 0 ? PSDF_OK : PSDF_ERR_ARG;
+    const DetBufs* dbuf = det_buffers();
+    int* winner = (dbuf && idx) ? dbuf->winner : nullptr;
+    if (winner && (long long)V * V * V > dbuf->voxels) return PSDF_ERR_UNSUPPORTED;   // reserve more with psdf_set_deterministic
+    if (winner) k_occ_claim<<<div_up(n, kThreads), kThreads, 0, ST>>>(n, idx, winner, dbuf->voxels);
     // error range of the sdf inside a voxel: 1.3 (full grid, :437) or 1.0 (random subset, :497) half diagonals
     float voxel = extent / (float)V;
     float half = (float)((double)voxel / 2.0);
     float half_diag = sqrtf(3.0f) * half;
     float range = random_sample_variant ? (float)(1.0 * (double)half_diag) : (float)(1.3 * (double)half_diag);
-    k_occ_update_sdf<<<div_up(n, kThreads), kThreads, 0, ST>>>(n, sdf, idx, range, inv_s, inv_s_dev, thresh, values, occ);
+    k_occ_update_sdf<<<div_up(n, kThreads), kThreads, 0, ST>>>(n, sdf, idx, range, inv_s, inv_s_dev, thresh, values, occ, winner, winner ? dbuf->voxels : 0);
     PSDF_CHECK_LAUNCH();
     return PSDF_OK;
 }
@@ -820,7 +845,7 @@ long long psdf_packed_compact_workspace_bytes(int nr_rays) {
 int psdf_packed_count_samples(int nr_rays, const int* ray_start_end, int* total_dev, void* stream) {
     cudaMemsetAsync(total_dev, 0, sizeof(int), ST);
     if (nr_rays <= 0) return nr_rays == 0 ? PSDF_OK : PSDF_ERR_ARG;
-    int blocks = min(div_up(nr_rays, kScanThreads), 148);
+    int blocks = min(div_up(nr_rays, kScanThreads), 132);
     k_count_samples<<<blocks, kScanThreads, 0, ST>>>(nr_rays, ray_start_end, total_dev);
     PSDF_CHECK_LAUNCH();
     return PSDF_OK;

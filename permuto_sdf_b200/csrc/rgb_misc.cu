@@ -1,4 +1,4 @@
-// Small fused pieces around the colour network (sm_100a), each replacing a chain of tiny element-wise PyTorch launches:
+// Small fused pieces around the colour network (sm_90a), each replacing a chain of tiny element-wise PyTorch launches:
 //   * Lipschitz weight normalisation of LipshitzMLP (permuto_sdf_py/models/models.py:96-110):
 //       W_eff[r,:] = W[r,:] * min(1, softplus(c) / sum_j |W[r,j]|)           forward + backward, one warp per row
 //   * per-image colour calibration + sigmoid on packed samples (models.py:395-414, Colorcal :677-741):

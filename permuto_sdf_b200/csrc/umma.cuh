@@ -1,10 +1,18 @@
-// Minimal hand-written tcgen05 / TMEM / mbarrier / bulk-copy (TMA) primitives for sm_100a, inline PTX only
-// (no CUTLASS). Used by fused_sdf.cu for the dense layers of the small MLPs.
+// Minimal hand-written wgmma / mbarrier / bulk-copy (TMA) primitives for sm_90a, inline PTX only (no CUTLASS). Used by the
+// fused kernels for the dense layers of the small MLPs.
 //
-// Operand layout used everywhere: K-major, SWIZZLE_NONE ("interleaved") canonical layout made of core matrices
+// Operand layout used everywhere: K-major, no-swizzle ("interleaved") canonical layout made of core matrices
 // of 8 rows x 16 bytes stored as 128 contiguous bytes:
 //     byte_offset(row, k) = (row / 8) * SBO + (k_bytes / 16) * LBO + (row % 8) * 16 + (k_bytes % 16)
-// LBO = distance between core matrices adjacent along K, SBO = distance between 8-row groups along M/N.
+// LBO = distance between core matrices adjacent along K, SBO = distance between 8-row groups along M/N. A tile in this
+// layout read with the transpose flag is the MN-major operand of the product that reduces over its rows.
+//
+// Accumulators. wgmma leaves D in the registers of the issuing warpgroup (M = 64 rows per instruction): wg_mma_regs, for kernels
+// whose epilogue consumes the fragments in place. Kernels that keep accumulators across phases (pre-activations reused by the
+// backward sweep, weight gradients summed over all tiles of a CTA) or read them back in a per-row layout use wg_gemm, which stores
+// every product to a per-CTA accumulator area [128 lanes][cols] fp32 in global memory (L2 resident: at most 256 KB per CTA),
+// addressed like a tensor-memory address: taddr = (lane << 16) | column. Each kernel owns one static area (a __device__ array
+// per device, sized for kAccCtas persistent CTAs), so launches of the same kernel must not run concurrently on one device.
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
@@ -14,104 +22,172 @@ namespace umma {
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
-// ---- shared memory matrix descriptor (64 bit), SWIZZLE_NONE ------------------------------------------------
-// [0,14) start address >> 4 | [16,30) LBO >> 4 | [32,46) SBO >> 4 | [46,48) version = 1 | [61,64) layout type = 0
+// ---- shared memory matrix descriptor (64 bit), no swizzle ------------------------------------------------------
+// [0,14) start address >> 4 | [16,30) LBO >> 4 | [32,46) SBO >> 4 | [49,52) base offset = 0 | [62,64) swizzle = 0
 __device__ __forceinline__ uint64_t make_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
     uint64_t d = 0;
     d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
     d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
     d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-    d |= (uint64_t)1 << 46;
     return d;
 }
 
-// ---- instruction descriptor (32 bit) for kind::f16 (bf16 x bf16 -> f32) / kind::tf32 ---------------------------
-// [4,6) D format (1 = f32) | [7,10) A format | [10,13) B format (f16:0, bf16:1, tf32:2) | 15 A major | 16 B major (0 = K)
-// [17,23) N >> 3 | [24,29) M >> 4
-__device__ __forceinline__ uint32_t make_idesc(int M, int N, int ab_format) {
-    uint32_t d = 0;
-    d |= 1u << 4;
-    d |= (uint32_t)ab_format << 7;
-    d |= (uint32_t)ab_format << 10;
-    d |= (uint32_t)(N >> 3) << 17;
-    d |= (uint32_t)(M >> 4) << 24;
-    return d;
+// ---- per-CTA accumulator area --------------------------------------------------------------------------------
+struct AccArea { float* base; int cols; };
+__device__ __forceinline__ AccArea& acc_area() { __shared__ AccArea a; return a; }
+// thread 0 binds the CTA's area (`cols` fp32 columns per lane); a __syncthreads must follow before any access
+__device__ __forceinline__ void acc_attach(float* base, int cols) { acc_area().base = base; acc_area().cols = cols; }
+__device__ __forceinline__ float* acc_ptr(uint32_t lane, uint32_t col) {
+    const AccArea a = acc_area();
+    return a.base + (size_t)lane * a.cols + col;
 }
-constexpr int kFmtF16 = 0, kFmtBF16 = 1, kFmtTF32 = 2;
-// same with both operands MN-major (bits 15, 16): D[M x N] = A^T B for A stored [K x M], B stored [K x N]
-__device__ __forceinline__ uint32_t make_idesc_mn(int M, int N, int ab_format) {
-    return make_idesc(M, N, ab_format) | (1u << 15) | (1u << 16);
+// 32 lanes x 16 consecutive columns: thread t of the warp gets lane (base_lane + t)
+__device__ __forceinline__ void tmem_ld16(uint32_t taddr, float* v) {
+    const float4* p = reinterpret_cast<const float4*>(acc_ptr((taddr >> 16) + (threadIdx.x & 31), taddr & 0xffff));
+#pragma unroll
+    for (int i = 0; i < 4; i++) { const float4 q = p[i]; v[4 * i] = q.x; v[4 * i + 1] = q.y; v[4 * i + 2] = q.z; v[4 * i + 3] = q.w; }
+}
+// 16 lanes x 32 consecutive columns in the layout of an M = 64 accumulator quadrant (rows 16q .. 16q+15 live in lanes
+// 32q .. 32q+15): thread t of the warp gets, for j = 0..3, h = 0..1, b = 0..1,
+//     v[4 j + 2 h + b] = lane (base_lane + t / 4 + 8 h), column (base_col + 8 j + 2 (t % 4) + b)
+// i.e. the m16n8 accumulator fragment repeated over four 8-column blocks
+__device__ __forceinline__ void tmem_ld16x32(uint32_t taddr, float* v) {
+    const int t = threadIdx.x & 31;
+#pragma unroll
+    for (int h = 0; h < 2; h++) {
+        const float* p = acc_ptr((taddr >> 16) + t / 4 + 8 * h, (taddr & 0xffff) + 2 * (t % 4));
+#pragma unroll
+        for (int j = 0; j < 4; j++) { const float2 q = *reinterpret_cast<const float2*>(p + 8 * j); v[4 * j + 2 * h] = q.x; v[4 * j + 2 * h + 1] = q.y; }
+    }
+}
+// store counterpart of tmem_ld16
+__device__ __forceinline__ void tmem_st16(uint32_t taddr, const float* v) {
+    float4* p = reinterpret_cast<float4*>(acc_ptr((taddr >> 16) + (threadIdx.x & 31), taddr & 0xffff));
+#pragma unroll
+    for (int i = 0; i < 4; i++) p[i] = make_float4(v[4 * i], v[4 * i + 1], v[4 * i + 2], v[4 * i + 3]);
 }
 
-// D[tmem] (+)= A[smem] * B[smem]^T ; issued by ONE thread
-__device__ __forceinline__ void mma_bf16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-        "}\n" ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// arrive on an mbarrier when all previously issued MMAs of this thread have completed
-__device__ __forceinline__ void commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void fence_before_sync() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void fence_after_sync() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
+// named barrier over a subset of the CTA's warps (ids 1..15; id 0 is __syncthreads)
+__device__ __forceinline__ void bar_sync(int id, int nthreads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory"); }
 // make generic-proxy shared-memory writes visible to the async proxy (tensor core / TMA reads)
 __device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
-// ---- TMEM allocation (one full warp) ------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_dst, uint32_t ncols) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)), "r"(ncols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// 32 lanes x 16 consecutive 32-bit columns: thread t of the warp gets lane (base_lane + t)
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, float* v) {
-    uint32_t r[16];
+// ---- wgmma (bf16 x bf16 -> f32, D in registers, issued by a whole warpgroup) ---------------------------------------
+// TA / TB: 0 = K-major operand, 1 = MN-major (transposed) operand
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_n16(float* d, uint64_t a, uint64_t b, uint32_t scale_d) {
     asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-          "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr)
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1, %11, %12;\n\t}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+        : "l"(a), "l"(b), "r"(scale_d), "n"(TA), "n"(TB)
         : "memory");
+}
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_n32(float* d, uint64_t a, uint64_t b, uint32_t scale_d) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, %19, %20;\n\t}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "l"(a), "l"(b), "r"(scale_d), "n"(TA), "n"(TB)
+        : "memory");
+}
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_n48(float* d, uint64_t a, uint64_t b, uint32_t scale_d) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %26, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n48k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23}, %24, %25, p, 1, 1, %27, %28;\n\t}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23])
+        : "l"(a), "l"(b), "r"(scale_d), "n"(TA), "n"(TB)
+        : "memory");
+}
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_n64(float* d, uint64_t a, uint64_t b, uint32_t scale_d) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, %35, %36;\n\t}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(a), "l"(b), "r"(scale_d), "n"(TA), "n"(TB)
+        : "memory");
+}
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait0() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+
+template <int N, int TA, int TB>
+__device__ __forceinline__ void wgmma_n(float* d, uint64_t a, uint64_t b, uint32_t scale_d) {
+    if constexpr (N == 16) wgmma_n16<TA, TB>(d, a, b, scale_d);
+    else if constexpr (N == 32) wgmma_n32<TA, TB>(d, a, b, scale_d);
+    else if constexpr (N == 48) wgmma_n48<TA, TB>(d, a, b, scale_d);
+    else wgmma_n64<TA, TB>(d, a, b, scale_d);
+}
+
+// Accumulator lane of fragment row r (0..63) of an M = 64 product: `m64` places it like an M = 64 tensor-memory accumulator
+// (lane (r / 16) * 32 + r % 16, the other 16 lanes of each quadrant free for a second accumulator at lane offset 16),
+// otherwise lane r (the caller's lane field selects rows 0..63 or 64..127 of an M = 128 accumulator).
+__device__ __forceinline__ uint32_t frag_lane(int r, bool m64) { return m64 ? (uint32_t)(32 * (r >> 4) + (r & 15)) : (uint32_t)r; }
+
+// The three split products D (+)= A_hi B_hi + A_hi B_lo + A_lo B_hi of one warpgroup's M = 64 x N block, D in its registers in the
+// m16n8 fragment layout (warp w of the warpgroup, lane t: d[4 j + 2 h + b] = row 16 w + t / 4 + 8 h, column 8 j + 2 (t % 4) + b, the
+// layout tmem_ld16x32 returns). Issue only: the caller brackets a batch with wgmma_fence() and wgmma_commit() + wgmma_wait0().
+template <int N, int TA, int TB>
+__device__ __forceinline__ void wg_mma_regs(float* d, uint64_t ah, uint64_t al, uint64_t bh, uint64_t bl, uint32_t a_step, uint32_t b_step,
+                                            int ksteps, bool accumulate) {
+#pragma unroll 1
+    for (int kk = 0; kk < ksteps; kk++) {
+        const uint64_t oa = (uint64_t)kk * a_step, ob = (uint64_t)kk * b_step;
+        wgmma_n<N, TA, TB>(d, ah + oa, bh + ob, (kk > 0 || accumulate) ? 1u : 0u);
+        wgmma_n<N, TA, TB>(d, ah + oa, bl + ob, 1u);
+        wgmma_n<N, TA, TB>(d, al + oa, bh + ob, 1u);
+    }
+}
+
+template <int N, int TA, int TB>
+__device__ __forceinline__ void wg_gemm_n(uint32_t tdst, bool m64, uint64_t ah, uint64_t al, uint64_t bh, uint64_t bl, uint32_t a_step,
+                                          uint32_t b_step, int ksteps, bool accumulate) {
+    float d[N / 2];
+    const int w = (threadIdx.x >> 5) & 3, t = threadIdx.x & 31;
+    const uint32_t lane0 = tdst >> 16, col0 = (tdst & 0xffff) + 2 * (t % 4);
 #pragma unroll
-    for (int i = 0; i < 16; i++) v[i] = __uint_as_float(r[i]);
-}
-// 16 lanes x 32 consecutive 32-bit columns in the layout of an M = 64 accumulator quadrant (rows 16q .. 16q+15 live in lanes
-// 32q .. 32q+15): thread t of the warp gets, for j = 0..3, h = 0..1, b = 0..1,
-//     v[4 j + 2 h + b] = lane (base_lane + t / 4 + 8 h), column (base_col + 8 j + 2 (t % 4) + b)
-// i.e. the m16n8 accumulator fragment repeated over four 8-column blocks -- all 32 threads hold useful data (a 32x32b load of an
-// M = 64 accumulator fills only half of the warp). Validated on B200 by tools/probes/tmem_ld16_probe.cu.
-__device__ __forceinline__ void tmem_ld16x32(uint32_t taddr, float* v) {
-    uint32_t r[16];
-    asm volatile(
-        "tcgen05.ld.sync.aligned.16x256b.x4.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-          "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr)
-        : "memory");
+    for (int h = 0; h < 2; h++) {
+        const float* p = acc_ptr(lane0 + frag_lane(16 * w + t / 4 + 8 * h, m64), col0);
 #pragma unroll
-    for (int i = 0; i < 16; i++) v[i] = __uint_as_float(r[i]);
+        for (int j = 0; j < N / 8; j++) {
+            float2 q = accumulate ? *reinterpret_cast<const float2*>(p + 8 * j) : make_float2(0.f, 0.f);
+            d[4 * j + 2 * h] = q.x; d[4 * j + 2 * h + 1] = q.y;
+        }
+    }
+    wgmma_fence();
+    wg_mma_regs<N, TA, TB>(d, ah, al, bh, bl, a_step, b_step, ksteps, accumulate);
+    wgmma_commit();
+    wgmma_wait0();
+#pragma unroll
+    for (int h = 0; h < 2; h++) {
+        float* p = acc_ptr(lane0 + frag_lane(16 * w + t / 4 + 8 * h, m64), col0);
+#pragma unroll
+        for (int j = 0; j < N / 8; j++) *reinterpret_cast<float2*>(p + 8 * j) = make_float2(d[4 * j + 2 * h], d[4 * j + 2 * h + 1]);
+    }
 }
-// named barrier over a subset of the CTA's warps (ids 1..15; id 0 is __syncthreads)
-__device__ __forceinline__ void bar_sync(int id, int nthreads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory"); }
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-// store counterpart: thread t of the warp writes lane (base_lane + t), 16 consecutive columns
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const float* v) {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};" ::"r"(taddr),
-        "r"(__float_as_uint(v[0])), "r"(__float_as_uint(v[1])), "r"(__float_as_uint(v[2])), "r"(__float_as_uint(v[3])),
-        "r"(__float_as_uint(v[4])), "r"(__float_as_uint(v[5])), "r"(__float_as_uint(v[6])), "r"(__float_as_uint(v[7])),
-        "r"(__float_as_uint(v[8])), "r"(__float_as_uint(v[9])), "r"(__float_as_uint(v[10])), "r"(__float_as_uint(v[11])),
-        "r"(__float_as_uint(v[12])), "r"(__float_as_uint(v[13])), "r"(__float_as_uint(v[14])), "r"(__float_as_uint(v[15]))
-        : "memory");
+
+// One warpgroup (all 128 threads, warp-aligned) forms the three split products of an M = 64 x nn block,
+//     D (+)= A_hi B_hi + A_hi B_lo + A_lo B_hi      (K = 16 ksteps, fp32 accumulation)
+// and stores it to the accumulator columns [col(tdst), col(tdst) + nn). Descriptors address the block's origin; a_step / b_step
+// advance them by one K16 step, b_n64 moves B by 64 columns (nn > 64 runs in 64-column pieces). nn % 16 == 0.
+// Returns with the results stored; the caller orders them for other warps (barrier or mbarrier arrive).
+template <int TA, int TB>
+__device__ __forceinline__ void wg_gemm(uint32_t tdst, bool m64, uint64_t ah, uint64_t al, uint64_t bh, uint64_t bl, uint32_t a_step,
+                                        uint32_t b_step, uint32_t b_n64, int ksteps, int nn, bool accumulate) {
+    for (int n0 = 0; n0 < nn; n0 += 64) {
+        const uint64_t ob = (uint64_t)(n0 / 64) * b_n64;
+        const uint32_t td = tdst + (uint32_t)n0;
+        switch (min(nn - n0, 64) / 16) {
+            case 1: wg_gemm_n<16, TA, TB>(td, m64, ah, al, bh + ob, bl + ob, a_step, b_step, ksteps, accumulate); break;
+            case 2: wg_gemm_n<32, TA, TB>(td, m64, ah, al, bh + ob, bl + ob, a_step, b_step, ksteps, accumulate); break;
+            case 3: wg_gemm_n<48, TA, TB>(td, m64, ah, al, bh + ob, bl + ob, a_step, b_step, ksteps, accumulate); break;
+            default: wg_gemm_n<64, TA, TB>(td, m64, ah, al, bh + ob, bl + ob, a_step, b_step, ksteps, accumulate); break;
+        }
+    }
 }
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
 
 // ---- mbarrier ------------------------------------------------------------------------------------------------
 __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
@@ -136,7 +212,7 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
         "}\n" ::"r"(smem_u32(bar)), "r"(parity)
         : "memory");
 }
-// 1-D bulk copy global -> shared through the TMA unit (SASS: UBLKCP), completion on an mbarrier (bytes % 16 == 0)
+// 1-D bulk copy global -> shared through the TMA unit, completion on an mbarrier (bytes % 16 == 0)
 __device__ __forceinline__ void bulk_g2s(void* smem_dst, const void* gmem_src, uint32_t bytes, uint64_t* bar) {
     asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(smem_u32(smem_dst)),
                  "l"(gmem_src), "r"(bytes), "r"(smem_u32(bar))

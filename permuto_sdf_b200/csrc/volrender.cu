@@ -1,5 +1,5 @@
 // SDF->density volume compositing, CDF / importance resampling and their hand-written backward
-// kernels for sm_100a. One warp per ray over the packed sample container.
+// kernels for sm_90a. One warp per ray over the packed sample container.
 //
 // Reference: kernels/permuto_sdf/VolumeRenderingGPU.cuh (one thread per ray, serial loop, strided
 // accessor loads). Here every per-sample array is read/written with lane-contiguous (coalesced)

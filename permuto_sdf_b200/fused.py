@@ -1,4 +1,4 @@
-"""Fused evaluation of the SDF model (encoding + MLP in one tcgen05 kernel, csrc/fused_sdf.cu).
+"""Fused evaluation of the SDF model (encoding + MLP in one tensor-core kernel, csrc/fused_sdf.cu).
 
 `FusedSDF(model_sdf)` wraps a `models.SDF` and evaluates sdf / d sdf/dx / geometric feature without
 materialising encoded features or hidden activations in HBM. It is used where no parameter gradient is
@@ -13,7 +13,7 @@ from .permuto_sdf import RaySamplesPacked
 
 def splitk_tn(a, b, slabs=64):
     """a^T b for tall operands a [R, M], b [R, K] (weight gradients: the reduction runs over the sample axis). A plain library
-    GEMM gives this to one or two CTAs looping over all R rows (latency bound, ~180 us at R = 128 k); as a batched GEMM over
+    GEMM gives this to one or two CTAs looping over all R rows (latency bound); as a batched GEMM over
     `slabs` row slabs followed by a small sum it fills the GPU."""
     R = a.shape[0]
     if R < 32 * slabs:
@@ -150,7 +150,7 @@ def _pad16(v):
 
 class _FusedSDFTrainFn(torch.autograd.Function):
     """forward: psdf_sdf_fused_forward (value + 3 tangent streams); backward: psdf_sdf_fused_backward (value + the tangent
-    along the upstream gradient, reverse sweep on the tensor cores, lattice scatter fused, then the tcgen05 weight-gradient kernel)."""
+    along the upstream gradient, reverse sweep on the tensor cores, lattice scatter fused, then the tensor-core weight-gradient kernel)."""
 
     @staticmethod
     def forward(ctx, points, lattice, W0, b0, W1, b1, W2, b2, W3, b3, window, fused):

@@ -3,8 +3,8 @@ explicit sequence of C-ABI calls.
 
 `Trainer.losses()` + `loss.backward()` formulate the iteration with torch.autograd around the fused kernels: correct, but between the
 big kernels autograd and the schedule / loss arithmetic spend ~70 one-block launches per iteration (zero-fills, `mul`, `add`, `exp`,
-`sum`, per-layer Lipschitz normalisation, calibration, gradient accumulation) -- a quarter of the step time on a B200 even inside a
-CUDA graph (profiles/README.md). Here the same mathematics is issued directly:
+`sum`, per-layer Lipschitz normalisation, calibration, gradient accumulation) -- a large share of the step time even inside a
+CUDA graph. Here the same mathematics is issued directly:
 
     sampling (occupancy grid + 2 importance rounds)                                    unchanged, no gradients
     psdf_iter_scalars                   cos-anneal ratio, inv_s = exp(10 forced_variance), curvature ramp          1 launch

@@ -215,7 +215,7 @@ class SDF(torch.nn.Module, _Checkpointed):
 
     def enable_fused_inference(self):
         """route gradient-free evaluations (importance sampling, occupancy refresh, sphere tracing) through the fused
-        encoding+MLP tcgen05 kernel (csrc/fused_sdf.cu); differentiable calls keep using the modular path"""
+        encoding+MLP tensor-core kernel (csrc/fused_sdf.cu); differentiable calls keep using the modular path"""
         from .fused import FusedSDF
         self.fused = FusedSDF(self)
         return self.fused

@@ -90,7 +90,7 @@ class FusedAdamW:
             pptrs.append(torch.tensor([int(hp.buffer_ptrs[r]) + 4 * g["_off"] for r in range(world)], dtype=torch.int64))
         import os
         # NVSwitch multicast (in-switch reduction + replication) cuts the per-rank NVLink bytes from (W-1)/W to 1/W of the buffers: pays
-        # from 4 ranks on; at 2 ranks the unicast kernel is faster (measured on B200: 161 vs 241 us, tools/dp_step_timing.py)
+        # from 4 ranks on; at 2 ranks the unicast kernel is expected to be faster (compare with tools/dp_step_timing.py)
         want = os.environ.get("PSDF_DP_MULTICAST", "auto")
         mc = (want == "1" or (want == "auto" and world >= 4)) and bool(getattr(hp, "has_multicast_support", False)) and \
             int(hp.multicast_ptr) != 0 and int(hg.multicast_ptr) != 0

@@ -1,4 +1,4 @@
-"""Make the fused tcgen05 path reachable from the REFERENCE's own model classes.
+"""Make the fused tensor-core path reachable from the REFERENCE's own model classes.
 
 Over compat/ the unmodified permuto_sdf_py/models/models.py runs on the per-op kernels (encoding kernels + torch.nn.Linear +
 autograd). `patch_reference_models(M)` grafts the methods of this package's SDF / RGB onto the reference classes of the imported

@@ -718,7 +718,7 @@ class NGPGui:
 
     @staticmethod
     def create(view=None):
-        raise RuntimeError("NGPGui needs the EasyPBR viewer; out of scope for the B200 hot path")
+        raise RuntimeError("NGPGui needs the EasyPBR viewer; out of scope for the GPU hot path")
 
 
 __all__ = ["PermutoSDF", "Sphere", "OccupancyGrid", "RaySamplesPacked", "VolumeRendering", "RaySampler", "TrainParams", "NGPGui"]

@@ -1,6 +1,6 @@
 """Drop-in replacement of the external `permutohedral_encoding` package the reference imports
 (permuto_sdf_py/models/models.py:20; constructor call :149, forward :186, `.output_dims()` :154,
-`Coarse2Fine` :172,183). Semantics: SURVEY.md Appendix B. The device work is done by the sm_100a kernels in
+`Coarse2Fine` :172,183). Semantics: SURVEY.md Appendix B. The device work is done by the sm_90a kernels in
 csrc/encoding.cu through the C ABI (psdf_enc_forward / psdf_enc_backward / psdf_enc_double_backward).
 
 Differentiability contract (SURVEY.md F7): out is differentiable wrt `lattice_values` and wrt `positions`;

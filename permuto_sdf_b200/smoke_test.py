@@ -22,7 +22,7 @@ def run(verbose=True):
     from permuto_sdf_b200.train import HyperParams, Trainer
 
     lib = load_library()
-    assert lib.psdf_device_ok() == 1, "libpsdf_b200.so is loaded but no sm_100 device is visible"
+    assert lib.psdf_device_ok() == 1, "libpsdf_b200.so is loaded but no sm_90 (H100) device is visible"
     torch.cuda.set_device(0)
     torch.manual_seed(0)
 

@@ -89,9 +89,8 @@ def create_samples(with_mask, hyperparams, ray_origins, ray_dirs, jitter_samples
     return fg, bg
 
 
-# sphere_trace's loop as one tcgen05 kernel instead of ~12 launches + a host sync per iteration (csrc/fused_sdf.cu k_sdf_sphere_trace:
-# persistent CTAs over a global ray queue, finished slots refilled, resumable marches). Measured on B200 at 1920x1080, 256 iterations
-# max (profiles/README.md): 10 ms for the trace against 136 ms for the masked loop; it wins at every frame size, so there is no ray limit.
+# sphere_trace's loop as one tensor-core kernel instead of ~12 launches + a host sync per iteration (csrc/fused_sdf.cu k_sdf_sphere_trace:
+# persistent CTAs over a global ray queue, finished slots refilled, resumable marches); no ray limit.
 FUSED_SPHERE_TRACE = True
 FUSED_SPHERE_TRACE_MAX_RAYS = 1 << 30
 FUSED_IMPORTANCE_ROUND = True     # one launch per round (csrc/volrender.cu k_importance_round) instead of 9
@@ -339,9 +338,13 @@ class Trainer:
     per-iteration step of train_permuto_sdf.py:311-422 (after sphere init), with `--with_mask` semantics."""
 
     def __init__(self, hyperparams=None, nr_levels=24, capacity=2 ** 18, sdf_hidden=32, nr_images=8, occupancy_resolution=256,
-                 seed=0, with_colorcal=True, optimizer="adamw", fused_inference=True, fused_training=True, fused_render=True, direct=None):
+                 seed=0, with_colorcal=True, optimizer="adamw", fused_inference=True, fused_training=True, fused_render=True, direct=None,
+                 deterministic=False):
         """direct: None = run the iteration through the autograd-free sequence of iteration.DirectIteration whenever the configuration
-        allows it (fused kernels, flat-buffer optimizer, --with_mask); True = require it (raise otherwise); False = autograd formulation"""
+        allows it (fused kernels, flat-buffer optimizer, --with_mask); True = require it (raise otherwise); False = autograd formulation.
+        deterministic: switch the library's deterministic mode on for this device (psdf_set_deterministic: order-independent gradient
+        reductions, so runs with the same inputs give the same bits; the direct iteration is fully covered) -- or off (the default,
+        float atomics)."""
         torch.manual_seed(seed)
         self.fused_render = fused_render
         self._fused_inference = fused_inference
@@ -353,18 +356,20 @@ class Trainer:
         self.model_bg = None if hp.with_mask else NerfHash(4, self.aabb, hp.background_nr_iters_for_c2f, nr_levels, capacity).to("cuda")
         self.model_colorcal = Colorcal(nr_images, 0) if (hp.use_color_calibration and with_colorcal) else None
         self.occupancy_grid = OccupancyGrid(occupancy_resolution, 1.0, [0, 0, 0]) if hp.use_occupancy_grid else None
-        # No silent fall-back: asking for the fused (tcgen05) path with a shape it does not cover raises here (FusedSDF / FusedRGB
+        from ._lib import call as _call
+        _call("psdf_set_deterministic", 1 if deterministic else 0, nr_levels * capacity * 2, occupancy_resolution ** 3)
+        # No silent fall-back: asking for the fused (tensor-core) path with a shape it does not cover raises here (FusedSDF / FusedRGB
         # say which constraint failed); the per-op path is only taken when the caller asks for it (fused_inference=False /
         # fused_training=False). `self.execution` records which path each model runs on.
         self.execution = {"sdf_inference": "per-op kernels", "sdf_training": "per-op kernels + autograd", "rgb": "per-op kernels + autograd",
                           "background": "per-op kernels + autograd" if self.model_bg is not None else None}
         if fused_inference:
             self.model_sdf.enable_fused_inference()
-            self.execution["sdf_inference"] = "fused tcgen05"
+            self.execution["sdf_inference"] = "fused wgmma"
             if fused_training:
                 self.model_sdf.enable_fused_training()
                 self.model_rgb.enable_fused()
-                self.execution["sdf_training"] = self.execution["rgb"] = "fused tcgen05"
+                self.execution["sdf_training"] = self.execution["rgb"] = "fused wgmma"
         groups = [{"params": list(self.model_sdf.parameters()), "weight_decay": 0.0, "lr": hp.lr, "name": "model_sdf"}]
         if self.model_bg is not None:
             groups.append({"params": list(self.model_bg.parameters()), "weight_decay": 0.0, "lr": hp.lr, "name": "model_bg"})
@@ -716,11 +721,10 @@ class Trainer:
         it = self.iter_nr
         if self._dp is not None:
             # data-parallel runs: keep the host at most TWO iterations ahead of the GPU (wait for the end of the forward/backward graph of
-            # the iteration before the previous one). Measured on 2 B200s (profiles/README.md): with the host free to queue many iterations
-            # of graph replays + eagerly launched cross-rank barrier / peer-step kernels on two streams, the step time was 1.34 ms in two
-            # runs and 1.69 / 3.19 ms in two others (and the NVML sampler thread of the slow runs got a third of its time slices: the
-            # process was spinning), while the end-to-end path -- which reads the loss every step and so never runs ahead -- gave
-            # 1.30-1.33 ms in every run. Two iterations of queued work keep the GPU fed; the wait costs nothing then.
+            # the iteration before the previous one). With the host free to queue many iterations of graph replays + eagerly launched
+            # cross-rank barrier / peer-step kernels on two streams, data-parallel step times were unstable from run to run (the process
+            # spun), while the end-to-end path -- which reads the loss every step and so never runs ahead -- was steady. Two iterations of
+            # queued work keep the GPU fed; the wait costs nothing then.
             hist = cg.setdefault("ev_hist", [])
             if len(hist) >= 2:
                 hist[-2].synchronize()

@@ -2,7 +2,7 @@
 
 Mirror of permuto_sdf_py/volume_rendering/volume_rendering_funcs.py:55-223 (CumprodAlpha2TransmittanceFunc,
 IntegrateWithWeightsFunc, SumOverRayFunc) and volume_rendering_modules.py:61-182 (VolumeRenderingNerf,
-SingleVarianceNetwork, VolumeRenderingNeus), running on the sm_100a kernels through `permuto_sdf`.
+SingleVarianceNetwork, VolumeRenderingNeus), running on the sm_90a kernels through `permuto_sdf`.
 """
 import torch
 import torch.nn.functional as F

@@ -10,7 +10,7 @@ for p in (ROOT, os.path.join(ROOT, "compat")):
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with `-m gpu`)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run with `-m gpu` on an H100)")
 
 
 @pytest.fixture(scope="session")
@@ -20,5 +20,5 @@ def cuda():
         pytest.skip("no CUDA device")
     from permuto_sdf_b200 import load_library
     lib = load_library()
-    assert lib.psdf_device_ok() == 1, "libpsdf_b200.so loaded but the device is not sm_100"
+    assert lib.psdf_device_ok() == 1, "libpsdf_b200.so loaded but the device is not sm_90 (H100)"
     return torch.device("cuda", 0)

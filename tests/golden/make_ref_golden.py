@@ -1,7 +1,7 @@
-"""Generate reference-made golden fixtures (run on a B200: `python tests/golden/make_ref_golden.py`).
+"""Generate reference-made golden fixtures (run on a GPU: `python tests/golden/make_ref_golden.py`).
 
-Runs the UNMODIFIED reference CUDA kernels (oracle/_ref/libpsdf_ref_gpu.so, built from
-/root/reference/kernels/permuto_sdf/*GPU.cuh by oracle/ref_shim/Makefile) on small seeded inputs and stores
+Runs the UNMODIFIED reference CUDA kernels (oracle/_ref/libpsdf_ref_gpu.so, built from the original project's
+kernels/permuto_sdf/*GPU.cuh by oracle/ref_shim/Makefile) on small seeded inputs and stores
 inputs + outputs in tests/golden/ref_rayops.npz. Packed outputs are canonicalised per ray (the reference hands
 out sample slots with an atomic counter, SURVEY.md F8): per-ray counts plus the per-sample arrays concatenated
 in ray order. tests/golden/check_golden.py replays the same inputs through the C oracle on the CPU.
@@ -46,7 +46,7 @@ def put(dst, prefix, d):
 
 
 def main():
-    assert ref.available(), "oracle/_ref/libpsdf_ref_gpu.so missing: run `make -C oracle/ref_shim` where /root/reference exists"
+    assert ref.available(), "oracle/_ref/libpsdf_ref_gpu.so missing: run `make -C oracle/ref_shim REF=<checkout of the original project>`"
     G = {}
     o, d = scenes.make_rays(R, seed=11)
     G["in.o"], G["in.d"] = o, d
@@ -169,10 +169,6 @@ def main():
     out = os.path.join(HERE, "ref_rayops.npz")
     np.savez_compressed(out, **G)
     print("wrote", out, os.path.getsize(out), "bytes,", len(G), "arrays; gpu:", torch.cuda.get_device_name(0))
-    # also drop a copy where gpurun brings it back
-    od = os.path.join(ROOT, "gpurun_out")
-    os.makedirs(od, exist_ok=True)
-    np.savez_compressed(os.path.join(od, "ref_rayops.npz"), **G)
 
 
 if __name__ == "__main__":

@@ -1,6 +1,6 @@
 """Fixture generator: runs the reference's UNMODIFIED Python classes (permuto_sdf_py/models/models.py, volume_rendering/*.py,
 utils/sdf_utils.py) on the CPU through oracle/refpy.py and stores seeded inputs, parameters, outputs and gradients in
-tests/golden/refpy_golden.npz. Runs only in the build container (needs /root/reference); the GPU tests
+tests/golden/refpy_golden.npz (+ refpy_golden_bg.npz). Needs a checkout of the original project, named by PERMUTO_SDF_REFERENCE; the GPU tests
 (tests/test_refpy_golden_gpu.py) load the .npz, put the same parameters into the CUDA path and compare.
 
     python tests/golden/make_refpy_golden.py
@@ -209,9 +209,11 @@ def main():
                 "trace_out.points": pts_t.numpy(), "trace_out.sdf": sdf_t.detach().numpy(),
                 "trace_out.ray_start_end_idx": traced.ray_start_end_idx.numpy()})
 
+    # two files, each under 1 MB: the background model's arrays (keys bg*) go to <name>_bg.npz
     path = os.environ.get("REFPY_GOLDEN_OUT") or os.path.join(ROOT, "tests", "golden", "refpy_golden.npz")
-    np.savez_compressed(path, **out)
-    print("wrote %s: %d arrays, %.1f KB" % (path, len(out), os.path.getsize(path) / 1024))
+    np.savez_compressed(path, **{k: v for k, v in out.items() if not k.startswith("bg")})
+    np.savez_compressed(path[:-len(".npz")] + "_bg.npz", **{k: v for k, v in out.items() if k.startswith("bg")})
+    print("wrote %s (+ _bg): %d arrays, %.1f KB" % (path, len(out), os.path.getsize(path) / 1024))
 
 
 if __name__ == "__main__":

@@ -1,7 +1,7 @@
-// Hardware probes for the tcgen05 conventions the fused backward kernels rely on (test infrastructure, NOT part of the product
-// library: built into tests/probe/libumma_probe.so, loaded only by tests/test_umma_probe_gpu.py).
-//   mode 0: two M = 64 accumulators sharing the same TMEM columns, one at lane offset 0 and one at lane offset 16
-//           (an M = 64 instruction writes lanes (m / 16) * 32 + m % 16; does a D address with lane field 16 fill the other half?)
+// Hardware probes for the wgmma conventions the fused kernels rely on (test infrastructure, NOT part of the product library: built
+// into tests/probe/libumma_probe.so, loaded only by tests/test_umma_probe_gpu.py and tests/test_fused_gpu.py).
+//   mode 0: two M = 64 accumulators sharing the same columns, one at lane offset 0 and one at lane offset 16 (an M = 64 product is
+//           stored to lanes (m / 16) * 32 + m % 16), both formed from MN-major operands (sample axis = MMA K dimension)
 //   mode 1: D[128 x Kp] = A[128 x Np] * W[Np x Kp] with A K-major and B = the FORWARD weight tile ([Np rows][Kp] K-major along k)
 //           consumed as an MN-major operand (reduction over the rows): the reverse GEMM without a transposed weight copy.
 //   umma_probe_gemm / umma_probe_gemm_tn: self-tests of the descriptor conventions (K-major forward GEMM with the kernels' own split /
@@ -11,6 +11,36 @@
 using namespace psdf_fused;
 
 namespace {
+__device__ float g_acc_probe[kTile * 64];     // accumulator area of the single probe CTA
+
+__device__ __forceinline__ void attach_and_fill(float value) {
+    if (threadIdx.x == 0) umma::acc_attach(g_acc_probe, 64);
+    __syncthreads();
+    float z[16];
+#pragma unroll
+    for (int i = 0; i < 16; i++) z[i] = value;
+    for (int c = 0; c < 4; c++) umma::tmem_st16(((uint32_t)((threadIdx.x >> 5) * 32) << 16) + c * 16, z);
+    umma::fence_async_smem();
+    __syncthreads();
+}
+__device__ __forceinline__ void dump_all(float* dump, int N) {
+    __syncthreads();
+    const int tid = threadIdx.x;
+    for (int c = 0; c < 4; c++) {
+        float z[16];
+        umma::tmem_ld16(((uint32_t)((tid >> 5) * 32) << 16) + c * 16, z);
+#pragma unroll
+        for (int i = 0; i < 16; i++) if (c * 16 + i < N) dump[tid * N + c * 16 + i] = z[i];
+    }
+}
+// dW-style product of two [128 x 64] tiles as MN-major operands into an M = 64 accumulator (one warpgroup)
+__device__ __forceinline__ void gemm_tn(uint32_t tdst, const uint8_t* a_hi, const uint8_t* a_lo, const uint8_t* b_hi, const uint8_t* b_lo, int nn) {
+    // MN-major, no swizzle: LBO = stride between 8-sample groups (K), SBO = stride between 8-column cores (MN)
+    const uint64_t dah = umma::make_desc(umma::smem_u32(a_hi), kSBO_A, kLBO), dal = umma::make_desc(umma::smem_u32(a_lo), kSBO_A, kLBO);
+    const uint64_t dbh = umma::make_desc(umma::smem_u32(b_hi), kSBO_A, kLBO), dbl = umma::make_desc(umma::smem_u32(b_lo), kSBO_A, kLBO);
+    umma::wg_gemm<1, 1>(tdst, true, dah, dal, dbh, dbl, (2 * kSBO_A) >> 4, (2 * kSBO_A) >> 4, (8 * kLBO) >> 4, kTile / 16, nn, false);
+}
+
 __global__ void __launch_bounds__(kTile) k_probe(int mode, const float* __restrict__ A, const float* __restrict__ A2,
                                                 const float* __restrict__ B, float* __restrict__ dump) {
     extern __shared__ __align__(128) uint8_t smem[];
@@ -20,10 +50,7 @@ __global__ void __launch_bounds__(kTile) k_probe(int mode, const float* __restri
     uint8_t* a2_lo = a2_hi + kATileBytes;
     uint8_t* b_hi = a2_lo + kATileBytes;
     uint8_t* b_lo = b_hi + kATileBytes;
-    uint64_t* bar = reinterpret_cast<uint64_t*>(b_lo + kATileBytes);
-    uint32_t* slot = reinterpret_cast<uint32_t*>(bar + 1);
-    const int tid = threadIdx.x, warp = tid >> 5;
-    if (tid == 0) { umma::mbar_init(bar, 1); umma::mbar_fence_init(); }
+    const int tid = threadIdx.x;
     // all three inputs are [128][64] row-major fp32, stored as K-major core-matrix tiles (row = tid)
     for (int kc = 0; kc < 8; kc++) {
         float va[8], va2[8], vb[8];
@@ -37,66 +64,22 @@ __global__ void __launch_bounds__(kTile) k_probe(int mode, const float* __restri
         store8(a2_hi, a2_lo, tid, kc, va2);
         store8(b_hi, b_lo, tid, kc, vb);
     }
-    __syncthreads();
-    if (warp == 0) umma::tmem_alloc(slot, 64);
-    umma::fence_async_smem();
-    umma::fence_before_sync();
-    __syncthreads();
-    umma::fence_after_sync();
-    const uint32_t tmem_base = *slot;
-    {
-        float z[16];
-#pragma unroll
-        for (int i = 0; i < 16; i++) z[i] = -7.0f;        // sentinel: lanes no MMA writes keep it
-        for (int c = 0; c < 4; c++) umma::tmem_st16(tmem_base + ((uint32_t)(warp * 32) << 16) + c * 16, z);
-        umma::tmem_st_wait();
-    }
-    umma::fence_before_sync();
-    __syncthreads();
-    if (tid == 0) {
-        umma::fence_after_sync();
-        if (mode == 0) {
-            const uint32_t idesc = umma::make_idesc_mn(64, 64, umma::kFmtBF16);
-            for (int which = 0; which < 2; which++) {
-                const uint32_t ah = umma::smem_u32(which ? a2_hi : a_hi), al = umma::smem_u32(which ? a2_lo : a_lo);
-                const uint32_t bh = umma::smem_u32(b_hi), bl = umma::smem_u32(b_lo);
-                const uint32_t d = tmem_base + (which ? (16u << 16) : 0u);
-                for (int kk = 0; kk < kTile / 16; kk++) {
-                    const uint32_t ko = kk * 2 * kSBO_A;
-                    uint64_t dah = umma::make_desc(ah + ko, kSBO_A, kLBO), dal = umma::make_desc(al + ko, kSBO_A, kLBO);
-                    uint64_t dbh = umma::make_desc(bh + ko, kSBO_A, kLBO), dbl = umma::make_desc(bl + ko, kSBO_A, kLBO);
-                    umma::mma_bf16(d, dah, dbh, idesc, kk > 0 ? 1u : 0u);
-                    umma::mma_bf16(d, dah, dbl, idesc, 1u);
-                    umma::mma_bf16(d, dal, dbh, idesc, 1u);
-                }
-            }
-        } else {
-            // A = a tile [128 x 64] K-major; B = first 64 rows of the b tile = W[n = 0..63][k = 0..63], forward layout
-            const uint32_t idesc = umma::make_idesc(128, 64, umma::kFmtBF16) | (1u << 16);
-            const uint32_t ah = umma::smem_u32(a_hi), al = umma::smem_u32(a_lo), bh = umma::smem_u32(b_hi), bl = umma::smem_u32(b_lo);
-            for (int kk = 0; kk < 4; kk++) {
-                uint64_t dah = umma::make_desc(ah + kk * 2 * kLBO, kLBO, kSBO_A), dal = umma::make_desc(al + kk * 2 * kLBO, kLBO, kSBO_A);
-                // reduction index n: 8-row groups of the weight tile are kSBO_A apart (K direction), the k cores kLBO (N direction)
-                uint64_t dbh = umma::make_desc(bh + kk * 2 * kSBO_A, kSBO_A, kLBO), dbl = umma::make_desc(bl + kk * 2 * kSBO_A, kSBO_A, kLBO);
-                umma::mma_bf16(tmem_base, dah, dbh, idesc, kk > 0 ? 1u : 0u);
-                umma::mma_bf16(tmem_base, dah, dbl, idesc, 1u);
-                umma::mma_bf16(tmem_base, dal, dbh, idesc, 1u);
-            }
+    attach_and_fill(-7.0f);        // sentinel: lanes no product writes keep it
+    if (mode == 0) {
+        gemm_tn(0, a_hi, a_lo, b_hi, b_lo, 64);
+        gemm_tn(16u << 16, a2_hi, a2_lo, b_hi, b_lo, 64);
+    } else {
+        // A = a tile [128 x 64] K-major; B = first 64 rows of the b tile = W[n = 0..63][k = 0..63], forward layout. Reduction index n:
+        // 8-row groups of the weight tile are kSBO_A apart (K direction), the k cores kLBO (N direction)
+        const uint64_t dbh = umma::make_desc(umma::smem_u32(b_hi), kSBO_A, kLBO), dbl = umma::make_desc(umma::smem_u32(b_lo), kSBO_A, kLBO);
+        for (int mh = 0; mh < 2; mh++) {
+            const uint32_t ao = (uint32_t)(mh * 8 * kSBO_A);
+            const uint64_t dah = umma::make_desc(umma::smem_u32(a_hi) + ao, kLBO, kSBO_A), dal = umma::make_desc(umma::smem_u32(a_lo) + ao, kLBO, kSBO_A);
+            umma::wg_gemm<0, 1>((uint32_t)(64 * mh) << 16, false, dah, dal, dbh, dbl, (2 * kLBO) >> 4, (2 * kSBO_A) >> 4, (8 * kLBO) >> 4, 4, 64,
+                                false);
         }
-        umma::commit(bar);
     }
-    umma::mbar_wait(bar, 0);
-    umma::fence_after_sync();
-    for (int c = 0; c < 4; c++) {
-        float z[16];
-        umma::tmem_ld16(tmem_base + ((uint32_t)(warp * 32) << 16) + c * 16, z);
-        umma::tmem_ld_wait();
-#pragma unroll
-        for (int i = 0; i < 16; i++) dump[tid * 64 + c * 16 + i] = z[i];
-    }
-    umma::fence_before_sync();
-    __syncthreads();
-    if (warp == 0) umma::tmem_dealloc(tmem_base, 64);
+    dump_all(dump, 64);
 }
 // ---------------------------------------------------------------------------------------------- debug GEMM (descriptor check)
 // D[128 x N] = A[128 x K] * B[N x K]^T with the same split/pack/issue/load helpers as the fused kernel.
@@ -108,10 +91,7 @@ __global__ void __launch_bounds__(kTile) k_debug_gemm(int N, int K, const float*
     uint8_t* a_lo = a_hi + kATileBytes;
     uint8_t* w_hi = a_lo + kATileBytes;
     uint8_t* w_lo = w_hi + Np * Kp * 2;
-    uint64_t* bar = reinterpret_cast<uint64_t*>(w_lo + Np * Kp * 2);
-    uint32_t* slot = reinterpret_cast<uint32_t*>(bar + 1);
-    const int tid = threadIdx.x, warp = tid >> 5;
-    if (tid == 0) { umma::mbar_init(bar, 1); umma::mbar_fence_init(); }
+    const int tid = threadIdx.x;
     for (int kc = 0; kc < Kp / 8; kc++) {
         float v[8];
 #pragma unroll
@@ -128,36 +108,15 @@ __global__ void __launch_bounds__(kTile) k_debug_gemm(int N, int K, const float*
         *reinterpret_cast<__nv_bfloat16*>(w_hi + off) = hi;
         *reinterpret_cast<__nv_bfloat16*>(w_lo + off) = lo;
     }
-    __syncthreads();
-    if (warp == 0) umma::tmem_alloc(slot, 64);
-    umma::fence_async_smem();
-    umma::fence_before_sync();
-    __syncthreads();
-    umma::fence_after_sync();
-    const uint32_t tmem_base = *slot;
-    if (tid == 0) {
-        if (K == 63) issue_gemm_rebuild(tmem_base, a_hi, a_lo, w_hi, w_lo, Kp, Np);     // K = 63 selects the rebuild-per-step variant
-        else issue_gemm(tmem_base, a_hi, a_lo, w_hi, w_lo, Kp, Np);
-        umma::commit(bar);
-    }
-    umma::mbar_wait(bar, 0);
-    umma::fence_after_sync();
-    for (int c = 0; c < Np / 16; c++) {
-        float z[16];
-        umma::tmem_ld16(tmem_base + ((uint32_t)(warp * 32) << 16) + c * 16, z);
-        umma::tmem_ld_wait();
-#pragma unroll
-        for (int i = 0; i < 16; i++) if (c * 16 + i < N) D[tid * N + c * 16 + i] = z[i];
-    }
-    umma::fence_before_sync();
-    __syncthreads();
-    if (warp == 0) umma::tmem_dealloc(tmem_base, 64);
+    attach_and_fill(0.0f);
+    for (int mh = 0; mh < 2; mh++) issue_gemm(0, mh, a_hi, a_lo, w_hi, w_lo, Kp, Np);
+    dump_all(D, N);
 }
 
 // D[M x N] = A^T B over the 128 rows of two operand tiles (A [128 x M], B [128 x N], both stored like every activation tile:
 // row = sample, 16-byte core rows along the columns), i.e. the weight-gradient product dW = zbar^T a with the sample axis as the
-// MMA K dimension and both operands MN-major. `dump` receives all 128 TMEM lanes x N columns so that the accumulator layout of
-// an M = 64 instruction can be read off on the host.
+// MMA K dimension and both operands MN-major. `dump` receives all 128 accumulator lanes x 64 columns so that the lane of every
+// accumulator row can be read off on the host.
 __global__ void __launch_bounds__(kTile) k_debug_gemm_tn(int M, int N, const float* __restrict__ A, const float* __restrict__ B,
                                                          float* __restrict__ dump) {
     extern __shared__ __align__(128) uint8_t smem[];
@@ -165,10 +124,7 @@ __global__ void __launch_bounds__(kTile) k_debug_gemm_tn(int M, int N, const flo
     uint8_t* a_lo = a_hi + kATileBytes;
     uint8_t* b_hi = a_lo + kATileBytes;
     uint8_t* b_lo = b_hi + kATileBytes;
-    uint64_t* bar = reinterpret_cast<uint64_t*>(b_lo + kATileBytes);
-    uint32_t* slot = reinterpret_cast<uint32_t*>(bar + 1);
-    const int tid = threadIdx.x, warp = tid >> 5;
-    if (tid == 0) { umma::mbar_init(bar, 1); umma::mbar_fence_init(); }
+    const int tid = threadIdx.x;
     for (int kc = 0; kc < 8; kc++) {
         float va[8], vb[8];
 #pragma unroll
@@ -180,59 +136,15 @@ __global__ void __launch_bounds__(kTile) k_debug_gemm_tn(int M, int N, const flo
         store8(a_hi, a_lo, tid, kc, va);
         store8(b_hi, b_lo, tid, kc, vb);
     }
-    __syncthreads();
-    if (warp == 0) umma::tmem_alloc(slot, 64);
-    umma::fence_async_smem();
-    umma::fence_before_sync();
-    __syncthreads();
-    umma::fence_after_sync();
-    const uint32_t tmem_base = *slot;
-    // clear the accumulator columns first so that lanes the MMA does not write read back as zero
-    {
-        float z[16];
-#pragma unroll
-        for (int i = 0; i < 16; i++) z[i] = 0.f;
-        for (int c = 0; c < 4; c++) umma::tmem_st16(tmem_base + ((uint32_t)(warp * 32) << 16) + c * 16, z);
-        umma::tmem_st_wait();
-    }
-    umma::fence_before_sync();
-    __syncthreads();
-    if (tid == 0) {
-        umma::fence_after_sync();
-        const int Mp = 64, Np = pad16(N);      // cta_group::1 accepts M = 64 or 128 only; columns past M are zero
-        const uint32_t idesc = umma::make_idesc_mn(Mp, Np, umma::kFmtBF16);
-        const uint32_t ah = umma::smem_u32(a_hi), al = umma::smem_u32(a_lo), bh = umma::smem_u32(b_hi), bl = umma::smem_u32(b_lo);
-        for (int kk = 0; kk < kTile / 16; kk++) {
-            const uint32_t ko = kk * 2 * kSBO_A;          // 16 samples = 2 eight-row groups
-            // MN-major, no swizzle: LBO = stride between 8-sample groups (K), SBO = stride between 8-column cores (MN)
-            uint64_t dah = umma::make_desc(ah + ko, kSBO_A, kLBO), dal = umma::make_desc(al + ko, kSBO_A, kLBO);
-            uint64_t dbh = umma::make_desc(bh + ko, kSBO_A, kLBO), dbl = umma::make_desc(bl + ko, kSBO_A, kLBO);
-            umma::mma_bf16(tmem_base, dah, dbh, idesc, kk > 0 ? 1u : 0u);
-            umma::mma_bf16(tmem_base, dah, dbl, idesc, 1u);
-            umma::mma_bf16(tmem_base, dal, dbh, idesc, 1u);
-        }
-        umma::commit(bar);
-    }
-    umma::mbar_wait(bar, 0);
-    umma::fence_after_sync();
-    for (int c = 0; c < 4; c++) {
-        float z[16];
-        umma::tmem_ld16(tmem_base + ((uint32_t)(warp * 32) << 16) + c * 16, z);
-        umma::tmem_ld_wait();
-#pragma unroll
-        for (int i = 0; i < 16; i++) dump[tid * 64 + c * 16 + i] = z[i];
-    }
-    umma::fence_before_sync();
-    __syncthreads();
-    if (warp == 0) umma::tmem_dealloc(tmem_base, 64);
+    attach_and_fill(0.0f);         // lanes the product does not write read back as zero
+    gemm_tn(0, a_hi, a_lo, b_hi, b_lo, pad16(N));      // M = 64 product; rows past M are zero
+    dump_all(dump, 64);
 }
-
-
 
 }  // namespace
 
 extern "C" int umma_probe(int mode, const float* A, const float* A2, const float* B, float* dump, void* stream) {
-    size_t smem = 6 * kATileBytes + 64;
+    size_t smem = 6 * kATileBytes;
     cudaFuncSetAttribute(k_probe, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     k_probe<<<1, kTile, smem, (cudaStream_t)stream>>>(mode, A, A2, B, dump);
     return cudaGetLastError() == cudaSuccess ? 0 : -1;
@@ -240,7 +152,7 @@ extern "C" int umma_probe(int mode, const float* A, const float* A2, const float
 
 extern "C" int umma_probe_gemm_tn(int M, int N, const float* A, const float* B, float* dump, void* stream) {
     if (M < 1 || M > 64 || N < 1 || N > 64) return -2;
-    int smem = 4 * kATileBytes + 64;
+    int smem = 4 * kATileBytes;
     cudaFuncSetAttribute(k_debug_gemm_tn, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     k_debug_gemm_tn<<<1, kTile, smem, (cudaStream_t)stream>>>(M, N, A, B, dump);
     return cudaGetLastError() == cudaSuccess ? 0 : -1;
@@ -248,7 +160,7 @@ extern "C" int umma_probe_gemm_tn(int M, int N, const float* A, const float* B, 
 
 extern "C" int umma_probe_gemm(int N, int K, const float* A, const float* B, float* D, void* stream) {
     if (N < 1 || N > 64 || K < 1 || K > 64) return -2;
-    size_t smem = 2 * kATileBytes + 2 * (size_t)pad16(N) * pad16(K) * 2 + 64;
+    size_t smem = 2 * kATileBytes + 2 * (size_t)pad16(N) * pad16(K) * 2;
     cudaFuncSetAttribute(k_debug_gemm, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024);
     k_debug_gemm<<<1, kTile, smem, (cudaStream_t)stream>>>(N, K, A, B, D);
     return cudaGetLastError() == cudaSuccess ? 0 : -1;

@@ -1,4 +1,4 @@
-"""GPU tests of the tcgen05 path: the raw tensor-core GEMM self test (descriptor / layout check) and the fused
+"""GPU tests of the tensor-core (wgmma) path: the raw tensor-core GEMM self test (descriptor / layout check) and the fused
 encoding+MLP SDF kernel against (a) the CPU oracle and (b) the unfused differentiable model. Tolerance: the
 north star's 1e-3 relative; the bf16x2 split keeps it ~1e-5."""
 import numpy as np
@@ -16,7 +16,7 @@ def rel(a, b):
 
 
 def _probe_call(name, *args):
-    """tcgen05 self tests live in the probe library (tests/probe/libumma_probe.so, test infrastructure), not in the product ABI"""
+    """tensor-core self tests live in the probe library (tests/probe/libumma_probe.so, test infrastructure), not in the product ABI"""
     import ctypes
     import os
     so = os.path.join(os.path.dirname(os.path.abspath(__file__)), "probe", "libumma_probe.so")
@@ -144,7 +144,7 @@ def test_fused_sdf_large_and_ragged(cuda):
 @pytest.mark.parametrize("M,N", [(64, 64), (64, 48), (16, 64), (48, 16)])
 def test_umma_transposed_gemm_weight_gradient_layout(cuda, M, N):
     """dW-style product D = A^T B with the sample axis as the MMA K dimension (MN-major operands straight from activation tiles).
-    The kernel dumps every TMEM lane; the test also reports where the M = 64 accumulator rows live."""
+    The kernel dumps every accumulator lane; the test also reports where the M = 64 accumulator rows live."""
     from permuto_sdf_b200._lib import call
     torch.manual_seed(M * 100 + N)
     A = torch.randn(128, M, device="cuda")
@@ -159,18 +159,15 @@ def test_umma_transposed_gemm_weight_gradient_layout(cuda, M, N):
     for m in range(M):
         err = (dump[:, :N] - want[m][None, :]).abs().max(dim=1).values
         lane = int(err.argmin())
-        assert float(err[lane]) < 2e-3 * float(want.abs().max()), "row %d not found in TMEM (best lane %d, err %g)" % (m, lane, float(err[lane]))
+        assert float(err[lane]) < 2e-3 * float(want.abs().max()), "row %d not found (best lane %d, err %g)" % (m, lane, float(err[lane]))
         lanes.append(lane)
-    import os
-    os.makedirs("gpurun_out", exist_ok=True)
-    with open("gpurun_out/umma_m64_layout.txt", "a") as f:
-        f.write("M=%d N=%d accumulator row -> TMEM lane: %s\n" % (M, N, lanes))
+    print("M=%d N=%d accumulator row -> lane: %s" % (M, N, lanes))
     assert lanes == list(range(M)) or lanes == [(m // 16) * 32 + (m % 16) for m in range(M)], lanes
 
 
 @pytest.mark.parametrize("L,N,it", [(16, 5000, 20000), (8, 129, 0), (24, 2000, 20000), (16, 65536, 20000)])
 def test_fused_rgb_forward_matches_model(cuda, L, N, it):
-    """fused colour network (encoding + SH + normal + geom -> Lipschitz MLP on tcgen05) against the modular RGB model"""
+    """fused colour network (encoding + SH + normal + geom -> Lipschitz MLP on the tensor cores) against the modular RGB model"""
     from permuto_sdf import Sphere
     from permuto_sdf_b200.fused import FusedRGB
     from permuto_sdf_b200.models import RGB
@@ -293,7 +290,7 @@ def test_fused_kernels_tile_boundaries(cuda, N):
 
 @pytest.mark.parametrize("n", [1000, 128 * 37 + 5, 65536])
 def test_dual_group_forward_equals_lock_step_forward(cuda, n):
-    """k_sdf_fused_dual (two independent 64-sample groups per CTA, M = 64 MMAs, 16x256b TMEM loads) against k_sdf_fused<true> (one
+    """k_sdf_fused_dual (two independent 64-sample groups per CTA, M = 64 MMAs, fragment-layout accumulator loads) against k_sdf_fused<true> (one
     128-sample tile per CTA): same arithmetic per sample -> identical sdf, gradient and geometric feature"""
     from permuto_sdf import Sphere
     from permuto_sdf_b200 import call

@@ -1,6 +1,6 @@
 """CPU tests that pin the C ray-path oracle (oracle/rayops_oracle.c): known-answer vectors, structural
 invariants, and -- when tests/golden/ref_*.npz exist -- fixtures produced by the reference's own CUDA
-kernels on a B200 (tests/golden/make_ref_golden.py)."""
+kernels (tests/golden/make_ref_golden.py)."""
 import glob
 import os
 
@@ -202,7 +202,7 @@ def test_backward_kernels_against_finite_differences(scene):
 GOLDEN = sorted(glob.glob(os.path.join(os.path.dirname(__file__), "golden", "ref_*.npz")))
 
 
-@pytest.mark.skipif(not GOLDEN, reason="reference-made fixtures not generated yet (tests/golden/make_ref_golden.py on a B200)")
+@pytest.mark.skipif(not GOLDEN, reason="reference-made fixtures not generated yet (tests/golden/make_ref_golden.py on a GPU)")
 def test_oracle_matches_reference_made_fixtures():
     """Fixtures = outputs of the reference's own kernels (oracle/_ref) on seeded inputs; see make_ref_golden.py"""
     import golden.check_golden as cg

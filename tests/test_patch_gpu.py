@@ -1,5 +1,5 @@
 """permuto_sdf_b200.patch_reference_models: reference-shaped classes (tests/refshape_models.py: the layout and formulas of
-permuto_sdf_py/models/models.py, per-op kernels + autograd) evaluate through the fused tcgen05 kernels after the graft, with the same
+permuto_sdf_py/models/models.py, per-op kernels + autograd) evaluate through the fused tensor-core kernels after the graft, with the same
 values and parameter gradients; unpatch restores the per-op path."""
 import types
 

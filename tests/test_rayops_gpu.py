@@ -1,6 +1,6 @@
 """GPU parity tests of the ray-path kernels (through the C ABI / the `permuto_sdf` mirror) against
  (a) the C oracle (oracle/rayops_oracle.c) and
- (b) the reference's own CUDA kernels compiled for sm_100a (oracle/_ref/libpsdf_ref_gpu.so) when present.
+ (b) the reference's own CUDA kernels compiled for sm_90a (oracle/_ref/libpsdf_ref_gpu.so) when present.
 Integer / index results must match bit for bit; float results within the tolerance written in each test
 (north star: <= 1e-3 relative; we hold the ray path to <= 1e-6 absolute and report bit-exact fractions)."""
 import numpy as np

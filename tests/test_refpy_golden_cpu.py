@@ -1,5 +1,6 @@
-"""The reference-Python fixture (tests/golden/refpy_golden.npz) is reproducible: where /root/reference exists (the build container)
-the committed generator, run again, must give the committed arrays. Also checks the fixture's internal consistency everywhere."""
+"""The reference-Python fixture (tests/golden/refpy_golden.npz + refpy_golden_bg.npz) is reproducible: where a checkout of the original
+project is present (PERMUTO_SDF_REFERENCE, else its default location) the committed generator, run again, must give the committed arrays,
+and the graft works on the original classes. Also checks the fixture's internal consistency everywhere."""
 import os
 import subprocess
 import sys
@@ -10,10 +11,19 @@ import pytest
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
 FIX = os.path.join(HERE, "golden", "refpy_golden.npz")
+REF_PY = os.path.join(os.environ.get("PERMUTO_SDF_REFERENCE") or "/root/reference", "permuto_sdf_py")
+NO_REF = "needs a checkout of the original project (PERMUTO_SDF_REFERENCE or its default location)"
+
+
+def load_fixture(path):
+    """the fixture and its background-model part (<name>_bg.npz) as one dict"""
+    g = dict(np.load(path))
+    g.update(np.load(path[:-len(".npz")] + "_bg.npz"))
+    return g
 
 
 def test_fixture_is_complete():
-    G = np.load(FIX)
+    G = load_fixture(FIX)
     keys = set(G.keys())
     for need in ("sdf_out.sdf", "sdf_grad.lattice_rows", "curv_out.curvature", "rgb_out.rgb", "rgb_grad.mlp.lipshitz_bound_per_layer.0",
                  "rgb_grad.cal.weight_delta", "bg_out.density", "neus_free.weights", "neus_forced.g_sdf", "imp_out.samples_z", "trace_out.points"):
@@ -32,12 +42,12 @@ def test_fixture_is_complete():
         pytest.fail("no active Lipschitz clamp in the fixture")
 
 
-@pytest.mark.skipif(not os.path.isdir("/root/reference/permuto_sdf_py"), reason="the reference's Python exists only in the build container")
+@pytest.mark.skipif(not os.path.isdir(REF_PY), reason=NO_REF)
 def test_fixture_regenerates_from_the_reference(tmp_path):
     env = dict(os.environ, REFPY_GOLDEN_OUT=str(tmp_path / "again.npz"))
     r = subprocess.run([sys.executable, os.path.join(HERE, "golden", "make_refpy_golden.py")], env=env, capture_output=True, text=True, timeout=600)
     assert r.returncode == 0, r.stderr[-2000:]
-    a, b = np.load(FIX), np.load(str(tmp_path / "again.npz"))
+    a, b = load_fixture(FIX), load_fixture(str(tmp_path / "again.npz"))
     assert set(a.keys()) == set(b.keys())
     for k in a.keys():
         if a[k].dtype.kind == "f":
@@ -73,7 +83,7 @@ print("PATCH-OK")
 """
 
 
-@pytest.mark.skipif(not os.path.isdir("/root/reference/permuto_sdf_py"), reason="the reference's Python exists only in the build container")
+@pytest.mark.skipif(not os.path.isdir(REF_PY), reason=NO_REF)
 def test_patch_grafts_onto_the_real_reference_classes():
     """permuto_sdf_b200.patch_reference_models on the UNMODIFIED permuto_sdf_py/models/models.py (own process: oracle/refpy.py replaces
     sys.modules entries): methods replaced, instances keep parameters / state_dict keys / results, unpatch restores"""

@@ -2,7 +2,7 @@
 permuto_sdf_py/models/models.py (SDF, RGB + LipshitzMLP + Colorcal, NerfHash), volume_rendering_modules.py (VolumeRenderingNeus) and
 utils/sdf_utils.py (importance_sampling_sdf_model, sphere_trace) compute on seeded inputs when they run on CPU stand-ins of the two
 compiled modules (oracle/refpy.py; generator: tests/golden/make_refpy_golden.py, run in the build container). Here the same parameters
-are loaded through the reference's state_dict key names into this package's models and every path -- fused tcgen05 kernels and the
+are loaded through the reference's state_dict key names into this package's models and every path -- fused tensor-core kernels and the
 per-op kernels + autograd -- must reproduce values and gradients to <= 1e-3 relative (the north-star tolerance); the sampling drivers,
 run on an analytic SDF whose arithmetic is identical on both sides, must match bit for bit."""
 import os
@@ -18,7 +18,9 @@ TOL = 1e-3
 
 @pytest.fixture(scope="module")
 def G():
-    return dict(np.load(os.path.join(HERE, "golden", "refpy_golden.npz")))
+    g = dict(np.load(os.path.join(HERE, "golden", "refpy_golden.npz")))
+    g.update(np.load(os.path.join(HERE, "golden", "refpy_golden_bg.npz")))
+    return g
 
 
 def lattice_from_seed(seed, L, T, F, amp):          # same generator as tests/golden/make_refpy_golden.py

@@ -44,7 +44,7 @@ def test_sdf_and_gradient_match_oracle(trainer):
     # finite-difference variant of the reference API
     s1, g1, _ = m.get_sdf_and_gradient(pos.cuda(), it, method="finite_difference")
     assert rel(s1, s0) < 1e-3
-    # gradient-free evaluations are routed through the fused tcgen05 kernel
+    # gradient-free evaluations are routed through the fused tensor-core kernel
     assert getattr(m, "fused", None) is not None
     with torch.no_grad():
         s2, f2 = m(pos.cuda(), it)
@@ -197,7 +197,7 @@ def test_fused_sphere_trace_equals_masked_loop(trainer, with_grid):
     res = {}
     for fused in (False, True):
         tr.FUSED_SPHERE_TRACE = fused
-        with torch.no_grad():           # rendering context: the loop's network evaluations take the same fused tcgen05 path
+        with torch.no_grad():           # rendering context: the loop's network evaluations take the same fused tensor-core path
             pts, sdf, grads, geom, rsp = tr.sphere_trace(12, to, td, m, True, 0.9, 1e-3, grid)
         res[fused] = (pts.clone(), sdf.clone(), grads.clone())
     tr.FUSED_SPHERE_TRACE = True
@@ -354,3 +354,45 @@ def test_trainer_checkpoint_roundtrip_and_chunked_render(cuda, tmp_path):
     assert bg_c is None and rgb_c.shape == (256, 3)
     assert float((rgb_c - full[0][0]).abs().max()) < 1e-5 and float((ws_c - full[0][4]).abs().max()) < 1e-5
     test_graph_gpu._fresh_rngs()
+
+
+def test_deterministic_mode_reproduces_training_bits(cuda):
+    """Trainer(deterministic=True): two runs of the direct iteration from the same seed and inputs (occupancy refresh included) give
+    bit-identical losses, gradients and parameters -- the fixed-point gradient reductions do not depend on the order of the atomics"""
+    from permuto_sdf import OccupancyGrid, RaySampler, VolumeRendering
+    from permuto_sdf_b200.train import HyperParams, Trainer
+    g = torch.Generator().manual_seed(7)
+    pix = [torch.randint(0, 32 * 32, (256,), generator=g, dtype=torch.int32).cuda() for _ in range(3)]
+    img = [torch.randint(0, 2, (256,), generator=g, dtype=torch.int32).cuda() for _ in range(3)]
+    rgb, mask, K, tf = (torch.from_numpy(a).cuda() for a in scenes.synthetic_reel(nimg=2, H=32, W=32))
+
+    class Reel:
+        rgb_reel, mask_reel, K_reel, tf_world_cam_reel = rgb, mask, K, tf
+
+    def run():
+        for c in (OccupancyGrid, RaySampler, VolumeRendering):      # the class generators start from their initial state
+            c.m_rng.to_host()
+            fresh = type(c.m_rng)()
+            c.m_rng.state, c.m_rng.inc = fresh.state, fresh.inc
+        hp = HyperParams()
+        hp.nr_rays = 256
+        tr = Trainer(hp, nr_levels=8, capacity=2 ** 14, sdf_hidden=32, nr_images=2, occupancy_resolution=64, seed=3, optimizer="fused",
+                     deterministic=True)
+        tr.set_analytic_scene()
+        tr.iter_nr = 20000
+        out = []
+        for i in range(3):
+            loss = tr.step_from_reel(Reel, pix[i], img[i], update_occupancy=True, optimizer_step=False)
+            torch.cuda.synchronize()
+            out.append(torch.tensor([float(loss)]))
+            out += [p.grad.detach().clone() for p in tr.params if p.grad is not None]
+            tr.optimizer_step()
+        out += [p.detach().clone() for p in tr.params] + [tr.occupancy_grid.get_grid_values().clone()]
+        return out
+
+    try:
+        a, b = run(), run()
+    finally:
+        from permuto_sdf_b200._lib import call
+        call("psdf_set_deterministic", 0, 0, 0)
+    assert len(a) == len(b) and all(torch.equal(x, y) for x, y in zip(a, b))

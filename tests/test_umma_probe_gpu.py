@@ -1,4 +1,4 @@
-"""tcgen05 conventions the fused backward kernels rely on, read off the hardware (tests/probe/umma_probe.cu)."""
+"""wgmma conventions the fused backward kernels rely on, read off the hardware (tests/probe/umma_probe.cu)."""
 import ctypes
 import os
 

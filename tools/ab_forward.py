@@ -1,4 +1,4 @@
-"""A/B timing of the value + tangent SDF forward variants (lock-step 128-sample tiles vs two 64-sample groups per CTA) on a B200.
+"""A/B timing of the value + tangent SDF forward variants (lock-step 128-sample tiles vs two 64-sample groups per CTA) on the GPU.
 usage (under gpurun): python tools/ab_forward.py   -> prints us per launch for N = 8192, 65536, 1048576 samples along rays"""
 import os
 import sys

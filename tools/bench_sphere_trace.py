@@ -46,7 +46,7 @@ def main():
     d = torch.nn.functional.normalize(d, dim=-1).contiguous()
     o = torch.tensor([0.0, 0.0, -1.5], device="cuda").expand_as(d).contiguous()
     out = {}
-    torch.set_grad_enabled(False)          # rendering: every network evaluation takes the fused tcgen05 path
+    torch.set_grad_enabled(False)          # rendering: every network evaluation takes the fused tensor-core path
     tr.FUSED_SPHERE_TRACE_MAX_RAYS = 1 << 30          # compare both paths at every size
     for fused in (True, False):
         tr.FUSED_SPHERE_TRACE = fused

@@ -1,6 +1,6 @@
 """'What would this phase cost if it were free' timings of the lock-step value + tangent forward (k_sdf_fused<true>) at 65 536 samples:
-PSDF_EXPERIMENT_KNOCKOUT bit 0 skips the encoder, bit 1 the MMAs, bit 2 the GELU arithmetic, bit 3 the operand-tile stores, bit 4 the TMEM loads, bit 5 the output stores (results are
-garbage; diagnostics). usage (under gpurun): python tools/knockout_forward.py"""
+PSDF_EXPERIMENT_KNOCKOUT bit 0 skips the encoder, bit 1 the MMAs, bit 2 the GELU arithmetic, bit 3 the operand-tile stores, bit 4 the accumulator loads, bit 5 the output stores (results are
+garbage; diagnostics). usage, on the GPU: python tools/knockout_forward.py"""
 import os
 import subprocess
 import sys
@@ -31,9 +31,8 @@ with torch.no_grad():
     print("%%.1f" %% t(lambda: f(pos, 20000, with_gradient=True)))
 ''' % (ROOT, os.path.join(ROOT, "tests"), os.path.join(ROOT, "compat"))
 NAMES = {0: "everything", 1: "no encoder", 2: "no MMA", 4: "no GELU", 8: "no operand stores", 12: "no GELU, no stores",
-         14: "no MMA, GELU, stores", 16: "no TMEM loads", 32: "no output stores", 15: "TMEM loads + barriers + outputs",
-         63: "barriers only (sync skeleton)", 127: "skeleton, mbarrier.arrive instead of tcgen05.commit",
-         191: "skeleton, no fence.proxy.async", 128: "everything but fence.proxy.async (wrong results)"}
+         14: "no MMA, GELU, stores", 16: "no accumulator loads", 32: "no output stores", 15: "accumulator loads + barriers + outputs",
+         63: "barriers only (sync skeleton)", 191: "skeleton, no fence.proxy.async", 128: "everything but fence.proxy.async (wrong results)"}
 for k, name in NAMES.items():
     env = dict(os.environ, PSDF_EXPERIMENT_KNOCKOUT=str(k))
     out = subprocess.run([sys.executable, "-c", CODE], env=env, capture_output=True, text=True)

@@ -1,4 +1,4 @@
-"""Per-kernel timings on a B200 (CUDA events, warm, median of reps): our kernels, and the reference's own
+"""Per-kernel timings on the GPU (CUDA events, warm, median of reps): our kernels, and the reference's own
 kernels (oracle/_ref) on the same inputs where available. Writes gpurun_out/microbench.json.
 usage: python tools/microbench.py [--rays 512] [--samples 128] [--levels 16]"""
 import argparse
@@ -41,7 +41,7 @@ def main():
     import permutohedral_encoding as pe
     from permuto_sdf import OccupancyGrid, Sphere, VolumeRendering as VR
     res = {}
-    peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json"))) if os.path.exists(os.path.join(ROOT, "MEASURED_PEAKS.json")) else {"hbm_gbs": 6650.0}
+    peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json"))) if os.path.exists(os.path.join(ROOT, "MEASURED_PEAKS.json")) else {"hbm_gbs": 3350.0}
     hbm = peaks["hbm_gbs"]
     flush = torch.empty(256 * 1024 * 1024 // 4, device="cuda")
     N, L, T = a.rays * a.samples, a.levels, a.capacity

@@ -1,6 +1,6 @@
 """Per-kernel summary (one CSV row per kernel launch) of an `ncu --set full` report: duration, DRAM bytes, registers, issue / tensor-pipe
 utilisation. usage (CPU container, on a .ncu-rep brought back from the GPU box):
-  python tools/ncu_summary.py gpurun_out/prof.ncu-rep > profiles/rN_ncu_kernels.csv"""
+  python tools/ncu_summary.py prof.ncu-rep > ncu_kernels.csv"""
 import csv
 import re
 import subprocess
