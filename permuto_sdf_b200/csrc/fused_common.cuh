@@ -204,6 +204,36 @@ __device__ __forceinline__ void store8(uint8_t* a_hi, uint8_t* a_lo, int row, in
     *reinterpret_cast<uint4*>(a_hi + off) = make_uint4(h[0], h[1], h[2], h[3]);
     *reinterpret_cast<uint4*>(a_lo + off) = make_uint4(l[0], l[1], l[2], l[3]);
 }
+// bf16 hi / lo pair of two adjacent columns of one row -> the two operand tiles (4-byte stores; a warp covers whole 128-byte cores)
+__device__ __forceinline__ void store_pair(uint8_t* t_hi, uint8_t* t_lo, int row, int col, float x0, float x1) {
+    uint32_t h, l;
+    umma::split2_bf16(x0, x1, h, l);
+    const int off = (row >> 3) * kSBO_A + (col >> 3) * kLBO + (row & 7) * 16 + (col & 7) * 2;
+    *reinterpret_cast<uint32_t*>(t_hi + off) = h;
+    *reinterpret_cast<uint32_t*>(t_lo + off) = l;
+}
+// fragment row / column of accumulator entry 4 j + 2 h + b of rows 64 mh .. 64 mh + 63 (umma::wg_mma_regs layout; warp w of the
+// warpgroup, lane t)
+__device__ __forceinline__ int frag_row(int mh, int h) { return 64 * mh + 16 * ((threadIdx.x >> 5) & 3) + (threadIdx.x & 31) / 4 + 8 * h; }
+__device__ __forceinline__ int frag_col(int j) { return 8 * j + 2 * (threadIdx.x & 3); }
+// columns [n0, n0 + N) of rows 64 mh .. 64 mh + 63 of D_s = A_s W^T for the value (s = 0) and tangent (s = 1) stream into the issuing
+// warpgroup's registers: the value and the tangent of one (row, column) land in the same thread. Stream s's A tiles are
+// set + 2 s kATileBytes (hi, lo); the weight tile is [Np rows][Kp] K-major.
+template <int N>
+__device__ __forceinline__ void rows_product2(float (*acc)[16], int mh, const uint8_t* set, const uint8_t* w_hi, const uint8_t* w_lo, int Kp,
+                                              int n0) {
+    const uint32_t sbo_w = (Kp / 8) * kLBO, wo = (uint32_t)(n0 / 8) * sbo_w, ao = (uint32_t)(mh * 8 * kSBO_A);
+    const uint64_t dwh = umma::make_desc(umma::smem_u32(w_hi) + wo, kLBO, sbo_w), dwl = umma::make_desc(umma::smem_u32(w_lo) + wo, kLBO, sbo_w);
+    umma::wgmma_fence();
+#pragma unroll
+    for (int s = 0; s < 2; s++) {
+        const uint8_t* a = set + s * 2 * kATileBytes;
+        const uint64_t dah = umma::make_desc(umma::smem_u32(a) + ao, kLBO, kSBO_A), dal = umma::make_desc(umma::smem_u32(a + kATileBytes) + ao, kLBO, kSBO_A);
+        umma::wg_mma_regs<N, 0, 0>(acc[s], dah, dal, dwh, dwl, (2 * kLBO) >> 4, (2 * kLBO) >> 4, Kp / 16, false);
+    }
+    umma::wgmma_commit();
+    umma::wgmma_wait0();
+}
 
 
 // column halves of an N-column product in units of 16 columns (MMA N % 16 == 0); the second half may be empty

@@ -11,17 +11,17 @@
 //   3. reverse sweep l = 3..0: zbar^(l) tile -> MMA with W_l^T -> abar_l -> zbar^(l-1) = abar_l gelu'(z^(l-1)); beside that GEMM the
 //      layer's input a_l is rebuilt from the stored z^(l-1) (a_0 returns by TMA) and the WEIGHT GRADIENT dW_l = zbar^(l)^T a_l is
 //      formed on the tensor cores from the two tiles as they sit in shared memory: the sample axis is the MMA K dimension and an
-//      operand tile in the K-major core-matrix layout is an MN-major operand for that product (see fused_sdf_bwd.cu). The four
-//      accumulators do not fit beside the z^(l) (320 + 128 work + 416 columns), so dW_l lives in the columns of the z^(l) that is
-//      already dead and is flushed per tile and layer with red.global.add.v4.f32 (instead of a 512 KB spill per tile + a second
-//      kernel that re-reads it);
+//      operand tile in the K-major core-matrix layout is an MN-major operand for that product (see fused_sdf_bwd.cu). The issuing
+//      warpgroups add the product from their registers to the CTA's fixed-point sums (each slot owned by one thread: no atomics); the
+//      CTA flushes the four sums once, after its last tile -- 37 k reductions per CTA instead of per tile, with the same totals as a
+//      per-tile fixed-point flush;
 //      bias gradients = column sums (shuffles + shared atomics);
 //   4. abar_0 -> lattice scatter (warp-aggregated red.global.add.v2.f32), normal -> sdf-gradient, geom gradient.
 // Deterministic mode (common.cuh): every gradient is summed in fixed point instead and added to the float gradients by the flush that
 // follows the launch.
 // Weights stream per layer through one 64 KB buffer by TMA; the next block is requested as soon as the MMAs that read the
 // current one have retired, so the copy hides behind the epilogue.
-// Accumulator map (umma.cuh): [0,128) z^(0) then dW_0 | [128,256) z^(1) then dW_1 | [256,320) z^(2), [256,384) dW_2, [320,384) dW_3 | [384,512) work.
+// Accumulator map (umma.cuh): [0,128) z^(0) | [128,256) z^(1) | [256,384) z^(2) | [384,512) work. Weight-gradient sums: g_dw_rgb_bwd.
 #include "fused_common.cuh"
 #include "fused_rgb_common.cuh"
 #include "../../include/psdf_b200.h"
@@ -31,6 +31,9 @@ using namespace psdf_rgb;
 
 namespace {
 __device__ float g_acc_rgb_bwd[(size_t)kAccCtas * kTile * 512];     // accumulator areas (umma.cuh)
+// weight-gradient sums of each CTA in fixed point (common.cuh fx_of), [CTA][layer][128 rows][128 columns]
+constexpr int kDwSlots = kNL * 128 * 128;
+__device__ unsigned long long g_dw_rgb_bwd[(size_t)kAccCtas * kDwSlots];
 constexpr int kFxW = kDetRgbW, kFxB = 4 * kDetRgbW;    // weight / bias offsets in DetBufs::rgb_mlp
 constexpr int kRgbSpillBytes = 2 * kWTileBytes;      // [hi | lo] of one operand tile
 
@@ -41,20 +44,50 @@ struct RgbSpill {
     unsigned long long* fx_lattice;   // deterministic mode: fixed-point accumulators (DetBufs::rgb_lattice, ::rgb_mlp), else NULL
     unsigned long long* fx_mlp;
 };
+// Rows [m0, m0 + 64) x columns [c0, c0 + N) of this tile's dW_l in the issuing warpgroup's registers, then added in fixed point to the
+// CTA's sums `dw` ([128 rows][128 columns] of the layer; `first`: the CTA's first tile, which sets them). Every slot belongs to one
+// thread for the whole launch (the fragment position), so the read-modify-write needs no atomics. Each tile's product is rounded to
+// the fixed-point grid before it is added, as a per-tile flush would round it: the totals do not depend on how tiles map to CTAs.
+template <int N>
+__device__ __forceinline__ void dw_rows_fx(unsigned long long* dw, int m0, int c0, uint64_t dzh, uint64_t dzl, uint64_t dah, uint64_t dal,
+                                           bool first) {
+    float d[N / 2];
+#pragma unroll
+    for (int i = 0; i < N / 2; i++) d[i] = 0.f;
+    umma::wgmma_fence();
+    // 16 samples = 2 eight-row groups per K step
+    umma::wg_mma_regs<N, 1, 1>(d, dzh, dzl, dah, dal, (2 * kWSBO) >> 4, (2 * kWSBO) >> 4, kTile / 16, false);
+    umma::wgmma_commit();
+    umma::wgmma_wait0();
+#pragma unroll
+    for (int h = 0; h < 2; h++) {
+        unsigned long long* p = dw + (size_t)frag_row(0, h) * 128 + m0 * 128 + c0;
+#pragma unroll
+        for (int j = 0; j < N / 8; j++) {
+            ulonglong2* q = reinterpret_cast<ulonglong2*>(p + frag_col(j));
+            ulonglong2 v = first ? make_ulonglong2(0ull, 0ull) : *q;
+            v.x += fx_of(d[4 * j + 2 * h]);
+            v.y += fx_of(d[4 * j + 2 * h + 1]);
+            *q = v;
+        }
+    }
+}
 // dW_l = zbar^(l)^T a_l over the 128 samples of the tile: both tiles consumed as MN-major operands (one warpgroup, `half` = 0 / 1).
-// M = 128: the two warpgroups take rows 0..63 / 64..127 (accumulator lane m); M = 64: columns [0, na) / [na, N) of one M = 64 product
-// (lane (m / 16) * 32 + m % 16).
-__device__ __forceinline__ void issue_dw_w(uint32_t tmem_d, int half, const uint8_t* z_hi, const uint8_t* a_hi, int M, int N) {
+// M = 128: the two warpgroups take rows 0..63 / 64..127; M = 64: columns [0, na) / [na, N) of one M = 64 product. Added to the CTA's
+// fixed-point sums (dw_rows_fx) in pieces of at most 32 columns (register budget).
+__device__ __forceinline__ void issue_dw_w(unsigned long long* dw, int half, const uint8_t* z_hi, const uint8_t* a_hi, int M, int N, bool first) {
     int m0 = 0, n0 = 0, nn = N;
     if (M == 128) m0 = 64 * half;
     else split_n(N, half, n0, nn);
     if (nn <= 0) return;
-    const uint32_t zh = umma::smem_u32(z_hi) + (uint32_t)(m0 / 8) * kLBO, ah = umma::smem_u32(a_hi) + (uint32_t)(n0 / 8) * kLBO;
+    const uint32_t zh = umma::smem_u32(z_hi) + (uint32_t)(m0 / 8) * kLBO;
     const uint64_t dzh = umma::make_desc(zh, kWSBO, kLBO), dzl = umma::make_desc(zh + kWTileBytes, kWSBO, kLBO);
-    const uint64_t dah = umma::make_desc(ah, kWSBO, kLBO), dal = umma::make_desc(ah + kWTileBytes, kWSBO, kLBO);
-    // 16 samples = 2 eight-row groups per K step
-    umma::wg_gemm<1, 1>(tmem_d + (uint32_t)n0 + ((uint32_t)m0 << 16), M == 64, dzh, dzl, dah, dal, (2 * kWSBO) >> 4, (2 * kWSBO) >> 4,
-                        (8 * kLBO) >> 4, kTile / 16, nn, false);
+    for (int p0 = 0; p0 < nn; p0 += 32) {
+        const uint32_t ah = umma::smem_u32(a_hi) + (uint32_t)((n0 + p0) / 8) * kLBO;
+        const uint64_t dah = umma::make_desc(ah, kWSBO, kLBO), dal = umma::make_desc(ah + kWTileBytes, kWSBO, kLBO);
+        if (nn - p0 >= 32) dw_rows_fx<32>(dw, m0, n0 + p0, dzh, dzl, dah, dal, first);
+        else dw_rows_fx<16>(dw, m0, n0 + p0, dzh, dzl, dah, dal, first);
+    }
 }
 
 __global__ void __launch_bounds__(kRgbThreads, 1)
@@ -102,12 +135,12 @@ k_rgb_fused_backward(RgbParams P, const float* __restrict__ pos, const float* __
     const uint32_t tmem_work = tmem_base + 384;
     const uint32_t lane_off = (uint32_t)((warp & 3) * 32) << 16;
     uint32_t w_phase = 0, mma_phase = 0, dw_phase = 0, a0_phase = 0;
-    // accumulator columns of dW_l (see the accumulator map above)
-    auto tmem_dw = [tmem_base](int l) -> uint32_t { return tmem_base + (l == 0 ? 0u : (l == 1 ? 128u : (l == 2 ? 256u : 320u))); };
+    unsigned long long* dw_cta = g_dw_rgb_bwd + (size_t)blockIdx.x * kDwSlots;    // this CTA's weight-gradient sums, layer l at l * 128 * 128
 
     const int ntiles = (P.N + kTile - 1) / kTile;
     if (tid == 0 && blockIdx.x < ntiles) load_layer_weights(s_w, blob, P.g, 0, false, &bars[0]);
     for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
+        const bool first_tile = tile == (int)blockIdx.x;
         const int n = tile * kTile + row;
         const bool valid = n < P.N;
         build_input_tile(P, lc, lattice, pos, dirs, sdf_grad, geom, n, valid, row, grp, s_a, s_a + kWTileBytes);
@@ -165,7 +198,7 @@ k_rgb_fused_backward(RgbParams P, const float* __restrict__ pos, const float* __
                 umma::mbar_arrive(&bars[1]);
             }
             if (dw_issuer && l == 3) {                    // a_3 | zbar^(3) are both in place
-                issue_dw_w(tmem_dw(3), wgi - 2, s_z, s_a, Mdw, P.g.Kp[3]);
+                issue_dw_w(dw_cta + 3 * 128 * 128, wgi - 2, s_z, s_a, Mdw, P.g.Kp[3], first_tile);
                 umma::mbar_arrive(&bars[2]);
             }
             // beside the MMAs: gelu'(z^(l-1)) of this thread's column chunks from the stored pre-activations, and the layer's
@@ -204,7 +237,7 @@ k_rgb_fused_backward(RgbParams P, const float* __restrict__ pos, const float* __
                 __syncthreads();
                 if (dw_issuer) {
                     if (l == 0) umma::mbar_wait(&bars[3], a0_phase);
-                    issue_dw_w(tmem_dw(l), wgi - 2, s_z, s_a, Mdw, Kp);
+                    issue_dw_w(dw_cta + l * 128 * 128, wgi - 2, s_z, s_a, Mdw, Kp, first_tile);
                     umma::mbar_arrive(&bars[2]);
                 }
             }
@@ -245,35 +278,6 @@ k_rgb_fused_backward(RgbParams P, const float* __restrict__ pos, const float* __
                     umma::tmem_ld16(tmem_work + lane_off + c * 16, ab);
 #pragma unroll
                     for (int i = 0; i < 16; i++) s_x[row * (K0 + 1) + c * 16 + i] = ab[i];
-                }
-            }
-            // ---- flush dW_l of this tile: accumulators -> global (+=). M = 128: accumulator row m in lane m; M = 64: row m in lane
-            // (m / 16) * 32 + m % 16. The four warps of a lane quadrant share the 16-column chunks.
-            {
-                const int q = warp & 3;
-                const int m = Mdw == 128 ? q * 32 + lane : q * 16 + lane;
-                const bool has_row = (Mdw == 128 || lane < 16) && m < P.g.N[l];
-                const int K = P.g.K[l];
-                float* dst_row = sp.gW[l] + (size_t)m * K;
-                unsigned long long* fx_row = det ? sp.fx_mlp + l * kFxW + (size_t)m * K : nullptr;
-                const bool vec = (K & 3) == 0 && ((uintptr_t)sp.gW[l] & 15) == 0;
-                for (int c = warp >> 2; c < Kp / 16; c += kRgbThreads / 128) {
-                    float acc[16];
-                    umma::tmem_ld16(tmem_dw(l) + lane_off + c * 16, acc);
-                    if (has_row && det) {
-#pragma unroll
-                        for (int i = 0; i < 16; i++) if (c * 16 + i < K) fx_add(fx_row + c * 16 + i, acc[i]);
-                    } else if (has_row) {
-#pragma unroll
-                        for (int i = 0; i < 16; i += 4) {
-                            const int k = c * 16 + i;
-                            if (vec && k + 3 < K) red_v4(dst_row + k, acc[i], acc[i + 1], acc[i + 2], acc[i + 3]);
-                            else {
-#pragma unroll
-                                for (int jj = 0; jj < 4; jj++) if (k + jj < K) atomicAdd(dst_row + k + jj, acc[i + jj]);
-                            }
-                        }
-                    }
                 }
             }
         }
@@ -338,6 +342,22 @@ k_rgb_fused_backward(RgbParams P, const float* __restrict__ pos, const float* __
         __syncthreads();     // exchange tile / accumulators free for the next tile
     }
     __syncthreads();
+    // ---- weight gradients of this CTA: fixed-point sums -> the deterministic accumulators (integer atomics, exact), or their float
+    // value -> the gradients (+=)
+    if ((int)blockIdx.x < ntiles) {
+#pragma unroll 1
+        for (int l = 0; l < kNL; l++) {
+            const int K = P.g.K[l];
+            const unsigned long long* src = dw_cta + l * 128 * 128;
+            for (int i = tid; i < P.g.N[l] * K; i += kRgbThreads) {
+                const int m = i / K, k = i - m * K;
+                const unsigned long long v = src[m * 128 + k];
+                if (v == 0ull) continue;
+                if (det) atomicAdd(sp.fx_mlp + l * kFxW + i, v);
+                else atomicAdd(sp.gW[l] + i, (float)((double)(long long)v / kFxScale));
+            }
+        }
+    }
     for (int i = tid; i < kNL * 128; i += kRgbThreads) {
         int l = i >> 7, c = i & 127;
         if (det) { if (c < P.g.N[l] && s_gb[i] != 0ull) atomicAdd(sp.fx_mlp + kFxB + l * 128 + c, s_gb[i]); }

@@ -49,15 +49,6 @@ template <bool TAN> struct FwdCfg { static constexpr int kThreads = TAN ? kFused
 // accumulator areas (umma.cuh) of the kernels of this file
 __device__ float g_acc_tan[(size_t)kAccCtas * kTile * 256];
 
-// bf16 hi / lo pair of two adjacent columns of one row -> the two operand tiles (4-byte stores; a warp covers whole 128-byte cores)
-__device__ __forceinline__ void store_pair(uint8_t* t_hi, uint8_t* t_lo, int row, int col, float x0, float x1) {
-    uint32_t h, l;
-    umma::split2_bf16(x0, x1, h, l);
-    const int off = (row >> 3) * kSBO_A + (col >> 3) * kLBO + (row & 7) * 16 + (col & 7) * 2;
-    *reinterpret_cast<uint32_t*>(t_hi + off) = h;
-    *reinterpret_cast<uint32_t*>(t_lo + off) = l;
-}
-
 // ---------------------------------------------------------------------------------------------- value-only layers in registers
 // Layer l of a value-only 128-row tile (inference forward, sphere tracer): warpgroup mh forms rows 64 mh .. 64 mh + 63 of D = A W^T in
 // its registers (umma::wg_mma_regs fragments) and consumes them itself -- bias + GELU into the next layer's operand cores, or the
@@ -84,9 +75,6 @@ __device__ __forceinline__ void value_rows(float* acc, const MlpGeom& g, int l, 
         default: rows_product<64>(acc, mh, s_a, wh, wl, g.Kp[l]); break;
     }
 }
-// fragment row / column of accumulator entry 4 j + 2 h + b (warp w of the warpgroup, lane t)
-__device__ __forceinline__ int frag_row(int mh, int h) { return 64 * mh + 16 * ((threadIdx.x >> 5) & 3) + (threadIdx.x & 31) / 4 + 8 * h; }
-__device__ __forceinline__ int frag_col(int j) { return 8 * j + 2 * (threadIdx.x & 3); }
 // bias + GELU of a hidden layer's fragment -> the next layer's operand cores
 __device__ __forceinline__ void gelu_to_tiles(const float* acc, const float* bias, int Np, int mh, uint8_t* s_a) {
 #pragma unroll

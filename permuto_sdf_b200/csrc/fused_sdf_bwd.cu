@@ -22,8 +22,10 @@
 // Per 128-sample tile (512 threads: row = tid & 127, group g = tid >> 7 owns operand cores g, g+4, .. in the encoder phases
 // and the 16-column chunk g in the epilogues). Two 64 KB operand-tile buffers X, Y ([value hi | value lo | tangent hi | tangent lo]):
 //   1. encoder: a_0, ta_0 -> X; X leaves by ONE TMA store (64 KB / tile, re-read from L2 in step 4: the only spill left)
-//   2. forward recompute, layers 0..2: z_1, z_2 (value + tangent) STAY in the accumulator area (4 x 64 columns); a_1 -> Y, a_2 -> X, a_3 -> Y;
-//      gelu'(z_3), gelu''(z_3) tz_3 stay in registers (layer 3 is reversed right away)
+//   2. forward recompute, layers 0..2: each warpgroup forms a row half x column half of both streams in its registers (value and tangent
+//      of one (row, column) in the same thread) and writes a_1 -> Y, a_2 -> X, a_3 -> Y straight from the fragments; the raw z_1, z_2
+//      (value + tangent) STAY in the accumulator area (4 x 64 columns), z_3 passes through the work columns to give gelu'(z_3),
+//      gelu''(z_3) tz_3 in registers (layer 3 is reversed right away)
 //   3. seed zbar_4 -> X
 //   4. reverse sweep l = 3..0:  abar_l = zbar_{l+1} W_l uses the FORWARD weight tile as an MN-major B operand (no transposed
 //      copy, weights resident for the CTA's lifetime); while it runs, a_l / ta_l are rebuilt into Y from the stored z_l
@@ -102,8 +104,8 @@ __device__ __forceinline__ void store_set16(uint8_t* set, int row, int c, const 
     store8(set + 2 * kATileBytes, set + 3 * kATileBytes, row, 2 * c + 1, ta + 8);
 }
 
-// The wgmma sequences of a phase are issued by several warpgroups: warpgroups 0 / 1 issue the value / tangent stream of the forward
-// and reverse GEMMs, warpgroups 2 / 3 one half of the weight-gradient columns each. Every issuer owns its accumulator columns and
+// The wgmma sequences of a reverse step are issued by several warpgroups: warpgroups 0 / 1 issue the value / tangent stream of the
+// reverse GEMM, warpgroups 2 / 3 one half of the weight-gradient columns each. Every issuer owns its accumulator columns and
 // all its threads arrive on the phase's mbarrier (initialised with the issuers' thread count) once the results are stored.
 // one stream of  abar[128 x Kp] = zbar[128 x Np] W : A = zbar tiles K-major, B = the FORWARD weight tile [Np rows][Kp] read as an
 // MN-major operand (reduction over the rows: 8-row groups are sbo_w apart, the k cores kLBO); both row halves, one warpgroup
@@ -261,27 +263,22 @@ k_sdf_fused_backward(FusedParams P, Segments S, const float2* __restrict__ latti
         }
 
         PSDF_PHASE(kPhEncoder);
-        // ---------------- 2. forward recompute, layers 0..2. z_{l+1} | tz_{l+1} -> accumulator columns l * 128 (l = 0, 1) or the work columns (l = 2)
+        // ---------------- 2. forward recompute, layers 0..2. Warpgroup (mh, nh) = (wgi & 1, wgi >> 1) forms rows 64 mh .. 64 mh + 63 x column
+        // half nh of both streams in its registers and consumes them in place: a_{l+1} | ta_{l+1} -> the next operand set, and the raw
+        // z_{l+1} | tz_{l+1} -> accumulator columns l * 128 (l = 0, 1) or the work columns (l = 2) for the reverse sweep
         float g1[16], g2t[16];                 // gelu'(z_3), gelu''(z_3) tz_3 of this thread's chunk: consumed by the first reverse step
-        float seed[2][8];                      // upstream gradient columns of this thread (prefetched behind the layer-2 MMAs)
+        float seed[2][8];                      // upstream gradient columns of this thread (prefetched before the layer-2 MMAs)
 #pragma unroll 1
         for (int l = 0; l < 3; l++) {
+            if (l == 1 && tid == 0) umma::bulk_wait_read0();   // X is overwritten by this layer's epilogue: the store must have read it
             umma::fence_async_smem();
             __syncthreads();
             const uint8_t* at = (l == 1) ? s_Y : s_X;
             uint8_t* dst = (l == 1) ? s_X : s_Y;
             const uint32_t col = (l == 2) ? kColWork : (uint32_t)(l * 128);
-            if (gemm_issuer) {
-                if (l == 0 && tid == 0) {      // a_0 | ta_0 leave as they are (needed again for dW_0 at the end of the reverse sweep)
-                    umma::bulk_s2g(out.a0_spill + (size_t)tile * kSetBytes, s_X, kSetBytes);
-                    umma::bulk_commit();
-                }
-                const int s = wgi;
-                for (int mh = 0; mh < 2; mh++)
-                    issue_gemm(tmem_base + col + s * 64, mh, at + s * 2 * kATileBytes, at + s * 2 * kATileBytes + kATileBytes, s_w + P.g.w_hi[l],
-                               s_w + P.g.w_lo[l], P.g.Kp[l], P.g.Np[l]);
-                if (l == 1 && tid == 0) umma::bulk_wait_read0();   // X is overwritten by this layer's epilogue: the store must have read it
-                umma::mbar_arrive(&bars[1]);
+            if (l == 0 && tid == 0) {          // a_0 | ta_0 leave as they are (needed again for dW_0 at the end of the reverse sweep)
+                umma::bulk_s2g(out.a0_spill + (size_t)tile * kSetBytes, s_X, kSetBytes);
+                umma::bulk_commit();
             }
             if (l == 2) {                      // zbar_4 = [g_sdf, g_geom...] columns of this thread, loaded while the MMAs run
                 const int Np = P.g.Np[3], nout = P.g.N[3];
@@ -300,19 +297,50 @@ k_sdf_fused_backward(FusedParams P, Segments S, const float2* __restrict__ latti
                     }
                 }
             }
-            umma::mbar_wait(&bars[1], mma_phase);
-            mma_phase ^= 1;
-            const int c = grp;
-            if (c < P.g.Np[l] / 16) {
-                float z[16], tz[16];
-                umma::tmem_ld16(tlane + col + c * 16, z);
-                umma::tmem_ld16(tlane + col + 64 + c * 16, tz);
-                activations16(z, tz, reinterpret_cast<const float*>(s_w + P.g.bias[l]) + c * 16, g1, g2t);
-                store_set16(dst, row, c, z, tz);
+            const int mh = wgi & 1;
+            int n0, nn;
+            split_n(P.g.Np[l], wgi >> 1, n0, nn);
+            float acc[2][16];
+#pragma unroll
+            for (int i = 0; i < 16; i++) { acc[0][i] = 0.f; acc[1][i] = 0.f; }
+            if (nn == 32) rows_product2<32>(acc, mh, at, s_w + P.g.w_hi[l], s_w + P.g.w_lo[l], P.g.Kp[l], n0);
+            else if (nn == 16) rows_product2<16>(acc, mh, at, s_w + P.g.w_hi[l], s_w + P.g.w_lo[l], P.g.Kp[l], n0);
+            const float* bias = reinterpret_cast<const float*>(s_w + P.g.bias[l]);
+#pragma unroll
+            for (int j = 0; j < 4; j++) {
+                if (8 * j < nn) {
+#pragma unroll
+                    for (int h = 0; h < 2; h++) {
+                        const int r = frag_row(mh, h), c = n0 + frag_col(j);
+                        const float z[2] = {acc[0][4 * j + 2 * h], acc[0][4 * j + 2 * h + 1]}, tz[2] = {acc[1][4 * j + 2 * h], acc[1][4 * j + 2 * h + 1]};
+                        float* zp = umma::acc_ptr((uint32_t)r, col + (uint32_t)c);
+                        *reinterpret_cast<float2*>(zp) = make_float2(z[0], z[1]);
+                        *reinterpret_cast<float2*>(zp + 64) = make_float2(tz[0], tz[1]);
+                        float a[2], ta[2];
+#pragma unroll
+                        for (int b = 0; b < 2; b++) {
+                            const float zz = z[b] + bias[c + b];
+                            const GeluEval ge = gelu_eval(zz);
+                            a[b] = zz * ge.cdf;
+                            ta[b] = fmaf(zz, ge.pdf, ge.cdf) * tz[b];
+                        }
+                        store_pair(dst, dst + kATileBytes, r, c, a[0], a[1]);
+                        store_pair(dst + 2 * kATileBytes, dst + 3 * kATileBytes, r, c, ta[0], ta[1]);
+                    }
+                }
             }
         }
+        // every layer-2 product has completed (a_2 in X is dead) and z_3 | tz_3 are stored: the GELU' / GELU'' factors of the first
+        // reverse step, in the per-row layout of the reverse epilogues
+        __syncthreads();
+        if (grp < P.g.Np[2] / 16) {
+            float z[16], tz[16];
+            umma::tmem_ld16(tlane + kColWork + grp * 16, z);
+            umma::tmem_ld16(tlane + kColWork + 64 + grp * 16, tz);
+            activations16(z, tz, reinterpret_cast<const float*>(s_w + P.g.bias[2]) + grp * 16, g1, g2t);
+        }
         PSDF_PHASE(kPhForward);
-        // ---------------- 3. seed: zbar_4 = upstream gradient, tzbar_4 = e_0 -> X (a_2 in X is dead: the layer-2 MMAs completed)
+        // ---------------- 3. seed: zbar_4 = upstream gradient, tzbar_4 = e_0 -> X
         {
             const int Np = P.g.Np[3];
 #pragma unroll
