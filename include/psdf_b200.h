@@ -253,13 +253,13 @@ int psdf_sdf_sphere_trace(int N, int L, int T, const float* pos, const float* di
                           int nr_iters, float sdf_multiplier, float sdf_converged_tresh, const uint8_t* occupancy, int V, float extent,
                           const float trans[3], float sphere_radius, const float sphere_center[3], float* pos_out, uint8_t* converged,
                           int* queue_counter, void* stream);
-/* Training backward of psdf_sdf_fused_forward (double backward of encoding + MLP on the tensor cores, ONE kernel, weight gradients
- * formed on chip):
+/* Training backward of psdf_sdf_fused_forward (double backward of encoding + MLP on the tensor cores, weight gradients formed on
+ * chip; the lattice scatter is a second kernel at full occupancy):
  * upstream gradients g_sdf [N], g_grad [N,3], g_geom [N,out_dim-1] (any may be NULL) -> grad_lattice (+=), weight gradients
  * gW_l [N_l, K_l] (+=) and bias gradients gb_l [N_l] (+=). workspace: psdf_sdf_fused_backward_workspace_bytes(N) bytes of
- * scratch (the encoder operand tile of every 128-sample tile, written and re-read by the same CTA). Replaces loss.backward() through
- * SDF.get_sdf_and_gradient
- * (models.py:199-259). */
+ * scratch, per 128-sample tile 64 KB for the encoder operand tile (written and re-read by the same CTA) and 64 KB for the
+ * per-level encoder gradients handed to the scatter kernel (16 bytes per sample and level, sized for 32 levels). Replaces
+ * loss.backward() through SDF.get_sdf_and_gradient (models.py:199-259). */
 long long psdf_sdf_fused_backward_workspace_bytes(int N);
 int psdf_sdf_fused_backward(int N, int L, int T, const float* pos, const float* lattice, const float* scale_factor, const float* shift,
                             const float* window, float points_scaling, int hidden, int out_dim, const uint8_t* blob, const float* g_sdf,

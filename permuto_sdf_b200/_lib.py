@@ -168,10 +168,11 @@ def call(name, *args):
 
 # ---- instrumentation used by bench.py: count C-ABI calls / kernel launches and time them with CUDA events on the
 # launching stream. Kernel launches per entry point (the rest launch exactly one kernel):
-_KERNELS_PER_CALL = {"psdf_packed_compact_scan": 2, "psdf_vr_combine_uniform_samples_with_imp": 3}
+_KERNELS_PER_CALL = {"psdf_packed_compact_scan": 2, "psdf_vr_combine_uniform_samples_with_imp": 3,
+                     "psdf_sdf_fused_backward": 2, "psdf_sdf_fused_backward_multi": 2}     # tensor-core kernel + lattice scatter
 
 
-_KERNELS_FN = {}        # entry point -> launches as a function of its arguments (none at present: every backward is one kernel)
+_KERNELS_FN = {}        # entry point -> launches as a function of its arguments (none at present)
 _UNITS_FN = {"psdf_sdf_fused_forward_multi": lambda a: int(a[10]) + int(a[15]),
              "psdf_sdf_fused_backward_multi": lambda a: int(a[10]) + int(a[15]) + int(a[20])}
 _STATS = None

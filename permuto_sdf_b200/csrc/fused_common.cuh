@@ -295,6 +295,40 @@ __device__ __forceinline__ void scatter2(float* gtab, unsigned long long* ftab, 
     if (ftab) { fx_add(ftab + (size_t)idx * 2, cv.x); fx_add(ftab + (size_t)idx * 2 + 1, cv.y); }
     else red_v2(gtab + (size_t)idx * 2, cv);
 }
+// Encoder backward of one sample at one level, called by a whole warp (one sample per lane):
+//     lattice[idx_r] += w (B_r abar + dB_r tabar),  r = 0..3,   abar = (a0, a1), tabar = (t0, t1) of the level's two features
+// x, v: position and tangent direction; scale3 / shift3: the level's scale and shift; gtab / ftab: the level's float / fixed-point
+// gradient table (scatter2). Invalid lanes add nothing. aggregate: warp-uniform, sum the lanes that share a vertex first (match_any +
+// add_peers2, one reduction per distinct vertex); do_red = false issues no reduction (diagnostics, PSDF_EXPERIMENT_KNOCKOUT).
+__device__ __forceinline__ void scatter_level(const float* x, const float* v, const float* scale3, const float* shift3, float w, float a0,
+                                              float a1, float t0, float t1, bool valid, bool aggregate, bool do_red, int lane,
+                                              unsigned cap_mask, unsigned T, float* gtab, unsigned long long* ftab) {
+    float cf[3], dcf[3], e[4];
+#pragma unroll
+    for (int i = 0; i < 3; i++) {
+        cf[i] = __fmul_rn(__fadd_rn(x[i], shift3[i]), scale3[i]);
+        dcf[i] = v[i] * scale3[i];
+    }
+    elevate3(cf, e);
+    Simplex3 s;
+    locate3(e, s);
+    float db[5];
+    bary_tangent3(dcf, s, db);
+#pragma unroll
+    for (int r = 0; r < 4; r++) {
+        unsigned idx = vindex3(s, r, cap_mask, T);
+        float cb = s.bary[r] * w, cd = db[r] * w;
+        float2 cv = make_float2(cb * a0 + cd * t0, cb * a1 + cd * t1);
+        if (aggregate) {
+            unsigned key = valid ? idx : 0xffffffffu;
+            unsigned peers = __match_any_sync(kFull, key);
+            cv = add_peers2(peers, cv, lane);
+            if (valid && lane == __ffs(peers) - 1 && do_red) scatter2(gtab, ftab, idx, cv);
+        } else if (valid && (do_red || cv.x == 123.456f)) {
+            scatter2(gtab, ftab, idx, cv);
+        }
+    }
+}
 // column sums of 16 per-lane values over the 32 lanes of a warp with 16 shuffles (halving butterfly): afterwards both
 // lanes of the pair {2p, 2p+1} hold the sum of column `col` = bit-reversal-free index built from lane bits 4..1.
 __device__ __forceinline__ float colsum16(const float* v, int lane, int& col) {

@@ -1,7 +1,8 @@
 // Training backward of the fused encoding + SDF MLP (sm_90a, wgmma): given d loss / d {sdf, d sdf/dx, geom}
-// per sample it produces the lattice gradient (scatter-add fused in the kernel), the bias gradients and the weight
-// gradients -- ONE kernel, the weight-gradient products are formed on the tensor cores from the operand tiles while they
-// are still in shared memory and accumulate in the CTA's accumulator area (umma.cuh) over all tiles of the CTA.
+// per sample it produces the lattice gradient, the bias gradients and the weight gradients. Two kernels: the persistent
+// tensor-core kernel forms the weight-gradient products from the operand tiles while they are still in shared memory
+// (accumulated in the CTA's accumulator area, umma.cuh, over all tiles of the CTA) and hands abar_0 | tabar_0 to a
+// full-occupancy kernel that scatters them into the lattice gradient.
 //
 // What it replaces in the reference: `loss.backward()` through SDF.get_sdf_and_gradient
 // (permuto_sdf_py/models/models.py:199-259, create_graph=True) -- i.e. the double backward of the
@@ -33,9 +34,14 @@
 //      K-major operand tile IS an MN-major operand for that product, so X and Y are multiplied as they sit. The four dW
 //      accumulators (M = 64) share 2 x 64 columns: an M = 64 product is stored to lanes (m / 16) * 32 + m % 16, so a second
 //      accumulator lives at lane offset 16 of the same columns (tests/test_umma_probe_gpu.py).
-//   5. encoder backward: warp-aggregated red.global.add.v2.f32 into the lattice gradient.
+//      In the last step (l = 0) abar_0 | tabar_0 leave from the registers to the exchange region of the workspace, one float4
+//      (a0, a1, t0, t1) per level and sample, [level][sample slot]: a warp's 32 rows of one level are one contiguous 512-byte store.
+// The encoder backward is its own launch, k_sdf_lattice_scatter: warp-aggregated red.global.add.v2.f32 into the lattice gradient.
+// Inside the persistent kernel it was the longest phase of a tile (one CTA of 16 warps per SM, tensor cores idle, long dependent chains
+// of simplex recompute, match_any, shuffle sums and reductions); on its own it runs with every warp slot of the SM occupied. Its warps
+// are the rows of the persistent kernel's warps, so the match_any groups and the float peer sums are the same.
 // Deterministic mode (common.cuh): every gradient (lattice, weights, biases) is summed in fixed point instead and added to the float
-// gradients by the flush that follows the launch.
+// gradients by the flush that follows the two launches.
 // Accumulator map (512 columns): [0,256) z_1 | tz_1 | z_2 | tz_2, [256,384) work (value | tangent), [384,512) dW_0/dW_1, dW_2/dW_3.
 #include <cstdio>
 #include <cstdlib>
@@ -54,10 +60,11 @@ constexpr int kFxW = kDetSdfW, kFxB = 4 * kDetSdfW;    // weight / bias offsets 
 
 struct BwdOut {
     uint8_t* a0_spill;  // [ntiles][64 KB] encoder operand tiles, written and re-read by the same CTA
+    float4* xch;        // [L][xch_stride] abar_0 | tabar_0 (a0, a1, t0, t1) per level and sample slot (tile * 128 + row)
+    int xch_stride;     // sample slots = ntiles * 128
     float* gW[kNL];     // [N_l, K_l] (+=)
     float* gbias[kNL];  // [N_l]      (+=)
-    unsigned long long* fx_lattice;   // deterministic mode: fixed-point accumulators (DetBufs::sdf_lattice, ::sdf_mlp), else NULL
-    unsigned long long* fx_mlp;
+    unsigned long long* fx_mlp;       // deterministic mode: fixed-point accumulators (DetBufs::sdf_mlp), else NULL
     unsigned long long* phase_cycles;   // [16] += clock64 deltas of thread 0 per phase (PSDF_PHASE_TIMING=1, diagnostics), else NULL
 };
 // Up to kMaxSeg independent sample sets (the main samples, the curvature pass' shifted samples, the off-surface points of one training
@@ -73,8 +80,8 @@ struct Segments {
     const float* g_geom[kMaxSeg];
 };
 // phase ids of the diagnostic counters
-enum { kPhEncoder = 0, kPhForward = 1, kPhSeed = 2, kPhReverse3 = 3, kPhReverse2 = 4, kPhReverse1 = 5, kPhReverse0 = 6, kPhEncoderBwd = 7,
-       kPhFlush = 8, kPhTiles = 9 };
+enum { kPhEncoder = 0, kPhForward = 1, kPhSeed = 2, kPhReverse3 = 3, kPhReverse2 = 4, kPhReverse1 = 5, kPhReverse0 = 6, kPhFlush = 7,
+       kPhTiles = 8 };
 #define PSDF_PHASE(id)                                                                     \
     do {                                                                                   \
         if (out.phase_cycles && tid == 0) {                                                \
@@ -139,8 +146,7 @@ __device__ __forceinline__ void issue_dw_part(uint32_t tmem_d, const uint8_t* zs
 
 __global__ void __launch_bounds__(kBwdThreads, 1)
 k_sdf_fused_backward(FusedParams P, Segments S, const float2* __restrict__ lattice, const float* __restrict__ scale,
-                     const float* __restrict__ shift, const float* __restrict__ window, const uint8_t* __restrict__ blob,
-                     float* __restrict__ grad_lattice, BwdOut out) {
+                     const float* __restrict__ shift, const float* __restrict__ window, const uint8_t* __restrict__ blob, BwdOut out) {
     extern __shared__ __align__(128) uint8_t smem[];
     uint8_t* s_w = smem;                                   // forward operand blob (weights hi/lo + biases), resident
     uint8_t* s_X = smem + P.g.total;
@@ -152,7 +158,6 @@ k_sdf_fused_backward(FusedParams P, Segments S, const float2* __restrict__ latti
     const bool det = out.fx_mlp != nullptr;
     uint64_t* bars = reinterpret_cast<uint64_t*>(s_gb + kNL * 64);   // [0] TMA loads, [1] mma, [2] dW mma
     float* s_seed = reinterpret_cast<float*>(bars + 5);   // [128][(out_dim - 1) | 1] upstream d loss / d geom of the tile (coalesced copy)
-    float* s_x = reinterpret_cast<float*>(s_X);            // exchange tile abar_0 | tabar_0 : [128][2*Kp0+1] fp32 (aliases X, Y)
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int row = tid & 127, grp = tid >> 7;
@@ -445,60 +450,20 @@ k_sdf_fused_backward(FusedParams P, Segments S, const float2* __restrict__ latti
                         else atomicAdd(&s_gbf[(l - 1) * 64 + c * 16 + colb], cs);
                     }
                 }
-            } else {
-                // abar_0 | tabar_0 for the encoder backward (fp32 exchange tile over X and Y, which no MMA reads any more)
-                if (have) {
+            } else if (have) {
+                // abar_0 | tabar_0 of this row's levels (columns 2 l, 2 l + 1) -> the exchange region, for k_sdf_lattice_scatter
+                float4* dst = out.xch + (size_t)tile * kTile + row;
 #pragma unroll
-                    for (int i = 0; i < 16; i++) {
-                        s_x[row * (2 * K0 + 1) + c * 16 + i] = ab[i];
-                        s_x[row * (2 * K0 + 1) + K0 + c * 16 + i] = tab_[i];
-                    }
+                for (int i = 0; i < 8; i++) {
+                    const int lv = c * 8 + i;
+                    if (lv < P.L) dst[(size_t)lv * out.xch_stride] = make_float4(ab[2 * i], ab[2 * i + 1], tab_[2 * i], tab_[2 * i + 1]);
                 }
             }
             PSDF_PHASE(kPhReverse3 + (3 - l));
         }
         ld_phase ^= 1;
-        __syncthreads();
-
-        // ---------------- 5. encoder backward: lattice[l][idx_r] += window_l (B_r abar_0[l] + dB_r tabar_0[l])
-        {
-            const float* xr = s_x + row * (2 * K0 + 1);
-            for (int l = grp; l < P.L; l += kGroups) {
-                float cf[3], dcf[3], e[4];
-#pragma unroll
-                for (int i = 0; i < 3; i++) {
-                    cf[i] = __fmul_rn(__fadd_rn(x[i], lc->shift[l * 4 + i]), lc->scale[l * 4 + i]);
-                    dcf[i] = v[i] * lc->scale[l * 4 + i];
-                }
-                elevate3(cf, e);
-                Simplex3 s;
-                locate3(e, s);
-                float db[5];
-                bary_tangent3(dcf, s, db);
-                const float w = lc->window[l];
-                const float a0 = xr[2 * l], a1 = xr[2 * l + 1], t0 = xr[K0 + 2 * l], t1 = xr[K0 + 2 * l + 1];
-                float* gtab = grad_lattice + (size_t)l * P.T * 2;
-                unsigned long long* ftab = det ? out.fx_lattice + (size_t)l * P.T * 2 : nullptr;
-                const bool aggregate = lc->scale[l * 4] < kAggregateBelowScale && !(P.knockout & 2);       // warp-uniform (l is)
-                const bool do_red = !(P.knockout & 1);            // diagnostics (PSDF_EXPERIMENT_KNOCKOUT): bit 0 no atomics, bit 1 no aggregation
-#pragma unroll
-                for (int r = 0; r < 4; r++) {
-                    unsigned idx = vindex3(s, r, P.cap_mask, (unsigned)P.T);
-                    float cb = s.bary[r] * w, cd = db[r] * w;
-                    float2 cv = make_float2(cb * a0 + cd * t0, cb * a1 + cd * t1);
-                    if (aggregate) {
-                        unsigned key = valid ? idx : 0xffffffffu;
-                        unsigned peers = __match_any_sync(kFull, key);
-                        cv = add_peers2(peers, cv, lane);
-                        if (valid && lane == __ffs(peers) - 1 && do_red) scatter2(gtab, ftab, idx, cv);
-                    } else if (valid && (do_red || cv.x == 123.456f)) {
-                        scatter2(gtab, ftab, idx, cv);
-                    }
-                }
-            }
-        }
-        __syncthreads();     // exchange tile / accumulators free for the next tile
-        PSDF_PHASE(kPhEncoderBwd);
+        // no barrier before the next tile: every thread has waited for this tile's last MMAs (bars[1], bars[2]), the only readers of
+        // X and Y, and the accumulator columns read above are rewritten only after the next tile's first __syncthreads
         if (out.phase_cycles && tid == 0) atomicAdd(out.phase_cycles + kPhTiles, 1ull);
     }
     // ---------------- weight gradients of this CTA: accumulators -> global (+=). Warp w reads lanes 32 (w & 3) .. +31 of column chunk w >> 2:
@@ -540,16 +505,54 @@ k_sdf_fused_backward(FusedParams P, Segments S, const float2* __restrict__ latti
     if (tid == 0) umma::bulk_wait0();      // spill stores complete before the CTA retires
 }
 
+// Encoder backward: lattice[l][idx_r] += window_l (B_r abar_0[l] + dB_r tabar_0[l]) from the exchange rows of k_sdf_fused_backward.
+// blockIdx.y = level (blocks of one level run together: its table of gradient accumulators stays in L2 while they land), warp =
+// 32 consecutive sample slots, i.e. the rows of one warp of the persistent kernel. The simplex and the barycentric tangent are
+// recomputed from the positions and upstream gradients.
+constexpr int kScatterThreads = 256;
+__global__ void __launch_bounds__(kScatterThreads, 8)
+k_sdf_lattice_scatter(FusedParams P, Segments S, const float4* __restrict__ xch, int xch_stride, const float* __restrict__ scale,
+                      const float* __restrict__ shift, const float* __restrict__ window, float* __restrict__ grad_lattice,
+                      unsigned long long* __restrict__ fx_lattice) {
+    const int slot = blockIdx.x * kScatterThreads + threadIdx.x;      // tile * 128 + row
+    if (slot >= xch_stride) return;                                  // whole warps (xch_stride % 128 == 0)
+    const int l = blockIdx.y, lane = threadIdx.x & 31, tile = slot / kTile;
+    const int seg = tile >= S.tile0[2] ? 2 : (tile >= S.tile0[1] ? 1 : 0);
+#define PSDF_SEG(f) (seg == 2 ? S.f[2] : (seg == 1 ? S.f[1] : S.f[0]))
+    const int n = (tile - PSDF_SEG(tile0)) * kTile + (slot % kTile);
+    const bool valid = n < PSDF_SEG(n);
+    const float* __restrict__ pos = PSDF_SEG(pos);
+    const float* __restrict__ g_grad = PSDF_SEG(g_grad);
+#undef PSDF_SEG
+    float x[3], v[3], sc[3], sh[3];
+#pragma unroll
+    for (int i = 0; i < 3; i++) {
+        x[i] = valid ? pos[(size_t)n * 3 + i] : 0.0f;
+        v[i] = (valid && g_grad) ? g_grad[(size_t)n * 3 + i] : 0.0f;
+        sc[i] = scale[l * 3 + i];
+        sh[i] = shift ? shift[l * 3 + i] : 0.0f;
+    }
+    const float w = window ? window[l] : 1.0f;
+    const float4 a = xch[(size_t)l * xch_stride + slot];
+    const bool aggregate = sc[0] < kAggregateBelowScale && !(P.knockout & 2);      // warp-uniform (l is)
+    const bool do_red = !(P.knockout & 1);            // diagnostics (PSDF_EXPERIMENT_KNOCKOUT): bit 0 no atomics, bit 1 no aggregation
+    scatter_level(x, v, sc, sh, w, a.x, a.y, a.z, a.w, valid, aggregate, do_red, lane, P.cap_mask, (unsigned)P.T,
+                  grad_lattice + (size_t)l * P.T * 2, fx_lattice ? fx_lattice + (size_t)l * P.T * 2 : nullptr);
+}
+
+// workspace per 128-sample tile: the encoder operand tiles (a_0 | ta_0, 64 KB), written by TMA store in the forward recompute and read
+// back by the same CTA for the first layer's weight gradient, and the exchange rows abar_0 | tabar_0 (16 bytes per sample and level,
+// sized for kMaxLevels so that the size depends on the sample count alone)
+constexpr long long kWsTileBytes = kSetBytes + (long long)kTile * kMaxLevels * sizeof(float4);
+
 #define ST ((cudaStream_t)stream)
 }  // namespace
 
 extern "C" {
 
-// workspace: the encoder operand tiles (a_0 | ta_0, 64 KB per 128-sample tile), written by TMA store in the forward recompute and read
-// back by the same CTA for the first layer's weight gradient
 long long psdf_sdf_fused_backward_workspace_bytes(int N) {
     const int ntiles = div_up(N > 0 ? N : 1, kTile);
-    return (long long)ntiles * kSetBytes;
+    return (long long)ntiles * kWsTileBytes;
 }
 
 static int launch_backward(int nseg, const int* Ns, const float* const* pos, const float* const* g_sdf, const float* const* g_grad,
@@ -584,27 +587,38 @@ static int launch_backward(int nseg, const int* Ns, const float* const* pos, con
     if (dbuf && (long long)L * T * 2 > dbuf->lattice_len) return PSDF_ERR_UNSUPPORTED;   // reserve more with psdf_set_deterministic
     BwdOut out;
     for (int l = 0; l < kNL; l++) { out.gW[l] = gW[l]; out.gbias[l] = gb[l]; }
-    out.fx_lattice = dbuf ? dbuf->sdf_lattice : nullptr;
     out.fx_mlp = dbuf ? dbuf->sdf_mlp : nullptr;
     out.a0_spill = workspace;
+    out.xch = reinterpret_cast<float4*>(workspace + (size_t)tiles * kSetBytes);
+    out.xch_stride = tiles * kTile;
     // diagnostics: PSDF_PHASE_TIMING=1 prints thread 0's clock64 breakdown per phase (average cycles per tile) after every launch
     static const bool timing = getenv("PSDF_PHASE_TIMING") && atoi(getenv("PSDF_PHASE_TIMING")) != 0;
     static unsigned long long* d_cycles = nullptr;
+    static cudaEvent_t ev[3];
     out.phase_cycles = nullptr;
     if (timing) {
-        if (!d_cycles) cudaMalloc(&d_cycles, 16 * sizeof(unsigned long long));
+        if (!d_cycles) {
+            cudaMalloc(&d_cycles, 16 * sizeof(unsigned long long));
+            for (auto& e : ev) cudaEventCreate(&e);
+        }
         cudaMemsetAsync(d_cycles, 0, 16 * sizeof(unsigned long long), ST);
         out.phase_cycles = d_cycles;
+        cudaEventRecord(ev[0], ST);
     }
     int dev = 0, sms = 132;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     const size_t smem = (size_t)P.g.total + 2 * kSetBytes + sizeof(LevelC) + kNL * 64 * sizeof(unsigned long long) + 64 + (size_t)kTile * (size_t)((out_dim - 1) | 1) * sizeof(float);
-    if ((size_t)128 * (2 * P.g.Kp[0] + 1) * 4 > (size_t)2 * kSetBytes || smem > 227 * 1024) return PSDF_ERR_UNSUPPORTED;
+    if (smem > 227 * 1024) return PSDF_ERR_UNSUPPORTED;
     { static bool optin_[64]; psdf::psdf_optin_smem(k_sdf_fused_backward, 227 * 1024, optin_); }
     k_sdf_fused_backward<<<min(min(tiles, sms), kAccCtas), kBwdThreads, smem, ST>>>(P, S, reinterpret_cast<const float2*>(lattice), scale_factor, shift, window,
-                                                                    blob, grad_lattice, out);
+                                                                    blob, out);
     PSDF_CHECK_LAUNCH();
+    if (timing) cudaEventRecord(ev[1], ST);
+    k_sdf_lattice_scatter<<<dim3(div_up(out.xch_stride, kScatterThreads), L), kScatterThreads, 0, ST>>>(
+        P, S, out.xch, out.xch_stride, scale_factor, shift, window, grad_lattice, dbuf ? dbuf->sdf_lattice : nullptr);
+    PSDF_CHECK_LAUNCH();
+    if (timing) cudaEventRecord(ev[2], ST);
     if (dbuf) {      // deterministic mode: fixed-point totals -> the float gradients (+=)
         FxSegs F;
         F.add(dbuf->sdf_lattice, grad_lattice, (long long)L * T * 2);
@@ -619,16 +633,19 @@ static int launch_backward(int nseg, const int* Ns, const float* const* pos, con
         cudaMemcpyAsync(h, d_cycles, sizeof(h), cudaMemcpyDeviceToHost, ST);
         cudaStreamSynchronize(ST);
         const double t = h[kPhTiles] ? (double)h[kPhTiles] : 1.0;
+        float ms_fused = 0.f, ms_scatter = 0.f;
+        cudaEventElapsedTime(&ms_fused, ev[0], ev[1]);
+        cudaEventElapsedTime(&ms_scatter, ev[1], ev[2]);
         fprintf(stderr, "[psdf_sdf_fused_backward N=%d tiles=%llu] cycles/tile: encoder %.0f forward %.0f seed %.0f rev3 %.0f rev2 %.0f rev1 %.0f rev0 %.0f "
-                        "encoder_bwd %.0f | flush/CTA %.0f\n", total, h[kPhTiles], h[0] / t, h[1] / t, h[2] / t, h[3] / t, h[4] / t, h[5] / t, h[6] / t, h[7] / t,
-                (double)h[kPhFlush] / min(tiles, sms));
+                        "| flush/CTA %.0f | fused kernel %.3f ms, lattice scatter %.3f ms\n", total, h[kPhTiles], h[0] / t, h[1] / t, h[2] / t, h[3] / t,
+                h[4] / t, h[5] / t, h[6] / t, (double)h[kPhFlush] / min(tiles, sms), ms_fused, ms_scatter);
     }
     return PSDF_OK;
 }
 
 // workspace of a multi-set launch: every set is padded to whole tiles
 long long psdf_sdf_fused_backward_multi_workspace_bytes(int N0, int N1, int N2) {
-    return (long long)(div_up(N0 > 0 ? N0 : 0, kTile) + div_up(N1 > 0 ? N1 : 0, kTile) + div_up(N2 > 0 ? N2 : 0, kTile) + 1) * kSetBytes;
+    return (long long)(div_up(N0 > 0 ? N0 : 0, kTile) + div_up(N1 > 0 ? N1 : 0, kTile) + div_up(N2 > 0 ? N2 : 0, kTile) + 1) * kWsTileBytes;
 }
 
 // grad_lattice, grad_W_l [N_l, K_l] and grad_bias_l are accumulated (+=).

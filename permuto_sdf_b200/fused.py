@@ -150,7 +150,7 @@ def _pad16(v):
 
 class _FusedSDFTrainFn(torch.autograd.Function):
     """forward: psdf_sdf_fused_forward (value + 3 tangent streams); backward: psdf_sdf_fused_backward (value + the tangent
-    along the upstream gradient, reverse sweep on the tensor cores, lattice scatter fused, then the tensor-core weight-gradient kernel)."""
+    along the upstream gradient, reverse sweep and weight gradients on the tensor cores, then the lattice-scatter kernel)."""
 
     @staticmethod
     def forward(ctx, points, lattice, W0, b0, W1, b1, W2, b2, W3, b3, window, fused):

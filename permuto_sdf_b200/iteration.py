@@ -18,7 +18,7 @@ CUDA graph. Here the same mathematics is issued directly:
     psdf_neus_head_loss_backward        d / d {sdf, grad, raw colour, shifted grad}, calibration gradients, tail zero-fill   1
     psdf_rgb_fused_backward_acc         colour network backward, d / d sdf-gradient accumulated in place            2 kernels
     psdf_lipschitz_backward4            4 normalisation backwards (+ Lipschitz-bound loss), into .grad               1
-    psdf_sdf_fused_backward_multi       the three SDF sample sets                                                    1
+    psdf_sdf_fused_backward_multi       the three SDF sample sets (tensor-core kernel + lattice scatter)             2 kernels
 
 Parameter gradients are accumulated straight into the flat-buffer optimizer's `.grad` views (which the AdamW kernel leaves zeroed).
 Every formula is the one of the autograd path; `tests/test_direct_iteration_gpu.py` compares loss and all parameter gradients of the
