@@ -1,6 +1,7 @@
 // Shared pieces of the fused encoding + MLP kernels (fused_sdf.cu: forward / inference, fused_sdf_bwd.cu: training
-// backward): MLP operand-blob geometry, permutohedral simplex helpers for D = 3, GELU and its derivatives, operand
-// tile stores (bf16 hi/lo split in the core-matrix operand layout) and the split-product GEMM issue.
+// backward, fused_rgb*.cu: colour network): MLP operand-blob geometry, permutohedral simplex helpers for D = 3, the encoder of
+// one level and its lattice scatter, GELU and its derivatives, operand tile stores (bf16 hi/lo split in the core-matrix operand
+// layout) and the split-product GEMM issue.
 #pragma once
 #include "common.cuh"
 #include "umma.cuh"
@@ -182,16 +183,81 @@ struct FusedParams {
     unsigned cap_mask;   // t_magic(T): multiplier of the division-free h mod T (any capacity, not only powers of two)
     float points_scaling;
     int in_dim;          // (L + E) * 2 feature columns
-    int free_levels = 0; // diagnostics only (PSDF_EXPERIMENT_FREE_LEVELS): the gathers of levels < free_levels read nothing (upper bound of
-                         // what staging those levels' table entries in shared memory could save); 0 in production
-    int skew = 1;        // k_sdf_fused_dual: group 1 starts half a sub-tile after group 0 (PSDF_SDF_FWD_SKEW=0 disables, A/B measurements)
-    int knockout = 0;    // diagnostics only (PSDF_EXPERIMENT_KNOCKOUT, k_sdf_fused<true>): bit 0 skip the encoder, bit 1 issue no MMA, bit 2 skip
-                         // the GELU arithmetic, bit 3 skip the operand-tile stores of the epilogue -- "what would this phase cost if it were
-                         // free" timings (results are garbage); 0 in production
+    int knockout = 0;    // diagnostics only (PSDF_EXPERIMENT_KNOCKOUT, k_sdf_lattice_scatter): bit 0 issue no reduction, bit 1 no warp
+                         // aggregation -- "what would this cost if it were free" timings (results are garbage); 0 in production
     MlpGeom g;
 };
 
+// ---------------------------------------------------------------------------------------------- encoder of one level (D = 3, F = 2)
+// Level constants in shared memory; scale / shift rows padded to 4 floats.
 struct LevelC { float scale[kMaxLevels * 4]; float shift[kMaxLevels * 4]; float window[kMaxLevels]; };
+__device__ __forceinline__ void load_level_consts(LevelC* lc, int L, const float* scale, const float* shift, const float* window, int tid,
+                                                  int nthreads) {
+    for (int i = tid; i < L * 3; i += nthreads) {
+        lc->scale[(i / 3) * 4 + (i % 3)] = scale[i];
+        lc->shift[(i / 3) * 4 + (i % 3)] = shift ? shift[i] : 0.0f;
+    }
+    for (int i = tid; i < L; i += nthreads) lc->window[i] = window ? window[i] : 1.0f;
+}
+// The two window-weighted features (a0, a1) = w sum_r B_r v_r of position x at level l. Also returns the simplex s and the four vertex
+// values v, from which the callers form tangents.
+__device__ __forceinline__ float2 level_features(const float* x, const LevelC* lc, int l, const float2* __restrict__ lattice, int T,
+                                                 unsigned cap_mask, Simplex3& s, float2* v) {
+    float cf[3], e[4];
+#pragma unroll
+    for (int i = 0; i < 3; i++) cf[i] = __fmul_rn(__fadd_rn(x[i], lc->shift[l * 4 + i]), lc->scale[l * 4 + i]);
+    elevate3(cf, e);
+    locate3(e, s);
+    const float w = lc->window[l];      // read before the gathers: with this order ptxas spills the least in k_sdf_fused_backward
+    const float2* tab = lattice + (size_t)l * T;
+#pragma unroll
+    for (int r = 0; r < 4; r++) v[r] = __ldg(tab + vindex3(s, r, cap_mask, (unsigned)T));
+    float a0 = 0.f, a1 = 0.f;
+#pragma unroll
+    for (int r = 0; r < 4; r++) { const float wr = s.bary[r] * w; a0 = fmaf(v[r].x, wr, a0); a1 = fmaf(v[r].y, wr, a1); }
+    return make_float2(a0, a1);
+}
+// d feat / d x_j (j = 0..2) of one level's two features: ft[j] = w scale_j / 4 * sum_i E[i][j] G_i, with G_i = u_{rank_i},
+// u_k = d feat / d D_k (by_rank) and E the elevation matrix rows {1,1,1},{-1,1,1},{0,-2,1},{0,0,-3}
+__device__ __forceinline__ void spatial_tangents(const Simplex3& s, const float2* v, float w, const float* scale3, float2* ft) {
+    float2 u[4], G[4];
+    u[0] = make_float2(v[3].x - v[0].x, v[3].y - v[0].y);
+    u[1] = make_float2(v[2].x - v[3].x, v[2].y - v[3].y);
+    u[2] = make_float2(v[1].x - v[2].x, v[1].y - v[2].y);
+    u[3] = make_float2(v[0].x - v[1].x, v[0].y - v[1].y);
+#pragma unroll
+    for (int i = 0; i < 4; i++) {
+        const int rk = s.rank[i];
+        G[i].x = rk == 0 ? u[0].x : (rk == 1 ? u[1].x : (rk == 2 ? u[2].x : u[3].x));
+        G[i].y = rk == 0 ? u[0].y : (rk == 1 ? u[1].y : (rk == 2 ? u[2].y : u[3].y));
+    }
+    const float c0 = 0.25f * w * scale3[0], c1 = 0.25f * w * scale3[1], c2 = 0.25f * w * scale3[2];
+    const float s01x = G[0].x + G[1].x, s01y = G[0].y + G[1].y;
+    ft[0] = make_float2(c0 * (G[0].x - G[1].x), c0 * (G[0].y - G[1].y));
+    ft[1] = make_float2(c1 * fmaf(-2.0f, G[2].x, s01x), c1 * fmaf(-2.0f, G[2].y, s01y));
+    ft[2] = make_float2(c2 * fmaf(-3.0f, G[3].x, s01x + G[2].x), c2 * fmaf(-3.0f, G[3].y, s01y + G[2].y));
+}
+// Operand core kc past the 2L lattice features: column 2L + d = x_d * points_scaling for d < 3 (and below in_dim), zero padding up to
+// Kp[0]. With NT tangents, column 2L + d of tangent j is dx[j][d] * points_scaling.
+template <int NT>
+__device__ __forceinline__ void concat_core(const FusedParams& P, int kc, const float* x, const float (*dx)[3], float* fv, float (*ft)[8]) {
+    const int c0 = 2 * P.L;
+#pragma unroll
+    for (int i = 0; i < 8; i++) {
+        const int c = kc * 8 + i - c0;
+        fv[i] = 0.f;
+#pragma unroll
+        for (int j = 0; j < NT; j++) ft[j][i] = 0.f;
+#pragma unroll
+        for (int d = 0; d < 3; d++) {
+            if (c == d && (c0 + c) < P.in_dim) {
+                fv[i] = x[d] * P.points_scaling;
+#pragma unroll
+                for (int j = 0; j < NT; j++) ft[j][i] = dx[j][d] * P.points_scaling;
+            }
+        }
+    }
+}
 
 // store 8 consecutive K values of one row into a hi/lo operand tile pair (one 16-byte core-matrix row each)
 __device__ __forceinline__ void store8(uint8_t* a_hi, uint8_t* a_lo, int row, int kcore, const float* v) {
@@ -216,20 +282,22 @@ __device__ __forceinline__ void store_pair(uint8_t* t_hi, uint8_t* t_lo, int row
 // warpgroup, lane t)
 __device__ __forceinline__ int frag_row(int mh, int h) { return 64 * mh + 16 * ((threadIdx.x >> 5) & 3) + (threadIdx.x & 31) / 4 + 8 * h; }
 __device__ __forceinline__ int frag_col(int j) { return 8 * j + 2 * (threadIdx.x & 3); }
-// columns [n0, n0 + N) of rows 64 mh .. 64 mh + 63 of D_s = A_s W^T for the value (s = 0) and tangent (s = 1) stream into the issuing
-// warpgroup's registers: the value and the tangent of one (row, column) land in the same thread. Stream s's A tiles are
-// set + 2 s kATileBytes (hi, lo); the weight tile is [Np rows][Kp] K-major.
-template <int N>
-__device__ __forceinline__ void rows_product2(float (*acc)[16], int mh, const uint8_t* set, const uint8_t* w_hi, const uint8_t* w_lo, int Kp,
-                                              int n0) {
-    const uint32_t sbo_w = (Kp / 8) * kLBO, wo = (uint32_t)(n0 / 8) * sbo_w, ao = (uint32_t)(mh * 8 * kSBO_A);
+// Columns [n0, n0 + N) of D_s = A_s W^T, s = 0 .. S-1, for the 64 rows starting `row_off` bytes into the A tiles, into the issuing
+// warpgroup's registers (umma::wg_mma_regs fragments): stream s lands in acc + 16 s, so the values of all streams at one (row, column)
+// are in the same thread. Stream s's A tiles are a + s * stream_bytes (hi) and + lo_bytes (lo); the weight tile is [Np rows][Kp] K-major.
+template <int N, int S>
+__device__ __forceinline__ void streams_product(float* acc, const uint8_t* a, int stream_bytes, int lo_bytes, uint32_t row_off,
+                                                const uint8_t* w_hi, const uint8_t* w_lo, int Kp, int n0) {
+    static_assert(S == 1 || N <= 32, "a stream's fragment holds 16 floats");
+    const uint32_t sbo_w = (Kp / 8) * kLBO, wo = (uint32_t)(n0 / 8) * sbo_w;
     const uint64_t dwh = umma::make_desc(umma::smem_u32(w_hi) + wo, kLBO, sbo_w), dwl = umma::make_desc(umma::smem_u32(w_lo) + wo, kLBO, sbo_w);
     umma::wgmma_fence();
 #pragma unroll
-    for (int s = 0; s < 2; s++) {
-        const uint8_t* a = set + s * 2 * kATileBytes;
-        const uint64_t dah = umma::make_desc(umma::smem_u32(a) + ao, kLBO, kSBO_A), dal = umma::make_desc(umma::smem_u32(a + kATileBytes) + ao, kLBO, kSBO_A);
-        umma::wg_mma_regs<N, 0, 0>(acc[s], dah, dal, dwh, dwl, (2 * kLBO) >> 4, (2 * kLBO) >> 4, Kp / 16, false);
+    for (int s = 0; s < S; s++) {
+        const uint8_t* as = a + s * stream_bytes;
+        const uint64_t dah = umma::make_desc(umma::smem_u32(as) + row_off, kLBO, kSBO_A);
+        const uint64_t dal = umma::make_desc(umma::smem_u32(as + lo_bytes) + row_off, kLBO, kSBO_A);
+        umma::wg_mma_regs<N, 0, 0>(acc + 16 * s, dah, dal, dwh, dwl, (2 * kLBO) >> 4, (2 * kLBO) >> 4, Kp / 16, false);
     }
     umma::wgmma_commit();
     umma::wgmma_wait0();
@@ -298,8 +366,10 @@ __device__ __forceinline__ void scatter2(float* gtab, unsigned long long* ftab, 
 // Encoder backward of one sample at one level, called by a whole warp (one sample per lane):
 //     lattice[idx_r] += w (B_r abar + dB_r tabar),  r = 0..3,   abar = (a0, a1), tabar = (t0, t1) of the level's two features
 // x, v: position and tangent direction; scale3 / shift3: the level's scale and shift; gtab / ftab: the level's float / fixed-point
-// gradient table (scatter2). Invalid lanes add nothing. aggregate: warp-uniform, sum the lanes that share a vertex first (match_any +
-// add_peers2, one reduction per distinct vertex); do_red = false issues no reduction (diagnostics, PSDF_EXPERIMENT_KNOCKOUT).
+// gradient table (scatter2). TAN = false: no tangent term (v, t0, t1 unused), lattice[idx_r] += w B_r abar. Invalid lanes add nothing.
+// aggregate: warp-uniform, sum the lanes that share a vertex first (match_any + add_peers2, one reduction per distinct vertex);
+// do_red = false issues no reduction (diagnostics, PSDF_EXPERIMENT_KNOCKOUT).
+template <bool TAN>
 __device__ __forceinline__ void scatter_level(const float* x, const float* v, const float* scale3, const float* shift3, float w, float a0,
                                               float a1, float t0, float t1, bool valid, bool aggregate, bool do_red, int lane,
                                               unsigned cap_mask, unsigned T, float* gtab, unsigned long long* ftab) {
@@ -307,18 +377,24 @@ __device__ __forceinline__ void scatter_level(const float* x, const float* v, co
 #pragma unroll
     for (int i = 0; i < 3; i++) {
         cf[i] = __fmul_rn(__fadd_rn(x[i], shift3[i]), scale3[i]);
-        dcf[i] = v[i] * scale3[i];
+        if constexpr (TAN) dcf[i] = v[i] * scale3[i];
     }
     elevate3(cf, e);
     Simplex3 s;
     locate3(e, s);
     float db[5];
-    bary_tangent3(dcf, s, db);
+    if constexpr (TAN) bary_tangent3(dcf, s, db);
 #pragma unroll
     for (int r = 0; r < 4; r++) {
         unsigned idx = vindex3(s, r, cap_mask, T);
-        float cb = s.bary[r] * w, cd = db[r] * w;
-        float2 cv = make_float2(cb * a0 + cd * t0, cb * a1 + cd * t1);
+        float cb = s.bary[r] * w;
+        float2 cv;
+        if constexpr (TAN) {
+            float cd = db[r] * w;
+            cv = make_float2(cb * a0 + cd * t0, cb * a1 + cd * t1);
+        } else {
+            cv = make_float2(cb * a0, cb * a1);
+        }
         if (aggregate) {
             unsigned key = valid ? idx : 0xffffffffu;
             unsigned peers = __match_any_sync(kFull, key);

@@ -16,7 +16,8 @@
 //      CTA flushes the four sums once, after its last tile -- 37 k reductions per CTA instead of per tile, with the same totals as a
 //      per-tile fixed-point flush;
 //      bias gradients = column sums (shuffles + shared atomics);
-//   4. abar_0 -> lattice scatter (warp-aggregated red.global.add.v2.f32), normal -> sdf-gradient, geom gradient.
+//   4. abar_0 -> lattice scatter (scatter_level without the tangent term: warp-aggregated red.global.add.v2.f32), normal -> sdf-gradient,
+//      geom gradient.
 // Deterministic mode (common.cuh): every gradient is summed in fixed point instead and added to the float gradients by the flush that
 // follows the launch.
 // Weights stream per layer through one 64 KB buffer by TMA; the next block is requested as soon as the MMAs that read the
@@ -289,31 +290,10 @@ k_rgb_fused_backward(RgbParams P, const float* __restrict__ pos, const float* __
             float x[3] = {0.f, 0.f, 0.f};
             if (valid) { x[0] = pos[(size_t)n * 3]; x[1] = pos[(size_t)n * 3 + 1]; x[2] = pos[(size_t)n * 3 + 2]; }
             for (int l = grp; l < P.L; l += kRgbGroups) {
-                float cf[3], e[4];
-#pragma unroll
-                for (int i = 0; i < 3; i++) cf[i] = __fmul_rn(__fadd_rn(x[i], lc->shift[l * 4 + i]), lc->scale[l * 4 + i]);
-                elevate3(cf, e);
-                Simplex3 s;
-                locate3(e, s);
-                const float w = lc->window[l];
-                const float a0 = xr[2 * l], a1 = xr[2 * l + 1];
-                float* gtab = grad_lattice + (size_t)l * P.T * 2;
-                unsigned long long* ftab = det ? sp.fx_lattice + (size_t)l * P.T * 2 : nullptr;
                 const bool aggregate = lc->scale[l * 4] < kAggregateBelowScale;       // warp-uniform (l is)
-#pragma unroll
-                for (int r = 0; r < 4; r++) {
-                    const unsigned idx = vindex3(s, r, P.cap_mask, (unsigned)P.T);
-                    const float cb = s.bary[r] * w;
-                    float2 cv = make_float2(cb * a0, cb * a1);
-                    if (aggregate) {
-                        const unsigned key = valid ? idx : 0xffffffffu;
-                        const unsigned peers = __match_any_sync(kFull, key);
-                        cv = add_peers2(peers, cv, lane);
-                        if (valid && lane == __ffs(peers) - 1) scatter2(gtab, ftab, idx, cv);
-                    } else if (valid) {
-                        scatter2(gtab, ftab, idx, cv);
-                    }
-                }
+                scatter_level<false>(x, nullptr, lc->scale + l * 4, lc->shift + l * 4, lc->window[l], xr[2 * l], xr[2 * l + 1], 0.f, 0.f, valid,
+                                     aggregate, true, lane, P.cap_mask, (unsigned)P.T, grad_lattice + (size_t)l * P.T * 2,
+                                     det ? sp.fx_lattice + (size_t)l * P.T * 2 : nullptr);
             }
             if (valid) {
                 const int tail = P.enc_cols;          // SH at [tail, tail+25), normal at tail+25.., geom at tail+28..

@@ -44,15 +44,6 @@ inline int make_rgb_params(RgbParams& P, int N, int L, int T, int geom_dim, floa
     return 0;
 }
 
-__device__ __forceinline__ void load_level_consts(LevelC* lc, int L, const float* scale, const float* shift, const float* window, int tid,
-                                                  int nthreads) {
-    for (int i = tid; i < L * 3; i += nthreads) {
-        lc->scale[(i / 3) * 4 + (i % 3)] = scale[i];
-        lc->shift[(i / 3) * 4 + (i % 3)] = shift ? shift[i] : 0.0f;
-    }
-    for (int i = tid; i < L; i += nthreads) lc->window[i] = window ? window[i] : 1.0f;
-}
-
 // hi + lo block of one layer (adjacent in the blob) -> the weight buffer, one TMA bulk copy (single thread)
 __device__ __forceinline__ void load_layer_weights(uint8_t* s_w, const uint8_t* blob, const MlpGeom& g, int l, bool transposed, uint64_t* bar) {
     const uint32_t bytes = (uint32_t)(g.Np[l] * g.Kp[l] * 4);
@@ -99,22 +90,10 @@ __device__ __forceinline__ void build_input_tile(const RgbParams& P, const Level
         float fv[8];
 #pragma unroll
         for (int q = 0; q < 4; q++) {
-            const int l = kc * 4 + q;
-            float cf[3], e[4];
-#pragma unroll
-            for (int i = 0; i < 3; i++) cf[i] = __fmul_rn(__fadd_rn(x[i], lc->shift[l * 4 + i]), lc->scale[l * 4 + i]);
-            elevate3(cf, e);
             Simplex3 s;
-            locate3(e, s);
-            const float2* tab = lattice + (size_t)l * P.T;
             float2 v[4];
-#pragma unroll
-            for (int r = 0; r < 4; r++) v[r] = __ldg(tab + vindex3(s, r, P.cap_mask, (unsigned)P.T));
-            const float w = lc->window[l];
-            float a0 = 0.f, a1 = 0.f;
-#pragma unroll
-            for (int r = 0; r < 4; r++) { const float wr = s.bary[r] * w; a0 = fmaf(v[r].x, wr, a0); a1 = fmaf(v[r].y, wr, a1); }
-            fv[2 * q] = a0; fv[2 * q + 1] = a1;
+            const float2 a = level_features(x, lc, kc * 4 + q, lattice, P.T, P.cap_mask, s, v);
+            fv[2 * q] = a.x; fv[2 * q + 1] = a.y;
         }
         store8w(a_hi, a_lo, row, kc, fv);
     }

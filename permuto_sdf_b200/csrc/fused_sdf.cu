@@ -23,7 +23,6 @@
 // value_rows and k_sdf_fused_dual).
 // Weights (hi+lo, pre-packed in the core-matrix operand layout by k_pack_mlp) are fetched once per CTA with one
 // cp.async.bulk (TMA) and stay resident; CTAs are persistent over tiles (one CTA per SM).
-#include <cstdlib>
 #include "fused_common.cuh"
 #include "../../include/psdf_b200.h"
 
@@ -46,6 +45,8 @@ struct FwdSegs {
     float* geom[2];
 };
 template <bool TAN> struct FwdCfg { static constexpr int kThreads = TAN ? kFusedThreads : kValueThreads; static constexpr int kCtasPerSm = TAN ? 1 : 2; };
+// directions of the three spatial tangents d / d x_j (concat_core)
+__device__ constexpr float kUnit3[3][3] = {{1.f, 0.f, 0.f}, {0.f, 1.f, 0.f}, {0.f, 0.f, 1.f}};
 // accumulator areas (umma.cuh) of the kernels of this file
 __device__ float g_acc_tan[(size_t)kAccCtas * kTile * 256];
 
@@ -53,26 +54,17 @@ __device__ float g_acc_tan[(size_t)kAccCtas * kTile * 256];
 // Layer l of a value-only 128-row tile (inference forward, sphere tracer): warpgroup mh forms rows 64 mh .. 64 mh + 63 of D = A W^T in
 // its registers (umma::wg_mma_regs fragments) and consumes them itself -- bias + GELU into the next layer's operand cores, or the
 // output values. No other warp reads or writes those rows of the operand tiles in between, so no CTA barrier separates the two.
-template <int N>
-__device__ __forceinline__ void rows_product(float* acc, int mh, const uint8_t* s_a, const uint8_t* w_hi, const uint8_t* w_lo, int Kp) {
-    const uint32_t sbo_w = (Kp / 8) * kLBO, ao = (uint32_t)(mh * 8 * kSBO_A);
-    const uint64_t dah = umma::make_desc(umma::smem_u32(s_a) + ao, kLBO, kSBO_A), dal = umma::make_desc(umma::smem_u32(s_a + kATileBytes) + ao, kLBO, kSBO_A);
-    const uint64_t dwh = umma::make_desc(umma::smem_u32(w_hi), kLBO, sbo_w), dwl = umma::make_desc(umma::smem_u32(w_lo), kLBO, sbo_w);
-    umma::wgmma_fence();
-    umma::wg_mma_regs<N, 0, 0>(acc, dah, dal, dwh, dwl, (2 * kLBO) >> 4, (2 * kLBO) >> 4, Kp / 16, false);
-    umma::wgmma_commit();
-    umma::wgmma_wait0();
-}
 // the fragment (32 floats, the first Np / 2 used) of rows 64 mh .. 64 mh + 63 of layer l
 __device__ __forceinline__ void value_rows(float* acc, const MlpGeom& g, int l, int mh, const uint8_t* s_a, const uint8_t* s_blob) {
 #pragma unroll
     for (int i = 0; i < 32; i++) acc[i] = 0.f;
     const uint8_t *wh = s_blob + g.w_hi[l], *wl = s_blob + g.w_lo[l];
+    const uint32_t ro = (uint32_t)(mh * 8 * kSBO_A);
     switch (g.Np[l] / 16) {
-        case 1: rows_product<16>(acc, mh, s_a, wh, wl, g.Kp[l]); break;
-        case 2: rows_product<32>(acc, mh, s_a, wh, wl, g.Kp[l]); break;
-        case 3: rows_product<48>(acc, mh, s_a, wh, wl, g.Kp[l]); break;
-        default: rows_product<64>(acc, mh, s_a, wh, wl, g.Kp[l]); break;
+        case 1: streams_product<16, 1>(acc, s_a, 0, kATileBytes, ro, wh, wl, g.Kp[l], 0); break;
+        case 2: streams_product<32, 1>(acc, s_a, 0, kATileBytes, ro, wh, wl, g.Kp[l], 0); break;
+        case 3: streams_product<48, 1>(acc, s_a, 0, kATileBytes, ro, wh, wl, g.Kp[l], 0); break;
+        default: streams_product<64, 1>(acc, s_a, 0, kATileBytes, ro, wh, wl, g.Kp[l], 0); break;
     }
 }
 // bias + GELU of a hidden layer's fragment -> the next layer's operand cores
@@ -109,11 +101,7 @@ k_sdf_fused(FusedParams P, FwdSegs G, const float2* __restrict__ lattice, const 
         umma::mbar_fence_init();
         if (TAN) umma::acc_attach(g_acc_tan + (size_t)blockIdx.x * kTile * (S * 64), S * 64);
     }
-    for (int i = tid; i < P.L * 3; i += kThreads) {
-        lc->scale[(i / 3) * 4 + (i % 3)] = scale[i];
-        lc->shift[(i / 3) * 4 + (i % 3)] = shift ? shift[i] : 0.0f;
-    }
-    for (int i = tid; i < P.L; i += kThreads) lc->window[i] = window ? window[i] : 1.0f;
+    load_level_consts(lc, P.L, scale, shift, window, tid, kThreads);
     __syncthreads();
     if (tid == 0) {
         umma::mbar_expect_tx(&bars[0], (uint32_t)P.g.total);
@@ -138,66 +126,25 @@ k_sdf_fused(FusedParams P, FwdSegs G, const float2* __restrict__ lattice, const 
         for (int i = 0; i < 3; i++) x[i] = valid ? pos[(size_t)n * 3 + i] : 0.0f;
 
         // ---------------- encoder: operand cores grp, grp+4, ... of this row
-        for (int kc = grp; kc < ((P.knockout & 1) ? 0 : all_cores); kc += kGroups) {
+        for (int kc = grp; kc < all_cores; kc += kGroups) {
             float fv[8], ft[3][8];
             if (kc < level_cores) {
 #pragma unroll
                 for (int q = 0; q < 4; q++) {
                     const int l = kc * 4 + q;
-                    float cf[3], e[4];
-#pragma unroll
-                    for (int i = 0; i < 3; i++) cf[i] = __fmul_rn(__fadd_rn(x[i], lc->shift[l * 4 + i]), lc->scale[l * 4 + i]);
-                    elevate3(cf, e);
                     Simplex3 s;
-                    locate3(e, s);
-                    const float2* tab = lattice + (size_t)l * P.T;
                     float2 v[4];
-#pragma unroll
-                    for (int r = 0; r < 4; r++) {
-                        const unsigned vi = vindex3(s, r, P.cap_mask, (unsigned)P.T);
-                        v[r] = (l < P.free_levels) ? make_float2(1e-6f * (float)(vi & 7u), 0.f) : __ldg(tab + vi);
-                    }
-                    const float w = lc->window[l];
-                    float a0 = 0.f, a1 = 0.f;
-#pragma unroll
-                    for (int r = 0; r < 4; r++) { float wr = s.bary[r] * w; a0 = fmaf(v[r].x, wr, a0); a1 = fmaf(v[r].y, wr, a1); }
-                    fv[2 * q] = a0; fv[2 * q + 1] = a1;
+                    const float2 a = level_features(x, lc, l, lattice, P.T, P.cap_mask, s, v);
+                    fv[2 * q] = a.x; fv[2 * q + 1] = a.y;
                     if (TAN) {
-                        // d feat / d x_j = w scale_j / 4 * sum_i E[i][j] G_i, with G_i = u_{rank_i}, u_k = d feat / d D_k
-                        // (fused_common.cuh by_rank) and E the elevation matrix rows {1,1,1},{-1,1,1},{0,-2,1},{0,0,-3}
-                        float2 u[4], G[4];
-                        u[0] = make_float2(v[3].x - v[0].x, v[3].y - v[0].y);
-                        u[1] = make_float2(v[2].x - v[3].x, v[2].y - v[3].y);
-                        u[2] = make_float2(v[1].x - v[2].x, v[1].y - v[2].y);
-                        u[3] = make_float2(v[0].x - v[1].x, v[0].y - v[1].y);
+                        float2 t[3];
+                        spatial_tangents(s, v, lc->window[l], lc->scale + l * 4, t);
 #pragma unroll
-                        for (int i = 0; i < 4; i++) {
-                            const int rk = s.rank[i];
-                            G[i].x = rk == 0 ? u[0].x : (rk == 1 ? u[1].x : (rk == 2 ? u[2].x : u[3].x));
-                            G[i].y = rk == 0 ? u[0].y : (rk == 1 ? u[1].y : (rk == 2 ? u[2].y : u[3].y));
-                        }
-                        const float c0 = 0.25f * w * lc->scale[l * 4], c1 = 0.25f * w * lc->scale[l * 4 + 1], c2 = 0.25f * w * lc->scale[l * 4 + 2];
-                        const float s01x = G[0].x + G[1].x, s01y = G[0].y + G[1].y;
-                        ft[0][2 * q] = c0 * (G[0].x - G[1].x); ft[0][2 * q + 1] = c0 * (G[0].y - G[1].y);
-                        ft[1][2 * q] = c1 * fmaf(-2.0f, G[2].x, s01x); ft[1][2 * q + 1] = c1 * fmaf(-2.0f, G[2].y, s01y);
-                        ft[2][2 * q] = c2 * fmaf(-3.0f, G[3].x, s01x + G[2].x); ft[2][2 * q + 1] = c2 * fmaf(-3.0f, G[3].y, s01y + G[2].y);
+                        for (int j = 0; j < 3; j++) { ft[j][2 * q] = t[j].x; ft[j][2 * q + 1] = t[j].y; }
                     }
                 }
             } else {
-                // concat-points columns (x * scaling) and zero padding up to Kp[0]
-                const int c0 = 2 * P.L;
-#pragma unroll
-                for (int i = 0; i < 8; i++) {
-                    int c = kc * 8 + i - c0;
-                    float val = 0.f;
-#pragma unroll
-                    for (int d = 0; d < 3; d++) if (c == d && (c0 + c) < P.in_dim) val = x[d] * P.points_scaling;
-                    fv[i] = val;
-                    if (TAN) {
-#pragma unroll
-                        for (int j = 0; j < 3; j++) ft[j][i] = (c == j && (c0 + c) < P.in_dim) ? P.points_scaling : 0.f;
-                    }
-                }
+                concat_core<TAN ? 3 : 0>(P, kc, x, kUnit3, fv, ft);
             }
             store8(s_a, s_a + kATileBytes, row, kc, fv);
             if (TAN) {
@@ -209,7 +156,7 @@ k_sdf_fused(FusedParams P, FwdSegs G, const float2* __restrict__ lattice, const 
         // ---------------- MLP: 4 dense layers on the tensor cores
 #pragma unroll 1
         for (int l = 0; l < kNL; l++) {
-            if (!(P.knockout & 128)) umma::fence_async_smem();
+            umma::fence_async_smem();
             __syncthreads();
             if constexpr (!TAN) {
                 // value only: warpgroup mh owns rows 64 mh .. 64 mh + 63 from the product to the outputs (see value_rows)
@@ -239,49 +186,33 @@ k_sdf_fused(FusedParams P, FwdSegs G, const float2* __restrict__ lattice, const 
                 continue;
             }
             // value + tangents: warpgroup s issues stream s (both row halves)
-            if (!(P.knockout & 2)) {
-                const int wgi = warp >> 2;
-                for (int mh = 0; mh < 2; mh++)
-                    issue_gemm(tmem_base + wgi * 64, mh, s_a + wgi * 2 * kATileBytes, s_a + wgi * 2 * kATileBytes + kATileBytes,
-                               s_blob + P.g.w_hi[l], s_blob + P.g.w_lo[l], P.g.Kp[l], P.g.Np[l]);
-            }
+            const int wgi = warp >> 2;
+            for (int mh = 0; mh < 2; mh++)
+                issue_gemm(tmem_base + wgi * 64, mh, s_a + wgi * 2 * kATileBytes, s_a + wgi * 2 * kATileBytes + kATileBytes,
+                           s_blob + P.g.w_hi[l], s_blob + P.g.w_lo[l], P.g.Kp[l], P.g.Np[l]);
             __syncthreads();
             const float* bias = reinterpret_cast<const float*>(s_blob + P.g.bias[l]);
             const uint32_t trow = tmem_base + ((uint32_t)((warp & 3) * 32) << 16);
             const bool last = (l == kNL - 1);
             for (int c = grp; c < P.g.Np[l] / 16; c += kGroups) {     // this thread's 16-column chunks
                 float z[16], tz[3][16];
-                if (P.knockout & 16) {                 // diagnostics: no accumulator reads
+                umma::tmem_ld16(trow + c * 16, z);
+                if (TAN) {
 #pragma unroll
-                    for (int i = 0; i < 16; i++) { z[i] = 0.f; tz[0][i] = 0.f; tz[1][i] = 0.f; tz[2][i] = 0.f; }
-                } else {
-                    umma::tmem_ld16(trow + c * 16, z);
-                    if (TAN) {
-#pragma unroll
-                        for (int j = 0; j < 3; j++) umma::tmem_ld16(trow + (1 + j) * 64 + c * 16, tz[j]);
-                    }
+                    for (int j = 0; j < 3; j++) umma::tmem_ld16(trow + (1 + j) * 64 + c * 16, tz[j]);
                 }
 #pragma unroll
                 for (int i = 0; i < 16; i++) z[i] += bias[c * 16 + i];
                 if (!last) {
-                    if (!(P.knockout & 4)) {
 #pragma unroll
-                        for (int i = 0; i < 16; i++) {
-                            const GeluEval ge = gelu_eval(z[i]);
-                            if (TAN) {
-                                const float g1 = fmaf(z[i], ge.pdf, ge.cdf);
+                    for (int i = 0; i < 16; i++) {
+                        const GeluEval ge = gelu_eval(z[i]);
+                        if (TAN) {
+                            const float g1 = fmaf(z[i], ge.pdf, ge.cdf);
 #pragma unroll
-                                for (int j = 0; j < 3; j++) tz[j][i] *= g1;
-                            }
-                            z[i] *= ge.cdf;
+                            for (int j = 0; j < 3; j++) tz[j][i] *= g1;
                         }
-                    }
-                    if (P.knockout & 8) {             // keep the values alive without the split / store work
-                        float acc = 0.f;
-#pragma unroll
-                        for (int i = 0; i < 16; i++) { acc += z[i]; if (TAN) acc += tz[0][i] + tz[1][i] + tz[2][i]; }
-                        if (acc == 123.456f) s_a[0] = 1;
-                        continue;
+                        z[i] *= ge.cdf;
                     }
                     store8(s_a, s_a + kATileBytes, row, 2 * c, z);
                     store8(s_a, s_a + kATileBytes, row, 2 * c + 1, z + 8);
@@ -293,7 +224,7 @@ k_sdf_fused(FusedParams P, FwdSegs G, const float2* __restrict__ lattice, const 
                             store8(hi, hi + kATileBytes, row, 2 * c + 1, tz[j] + 8);
                         }
                     }
-                } else if (valid && !(P.knockout & 32)) {
+                } else if (valid) {
                     const int nout = P.g.N[l];
                     if (c == 0) {
                         sdf_out[n] = z[0];
@@ -327,23 +258,6 @@ constexpr int kSubTileBytes = kSub * 64 * 2;    // one bf16 operand tile [64 x 6
 constexpr int kGroupThreads = 256;
 constexpr int kStg = 69;                         // row stride (floats) of the output staging tile: 64 value columns max + 3 gradient columns
 
-// columns [n0, n0 + N) of the four streams' D[64 x Np] = A[64 x Kp] W^T into registers (one warpgroup; fragment layout of
-// umma::wg_mma_regs). Stream s's A tiles are s_a + s * 2 * kSubTileBytes (hi, lo).
-template <int N>
-__device__ __forceinline__ void issue_streams_regs(float (*acc)[16], const uint8_t* s_a, const uint8_t* w_hi, const uint8_t* w_lo, int Kp, int n0) {
-    const uint32_t sbo_w = (Kp / 8) * kLBO, wo = (uint32_t)(n0 / 8) * sbo_w;
-    const uint64_t dwh = umma::make_desc(umma::smem_u32(w_hi) + wo, kLBO, sbo_w), dwl = umma::make_desc(umma::smem_u32(w_lo) + wo, kLBO, sbo_w);
-    umma::wgmma_fence();
-#pragma unroll
-    for (int s = 0; s < 4; s++) {
-        const uint8_t* a = s_a + s * 2 * kSubTileBytes;
-        const uint64_t dah = umma::make_desc(umma::smem_u32(a), kLBO, kSBO_A), dal = umma::make_desc(umma::smem_u32(a + kSubTileBytes), kLBO, kSBO_A);
-        umma::wg_mma_regs<N, 0, 0>(acc[s], dah, dal, dwh, dwl, (2 * kLBO) >> 4, (2 * kLBO) >> 4, Kp / 16, false);
-    }
-    umma::wgmma_commit();
-    umma::wgmma_wait0();
-}
-
 __global__ void __launch_bounds__(2 * kGroupThreads, 1)
 k_sdf_fused_dual(FusedParams P, FwdSegs G, const float2* __restrict__ lattice, const float* __restrict__ scale,
                  const float* __restrict__ shift, const float* __restrict__ window, const uint8_t* __restrict__ blob) {
@@ -364,11 +278,7 @@ k_sdf_fused_dual(FusedParams P, FwdSegs G, const float2* __restrict__ lattice, c
         umma::mbar_init(&bars[3], 1);
         umma::mbar_fence_init();
     }
-    for (int i = tid; i < P.L * 3; i += 2 * kGroupThreads) {
-        lc->scale[(i / 3) * 4 + (i % 3)] = scale[i];
-        lc->shift[(i / 3) * 4 + (i % 3)] = shift ? shift[i] : 0.0f;
-    }
-    for (int i = tid; i < P.L; i += 2 * kGroupThreads) lc->window[i] = window ? window[i] : 1.0f;
+    load_level_consts(lc, P.L, scale, shift, window, tid, 2 * kGroupThreads);
     __syncthreads();
     if (tid == 0) {
         umma::mbar_expect_tx(&bars[0], (uint32_t)P.g.total);
@@ -385,8 +295,8 @@ k_sdf_fused_dual(FusedParams P, FwdSegs G, const float2* __restrict__ lattice, c
     // Two identical groups that start together stay in lock step (every unit is shared fairly), waiting for the tensor core at the same
     // time. Group 1 therefore starts half a sub-tile late: it waits until group 0 has finished the second layer of its first sub-tile;
     // from then on one group's MMA / accumulator-read phases meet the other's encoder / GELU / store phases.
-    bool skew_pending = P.skew != 0;
-    if (skew_pending && grp2 == 1 && blockIdx.x * 2 < nsub) { umma::mbar_wait(&bars[3], 0); skew_pending = false; }
+    bool skew_pending = true;
+    if (grp2 == 1 && blockIdx.x * 2 < nsub) { umma::mbar_wait(&bars[3], 0); skew_pending = false; }
     for (int sub = blockIdx.x * 2 + grp2; sub < nsub; sub += 2 * gridDim.x) {
         const bool seg1 = sub >= G.tile0[1];
         const int sub0 = seg1 ? G.tile0[1] : 0, nseg = seg1 ? G.n[1] : G.n[0];
@@ -400,57 +310,23 @@ k_sdf_fused_dual(FusedParams P, FwdSegs G, const float2* __restrict__ lattice, c
 #pragma unroll
         for (int i = 0; i < 3; i++) x[i] = valid ? pos[(size_t)n * 3 + i] : 0.0f;
 
-        // ---------------- encoder (same arithmetic as k_sdf_fused<true>): operand cores eg, eg + 4, ... of this row
+        // ---------------- encoder: operand cores eg, eg + 4, ... of this row
         for (int kc = eg; kc < all_cores; kc += kEnc) {
             float fv[8], ft[3][8];
             if (kc < level_cores) {
 #pragma unroll
                 for (int qq = 0; qq < 4; qq++) {
                     const int l = kc * 4 + qq;
-                    float cf[3], e[4];
-#pragma unroll
-                    for (int i = 0; i < 3; i++) cf[i] = __fmul_rn(__fadd_rn(x[i], lc->shift[l * 4 + i]), lc->scale[l * 4 + i]);
-                    elevate3(cf, e);
                     Simplex3 s;
-                    locate3(e, s);
-                    const float2* tab = lattice + (size_t)l * P.T;
-                    float2 v[4];
+                    float2 v[4], t[3];
+                    const float2 a = level_features(x, lc, l, lattice, P.T, P.cap_mask, s, v);
+                    spatial_tangents(s, v, lc->window[l], lc->scale + l * 4, t);
+                    fv[2 * qq] = a.x; fv[2 * qq + 1] = a.y;
 #pragma unroll
-                    for (int r = 0; r < 4; r++) v[r] = __ldg(tab + vindex3(s, r, P.cap_mask, (unsigned)P.T));
-                    const float w = lc->window[l];
-                    float a0 = 0.f, a1 = 0.f;
-#pragma unroll
-                    for (int r = 0; r < 4; r++) { float wr = s.bary[r] * w; a0 = fmaf(v[r].x, wr, a0); a1 = fmaf(v[r].y, wr, a1); }
-                    fv[2 * qq] = a0; fv[2 * qq + 1] = a1;
-                    float2 u[4], Gv[4];
-                    u[0] = make_float2(v[3].x - v[0].x, v[3].y - v[0].y);
-                    u[1] = make_float2(v[2].x - v[3].x, v[2].y - v[3].y);
-                    u[2] = make_float2(v[1].x - v[2].x, v[1].y - v[2].y);
-                    u[3] = make_float2(v[0].x - v[1].x, v[0].y - v[1].y);
-#pragma unroll
-                    for (int i = 0; i < 4; i++) {
-                        const int rk = s.rank[i];
-                        Gv[i].x = rk == 0 ? u[0].x : (rk == 1 ? u[1].x : (rk == 2 ? u[2].x : u[3].x));
-                        Gv[i].y = rk == 0 ? u[0].y : (rk == 1 ? u[1].y : (rk == 2 ? u[2].y : u[3].y));
-                    }
-                    const float c0 = 0.25f * w * lc->scale[l * 4], c1 = 0.25f * w * lc->scale[l * 4 + 1], c2 = 0.25f * w * lc->scale[l * 4 + 2];
-                    const float s01x = Gv[0].x + Gv[1].x, s01y = Gv[0].y + Gv[1].y;
-                    ft[0][2 * qq] = c0 * (Gv[0].x - Gv[1].x); ft[0][2 * qq + 1] = c0 * (Gv[0].y - Gv[1].y);
-                    ft[1][2 * qq] = c1 * fmaf(-2.0f, Gv[2].x, s01x); ft[1][2 * qq + 1] = c1 * fmaf(-2.0f, Gv[2].y, s01y);
-                    ft[2][2 * qq] = c2 * fmaf(-3.0f, Gv[3].x, s01x + Gv[2].x); ft[2][2 * qq + 1] = c2 * fmaf(-3.0f, Gv[3].y, s01y + Gv[2].y);
+                    for (int j = 0; j < 3; j++) { ft[j][2 * qq] = t[j].x; ft[j][2 * qq + 1] = t[j].y; }
                 }
             } else {
-                const int c0 = 2 * P.L;
-#pragma unroll
-                for (int i = 0; i < 8; i++) {
-                    int c = kc * 8 + i - c0;
-                    float val = 0.f;
-#pragma unroll
-                    for (int d = 0; d < 3; d++) if (c == d && (c0 + c) < P.in_dim) val = x[d] * P.points_scaling;
-                    fv[i] = val;
-#pragma unroll
-                    for (int j = 0; j < 3; j++) ft[j][i] = (c == j && (c0 + c) < P.in_dim) ? P.points_scaling : 0.f;
-                }
+                concat_core<3>(P, kc, x, kUnit3, fv, ft);
             }
             store8(s_a, s_a + kSubTileBytes, row, kc, fv);
 #pragma unroll
@@ -469,8 +345,8 @@ k_sdf_fused_dual(FusedParams P, FwdSegs G, const float2* __restrict__ lattice, c
 #pragma unroll
                 for (int i = 0; i < 16; i++) acc[s][i] = 0.f;
             const int ncols = min(32, P.g.Np[l] - hc * 32);
-            if (ncols == 32) issue_streams_regs<32>(acc, s_a, s_blob + P.g.w_hi[l], s_blob + P.g.w_lo[l], P.g.Kp[l], hc * 32);
-            else if (ncols == 16) issue_streams_regs<16>(acc, s_a, s_blob + P.g.w_hi[l], s_blob + P.g.w_lo[l], P.g.Kp[l], hc * 32);
+            if (ncols == 32) streams_product<32, S>(acc[0], s_a, 2 * kSubTileBytes, kSubTileBytes, 0, s_blob + P.g.w_hi[l], s_blob + P.g.w_lo[l], P.g.Kp[l], hc * 32);
+            else if (ncols == 16) streams_product<16, S>(acc[0], s_a, 2 * kSubTileBytes, kSubTileBytes, 0, s_blob + P.g.w_hi[l], s_blob + P.g.w_lo[l], P.g.Kp[l], hc * 32);
             umma::bar_sync(1 + grp2, kGroupThreads);     // every product of the group has read this layer's operand tiles
             const float* bias = reinterpret_cast<const float*>(s_blob + P.g.bias[l]);
             const bool last = (l == kNL - 1);
@@ -592,11 +468,7 @@ k_sdf_sphere_trace(FusedParams P, TraceParams Q, const float* __restrict__ pos_i
         umma::mbar_fence_init();
         s_flag[0] = 0;
     }
-    for (int i = tid; i < P.L * 3; i += kValueThreads) {
-        lc->scale[(i / 3) * 4 + (i % 3)] = scale[i];
-        lc->shift[(i / 3) * 4 + (i % 3)] = shift ? shift[i] : 0.0f;
-    }
-    for (int i = tid; i < P.L; i += kValueThreads) lc->window[i] = window ? window[i] : 1.0f;
+    load_level_consts(lc, P.L, scale, shift, window, tid, kValueThreads);
     __syncthreads();
     if (tid == 0) {
         umma::mbar_expect_tx(&bars[0], (uint32_t)P.g.total);
@@ -643,33 +515,13 @@ k_sdf_sphere_trace(FusedParams P, TraceParams Q, const float* __restrict__ pos_i
                 if (kc < level_cores) {
 #pragma unroll
                     for (int q = 0; q < 4; q++) {
-                        const int l = kc * 4 + q;
-                        float cf[3], e[4];
-#pragma unroll
-                        for (int i = 0; i < 3; i++) cf[i] = __fmul_rn(__fadd_rn(x[i], lc->shift[l * 4 + i]), lc->scale[l * 4 + i]);
-                        elevate3(cf, e);
                         Simplex3 s;
-                        locate3(e, s);
-                        const float2* tab = lattice + (size_t)l * P.T;
                         float2 v[4];
-#pragma unroll
-                        for (int r = 0; r < 4; r++) v[r] = __ldg(tab + vindex3(s, r, P.cap_mask, (unsigned)P.T));
-                        const float w = lc->window[l];
-                        float a0 = 0.f, a1 = 0.f;
-#pragma unroll
-                        for (int r = 0; r < 4; r++) { float wr = s.bary[r] * w; a0 = fmaf(v[r].x, wr, a0); a1 = fmaf(v[r].y, wr, a1); }
-                        fv[2 * q] = a0; fv[2 * q + 1] = a1;
+                        const float2 a = level_features(x, lc, kc * 4 + q, lattice, P.T, P.cap_mask, s, v);
+                        fv[2 * q] = a.x; fv[2 * q + 1] = a.y;
                     }
                 } else {
-                    const int c0 = 2 * P.L;
-#pragma unroll
-                    for (int i = 0; i < 8; i++) {
-                        int c = kc * 8 + i - c0;
-                        float val = 0.f;
-#pragma unroll
-                        for (int d = 0; d < 3; d++) if (c == d && (c0 + c) < P.in_dim) val = x[d] * P.points_scaling;
-                        fv[i] = val;
-                    }
+                    concat_core<0>(P, kc, x, nullptr, fv, nullptr);
                 }
                 store8(s_a, s_a + kATileBytes, row, kc, fv);
             }
@@ -840,15 +692,12 @@ int psdf_sdf_mlp_pack_advance(int in_dim, int hidden, int out_dim, const float* 
     return PSDF_OK;
 }
 
-// kernel choice of the value + tangent forward: 1 = two 64-sample groups per CTA (default), 0 = lock-step 128-sample tiles.
-// Initialised from PSDF_SDF_FWD_DUAL, switchable at run time for A/B measurements (psdf_sdf_forward_variant).
-static int& forward_dual_mode() {
-    static int mode = (getenv("PSDF_SDF_FWD_DUAL") && atoi(getenv("PSDF_SDF_FWD_DUAL")) == 0) ? 0 : 1;
-    return mode;
-}
+// kernel choice of the value + tangent forward: 1 = two 64-sample groups per CTA (default), 0 = lock-step 128-sample tiles; switchable at
+// run time for tests and A/B measurements (psdf_sdf_forward_variant)
+static int forward_dual_mode = 1;
 int psdf_sdf_forward_variant(int variant) {
-    if (variant == 0 || variant == 1) forward_dual_mode() = variant;
-    return forward_dual_mode();
+    if (variant == 0 || variant == 1) forward_dual_mode = variant;
+    return forward_dual_mode;
 }
 
 static int launch_forward(int L, int T, const float* lattice, const float* scale_factor, const float* shift, const float* window,
@@ -861,10 +710,6 @@ static int launch_forward(int L, int T, const float* lattice, const float* scale
     P.points_scaling = points_scaling;
     P.in_dim = (L + 2) * 2;                       // D = 3, F = 2: E = 2 concat levels
     if (P.in_dim > 64) return PSDF_ERR_UNSUPPORTED;
-    static const int free_levels = getenv("PSDF_EXPERIMENT_FREE_LEVELS") ? atoi(getenv("PSDF_EXPERIMENT_FREE_LEVELS")) : 0;
-    P.free_levels = free_levels;
-    static const int knockout = getenv("PSDF_EXPERIMENT_KNOCKOUT") ? atoi(getenv("PSDF_EXPERIMENT_KNOCKOUT")) : 0;
-    P.knockout = knockout;
     P.g = make_geom(P.in_dim, hidden, out_dim);
     FwdSegs G;
     int tiles = 0, total = 0;
@@ -886,10 +731,9 @@ static int launch_forward(int L, int T, const float* lattice, const float* scale
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     const float2* lat = reinterpret_cast<const float2*>(lattice);
-    // value + tangents: two independent 64-sample groups per CTA (k_sdf_fused_dual) unless PSDF_SDF_FWD_DUAL=0 (the lock-step kernel)
-    const bool dual = forward_dual_mode() != 0;
-    static const int skew = getenv("PSDF_SDF_FWD_SKEW") ? atoi(getenv("PSDF_SDF_FWD_SKEW")) : 1;
-    P.skew = skew;
+    // value + tangents: two independent 64-sample groups per CTA (k_sdf_fused_dual) unless psdf_sdf_forward_variant(0) chose the lock-step
+    // kernel
+    const bool dual = forward_dual_mode != 0;
     if (tangents && dual) {
         FwdSegs H = G;
         int subs = 0;

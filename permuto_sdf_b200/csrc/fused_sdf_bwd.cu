@@ -174,11 +174,7 @@ k_sdf_fused_backward(FusedParams P, Segments S, const float2* __restrict__ latti
         umma::mbar_fence_init();
         umma::acc_attach(g_acc_bwd + (size_t)blockIdx.x * kTile * 512, 512);
     }
-    for (int i = tid; i < P.L * 3; i += kBwdThreads) {
-        lc->scale[(i / 3) * 4 + (i % 3)] = scale[i];
-        lc->shift[(i / 3) * 4 + (i % 3)] = shift ? shift[i] : 0.0f;
-    }
-    for (int i = tid; i < P.L; i += kBwdThreads) lc->window[i] = window ? window[i] : 1.0f;
+    load_level_consts(lc, P.L, scale, shift, window, tid, kBwdThreads);
     for (int i = tid; i < kNL * 64; i += kBwdThreads) s_gb[i] = 0ull;     // also clears s_gbf
     __syncthreads();
     if (tid == 0) {
@@ -222,49 +218,30 @@ k_sdf_fused_backward(FusedParams P, Segments S, const float2* __restrict__ latti
         }
         // ---------------- 1. encoder -> X: operand cores grp, grp+4, ... (4 levels = 8 features = one 16-byte core row)
         for (int kc = grp; kc < K0 / 8; kc += kGroups) {
-            float fv[8], ft[8];
+            float fv[8], ft[1][8];
             if (kc < level_cores) {
 #pragma unroll
                 for (int q = 0; q < 4; q++) {
                     const int l = kc * 4 + q;
-                    float cf[3], dcf[3], e[4];
+                    // directional tangent along v: the barycentric weights' tangent dB_r applied to the same vertex values
+                    float dcf[3], db[5];
 #pragma unroll
-                    for (int i = 0; i < 3; i++) {
-                        cf[i] = __fmul_rn(__fadd_rn(x[i], lc->shift[l * 4 + i]), lc->scale[l * 4 + i]);
-                        dcf[i] = v[i] * lc->scale[l * 4 + i];
-                    }
-                    elevate3(cf, e);
+                    for (int i = 0; i < 3; i++) dcf[i] = v[i] * lc->scale[l * 4 + i];
                     Simplex3 s;
-                    locate3(e, s);
-                    float db[5];
-                    bary_tangent3(dcf, s, db);
-                    const float2* tab = lattice + (size_t)l * P.T;
                     float2 val[4];
-#pragma unroll
-                    for (int r = 0; r < 4; r++) val[r] = __ldg(tab + vindex3(s, r, P.cap_mask, (unsigned)P.T));
+                    const float2 a = level_features(x, lc, l, lattice, P.T, P.cap_mask, s, val);
+                    bary_tangent3(dcf, s, db);
                     const float w = lc->window[l];
-                    float a0 = 0.f, a1 = 0.f, t0 = 0.f, t1 = 0.f;
+                    float t0 = 0.f, t1 = 0.f;
 #pragma unroll
-                    for (int r = 0; r < 4; r++) {
-                        float wr = s.bary[r] * w, cr = db[r] * w;
-                        a0 = fmaf(val[r].x, wr, a0); a1 = fmaf(val[r].y, wr, a1);
-                        t0 = fmaf(val[r].x, cr, t0); t1 = fmaf(val[r].y, cr, t1);
-                    }
-                    fv[2 * q] = a0; fv[2 * q + 1] = a1; ft[2 * q] = t0; ft[2 * q + 1] = t1;
+                    for (int r = 0; r < 4; r++) { const float cr = db[r] * w; t0 = fmaf(val[r].x, cr, t0); t1 = fmaf(val[r].y, cr, t1); }
+                    fv[2 * q] = a.x; fv[2 * q + 1] = a.y; ft[0][2 * q] = t0; ft[0][2 * q + 1] = t1;
                 }
-            } else {        // concat-points columns + zero padding
-                const int c0 = 2 * P.L;
-#pragma unroll
-                for (int i = 0; i < 8; i++) {
-                    int c = kc * 8 + i - c0;
-                    float a = 0.f, t = 0.f;
-#pragma unroll
-                    for (int d = 0; d < 3; d++) if (c == d && (c0 + c) < P.in_dim) { a = x[d] * P.points_scaling; t = v[d] * P.points_scaling; }
-                    fv[i] = a; ft[i] = t;
-                }
+            } else {
+                concat_core<1>(P, kc, x, &v, fv, ft);
             }
             store8(s_X, s_X + kATileBytes, row, kc, fv);
-            store8(s_X + 2 * kATileBytes, s_X + 3 * kATileBytes, row, kc, ft);
+            store8(s_X + 2 * kATileBytes, s_X + 3 * kATileBytes, row, kc, ft[0]);
         }
 
         PSDF_PHASE(kPhEncoder);
@@ -308,8 +285,9 @@ k_sdf_fused_backward(FusedParams P, Segments S, const float2* __restrict__ latti
             float acc[2][16];
 #pragma unroll
             for (int i = 0; i < 16; i++) { acc[0][i] = 0.f; acc[1][i] = 0.f; }
-            if (nn == 32) rows_product2<32>(acc, mh, at, s_w + P.g.w_hi[l], s_w + P.g.w_lo[l], P.g.Kp[l], n0);
-            else if (nn == 16) rows_product2<16>(acc, mh, at, s_w + P.g.w_hi[l], s_w + P.g.w_lo[l], P.g.Kp[l], n0);
+            const uint32_t ro = (uint32_t)(mh * 8 * kSBO_A);
+            if (nn == 32) streams_product<32, 2>(acc[0], at, 2 * kATileBytes, kATileBytes, ro, s_w + P.g.w_hi[l], s_w + P.g.w_lo[l], P.g.Kp[l], n0);
+            else if (nn == 16) streams_product<16, 2>(acc[0], at, 2 * kATileBytes, kATileBytes, ro, s_w + P.g.w_hi[l], s_w + P.g.w_lo[l], P.g.Kp[l], n0);
             const float* bias = reinterpret_cast<const float*>(s_w + P.g.bias[l]);
 #pragma unroll
             for (int j = 0; j < 4; j++) {
@@ -536,7 +514,7 @@ k_sdf_lattice_scatter(FusedParams P, Segments S, const float4* __restrict__ xch,
     const float4 a = xch[(size_t)l * xch_stride + slot];
     const bool aggregate = sc[0] < kAggregateBelowScale && !(P.knockout & 2);      // warp-uniform (l is)
     const bool do_red = !(P.knockout & 1);            // diagnostics (PSDF_EXPERIMENT_KNOCKOUT): bit 0 no atomics, bit 1 no aggregation
-    scatter_level(x, v, sc, sh, w, a.x, a.y, a.z, a.w, valid, aggregate, do_red, lane, P.cap_mask, (unsigned)P.T,
+    scatter_level<true>(x, v, sc, sh, w, a.x, a.y, a.z, a.w, valid, aggregate, do_red, lane, P.cap_mask, (unsigned)P.T,
                   grad_lattice + (size_t)l * P.T * 2, fx_lattice ? fx_lattice + (size_t)l * P.T * 2 : nullptr);
 }
 
