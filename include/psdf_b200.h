@@ -297,6 +297,38 @@ int psdf_rgb_fused_backward(int N, int L, int T, const float* pos, const float* 
                             float* g_geom, uint8_t* workspace, float* gW0, float* gW1, float* gW2, float* gW3, float* gb0, float* gb1,
                             float* gb2, float* gb3, void* stream);
 
+/* ---------------------------------------------------------------- fused background network (NerfHash.forward, permuto_sdf_py/models/models.py:425-563)
+ * encoding(pos [N,4]) (D = 4, concat points) -> trunk in -> 64 -> 64 -> 64 -> 65 (GELU between layers); density = softplus(z[:,0]);
+ * [gelu(z[:,1:65]) | SH_4(dirs)] -> 64 -> 64 -> 3 (GELU between layers) = rgb_raw, before colour calibration and sigmoid. Seven layers on
+ * the tensor cores; weights are passed as a packed operand blob (psdf_bg_mlp_pack of the seven torch.nn.Linear weights W_l [N_l,K_l] and
+ * biases of mlp_feat_and_density and mlp_rgb). in_dim = 2L + 4, L % 4 == 0, pad16(in_dim) <= 64 (L <= 28). */
+long long psdf_bg_mlp_blob_bytes(int in_dim);
+int psdf_bg_mlp_pack(int in_dim, const float* W0, const float* b0, const float* W1, const float* b1, const float* W2, const float* b2,
+                     const float* W3, const float* b3, const float* W4, const float* b4, const float* W5, const float* b5, const float* W6,
+                     const float* b6, uint8_t* blob, void* stream);
+int psdf_bg_fused_forward(int N, int L, int T, const float* pos, const float* dirs, const float* lattice, const float* scale_factor,
+                          const float* shift, const float* window, float points_scaling, const uint8_t* blob, float* rgb_raw, float* density,
+                          void* stream);
+/* backward of psdf_bg_fused_forward (loss.backward() through NerfHash.forward, first order): g_rgb_raw [N,3], g_density [N] ->
+ * grad_lattice (+=), weight gradients gW_l [N_l,K_l] (+=) and bias gradients gb_l (+=). workspace:
+ * psdf_bg_fused_backward_workspace_bytes(N) bytes of scratch. Launches the tensor-core kernel, then the lattice-scatter kernel. */
+long long psdf_bg_fused_backward_workspace_bytes(int N);
+int psdf_bg_fused_backward(int N, int L, int T, const float* pos, const float* dirs, const float* lattice, const float* scale_factor,
+                           const float* shift, const float* window, float points_scaling, const uint8_t* blob, const float* g_rgb_raw,
+                           const float* g_density, float* grad_lattice, uint8_t* workspace, float* gW0, float* gW1, float* gW2, float* gW3,
+                           float* gW4, float* gW5, float* gW6, float* gb0, float* gb1, float* gb2, float* gb3, float* gb4, float* gb5,
+                           float* gb6, void* stream);
+/* background compositing with the colour head folded in (one thread per ray): Colorcal.calib_RGB_samples_packed + sigmoid of x_raw [N,3]
+ * (models.py:677-741; img_idx [R] per ray, weight_delta / bias may be NULL: no calibration), then VolumeRenderingNerf.compute_weights +
+ * integrate (volume_rendering_modules.py:61-89): alpha = 1 - exp(-density dt), T = exclusive cumprod(1 - alpha + 1e-7), w = alpha T,
+ * bg_rgb [R,3] = sum w rgb. The backward takes g_bg_rgb [R,3] and writes g_x [N,3], g_density [N] (rows of the rays) and adds the
+ * calibration gradients (may be NULL). */
+int psdf_nerf_bg_composite_forward(PSDF_RSP, const float* x_raw, const float* density, const float* dt, const int* img_idx,
+                                   const float* weight_delta, const float* bias, int fixed_img, float* bg_rgb, void* stream);
+int psdf_nerf_bg_composite_backward(PSDF_RSP, const float* x_raw, const float* density, const float* dt, const int* img_idx,
+                                    const float* weight_delta, const float* bias, int fixed_img, const float* g_bg_rgb, float* g_x,
+                                    float* g_density, float* g_weight_delta, float* g_bias, void* stream);
+
 /* ---------------------------------------------------------------- direct (autograd-free) training iteration
  * The reference's iteration (permuto_sdf_py/train_permuto_sdf.py:311-422) spends ~70 one-block PyTorch launches between its big kernels
  * (schedule ramps, Lipschitz normalisation, calibration, loss reductions, zero-fills, gradient adds). These entry points fold them into
@@ -338,6 +370,21 @@ int psdf_neus_head_loss_backward(PSDF_RSP, const float* sdf, const float* grad, 
                                  const float* grad_shifted, float curv_scale, const float* curv_scale_dev, int n_rows, const int* nr_valid_dev,
                                  float* g_sdf, float* g_grad, float* g_x, float* g_grad_shifted, float* g_weight_delta, float* g_bias,
                                  void* stream);
+/* the same pair for scenes without masks (train_permuto_sdf.py:149-163): bg_rgb [R,3] (psdf_nerf_bg_composite_forward) is blended in
+ * behind every ray, as psdf_neus_render_loss_* do; the backward also writes g_bg_rgb [R,3]. */
+int psdf_neus_head_bg_loss_forward(PSDF_RSP, const float* sdf, const float* grad, const float* x_raw, const float* dirs, const float* dt,
+                                   const float* inv_s_dev, float cos_anneal_ratio, const float* cos_anneal_dev, const float* gt_rgb,
+                                   const float* gt_mask, const uint8_t* hit, const int* img_idx, const float* weight_delta, const float* bias,
+                                   int fixed_img, const float* bg_rgb, float* alpha, float* transmittance, float* weights, float* pred_rgb,
+                                   float* weights_sum, float* bg_transmittance, float* ray_loss, void* stream);
+int psdf_neus_head_bg_loss_backward(PSDF_RSP, const float* sdf, const float* grad, const float* x_raw, const float* dirs, const float* dt,
+                                    const float* inv_s_dev, float cos_anneal_ratio, const float* cos_anneal_dev, const float* gt_rgb,
+                                    const float* gt_mask, const uint8_t* hit, const int* img_idx, const float* weight_delta, const float* bias,
+                                    int fixed_img, const float* bg_rgb, const float* alpha, const float* transmittance, const float* pred_rgb,
+                                    const float* weights_sum, const float* bg_transmittance, float scale_rgb, float scale_mask, float scale_eik,
+                                    const int* nr_samples_dev, const float* grad_shifted, float curv_scale, const float* curv_scale_dev, int n_rows,
+                                    const int* nr_valid_dev, float* g_sdf, float* g_grad, float* g_x, float* g_grad_shifted, float* g_bg_rgb,
+                                    float* g_weight_delta, float* g_bias, void* stream);
 /* schedule ramps from the device-resident iteration (map_range_val, permuto_sdf_py/utils/common_utils.py:156-160): out[i] = out0 +
  * (out1 - out0) / (in1 - in0) * (clamp(it, in0, in1) - in0); kinds[i] = 1 / 2: exp(10 * ramp) unclipped / clipped to [1e-6, 1e6]
  * (inv_s of SingleVarianceNetwork with a forced variance). params [n,4] = {in0, in1, out0, out1} and kinds [n] are HOST arrays, n <= 8;

@@ -169,7 +169,8 @@ def call(name, *args):
 # ---- instrumentation used by bench.py: count C-ABI calls / kernel launches and time them with CUDA events on the
 # launching stream. Kernel launches per entry point (the rest launch exactly one kernel):
 _KERNELS_PER_CALL = {"psdf_packed_compact_scan": 2, "psdf_vr_combine_uniform_samples_with_imp": 3,
-                     "psdf_sdf_fused_backward": 2, "psdf_sdf_fused_backward_multi": 2}     # tensor-core kernel + lattice scatter
+                     "psdf_sdf_fused_backward": 2, "psdf_sdf_fused_backward_multi": 2,      # tensor-core kernel + lattice scatter
+                     "psdf_bg_fused_backward": 2}
 
 
 _KERNELS_FN = {}        # entry point -> launches as a function of its arguments (none at present)

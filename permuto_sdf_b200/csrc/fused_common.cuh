@@ -18,21 +18,25 @@ constexpr int kSBO_A = 1024;           // 8 core matrices (K = 64) per 8-row gro
 // two per SM; launches clamp their persistent grids to these counts.
 constexpr int kAccCtas = 132;
 
-struct MlpGeom {
-    int K[kNL], N[kNL];        // true dims
-    int Kp[kNL], Np[kNL];      // padded dims (K % 16 == 0, N % 16 == 0)
-    int w_hi[kNL], w_lo[kNL], bias[kNL];   // byte offsets in the forward blob [0, total)
+template <int NL>
+struct MlpGeomN {
+    int K[NL], N[NL];          // true dims
+    int Kp[NL], Np[NL];        // padded dims (K % 16 == 0, N % 16 == 0)
+    int w_hi[NL], w_lo[NL], bias[NL];      // byte offsets in the forward blob [0, total)
     int total;
-    int t_hi[kNL], t_lo[kNL];  // byte offsets of the transposed weights W_l^T ([Kp rows][Np cols]) in [total, total + total_t)
+    int t_hi[NL], t_lo[NL];    // byte offsets of the transposed weights W_l^T ([Kp rows][Np cols]) in [total, total + total_t)
     int total_t;
 };
+using MlpGeom = MlpGeomN<kNL>;
 __host__ __device__ inline int pad16(int v) { return (v + 15) & ~15; }
-inline MlpGeom make_geom_dims(const int* dims) {
-    MlpGeom g;
+// layer l maps K[l] inputs to N[l] outputs (a plain chain has K[l + 1] == N[l])
+template <int NL>
+inline MlpGeomN<NL> make_geom_kn(const int* K, const int* N) {
+    MlpGeomN<NL> g;
     int off = 0;
-    for (int l = 0; l < kNL; l++) {
-        g.K[l] = dims[l]; g.N[l] = dims[l + 1];
-        g.Kp[l] = pad16(dims[l]); g.Np[l] = pad16(dims[l + 1]);
+    for (int l = 0; l < NL; l++) {
+        g.K[l] = K[l]; g.N[l] = N[l];
+        g.Kp[l] = pad16(K[l]); g.Np[l] = pad16(N[l]);
         int wbytes = g.Np[l] * g.Kp[l] * 2;
         g.w_hi[l] = off; off += wbytes;
         g.w_lo[l] = off; off += wbytes;
@@ -40,7 +44,7 @@ inline MlpGeom make_geom_dims(const int* dims) {
     }
     g.total = (off + 127) & ~127;
     off = 0;
-    for (int l = 0; l < kNL; l++) {
+    for (int l = 0; l < NL; l++) {
         int wbytes = g.Np[l] * g.Kp[l] * 2;
         g.t_hi[l] = off; off += wbytes;
         g.t_lo[l] = off; off += wbytes;
@@ -48,31 +52,23 @@ inline MlpGeom make_geom_dims(const int* dims) {
     g.total_t = (off + 127) & ~127;
     return g;
 }
+inline MlpGeom make_geom_dims(const int* dims) { return make_geom_kn<kNL>(dims, dims + 1); }
 inline MlpGeom make_geom(int in_dim, int hidden, int out_dim) {
     int dims[kNL + 1] = {in_dim, hidden, hidden, hidden, out_dim};
     return make_geom_dims(dims);
 }
 
-// weights [N][K] fp32 (torch.nn.Linear layout) -> hi/lo bf16 in the K-major core-matrix operand layout + fp32 bias;
-// second half of the blob: the same weights transposed (rows = input features, K = output features) for the
-// backward GEMMs dA = dZ * W
-static __global__ void k_pack_mlp(MlpGeom g, const float* W0, const float* b0, const float* W1, const float* b1, const float* W2,
-                                  const float* b2, const float* W3, const float* b3, uint8_t* blob, int* step_inc = nullptr,
-                                  float* it_inc = nullptr) {
-    // end-of-iteration bookkeeping folded into the re-pack that closes an optimizer step: AdamW step count and iteration number, both
-    // device resident under CUDA-graph replay (every kernel that read them in this iteration has completed: same stream)
-    if (blockIdx.x == 0 && blockIdx.y == 0 && threadIdx.x == 0) {
-        if (step_inc) step_inc[0] += 1;
-        if (it_inc) it_inc[0] += 1.0f;
-    }
-    const float* W[kNL] = {W0, W1, W2, W3};
-    const float* B[kNL] = {b0, b1, b2, b3};
-    int l = blockIdx.y;
-    int e = blockIdx.x * blockDim.x + threadIdx.x;
+// Element e of layer l: weights [N][K] fp32 (torch.nn.Linear layout) -> hi/lo bf16 in the K-major core-matrix operand layout + fp32 bias;
+// second half of the blob: the same weights transposed (rows = input features, K = output features) for the backward GEMMs
+// dA = dZ * W. Packed row n holds source row (n + rot) % N (rot = 0: the same order).
+template <int NL>
+__device__ __forceinline__ void pack_layer_elem(const MlpGeomN<NL>& g, int l, int e, const float* Wl, const float* Bl, uint8_t* blob,
+                                                int rot = 0) {
     int total = g.Np[l] * g.Kp[l];
     if (e < total) {
         int n = e / g.Kp[l], k = e - n * g.Kp[l];
-        float v = (n < g.N[l] && k < g.K[l]) ? W[l][n * g.K[l] + k] : 0.0f;
+        const int src = rot ? (n + rot) % g.N[l] : n;
+        float v = (n < g.N[l] && k < g.K[l]) ? Wl[src * g.K[l] + k] : 0.0f;
         __nv_bfloat16 hi, lo;
         umma::split_bf16(v, hi, lo);
         int sbo = (g.Kp[l] / 8) * kLBO;
@@ -85,57 +81,82 @@ static __global__ void k_pack_mlp(MlpGeom g, const float* W0, const float* b0, c
         *reinterpret_cast<__nv_bfloat16*>(blob + g.total + g.t_hi[l] + off_t) = hi;
         *reinterpret_cast<__nv_bfloat16*>(blob + g.total + g.t_lo[l] + off_t) = lo;
     }
-    if (e < g.Np[l]) reinterpret_cast<float*>(blob + g.bias[l])[e] = (e < g.N[l]) ? B[l][e] : 0.0f;
+    if (e < g.Np[l]) reinterpret_cast<float*>(blob + g.bias[l])[e] = (e < g.N[l]) ? Bl[rot ? (e + rot) % g.N[l] : e] : 0.0f;
+}
+static __global__ void k_pack_mlp(MlpGeom g, const float* W0, const float* b0, const float* W1, const float* b1, const float* W2,
+                                  const float* b2, const float* W3, const float* b3, uint8_t* blob, int* step_inc = nullptr,
+                                  float* it_inc = nullptr) {
+    // end-of-iteration bookkeeping folded into the re-pack that closes an optimizer step: AdamW step count and iteration number, both
+    // device resident under CUDA-graph replay (every kernel that read them in this iteration has completed: same stream)
+    if (blockIdx.x == 0 && blockIdx.y == 0 && threadIdx.x == 0) {
+        if (step_inc) step_inc[0] += 1;
+        if (it_inc) it_inc[0] += 1.0f;
+    }
+    const float* W[kNL] = {W0, W1, W2, W3};
+    const float* B[kNL] = {b0, b1, b2, b3};
+    int l = blockIdx.y;
+    pack_layer_elem(g, l, blockIdx.x * blockDim.x + threadIdx.x, W[l], B[l], blob);
 }
 
-// ---------------------------------------------------------------------------------------------- lattice helpers (D = 3)
-struct Simplex3 { int rem0[4]; int rank[4]; float bary[5]; };
-__device__ __forceinline__ void elevate3(const float* cf, float* e) {
+// ---------------------------------------------------------------------------------------------- lattice helpers (D = 3, 4)
+// D = 3: the SDF and colour encoders; D = 4: the background encoder (NeRF++ parametrisation)
+template <int D>
+struct Simplex { int rem0[D + 1]; int rank[D + 1]; float bary[D + 2]; };
+using Simplex3 = Simplex<3>;
+template <int D>
+__device__ __forceinline__ void elevate(const float* cf, float* e) {
     float sm = 0.0f;
 #pragma unroll
-    for (int i = 3; i > 0; i--) { e[i] = __fmaf_rn(-(float)i, cf[i - 1], sm); sm = __fadd_rn(sm, cf[i - 1]); }
+    for (int i = D; i > 0; i--) { e[i] = __fmaf_rn(-(float)i, cf[i - 1], sm); sm = __fadd_rn(sm, cf[i - 1]); }
     e[0] = sm;
 }
-// D[k] = d[i] of the coordinate i whose rank is k (ranks are a permutation of 0..3)
-__device__ __forceinline__ void by_rank(const Simplex3& s, const float* d, float* D) {
-#pragma unroll
-    for (int k = 0; k < 4; k++) D[k] = s.rank[0] == k ? d[0] : (s.rank[1] == k ? d[1] : (s.rank[2] == k ? d[2] : d[3]));
+// R[k] = d[i] of the coordinate i whose rank is k (ranks are a permutation of 0..D)
+template <int D, int I = 0>
+__device__ __forceinline__ float rank_pick(const Simplex<D>& s, const float* d, int k) {
+    if constexpr (I == D) return d[D];
+    else return s.rank[I] == k ? d[I] : rank_pick<D, I + 1>(s, d, k);
 }
-__device__ __forceinline__ void locate3(const float* e, Simplex3& s) {
+template <int D>
+__device__ __forceinline__ void by_rank(const Simplex<D>& s, const float* d, float* R) {
+#pragma unroll
+    for (int k = 0; k <= D; k++) R[k] = rank_pick<D>(s, d, k);
+}
+template <int D>
+__device__ __forceinline__ void locate(const float* e, Simplex<D>& s) {
+    constexpr float kInv = 1.0f / (float)(D + 1), kD1 = (float)(D + 1);
     int sum = 0;
 #pragma unroll
-    for (int i = 0; i < 4; i++) {
-        float v = __fmul_rn(e[i], 0.25f);
-        // ceil(v) * 4 == floor(v) * 4 + 4 unless v is an integer, where both candidates coincide with e[i] and `down` wins either way
-        const float down = __fmul_rn(floorf(v), 4.0f), up = __fadd_rn(down, 4.0f);
+    for (int i = 0; i <= D; i++) {
+        float v = __fmul_rn(e[i], kInv);
+        // ceil(v) (D+1) == floor(v) (D+1) + D+1 unless v is an integer, where both candidates coincide with e[i] and `down` wins either way
+        const float down = __fmul_rn(floorf(v), kD1), up = __fadd_rn(down, kD1);
         s.rem0[i] = (__fsub_rn(up, e[i]) < __fsub_rn(e[i], down)) ? (int)up : (int)down;
         sum += s.rem0[i];
         s.rank[i] = 0;
     }
-    sum /= 4;
+    sum /= D + 1;
 #pragma unroll
-    for (int i = 0; i < 3; i++) {
+    for (int i = 0; i < D; i++) {
         float di = __fsub_rn(e[i], (float)s.rem0[i]);
 #pragma unroll
-        for (int j = i + 1; j < 4; j++) { if (di < __fsub_rn(e[j], (float)s.rem0[j])) s.rank[i]++; else s.rank[j]++; }
+        for (int j = i + 1; j <= D; j++) { if (di < __fsub_rn(e[j], (float)s.rem0[j])) s.rank[i]++; else s.rank[j]++; }
     }
 #pragma unroll
-    for (int i = 0; i < 4; i++) {
+    for (int i = 0; i <= D; i++) {
         s.rank[i] += sum;
-        if (s.rank[i] < 0) { s.rank[i] += 4; s.rem0[i] += 4; }
-        else if (s.rank[i] > 3) { s.rank[i] -= 4; s.rem0[i] -= 4; }
+        if (s.rank[i] < 0) { s.rank[i] += D + 1; s.rem0[i] += D + 1; }
+        else if (s.rank[i] > D) { s.rank[i] -= D + 1; s.rem0[i] -= D + 1; }
     }
-    // barycentric weights: with D_k the fractional offset of the coordinate of rank k, the reference's scatter
-    // (+delta at 3 - rank, -delta at 4 - rank) is bary_r = D_{3-r} - D_{4-r}, bary_0 = D_3 + (1 - D_0)
-    float delta[4], D[4];
+    // barycentric weights: with R_k the fractional offset of the coordinate of rank k, the reference's scatter
+    // (+delta at D - rank, -delta at D + 1 - rank) is bary_r = R_{D-r} - R_{D+1-r}, bary_0 = R_D + (1 - R_0)
+    float delta[D + 1], R[D + 1];
 #pragma unroll
-    for (int i = 0; i < 4; i++) delta[i] = __fmul_rn(__fsub_rn(e[i], (float)s.rem0[i]), 0.25f);
-    by_rank(s, delta, D);
-    s.bary[0] = __fadd_rn(D[3], __fsub_rn(1.0f, D[0]));
-    s.bary[1] = __fsub_rn(D[2], D[3]);
-    s.bary[2] = __fsub_rn(D[1], D[2]);
-    s.bary[3] = __fsub_rn(D[0], D[1]);
-    s.bary[4] = -D[0];
+    for (int i = 0; i <= D; i++) delta[i] = __fmul_rn(__fsub_rn(e[i], (float)s.rem0[i]), kInv);
+    by_rank<D>(s, delta, R);
+    s.bary[0] = __fadd_rn(R[D], __fsub_rn(1.0f, R[0]));
+#pragma unroll
+    for (int r = 1; r <= D; r++) s.bary[r] = __fsub_rn(R[D - r], R[D + 1 - r]);
+    s.bary[D + 1] = -R[0];
 }
 // tangent of the barycentric weights along the (scaled) direction dcf: the same rank scatter applied to its elevation
 __device__ __forceinline__ void bary_tangent3(const float* dcf, const Simplex3& s, float* db) {
@@ -143,22 +164,30 @@ __device__ __forceinline__ void bary_tangent3(const float* dcf, const Simplex3& 
 #pragma unroll
     for (int i = 3; i > 0; i--) { de[i] = (sm - (float)i * dcf[i - 1]) * 0.25f; sm += dcf[i - 1]; }
     de[0] = sm * 0.25f;
-    by_rank(s, de, dD);
+    by_rank<3>(s, de, dD);
     db[0] = dD[3] - dD[0]; db[1] = dD[2] - dD[3]; db[2] = dD[1] - dD[2]; db[3] = dD[0] - dD[1];
 }
 // h mod T without a division: q = umulhi(h, floor(2^32 / T)) is the quotient or one less, so one conditional subtraction finishes it
 // (exact for every 32-bit h; a power-of-two T needs no correction). `magic` = t_magic(T), computed on the host.
 inline unsigned t_magic(int T) { return T <= 1 ? 0xffffffffu : (unsigned)(0x100000000ull / (unsigned long long)(unsigned)T); }
-// The hash h = ((k0 P + k1) P + k2) P (mod 2^32) of the vertex key k_i = rem0[i] + r - 4 [rank[i] > 3 - r] is linear in the key over the
-// ring Z / 2^32: h_r = h_0 + r (P^3 + P^2 + P) - sum_i [rank[i] > 3 - r] 4 P^(3-i) with h_0 = rem0[0] P^3 + rem0[1] P^2 + rem0[2] P, so the
-// four vertices of a simplex share h_0 (3 multiply-adds) and each one costs 3 compare + subtract pairs -- same bits as the
+// The hash h = ((k0 P + k1) P + ...) P (mod 2^32) of the vertex key k_i = rem0[i] + r - (D+1) [rank[i] > D - r], i < D, is linear in the
+// key over the ring Z / 2^32: h_r = h_0 + r (P^D + ... + P) - sum_i [rank[i] > D - r] (D+1) P^(D-i) with h_0 = sum_i rem0[i] P^(D-i), so the
+// D+1 vertices of a simplex share h_0 (D multiply-adds) and each one costs D compare + subtract pairs -- same bits as the
 // multiply chain per vertex, less than half of its instructions.
-__device__ __forceinline__ unsigned vindex3(const Simplex3& s, int r, unsigned magic, unsigned T) {
-    constexpr unsigned P1 = 2531011u, P2 = P1 * P1, P3 = P2 * P1;
-    unsigned h = (unsigned)s.rem0[0] * P3 + (unsigned)s.rem0[1] * P2 + (unsigned)s.rem0[2] * P1 + (unsigned)r * (P3 + P2 + P1);
-    if (s.rank[0] > 3 - r) h -= 4u * P3;
-    if (s.rank[1] > 3 - r) h -= 4u * P2;
-    if (s.rank[2] > 3 - r) h -= 4u * P1;
+template <int D>
+__device__ __forceinline__ unsigned vindex(const Simplex<D>& s, int r, unsigned magic, unsigned T) {
+    constexpr unsigned P1 = 2531011u;
+    unsigned pw[D];                    // pw[i] = P^(D - i)
+    pw[D - 1] = P1;
+#pragma unroll
+    for (int i = D - 2; i >= 0; i--) pw[i] = pw[i + 1] * P1;
+    unsigned h = 0u, psum = 0u;
+#pragma unroll
+    for (int i = 0; i < D; i++) { h += (unsigned)s.rem0[i] * pw[i]; psum += pw[i]; }
+    h += (unsigned)r * psum;
+#pragma unroll
+    for (int i = 0; i < D; i++)
+        if (s.rank[i] > D - r) h -= (unsigned)(D + 1) * pw[i];
     unsigned rem = h - __umulhi(h, magic) * T;
     return rem >= T ? rem - T : rem;
 }
@@ -188,33 +217,35 @@ struct FusedParams {
     MlpGeom g;
 };
 
-// ---------------------------------------------------------------------------------------------- encoder of one level (D = 3, F = 2)
+// ---------------------------------------------------------------------------------------------- encoder of one level (D = 3, 4; F = 2)
 // Level constants in shared memory; scale / shift rows padded to 4 floats.
 struct LevelC { float scale[kMaxLevels * 4]; float shift[kMaxLevels * 4]; float window[kMaxLevels]; };
+template <int D = 3>
 __device__ __forceinline__ void load_level_consts(LevelC* lc, int L, const float* scale, const float* shift, const float* window, int tid,
                                                   int nthreads) {
-    for (int i = tid; i < L * 3; i += nthreads) {
-        lc->scale[(i / 3) * 4 + (i % 3)] = scale[i];
-        lc->shift[(i / 3) * 4 + (i % 3)] = shift ? shift[i] : 0.0f;
+    for (int i = tid; i < L * D; i += nthreads) {
+        lc->scale[(i / D) * 4 + (i % D)] = scale[i];
+        lc->shift[(i / D) * 4 + (i % D)] = shift ? shift[i] : 0.0f;
     }
     for (int i = tid; i < L; i += nthreads) lc->window[i] = window ? window[i] : 1.0f;
 }
-// The two window-weighted features (a0, a1) = w sum_r B_r v_r of position x at level l. Also returns the simplex s and the four vertex
+// The two window-weighted features (a0, a1) = w sum_r B_r v_r of position x at level l. Also returns the simplex s and the D+1 vertex
 // values v, from which the callers form tangents.
+template <int D>
 __device__ __forceinline__ float2 level_features(const float* x, const LevelC* lc, int l, const float2* __restrict__ lattice, int T,
-                                                 unsigned cap_mask, Simplex3& s, float2* v) {
-    float cf[3], e[4];
+                                                 unsigned cap_mask, Simplex<D>& s, float2* v) {
+    float cf[D], e[D + 1];
 #pragma unroll
-    for (int i = 0; i < 3; i++) cf[i] = __fmul_rn(__fadd_rn(x[i], lc->shift[l * 4 + i]), lc->scale[l * 4 + i]);
-    elevate3(cf, e);
-    locate3(e, s);
+    for (int i = 0; i < D; i++) cf[i] = __fmul_rn(__fadd_rn(x[i], lc->shift[l * 4 + i]), lc->scale[l * 4 + i]);
+    elevate<D>(cf, e);
+    locate<D>(e, s);
     const float w = lc->window[l];      // read before the gathers: with this order ptxas spills the least in k_sdf_fused_backward
     const float2* tab = lattice + (size_t)l * T;
 #pragma unroll
-    for (int r = 0; r < 4; r++) v[r] = __ldg(tab + vindex3(s, r, cap_mask, (unsigned)T));
+    for (int r = 0; r <= D; r++) v[r] = __ldg(tab + vindex<D>(s, r, cap_mask, (unsigned)T));
     float a0 = 0.f, a1 = 0.f;
 #pragma unroll
-    for (int r = 0; r < 4; r++) { const float wr = s.bary[r] * w; a0 = fmaf(v[r].x, wr, a0); a1 = fmaf(v[r].y, wr, a1); }
+    for (int r = 0; r <= D; r++) { const float wr = s.bary[r] * w; a0 = fmaf(v[r].x, wr, a0); a1 = fmaf(v[r].y, wr, a1); }
     return make_float2(a0, a1);
 }
 // d feat / d x_j (j = 0..2) of one level's two features: ft[j] = w scale_j / 4 * sum_i E[i][j] G_i, with G_i = u_{rank_i},
@@ -365,28 +396,29 @@ __device__ __forceinline__ void scatter2(float* gtab, unsigned long long* ftab, 
 }
 // Encoder backward of one sample at one level, called by a whole warp (one sample per lane):
 //     lattice[idx_r] += w (B_r abar + dB_r tabar),  r = 0..3,   abar = (a0, a1), tabar = (t0, t1) of the level's two features
-// x, v: position and tangent direction; scale3 / shift3: the level's scale and shift; gtab / ftab: the level's float / fixed-point
-// gradient table (scatter2). TAN = false: no tangent term (v, t0, t1 unused), lattice[idx_r] += w B_r abar. Invalid lanes add nothing.
-// aggregate: warp-uniform, sum the lanes that share a vertex first (match_any + add_peers2, one reduction per distinct vertex);
-// do_red = false issues no reduction (diagnostics, PSDF_EXPERIMENT_KNOCKOUT).
-template <bool TAN>
+// x, v: position and tangent direction (D coordinates); scale3 / shift3: the level's scale and shift; gtab / ftab: the level's float /
+// fixed-point gradient table (scatter2). TAN = false: no tangent term (v, t0, t1 unused), lattice[idx_r] += w B_r abar. Invalid lanes add
+// nothing. aggregate: warp-uniform, sum the lanes that share a vertex first (match_any + add_peers2, one reduction per distinct vertex);
+// do_red = false issues no reduction (diagnostics, PSDF_EXPERIMENT_KNOCKOUT). The tangent term exists for D = 3 only.
+template <bool TAN, int D = 3>
 __device__ __forceinline__ void scatter_level(const float* x, const float* v, const float* scale3, const float* shift3, float w, float a0,
                                               float a1, float t0, float t1, bool valid, bool aggregate, bool do_red, int lane,
                                               unsigned cap_mask, unsigned T, float* gtab, unsigned long long* ftab) {
-    float cf[3], dcf[3], e[4];
+    static_assert(D == 3 || !TAN, "the tangent term of the lattice scatter exists for D = 3 only");
+    float cf[D], dcf[D], e[D + 1];
 #pragma unroll
-    for (int i = 0; i < 3; i++) {
+    for (int i = 0; i < D; i++) {
         cf[i] = __fmul_rn(__fadd_rn(x[i], shift3[i]), scale3[i]);
         if constexpr (TAN) dcf[i] = v[i] * scale3[i];
     }
-    elevate3(cf, e);
-    Simplex3 s;
-    locate3(e, s);
-    float db[5];
+    elevate<D>(cf, e);
+    Simplex<D> s;
+    locate<D>(e, s);
+    float db[D + 2];
     if constexpr (TAN) bary_tangent3(dcf, s, db);
 #pragma unroll
-    for (int r = 0; r < 4; r++) {
-        unsigned idx = vindex3(s, r, cap_mask, T);
+    for (int r = 0; r <= D; r++) {
+        unsigned idx = vindex<D>(s, r, cap_mask, T);
         float cb = s.bary[r] * w;
         float2 cv;
         if constexpr (TAN) {

@@ -45,52 +45,6 @@ struct RgbSpill {
     unsigned long long* fx_lattice;   // deterministic mode: fixed-point accumulators (DetBufs::rgb_lattice, ::rgb_mlp), else NULL
     unsigned long long* fx_mlp;
 };
-// Rows [m0, m0 + 64) x columns [c0, c0 + N) of this tile's dW_l in the issuing warpgroup's registers, then added in fixed point to the
-// CTA's sums `dw` ([128 rows][128 columns] of the layer; `first`: the CTA's first tile, which sets them). Every slot belongs to one
-// thread for the whole launch (the fragment position), so the read-modify-write needs no atomics. Each tile's product is rounded to
-// the fixed-point grid before it is added, as a per-tile flush would round it: the totals do not depend on how tiles map to CTAs.
-template <int N>
-__device__ __forceinline__ void dw_rows_fx(unsigned long long* dw, int m0, int c0, uint64_t dzh, uint64_t dzl, uint64_t dah, uint64_t dal,
-                                           bool first) {
-    float d[N / 2];
-#pragma unroll
-    for (int i = 0; i < N / 2; i++) d[i] = 0.f;
-    umma::wgmma_fence();
-    // 16 samples = 2 eight-row groups per K step
-    umma::wg_mma_regs<N, 1, 1>(d, dzh, dzl, dah, dal, (2 * kWSBO) >> 4, (2 * kWSBO) >> 4, kTile / 16, false);
-    umma::wgmma_commit();
-    umma::wgmma_wait0();
-#pragma unroll
-    for (int h = 0; h < 2; h++) {
-        unsigned long long* p = dw + (size_t)frag_row(0, h) * 128 + m0 * 128 + c0;
-#pragma unroll
-        for (int j = 0; j < N / 8; j++) {
-            ulonglong2* q = reinterpret_cast<ulonglong2*>(p + frag_col(j));
-            ulonglong2 v = first ? make_ulonglong2(0ull, 0ull) : *q;
-            v.x += fx_of(d[4 * j + 2 * h]);
-            v.y += fx_of(d[4 * j + 2 * h + 1]);
-            *q = v;
-        }
-    }
-}
-// dW_l = zbar^(l)^T a_l over the 128 samples of the tile: both tiles consumed as MN-major operands (one warpgroup, `half` = 0 / 1).
-// M = 128: the two warpgroups take rows 0..63 / 64..127; M = 64: columns [0, na) / [na, N) of one M = 64 product. Added to the CTA's
-// fixed-point sums (dw_rows_fx) in pieces of at most 32 columns (register budget).
-__device__ __forceinline__ void issue_dw_w(unsigned long long* dw, int half, const uint8_t* z_hi, const uint8_t* a_hi, int M, int N, bool first) {
-    int m0 = 0, n0 = 0, nn = N;
-    if (M == 128) m0 = 64 * half;
-    else split_n(N, half, n0, nn);
-    if (nn <= 0) return;
-    const uint32_t zh = umma::smem_u32(z_hi) + (uint32_t)(m0 / 8) * kLBO;
-    const uint64_t dzh = umma::make_desc(zh, kWSBO, kLBO), dzl = umma::make_desc(zh + kWTileBytes, kWSBO, kLBO);
-    for (int p0 = 0; p0 < nn; p0 += 32) {
-        const uint32_t ah = umma::smem_u32(a_hi) + (uint32_t)((n0 + p0) / 8) * kLBO;
-        const uint64_t dah = umma::make_desc(ah, kWSBO, kLBO), dal = umma::make_desc(ah + kWTileBytes, kWSBO, kLBO);
-        if (nn - p0 >= 32) dw_rows_fx<32>(dw, m0, n0 + p0, dzh, dzl, dah, dal, first);
-        else dw_rows_fx<16>(dw, m0, n0 + p0, dzh, dzl, dah, dal, first);
-    }
-}
-
 __global__ void __launch_bounds__(kRgbThreads, 1)
 k_rgb_fused_backward(RgbParams P, const float* __restrict__ pos, const float* __restrict__ dirs, const float* __restrict__ sdf_grad,
                      const float* __restrict__ geom, const float2* __restrict__ lattice, const float* __restrict__ scale,

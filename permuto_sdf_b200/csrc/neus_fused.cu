@@ -426,4 +426,38 @@ int psdf_neus_head_loss_backward(int nr_rays, int max_nr_samples, const int* ray
                               cos_anneal_dev, gt_rgb, gt_mask, hit, nullptr, alpha, transmittance, pred_rgb, weights_sum, bg_transmittance,
                               nullptr, scale_rgb, scale_mask, scale_eik, nr_samples_dev, g_sdf, g_grad, g_x, nullptr, nullptr, e, stream);
 }
+// The head-loss pair of a scene without masks: bg_rgb [R,3] (the composited background colour) is blended in behind every ray, and the
+// backward also returns g_bg_rgb [R,3] (=).
+int psdf_neus_head_bg_loss_forward(int nr_rays, int max_nr_samples, const int* ray_start_end, int equal, int fixed_n, const float* sdf,
+                                   const float* grad, const float* x_raw, const float* dirs, const float* dt, const float* inv_s_dev,
+                                   float cos_anneal_ratio, const float* cos_anneal_dev, const float* gt_rgb, const float* gt_mask, const uint8_t* hit,
+                                   const int* img_idx, const float* weight_delta, const float* bias, int fixed_img, const float* bg_rgb,
+                                   float* alpha, float* transmittance, float* weights, float* pred_rgb, float* weights_sum,
+                                   float* bg_transmittance, float* ray_loss, void* stream) {
+    NeusExt e = no_ext();
+    e.head = 1; e.img_idx = weight_delta ? img_idx : nullptr; e.weight_delta = weight_delta; e.bias = bias; e.fixed_img = fixed_img;
+    return neus_forward_impl(nr_rays, max_nr_samples, ray_start_end, equal, fixed_n, sdf, grad, x_raw, dirs, dt, inv_s_dev, cos_anneal_ratio,
+                             cos_anneal_dev, gt_rgb, gt_mask, hit, bg_rgb, alpha, transmittance, weights, pred_rgb, weights_sum, bg_transmittance,
+                             ray_loss, e, stream);
+}
+int psdf_neus_head_bg_loss_backward(int nr_rays, int max_nr_samples, const int* ray_start_end, int equal, int fixed_n, const float* sdf,
+                                    const float* grad, const float* x_raw, const float* dirs, const float* dt, const float* inv_s_dev,
+                                    float cos_anneal_ratio, const float* cos_anneal_dev, const float* gt_rgb, const float* gt_mask, const uint8_t* hit,
+                                    const int* img_idx, const float* weight_delta, const float* bias, int fixed_img, const float* bg_rgb,
+                                    const float* alpha, const float* transmittance, const float* pred_rgb, const float* weights_sum,
+                                    const float* bg_transmittance, float scale_rgb, float scale_mask, float scale_eik, const int* nr_samples_dev,
+                                    const float* grad_shifted, float curv_scale, const float* curv_scale_dev, int n_rows, const int* nr_valid_dev,
+                                    float* g_sdf, float* g_grad, float* g_x, float* g_grad_shifted, float* g_bg_rgb, float* g_weight_delta,
+                                    float* g_bias, void* stream) {
+    NeusExt e = no_ext();
+    e.head = 1; e.img_idx = weight_delta ? img_idx : nullptr; e.weight_delta = weight_delta; e.bias = bias; e.fixed_img = fixed_img;
+    e.g_weight_delta = g_weight_delta; e.g_bias = g_bias;
+    e.gs = grad_shifted; e.ggs = g_grad_shifted; e.curv_scale = curv_scale; e.curv_scale_dev = curv_scale_dev;
+    if (grad_shifted && !g_grad_shifted) return PSDF_ERR_ARG;
+    e.n_rows = nr_valid_dev ? n_rows : 0;
+    e.nr_valid_dev = nr_valid_dev;
+    return neus_backward_impl(nr_rays, max_nr_samples, ray_start_end, equal, fixed_n, sdf, grad, x_raw, dirs, dt, inv_s_dev, cos_anneal_ratio,
+                              cos_anneal_dev, gt_rgb, gt_mask, hit, bg_rgb, alpha, transmittance, pred_rgb, weights_sum, bg_transmittance,
+                              nullptr, scale_rgb, scale_mask, scale_eik, nr_samples_dev, g_sdf, g_grad, g_x, g_bg_rgb, nullptr, e, stream);
+}
 }  // extern "C"

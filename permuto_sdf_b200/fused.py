@@ -471,6 +471,103 @@ def _fused_rgb_train_forward(self, points, samples_dirs, sdf_gradients, geom_fea
 FusedRGB.train_forward = _fused_rgb_train_forward
 
 
+# ================================================================================================ fused background network
+class FusedNerfHash:
+    """models.NerfHash on the tensor cores (csrc/fused_bg.cu): 4-D encoding -> trunk (density) -> colour head, seven layers in one kernel
+    each way. Produces the linear colour (before calibration / sigmoid) and the density."""
+
+    def __init__(self, model_bg):
+        self.model = model_bg
+        enc = model_bg.encoding
+        trunk = [m for m in model_bg.mlp_feat_and_density if isinstance(m, torch.nn.Linear)]
+        head = [m for m in model_bg.mlp_rgb if isinstance(m, torch.nn.Linear)]
+        self.lin = trunk + head
+        dims = [(l.in_features, l.out_features) for l in self.lin]
+        if enc.pos_dim != 4 or enc.nr_feat_per_level != 2 or not enc.concat_points or enc.nr_levels % 4 != 0:
+            raise RuntimeError("FusedNerfHash needs pos_dim 4, 2 features per level, concat_points and nr_levels % 4 == 0")
+        self.in_dim = enc.output_dims()
+        want = [(self.in_dim, 64), (64, 64), (64, 64), (64, 65), (80, 64), (64, 64), (64, 3)]
+        if dims != want:
+            raise RuntimeError("FusedNerfHash supports the 7-layer NerfHash MLPs of the reference (models.py:437-447), got %s" % dims)
+        lib = load_library()
+        nbytes = int(lib.psdf_bg_mlp_blob_bytes(self.in_dim))
+        if nbytes == 0:
+            raise RuntimeError("FusedNerfHash: %d encoder columns are more than the fused kernel takes (nr_levels <= 28)" % self.in_dim)
+        self.blob = torch.empty(nbytes, dtype=torch.uint8, device=enc.lattice_values.device)
+
+    def params(self):
+        return [p for l in self.lin for p in (l.weight, l.bias)]
+
+    def pack(self, params):
+        call("psdf_bg_mlp_pack", self.in_dim, *[p.detach() for p in params], self.blob)
+        self.packed_versions = tuple(p._version for p in params)
+
+    def _window(self, iter_nr):
+        from .models import map_range_val
+        m = self.model
+        m.last_iter_nr = int(iter_nr)
+        return m.c2f(map_range_val(iter_nr, 0.0, m.nr_iters_for_c2f, 0.3, 1.0)).view(-1).contiguous()
+
+    def _forward(self, pos, dirs, lattice, window):
+        enc = self.model.encoding
+        N = pos.shape[0]
+        rgb = torch.empty(N, 3, device=pos.device)
+        density = torch.empty(N, 1, device=pos.device)
+        call("psdf_bg_fused_forward", N, enc.nr_levels, enc.capacity, pos, dirs, lattice.detach(), enc.scale_factor, enc.shift_tensor(), window,
+             enc.concat_points_scaling, self.blob, rgb, density)
+        return rgb, density
+
+    @torch.no_grad()
+    def __call__(self, samples_pos, samples_dirs, iter_nr):
+        """-> (linear colour [N,3], density [N,1]), no autograd"""
+        self.pack(self.params())
+        return self._forward(samples_pos.detach().contiguous(), samples_dirs.detach().contiguous(), self.model.encoding.lattice_values,
+                             self._window(iter_nr))
+
+    def train_forward(self, samples_pos, samples_dirs, iter_nr):
+        """differentiable (wrt the hash table, weights and biases) linear colour [N,3] and density [N,1]"""
+        return _FusedNerfHashFn.apply(samples_pos.detach().contiguous(), samples_dirs.detach().contiguous(), self.model.encoding.lattice_values,
+                                      self._window(iter_nr), self, *self.params())
+
+
+class _FusedNerfHashFn(torch.autograd.Function):
+    """forward: psdf_bg_fused_forward; backward: psdf_bg_fused_backward (reverse sweep + tensor-core dW, then the lattice scatter)"""
+
+    @staticmethod
+    def forward(ctx, pos, dirs, lattice, window, fb, *params):
+        fb.pack(params)
+        ctx.fb, ctx.versions = fb, fb.packed_versions
+        ctx.save_for_backward(pos, dirs, lattice, window)
+        return fb._forward(pos, dirs, lattice, window)
+
+    @staticmethod
+    def backward(ctx, g_rgb, g_density):
+        fb = ctx.fb
+        pos, dirs, lattice, window = ctx.saved_tensors
+        enc = fb.model.encoding
+        N = pos.shape[0]
+        dev = pos.device
+        params = fb.params()
+        # with a flat-buffer optimizer the gradients accumulate straight into the persistent .grad buffers (as in the colour network)
+        in_place = getattr(enc, "grad_in_place", False) and lattice.grad is not None and lattice.grad.is_contiguous() and \
+            all(p.grad is not None and p.grad.is_contiguous() for p in params)
+        grads = [p.grad for p in params] if in_place else [torch.zeros_like(p) for p in params]
+        g_lat = lattice.grad if in_place else torch.zeros_like(lattice)
+        g_rgb = torch.zeros(N, 3, device=dev) if g_rgb is None else g_rgb.contiguous()
+        g_density = torch.zeros(N, 1, device=dev) if g_density is None else g_density.contiguous()
+        ws = torch.empty(int(load_library().psdf_bg_fused_backward_workspace_bytes(N)), dtype=torch.uint8, device=dev)
+        # the backward needs the weights of its forward: unchanged parameters, and the blob packed from them
+        if tuple(p._version for p in params) != ctx.versions:
+            raise RuntimeError("FusedNerfHash: a parameter was modified in place between the forward and its backward")
+        if fb.packed_versions != ctx.versions:
+            fb.pack(params)
+        call("psdf_bg_fused_backward", N, enc.nr_levels, enc.capacity, pos, dirs, lattice.detach(), enc.scale_factor, enc.shift_tensor(),
+             window, enc.concat_points_scaling, fb.blob, g_rgb, g_density, g_lat, ws, *grads[0::2], *grads[1::2])
+        if in_place:
+            return (None,) * (5 + len(params))
+        return (None, None, g_lat, None, None) + tuple(grads)
+
+
 # ================================================================================================ curvature loss
 class CurvatureLossFn(torch.autograd.Function):
     """mean over the valid samples of acos(clamp(normalize(g) . normalize(g_shifted))) / pi (models.py:283-294 +

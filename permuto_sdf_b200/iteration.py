@@ -46,8 +46,8 @@ class DirectIteration:
     @staticmethod
     def unsupported_reason(tr):
         hp = tr.hp
-        if not hp.with_mask or tr.model_bg is not None:
-            return "background model (no --with_mask) runs on the autograd formulation"
+        if tr.model_bg is not None and getattr(tr.model_bg, "fused", None) is None:
+            return "background model (no --with_mask) on the per-op kernels (Trainer(fused_background=True) fuses it)"
         if not tr.fused_render:
             return "fused_render is off"
         if getattr(tr.model_sdf, "fused", None) is None or not getattr(tr.model_sdf, "fused_training", False):
@@ -99,6 +99,17 @@ class DirectIteration:
         self._ws, self._ws_key = ws, key
         return ws
 
+    def _bg_workspace(self, Nb, R, dev):
+        key = (Nb, R, str(dev))
+        if getattr(self, "_bg_key", None) != key:
+            from ._lib import load_library
+            f = lambda *s: torch.empty(*s, device=dev)
+            self._bg_ws = dict(x=f(Nb, 3), density=f(Nb, 1), bg_rgb=f(R, 3), g_bg_rgb=f(R, 3), g_x=torch.zeros(Nb, 3, device=dev),
+                               g_density=torch.zeros(Nb, device=dev),
+                               ws=torch.empty(int(load_library().psdf_bg_fused_backward_workspace_bytes(Nb)), dtype=torch.uint8, device=dev))
+            self._bg_key = key
+        return self._bg_ws
+
     def _scalars(self, it, ws):
         """cos-anneal ratio [0], inv_s unclipped [1] / clipped [2], curvature ramp [3] from the (device-resident) iteration"""
         hp = self.tr.hp
@@ -126,7 +137,12 @@ class DirectIteration:
             jitter = tr.model_sdf.training if getattr(hp, "jitter_samples", None) is None else bool(hp.jitter_samples)
             fg = tr.occupancy_grid.compute_samples_in_occupied_regions(ray_origins, ray_dirs, t_entry, t_exit, hp.min_dist_between_samples,
                                                                        hp.max_nr_samples_per_ray, jitter).compact_to_valid_samples()
-        return dict(t_exit=t_exit, does_hit=does_hit, fg=fg, jitter=jitter)
+            bg = None
+            if tr.model_bg is not None:       # the same sampler calls, in the same order, as train.create_samples
+                from .permuto_sdf import RaySampler
+                bg = RaySampler.compute_samples_bg(ray_origins, ray_dirs, t_exit, hp.nr_samples_bg, tr.aabb.m_radius, tr.aabb.m_center, jitter,
+                                                   False)
+        return dict(t_exit=t_exit, does_hit=does_hit, fg=fg, jitter=jitter, bg=bg)
 
     def run(self, ray_origins, ray_dirs, gt_rgb, gt_mask, img_indices, it, pre=None):
         """forward + losses + backward; parameter gradients land in the optimizer's .grad views. -> detached 0-d loss tensor.
@@ -208,7 +224,23 @@ class DirectIteration:
                 head = (None, None, None, -1)
             sdf_flat = ws["sdf"].view(-1)
             neus_in = (*fg._rsp(), sdf_flat, ws["grad"], ws["x_raw"], fg.samples_dirs, fg.samples_dt, inv_s, 0.0, cos_dev, gt, mask, hit, *head)
-            call("psdf_neus_head_loss_forward", *neus_in, ws["alpha"], ws["T"], None, ws["pred"], ws["wsum"], ws["bgT"], ws["ray_loss"])
+            bg = pre.get("bg")
+            if bg is not None and bg.samples_pos_4d.shape[0] != 0:
+                # ---------------- background: fused NerfHash, then its compositing with the colour head folded in
+                fb, enc_b = tr.model_bg.fused, tr.model_bg.encoding
+                Nb = bg.samples_pos_4d.shape[0]
+                bws = self._bg_workspace(Nb, R, dev)
+                fb.pack(fb.params())
+                bg_args = (Nb, enc_b.nr_levels, enc_b.capacity, bg.samples_pos_4d, bg.samples_dirs, enc_b.lattice_values.detach(),
+                           enc_b.scale_factor, enc_b.shift_tensor(), fb._window(it), enc_b.concat_points_scaling, fb.blob)
+                call("psdf_bg_fused_forward", *bg_args, bws["x"], bws["density"])
+                comp_in = (*bg._rsp(), bws["x"], bws["density"].view(-1), bg.samples_dt.view(-1).contiguous(), *head)
+                call("psdf_nerf_bg_composite_forward", *comp_in, bws["bg_rgb"])
+                call("psdf_neus_head_bg_loss_forward", *neus_in, bws["bg_rgb"], ws["alpha"], ws["T"], None, ws["pred"], ws["wsum"], ws["bgT"],
+                     ws["ray_loss"])
+            else:
+                bg = None
+                call("psdf_neus_head_loss_forward", *neus_in, ws["alpha"], ws["T"], None, ws["pred"], ws["wsum"], ws["bgT"], ws["ray_loss"])
             # ---------------- curvature pass (models.py:261-294)
             gs = None
             if curv_on:
@@ -230,9 +262,16 @@ class DirectIteration:
             scale_eik = float(hp.eikonal_weight) if n_cnt is not None else float(hp.eikonal_weight) / max(N, 1)
             g_wd = cal.weight_delta.grad if head[1] is not None else None
             g_cb = cal.bias.grad if head[1] is not None else None
-            call("psdf_neus_head_loss_backward", *neus_in, ws["alpha"], ws["T"], ws["pred"], ws["wsum"], ws["bgT"], c_rgb, c_mask, scale_eik, n_cnt,
-                 gs, w_curv, scal[3:4], N, n_valid, ws["g_sdf"].view(-1), ws["g_grad"], ws["g_x"], ws["g_grad_s"] if gs is not None else None,
-                 g_wd, g_cb)
+            head_out = (ws["g_sdf"].view(-1), ws["g_grad"], ws["g_x"], ws["g_grad_s"] if gs is not None else None)
+            if bg is None:
+                call("psdf_neus_head_loss_backward", *neus_in, ws["alpha"], ws["T"], ws["pred"], ws["wsum"], ws["bgT"], c_rgb, c_mask, scale_eik,
+                     n_cnt, gs, w_curv, scal[3:4], N, n_valid, *head_out, g_wd, g_cb)
+            else:
+                call("psdf_neus_head_bg_loss_backward", *neus_in, bws["bg_rgb"], ws["alpha"], ws["T"], ws["pred"], ws["wsum"], ws["bgT"], c_rgb,
+                     c_mask, scale_eik, n_cnt, gs, w_curv, scal[3:4], N, n_valid, *head_out, bws["g_bg_rgb"], g_wd, g_cb)
+                call("psdf_nerf_bg_composite_backward", *comp_in, bws["g_bg_rgb"], bws["g_x"], bws["g_density"], g_wd, g_cb)
+                call("psdf_bg_fused_backward", *bg_args, bws["g_x"], bws["g_density"], enc_b.lattice_values.grad, bws["ws"],
+                     *[l.weight.grad for l in fb.lin], *[l.bias.grad for l in fb.lin])
             gW = ws["gweff"]
             call("psdf_rgb_fused_backward_acc", *rgb_args, ws["g_x"], enc_c.lattice_values.grad, ws["g_grad"], ws["g_geom"], ws["rgb_ws"],
                  gW[0], gW[1], gW[2], gW[3], L[0].bias.grad, L[1].bias.grad, L[2].bias.grad, L[3].bias.grad)

@@ -371,10 +371,23 @@ class NerfHash(torch.nn.Module, _Checkpointed):
         self.c2f = permuto_enc.Coarse2Fine(nr_levels)
         self.nr_iters_for_c2f = nr_iters_for_c2f
         self.last_iter_nr = sys.maxsize
+        self.fused = None
+
+    def enable_fused(self):
+        """route forward / backward through the fused background kernels (csrc/fused_bg.cu)"""
+        from .fused import FusedNerfHash
+        self.fused = FusedNerfHash(self)
+        return self.fused
 
     def forward(self, samples_pos, samples_dirs, iter_nr, model_colorcal=None, img_indices=None, ray_start_end_idx=None):
         assert samples_pos.shape[1] == self.in_channels
         self.last_iter_nr = int(iter_nr)
+        if getattr(self, "fused", None) is not None and samples_pos.is_cuda:
+            rgb, density = self.fused.train_forward(samples_pos, samples_dirs, iter_nr) if torch.is_grad_enabled() else \
+                self.fused(samples_pos, samples_dirs, iter_nr)
+            if model_colorcal is not None:
+                rgb = model_colorcal.calib_RGB_samples_packed(rgb, img_indices, ray_start_end_idx)
+            return torch.sigmoid(rgb), density
         window = self.c2f(map_range_val(iter_nr, 0.0, self.nr_iters_for_c2f, 0.3, 1.0))
         feat = self.encoding(samples_pos, window.view(-1))
         with torch.no_grad():

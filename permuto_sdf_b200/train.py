@@ -339,12 +339,14 @@ class Trainer:
 
     def __init__(self, hyperparams=None, nr_levels=24, capacity=2 ** 18, sdf_hidden=32, nr_images=8, occupancy_resolution=256,
                  seed=0, with_colorcal=True, optimizer="adamw", fused_inference=True, fused_training=True, fused_render=True, direct=None,
-                 deterministic=False):
+                 deterministic=False, fused_background=False):
         """direct: None = run the iteration through the autograd-free sequence of iteration.DirectIteration whenever the configuration
         allows it (fused kernels, flat-buffer optimizer, --with_mask); True = require it (raise otherwise); False = autograd formulation.
         deterministic: switch the library's deterministic mode on for this device (psdf_set_deterministic: order-independent gradient
         reductions, so runs with the same inputs give the same bits; the direct iteration is fully covered) -- or off (the default,
-        float atomics)."""
+        float atomics).
+        fused_background: run the background NerfHash of scenes without masks on the fused tensor-core kernels (csrc/fused_bg.cu)
+        instead of the per-op encoding kernels + autograd; a background shape the kernels do not cover raises."""
         torch.manual_seed(seed)
         self.fused_render = fused_render
         self._fused_inference = fused_inference
@@ -370,6 +372,9 @@ class Trainer:
                 self.model_sdf.enable_fused_training()
                 self.model_rgb.enable_fused()
                 self.execution["sdf_training"] = self.execution["rgb"] = "fused wgmma"
+        if fused_background and self.model_bg is not None:
+            self.model_bg.enable_fused()
+            self.execution["background"] = "fused wgmma"
         groups = [{"params": list(self.model_sdf.parameters()), "weight_decay": 0.0, "lr": hp.lr, "name": "model_sdf"}]
         if self.model_bg is not None:
             groups.append({"params": list(self.model_bg.parameters()), "weight_decay": 0.0, "lr": hp.lr, "name": "model_bg"})
