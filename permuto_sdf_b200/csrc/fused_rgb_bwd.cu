@@ -62,7 +62,9 @@ k_rgb_fused_backward(RgbParams P, const float* __restrict__ pos, const float* __
     float* s_gbf = reinterpret_cast<float*>(s_gb);
     const bool det = sp.fx_mlp != nullptr;
     uint64_t* bars = reinterpret_cast<uint64_t*>(s_gb + kNL * 128);   // [0] weights, [1] reverse MMAs, [2] dW MMAs, [3] a_0 reload
-    float* s_x = reinterpret_cast<float*>(s_a);            // exchange tile abar_0: [128][K0 + 1] fp32, aliases s_a
+    // exchange tile abar_0: [128][K0 + 1] fp32 over s_a and, for K0 = 128 (L >= 28), the start of s_z; written after the last reverse
+    // step's MMAs, the only readers of both, have completed
+    float* s_x = reinterpret_cast<float*>(s_a);
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int row = tid & 127, grp = tid >> 7;
@@ -322,7 +324,7 @@ static int rgb_backward_impl(int N, int L, int T, const float* pos, const float*
     if (rc != PSDF_OK) return rc;
     P.acc_sdf_grad = accumulate_sdf_grad ? 1 : 0;
     if (N == 0) return PSDF_OK;
-    if ((size_t)128 * (P.g.Kp[0] + 1) * 4 > (size_t)2 * kWTileBytes) return PSDF_ERR_UNSUPPORTED;
+    static_assert((size_t)kTile * (128 + 1) * 4 <= (size_t)4 * kWTileBytes, "the exchange tile of K0 = 128 fits in s_a | s_z");
     const DetBufs* dbuf = det_buffers();
     if (dbuf && (long long)L * T * 2 > dbuf->lattice_len) return PSDF_ERR_UNSUPPORTED;   // reserve more with psdf_set_deterministic
     RgbSpill sp;
