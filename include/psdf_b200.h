@@ -407,6 +407,13 @@ int psdf_loss_terms(int N, const int* nr_valid_dev, const int* nr_mean_dev, cons
                     const float* ray_loss, int n_off, const float* sdf_off, float* g_off, float c_rgb, float c_mask, float w_eik, float w_curv,
                     const float* w_curv_dev, float w_off, float w_lip, const float* lip_c0, const float* lip_c1, const float* lip_c2,
                     const float* lip_c3, float* acc, float* loss, float* terms, void* stream);
+/* loss of one sphere-fit iteration (train_permuto_sdf.py:323-331, sdf_loss_sphere in permuto_sdf_utils.py:53-77) in one launch:
+ *   loss = w_sdf mean((sdf - (|pos - center| - radius) s)^2) + w_eik mean((|grad| - s)^2),  s = distance_scale
+ * pos [N,3], sdf [N], grad [N,3] (d sdf / d pos) -> g_sdf [N] = d loss / d sdf, g_grad [N,3] = d loss / d grad (=; zero where
+ * |grad| = 0, as torch's norm backward), loss [1], terms [2] = {mean sdf term, mean eikonal term}. center[3] is a HOST array.
+ * acc [4] scratch: zero before the first call, left zero by every call. Deterministic mode: fixed-point sums. */
+int psdf_sphere_fit_loss(int N, const float* pos, const float* sdf, const float* grad, float radius, const float center[3], float distance_scale,
+                         float w_sdf, float w_eik, float* g_sdf, float* g_grad, float* acc, float* loss, float* terms, void* stream);
 /* Sphere.rand_points_inside (src/Sphere.cu) from ONE uniform draw u01 [3,n]: rows = phi / (2 pi), (cos(theta) + 1) / 2, u */
 int psdf_sphere_rand_points_inside_u01(int n, float radius, const float* u01, float* out, void* stream);
 /* psdf_adamw_step over up to 8 parameter groups in one launch: device-resident step count, per-group hyper_dev [2] = {lr, weight_decay};

@@ -310,7 +310,7 @@ struct DetBufs {
     unsigned long long* rgb_mlp;       // [4 x kDetRgbW weights | 4 x 128 biases]
     unsigned long long* neus;          // [3 kDetImages weight delta | 3 kDetImages bias | inv_s]
     unsigned long long* lip;           // [4]
-    unsigned long long* loss;          // [5]
+    unsigned long long* loss;          // [8]: [0, 5) psdf_loss_terms, [5, 7) psdf_sphere_fit_loss
     int* winner;                       // [voxels]: occupancy-update arbitration (rayops.cu)
     long long lattice_len, voxels;
 };

@@ -6,6 +6,8 @@
 //   k_lipschitz_bwd4    its backward for the four layers, accumulated into the persistent .grad buffers (+ the Lipschitz-bound loss) 1 for 4 + 8
 //   k_loss_terms        curvature values (models.py:283-294), all loss reductions (rgb L1, mask BCE, eikonal, curvature, off-surface
 //                       exp(-100 |sdf|), Lipschitz bound), the weighted total and the off-surface gradient seed                      1 for ~30
+//   k_sphere_fit_loss   sdf_loss_sphere of the sphere-fit phase (train_permuto_sdf.py:323-331): both reductions, the weighted total and
+//                       the seeds d loss / d {sdf, grad}                                                                             1 for ~15
 //   k_rand_points_u01   Sphere.rand_points_inside from one uniform draw [3,n]                                                          1 for 3
 //   k_adamw_multi       AdamW over several parameter groups in one launch (optim.cu k_adamw per group otherwise)
 #include <cstdlib>
@@ -236,6 +238,82 @@ k_loss_terms(LossArgs A) {
     for (int q = 0; q < 8; q++) A.acc[q] = 0.0f;      // ticket (acc[7], as bits) included: ready for the next launch
 }
 
+// ---------------------------------------------------------------------------------------------- sphere-fit loss
+struct SphereFitArgs {
+    unsigned long long* fx;          // deterministic mode: DetBufs::loss + 5 (the two sums in fixed point), else NULL
+    int N;
+    const float* pos;                // [N,3]
+    const float* sdf;                // [N]
+    const float* g;                  // [N,3] d sdf/dx
+    float radius, cx, cy, cz, scale, w_sdf, w_eik;
+    float* g_sdf;                    // [N]   d loss / d sdf (=)
+    float* g_grad;                   // [N,3] d loss / d (d sdf/dx) (=)
+    float* acc;                      // [4] accumulators + ticket (zero on entry, left zero)
+    float* loss;                     // [1]
+    float* terms;                    // [2]: loss_sdf, loss_eik
+};
+// sdf_loss_sphere (train.py, permuto_sdf_utils.py:53-77): w_sdf mean((sdf - (|p - c| - r) s)^2) + w_eik mean((|g| - s)^2), with the
+// seeds of both terms written per row. |g| = 0 gives a zero eikonal seed (torch's norm backward at 0).
+__global__ void __launch_bounds__(kThreads)
+k_sphere_fit_loss(SphereFitArgs A) {
+    __shared__ float red[2][kThreads / 32];
+    __shared__ bool last;
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    float v[2] = {0.f, 0.f};
+    if (i < A.N) {
+        const float inv_n = 1.0f / (float)A.N;
+        const float px = A.pos[3 * i] - A.cx, py = A.pos[3 * i + 1] - A.cy, pz = A.pos[3 * i + 2] - A.cz;
+        const float d = (sqrtf(px * px + py * py + pz * pz) - A.radius) * A.scale;
+        const float e = A.sdf[i] - d;
+        v[0] = e * e;
+        A.g_sdf[i] = 2.0f * A.w_sdf * e * inv_n;
+        const float gx = A.g[3 * i], gy = A.g[3 * i + 1], gz = A.g[3 * i + 2];
+        const float n = sqrtf(gx * gx + gy * gy + gz * gz);
+        const float r = n - A.scale;
+        v[1] = r * r;
+        const float k = n > 0.0f ? 2.0f * A.w_eik * r / n * inv_n : 0.0f;
+        A.g_grad[3 * i] = k * gx; A.g_grad[3 * i + 1] = k * gy; A.g_grad[3 * i + 2] = k * gz;
+    }
+#pragma unroll
+    for (int q = 0; q < 2; q++) {
+        const float s = warp_sum(v[q]);
+        if (lane == 0) red[q][warp] = s;
+    }
+    __syncthreads();
+    if (threadIdx.x < 2) {
+        float s = 0.f;
+        for (int w = 0; w < kThreads / 32; w++) s += red[threadIdx.x][w];
+        if (s != 0.0f) {
+            if (A.fx) fx_add(A.fx + threadIdx.x, s);
+            else atomicAdd(A.acc + threadIdx.x, s);
+        }
+    }
+    __threadfence();
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        const unsigned t = atomicAdd(reinterpret_cast<unsigned*>(A.acc + 3), 1u);
+        last = (t == gridDim.x - 1);
+    }
+    __syncthreads();
+    if (!last || threadIdx.x != 0) return;
+    __threadfence();
+    float sums[2];
+    if (A.fx) {
+        volatile unsigned long long* fx = A.fx;
+        for (int q = 0; q < 2; q++) { sums[q] = (float)((double)(long long)fx[q] / kFxScale); fx[q] = 0ull; }
+    } else {
+        volatile float* acc = A.acc;
+        for (int q = 0; q < 2; q++) sums[q] = acc[q];
+    }
+    const float l_sdf = sums[0] / (float)A.N, l_eik = sums[1] / (float)A.N;
+    A.loss[0] = l_sdf * A.w_sdf + l_eik * A.w_eik;
+    A.terms[0] = l_sdf;
+    A.terms[1] = l_eik;
+#pragma unroll
+    for (int q = 0; q < 4; q++) A.acc[q] = 0.0f;      // ticket (acc[3], as bits) included: ready for the next launch
+}
+
 // ---------------------------------------------------------------------------------------------- random points in a sphere
 // src/Sphere.cu rand_points_inside: phi in [0, 2 pi), cos(theta) in [-1, 1), u in [0, 1) -> r = R u^(1/3) along the sphere direction
 __global__ void k_rand_points_u01(int n, float radius, const float* __restrict__ u01 /* [3,n] */, float* __restrict__ out) {
@@ -396,6 +474,22 @@ int psdf_loss_terms(int N, const int* nr_valid_dev, const int* nr_mean_dev, cons
     A.acc = acc; A.loss = loss; A.terms = terms;
     const int work = max(max(grad_shifted ? N : 0, R), max(A.n_off, 1));
     k_loss_terms<<<div_up(work, kThreads), kThreads, 0, ST>>>(A);
+    PSDF_CHECK_LAUNCH();
+    return PSDF_OK;
+}
+
+// Loss of one sphere-fit iteration (train_permuto_sdf.py:323-331) in one launch, see k_sphere_fit_loss. acc [4]: scratch, ZERO before the
+// first call, left zero by every call. terms [2] = {loss_sdf, loss_eik} (unweighted means).
+int psdf_sphere_fit_loss(int N, const float* pos, const float* sdf, const float* grad, float radius, const float center[3], float distance_scale,
+                         float w_sdf, float w_eik, float* g_sdf, float* g_grad, float* acc, float* loss, float* terms, void* stream) {
+    if (N < 1 || !pos || !sdf || !grad || !center || !g_sdf || !g_grad || !acc || !loss || !terms) return PSDF_ERR_ARG;
+    SphereFitArgs A;
+    const DetBufs* dbuf = det_buffers();
+    A.fx = dbuf ? dbuf->loss + 5 : nullptr;
+    A.N = N; A.pos = pos; A.sdf = sdf; A.g = grad;
+    A.radius = radius; A.cx = center[0]; A.cy = center[1]; A.cz = center[2]; A.scale = distance_scale; A.w_sdf = w_sdf; A.w_eik = w_eik;
+    A.g_sdf = g_sdf; A.g_grad = g_grad; A.acc = acc; A.loss = loss; A.terms = terms;
+    k_sphere_fit_loss<<<div_up(N, kThreads), kThreads, 0, ST>>>(A);
     PSDF_CHECK_LAUNCH();
     return PSDF_OK;
 }

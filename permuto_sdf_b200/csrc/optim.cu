@@ -173,11 +173,11 @@ int psdf_set_deterministic(int on, long long lattice_entries, long long voxels) 
     bool ok = cudaMalloc(&d.sdf_lattice, lat * sizeof(U)) == cudaSuccess && cudaMalloc(&d.rgb_lattice, lat * sizeof(U)) == cudaSuccess &&
               cudaMalloc(&d.sdf_mlp, n_sdf * sizeof(U)) == cudaSuccess && cudaMalloc(&d.rgb_mlp, n_rgb * sizeof(U)) == cudaSuccess &&
               cudaMalloc(&d.neus, n_neus * sizeof(U)) == cudaSuccess && cudaMalloc(&d.lip, 4 * sizeof(U)) == cudaSuccess &&
-              cudaMalloc(&d.loss, 5 * sizeof(U)) == cudaSuccess && cudaMalloc(&d.winner, vox * sizeof(int)) == cudaSuccess;
+              cudaMalloc(&d.loss, 8 * sizeof(U)) == cudaSuccess && cudaMalloc(&d.winner, vox * sizeof(int)) == cudaSuccess;
     ok = ok && cudaMemset(d.sdf_lattice, 0, lat * sizeof(U)) == cudaSuccess && cudaMemset(d.rgb_lattice, 0, lat * sizeof(U)) == cudaSuccess &&
          cudaMemset(d.sdf_mlp, 0, n_sdf * sizeof(U)) == cudaSuccess && cudaMemset(d.rgb_mlp, 0, n_rgb * sizeof(U)) == cudaSuccess &&
          cudaMemset(d.neus, 0, n_neus * sizeof(U)) == cudaSuccess && cudaMemset(d.lip, 0, 4 * sizeof(U)) == cudaSuccess &&
-         cudaMemset(d.loss, 0, 5 * sizeof(U)) == cudaSuccess && cudaMemset(d.winner, 0, vox * sizeof(int)) == cudaSuccess &&
+         cudaMemset(d.loss, 0, 8 * sizeof(U)) == cudaSuccess && cudaMemset(d.winner, 0, vox * sizeof(int)) == cudaSuccess &&
          cudaDeviceSynchronize() == cudaSuccess;
     if (!ok) { cudaGetLastError(); return PSDF_ERR_LAUNCH; }
     d.lattice_len = lattice_entries; d.voxels = voxels;

@@ -22,7 +22,19 @@ CUDA graph. Here the same mathematics is issued directly:
 
 Parameter gradients are accumulated straight into the flat-buffer optimizer's `.grad` views (which the AdamW kernel leaves zeroed).
 Every formula is the one of the autograd path; `tests/test_direct_iteration_gpu.py` compares loss and all parameter gradients of the
-two formulations."""
+two formulations.
+
+`DirectIteration.sphere_fit` is the same for an iteration of the sphere-fit phase that precedes training (train_permuto_sdf.py:323-331:
+SDF only, no colour, no compositing):
+
+    torch.rand + psdf_sphere_rand_points_inside_u01      30 000 points inside the bounding sphere                   2 launches
+    psdf_sdf_fused_forward              sdf and d sdf/dx at the points (no geometric feature)                         1
+    psdf_sphere_fit_loss                both loss terms, the weighted total and the seeds d loss / d {sdf, d sdf/dx}  1
+    psdf_sdf_fused_backward_multi       one sample set, into the SDF .grad views                                      2 kernels
+
+Trainer.fit_sphere adds AdamW over the SDF group (psdf_adamw_multi_step) and the re-pack that advances the counters
+(psdf_sdf_mlp_pack_advance): 8 launches per fit iteration, plus the ~13 element-wise torch ops of the coarse-to-fine window, which ramps
+over the whole phase (22 GPU operations per iteration in a torch.profiler trace, tools/bench_sphere_fit.py)."""
 import ctypes
 
 import torch
@@ -124,6 +136,44 @@ class DirectIteration:
         it_dev = it.dev if isinstance(it, DeviceIter) else None
         call("psdf_iter_scalars", 4, ctypes.addressof(P), ctypes.addressof(K), it_dev, float(int(it)), ws["scal"])
         return ws["scal"]
+
+    # ------------------------------------------------------------------------------------------ sphere fit
+    def sphere_fit(self, it, nr_points, radius, center, distance_scale=1.0):
+        """forward + loss + backward of sphere-fit iteration `it` (also the anneal iteration of the SDF window); the SDF parameter
+        gradients land in the optimizer's .grad views. Buffers are sized by nr_points only, so the sequence replays from one graph.
+        -> detached 0-d loss tensor; tr.last['sphere_fit_terms'] = {loss_sdf, loss_eik}"""
+        tr = self.tr
+        m_sdf, fs, enc = tr.model_sdf, tr.model_sdf.fused, tr.model_sdf.encoding
+        dev = enc.lattice_values.device
+        n = int(nr_points)
+        fw = getattr(self, "_fit_ws", None)
+        if fw is None or fw["key"] != (n, str(dev)):
+            from ._lib import load_library
+            f = lambda *s: torch.empty(*s, device=dev)
+            fw = self._fit_ws = dict(key=(n, str(dev)), pts=f(n, 3), sdf=f(n), grad=f(n, 3), g_sdf=f(n), g_grad=f(n, 3),
+                                     acc=torch.zeros(4, device=dev), loss=torch.zeros(1, device=dev), terms=torch.zeros(2, device=dev),
+                                     ws=torch.empty(int(load_library().psdf_sdf_fused_backward_multi_workspace_bytes(n, 0, 0)),
+                                                    dtype=torch.uint8, device=dev))
+        with torch.no_grad():
+            u01 = tr.draw("sphere_fit_u01", lambda: torch.rand(3, n, device=dev))
+            call("psdf_sphere_rand_points_inside_u01", n, tr.aabb.m_radius, u01, fw["pts"])
+            if fs._versions != fs._cur_versions():
+                fs.repack()
+            m_sdf.last_iter_nr = int(it)
+            win = m_sdf.window(it).view(-1).contiguous()
+            sdf_args = (enc.nr_levels, enc.capacity, enc.lattice_values.detach(), enc.scale_factor, enc.shift_tensor(), win,
+                        enc.concat_points_scaling, fs.hidden, fs.out_dim, fs.blob)
+            call("psdf_sdf_fused_forward", n, enc.nr_levels, enc.capacity, fw["pts"], enc.lattice_values.detach(), enc.scale_factor,
+                 enc.shift_tensor(), win, enc.concat_points_scaling, fs.hidden, fs.out_dim, fs.blob, fw["sdf"], fw["grad"], None)
+            call("psdf_sphere_fit_loss", n, fw["pts"], fw["sdf"], fw["grad"], radius, center, distance_scale, 3e3, 5e1, fw["g_sdf"],
+                 fw["g_grad"], fw["acc"], fw["loss"], fw["terms"])
+            lin = fs.lin
+            call("psdf_sdf_fused_backward_multi", *sdf_args, n, fw["pts"], fw["g_sdf"], fw["g_grad"], None, 0, None, None, None, None,
+                 0, None, None, None, None, enc.lattice_values.grad, fw["ws"],
+                 lin[0].weight.grad, lin[1].weight.grad, lin[2].weight.grad, lin[3].weight.grad,
+                 lin[0].bias.grad, lin[1].bias.grad, lin[2].bias.grad, lin[3].bias.grad)
+        tr.last = dict(sphere_fit_terms=fw["terms"])
+        return fw["loss"].view(())
 
     # ------------------------------------------------------------------------------------------ the iteration
     def sample_uniform(self, ray_origins, ray_dirs):

@@ -156,17 +156,31 @@ class FusedAdamW:
             self.hyper_dev.copy_(self._hyper_host, non_blocking=True)
             self._hyper_cached = cur
 
-    def _multi_tables(self):
-        """host tables of device addresses for psdf_adamw_multi_step (all groups in one launch)"""
+    def _multi_tables(self, groups=None):
+        """host tables of device addresses for psdf_adamw_multi_step (the chosen groups, default all, in one launch)"""
         import ctypes
-        gs = [g for g in self.param_groups if g["_n"] > 0]
+        idx = [i for i, g in enumerate(self.param_groups) if g["_n"] > 0 and (groups is None or i in groups)]
+        gs = [self.param_groups[i] for i in idx]
         k = len(gs)
         n = (ctypes.c_longlong * k)(*[g["_n"] for g in gs])
         tab = lambda base: (ctypes.c_uint64 * k)(*[base.data_ptr() + 4 * g["_off"] for g in gs])
-        idx = [self.param_groups.index(g) for g in gs]
         hyper = (ctypes.c_uint64 * k)(*[self.hyper_dev.data_ptr() + 8 * i for i in idx])
-        key = (self.flat_param.data_ptr(), self.flat_grad.data_ptr(), self.hyper_dev.data_ptr())
+        key = (self.flat_param.data_ptr(), self.flat_grad.data_ptr(), self.hyper_dev.data_ptr(), None if groups is None else tuple(groups))
         return dict(key=key, k=k, n=n, p=tab(self.flat_param), g=tab(self.flat_grad), m=tab(self.exp_avg), v=tab(self.exp_avg_sq), h=hyper)
+
+    def step_groups_deferred(self, groups, step_dev, grad_scale=1.0):
+        """ONE psdf_adamw_multi_step launch over the param groups `groups` (indices) with step = step_dev + 1, reading lr / weight decay
+        from hyper_dev (sync_hyper() first); the swept gradients are left zero. Neither step_dev nor step_count is advanced here: the
+        caller's psdf_sdf_mlp_pack_advance advances step_dev, the caller the host count. Capturable (no host sync, no allocation)."""
+        import ctypes
+        mt = getattr(self, "_multi_sel", None)
+        key = (self.flat_param.data_ptr(), self.flat_grad.data_ptr(), self.hyper_dev.data_ptr(), tuple(groups))
+        if mt is None or mt["key"] != key:
+            mt = self._multi_sel = self._multi_tables(groups)
+        b1, b2 = self.betas
+        call("psdf_adamw_multi_step", mt["k"], ctypes.addressof(mt["n"]), ctypes.addressof(mt["p"]), ctypes.addressof(mt["g"]),
+             ctypes.addressof(mt["m"]), ctypes.addressof(mt["v"]), ctypes.addressof(mt["h"]), b1, b2, self.eps, step_dev, 1,
+             float(grad_scale), 0)
 
     @torch.no_grad()
     def step(self, grad_scale=1.0, groups=None, advance=True, defer_counter=False, leave_room=False):
@@ -187,7 +201,7 @@ class FusedAdamW:
             if self.hyper_dev is None:
                 self.sync_hyper()
             mt = getattr(self, "_multi", None)
-            if mt is None or mt["key"] != (self.flat_param.data_ptr(), self.flat_grad.data_ptr(), self.hyper_dev.data_ptr()):
+            if mt is None or mt["key"] != (self.flat_param.data_ptr(), self.flat_grad.data_ptr(), self.hyper_dev.data_ptr(), None):
                 mt = self._multi = self._multi_tables()
             call("psdf_adamw_multi_step", mt["k"], ctypes.addressof(mt["n"]), ctypes.addressof(mt["p"]), ctypes.addressof(mt["g"]),
                  ctypes.addressof(mt["m"]), ctypes.addressof(mt["v"]), ctypes.addressof(mt["h"]), b1, b2, self.eps, self.step_dev, 1,

@@ -203,10 +203,11 @@ def sdf_loss_sphere(points, sdf, sdf_gradients, sphere_radius, sphere_center, di
     return loss_sdf * 3e3 + loss_eik * 5e1, loss_sdf, loss_eik
 
 
-def loss_sphere_init(nr_points, aabb, model, iter_nr_for_anneal):
-    pts = aabb.rand_points_inside(nr_points=nr_points)
+def loss_sphere_init(nr_points, aabb, model, iter_nr_for_anneal, points=None, sphere_radius=0.3, sphere_center=(0, 0, 0)):
+    """points: [nr_points, 3] to evaluate instead of a fresh aabb.rand_points_inside draw"""
+    pts = aabb.rand_points_inside(nr_points=nr_points) if points is None else points
     sdf, grads, _ = model.get_sdf_and_gradient(pts, iter_nr_for_anneal)
-    return sdf_loss_sphere(pts, sdf, grads, sphere_radius=0.3, sphere_center=[0, 0, 0])
+    return sdf_loss_sphere(pts, sdf, grads, sphere_radius=sphere_radius, sphere_center=list(sphere_center))
 
 
 def sphere_trace(nr_sphere_traces, ray_origins, ray_dirs, model, return_gradients, sdf_multiplier, sdf_converged_tresh,
@@ -334,8 +335,11 @@ class HostLoss:
 
 
 class Trainer:
-    """State of one PermutoSDF training run on synthetic data (models, occupancy grid, optimizer) and the
-    per-iteration step of train_permuto_sdf.py:311-422 (after sphere init), with `--with_mask` semantics."""
+    """State of one PermutoSDF training run on synthetic data (models, occupancy grid, optimizer) and its two phases:
+      * the sphere-fit phase (train_permuto_sdf.py:323-331), `fit_sphere()`: hp.nr_iter_sphere_fit iterations that fit the SDF to a
+        sphere of radius 0.3 before training; counted by `sphere_fit_iter`;
+      * the per-iteration training step of train_permuto_sdf.py:311-422 after the fit, `step()`, with `--with_mask` semantics; counted
+        by `iter_nr`, which the fit leaves at 0."""
 
     def __init__(self, hyperparams=None, nr_levels=24, capacity=2 ** 18, sdf_hidden=32, nr_images=8, occupancy_resolution=256,
                  seed=0, with_colorcal=True, optimizer="adamw", fused_inference=True, fused_training=True, fused_render=True, direct=None,
@@ -402,7 +406,11 @@ class Trainer:
         elif direct:
             raise RuntimeError("Trainer(direct=True): " + why)
         self.execution["iteration"] = "direct kernel sequence (iteration.py)" if self._direct is not None else "torch.autograd (%s)" % why
+        self._direct_why = why
+        self.execution["sphere_fit"] = None      # set by fit_sphere()
         self.iter_nr = 0
+        self.sphere_fit_iter = 0        # sphere-fit iterations run so far (fit_sphere)
+        self._fit = None                # device counters and captured graph of the direct sphere fit
         self._cg = None                 # CUDA-graph state (enable_cuda_graph)
         self._dp = None                 # data-parallel state (enable_data_parallel)
         self.nr_rays_to_create = hp.nr_rays
@@ -423,9 +431,21 @@ class Trainer:
             torch.save(self.occupancy_grid.get_grid_values(), os.path.join(path, "grid_values.pt"))
             torch.save(self.occupancy_grid.get_grid_occupancy(), os.path.join(path, "grid_occupancy.pt"))
         if with_optimizer:
-            torch.save({"optimizer": self.optimizer.state_dict(), "iter_nr": self.iter_nr,
-                        "nr_rays_to_create": self.nr_rays_to_create}, os.path.join(path, "trainer_state.pt"))
+            torch.save(self._trainer_state(), os.path.join(path, "trainer_state.pt"))
         return path
+
+    def _trainer_state(self):
+        return {"optimizer": self.optimizer.state_dict(), "iter_nr": self.iter_nr, "nr_rays_to_create": self.nr_rays_to_create,
+                "sphere_fit_iter": self.sphere_fit_iter}
+
+    def _restore_trainer_state(self, sd):
+        """inverse of _trainer_state(); sd None: no trainer_state.pt (a reference checkpoint). A state without `sphere_fit_iter` (older
+        files, reference checkpoints) comes from a run past its sphere fit: the fit counts as finished."""
+        if sd is not None:
+            self.optimizer.load_state_dict(sd["optimizer"])
+            self.iter_nr = int(sd["iter_nr"])
+            self.nr_rays_to_create = int(sd.get("nr_rays_to_create", self.nr_rays_to_create))
+        self.sphere_fit_iter = int(sd["sphere_fit_iter"]) if (sd is not None and "sphere_fit_iter" in sd) else int(self.hp.nr_iter_sphere_fit)
 
     def load(self, ckpt_path_full, with_optimizer=True):
         """inverse of save(); also reads checkpoints written by the reference (no trainer_state.pt: models + grid only).
@@ -434,10 +454,9 @@ class Trainer:
         load_from_checkpoint(ckpt_path_full, self.model_sdf, self.model_rgb, self.model_bg, self.occupancy_grid, self.model_colorcal)
         st = os.path.join(ckpt_path_full, "trainer_state.pt")
         if with_optimizer and os.path.exists(st):
-            sd = torch.load(st, map_location=next(self.model_sdf.parameters()).device)
-            self.optimizer.load_state_dict(sd["optimizer"])
-            self.iter_nr = int(sd["iter_nr"])
-            self.nr_rays_to_create = int(sd.get("nr_rays_to_create", self.nr_rays_to_create))
+            self._restore_trainer_state(torch.load(st, map_location=next(self.model_sdf.parameters()).device))
+        else:
+            self._restore_trainer_state(None)
         if getattr(self.model_sdf, "fused", None) is not None:
             self.model_sdf.fused.repack()           # load_state_dict copies in place
         if self._cg is not None:
@@ -665,6 +684,107 @@ class Trainer:
         self.iter_nr += 1
         return loss
 
+    # ------------------------------------------------------------------------------------ sphere-fit phase
+    def fit_sphere(self, nr_iters=None, nr_points=30000, radius=0.3, center=(0, 0, 0)):
+        """The sphere-fit phase that precedes training (train_permuto_sdf.py:323-331): per iteration `nr_points` uniform points inside
+        the bounding sphere, loss sdf_loss_sphere (3e3 mean (sdf - (|p - c| - r))^2 + 5e1 mean (|d sdf/dx| - 1)^2) and AdamW at the
+        constant hp.lr over the SDF parameters only. The other groups' parameters and Adam moments do not change; FusedAdamW's single
+        step count advances (apex FusedAdam advances every group's step, the reference's optimizer when apex is installed), torch AdamW
+        creates no state for them. The fit iteration is the anneal iteration of the SDF coarse-to-fine window.
+        Runs the rest of the phase, at most `nr_iters` iterations: min(nr_iters, hp.nr_iter_sphere_fit - sphere_fit_iter); iter_nr
+        does not change. Whenever the trainer runs the direct iteration the fit is the direct kernel sequence (DirectIteration.sphere_fit),
+        replayed from one captured graph after enable_cuda_graph(); otherwise loss_sphere_init + loss.backward().
+        -> detached 0-d loss of the last iteration (no host sync), None when no iteration ran."""
+        if self._dp is not None:
+            raise RuntimeError("fit_sphere: the sphere fit runs on one GPU (the reference has no data-parallel fit); fit before "
+                               "enable_data_parallel()")
+        hp = self.hp
+        left = max(int(hp.nr_iter_sphere_fit) - self.sphere_fit_iter, 0)
+        n = left if nr_iters is None else min(max(int(nr_iters), 0), left)
+        self.model_sdf.train()
+        opt = self.optimizer
+        for g in opt.param_groups:
+            g["lr"] = hp.lr               # constant during the fit: the reference creates its LR scheduler when the fit ends
+        gi = [i for i, g in enumerate(opt.param_groups) if g.get("name") == "model_sdf"]
+        args = (int(nr_points), float(radius), [float(c) for c in center])
+        loss = None
+        if self._direct is None:
+            self.execution["sphere_fit"] = "torch.autograd (%s)" % self._direct_why
+            for _ in range(n):
+                loss = self._fit_sphere_autograd(gi, *args)
+            return loss
+        self.execution["sphere_fit"] = "direct kernel sequence (iteration.py)" + (", CUDA-graph replay" if self._cg is not None else "")
+        dev = opt.flat_param.device
+        fit = self._fit
+        if fit is None:
+            fit = self._fit = dict(it_dev=torch.zeros((), device=dev), step_dev=torch.zeros(1, dtype=torch.int32, device=dev), graph=None,
+                                   warm=None)
+        # device-resident fit iteration and AdamW step count: the same sequence runs eagerly and from the captured graph
+        fit["it_dev"].fill_(float(self.sphere_fit_iter))
+        step_dev = opt.step_dev if opt.device_step else fit["step_dev"]
+        if not opt.device_step:
+            step_dev.fill_(opt.step_count)
+        opt.sync_hyper()
+        opt.zero_grad(set_to_none=False)          # every gradient starts clean; the AdamW sweep re-zeroes the SDF group's
+        u01 = (self.fixed_random or {}).get("sphere_fit_u01")
+        key = args[:2] + (tuple(args[2]), None if u01 is None else u01.data_ptr(), step_dev.data_ptr())
+
+        def one(dit):
+            out = self._direct.sphere_fit(dit, *args)
+            opt.step_groups_deferred(gi, step_dev)
+            self.model_sdf.fused.repack(advance=(step_dev, fit["it_dev"]))
+            return out
+
+        for _ in range(n):
+            dit = DeviceIter(self.sphere_fit_iter, fit["it_dev"])
+            g = fit["graph"]
+            if self._cg is None:
+                loss = one(dit)
+            elif g is not None and g["key"] == key and g["lo"] <= self.sphere_fit_iter < g["hi"]:
+                g["graph"].replay()
+                loss = g["loss"]
+            elif fit["warm"] != key:
+                # first iteration of this shape: eager, on the capture stream (workspace and lazy library state are created there)
+                side, cur = self._cg["stream"], torch.cuda.current_stream()
+                side.wait_stream(cur)
+                with torch.cuda.stream(side):
+                    loss = one(dit)
+                cur.wait_stream(side)
+                fit["warm"] = key
+            else:
+                torch.cuda.synchronize()
+                graph = torch.cuda.CUDAGraph()
+                with torch.cuda.graph(graph, stream=self._cg["stream"]):
+                    loss = one(dit)
+                fit["graph"] = dict(graph=graph, key=key, lo=dit.lo, hi=dit.hi, loss=loss, last=self.last)
+                graph.replay()                    # the capture recorded the iteration, it did not run it
+            opt.step_count += 1
+            self.sphere_fit_iter += 1
+        if fit["graph"] is not None and self._cg is not None:
+            self.last = fit["graph"]["last"]
+        opt._clean = True
+        return loss
+
+    def _fit_sphere_autograd(self, gi, nr_points, radius, center):
+        """one sphere-fit iteration in the autograd formulation: loss_sphere_init, loss.backward(), AdamW over the SDF group"""
+        opt = self.optimizer
+        fused_opt = hasattr(opt, "flat_grad")
+        dev = next(self.model_sdf.parameters()).device
+        u01 = self.draw("sphere_fit_u01", lambda: torch.rand(3, nr_points, device=dev))
+        opt.zero_grad(set_to_none=not fused_opt)        # torch AdamW: parameters without a gradient keep no optimizer state
+        loss, l_sdf, l_eik = loss_sphere_init(nr_points, self.aabb, self.model_sdf, self.sphere_fit_iter,
+                                              points=self.aabb.rand_points_inside_u01(u01), sphere_radius=radius, sphere_center=center)
+        loss.backward()
+        if fused_opt:
+            opt.step(groups=gi)
+            if getattr(self.model_sdf, "fused", None) is not None:
+                self.model_sdf.fused.repack()          # raw-pointer updates do not bump tensor versions
+        else:
+            opt.step()
+        self.sphere_fit_iter += 1
+        self.last = dict(sphere_fit_terms=torch.stack([l_sdf.detach(), l_eik.detach()]))
+        return loss.detach()
+
     # ------------------------------------------------------------------------------------ CUDA-graph replay
     def enable_cuda_graph(self, warmup_steps=3):
         """Run the iteration from CUDA graphs: sync-free static-capacity containers, device-resident pcg32 generators,
@@ -698,6 +818,8 @@ class Trainer:
         self.optimizer.device_step = False
         self.optimizer.step_dev = None
         self._cg = None
+        if self._fit is not None:
+            self._fit["graph"], self._fit["warm"] = None, None      # the captured fit reads the step count just dropped
 
     def _sync_device_iter(self):
         cg = self._cg
