@@ -385,6 +385,19 @@ int psdf_neus_head_bg_loss_backward(PSDF_RSP, const float* sdf, const float* gra
                                     const int* nr_samples_dev, const float* grad_shifted, float curv_scale, const float* curv_scale_dev, int n_rows,
                                     const int* nr_valid_dev, float* g_sdf, float* g_grad, float* g_x, float* g_grad_shifted, float* g_bg_rgb,
                                     float* g_weight_delta, float* g_bias, void* stream);
+/* Forward-only NeuS compositing of a rendered frame: VolumeRenderingNeus.compute_weights + integrate of the colour and of the SDF gradient
+ * (permuto_sdf_py/volume_rendering/volume_rendering_modules.py:129-176) and the background blend of run_net
+ * (permuto_sdf_py/train_permuto_sdf.py:133-162), with the colour head (calibration + sigmoid) folded in. It is the render mode of the kernel
+ * behind psdf_neus_head_loss_forward: the same alpha / transmittance chain and colour head, no loss terms, nothing stored per sample.
+ * sdf [N], grad [N,3] (d sdf / dx), x_raw [N,3] (colour network's linear output), dirs [N,3], dt [N], inv_s_dev [1] (device, clipped to
+ * [1e-6,1e6] inside); img_idx [R] / weight_delta / bias [nr_imgs,3] may be NULL (no calibration); bg_rgb [R,3] or NULL. Per ray:
+ *   pred_rgb [R,3] = sum w sigmoid(head(x_raw)) + T_last bg_rgb, pred_rgb_bg [R,3] = T_last bg_rgb (only with bg_rgb, else not written),
+ *   pred_normals [R,3] = F.normalize(sum w grad) (eps 1e-12), weights_sum [R,1] = sum w.
+ * Skipped rays (no sample, or end > max_nr_samples): pred_rgb = the background term, normal 0, weights_sum 0. */
+int psdf_neus_render_forward(PSDF_RSP, const float* sdf, const float* grad, const float* x_raw, const float* dirs, const float* dt,
+                             const float* inv_s_dev, float cos_anneal_ratio, const int* img_idx, const float* weight_delta, const float* bias,
+                             int fixed_img, const float* bg_rgb, float* pred_rgb, float* pred_rgb_bg, float* pred_normals, float* weights_sum,
+                             void* stream);
 /* schedule ramps from the device-resident iteration (map_range_val, permuto_sdf_py/utils/common_utils.py:156-160): out[i] = out0 +
  * (out1 - out0) / (in1 - in0) * (clamp(it, in0, in1) - in0); kinds[i] = 1 / 2: exp(10 * ramp) unclipped / clipped to [1e-6, 1e6]
  * (inv_s of SingleVarianceNetwork with a forced variance). params [n,4] = {in0, in1, out0, out1} and kinds [n] are HOST arrays, n <= 8;

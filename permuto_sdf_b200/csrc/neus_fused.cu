@@ -75,13 +75,18 @@ __device__ __forceinline__ NeusSample neus_alpha(float sdf, float gx, float gy, 
     return o;
 }
 
+// kRender: the forward of a rendered frame (psdf_neus_render_forward). The alpha / transmittance chain and the colour head are the
+// training kernel's code; there are no loss terms and nothing is stored per sample (gt_rgb, gt_mask, hit, alpha_out, T_out, w_out, bg_T
+// and ray_loss are not read), and the warp also accumulates sum w grad in the order of sum w rgb. Per ray it writes pred_rgb, w_sum,
+// pred_normals = F.normalize(sum w grad) (eps 1e-12) and, with bg_rgb, pred_rgb_bg = T_last bg_rgb.
+template <bool kRender>
 __global__ void __launch_bounds__(kThreads)
 k_neus_forward(int nr_rays, int max_nr_samples, const int* __restrict__ start_end, bool equal, int fixed_n, const float* __restrict__ sdf,
                const float* __restrict__ grad, const float* __restrict__ rgb, const float* __restrict__ dirs, const float* __restrict__ dt_,
                const float* __restrict__ inv_s_dev, float cos_anneal, const float* __restrict__ cos_anneal_dev, const float* __restrict__ gt_rgb, const float* __restrict__ gt_mask,
                const uint8_t* __restrict__ hit, const float* __restrict__ bg_rgb, float* __restrict__ alpha_out, float* __restrict__ T_out, float* __restrict__ w_out,
                float* __restrict__ pred_rgb, float* __restrict__ w_sum, float* __restrict__ bg_T, float* __restrict__ ray_loss /* [R,3] */,
-               NeusExt ext) {
+               NeusExt ext, float* __restrict__ pred_rgb_bg, float* __restrict__ pred_normals) {
     int ray = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     int lane = threadIdx.x & 31;
     if (ray >= nr_rays) return;
@@ -98,20 +103,24 @@ k_neus_forward(int nr_rays, int max_nr_samples, const int* __restrict__ start_en
         }
     }
     float T = 1.0f, ax = 0.f, ay = 0.f, az = 0.f, ws = 0.f, eik = 0.f;
+    float nx = 0.f, ny = 0.f, nz = 0.f;     // render mode: sum w grad
     if (!skip) {
         for (int base = 0; base < rr.n; base += 32) {
             int i = base + lane;
             float al = 0.f, cr = 0.f, cg = 0.f, cb = 0.f;
+            float gx = 0.f, gy = 0.f, gz = 0.f;
             if (i < rr.n) {
                 int k = rr.start + i;
-                float gx = grad[3 * k], gy = grad[3 * k + 1], gz = grad[3 * k + 2];
+                gx = grad[3 * k]; gy = grad[3 * k + 1]; gz = grad[3 * k + 2];
                 NeusSample ns = neus_alpha(sdf[k], gx, gy, gz, dirs[3 * k], dirs[3 * k + 1], dirs[3 * k + 2], dt_[k], s, cos_anneal);
                 al = ns.alpha;
                 cr = rgb[3 * k]; cg = rgb[3 * k + 1]; cb = rgb[3 * k + 2];
                 if (ext.head) { cr = sigmoid_exact(cr * hw[0] + hb[0]); cg = sigmoid_exact(cg * hw[1] + hb[1]); cb = sigmoid_exact(cb * hw[2] + hb[2]); }
-                float nrm = sqrtf(gx * gx + gy * gy + gz * gz) - 1.0f;
-                eik += nrm * nrm;
-                alpha_out[k] = al;
+                if constexpr (!kRender) {
+                    float nrm = sqrtf(gx * gx + gy * gy + gz * gz) - 1.0f;
+                    eik += nrm * nrm;
+                    alpha_out[k] = al;
+                }
             }
             float myT = 1.0f;
             int cnt = min(32, rr.n - base);
@@ -122,18 +131,37 @@ k_neus_forward(int nr_rays, int max_nr_samples, const int* __restrict__ start_en
                 ax = fmaf(wk, __shfl_sync(kFull, cr, k), ax);
                 ay = fmaf(wk, __shfl_sync(kFull, cg, k), ay);
                 az = fmaf(wk, __shfl_sync(kFull, cb, k), az);
+                if constexpr (kRender) {
+                    nx = fmaf(wk, __shfl_sync(kFull, gx, k), nx);
+                    ny = fmaf(wk, __shfl_sync(kFull, gy, k), ny);
+                    nz = fmaf(wk, __shfl_sync(kFull, gz, k), nz);
+                }
                 ws += wk;
                 if (base + k < rr.n - 1) T *= (1.0f - ak + 1e-7f);
             }
-            if (i < rr.n) { T_out[rr.start + i] = myT; if (w_out) w_out[rr.start + i] = al * myT; }
+            if constexpr (!kRender) {
+                if (i < rr.n) { T_out[rr.start + i] = myT; if (w_out) w_out[rr.start + i] = al * myT; }
+            }
         }
+        if constexpr (!kRender) {
 #pragma unroll
-        for (int o = 16; o > 0; o >>= 1) eik += __shfl_xor_sync(kFull, eik, o);
+            for (int o = 16; o > 0; o >>= 1) eik += __shfl_xor_sync(kFull, eik, o);
+        }
     }
     if (lane == 0) {
         if (bg_rgb) { ax = fmaf(T, bg_rgb[3 * ray], ax); ay = fmaf(T, bg_rgb[3 * ray + 1], ay); az = fmaf(T, bg_rgb[3 * ray + 2], az); }
         pred_rgb[3 * ray] = ax; pred_rgb[3 * ray + 1] = ay; pred_rgb[3 * ray + 2] = az;
         w_sum[ray] = ws;
+        if constexpr (kRender) {
+            if (bg_rgb && pred_rgb_bg) {
+#pragma unroll
+                for (int c = 0; c < 3; c++) pred_rgb_bg[3 * ray + c] = T * bg_rgb[3 * ray + c];
+            }
+            // F.normalize(v, dim=1): v / max(||v||_2, 1e-12)
+            const float den = fmaxf(sqrtf(nx * nx + ny * ny + nz * nz), 1e-12f);
+            pred_normals[3 * ray] = nx / den; pred_normals[3 * ray + 1] = ny / den; pred_normals[3 * ray + 2] = nz / den;
+            return;
+        }
         bg_T[ray] = T;
         float h = hit ? (hit[ray] ? 1.0f : 0.0f) : 1.0f;
         float l1 = (fabsf(gt_rgb[3 * ray] - ax) + fabsf(gt_rgb[3 * ray + 1] - ay) + fabsf(gt_rgb[3 * ray + 2] - az)) * h;
@@ -322,9 +350,10 @@ static int neus_forward_impl(int nr_rays, int max_nr_samples, const int* ray_sta
                              const float* bg_rgb, float* alpha, float* transmittance, float* weights, float* pred_rgb, float* weights_sum,
                              float* bg_transmittance, float* ray_loss, const NeusExt& ext, void* stream) {
     if (nr_rays <= 0) return nr_rays == 0 ? PSDF_OK : PSDF_ERR_ARG;
-    k_neus_forward<<<ray_blocks(nr_rays), kThreads, 0, ST>>>(nr_rays, max_nr_samples, ray_start_end, equal != 0, fixed_n, sdf, grad, rgb, dirs, dt,
-                                                            inv_s_dev, cos_anneal_ratio, cos_anneal_dev, gt_rgb, gt_mask, hit, bg_rgb, alpha, transmittance, weights,
-                                                            pred_rgb, weights_sum, bg_transmittance, ray_loss, ext);
+    k_neus_forward<false><<<ray_blocks(nr_rays), kThreads, 0, ST>>>(nr_rays, max_nr_samples, ray_start_end, equal != 0, fixed_n, sdf, grad, rgb, dirs,
+                                                                   dt, inv_s_dev, cos_anneal_ratio, cos_anneal_dev, gt_rgb, gt_mask, hit, bg_rgb, alpha,
+                                                                   transmittance, weights, pred_rgb, weights_sum, bg_transmittance, ray_loss, ext, nullptr,
+                                                                   nullptr);
     PSDF_CHECK_LAUNCH();
     return PSDF_OK;
 }
@@ -459,5 +488,22 @@ int psdf_neus_head_bg_loss_backward(int nr_rays, int max_nr_samples, const int* 
     return neus_backward_impl(nr_rays, max_nr_samples, ray_start_end, equal, fixed_n, sdf, grad, x_raw, dirs, dt, inv_s_dev, cos_anneal_ratio,
                               cos_anneal_dev, gt_rgb, gt_mask, hit, bg_rgb, alpha, transmittance, pred_rgb, weights_sum, bg_transmittance,
                               nullptr, scale_rgb, scale_mask, scale_eik, nr_samples_dev, g_sdf, g_grad, g_x, g_bg_rgb, nullptr, e, stream);
+}
+// Forward-only compositing of a rendered frame (Trainer.render): the render mode of k_neus_forward, colour head on, no loss terms, nothing
+// stored per sample. x_raw [N,3] is the colour network's linear output; img_idx / weight_delta / bias may be NULL (no calibration),
+// bg_rgb [R,3] may be NULL (no background). pred_rgb_bg is written only with bg_rgb.
+int psdf_neus_render_forward(int nr_rays, int max_nr_samples, const int* ray_start_end, int equal, int fixed_n, const float* sdf, const float* grad,
+                             const float* x_raw, const float* dirs, const float* dt, const float* inv_s_dev, float cos_anneal_ratio, const int* img_idx,
+                             const float* weight_delta, const float* bias, int fixed_img, const float* bg_rgb, float* pred_rgb, float* pred_rgb_bg,
+                             float* pred_normals, float* weights_sum, void* stream) {
+    if (nr_rays <= 0) return nr_rays == 0 ? PSDF_OK : PSDF_ERR_ARG;
+    if (!pred_rgb || !pred_normals || !weights_sum || (bg_rgb && !pred_rgb_bg)) return PSDF_ERR_ARG;
+    NeusExt e = no_ext();
+    e.head = 1; e.img_idx = weight_delta ? img_idx : nullptr; e.weight_delta = weight_delta; e.bias = bias; e.fixed_img = fixed_img;
+    k_neus_forward<true><<<ray_blocks(nr_rays), kThreads, 0, ST>>>(nr_rays, max_nr_samples, ray_start_end, equal != 0, fixed_n, sdf, grad, x_raw, dirs,
+                                                                  dt, inv_s_dev, cos_anneal_ratio, nullptr, nullptr, nullptr, nullptr, bg_rgb, nullptr,
+                                                                  nullptr, nullptr, pred_rgb, weights_sum, nullptr, nullptr, e, pred_rgb_bg, pred_normals);
+    PSDF_CHECK_LAUNCH();
+    return PSDF_OK;
 }
 }  // extern "C"

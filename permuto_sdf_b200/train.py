@@ -124,18 +124,25 @@ def importance_sampling_sdf_model(model_sdf, rsp, ray_origins, ray_dirs, ray_t_e
     return rsp
 
 
+def run_net_samples(with_mask, hyperparams, ray_origins, ray_dirs, model_sdf, occupancy_grid, iter_nr_for_anneal):
+    """the sampling of run_net (train_permuto_sdf.py:111-135): occupancy-grid (or bounding-sphere) samples, compacted, then SDF
+    importance resampling; background samples for scenes without masks. Jitters while model_sdf is training unless
+    hyperparams.jitter_samples says otherwise. Call without autograd. -> (fg, bg or None)"""
+    _, _, _, ray_t_exit, _ = model_sdf.boundary_primitive.ray_intersection(ray_origins, ray_dirs)
+    jitter = model_sdf.training if getattr(hyperparams, "jitter_samples", None) is None else bool(hyperparams.jitter_samples)
+    fg, bg = create_samples(with_mask, hyperparams, ray_origins, ray_dirs, jitter, occupancy_grid, model_sdf.boundary_primitive)
+    if hyperparams.do_importance_sampling and fg.samples_pos.shape[0] != 0:
+        fg = importance_sampling_sdf_model(model_sdf, fg, ray_origins, ray_dirs, ray_t_exit, iter_nr_for_anneal,
+                                           hyperparams.nr_samples_imp_sampling, jitter=jitter)
+    return fg, bg
+
+
 def run_net(with_mask, hyperparams, ray_origins, ray_dirs, img_indices, model_sdf, model_rgb, model_bg, model_colorcal, occupancy_grid,
             iter_nr_for_anneal, cos_anneal_ratio, forced_variance, fused_loss=None):
     """train_permuto_sdf.py:88-177. With `fused_loss` (dict: gt_rgb, gt_mask, hit, w_eik, w_mask) the NeuS compositing and the
     rgb / mask / eikonal losses run in the fused kernel pair (csrc/neus_fused.cu); the result lands in fused_loss['loss']."""
     with torch.no_grad():
-        _, _, _, ray_t_exit, _ = model_sdf.boundary_primitive.ray_intersection(ray_origins, ray_dirs)
-        jitter = model_sdf.training if getattr(hyperparams, "jitter_samples", None) is None else bool(hyperparams.jitter_samples)
-        fg, bg = create_samples(with_mask, hyperparams, ray_origins, ray_dirs, jitter, occupancy_grid,
-                                model_sdf.boundary_primitive)
-        if hyperparams.do_importance_sampling and fg.samples_pos.shape[0] != 0:
-            fg = importance_sampling_sdf_model(model_sdf, fg, ray_origins, ray_dirs, ray_t_exit, iter_nr_for_anneal,
-                                               hyperparams.nr_samples_imp_sampling, jitter=jitter)
+        fg, bg = run_net_samples(with_mask, hyperparams, ray_origins, ray_dirs, model_sdf, occupancy_grid, iter_nr_for_anneal)
         if getattr(hyperparams, "dp_world", 1) > 1:
             # per-sample means (eikonal, curvature) are means over the samples of all ranks: one 4-byte all-reduce of the count
             import torch.distributed as dist
@@ -413,6 +420,7 @@ class Trainer:
         self._fit = None                # device counters and captured graph of the direct sphere fit
         self._cg = None                 # CUDA-graph state (enable_cuda_graph)
         self._dp = None                 # data-parallel state (enable_data_parallel)
+        self._render = None             # workspaces of render()
         self.nr_rays_to_create = hp.nr_rays
         self.last = {}
 
@@ -662,6 +670,21 @@ class Trainer:
             pts, idx = self.occupancy_grid.compute_random_sample_of_grid_points(256 * 256 * 4, True)
             sdf_grid, _ = self.model_sdf(pts, iter_nr_for_anneal)
             self.occupancy_grid.update_with_sdf_random_sample(idx, sdf_grid.contiguous(), self.model_rgb.volume_renderer_neus.get_last_inv_s(), 1e-4)
+
+    def render(self, ray_origins, ray_dirs, chunk_size=None, iter_nr_for_anneal=None, cos_anneal_ratio=1.0, forced_variance=None):
+        """Volume-render rays chunk by chunk on the fused kernels (render.VolumeRender): what run_net_in_chunks(ray_origins, ray_dirs,
+        chunk_size, hp.with_mask, hp, model_sdf, model_rgb, model_bg, occupancy_grid, iter_nr_for_anneal, cos_anneal_ratio,
+        forced_variance) computes, from the same samples. chunk_size: rays per chunk (default render.DEFAULT_CHUNK, at most
+        render.VolumeRender.max_chunk(hp)); iter_nr_for_anneal: default self.iter_nr; forced_variance None: the learned variance.
+        Samples are jittered while model_sdf is in training mode, as in run_net: put the models in eval() to render a frame.
+        Reads no parameter gradient and changes no parameter, .grad, occupancy grid or iteration counter; without jitter it advances no
+        generator. Raises when a model is not on the fused kernels.
+        -> (pred_rgb [R,3], pred_rgb_bg [R,3] or None (scenes with masks), pred_normals [R,3], pred_weights_sum [R,1])"""
+        from .render import DEFAULT_CHUNK, VolumeRender
+        if self._render is None:
+            self._render = VolumeRender(self)
+        return self._render.render(ray_origins, ray_dirs, DEFAULT_CHUNK if chunk_size is None else chunk_size,
+                                   self.iter_nr if iter_nr_for_anneal is None else iter_nr_for_anneal, cos_anneal_ratio, forced_variance)
 
     def step(self, ray_origins, ray_dirs, gt_rgb, gt_mask, img_indices, update_occupancy=None, optimizer_step=True):
         """forward + losses + backward (+ optimizer). Returns the detached loss tensor (no host sync)."""
