@@ -427,6 +427,23 @@ int psdf_loss_terms(int N, const int* nr_valid_dev, const int* nr_mean_dev, cons
  * acc [4] scratch: zero before the first call, left zero by every call. Deterministic mode: fixed-point sums. */
 int psdf_sphere_fit_loss(int N, const float* pos, const float* sdf, const float* grad, float radius, const float center[3], float distance_scale,
                          float w_sdf, float w_eik, float* g_sdf, float* g_grad, float* acc, float* loss, float* terms, void* stream);
+/* points of one SDF-from-point-cloud iteration (train_sdf_from_mesh.py:119-123) in one launch (csrc/surface_fit.cu):
+ *   x [Ns+No,3] = rows idx [Ns] (int64) of the cloud pts [P,3] (index_select), then the box rows u01 [No,3] * size - size / 2 +
+ *   translation (AABB.rand_points_inside, permuto_sdf_py/utils/aabb.py:110-114, each operation rounded on its own as torch does);
+ *   n [Ns,3] = rows idx of the normals nrm [P,3]. box_size / box_translation are HOST arrays. Ns = 0 is AABB.rand_points_inside from a
+ *   given draw (pts, nrm, idx and n may then be NULL). An index outside [0, P) gives a NaN row. More than 2^31 - 1 floats in x or in the
+ *   cloud: PSDF_ERR_UNSUPPORTED. */
+int psdf_surface_fit_points(int P, int Ns, int No, const float* pts, const float* nrm, const long long* idx, const float* u01,
+                            const float box_size[3], const float box_translation[3], float* x, float* n, void* stream);
+/* sdf_loss (permuto_sdf_py/utils/sdf_utils.py:16-57, eik_clamp=None) times scale (train_sdf_from_mesh.py:135-136) in one launch over the
+ * Ns surface rows followed by the No box rows of sdf [Ns+No], grad [Ns+No,3] (d sdf / d x), with the normals nrm [Ns,3]:
+ *   loss = scale (w_eik mean_all |‖grad‖ - 1| + w_nrm mean_surf (1 - cos(grad, nrm)) + w_sdf mean_surf |sdf| + w_off mean_box exp(-100 |sdf|))
+ * -> g_sdf [Ns+No] = d loss / d sdf, g_grad [Ns+No,3] = d loss / d grad (=, torch's autograd conventions: sign(0) = 0, a zero norm
+ * backward at ‖grad‖ = 0, F.cosine_similarity with eps 1e-8), loss [1], terms [4] = the unweighted means {eikonal, normal, sdf, off}.
+ * Ns >= 1 and No >= 1 (a mean over no rows is NaN in the reference). acc [5] scratch: zero before the first call, left zero by every
+ * call. Deterministic mode: fixed-point sums. */
+int psdf_surface_fit_loss(int Ns, int No, const float* sdf, const float* grad, const float* nrm, float w_eik, float w_nrm, float w_sdf,
+                          float w_off, float scale, float* g_sdf, float* g_grad, float* acc, float* loss, float* terms, void* stream);
 /* Sphere.rand_points_inside (src/Sphere.cu) from ONE uniform draw u01 [3,n]: rows = phi / (2 pi), (cos(theta) + 1) / 2, u */
 int psdf_sphere_rand_points_inside_u01(int n, float radius, const float* u01, float* out, void* stream);
 /* psdf_adamw_step over up to 8 parameter groups in one launch: device-resident step count, per-group hyper_dev [2] = {lr, weight_decay};

@@ -96,7 +96,8 @@ def _dtypes():
     global _DT
     if _DT is None:
         import torch
-        _DT = {"float": (torch.float32,), "int": (torch.int32,), "uint8_t": (torch.uint8, torch.bool), "uint64_t": (torch.int64, torch.uint64)}
+        _DT = {"float": (torch.float32,), "int": (torch.int32,), "uint8_t": (torch.uint8, torch.bool), "uint64_t": (torch.int64, torch.uint64),
+               "long long": (torch.int64,)}
     return _DT
 
 

@@ -266,6 +266,41 @@ class Sphere:
 
 
 # ======================================================================================================
+class AABB:
+    """permuto_sdf_py/utils/aabb.py:8-114: the axis-aligned bounding box of train_sdf_from_mesh.py, the SDF model's boundary_primitive
+    there (sizes and translation are 3-sequences). The sphere tracer and the samplers of this package take a bounding Sphere."""
+
+    def __init__(self, bounding_box_sizes_xyz, bounding_box_translation):
+        self.bounding_box_sizes_xyz = [float(v) for v in bounding_box_sizes_xyz]
+        self.bounding_box_translation = [float(v) for v in bounding_box_translation]
+        if len(self.bounding_box_sizes_xyz) != 3 or len(self.bounding_box_translation) != 3:
+            raise RuntimeError("AABB: sizes and translation must have 3 components")
+        half = [s / 2 for s in self.bounding_box_sizes_xyz]
+        self.max_bounds = torch.tensor(half)
+        self.min_bounds = torch.tensor([-h for h in half])
+
+    def check_point_inside_primitive(self, points):
+        """[N,3] -> [N,1] bool: every coordinate strictly inside the box (aabb.py:28-43)"""
+        d = points.device
+        p = points - torch.as_tensor(self.bounding_box_translation, device=d)
+        inside = torch.logical_and(p < self.max_bounds.to(d), p > self.min_bounds.to(d))
+        return (inside * 1.0).sum(dim=-1, keepdim=True) == 3
+
+    def rand_points_inside(self, nr_points):
+        """nr_points uniform points in the box (aabb.py:110-114): one torch.rand(nr_points, 3) draw, then rand_points_inside_u01"""
+        return self.rand_points_inside_u01(torch.rand(int(nr_points), 3, device=_dev()))
+
+    def rand_points_inside_u01(self, u01):
+        """the box points of a given uniform draw u01 [n,3]: u01 * size - size / 2 + translation, bit-identical to the reference's
+        expression (one kernel, psdf_surface_fit_points without cloud rows)"""
+        u = _f32(u01, "u01", 3)
+        out = torch.empty(u.shape[0], 3, device=u.device)
+        call("psdf_surface_fit_points", 0, 0, u.shape[0], None, None, None, u, self.bounding_box_sizes_xyz, self.bounding_box_translation,
+             out, None)
+        return out
+
+
+# ======================================================================================================
 class OccupancyGrid:
     """include/permuto_sdf/OccupancyGrid.cuh:19-64, src/OccupancyGrid.cu"""
 
