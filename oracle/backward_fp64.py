@@ -1,8 +1,9 @@
 """TEST INFRASTRUCTURE -- NOT PRODUCT CODE.
 
-fp64 reference of the three fused training backwards (csrc/fused_sdf_bwd.cu, fused_rgb_bwd.cu, fused_bg.cu): the same operations as
-the kernels, with every reduction in fp64, so that a kernel can be judged per level, per layer and per element rather than by one
-ratio per tensor.
+fp64 reference of the fused kernels: the three training backwards (csrc/fused_sdf_bwd.cu, fused_rgb_bwd.cu, fused_bg.cu) and the
+forwards (fused_sdf.cu: value + tangent, value-only and sphere-tracer kernels; fused_rgb.cu; fused_bg.cu). The same operations as the
+kernels, with every reduction in fp64, so that a kernel can be judged per level, per layer and per element rather than by one ratio
+per tensor.
 
 "The same operation" is defined as follows. The discrete decisions of the permutohedral encoder (remainder-0 point, rank, hashed
 vertex indices) and the barycentric weights are taken in fp32 from encoding_oracle, which the per-op encoder matches bit for bit. At
@@ -17,6 +18,24 @@ directional derivative along g_grad) under fp64 autograd and returns the per-sam
 which the lattice gradient is formed by an explicit fp64 index_add together with, per table entry, A = sum |contribution| and
 n = the number of (sample, vertex) contributions. `*_autograd` differentiates the whole forward (double backward for the SDF) with
 the lattice as an autograd leaf; tests/test_backward_fp64_reference_cpu.py checks that the two agree to 1e-12.
+
+The forward references (`*_forward_reference`) return, beside every output, its error scale A: the linearised propagation of the
+terms that form it, i.e. what the output's rounding error is proportional to when every operand of every product carries a small
+relative error. A kernel output is accepted per element when |got - ref| <= eps A (tests/test_forward_fp64_reference_cpu.py derives
+eps and shows that the kernels' arithmetic, emulated, stays well inside it while a one-pass bf16 product does not):
+  * layer-0 input A^a_0: w_l sum_k |B_k| |v_k| for the two columns of level l, |x * scaling| for the concat columns; colour inputs add
+    |SH|, |normal| and |geom|, background inputs |SH|. An input's error is its own bf16 split, relative to its value, so its scale is
+    the absolute sum (>= |value|);
+  * every layer: A^z_l = sqrt(W_l^2 (A^a_l)^2 + b_l^2), then A^a_{l+1} = sqrt((gelu'(z_l) A^z_l)^2 + a_{l+1}^2). The rounding errors of a
+    product's K terms are independent, so they add in quadrature: the absolute sum |W_l| A^a_l + |b_l| overstates them by ~sqrt(K)
+    per layer, compounding with depth (2^9 over the background's seven layers of 64), so that no single eps would both accept the
+    kernels' hidden-16 SDF and reject a one-pass product in the background network. The first term of A^a carries an error of z_l
+    through the activation; the second is the activation's own representation error (the next product splits a_{l+1} itself): near
+    z = -0.75 (gelu' = 0) the first vanishes while |gelu(z)| = 0.17 |z| does not;
+  * the density: |sigmoid(z)| A^z (softplus' = sigmoid);
+  * tangent streams (d / dx_j, input A^{ta}_0 = w_l sum_k |dB_k| |v_k| and the concat column's |scaling|): A^{tz}_l = sqrt(W_l^2
+    (A^{ta}_l)^2), A^{ta}_{l+1} = sqrt((gelu'(z_l) A^{tz}_l)^2 + (gelu''(z_l) tz_l A^z_l)^2 + ta_{l+1}^2); the middle term is where an
+    error of z_l enters the gradient through the GELU, the last the tangent's own representation error.
 """
 import math
 
@@ -398,3 +417,127 @@ def bg_autograd(pos, dirs, lattice, scale, shift, window, points_scaling, W, b, 
 def dense_lattice(lat_out):
     """per-level (grad, A, n) -> [L, T, 2] gradient"""
     return torch.stack([o[0] for o in lat_out], 0)
+
+
+# ------------------------------------------------------------------------------------------------ forwards with error scales
+def gelu_d2(z):
+    return torch.exp(-0.5 * z * z) * INV_SQRT_2PI * (2.0 - z * z)
+
+
+class Exact:
+    """the arithmetic of the forward references: fp64 products and the exact-erf GELU. A test may substitute an emulation of a
+    kernel's arithmetic (same interface) to run the same chain as the kernel would."""
+
+    def linear(self, l, a, W, b=None):
+        z = a @ W.t()
+        return z + b if b is not None else z
+
+    def gelu(self, z):
+        """-> gelu(z), gelu'(z)"""
+        return gelu(z), gelu_d1(z)
+
+
+def features_bound(plan, lattice64, pos64, window, points_scaling, tangents=False):
+    """encoder values and their A (see the module docstring); with tangents, the three tangents d / dx_j and their A as [3, N, E]"""
+    w = window.double().to(pos64.device)
+    N, D = pos64.shape
+    cols, acols, tcols, atcols = [], [], [], []
+    dirs = torch.eye(D, dtype=F64, device=pos64.device) if tangents else None
+    for l in range(plan.L):
+        vals = _gather(lattice64, plan, l)
+        B = plan.bary[l]
+        cols.append(w[l] * (B[:, :, None] * vals).sum(1))
+        acols.append(w[l] * (B.abs()[:, :, None] * vals.abs()).sum(1))
+        if tangents:
+            dB = torch.stack([bary_linear(dirs[j].expand(N, D) * plan.scale[l], plan.rank[l]) for j in range(D)], 0)    # [3, N, D+1]
+            tcols.append(w[l] * (dB[..., None] * vals[None]).sum(2))
+            atcols.append(w[l] * (dB.abs()[..., None] * vals.abs()[None]).sum(2))
+    cc = _concat(pos64, points_scaling)
+    feat = torch.cat(cols + cc, 1)
+    A = torch.cat(acols + [c.abs() for c in cc], 1)
+    if not tangents:
+        return feat, A, None, None
+    tc = torch.stack([torch.cat(_concat(dirs[j].expand(N, D), points_scaling), 1) for j in range(D)], 0)
+    tfeat = torch.cat([torch.cat(tcols, 2), tc], 2)
+    At = torch.cat([torch.cat(atcols, 2), tc.abs()], 2)
+    return feat, A, tfeat, At
+
+
+def chain_bound(ar, layers, a, A, ta=None, At=None, first=0):
+    """Linear -> GELU -> ... -> Linear over layers [(W, b)] (fp64) with the error scales of the module docstring. Returns the last
+    pre-activation z and A^z, and the tangents tz, A^{tz} (or None)."""
+    n = len(layers)
+    for i, (W, b) in enumerate(layers):
+        W2 = W * W
+        z = ar.linear(first + i, a, W, b)
+        Az = (A * A @ W2.t() + b * b).sqrt()
+        tz = Atz = None
+        if ta is not None:
+            tz = ar.linear(first + i, ta, W)
+            Atz = (At * At @ W2.t()).sqrt()
+        if i == n - 1:
+            return z, Az, tz, Atz
+        a, d1 = ar.gelu(z)
+        A = ((d1 * Az) ** 2 + a.double() ** 2).sqrt()
+        if ta is not None:
+            z64 = z.double()
+            ta = d1 * tz
+            At = ((d1 * Atz) ** 2 + (gelu_d2(z64) * tz * Az) ** 2 + ta.double() ** 2).sqrt()
+
+
+def _dev_layers(W, b, dev):
+    return [(w.detach().to(dev).double(), x.detach().to(dev).double()) for w, x in zip(W, b)]
+
+
+def sdf_forward_reference(pos, lattice, scale, shift, window, points_scaling, W, b, device=None, plan=None, arith=None):
+    """the SDF forward: sdf [N], grad = d sdf / dx [N, 3] (three tangent streams), geom [N, out_dim - 1] and their error scales
+    A_sdf, A_grad, A_geom (module docstring)"""
+    dev = _dev(device)
+    ar = arith or Exact()
+    plan = plan or Plan(pos, scale, shift, lattice.shape[1]).to(dev)
+    feat, A, tfeat, At = features_bound(plan, lattice.detach().to(dev).double(), pos.detach().to(dev).double(), window, points_scaling, True)
+    z, Az, tz, Atz = chain_bound(ar, _dev_layers(W, b, dev), feat, A, tfeat, At)
+    z, tz = z.double(), tz.double()
+    return dict(sdf=z[:, 0], grad=tz[:, :, 0].t(), geom=z[:, 1:], A_sdf=Az[:, 0], A_grad=Atz[:, :, 0].t(), A_geom=Az[:, 1:], plan=plan)
+
+
+def lipschitz_weights(W, c):
+    """LipshitzMLP.normalization in fp64: W * min(softplus(c) / sum_k |W|, 1) per row"""
+    W, c = W.double(), torch.as_tensor(c).double().reshape(())
+    return W * torch.clamp(torch.nn.functional.softplus(c) / W.abs().sum(1), max=1.0)[:, None]
+
+
+def rgb_forward_reference(pos, dirs, sdf_grad, geom, lattice, scale, shift, window, points_scaling, W_eff, b, device=None, sh=None,
+                          arith=None):
+    """the colour network's linear output out [N, 3] and A_out, W_eff the normalised matrices"""
+    dev = _dev(device)
+    ar = arith or Exact()
+    plan = Plan(pos, scale, shift, lattice.shape[1]).to(dev)
+    feat, A, _, _ = features_bound(plan, lattice.detach().to(dev).double(), pos.detach().to(dev).double(), window, points_scaling)
+    sh = (sh if sh is not None else sh_fp32(dirs, 5)).to(dev)
+    nrm = _normalize64(sdf_grad.detach().to(dev).double())
+    gm = geom.detach().to(dev).double()
+    x = torch.cat([feat, sh, nrm, gm], 1)
+    Ax = torch.cat([A, sh.abs(), nrm.abs(), gm.abs()], 1)
+    z, Az, _, _ = chain_bound(ar, _dev_layers(W_eff, b, dev), x, Ax)
+    return dict(out=z.double(), A_out=Az)
+
+
+def bg_forward_reference(pos, dirs, lattice, scale, shift, window, points_scaling, W, b, device=None, sh=None, arith=None):
+    """the background network: rgb_raw [N, 3], density [N] and A_rgb, A_density (torch.nn.Linear layout, trunk layer 3 unrotated);
+    z_density: the density's pre-activation"""
+    dev = _dev(device)
+    ar = arith or Exact()
+    plan = Plan(pos, scale, shift, lattice.shape[1]).to(dev)
+    feat, A, _, _ = features_bound(plan, lattice.detach().to(dev).double(), pos.detach().to(dev).double(), window, points_scaling)
+    layers = _dev_layers(W, b, dev)
+    z, Az, _, _ = chain_bound(ar, layers[:4], feat, A)
+    z0 = z[:, 0].double()
+    density = torch.nn.functional.softplus(z0)
+    A_density = torch.sigmoid(z0) * Az[:, 0]
+    sh = (sh if sh is not None else sh_fp32(dirs, 4)).to(dev)
+    a, d1 = ar.gelu(z[:, 1:65])
+    x = torch.cat([a, sh.to(a.dtype)], 1)
+    Ax = torch.cat([((d1 * Az[:, 1:65]) ** 2 + a.double() ** 2).sqrt(), sh.abs()], 1)
+    zr, Azr, _, _ = chain_bound(ar, layers[4:], x, Ax, first=4)
+    return dict(rgb_raw=zr.double(), density=density, A_rgb=Azr, A_density=A_density, z_density=z0)
