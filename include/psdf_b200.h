@@ -309,6 +309,13 @@ int psdf_bg_mlp_pack(int in_dim, const float* W0, const float* b0, const float* 
 int psdf_bg_fused_forward(int N, int L, int T, const float* pos, const float* dirs, const float* lattice, const float* scale_factor,
                           const float* shift, const float* window, float points_scaling, const uint8_t* blob, float* rgb_raw, float* density,
                           void* stream);
+/* NerfHash.forward at either input width (permuto_sdf_py/models/models.py:425-563; train_nerf.py:164-165 builds NerfHash(3) for the
+ * foreground and NerfHash(4) for the background): pos [N, pos_dim], pos_dim 3 or 4, otherwise the arguments of psdf_bg_fused_forward
+ * (the scale / shift rows of the encoding have pos_dim columns). Both widths give 2L + 4 encoder columns, so the blob of psdf_bg_mlp_pack
+ * serves both. psdf_bg_fused_forward is the pos_dim = 4 case. */
+int psdf_nerf_fused_forward(int pos_dim, int N, int L, int T, const float* pos, const float* dirs, const float* lattice,
+                            const float* scale_factor, const float* shift, const float* window, float points_scaling, const uint8_t* blob,
+                            float* rgb_raw, float* density, void* stream);
 /* backward of psdf_bg_fused_forward (loss.backward() through NerfHash.forward, first order): g_rgb_raw [N,3], g_density [N] ->
  * grad_lattice (+=), weight gradients gW_l [N_l,K_l] (+=) and bias gradients gb_l (+=). workspace:
  * psdf_bg_fused_backward_workspace_bytes(N) bytes of scratch. Launches the tensor-core kernel, then the lattice-scatter kernel. */
@@ -318,6 +325,13 @@ int psdf_bg_fused_backward(int N, int L, int T, const float* pos, const float* d
                            const float* g_density, float* grad_lattice, uint8_t* workspace, float* gW0, float* gW1, float* gW2, float* gW3,
                            float* gW4, float* gW5, float* gW6, float* gb0, float* gb1, float* gb2, float* gb3, float* gb4, float* gb5,
                            float* gb6, void* stream);
+/* backward of psdf_nerf_fused_forward (loss.backward() through NerfHash.forward), arguments of psdf_bg_fused_backward after pos_dim;
+ * workspace: psdf_bg_fused_backward_workspace_bytes(N). psdf_bg_fused_backward is the pos_dim = 4 case. */
+int psdf_nerf_fused_backward(int pos_dim, int N, int L, int T, const float* pos, const float* dirs, const float* lattice,
+                             const float* scale_factor, const float* shift, const float* window, float points_scaling, const uint8_t* blob,
+                             const float* g_rgb_raw, const float* g_density, float* grad_lattice, uint8_t* workspace, float* gW0, float* gW1,
+                             float* gW2, float* gW3, float* gW4, float* gW5, float* gW6, float* gb0, float* gb1, float* gb2, float* gb3,
+                             float* gb4, float* gb5, float* gb6, void* stream);
 /* background compositing with the colour head folded in (one thread per ray): Colorcal.calib_RGB_samples_packed + sigmoid of x_raw [N,3]
  * (models.py:677-741; img_idx [R] per ray, weight_delta / bias may be NULL: no calibration), then VolumeRenderingNerf.compute_weights +
  * integrate (volume_rendering_modules.py:61-89): alpha = 1 - exp(-density dt), T = exclusive cumprod(1 - alpha + 1e-7), w = alpha T,
@@ -328,6 +342,26 @@ int psdf_nerf_bg_composite_forward(PSDF_RSP, const float* x_raw, const float* de
 int psdf_nerf_bg_composite_backward(PSDF_RSP, const float* x_raw, const float* density, const float* dt, const int* img_idx,
                                     const float* weight_delta, const float* bias, int fixed_img, const float* g_bg_rgb, float* g_x,
                                     float* g_density, float* g_weight_delta, float* g_bias, void* stream);
+
+/* foreground NeRF compositing and the loss of train_nerf.py (one thread per ray, samples left to right): colour head as in
+ * psdf_nerf_bg_composite_forward, VolumeRenderingNerf.compute_weights + integrate (volume_rendering_modules.py:61-89),
+ * bg_transmittance = the transmittance of the ray's last sample (VolumeRenderingGPU.cuh:400-416; 1 for a ray without samples),
+ * pred_rgb = sum w rgb + bg_transmittance bg_rgb (train_nerf.py:76-95; bg_rgb [R,3] or NULL), weights_sum [R] = sum w, and
+ * loss [1] = ((gt - pred)^2 hit).mean() + mask_weight BCE(weights_sum.clip(1e-3, 1 - 1e-3), gt_mask) (train_nerf.py:176-182; gt_mask [R]
+ * or NULL: no mask term), terms [2] = {loss_rgb, BCE mean}. hit [R] u8. acc [3] scratch: zero before the first call, left zero by every
+ * call. Deterministic mode: fixed-point sums. gt_rgb == NULL renders: no loss (hit, acc, loss, terms unused), and pred_rgb_bg [R,3]
+ * (may be NULL) receives bg_transmittance bg_rgb.
+ * The backward differentiates that loss (seed 1): g_x [N,3] and g_density [N] on the rows of the rays (=; other rows untouched),
+ * g_bg_rgb [R,3] (=, with bg_rgb), calibration gradients (+=; may be NULL). torch's conventions: clamp passes the gradient on the closed
+ * interval, BCE backward (x - y) / max(x (1 - x), 1e-12). */
+int psdf_nerf_loss_forward(PSDF_RSP, const float* x_raw, const float* density, const float* dt, const int* img_idx, const float* weight_delta,
+                           const float* bias, int fixed_img, const float* bg_rgb, const float* gt_rgb, const uint8_t* hit, const float* gt_mask,
+                           float mask_weight, float* pred_rgb, float* weights_sum, float* bg_transmittance, float* pred_rgb_bg, float* acc,
+                           float* loss, float* terms, void* stream);
+int psdf_nerf_loss_backward(PSDF_RSP, const float* x_raw, const float* density, const float* dt, const int* img_idx, const float* weight_delta,
+                            const float* bias, int fixed_img, const float* bg_rgb, const float* gt_rgb, const uint8_t* hit, const float* gt_mask,
+                            float mask_weight, const float* pred_rgb, const float* weights_sum, const float* bg_transmittance, float* g_x,
+                            float* g_density, float* g_bg_rgb, float* g_weight_delta, float* g_bias, void* stream);
 
 /* ---------------------------------------------------------------- direct (autograd-free) training iteration
  * The reference's iteration (permuto_sdf_py/train_permuto_sdf.py:311-422) spends ~70 one-block PyTorch launches between its big kernels

@@ -7,6 +7,7 @@ sphere-tracing hot path behind the reference's own Python operator API.
                                               reference's permuto_sdf_py runs unchanged (see INTEGRATION.md)
     permuto_sdf_b200.patch_reference_models   routes the reference's own SDF / RGB classes through the fused tensor-core kernels
     permuto_sdf_b200.SurfaceFit / AABB        SDF from an oriented point cloud (train_sdf_from_mesh.py) on the fused kernels
+    permuto_sdf_b200.NerfTrainer              NeRF training (train_nerf.py) on the fused kernels
 
 All device work goes through the C ABI in include/psdf_b200.h (libpsdf_b200.so, hand-written CUDA).
 There is no CPU or PyTorch fallback: importing is cheap, but any op raises if the library is missing
@@ -23,6 +24,9 @@ def __getattr__(name):
     if name == "SurfaceFit":
         from .surface_fit import SurfaceFit
         return SurfaceFit
+    if name == "NerfTrainer":
+        from .nerf_train import NerfTrainer
+        return NerfTrainer
     if name == "AABB":
         from .permuto_sdf import AABB
         return AABB

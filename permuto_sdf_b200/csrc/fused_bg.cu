@@ -72,23 +72,25 @@ __global__ void k_pack_bg(BgGeom g, BgLayers p, uint8_t* blob) {
 }
 
 // Layer-0 operand tile of one sample row and the SH_4 columns of layer 4: thread (row, grp) builds the lattice cores grp, grp + 4, ...;
-// group 0 the concat-point core, groups 1 / 2 the two SH cores, group 3 the zero padding up to Kp0.
+// group 0 the concat-point core, groups 1 / 2 the two SH cores, group 3 the zero padding up to Kp0. D = 3 (foreground NeRF) or 4
+// (NeRF++ background): both give 2L + 4 columns, the concat core {x0, x1, x2, 0} * scaling at D = 3.
+template <int D>
 __device__ __forceinline__ void build_bg_input(const BgParams& P, const LevelC* lc, const float2* __restrict__ lattice,
                                                const float* __restrict__ pos, const float* __restrict__ dirs, int n, bool valid, int row,
                                                int grp, uint8_t* a_hi, uint8_t* a_lo, bool with_sh) {
     float x[4] = {0.f, 0.f, 0.f, 0.f};
     if (valid) {
 #pragma unroll
-        for (int i = 0; i < 4; i++) x[i] = pos[(size_t)n * 4 + i];
+        for (int i = 0; i < D; i++) x[i] = pos[(size_t)n * D + i];
     }
     const int level_cores = P.L / 4;
     for (int kc = grp; kc < level_cores; kc += kRgbGroups) {
         float fv[8];
 #pragma unroll
         for (int q = 0; q < 4; q++) {
-            Simplex<4> s;
-            float2 v[5];
-            const float2 a = level_features(x, lc, kc * 4 + q, lattice, P.T, P.cap_mask, s, v);
+            Simplex<D> s;
+            float2 v[D + 1];
+            const float2 a = level_features<D>(x, lc, kc * 4 + q, lattice, P.T, P.cap_mask, s, v);
             fv[2 * q] = a.x; fv[2 * q + 1] = a.y;
         }
         store8w(a_hi, a_lo, row, kc, fv);
@@ -129,6 +131,7 @@ __device__ __forceinline__ void gelu_chunk_to_tile(uint32_t taddr, const float* 
 // chunks of layer l's output that feed the next layer (the trunk output's density chunk does not)
 __device__ __forceinline__ int act_chunks(const BgGeom& g, int l) { return l == 3 ? kBgFeat / 16 : g.Np[l] / 16; }
 
+template <int D>
 __global__ void __launch_bounds__(kRgbThreads, 1)
 k_bg_fused(BgParams P, const float* __restrict__ pos, const float* __restrict__ dirs, const float2* __restrict__ lattice,
            const float* __restrict__ scale, const float* __restrict__ shift, const float* __restrict__ window, const uint8_t* __restrict__ blob,
@@ -147,7 +150,7 @@ k_bg_fused(BgParams P, const float* __restrict__ pos, const float* __restrict__ 
         umma::mbar_fence_init();
         umma::acc_attach(g_acc_bg + (size_t)blockIdx.x * kTile * kAccFwdCols, kAccFwdCols);
     }
-    load_level_consts<4>(lc, P.L, scale, shift, window, tid, kRgbThreads);
+    load_level_consts<D>(lc, P.L, scale, shift, window, tid, kRgbThreads);
     for (int i = tid; i < kBgNL * 128; i += kRgbThreads) {
         int l = i >> 7, c = i & 127;
         s_bias[i] = (c < P.g.Np[l]) ? reinterpret_cast<const float*>(blob + P.g.bias[l])[c] : 0.0f;
@@ -159,7 +162,7 @@ k_bg_fused(BgParams P, const float* __restrict__ pos, const float* __restrict__ 
     for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
         const int n = tile * kTile + row;
         const bool valid = n < P.N;
-        build_bg_input(P, lc, lattice, pos, dirs, n, valid, row, grp, s_a, s_a + kWTileBytes, true);
+        build_bg_input<D>(P, lc, lattice, pos, dirs, n, valid, row, grp, s_a, s_a + kWTileBytes, true);
 #pragma unroll 1
         for (int l = 0; l < kBgNL; l++) {
             umma::mbar_wait(&bars[0], w_phase);
@@ -199,6 +202,7 @@ struct BgBwdOut {
     unsigned long long* fx_mlp;       // deterministic mode: DetBufs::rgb_mlp (layout kFxW / kFxB), else NULL
 };
 
+template <int D>
 __global__ void __launch_bounds__(kRgbThreads, 1)
 k_bg_fused_backward(BgParams P, const float* __restrict__ pos, const float* __restrict__ dirs, const float2* __restrict__ lattice,
                     const float* __restrict__ scale, const float* __restrict__ shift, const float* __restrict__ window,
@@ -221,7 +225,7 @@ k_bg_fused_backward(BgParams P, const float* __restrict__ pos, const float* __re
         umma::mbar_fence_init();
         umma::acc_attach(g_acc_bg_bwd + (size_t)blockIdx.x * kTile * kAccBwdCols, kAccBwdCols);
     }
-    load_level_consts<4>(lc, P.L, scale, shift, window, tid, kRgbThreads);
+    load_level_consts<D>(lc, P.L, scale, shift, window, tid, kRgbThreads);
     for (int i = tid; i < kBgNL * 128; i += kRgbThreads) {
         int l = i >> 7, c = i & 127;
         s_bias[i] = (c < P.g.Np[l]) ? reinterpret_cast<const float*>(blob + P.g.bias[l])[c] : 0.0f;
@@ -242,7 +246,7 @@ k_bg_fused_backward(BgParams P, const float* __restrict__ pos, const float* __re
         const bool first_tile = tile == (int)blockIdx.x;
         const int n = tile * kTile + row;
         const bool valid = n < P.N;
-        build_bg_input(P, lc, lattice, pos, dirs, n, valid, row, grp, s_a, s_a + kWTileBytes, true);
+        build_bg_input<D>(P, lc, lattice, pos, dirs, n, valid, row, grp, s_a, s_a + kWTileBytes, true);
         // ---------------- forward recompute, layers 0..5; afterwards s_a = a_6
 #pragma unroll 1
         for (int l = 0; l < kBgNL - 1; l++) {
@@ -322,7 +326,7 @@ k_bg_fused_backward(BgParams P, const float* __restrict__ pos, const float* __re
                     for (int c = grp; c < act_chunks(P.g, lp - 1); c += kRgbGroups)
                         gelu_chunk_to_tile(tz(lp - 1) + lane_off + c * 16, s_bias + (lp - 1) * 128 + c * 16, s_a, row, c);
                 } else {
-                    build_bg_input(P, lc, lattice, pos, dirs, n, valid, row, grp, s_a, s_a + kWTileBytes, false);
+                    build_bg_input<D>(P, lc, lattice, pos, dirs, n, valid, row, grp, s_a, s_a + kWTileBytes, false);
                 }
             } else {
                 // abar_0's lattice columns -> the exchange rows of k_bg_lattice_scatter
@@ -367,9 +371,10 @@ k_bg_fused_backward(BgParams P, const float* __restrict__ pos, const float* __re
     }
 }
 
-// Encoder backward: lattice[l][idx_r] += window_l B_r abar_0[l] (D = 4) from the exchange rows of k_bg_fused_backward. blockIdx.y = level,
-// warp = 32 consecutive sample slots.
+// Encoder backward: lattice[l][idx_r] += window_l B_r abar_0[l] from the exchange rows of k_bg_fused_backward. blockIdx.y = level,
+// warp = 32 consecutive sample slots. pos, scale and shift have D columns.
 constexpr int kScatterThreads = 256;
+template <int D>
 __global__ void __launch_bounds__(kScatterThreads, 8)
 k_bg_lattice_scatter(BgParams P, const float* __restrict__ pos, const float2* __restrict__ xch, int xch_stride, const float* __restrict__ scale,
                      const float* __restrict__ shift, const float* __restrict__ window, float* __restrict__ grad_lattice,
@@ -378,32 +383,57 @@ k_bg_lattice_scatter(BgParams P, const float* __restrict__ pos, const float2* __
     if (slot >= xch_stride) return;                                  // whole warps (xch_stride % 128 == 0)
     const int l = blockIdx.y, lane = threadIdx.x & 31;
     const bool valid = slot < P.N;
-    float x[4], sc[4], sh[4];
+    float x[D], sc[D], sh[D];
 #pragma unroll
-    for (int i = 0; i < 4; i++) {
-        x[i] = valid ? pos[(size_t)slot * 4 + i] : 0.0f;
-        sc[i] = scale[l * 4 + i];
-        sh[i] = shift ? shift[l * 4 + i] : 0.0f;
+    for (int i = 0; i < D; i++) {
+        x[i] = valid ? pos[(size_t)slot * D + i] : 0.0f;
+        sc[i] = scale[l * D + i];
+        sh[i] = shift ? shift[l * D + i] : 0.0f;
     }
     const float w = window ? window[l] : 1.0f;
     const float2 a = xch[(size_t)l * xch_stride + slot];
     const bool aggregate = sc[0] < kAggregateBelowScale;             // warp-uniform (l is)
-    scatter_level<false, 4>(x, nullptr, sc, sh, w, a.x, a.y, 0.f, 0.f, valid, aggregate, true, lane, P.cap_mask, (unsigned)P.T,
+    scatter_level<false, D>(x, nullptr, sc, sh, w, a.x, a.y, 0.f, 0.f, valid, aggregate, true, lane, P.cap_mask, (unsigned)P.T,
                             grad_lattice + (size_t)l * P.T * 2, fx_lattice ? fx_lattice + (size_t)l * P.T * 2 : nullptr);
 }
 
-// ---------------------------------------------------------------------------------------------- background compositing
+// ---------------------------------------------------------------------------------------------- NeRF compositing
 // Colour head + VolumeRenderingNerf.compute_weights + integrate (permuto_sdf_py/volume_rendering/volume_rendering_modules.py:61-89) per ray:
 //     c_i = sigmoid(x_i (1 + wd[img]) + b[img]),  alpha_i = 1 - exp(-sigma_i dt_i),  a_i = 1 - alpha_i + 1e-7,
 //     T_i = prod_{j<i} a_j,  w_i = alpha_i T_i,  bg_rgb = sum_i w_i c_i
-// One thread per ray, samples in order (the left-to-right products of the per-op path).
+// One thread per ray, samples in order (the left-to-right products of the per-op path). The background (k_bg_composite*) and the
+// foreground with its loss (k_nerf_loss*) share the per-sample chain below.
 struct CalibArgs { const int* img; const float* wd; const float* b; int fixed; };
+struct NerfAlpha { float e, alpha, a; };        // exp(-sigma dt), alpha, the factor 1 - alpha + 1e-7 of the transmittance
+__device__ __forceinline__ NerfAlpha nerf_alpha(float density, float dt) {
+    NerfAlpha s;
+    s.e = expf(-density * dt);
+    s.alpha = 1.0f - s.e;
+    s.a = 1.0f - s.alpha + 1e-7f;
+    return s;
+}
+__device__ __forceinline__ float calib_sigmoid(float x, float sc, float sh) { return 1.0f / (1.0f + expf(-(x * sc + sh))); }
 __device__ __forceinline__ void calib_of(const CalibArgs& C, int ray, float* sc, float* sh, int& img) {
     img = C.img ? C.img[ray] : -1;
     const bool on = C.wd != nullptr && img != C.fixed && img >= 0;
 #pragma unroll
     for (int k = 0; k < 3; k++) { sc[k] = on ? 1.0f + C.wd[img * 3 + k] : 1.0f; sh[k] = on ? C.b[img * 3 + k] : 0.0f; }
     if (!on) img = -1;
+}
+// per-sample colour backward: G . d c / d x_raw (=) with the calibration gradients summed over the ray
+__device__ __forceinline__ float nerf_colour_backward(float G, float w, float c, float x, float sc, float& gwd, float& gb) {
+    const float gz = G * w * c * (1.0f - c);            // d / d calibrated pre-activation
+    gwd = fmaf(gz, x, gwd);
+    gb += gz;
+    return gz * sc;
+}
+__device__ __forceinline__ void add_calib_grads(int img, const float* gwd, const float* gb, float* g_wd, float* g_b, unsigned long long* fx) {
+    if (img < 0 || !g_wd) return;
+#pragma unroll
+    for (int k = 0; k < 3; k++) {
+        if (fx && img < kDetImages) { fx_add(fx + img * 3 + k, gwd[k]); fx_add(fx + 3 * kDetImages + img * 3 + k, gb[k]); }
+        else { atomicAdd(g_wd + img * 3 + k, gwd[k]); atomicAdd(g_b + img * 3 + k, gb[k]); }
+    }
 }
 __global__ void __launch_bounds__(128)
 k_bg_composite(int nr_rays, int max_nr_samples, const int* __restrict__ start_end, bool equal, int fixed_n, const float* __restrict__ x_raw,
@@ -418,11 +448,11 @@ k_bg_composite(int nr_rays, int max_nr_samples, const int* __restrict__ start_en
         calib_of(C, ray, sc, sh, img);
         float T = 1.0f;
         for (int i = rr.start; i < rr.end; i++) {
-            const float alpha = 1.0f - expf(-density[i] * dt[i]);
-            const float w = alpha * T;
+            const NerfAlpha na = nerf_alpha(density[i], dt[i]);
+            const float w = na.alpha * T;
 #pragma unroll
-            for (int k = 0; k < 3; k++) acc[k] = fmaf(w, 1.0f / (1.0f + expf(-(x_raw[(size_t)i * 3 + k] * sc[k] + sh[k]))), acc[k]);
-            T *= 1.0f - alpha + 1e-7f;
+            for (int k = 0; k < 3; k++) acc[k] = fmaf(w, calib_sigmoid(x_raw[(size_t)i * 3 + k], sc[k], sh[k]), acc[k]);
+            T *= na.a;
         }
     }
 #pragma unroll
@@ -446,41 +476,206 @@ k_bg_composite_backward(int nr_rays, int max_nr_samples, const int* __restrict__
     // pass 1: the ray's total sum_i w_i c_i (suffix sums S_i = total - prefix_i)
     float T = 1.0f;
     for (int i = rr.start; i < rr.end; i++) {
-        const float alpha = 1.0f - expf(-density[i] * dt[i]);
-        const float w = alpha * T;
+        const NerfAlpha na = nerf_alpha(density[i], dt[i]);
+        const float w = na.alpha * T;
 #pragma unroll
-        for (int k = 0; k < 3; k++) tot[k] = fmaf(w, 1.0f / (1.0f + expf(-(x_raw[(size_t)i * 3 + k] * sc[k] + sh[k]))), tot[k]);
-        T *= 1.0f - alpha + 1e-7f;
+        for (int k = 0; k < 3; k++) tot[k] = fmaf(w, calib_sigmoid(x_raw[(size_t)i * 3 + k], sc[k], sh[k]), tot[k]);
+        T *= na.a;
     }
     // pass 2: d/d alpha_i = G . (T_i c_i - S_i / a_i), d alpha / d sigma = dt (1 - alpha); d/d c_i = G w_i
     T = 1.0f;
     float pre[3] = {0.f, 0.f, 0.f};
     for (int i = rr.start; i < rr.end; i++) {
-        const float e = expf(-density[i] * dt[i]);
-        const float alpha = 1.0f - e, a = 1.0f - alpha + 1e-7f;
-        const float w = alpha * T;
+        const NerfAlpha na = nerf_alpha(density[i], dt[i]);
+        const float w = na.alpha * T;
         float ga = 0.f;
 #pragma unroll
         for (int k = 0; k < 3; k++) {
             const float x = x_raw[(size_t)i * 3 + k];
-            const float c = 1.0f / (1.0f + expf(-(x * sc[k] + sh[k])));
+            const float c = calib_sigmoid(x, sc[k], sh[k]);
             pre[k] = fmaf(w, c, pre[k]);
-            ga = fmaf(G[k], T * c - (tot[k] - pre[k]) / a, ga);
-            const float gz = G[k] * w * c * (1.0f - c);            // d / d calibrated pre-activation
-            g_x[(size_t)i * 3 + k] = gz * sc[k];
-            gwd[k] = fmaf(gz, x, gwd[k]);
-            gb[k] += gz;
+            ga = fmaf(G[k], T * c - (tot[k] - pre[k]) / na.a, ga);
+            g_x[(size_t)i * 3 + k] = nerf_colour_backward(G[k], w, c, x, sc[k], gwd[k], gb[k]);
         }
-        g_density[i] = ga * dt[i] * e;
-        T *= a;
+        g_density[i] = ga * dt[i] * na.e;
+        T *= na.a;
     }
-    if (img >= 0 && g_wd) {
+    add_calib_grads(img, gwd, gb, g_wd, g_b, fx);
+}
+
+// ---------------------------------------------------------------------------------------------- foreground NeRF compositing + loss
+// train_nerf.py:67-76 + :176-182 per ray (one thread, samples left to right as in k_bg_composite):
+//     w_i, c_i as above,  weights_sum = sum_i w_i,  bg_T = T of the ray's last sample (its alpha excluded; 1 for a ray without samples),
+//     pred = sum_i w_i c_i + bg_T bg_rgb,
+//     loss = sum_r hit_r |gt_r - pred_r|^2 / (3R) + mask_weight / R sum_r BCE(clamp(weights_sum_r, 1e-3, 1 - 1e-3), gt_mask_r)
+// gt == NULL renders: no loss, pred_bg = bg_T bg_rgb.
+constexpr int kNerfLossThreads = 128;
+constexpr int kNerfDetSlot = 11;                 // DetBufs::loss [11, 13): the two sums in fixed point
+constexpr float kBceLo = 1e-3f, kBceHi = 1.0f - 1e-3f;
+struct NerfLossArgs {
+    int R, max_n, fixed_n;
+    const int* se;
+    bool equal;
+    const float* x_raw;            // [N,3]
+    const float* density;          // [N]
+    const float* dt;               // [N]
+    CalibArgs C;
+    const float* bg;               // [R,3] or NULL
+    const float* gt;               // [R,3] or NULL (render)
+    const uint8_t* hit;            // [R]
+    const float* mask;             // [R] or NULL (no mask term)
+    float mask_weight;
+};
+__device__ __forceinline__ float bce_term(float x, float y) {       // F.binary_cross_entropy (log clamped at -100)
+    return -(y * fmaxf(logf(x), -100.0f) + (1.0f - y) * fmaxf(logf(1.0f - x), -100.0f));
+}
+__global__ void __launch_bounds__(kNerfLossThreads)
+k_nerf_loss(NerfLossArgs A, float* __restrict__ pred, float* __restrict__ wsum_out, float* __restrict__ bgT_out, float* __restrict__ pred_bg,
+            unsigned long long* fx, float* acc, float* loss, float* terms) {
+    __shared__ float red[2][kNerfLossThreads / 32];
+    __shared__ bool last;
+    const int ray = blockIdx.x * blockDim.x + threadIdx.x;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    float v[2] = {0.f, 0.f};
+    if (ray < A.R) {
+        const RayRange rr = ray_range(ray, A.se, A.equal, A.fixed_n);
+        float col[3] = {0.f, 0.f, 0.f}, ws = 0.f, T_last = 1.0f;
+        if (rr.n > 0 && rr.end <= A.max_n) {
+            float sc[3], sh[3];
+            int img;
+            calib_of(A.C, ray, sc, sh, img);
+            float T = 1.0f;
+            for (int i = rr.start; i < rr.end; i++) {
+                const NerfAlpha na = nerf_alpha(A.density[i], A.dt[i]);
+                const float w = na.alpha * T;
+#pragma unroll
+                for (int k = 0; k < 3; k++) col[k] = fmaf(w, calib_sigmoid(A.x_raw[(size_t)i * 3 + k], sc[k], sh[k]), col[k]);
+                ws += w;
+                T_last = T;
+                T *= na.a;
+            }
+        }
+        float p[3];
 #pragma unroll
         for (int k = 0; k < 3; k++) {
-            if (fx && img < kDetImages) { fx_add(fx + img * 3 + k, gwd[k]); fx_add(fx + 3 * kDetImages + img * 3 + k, gb[k]); }
-            else { atomicAdd(g_wd + img * 3 + k, gwd[k]); atomicAdd(g_b + img * 3 + k, gb[k]); }
+            const float b = A.bg ? __fmul_rn(T_last, A.bg[(size_t)ray * 3 + k]) : 0.0f;
+            p[k] = __fadd_rn(col[k], b);
+            pred[(size_t)ray * 3 + k] = p[k];
+            if (pred_bg) pred_bg[(size_t)ray * 3 + k] = b;
+        }
+        wsum_out[ray] = ws;
+        bgT_out[ray] = T_last;
+        if (A.gt) {
+            if (A.hit[ray]) {
+#pragma unroll
+                for (int k = 0; k < 3; k++) { const float d = A.gt[(size_t)ray * 3 + k] - p[k]; v[0] = fmaf(d, d, v[0]); }
+            }
+            if (A.mask) v[1] = bce_term(fminf(fmaxf(ws, kBceLo), kBceHi), A.mask[ray]);
         }
     }
+    if (!A.gt) return;                       // render: no loss (grid-uniform)
+#pragma unroll
+    for (int q = 0; q < 2; q++) {
+        float t = v[q];
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) t += __shfl_xor_sync(0xffffffffu, t, o);
+        if (lane == 0) red[q][warp] = t;
+    }
+    __syncthreads();
+    if (threadIdx.x < 2) {
+        float t = 0.f;
+        for (int w = 0; w < kNerfLossThreads / 32; w++) t += red[threadIdx.x][w];
+        if (t != 0.0f) {
+            if (fx) fx_add(fx + threadIdx.x, t);
+            else atomicAdd(acc + threadIdx.x, t);
+        }
+    }
+    __threadfence();
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        const unsigned t = atomicAdd(reinterpret_cast<unsigned*>(acc + 2), 1u);
+        last = (t == gridDim.x - 1);
+    }
+    __syncthreads();
+    if (!last || threadIdx.x != 0) return;
+    __threadfence();
+    float sums[2];
+    if (fx) {
+        volatile unsigned long long* f = fx;
+        for (int q = 0; q < 2; q++) { sums[q] = (float)((double)(long long)f[q] / kFxScale); f[q] = 0ull; }
+    } else {
+        volatile float* a = acc;
+        for (int q = 0; q < 2; q++) sums[q] = a[q];
+    }
+    const float loss_rgb = sums[0] / (float)(3 * A.R), loss_mask = A.mask ? sums[1] / (float)A.R : 0.0f;
+    loss[0] = loss_rgb + loss_mask * A.mask_weight;
+    terms[0] = loss_rgb;
+    terms[1] = loss_mask;
+    for (int q = 0; q < 3; q++) acc[q] = 0.0f;        // ticket (acc[2], as bits) included: ready for the next launch
+}
+// d loss -> d x_raw [N,3], d density [N] (=, rows of the rays), d bg_rgb [R,3] (=) and the calibration gradients (+=):
+//     G = 2 (pred - gt) hit / (3R),  g_ws = mask_weight / R * (x - y) / max(x (1 - x), 1e-12) where 1e-3 <= x = weights_sum <= 1 - 1e-3,
+//     g_bgT = G . bg_rgb,  d / d alpha_i = G . (T_i c_i - S_i / a_i) + g_ws (T_i - Sw_i / a_i) - [i < n - 1] g_bgT bg_T / a_i
+__global__ void __launch_bounds__(kNerfLossThreads)
+k_nerf_loss_backward(NerfLossArgs A, const float* __restrict__ pred, const float* __restrict__ wsum, const float* __restrict__ bgT,
+                     float* __restrict__ g_x, float* __restrict__ g_density, float* __restrict__ g_bg, float* __restrict__ g_wd,
+                     float* __restrict__ g_b, unsigned long long* __restrict__ fx) {
+    const int ray = blockIdx.x * blockDim.x + threadIdx.x;
+    if (ray >= A.R) return;
+    const float c_rgb = 2.0f / (float)(3 * A.R);
+    float G[3];
+#pragma unroll
+    for (int k = 0; k < 3; k++) G[k] = A.hit[ray] ? c_rgb * (pred[(size_t)ray * 3 + k] - A.gt[(size_t)ray * 3 + k]) : 0.0f;
+    float g_ws = 0.0f;
+    if (A.mask) {
+        const float x = wsum[ray];
+        if (x >= kBceLo && x <= kBceHi) g_ws = A.mask_weight / (float)A.R * (x - A.mask[ray]) / fmaxf((1.0f - x) * x, 1e-12f);
+    }
+    const float bt = bgT[ray];
+    float g_bt = 0.0f;
+    if (A.bg) {
+#pragma unroll
+        for (int k = 0; k < 3; k++) {
+            const float b = A.bg[(size_t)ray * 3 + k];
+            g_bg[(size_t)ray * 3 + k] = G[k] * bt;
+            g_bt = fmaf(G[k], b, g_bt);
+        }
+    }
+    const RayRange rr = ray_range(ray, A.se, A.equal, A.fixed_n);
+    if (rr.n <= 0 || rr.end > A.max_n) return;
+    float sc[3], sh[3], tot[3] = {0.f, 0.f, 0.f}, gwd[3] = {0.f, 0.f, 0.f}, gb[3] = {0.f, 0.f, 0.f}, totw = 0.f;
+    int img;
+    calib_of(A.C, ray, sc, sh, img);
+    float T = 1.0f;
+    for (int i = rr.start; i < rr.end; i++) {
+        const NerfAlpha na = nerf_alpha(A.density[i], A.dt[i]);
+        const float w = na.alpha * T;
+#pragma unroll
+        for (int k = 0; k < 3; k++) tot[k] = fmaf(w, calib_sigmoid(A.x_raw[(size_t)i * 3 + k], sc[k], sh[k]), tot[k]);
+        totw += w;
+        T *= na.a;
+    }
+    T = 1.0f;
+    float pre[3] = {0.f, 0.f, 0.f}, prew = 0.f;
+    const float gb_last = g_bt * bt;
+    for (int i = rr.start; i < rr.end; i++) {
+        const NerfAlpha na = nerf_alpha(A.density[i], A.dt[i]);
+        const float w = na.alpha * T;
+        prew += w;
+        float ga = g_ws * (T - (totw - prew) / na.a);
+        if (i < rr.end - 1) ga -= gb_last / na.a;
+#pragma unroll
+        for (int k = 0; k < 3; k++) {
+            const float x = A.x_raw[(size_t)i * 3 + k];
+            const float c = calib_sigmoid(x, sc[k], sh[k]);
+            pre[k] = fmaf(w, c, pre[k]);
+            ga = fmaf(G[k], T * c - (tot[k] - pre[k]) / na.a, ga);
+            g_x[(size_t)i * 3 + k] = nerf_colour_backward(G[k], w, c, x, sc[k], gwd[k], gb[k]);
+        }
+        g_density[i] = ga * A.dt[i] * na.e;
+        T *= na.a;
+    }
+    add_calib_grads(img, gwd, gb, g_wd, g_b, fx);
 }
 
 int persistent_grid(int ntiles) {
@@ -491,6 +686,73 @@ int persistent_grid(int ntiles) {
 }
 
 #define ST ((cudaStream_t)stream)
+
+template <int D>
+int nerf_fused_forward(int N, int L, int T, const float* pos, const float* dirs, const float* lattice, const float* scale_factor,
+                       const float* shift, const float* window, float points_scaling, const uint8_t* blob, float* rgb_raw, float* density,
+                       void* stream) {
+    BgParams P;
+    int rc = make_bg_params(P, N, L, T, points_scaling);
+    if (rc != PSDF_OK) return rc;
+    if (N == 0) return PSDF_OK;
+    const size_t smem = (size_t)2 * kWTileBytes + kBgWBytes + sizeof(LevelC) + kBgNL * 128 * sizeof(float) + 64;
+    { static bool optin_[64]; psdf::psdf_optin_smem(k_bg_fused<D>, 227 * 1024, optin_); }
+    k_bg_fused<D><<<persistent_grid(div_up(N, kTile)), kRgbThreads, smem, ST>>>(P, pos, dirs, reinterpret_cast<const float2*>(lattice),
+                                                                               scale_factor, shift, window, blob, rgb_raw, density);
+    PSDF_CHECK_LAUNCH();
+    return PSDF_OK;
+}
+
+template <int D>
+int nerf_fused_backward(int N, int L, int T, const float* pos, const float* dirs, const float* lattice, const float* scale_factor,
+                        const float* shift, const float* window, float points_scaling, const uint8_t* blob, const float* g_rgb_raw,
+                        const float* g_density, float* grad_lattice, uint8_t* workspace, float* const* gw, float* const* gb, void* stream) {
+    BgParams P;
+    int rc = make_bg_params(P, N, L, T, points_scaling);
+    if (rc != PSDF_OK) return rc;
+    if (N == 0) return PSDF_OK;
+    const DetBufs* dbuf = det_buffers();
+    if (dbuf && (long long)L * T * 2 > dbuf->lattice_len) return PSDF_ERR_UNSUPPORTED;   // reserve more with psdf_set_deterministic
+    BgBwdOut out;
+    for (int l = 0; l < kBgNL; l++) { out.gW[l] = gw[l]; out.gbias[l] = gb[l]; }
+    out.fx_mlp = dbuf ? dbuf->rgb_mlp : nullptr;
+    const int ntiles = div_up(N, kTile);
+    out.xch = reinterpret_cast<float2*>(workspace);
+    out.xch_stride = ntiles * kTile;
+    const size_t smem = (size_t)4 * kWTileBytes + kBgWBytes + sizeof(LevelC) + kBgNL * 128 * (sizeof(float) + sizeof(unsigned long long)) + 64;
+    { static bool optin_[64]; psdf::psdf_optin_smem(k_bg_fused_backward<D>, 227 * 1024, optin_); }
+    k_bg_fused_backward<D><<<persistent_grid(ntiles), kRgbThreads, smem, ST>>>(P, pos, dirs, reinterpret_cast<const float2*>(lattice),
+                                                                              scale_factor, shift, window, blob, g_rgb_raw, g_density, out);
+    PSDF_CHECK_LAUNCH();
+    k_bg_lattice_scatter<D><<<dim3(div_up(out.xch_stride, kScatterThreads), L), kScatterThreads, 0, ST>>>(
+        P, pos, out.xch, out.xch_stride, scale_factor, shift, window, grad_lattice, dbuf ? dbuf->rgb_lattice : nullptr);
+    PSDF_CHECK_LAUNCH();
+    if (dbuf) {      // deterministic mode: fixed-point totals -> the float gradients (+=), 15 segments in two flushes
+        FxSegs F, Fb;
+        F.add(dbuf->rgb_lattice, grad_lattice, (long long)L * T * 2);
+        for (int l = 0; l < kBgNL; l++) {
+            F.add(dbuf->rgb_mlp + l * kFxW, gw[l], (long long)P.g.N[l] * P.g.K[l]);
+            Fb.add(dbuf->rgb_mlp + kFxB + l * kBgMaxCols, gb[l], P.g.N[l]);
+        }
+        if (fx_flush(F, ST) != 0 || fx_flush(Fb, ST) != 0) return PSDF_ERR_LAUNCH;
+    }
+    return PSDF_OK;
+}
+// the rows of N samples of pos_dim coordinates: 32-bit row and tile indexing
+inline bool nerf_rows_ok(int pos_dim, int N) { return (long long)N * pos_dim <= 0x7fffffffLL && (long long)N + kTile <= 0x7fffffffLL; }
+
+inline NerfLossArgs make_nerf_loss_args(int nr_rays, int max_nr_samples, const int* ray_start_end, int equal, int fixed_n, const float* x_raw,
+                                        const float* density, const float* dt, const int* img_idx, const float* weight_delta,
+                                        const float* bias, int fixed_img, const float* bg_rgb, const float* gt_rgb, const uint8_t* hit,
+                                        const float* gt_mask, float mask_weight) {
+    NerfLossArgs A;
+    A.R = nr_rays; A.max_n = max_nr_samples; A.se = ray_start_end; A.equal = equal != 0; A.fixed_n = fixed_n;
+    A.x_raw = x_raw; A.density = density; A.dt = dt;
+    A.C = {weight_delta ? img_idx : nullptr, weight_delta, bias, fixed_img};
+    A.bg = bg_rgb; A.gt = gt_rgb; A.hit = hit; A.mask = gt_mask; A.mask_weight = mask_weight;
+    return A;
+}
+
 }  // namespace
 
 extern "C" {
@@ -516,16 +778,16 @@ int psdf_bg_mlp_pack(int in_dim, const float* W0, const float* b0, const float* 
 int psdf_bg_fused_forward(int N, int L, int T, const float* pos, const float* dirs, const float* lattice, const float* scale_factor,
                           const float* shift, const float* window, float points_scaling, const uint8_t* blob, float* rgb_raw, float* density,
                           void* stream) {
-    BgParams P;
-    int rc = make_bg_params(P, N, L, T, points_scaling);
-    if (rc != PSDF_OK) return rc;
-    if (N == 0) return PSDF_OK;
-    const size_t smem = (size_t)2 * kWTileBytes + kBgWBytes + sizeof(LevelC) + kBgNL * 128 * sizeof(float) + 64;
-    { static bool optin_[64]; psdf::psdf_optin_smem(k_bg_fused, 227 * 1024, optin_); }
-    k_bg_fused<<<persistent_grid(div_up(N, kTile)), kRgbThreads, smem, ST>>>(P, pos, dirs, reinterpret_cast<const float2*>(lattice), scale_factor,
-                                                                            shift, window, blob, rgb_raw, density);
-    PSDF_CHECK_LAUNCH();
-    return PSDF_OK;
+    return nerf_fused_forward<4>(N, L, T, pos, dirs, lattice, scale_factor, shift, window, points_scaling, blob, rgb_raw, density, stream);
+}
+
+int psdf_nerf_fused_forward(int pos_dim, int N, int L, int T, const float* pos, const float* dirs, const float* lattice,
+                            const float* scale_factor, const float* shift, const float* window, float points_scaling, const uint8_t* blob,
+                            float* rgb_raw, float* density, void* stream) {
+    if (pos_dim != 3 && pos_dim != 4) return PSDF_ERR_UNSUPPORTED;
+    if (N < 0 || !nerf_rows_ok(pos_dim, N)) return PSDF_ERR_UNSUPPORTED;
+    return pos_dim == 3 ? nerf_fused_forward<3>(N, L, T, pos, dirs, lattice, scale_factor, shift, window, points_scaling, blob, rgb_raw, density, stream)
+                        : nerf_fused_forward<4>(N, L, T, pos, dirs, lattice, scale_factor, shift, window, points_scaling, blob, rgb_raw, density, stream);
 }
 
 // workspace: abar_0 of every level and sample slot (8 bytes each), sized for kMaxLevels so that the size depends on the sample count alone
@@ -539,38 +801,25 @@ int psdf_bg_fused_backward(int N, int L, int T, const float* pos, const float* d
                            const float* g_density, float* grad_lattice, uint8_t* workspace, float* gW0, float* gW1, float* gW2, float* gW3,
                            float* gW4, float* gW5, float* gW6, float* gb0, float* gb1, float* gb2, float* gb3, float* gb4, float* gb5,
                            float* gb6, void* stream) {
-    BgParams P;
-    int rc = make_bg_params(P, N, L, T, points_scaling);
-    if (rc != PSDF_OK) return rc;
-    if (N == 0) return PSDF_OK;
-    const DetBufs* dbuf = det_buffers();
-    if (dbuf && (long long)L * T * 2 > dbuf->lattice_len) return PSDF_ERR_UNSUPPORTED;   // reserve more with psdf_set_deterministic
     float* gw[kBgNL] = {gW0, gW1, gW2, gW3, gW4, gW5, gW6};
     float* gb[kBgNL] = {gb0, gb1, gb2, gb3, gb4, gb5, gb6};
-    BgBwdOut out;
-    for (int l = 0; l < kBgNL; l++) { out.gW[l] = gw[l]; out.gbias[l] = gb[l]; }
-    out.fx_mlp = dbuf ? dbuf->rgb_mlp : nullptr;
-    const int ntiles = div_up(N, kTile);
-    out.xch = reinterpret_cast<float2*>(workspace);
-    out.xch_stride = ntiles * kTile;
-    const size_t smem = (size_t)4 * kWTileBytes + kBgWBytes + sizeof(LevelC) + kBgNL * 128 * (sizeof(float) + sizeof(unsigned long long)) + 64;
-    { static bool optin_[64]; psdf::psdf_optin_smem(k_bg_fused_backward, 227 * 1024, optin_); }
-    k_bg_fused_backward<<<persistent_grid(ntiles), kRgbThreads, smem, ST>>>(P, pos, dirs, reinterpret_cast<const float2*>(lattice), scale_factor,
-                                                                           shift, window, blob, g_rgb_raw, g_density, out);
-    PSDF_CHECK_LAUNCH();
-    k_bg_lattice_scatter<<<dim3(div_up(out.xch_stride, kScatterThreads), L), kScatterThreads, 0, ST>>>(
-        P, pos, out.xch, out.xch_stride, scale_factor, shift, window, grad_lattice, dbuf ? dbuf->rgb_lattice : nullptr);
-    PSDF_CHECK_LAUNCH();
-    if (dbuf) {      // deterministic mode: fixed-point totals -> the float gradients (+=), 15 segments in two flushes
-        FxSegs F, Fb;
-        F.add(dbuf->rgb_lattice, grad_lattice, (long long)L * T * 2);
-        for (int l = 0; l < kBgNL; l++) {
-            F.add(dbuf->rgb_mlp + l * kFxW, gw[l], (long long)P.g.N[l] * P.g.K[l]);
-            Fb.add(dbuf->rgb_mlp + kFxB + l * kBgMaxCols, gb[l], P.g.N[l]);
-        }
-        if (fx_flush(F, ST) != 0 || fx_flush(Fb, ST) != 0) return PSDF_ERR_LAUNCH;
-    }
-    return PSDF_OK;
+    return nerf_fused_backward<4>(N, L, T, pos, dirs, lattice, scale_factor, shift, window, points_scaling, blob, g_rgb_raw, g_density,
+                                  grad_lattice, workspace, gw, gb, stream);
+}
+
+int psdf_nerf_fused_backward(int pos_dim, int N, int L, int T, const float* pos, const float* dirs, const float* lattice,
+                             const float* scale_factor, const float* shift, const float* window, float points_scaling, const uint8_t* blob,
+                             const float* g_rgb_raw, const float* g_density, float* grad_lattice, uint8_t* workspace, float* gW0, float* gW1,
+                             float* gW2, float* gW3, float* gW4, float* gW5, float* gW6, float* gb0, float* gb1, float* gb2, float* gb3,
+                             float* gb4, float* gb5, float* gb6, void* stream) {
+    if (pos_dim != 3 && pos_dim != 4) return PSDF_ERR_UNSUPPORTED;
+    if (N < 0 || !nerf_rows_ok(pos_dim, N)) return PSDF_ERR_UNSUPPORTED;
+    float* gw[kBgNL] = {gW0, gW1, gW2, gW3, gW4, gW5, gW6};
+    float* gb[kBgNL] = {gb0, gb1, gb2, gb3, gb4, gb5, gb6};
+    return pos_dim == 3 ? nerf_fused_backward<3>(N, L, T, pos, dirs, lattice, scale_factor, shift, window, points_scaling, blob, g_rgb_raw,
+                                                 g_density, grad_lattice, workspace, gw, gb, stream)
+                        : nerf_fused_backward<4>(N, L, T, pos, dirs, lattice, scale_factor, shift, window, points_scaling, blob, g_rgb_raw,
+                                                 g_density, grad_lattice, workspace, gw, gb, stream);
 }
 
 int psdf_nerf_bg_composite_forward(int nr_rays, int max_nr_samples, const int* ray_start_end, int equal, int fixed_n, const float* x_raw,
@@ -595,6 +844,49 @@ int psdf_nerf_bg_composite_backward(int nr_rays, int max_nr_samples, const int* 
     unsigned long long* fx = (dbuf && g_weight_delta) ? dbuf->neus : nullptr;
     k_bg_composite_backward<<<div_up(nr_rays, 128), 128, 0, ST>>>(nr_rays, max_nr_samples, ray_start_end, equal != 0, fixed_n, x_raw, density, dt,
                                                                   C, g_bg_rgb, g_x, g_density, g_weight_delta, g_bias, fx);
+    PSDF_CHECK_LAUNCH();
+    if (fx) {        // deterministic mode: fixed-point calibration totals -> the float gradients (+=)
+        FxSegs F;
+        F.add(dbuf->neus, g_weight_delta, 3 * kDetImages);
+        F.add(dbuf->neus + 3 * kDetImages, g_bias, 3 * kDetImages);
+        if (fx_flush(F, ST) != 0) return PSDF_ERR_LAUNCH;
+    }
+    return PSDF_OK;
+}
+
+int psdf_nerf_loss_forward(int nr_rays, int max_nr_samples, const int* ray_start_end, int equal, int fixed_n, const float* x_raw,
+                           const float* density, const float* dt, const int* img_idx, const float* weight_delta, const float* bias,
+                           int fixed_img, const float* bg_rgb, const float* gt_rgb, const uint8_t* hit, const float* gt_mask, float mask_weight,
+                           float* pred_rgb, float* weights_sum, float* bg_transmittance, float* pred_rgb_bg, float* acc, float* loss,
+                           float* terms, void* stream) {
+    if (nr_rays < 0 || !pred_rgb || !weights_sum || !bg_transmittance) return PSDF_ERR_ARG;
+    if (gt_rgb && (!hit || !acc || !loss || !terms)) return PSDF_ERR_ARG;
+    if (pred_rgb_bg && !bg_rgb) return PSDF_ERR_ARG;
+    if ((long long)nr_rays * 3 > 0x7fffffffLL) return PSDF_ERR_UNSUPPORTED;
+    if (nr_rays == 0) return gt_rgb ? PSDF_ERR_ARG : PSDF_OK;         // the mean over no rays is NaN in the reference
+    const NerfLossArgs A = make_nerf_loss_args(nr_rays, max_nr_samples, ray_start_end, equal, fixed_n, x_raw, density, dt, img_idx, weight_delta,
+                                               bias, fixed_img, bg_rgb, gt_rgb, hit, gt_mask, mask_weight);
+    const DetBufs* dbuf = det_buffers();
+    k_nerf_loss<<<div_up(nr_rays, kNerfLossThreads), kNerfLossThreads, 0, ST>>>(A, pred_rgb, weights_sum, bg_transmittance, pred_rgb_bg,
+                                                                                dbuf ? dbuf->loss + kNerfDetSlot : nullptr, acc, loss, terms);
+    PSDF_CHECK_LAUNCH();
+    return PSDF_OK;
+}
+
+int psdf_nerf_loss_backward(int nr_rays, int max_nr_samples, const int* ray_start_end, int equal, int fixed_n, const float* x_raw,
+                            const float* density, const float* dt, const int* img_idx, const float* weight_delta, const float* bias,
+                            int fixed_img, const float* bg_rgb, const float* gt_rgb, const uint8_t* hit, const float* gt_mask,
+                            float mask_weight, const float* pred_rgb, const float* weights_sum, const float* bg_transmittance, float* g_x,
+                            float* g_density, float* g_bg_rgb, float* g_weight_delta, float* g_bias, void* stream) {
+    if (nr_rays < 1 || !gt_rgb || !hit || !pred_rgb || !weights_sum || !bg_transmittance || !g_x || !g_density) return PSDF_ERR_ARG;
+    if (bg_rgb && !g_bg_rgb) return PSDF_ERR_ARG;
+    if ((long long)nr_rays * 3 > 0x7fffffffLL) return PSDF_ERR_UNSUPPORTED;
+    const NerfLossArgs A = make_nerf_loss_args(nr_rays, max_nr_samples, ray_start_end, equal, fixed_n, x_raw, density, dt, img_idx, weight_delta,
+                                               bias, fixed_img, bg_rgb, gt_rgb, hit, gt_mask, mask_weight);
+    const DetBufs* dbuf = det_buffers();
+    unsigned long long* fx = (dbuf && g_weight_delta) ? dbuf->neus : nullptr;
+    k_nerf_loss_backward<<<div_up(nr_rays, kNerfLossThreads), kNerfLossThreads, 0, ST>>>(A, pred_rgb, weights_sum, bg_transmittance, g_x,
+                                                                                         g_density, g_bg_rgb, g_weight_delta, g_bias, fx);
     PSDF_CHECK_LAUNCH();
     if (fx) {        // deterministic mode: fixed-point calibration totals -> the float gradients (+=)
         FxSegs F;

@@ -473,8 +473,9 @@ FusedRGB.train_forward = _fused_rgb_train_forward
 
 # ================================================================================================ fused background network
 class FusedNerfHash:
-    """models.NerfHash on the tensor cores (csrc/fused_bg.cu): 4-D encoding -> trunk (density) -> colour head, seven layers in one kernel
-    each way. Produces the linear colour (before calibration / sigmoid) and the density."""
+    """models.NerfHash on the tensor cores (csrc/fused_bg.cu): 3-D (foreground NeRF) or 4-D (NeRF++ background) encoding -> trunk
+    (density) -> colour head, seven layers in one kernel each way. Produces the linear colour (before calibration / sigmoid) and the
+    density."""
 
     def __init__(self, model_bg):
         self.model = model_bg
@@ -483,8 +484,9 @@ class FusedNerfHash:
         head = [m for m in model_bg.mlp_rgb if isinstance(m, torch.nn.Linear)]
         self.lin = trunk + head
         dims = [(l.in_features, l.out_features) for l in self.lin]
-        if enc.pos_dim != 4 or enc.nr_feat_per_level != 2 or not enc.concat_points or enc.nr_levels % 4 != 0:
-            raise RuntimeError("FusedNerfHash needs pos_dim 4, 2 features per level, concat_points and nr_levels % 4 == 0")
+        if enc.pos_dim not in (3, 4) or enc.nr_feat_per_level != 2 or not enc.concat_points or enc.nr_levels % 4 != 0:
+            raise RuntimeError("FusedNerfHash needs pos_dim 3 or 4, 2 features per level, concat_points and nr_levels % 4 == 0")
+        self.pos_dim = enc.pos_dim
         self.in_dim = enc.output_dims()
         want = [(self.in_dim, 64), (64, 64), (64, 64), (64, 65), (80, 64), (64, 64), (64, 3)]
         if dims != want:
@@ -513,8 +515,8 @@ class FusedNerfHash:
         N = pos.shape[0]
         rgb = torch.empty(N, 3, device=pos.device)
         density = torch.empty(N, 1, device=pos.device)
-        call("psdf_bg_fused_forward", N, enc.nr_levels, enc.capacity, pos, dirs, lattice.detach(), enc.scale_factor, enc.shift_tensor(), window,
-             enc.concat_points_scaling, self.blob, rgb, density)
+        call("psdf_nerf_fused_forward", self.pos_dim, N, enc.nr_levels, enc.capacity, pos, dirs, lattice.detach(), enc.scale_factor,
+             enc.shift_tensor(), window, enc.concat_points_scaling, self.blob, rgb, density)
         return rgb, density
 
     @torch.no_grad()
@@ -531,7 +533,7 @@ class FusedNerfHash:
 
 
 class _FusedNerfHashFn(torch.autograd.Function):
-    """forward: psdf_bg_fused_forward; backward: psdf_bg_fused_backward (reverse sweep + tensor-core dW, then the lattice scatter)"""
+    """forward: psdf_nerf_fused_forward; backward: psdf_nerf_fused_backward (reverse sweep + tensor-core dW, then the lattice scatter)"""
 
     @staticmethod
     def forward(ctx, pos, dirs, lattice, window, fb, *params):
@@ -561,8 +563,8 @@ class _FusedNerfHashFn(torch.autograd.Function):
             raise RuntimeError("FusedNerfHash: a parameter was modified in place between the forward and its backward")
         if fb.packed_versions != ctx.versions:
             fb.pack(params)
-        call("psdf_bg_fused_backward", N, enc.nr_levels, enc.capacity, pos, dirs, lattice.detach(), enc.scale_factor, enc.shift_tensor(),
-             window, enc.concat_points_scaling, fb.blob, g_rgb, g_density, g_lat, ws, *grads[0::2], *grads[1::2])
+        call("psdf_nerf_fused_backward", fb.pos_dim, N, enc.nr_levels, enc.capacity, pos, dirs, lattice.detach(), enc.scale_factor,
+             enc.shift_tensor(), window, enc.concat_points_scaling, fb.blob, g_rgb, g_density, g_lat, ws, *grads[0::2], *grads[1::2])
         if in_place:
             return (None,) * (5 + len(params))
         return (None, None, g_lat, None, None) + tuple(grads)
