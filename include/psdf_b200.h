@@ -29,6 +29,7 @@
 extern "C" {
 #endif
 
+/* changes when an existing entry point changes its signature or behaviour; entry points that are only added leave it as it is */
 #define PSDF_ABI_VERSION 1
 #define PSDF_ERR_ARG_ -1
 #define PSDF_ERR_LAUNCH_ -2
@@ -290,6 +291,25 @@ int psdf_sdf_fused_backward_multi(int L, int T, const float* lattice, const floa
                                   const float* g_sdf1, const float* g_grad1, const float* g_geom1, int N2, const float* pos2,
                                   const float* g_sdf2, const float* g_grad2, const float* g_geom2, float* grad_lattice, uint8_t* workspace,
                                   float* gW0, float* gW1, float* gW2, float* gW3, float* gb0, float* gb1, float* gb2, float* gb3, void* stream);
+/* ---------------------------------------------------------------- space-time SDF (SDF(in_channels=4, ...), train_4d_sdf.py:185)
+ * The fused SDF pair at either input width, pos_dim first; pos_dim 3 is psdf_sdf_fused_forward / psdf_sdf_fused_backward_multi, pos_dim 4
+ * takes space-time positions [N,4] (x, y, z, t) whose scale / shift rows have 4 columns. Both widths give 2L + 4 encoder columns (concat
+ * column 2L + 3 holds t * points_scaling), so the blob of psdf_sdf_mlp_pack serves both. grad / g_grad are [N,3] for both: the SPATIAL
+ * derivatives d sdf / d (x, y, z), which is all train_4d_sdf.py:212-217 reads of model.get_sdf_and_gradient (it keeps [:, 0:3] of the
+ * [N,4] gradient); the time derivative is not formed. The backward's tangent direction is (g_grad, 0). The workspace does not depend on
+ * pos_dim (psdf_sdf_fused_backward_multi_workspace_bytes). A pos_dim = 4 forward with grad always runs the two-group kernel (the
+ * lock-step variant of psdf_sdf_forward_variant is D = 3). Any other pos_dim: PSDF_ERR_UNSUPPORTED. Replaces
+ * model.get_sdf_and_gradient(points_time, iter_nr) (models.py:199-259) and loss.backward() through it (train_4d_sdf.py:212, 237). */
+int psdf_sdf_fused_forward_dim(int pos_dim, int N, int L, int T, const float* pos, const float* lattice, const float* scale_factor,
+                               const float* shift, const float* window, float points_scaling, int hidden, int out_dim, const uint8_t* blob,
+                               float* sdf, float* grad, float* geom, void* stream);
+int psdf_sdf_fused_backward_multi_dim(int pos_dim, int L, int T, const float* lattice, const float* scale_factor, const float* shift,
+                                      const float* window, float points_scaling, int hidden, int out_dim, const uint8_t* blob, int N0,
+                                      const float* pos0, const float* g_sdf0, const float* g_grad0, const float* g_geom0, int N1,
+                                      const float* pos1, const float* g_sdf1, const float* g_grad1, const float* g_geom1, int N2,
+                                      const float* pos2, const float* g_sdf2, const float* g_grad2, const float* g_geom2, float* grad_lattice,
+                                      uint8_t* workspace, float* gW0, float* gW1, float* gW2, float* gW3, float* gb0, float* gb1, float* gb2,
+                                      float* gb3, void* stream);
 long long psdf_rgb_fused_backward_workspace_bytes(int N);
 int psdf_rgb_fused_backward(int N, int L, int T, const float* pos, const float* dirs, const float* sdf_grad, const float* geom, int geom_dim,
                             const float* lattice, const float* scale_factor, const float* shift, const float* window, float points_scaling,
@@ -469,6 +489,12 @@ int psdf_sphere_fit_loss(int N, const float* pos, const float* sdf, const float*
  *   cloud: PSDF_ERR_UNSUPPORTED. */
 int psdf_surface_fit_points(int P, int Ns, int No, const float* pts, const float* nrm, const long long* idx, const float* u01,
                             const float box_size[3], const float box_translation[3], float* x, float* n, void* stream);
+/* points of one space-time iteration (train_4d_sdf.py:200-208): psdf_surface_fit_points with 4-column rows. x [Ns+No,4] = rows idx of the
+ * cloud pts [P,4] (x, y, z, t), then the box rows u01 [No,3] * size - size / 2 + translation followed by the time draw ut [No,1]
+ * (torch.cat([aabb.rand_points_inside(No), torch.rand(No, 1)], 1)); n [Ns,3] = rows idx of the normals nrm [P,3]. More than 2^31 - 1
+ * floats in x or in the cloud: PSDF_ERR_UNSUPPORTED. */
+int psdf_spacetime_fit_points(int P, int Ns, int No, const float* pts, const float* nrm, const long long* idx, const float* u01, const float* ut,
+                              const float box_size[3], const float box_translation[3], float* x, float* n, void* stream);
 /* sdf_loss (permuto_sdf_py/utils/sdf_utils.py:16-57, eik_clamp=None) times scale (train_sdf_from_mesh.py:135-136) in one launch over the
  * Ns surface rows followed by the No box rows of sdf [Ns+No], grad [Ns+No,3] (d sdf / d x), with the normals nrm [Ns,3]:
  *   loss = scale (w_eik mean_all |‖grad‖ - 1| + w_nrm mean_surf (1 - cos(grad, nrm)) + w_sdf mean_surf |sdf| + w_off mean_box exp(-100 |sdf|))

@@ -7,6 +7,7 @@ sphere-tracing hot path behind the reference's own Python operator API.
                                               reference's permuto_sdf_py runs unchanged (see INTEGRATION.md)
     permuto_sdf_b200.patch_reference_models   routes the reference's own SDF / RGB classes through the fused tensor-core kernels
     permuto_sdf_b200.SurfaceFit / AABB        SDF from an oriented point cloud (train_sdf_from_mesh.py) on the fused kernels
+    permuto_sdf_b200.SpaceTimeFit             space-time SDF from a point sequence (train_4d_sdf.py) on the fused kernels
     permuto_sdf_b200.NerfTrainer              NeRF training (train_nerf.py) on the fused kernels
 
 All device work goes through the C ABI in include/psdf_b200.h (libpsdf_b200.so, hand-written CUDA).
@@ -24,6 +25,9 @@ def __getattr__(name):
     if name == "SurfaceFit":
         from .surface_fit import SurfaceFit
         return SurfaceFit
+    if name == "SpaceTimeFit":
+        from .surface_fit import SpaceTimeFit
+        return SpaceTimeFit
     if name == "NerfTrainer":
         from .nerf_train import NerfTrainer
         return NerfTrainer

@@ -171,12 +171,15 @@ def call(name, *args):
 # launching stream. Kernel launches per entry point (the rest launch exactly one kernel):
 _KERNELS_PER_CALL = {"psdf_packed_compact_scan": 2, "psdf_vr_combine_uniform_samples_with_imp": 3,
                      "psdf_sdf_fused_backward": 2, "psdf_sdf_fused_backward_multi": 2,      # tensor-core kernel + lattice scatter
+                     "psdf_sdf_fused_backward_multi_dim": 2,
                      "psdf_bg_fused_backward": 2, "psdf_nerf_fused_backward": 2}
 
 
 _KERNELS_FN = {}        # entry point -> launches as a function of its arguments (none at present)
 _UNITS_FN = {"psdf_sdf_fused_forward_multi": lambda a: int(a[10]) + int(a[15]),
-             "psdf_sdf_fused_backward_multi": lambda a: int(a[10]) + int(a[15]) + int(a[20])}
+             "psdf_sdf_fused_forward_dim": lambda a: int(a[1]),
+             "psdf_sdf_fused_backward_multi": lambda a: int(a[10]) + int(a[15]) + int(a[20]),
+             "psdf_sdf_fused_backward_multi_dim": lambda a: int(a[11]) + int(a[16]) + int(a[21])}
 _STATS = None
 LAST_UNITS = {}        # {entry point: sum of its leading count argument} of the last stats window
 

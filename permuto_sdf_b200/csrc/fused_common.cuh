@@ -1,5 +1,5 @@
 // Shared pieces of the fused encoding + MLP kernels (fused_sdf.cu: forward / inference, fused_sdf_bwd.cu: training
-// backward, fused_rgb*.cu: colour network): MLP operand-blob geometry, permutohedral simplex helpers for D = 3, the encoder of
+// backward, fused_rgb*.cu: colour network): MLP operand-blob geometry, permutohedral simplex helpers for D = 3 and 4, the encoder of
 // one level and its lattice scatter, GELU and its derivatives, operand tile stores (bf16 hi/lo split in the core-matrix operand
 // layout) and the split-product GEMM issue.
 #pragma once
@@ -159,13 +159,17 @@ __device__ __forceinline__ void locate(const float* e, Simplex<D>& s) {
     s.bary[D + 1] = -R[0];
 }
 // tangent of the barycentric weights along the (scaled) direction dcf: the same rank scatter applied to its elevation
-__device__ __forceinline__ void bary_tangent3(const float* dcf, const Simplex3& s, float* db) {
-    float de[4], dD[4], sm = 0.f;
+template <int D>
+__device__ __forceinline__ void bary_tangent(const float* dcf, const Simplex<D>& s, float* db) {
+    constexpr float kInv = 1.0f / (float)(D + 1);
+    float de[D + 1], dD[D + 1], sm = 0.f;
 #pragma unroll
-    for (int i = 3; i > 0; i--) { de[i] = (sm - (float)i * dcf[i - 1]) * 0.25f; sm += dcf[i - 1]; }
-    de[0] = sm * 0.25f;
-    by_rank<3>(s, de, dD);
-    db[0] = dD[3] - dD[0]; db[1] = dD[2] - dD[3]; db[2] = dD[1] - dD[2]; db[3] = dD[0] - dD[1];
+    for (int i = D; i > 0; i--) { de[i] = (sm - (float)i * dcf[i - 1]) * kInv; sm += dcf[i - 1]; }
+    de[0] = sm * kInv;
+    by_rank<D>(s, de, dD);
+    db[0] = dD[D] - dD[0];
+#pragma unroll
+    for (int r = 1; r <= D; r++) db[r] = dD[D - r] - dD[D + 1 - r];
 }
 // h mod T without a division: q = umulhi(h, floor(2^32 / T)) is the quotient or one less, so one conditional subtraction finishes it
 // (exact for every 32-bit h; a power-of-two T needs no correction). `magic` = t_magic(T), computed on the host.
@@ -248,29 +252,47 @@ __device__ __forceinline__ float2 level_features(const float* x, const LevelC* l
     for (int r = 0; r <= D; r++) { const float wr = s.bary[r] * w; a0 = fmaf(v[r].x, wr, a0); a1 = fmaf(v[r].y, wr, a1); }
     return make_float2(a0, a1);
 }
-// d feat / d x_j (j = 0..2) of one level's two features: ft[j] = w scale_j / 4 * sum_i E[i][j] G_i, with G_i = u_{rank_i},
-// u_k = d feat / d D_k (by_rank) and E the elevation matrix rows {1,1,1},{-1,1,1},{0,-2,1},{0,0,-3}
-__device__ __forceinline__ void spatial_tangents(const Simplex3& s, const float2* v, float w, const float* scale3, float2* ft) {
-    float2 u[4], G[4];
-    u[0] = make_float2(v[3].x - v[0].x, v[3].y - v[0].y);
-    u[1] = make_float2(v[2].x - v[3].x, v[2].y - v[3].y);
-    u[2] = make_float2(v[1].x - v[2].x, v[1].y - v[2].y);
-    u[3] = make_float2(v[0].x - v[1].x, v[0].y - v[1].y);
+// d feat / d x_j (j = 0..2, the spatial coordinates) of one level's two features: ft[j] = w scale_j / (D+1) * sum_i E[i][j] G_i, with
+// G_i = u_{rank_i}, u_k = d feat / d D_k (by_rank) and E the (D+1) x D elevation matrix, rows {1,1,1,..},{-1,1,1,..},{0,-2,1,..},{0,0,-3,..},..;
+// E[i][j] = 0 for i > j + 1, so rows 0..3 suffice for j < 3 at any D
+template <int D, int K = 0>
+__device__ __forceinline__ float2 u_pick(const float2* u, int rk) {
+    if constexpr (K == D) return u[D];
+    else return rk == K ? u[K] : u_pick<D, K + 1>(u, rk);
+}
+template <int D>
+__device__ __forceinline__ void spatial_tangents(const Simplex<D>& s, const float2* v, float w, const float* scale, float2* ft) {
+    constexpr float kInv = 1.0f / (float)(D + 1);
+    float2 G[4];
+    if constexpr (D == 3) {
+        float2 u[4];
+        u[0] = make_float2(v[3].x - v[0].x, v[3].y - v[0].y);
+        u[1] = make_float2(v[2].x - v[3].x, v[2].y - v[3].y);
+        u[2] = make_float2(v[1].x - v[2].x, v[1].y - v[2].y);
+        u[3] = make_float2(v[0].x - v[1].x, v[0].y - v[1].y);
 #pragma unroll
-    for (int i = 0; i < 4; i++) {
-        const int rk = s.rank[i];
-        G[i].x = rk == 0 ? u[0].x : (rk == 1 ? u[1].x : (rk == 2 ? u[2].x : u[3].x));
-        G[i].y = rk == 0 ? u[0].y : (rk == 1 ? u[1].y : (rk == 2 ? u[2].y : u[3].y));
+        for (int i = 0; i < 4; i++) {
+            const int rk = s.rank[i];
+            G[i].x = rk == 0 ? u[0].x : (rk == 1 ? u[1].x : (rk == 2 ? u[2].x : u[3].x));
+            G[i].y = rk == 0 ? u[0].y : (rk == 1 ? u[1].y : (rk == 2 ? u[2].y : u[3].y));
+        }
+    } else {
+        float2 u[D + 1];
+        u[0] = make_float2(v[D].x - v[0].x, v[D].y - v[0].y);
+#pragma unroll
+        for (int k = 1; k <= D; k++) u[k] = make_float2(v[D - k].x - v[D + 1 - k].x, v[D - k].y - v[D + 1 - k].y);
+#pragma unroll
+        for (int i = 0; i < 4; i++) G[i] = u_pick<D>(u, s.rank[i]);
     }
-    const float c0 = 0.25f * w * scale3[0], c1 = 0.25f * w * scale3[1], c2 = 0.25f * w * scale3[2];
+    const float c0 = kInv * w * scale[0], c1 = kInv * w * scale[1], c2 = kInv * w * scale[2];
     const float s01x = G[0].x + G[1].x, s01y = G[0].y + G[1].y;
     ft[0] = make_float2(c0 * (G[0].x - G[1].x), c0 * (G[0].y - G[1].y));
     ft[1] = make_float2(c1 * fmaf(-2.0f, G[2].x, s01x), c1 * fmaf(-2.0f, G[2].y, s01y));
     ft[2] = make_float2(c2 * fmaf(-3.0f, G[3].x, s01x + G[2].x), c2 * fmaf(-3.0f, G[3].y, s01y + G[2].y));
 }
-// Operand core kc past the 2L lattice features: column 2L + d = x_d * points_scaling for d < 3 (and below in_dim), zero padding up to
-// Kp[0]. With NT tangents, column 2L + d of tangent j is dx[j][d] * points_scaling.
-template <int NT>
+// Operand core kc past the 2L lattice features: column 2L + d = x_d * points_scaling for d < D (and below in_dim), zero padding up to
+// Kp[0]. With NT tangents, column 2L + d of tangent j is dx[j][d] * points_scaling for the spatial d < 3 and zero for the time column.
+template <int NT, int D = 3>
 __device__ __forceinline__ void concat_core(const FusedParams& P, int kc, const float* x, const float (*dx)[3], float* fv, float (*ft)[8]) {
     const int c0 = 2 * P.L;
 #pragma unroll
@@ -280,11 +302,13 @@ __device__ __forceinline__ void concat_core(const FusedParams& P, int kc, const 
 #pragma unroll
         for (int j = 0; j < NT; j++) ft[j][i] = 0.f;
 #pragma unroll
-        for (int d = 0; d < 3; d++) {
+        for (int d = 0; d < D; d++) {
             if (c == d && (c0 + c) < P.in_dim) {
                 fv[i] = x[d] * P.points_scaling;
+                if (d < 3) {
 #pragma unroll
-                for (int j = 0; j < NT; j++) ft[j][i] = dx[j][d] * P.points_scaling;
+                    for (int j = 0; j < NT; j++) ft[j][i] = dx[j][d] * P.points_scaling;
+                }
             }
         }
     }
@@ -395,16 +419,15 @@ __device__ __forceinline__ void scatter2(float* gtab, unsigned long long* ftab, 
     else red_v2(gtab + (size_t)idx * 2, cv);
 }
 // Encoder backward of one sample at one level, called by a whole warp (one sample per lane):
-//     lattice[idx_r] += w (B_r abar + dB_r tabar),  r = 0..3,   abar = (a0, a1), tabar = (t0, t1) of the level's two features
+//     lattice[idx_r] += w (B_r abar + dB_r tabar),  r = 0..D,   abar = (a0, a1), tabar = (t0, t1) of the level's two features
 // x, v: position and tangent direction (D coordinates); scale3 / shift3: the level's scale and shift; gtab / ftab: the level's float /
 // fixed-point gradient table (scatter2). TAN = false: no tangent term (v, t0, t1 unused), lattice[idx_r] += w B_r abar. Invalid lanes add
 // nothing. aggregate: warp-uniform, sum the lanes that share a vertex first (match_any + add_peers2, one reduction per distinct vertex);
-// do_red = false issues no reduction (diagnostics, PSDF_EXPERIMENT_KNOCKOUT). The tangent term exists for D = 3 only.
+// do_red = false issues no reduction (diagnostics, PSDF_EXPERIMENT_KNOCKOUT).
 template <bool TAN, int D = 3>
 __device__ __forceinline__ void scatter_level(const float* x, const float* v, const float* scale3, const float* shift3, float w, float a0,
                                               float a1, float t0, float t1, bool valid, bool aggregate, bool do_red, int lane,
                                               unsigned cap_mask, unsigned T, float* gtab, unsigned long long* ftab) {
-    static_assert(D == 3 || !TAN, "the tangent term of the lattice scatter exists for D = 3 only");
     float cf[D], dcf[D], e[D + 1];
 #pragma unroll
     for (int i = 0; i < D; i++) {
@@ -415,7 +438,7 @@ __device__ __forceinline__ void scatter_level(const float* x, const float* v, co
     Simplex<D> s;
     locate<D>(e, s);
     float db[D + 2];
-    if constexpr (TAN) bary_tangent3(dcf, s, db);
+    if constexpr (TAN) bary_tangent<D>(dcf, s, db);
 #pragma unroll
     for (int r = 0; r <= D; r++) {
         unsigned idx = vindex<D>(s, r, cap_mask, T);

@@ -82,7 +82,8 @@ __device__ __forceinline__ void gelu_to_tiles(const float* acc, const float* bia
     }
 }
 
-template <bool TAN>
+// D = 3: positions [N,3]; D = 4: space-time positions [N,4] (x, y, z, t), value only (the tangent variants are D = 3)
+template <bool TAN, int D = 3>
 __global__ void __launch_bounds__(FwdCfg<TAN>::kThreads, FwdCfg<TAN>::kCtasPerSm)
 k_sdf_fused(FusedParams P, FwdSegs G, const float2* __restrict__ lattice, const float* __restrict__ scale,
             const float* __restrict__ shift, const float* __restrict__ window, const uint8_t* __restrict__ blob) {
@@ -101,7 +102,7 @@ k_sdf_fused(FusedParams P, FwdSegs G, const float2* __restrict__ lattice, const 
         umma::mbar_fence_init();
         if (TAN) umma::acc_attach(g_acc_tan + (size_t)blockIdx.x * kTile * (S * 64), S * 64);
     }
-    load_level_consts(lc, P.L, scale, shift, window, tid, kThreads);
+    load_level_consts<D>(lc, P.L, scale, shift, window, tid, kThreads);
     __syncthreads();
     if (tid == 0) {
         umma::mbar_expect_tx(&bars[0], (uint32_t)P.g.total);
@@ -121,9 +122,9 @@ k_sdf_fused(FusedParams P, FwdSegs G, const float2* __restrict__ lattice, const 
         float* __restrict__ sdf_out = seg1 ? G.sdf[1] : G.sdf[0];
         float* __restrict__ grad_out = seg1 ? G.grad[1] : G.grad[0];
         float* __restrict__ geom_out = seg1 ? G.geom[1] : G.geom[0];
-        float x[3];
+        float x[D];
 #pragma unroll
-        for (int i = 0; i < 3; i++) x[i] = valid ? pos[(size_t)n * 3 + i] : 0.0f;
+        for (int i = 0; i < D; i++) x[i] = valid ? pos[(size_t)n * D + i] : 0.0f;
 
         // ---------------- encoder: operand cores grp, grp+4, ... of this row
         for (int kc = grp; kc < all_cores; kc += kGroups) {
@@ -132,19 +133,19 @@ k_sdf_fused(FusedParams P, FwdSegs G, const float2* __restrict__ lattice, const 
 #pragma unroll
                 for (int q = 0; q < 4; q++) {
                     const int l = kc * 4 + q;
-                    Simplex3 s;
-                    float2 v[4];
-                    const float2 a = level_features(x, lc, l, lattice, P.T, P.cap_mask, s, v);
+                    Simplex<D> s;
+                    float2 v[D + 1];
+                    const float2 a = level_features<D>(x, lc, l, lattice, P.T, P.cap_mask, s, v);
                     fv[2 * q] = a.x; fv[2 * q + 1] = a.y;
                     if (TAN) {
                         float2 t[3];
-                        spatial_tangents(s, v, lc->window[l], lc->scale + l * 4, t);
+                        spatial_tangents<D>(s, v, lc->window[l], lc->scale + l * 4, t);
 #pragma unroll
                         for (int j = 0; j < 3; j++) { ft[j][2 * q] = t[j].x; ft[j][2 * q + 1] = t[j].y; }
                     }
                 }
             } else {
-                concat_core<TAN ? 3 : 0>(P, kc, x, kUnit3, fv, ft);
+                concat_core<TAN ? 3 : 0, D>(P, kc, x, kUnit3, fv, ft);
             }
             store8(s_a, s_a + kATileBytes, row, kc, fv);
             if (TAN) {
@@ -258,6 +259,8 @@ constexpr int kSubTileBytes = kSub * 64 * 2;    // one bf16 operand tile [64 x 6
 constexpr int kGroupThreads = 256;
 constexpr int kStg = 69;                         // row stride (floats) of the output staging tile: 64 value columns max + 3 gradient columns
 
+// D = 3: positions [N,3]; D = 4: space-time positions [N,4], whose three tangents are the spatial ones (d / d x, y, z)
+template <int D>
 __global__ void __launch_bounds__(2 * kGroupThreads, 1)
 k_sdf_fused_dual(FusedParams P, FwdSegs G, const float2* __restrict__ lattice, const float* __restrict__ scale,
                  const float* __restrict__ shift, const float* __restrict__ window, const uint8_t* __restrict__ blob) {
@@ -278,7 +281,7 @@ k_sdf_fused_dual(FusedParams P, FwdSegs G, const float2* __restrict__ lattice, c
         umma::mbar_init(&bars[3], 1);
         umma::mbar_fence_init();
     }
-    load_level_consts(lc, P.L, scale, shift, window, tid, 2 * kGroupThreads);
+    load_level_consts<D>(lc, P.L, scale, shift, window, tid, 2 * kGroupThreads);
     __syncthreads();
     if (tid == 0) {
         umma::mbar_expect_tx(&bars[0], (uint32_t)P.g.total);
@@ -306,9 +309,9 @@ k_sdf_fused_dual(FusedParams P, FwdSegs G, const float2* __restrict__ lattice, c
         float* __restrict__ geom_out = seg1 ? G.geom[1] : G.geom[0];
         const int n = (sub - sub0) * kSub + row;
         const bool valid = n < nseg;
-        float x[3];
+        float x[D];
 #pragma unroll
-        for (int i = 0; i < 3; i++) x[i] = valid ? pos[(size_t)n * 3 + i] : 0.0f;
+        for (int i = 0; i < D; i++) x[i] = valid ? pos[(size_t)n * D + i] : 0.0f;
 
         // ---------------- encoder: operand cores eg, eg + 4, ... of this row
         for (int kc = eg; kc < all_cores; kc += kEnc) {
@@ -317,16 +320,16 @@ k_sdf_fused_dual(FusedParams P, FwdSegs G, const float2* __restrict__ lattice, c
 #pragma unroll
                 for (int qq = 0; qq < 4; qq++) {
                     const int l = kc * 4 + qq;
-                    Simplex3 s;
-                    float2 v[4], t[3];
-                    const float2 a = level_features(x, lc, l, lattice, P.T, P.cap_mask, s, v);
-                    spatial_tangents(s, v, lc->window[l], lc->scale + l * 4, t);
+                    Simplex<D> s;
+                    float2 v[D + 1], t[3];
+                    const float2 a = level_features<D>(x, lc, l, lattice, P.T, P.cap_mask, s, v);
+                    spatial_tangents<D>(s, v, lc->window[l], lc->scale + l * 4, t);
                     fv[2 * qq] = a.x; fv[2 * qq + 1] = a.y;
 #pragma unroll
                     for (int j = 0; j < 3; j++) { ft[j][2 * qq] = t[j].x; ft[j][2 * qq + 1] = t[j].y; }
                 }
             } else {
-                concat_core<3>(P, kc, x, kUnit3, fv, ft);
+                concat_core<3, D>(P, kc, x, kUnit3, fv, ft);
             }
             store8(s_a, s_a + kSubTileBytes, row, kc, fv);
 #pragma unroll
@@ -700,6 +703,9 @@ int psdf_sdf_forward_variant(int variant) {
     return forward_dual_mode;
 }
 
+}  // extern "C"
+
+template <int D>
 static int launch_forward(int L, int T, const float* lattice, const float* scale_factor, const float* shift, const float* window,
                           float points_scaling, int hidden, int out_dim, const uint8_t* blob, int nseg, const int* Ns, const float* const* pos,
                           float* const* sdf, float* const* grad, float* const* geom, void* stream) {
@@ -708,7 +714,7 @@ static int launch_forward(int L, int T, const float* lattice, const float* scale
     P.L = L; P.T = T;
     P.cap_mask = t_magic(T);
     P.points_scaling = points_scaling;
-    P.in_dim = (L + 2) * 2;                       // D = 3, F = 2: E = 2 concat levels
+    P.in_dim = (L + 2) * 2;                       // D = 3 or 4, F = 2: E = 2 concat levels
     if (P.in_dim > 64) return PSDF_ERR_UNSUPPORTED;
     P.g = make_geom(P.in_dim, hidden, out_dim);
     FwdSegs G;
@@ -732,34 +738,38 @@ static int launch_forward(int L, int T, const float* lattice, const float* scale
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     const float2* lat = reinterpret_cast<const float2*>(lattice);
     // value + tangents: two independent 64-sample groups per CTA (k_sdf_fused_dual) unless psdf_sdf_forward_variant(0) chose the lock-step
-    // kernel
-    const bool dual = forward_dual_mode != 0;
+    // kernel, which exists for D = 3 only
+    const bool dual = forward_dual_mode != 0 || D != 3;
     if (tangents && dual) {
         FwdSegs H = G;
         int subs = 0;
         for (int i = 0; i < 2; i++) { H.tile0[i] = subs; subs += div_up(G.n[i], kSub); }
         H.tile0[2] = subs;
         size_t smem = (size_t)P.g.total + 2 * 4 * 2 * kSubTileBytes + sizeof(LevelC) + 64;
-        { static bool optin_[64]; psdf::psdf_optin_smem(k_sdf_fused_dual, 227 * 1024, optin_); }
-        k_sdf_fused_dual<<<min(min(div_up(subs, 2), sms), kAccCtas), 2 * kGroupThreads, smem, ST>>>(P, H, lat, scale_factor, shift, window, blob);
+        { static bool optin_[64]; psdf::psdf_optin_smem(k_sdf_fused_dual<D>, 227 * 1024, optin_); }
+        k_sdf_fused_dual<D><<<min(min(div_up(subs, 2), sms), kAccCtas), 2 * kGroupThreads, smem, ST>>>(P, H, lat, scale_factor, shift, window, blob);
     } else if (tangents) {
-        size_t smem = (size_t)P.g.total + 4 * 2 * kATileBytes + sizeof(LevelC) + 64;
-        { static bool optin_[64]; psdf::psdf_optin_smem(k_sdf_fused<true>, 227 * 1024, optin_); }
-        k_sdf_fused<true><<<min(min(tiles, sms), kAccCtas), kFusedThreads, smem, ST>>>(P, G, lat, scale_factor, shift, window, blob);
+        if constexpr (D == 3) {
+            size_t smem = (size_t)P.g.total + 4 * 2 * kATileBytes + sizeof(LevelC) + 64;
+            { static bool optin_[64]; psdf::psdf_optin_smem(k_sdf_fused<true>, 227 * 1024, optin_); }
+            k_sdf_fused<true><<<min(min(tiles, sms), kAccCtas), kFusedThreads, smem, ST>>>(P, G, lat, scale_factor, shift, window, blob);
+        }
     } else {
         size_t smem = (size_t)P.g.total + 2 * kATileBytes + sizeof(LevelC) + 64;
-        { static bool optin_[64]; psdf::psdf_optin_smem(k_sdf_fused<false>, 113 * 1024, optin_); }
-        k_sdf_fused<false><<<min(min(tiles, 2 * sms), 2 * kAccCtas), kValueThreads, smem, ST>>>(P, G, lat, scale_factor, shift, window, blob);
+        { static bool optin_[64]; psdf::psdf_optin_smem(k_sdf_fused<false, D>, 113 * 1024, optin_); }
+        k_sdf_fused<false, D><<<min(min(tiles, 2 * sms), 2 * kAccCtas), kValueThreads, smem, ST>>>(P, G, lat, scale_factor, shift, window, blob);
     }
     PSDF_CHECK_LAUNCH();
     return PSDF_OK;
 }
 
+extern "C" {
+
 int psdf_sdf_fused_forward(int N, int L, int T, const float* pos, const float* lattice, const float* scale_factor, const float* shift,
                            const float* window, float points_scaling, int hidden, int out_dim, const uint8_t* blob, float* sdf,
                            float* grad, float* geom, void* stream) {
     if (N < 0) return PSDF_ERR_UNSUPPORTED;
-    return launch_forward(L, T, lattice, scale_factor, shift, window, points_scaling, hidden, out_dim, blob, 1, &N, &pos, &sdf, &grad, &geom, stream);
+    return launch_forward<3>(L, T, lattice, scale_factor, shift, window, points_scaling, hidden, out_dim, blob, 1, &N, &pos, &sdf, &grad, &geom, stream);
 }
 
 // Two independent sample sets in ONE launch (the main samples of a training iteration and its off-surface points: 8 tiles more instead
@@ -772,7 +782,20 @@ int psdf_sdf_fused_forward_multi(int L, int T, const float* lattice, const float
     float* sdf[2] = {sdf0, sdf1};
     float* grad[2] = {grad0, grad1};
     float* geom[2] = {geom0, geom1};
-    return launch_forward(L, T, lattice, scale_factor, shift, window, points_scaling, hidden, out_dim, blob, 2, Ns, pos, sdf, grad, geom, stream);
+    return launch_forward<3>(L, T, lattice, scale_factor, shift, window, points_scaling, hidden, out_dim, blob, 2, Ns, pos, sdf, grad, geom, stream);
+}
+
+// psdf_sdf_fused_forward at either input width: pos [N, pos_dim], pos_dim 3 (psdf_sdf_fused_forward) or 4 (space-time positions; grad holds
+// the three spatial derivatives). A pos_dim = 4 launch with grad runs the two-group kernel whatever psdf_sdf_forward_variant chose.
+int psdf_sdf_fused_forward_dim(int pos_dim, int N, int L, int T, const float* pos, const float* lattice, const float* scale_factor,
+                               const float* shift, const float* window, float points_scaling, int hidden, int out_dim, const uint8_t* blob,
+                               float* sdf, float* grad, float* geom, void* stream) {
+    if (N < 0) return PSDF_ERR_UNSUPPORTED;
+    if (pos_dim == 3)
+        return launch_forward<3>(L, T, lattice, scale_factor, shift, window, points_scaling, hidden, out_dim, blob, 1, &N, &pos, &sdf, &grad, &geom, stream);
+    if (pos_dim == 4)
+        return launch_forward<4>(L, T, lattice, scale_factor, shift, window, points_scaling, hidden, out_dim, blob, 1, &N, &pos, &sdf, &grad, &geom, stream);
+    return PSDF_ERR_UNSUPPORTED;
 }
 
 

@@ -144,6 +144,8 @@ __device__ __forceinline__ void issue_dw_part(uint32_t tmem_d, const uint8_t* zs
     }
 }
 
+// D = 3: positions [N,3]; D = 4: space-time positions [N,4] with the tangent along (g_grad, 0) (g_grad holds spatial derivatives)
+template <int D>
 __global__ void __launch_bounds__(kBwdThreads, 1)
 k_sdf_fused_backward(FusedParams P, Segments S, const float2* __restrict__ lattice, const float* __restrict__ scale,
                      const float* __restrict__ shift, const float* __restrict__ window, const uint8_t* __restrict__ blob, BwdOut out) {
@@ -174,7 +176,7 @@ k_sdf_fused_backward(FusedParams P, Segments S, const float2* __restrict__ latti
         umma::mbar_fence_init();
         umma::acc_attach(g_acc_bwd + (size_t)blockIdx.x * kTile * 512, 512);
     }
-    load_level_consts(lc, P.L, scale, shift, window, tid, kBwdThreads);
+    load_level_consts<D>(lc, P.L, scale, shift, window, tid, kBwdThreads);
     for (int i = tid; i < kNL * 64; i += kBwdThreads) s_gb[i] = 0ull;     // also clears s_gbf
     __syncthreads();
     if (tid == 0) {
@@ -201,11 +203,11 @@ k_sdf_fused_backward(FusedParams P, Segments S, const float2* __restrict__ latti
         const float* __restrict__ g_grad = PSDF_SEG(g_grad);
         const float* __restrict__ g_geom = PSDF_SEG(g_geom);
 #undef PSDF_SEG
-        float x[3], v[3];
+        float x[D], v[3];
 #pragma unroll
-        for (int i = 0; i < 3; i++) {
-            x[i] = valid ? pos[(size_t)n * 3 + i] : 0.0f;
-            v[i] = (valid && g_grad) ? g_grad[(size_t)n * 3 + i] : 0.0f;
+        for (int i = 0; i < D; i++) {
+            x[i] = valid ? pos[(size_t)n * D + i] : 0.0f;
+            if (i < 3) v[i] = (valid && g_grad) ? g_grad[(size_t)n * 3 + i] : 0.0f;
         }
         if (g_geom) {
             // the tile's rows of the upstream geometric-feature gradient are contiguous: copy them with coalesced loads now (consumed by
@@ -224,21 +226,21 @@ k_sdf_fused_backward(FusedParams P, Segments S, const float2* __restrict__ latti
                 for (int q = 0; q < 4; q++) {
                     const int l = kc * 4 + q;
                     // directional tangent along v: the barycentric weights' tangent dB_r applied to the same vertex values
-                    float dcf[3], db[5];
+                    float dcf[D], db[D + 2];
 #pragma unroll
-                    for (int i = 0; i < 3; i++) dcf[i] = v[i] * lc->scale[l * 4 + i];
-                    Simplex3 s;
-                    float2 val[4];
-                    const float2 a = level_features(x, lc, l, lattice, P.T, P.cap_mask, s, val);
-                    bary_tangent3(dcf, s, db);
+                    for (int i = 0; i < D; i++) dcf[i] = i < 3 ? v[i] * lc->scale[l * 4 + i] : 0.0f;
+                    Simplex<D> s;
+                    float2 val[D + 1];
+                    const float2 a = level_features<D>(x, lc, l, lattice, P.T, P.cap_mask, s, val);
+                    bary_tangent<D>(dcf, s, db);
                     const float w = lc->window[l];
                     float t0 = 0.f, t1 = 0.f;
 #pragma unroll
-                    for (int r = 0; r < 4; r++) { const float cr = db[r] * w; t0 = fmaf(val[r].x, cr, t0); t1 = fmaf(val[r].y, cr, t1); }
+                    for (int r = 0; r <= D; r++) { const float cr = db[r] * w; t0 = fmaf(val[r].x, cr, t0); t1 = fmaf(val[r].y, cr, t1); }
                     fv[2 * q] = a.x; fv[2 * q + 1] = a.y; ft[0][2 * q] = t0; ft[0][2 * q + 1] = t1;
                 }
             } else {
-                concat_core<1>(P, kc, x, &v, fv, ft);
+                concat_core<1, D>(P, kc, x, &v, fv, ft);
             }
             store8(s_X, s_X + kATileBytes, row, kc, fv);
             store8(s_X + 2 * kATileBytes, s_X + 3 * kATileBytes, row, kc, ft[0]);
@@ -488,6 +490,7 @@ k_sdf_fused_backward(FusedParams P, Segments S, const float2* __restrict__ latti
 // 32 consecutive sample slots, i.e. the rows of one warp of the persistent kernel. The simplex and the barycentric tangent are
 // recomputed from the positions and upstream gradients.
 constexpr int kScatterThreads = 256;
+template <int D>
 __global__ void __launch_bounds__(kScatterThreads, 8)
 k_sdf_lattice_scatter(FusedParams P, Segments S, const float4* __restrict__ xch, int xch_stride, const float* __restrict__ scale,
                       const float* __restrict__ shift, const float* __restrict__ window, float* __restrict__ grad_lattice,
@@ -502,19 +505,19 @@ k_sdf_lattice_scatter(FusedParams P, Segments S, const float4* __restrict__ xch,
     const float* __restrict__ pos = PSDF_SEG(pos);
     const float* __restrict__ g_grad = PSDF_SEG(g_grad);
 #undef PSDF_SEG
-    float x[3], v[3], sc[3], sh[3];
+    float x[D], v[D], sc[D], sh[D];
 #pragma unroll
-    for (int i = 0; i < 3; i++) {
-        x[i] = valid ? pos[(size_t)n * 3 + i] : 0.0f;
-        v[i] = (valid && g_grad) ? g_grad[(size_t)n * 3 + i] : 0.0f;
-        sc[i] = scale[l * 3 + i];
-        sh[i] = shift ? shift[l * 3 + i] : 0.0f;
+    for (int i = 0; i < D; i++) {
+        x[i] = valid ? pos[(size_t)n * D + i] : 0.0f;
+        v[i] = (i < 3 && valid && g_grad) ? g_grad[(size_t)n * 3 + i] : 0.0f;
+        sc[i] = scale[l * D + i];
+        sh[i] = shift ? shift[l * D + i] : 0.0f;
     }
     const float w = window ? window[l] : 1.0f;
     const float4 a = xch[(size_t)l * xch_stride + slot];
     const bool aggregate = sc[0] < kAggregateBelowScale && !(P.knockout & 2);      // warp-uniform (l is)
     const bool do_red = !(P.knockout & 1);            // diagnostics (PSDF_EXPERIMENT_KNOCKOUT): bit 0 no atomics, bit 1 no aggregation
-    scatter_level<true>(x, v, sc, sh, w, a.x, a.y, a.z, a.w, valid, aggregate, do_red, lane, P.cap_mask, (unsigned)P.T,
+    scatter_level<true, D>(x, v, sc, sh, w, a.x, a.y, a.z, a.w, valid, aggregate, do_red, lane, P.cap_mask, (unsigned)P.T,
                   grad_lattice + (size_t)l * P.T * 2, fx_lattice ? fx_lattice + (size_t)l * P.T * 2 : nullptr);
 }
 
@@ -533,6 +536,9 @@ long long psdf_sdf_fused_backward_workspace_bytes(int N) {
     return (long long)ntiles * kWsTileBytes;
 }
 
+}  // extern "C"
+
+template <int D>
 static int launch_backward(int nseg, const int* Ns, const float* const* pos, const float* const* g_sdf, const float* const* g_grad,
                            const float* const* g_geom, int L, int T, const float* lattice, const float* scale_factor, const float* shift,
                            const float* window, float points_scaling, int hidden, int out_dim, const uint8_t* blob, float* grad_lattice,
@@ -588,12 +594,12 @@ static int launch_backward(int nseg, const int* Ns, const float* const* pos, con
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     const size_t smem = (size_t)P.g.total + 2 * kSetBytes + sizeof(LevelC) + kNL * 64 * sizeof(unsigned long long) + 64 + (size_t)kTile * (size_t)((out_dim - 1) | 1) * sizeof(float);
     if (smem > 227 * 1024) return PSDF_ERR_UNSUPPORTED;
-    { static bool optin_[64]; psdf::psdf_optin_smem(k_sdf_fused_backward, 227 * 1024, optin_); }
-    k_sdf_fused_backward<<<min(min(tiles, sms), kAccCtas), kBwdThreads, smem, ST>>>(P, S, reinterpret_cast<const float2*>(lattice), scale_factor, shift, window,
+    { static bool optin_[64]; psdf::psdf_optin_smem(k_sdf_fused_backward<D>, 227 * 1024, optin_); }
+    k_sdf_fused_backward<D><<<min(min(tiles, sms), kAccCtas), kBwdThreads, smem, ST>>>(P, S, reinterpret_cast<const float2*>(lattice), scale_factor, shift, window,
                                                                     blob, out);
     PSDF_CHECK_LAUNCH();
     if (timing) cudaEventRecord(ev[1], ST);
-    k_sdf_lattice_scatter<<<dim3(div_up(out.xch_stride, kScatterThreads), L), kScatterThreads, 0, ST>>>(
+    k_sdf_lattice_scatter<D><<<dim3(div_up(out.xch_stride, kScatterThreads), L), kScatterThreads, 0, ST>>>(
         P, S, out.xch, out.xch_stride, scale_factor, shift, window, grad_lattice, dbuf ? dbuf->sdf_lattice : nullptr);
     PSDF_CHECK_LAUNCH();
     if (timing) cudaEventRecord(ev[2], ST);
@@ -621,6 +627,8 @@ static int launch_backward(int nseg, const int* Ns, const float* const* pos, con
     return PSDF_OK;
 }
 
+extern "C" {
+
 // workspace of a multi-set launch: every set is padded to whole tiles
 long long psdf_sdf_fused_backward_multi_workspace_bytes(int N0, int N1, int N2) {
     return (long long)(div_up(N0 > 0 ? N0 : 0, kTile) + div_up(N1 > 0 ? N1 : 0, kTile) + div_up(N2 > 0 ? N2 : 0, kTile) + 1) * kWsTileBytes;
@@ -635,7 +643,7 @@ int psdf_sdf_fused_backward(int N, int L, int T, const float* pos, const float* 
     if (N == 0) return PSDF_OK;
     float* gW[kNL] = {gW0, gW1, gW2, gW3};
     float* gb[kNL] = {gb0, gb1, gb2, gb3};
-    return launch_backward(1, &N, &pos, &g_sdf, &g_grad, &g_geom, L, T, lattice, scale_factor, shift, window, points_scaling, hidden, out_dim, blob,
+    return launch_backward<3>(1, &N, &pos, &g_sdf, &g_grad, &g_geom, L, T, lattice, scale_factor, shift, window, points_scaling, hidden, out_dim, blob,
                            grad_lattice, workspace, gW, gb, stream);
 }
 
@@ -655,8 +663,33 @@ int psdf_sdf_fused_backward_multi(int L, int T, const float* lattice, const floa
     const float* gm[3] = {g_geom0, g_geom1, g_geom2};
     float* gW[kNL] = {gW0, gW1, gW2, gW3};
     float* gb[kNL] = {gb0, gb1, gb2, gb3};
-    return launch_backward(3, Ns, pos, gs, gg, gm, L, T, lattice, scale_factor, shift, window, points_scaling, hidden, out_dim, blob, grad_lattice,
-                           workspace, gW, gb, stream);
+    return launch_backward<3>(3, Ns, pos, gs, gg, gm, L, T, lattice, scale_factor, shift, window, points_scaling, hidden, out_dim, blob, grad_lattice,
+                              workspace, gW, gb, stream);
+}
+
+// psdf_sdf_fused_backward_multi at either input width: positions [N_i, pos_dim], pos_dim 3 (psdf_sdf_fused_backward_multi) or 4 (space-time
+// positions; g_grad [N_i,3] is the upstream gradient of the spatial derivatives, so the tangent direction is (g_grad, 0)). Same workspace.
+int psdf_sdf_fused_backward_multi_dim(int pos_dim, int L, int T, const float* lattice, const float* scale_factor, const float* shift,
+                                      const float* window, float points_scaling, int hidden, int out_dim, const uint8_t* blob, int N0,
+                                      const float* pos0, const float* g_sdf0, const float* g_grad0, const float* g_geom0, int N1,
+                                      const float* pos1, const float* g_sdf1, const float* g_grad1, const float* g_geom1, int N2,
+                                      const float* pos2, const float* g_sdf2, const float* g_grad2, const float* g_geom2, float* grad_lattice,
+                                      uint8_t* workspace, float* gW0, float* gW1, float* gW2, float* gW3, float* gb0, float* gb1, float* gb2,
+                                      float* gb3, void* stream) {
+    const int Ns[3] = {N0, N1, N2};
+    const float* pos[3] = {pos0, pos1, pos2};
+    const float* gs[3] = {g_sdf0, g_sdf1, g_sdf2};
+    const float* gg[3] = {g_grad0, g_grad1, g_grad2};
+    const float* gm[3] = {g_geom0, g_geom1, g_geom2};
+    float* gW[kNL] = {gW0, gW1, gW2, gW3};
+    float* gb[kNL] = {gb0, gb1, gb2, gb3};
+    if (pos_dim == 3)
+        return launch_backward<3>(3, Ns, pos, gs, gg, gm, L, T, lattice, scale_factor, shift, window, points_scaling, hidden, out_dim, blob,
+                                  grad_lattice, workspace, gW, gb, stream);
+    if (pos_dim == 4)
+        return launch_backward<4>(3, Ns, pos, gs, gg, gm, L, T, lattice, scale_factor, shift, window, points_scaling, hidden, out_dim, blob,
+                                  grad_lattice, workspace, gW, gb, stream);
+    return PSDF_ERR_UNSUPPORTED;
 }
 
 }  // extern "C"

@@ -1,6 +1,7 @@
-// SDF from an oriented point cloud (train_sdf_from_mesh.py:126-160), sm_90a. Two kernels replace the per-op chains of one iteration:
+// SDF from an oriented point cloud (train_sdf_from_mesh.py:126-160) or from a point sequence (train_4d_sdf.py:200-222), sm_90a. Two kernels
+// replace the per-op chains of one iteration:
 //   k_surface_fit_points   the iteration's points: index_select of the cloud (points + normals) and AABB.rand_points_inside
-//                          (aabb.py) from one uniform draw, into one contiguous [Ns + No, 3]                                      1 launch for ~8
+//                          (aabb.py) from one uniform draw, into one contiguous [Ns + No, D] (D = 4: plus the box rows' time draw)  1 launch for ~8
 //   k_surface_fit_loss     sdf_loss (sdf_utils.py:16-57, eik_clamp=None) over the Ns + No rows: the four means, the weighted total and
 //                          the seeds d loss / d {sdf, grad} with torch's autograd conventions                                       1 for ~40
 #include "common.cuh"
@@ -25,16 +26,19 @@ __device__ __forceinline__ float sign_f(float x) { return x > 0.0f ? 1.0f : (x <
 // ---------------------------------------------------------------------------------------------- points
 struct PointsArgs {
     int P, Ns, No;
-    const float* pts;              // [P,3]
+    const float* pts;              // [P,D]
     const float* nrm;              // [P,3]
     const long long* idx;          // [Ns]
     const float* u01;              // [No,3]
     float size[3], half[3], trans[3];
-    float* x;                      // [Ns + No, 3]: surface rows, then box rows
+    float* x;                      // [Ns + No, D]: surface rows, then box rows
     float* n;                      // [Ns, 3]
+    const float* ut;               // D = 4: [No] time column of the box rows
 };
 // Surface rows copy the drawn cloud rows (index_select); an index outside [0, P) gives a NaN row instead of reading out of bounds.
-// Box rows: u * size - size / 2 + translation, each operation rounded on its own as torch does (no contraction into an FMA).
+// Box rows: u * size - size / 2 + translation, each operation rounded on its own as torch does (no contraction into an FMA); at D = 4
+// followed by the time draw ut (torch.cat([box, ut], 1)).
+template <int D>
 __global__ void __launch_bounds__(kThreads)
 k_surface_fit_points(PointsArgs A) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -42,15 +46,16 @@ k_surface_fit_points(PointsArgs A) {
         const long long j = A.idx[i];
         const bool ok = j >= 0 && j < A.P;
 #pragma unroll
-        for (int k = 0; k < 3; k++) {
-            A.x[3 * i + k] = ok ? A.pts[3 * j + k] : __int_as_float(0x7fc00000);
-            A.n[3 * i + k] = ok ? A.nrm[3 * j + k] : __int_as_float(0x7fc00000);
+        for (int k = 0; k < D; k++) {
+            A.x[D * i + k] = ok ? A.pts[D * j + k] : __int_as_float(0x7fc00000);
+            if (k < 3) A.n[3 * i + k] = ok ? A.nrm[3 * j + k] : __int_as_float(0x7fc00000);
         }
     } else if (i < A.Ns + A.No) {
         const int r = i - A.Ns;
 #pragma unroll
         for (int k = 0; k < 3; k++)
-            A.x[3 * i + k] = __fadd_rn(__fsub_rn(__fmul_rn(A.u01[3 * r + k], A.size[k]), A.half[k]), A.trans[k]);
+            A.x[D * i + k] = __fadd_rn(__fsub_rn(__fmul_rn(A.u01[3 * r + k], A.size[k]), A.half[k]), A.trans[k]);
+        if constexpr (D == 4) A.x[D * i + 3] = A.ut[r];
     }
 }
 
@@ -149,6 +154,17 @@ k_surface_fit_loss(LossArgs A) {
 #pragma unroll
     for (int q = 0; q <= kSlots; q++) A.acc[q] = 0.0f;      // ticket (acc[4], as bits) included: ready for the next launch
 }
+PointsArgs points_args(int P, int Ns, int No, const float* pts, const float* nrm, const long long* idx, const float* u01,
+                       const float box_size[3], const float box_translation[3], float* x, float* n) {
+    PointsArgs A;
+    A.P = P; A.Ns = Ns; A.No = No; A.pts = pts; A.nrm = nrm; A.idx = idx; A.u01 = u01; A.x = x; A.n = n; A.ut = nullptr;
+    for (int k = 0; k < 3; k++) {
+        A.size[k] = box_size[k];
+        A.half[k] = box_size[k] / 2.0f;          // torch.as_tensor(size) / 2 in float32 (exact)
+        A.trans[k] = box_translation[k];
+    }
+    return A;
+}
 }  // namespace
 
 extern "C" {
@@ -162,14 +178,26 @@ int psdf_surface_fit_points(int P, int Ns, int No, const float* pts, const float
     if (rows * 3 > 0x7fffffffLL || (long long)P * 3 > 0x7fffffffLL) return PSDF_ERR_UNSUPPORTED;
     if (rows == 0) return PSDF_OK;
     if (!x) return PSDF_ERR_ARG;
-    PointsArgs A;
-    A.P = P; A.Ns = Ns; A.No = No; A.pts = pts; A.nrm = nrm; A.idx = idx; A.u01 = u01; A.x = x; A.n = n;
-    for (int k = 0; k < 3; k++) {
-        A.size[k] = box_size[k];
-        A.half[k] = box_size[k] / 2.0f;          // torch.as_tensor(size) / 2 in float32 (exact)
-        A.trans[k] = box_translation[k];
-    }
-    k_surface_fit_points<<<div_up((int)rows, kThreads), kThreads, 0, ST>>>(A);
+    PointsArgs A = points_args(P, Ns, No, pts, nrm, idx, u01, box_size, box_translation, x, n);
+    k_surface_fit_points<3><<<div_up((int)rows, kThreads), kThreads, 0, ST>>>(A);
+    PSDF_CHECK_LAUNCH();
+    return PSDF_OK;
+}
+
+// Points of one space-time iteration (train_4d_sdf.py:200-208), see k_surface_fit_points: cloud rows pts [P,4] (x, y, z, t), box rows from
+// u01 [No,3] and the time draw ut [No,1].
+int psdf_spacetime_fit_points(int P, int Ns, int No, const float* pts, const float* nrm, const long long* idx, const float* u01, const float* ut,
+                              const float box_size[3], const float box_translation[3], float* x, float* n, void* stream) {
+    if (Ns < 0 || No < 0 || P < 0 || !box_size || !box_translation || (Ns > 0 && (P < 1 || !pts || !nrm || !idx || !n)) ||
+        (No > 0 && (!u01 || !ut)))
+        return PSDF_ERR_ARG;
+    const long long rows = (long long)Ns + No;
+    if (rows * 4 > 0x7fffffffLL || (long long)P * 4 > 0x7fffffffLL) return PSDF_ERR_UNSUPPORTED;
+    if (rows == 0) return PSDF_OK;
+    if (!x) return PSDF_ERR_ARG;
+    PointsArgs A = points_args(P, Ns, No, pts, nrm, idx, u01, box_size, box_translation, x, n);
+    A.ut = ut;
+    k_surface_fit_points<4><<<div_up((int)rows, kThreads), kThreads, 0, ST>>>(A);
     PSDF_CHECK_LAUNCH();
     return PSDF_OK;
 }

@@ -4,6 +4,7 @@
 materialising encoded features or hidden activations in HBM. It is used where no parameter gradient is
 needed: SDF importance sampling, the occupancy-grid refresh, sphere tracing and normals. Training-time
 evaluations that need parameter gradients go through the differentiable modules (models.SDF).
+A space-time SDF (SDF(4, ...), positions (x, y, z, t)) is evaluated too; its gradient is the spatial one.
 """
 import torch
 
@@ -50,8 +51,9 @@ class FusedSDF:
         lin = [m for m in model_sdf.mlp_sdf if isinstance(m, torch.nn.Linear)]
         if len(lin) != 4:
             raise RuntimeError("FusedSDF supports the 4-linear-layer SDF MLP of the reference (models.py:153-161)")
-        if enc.pos_dim != 3 or enc.nr_feat_per_level != 2 or not enc.concat_points or enc.nr_levels % 4 != 0:
-            raise RuntimeError("FusedSDF needs pos_dim 3, 2 features per level, concat_points and nr_levels % 4 == 0")
+        if enc.pos_dim not in (3, 4) or enc.nr_feat_per_level != 2 or not enc.concat_points or enc.nr_levels % 4 != 0:
+            raise RuntimeError("FusedSDF needs pos_dim 3 or 4, 2 features per level, concat_points and nr_levels % 4 == 0")
+        self.pos_dim = enc.pos_dim
         self.lin = lin
         self.in_dim = lin[0].in_features
         self.hidden = lin[0].out_features
@@ -85,7 +87,12 @@ class FusedSDF:
     def train_forward(self, points, iter_nr):
         """differentiable (wrt lattice + MLP parameters) sdf, d sdf/dx, geom in two fused kernels (forward, backward).
         Equivalent to SDF.get_sdf_and_gradient(points, iter_nr) followed by loss.backward() through its double backward;
-        the gradient wrt `points` is not produced (it only matters for the 1e-4-scaled shift of the curvature loss)."""
+        the gradient wrt `points` is not produced (it only matters for the 1e-4-scaled shift of the curvature loss). pos_dim 3 only: the
+        space-time SDF's get_sdf_and_gradient returns the time derivative too ([N,4]), which the fused pair does not form."""
+        if self.pos_dim != 3:
+            raise RuntimeError("FusedSDF.train_forward: pos_dim %d; get_sdf_and_gradient of a space-time SDF returns the [N,4] gradient "
+                               "including d sdf / dt, which the fused pair does not form (SpaceTimeFit runs the fused kernels directly)"
+                               % self.pos_dim)
         if self._versions != self._cur_versions():
             self.repack()
         m = self.model
@@ -97,7 +104,9 @@ class FusedSDF:
 
     @torch.no_grad()
     def __call__(self, points, iter_nr, with_gradient=False, with_geom=True):
-        """-> (sdf [N,1], gradient [N,3] or None, geom_feat [N,out-1] or None)"""
+        """points [N, pos_dim] -> (sdf [N,1], gradient [N,3] or None, geom_feat [N,out-1] or None). For a space-time SDF (pos_dim 4,
+        points (x, y, z, t)) the gradient is the spatial one, d sdf / d (x, y, z): the first three columns of the reference's
+        get_sdf_and_gradient, all that train_4d_sdf.py reads of it."""
         if self._versions != self._cur_versions():
             self.repack()
         m, enc = self.model, self.model.encoding
@@ -109,7 +118,8 @@ class FusedSDF:
         grad = torch.empty(N, 3, device=dev) if with_gradient else None
         geom = torch.empty(N, self.out_dim - 1, device=dev) if (with_geom and self.out_dim > 1) else None
         window = m.window(iter_nr).view(-1).contiguous()
-        call("psdf_sdf_fused_forward", N, enc.nr_levels, enc.capacity, pts, enc.lattice_values.detach(), enc.scale_factor,
+        fwd = ("psdf_sdf_fused_forward",) if self.pos_dim == 3 else ("psdf_sdf_fused_forward_dim", self.pos_dim)
+        call(*fwd, N, enc.nr_levels, enc.capacity, pts, enc.lattice_values.detach(), enc.scale_factor,
              enc.shift_tensor(), window, enc.concat_points_scaling, self.hidden, self.out_dim, self.blob, sdf, grad, geom)
         return sdf, grad, geom
 
@@ -117,7 +127,10 @@ class FusedSDF:
 def _fused_sdf_sphere_trace(self, points, dirs, iter_nr, nr_iters, sdf_multiplier, sdf_converged_tresh, occupancy_grid=None):
     """sphere_trace's iteration loop (sdf_utils.py:150-200) in one kernel: -> (traced points [N,3], converged [N] bool).
     With an occupancy grid every step is followed by advance_sample_to_next_occupied_voxel, otherwise rays stop when they leave
-    the model's bounding sphere."""
+    the model's bounding sphere. pos_dim 3 only."""
+    if self.pos_dim != 3:
+        raise RuntimeError("FusedSDF.sphere_trace: pos_dim %d; the fused sphere tracer evaluates 3-D positions (a space-time SDF "
+                           "would need the time value and an AABB boundary)" % self.pos_dim)
     if self._versions != self._cur_versions():
         self.repack()
     m, enc = self.model, self.model.encoding

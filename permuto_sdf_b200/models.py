@@ -221,7 +221,13 @@ class SDF(torch.nn.Module, _Checkpointed):
         return self.fused
 
     def enable_fused_training(self, flag=True):
-        """get_sdf_and_gradient (autograd mode) through the fused forward/backward kernels"""
+        """get_sdf_and_gradient (autograd mode) through the fused forward/backward kernels. Not for a space-time SDF (in_channels 4):
+        its get_sdf_and_gradient returns d sdf / d (x, y, z, t), and the fused pair forms the spatial derivatives only; the per-op
+        autograd path keeps serving it (SpaceTimeFit runs the fused kernels directly)."""
+        D = self.encoding.pos_dim
+        if flag and D != 3:
+            raise RuntimeError("SDF.enable_fused_training: in_channels %d; get_sdf_and_gradient returns the [N,%d] gradient including "
+                               "d sdf / dt, which the fused kernels do not form (they give d sdf / d(x, y, z) only)" % (D, D))
         if getattr(self, "fused", None) is None:
             self.enable_fused_inference()
         self.fused_training = bool(flag)
