@@ -10,7 +10,7 @@
  *
  * Conventions
  *   - all pointers are DEVICE pointers (contiguous, fp32 / int32 / uint8 bool) unless the name ends in
- *     `[3]` (small host arrays passed by the caller); no allocation happens inside the library;
+ *     `[3]` or `[6]` (small host arrays passed by the caller); no allocation happens inside the library;
  *   - `stream` is a cudaStream_t; kernels are asynchronous on it; the library never synchronises;
  *   - return value: 0 = ok, <0 = error (PSDF_ERR_*); no global state: RNG state is passed explicitly
  *     as the (state, inc) pair of a pcg32 generator (kernels/permuto_sdf/pcg32.h:45-171). rng_inc == 0 (never a
@@ -57,6 +57,12 @@ int psdf_sphere_rand_points_inside(int n, float radius, const float* phi, const 
                                    void* stream);
 /* Sphere::check_point_inside_primitive, src/Sphere.cu:111-119 */
 int psdf_sphere_check_point_inside(int n, float radius, const float center[3], const float* points, uint8_t* out, void* stream);
+
+/* ---------------------------------------------------------------- AABB (permuto_sdf_py/utils/aabb.py:7-114) */
+/* AABB.ray_intersection, aabb.py:47-100, bit-identical to its torch ops: box of sizes[3] centred at translation[3]; -> entry points
+ * [N,3] and t [N], exit points [N,3] and t [N], hit [N] (misses: t = 0 at both ends); t_entry is clamped at 0 */
+int psdf_aabb_ray_intersection(int nr_rays, const float sizes[3], const float translation[3], const float* origins, const float* dirs,
+                               float* pts_entry, float* t_entry, float* pts_exit, float* t_exit, uint8_t* hit, void* stream);
 
 /* ---------------------------------------------------------------- OccupancyGrid (include/permuto_sdf/OccupancyGrid.cuh:19-64) */
 /* compute_grid_points (idx==NULL, n==V^3) / compute_random_sample_of_grid_points (idx = chosen voxels),
@@ -254,6 +260,17 @@ int psdf_sdf_sphere_trace(int N, int L, int T, const float* pos, const float* di
                           int nr_iters, float sdf_multiplier, float sdf_converged_tresh, const uint8_t* occupancy, int V, float extent,
                           const float trans[3], float sphere_radius, const float sphere_center[3], float* pos_out, uint8_t* converged,
                           int* queue_counter, void* stream);
+/* psdf_sdf_sphere_trace at either input width and with either boundary primitive (sphere_trace with occupancy_grid and time_val,
+ * sdf_utils.py:120-218). pos_dim 3, or 4: the network input is (x, y, z, time_val), time_val one fp32 per launch; positions, directions
+ * and steps stay 3-D. boundary_kind 0: bounding sphere, boundary = {radius, centre x, y, z, -, -}; 1: box (AABB.check_point_inside_primitive,
+ * aabb.py:28-43), boundary = {max bounds x, y, z, translation x, y, z}, a point is inside when min < p - t < max per coordinate with
+ * min = -max. The occupancy grid, when given, replaces the boundary test as in psdf_sdf_sphere_trace. Other arguments as there;
+ * psdf_sdf_sphere_trace is the (3, sphere) case. Returns PSDF_ERR_UNSUPPORTED for another pos_dim or boundary_kind. */
+int psdf_sdf_sphere_trace_dim(int pos_dim, float time_val, int boundary_kind, const float boundary[6], int N, int L, int T, const float* pos,
+                              const float* dirs, const float* lattice, const float* scale_factor, const float* shift, const float* window,
+                              float points_scaling, int hidden, int out_dim, const uint8_t* blob, int nr_iters, float sdf_multiplier,
+                              float sdf_converged_tresh, const uint8_t* occupancy, int V, float extent, const float trans[3],
+                              float* pos_out, uint8_t* converged, int* queue_counter, void* stream);
 /* Training backward of psdf_sdf_fused_forward (double backward of encoding + MLP on the tensor cores, weight gradients formed on
  * chip; the lattice scatter is a second kernel at full occupancy):
  * upstream gradients g_sdf [N], g_grad [N,3], g_geom [N,out_dim-1] (any may be NULL) -> grad_lattice (+=), weight gradients

@@ -36,13 +36,13 @@ def _parse_header(path=HEADER):
         if args and args != "void":
             for a in args.split(","):
                 a = a.strip()
-                m = re.match(r"(const\s+)?([\w ]+?)\s*(\*?)\s*(\w+)(\[3\])?$", a)
+                m = re.match(r"(const\s+)?([\w ]+?)\s*(\*?)\s*(\w+)(\[\d+\])?$", a)
                 if not m:
                     raise RuntimeError("cannot parse argument %r of %s" % (a, name))
                 const, base, ptr, aname, arr = m.groups()
                 base = base.strip()
                 if arr:
-                    kind = "float3"
+                    kind = "float" + arr           # small host array, e.g. float[3]
                 elif ptr:
                     kind = "void*" if base == "void" else "ptr:" + base
                 else:
@@ -78,8 +78,8 @@ def load_library(path=LIB_PATH):
         fn.restype = _CTYPES[ret]
         at = []
         for _, kind in args:
-            if kind == "float3":
-                at.append(ctypes.c_float * 3)
+            if kind.startswith("float["):
+                at.append(ctypes.c_float * int(kind[6:-1]))
             elif kind.startswith("ptr:") or kind == "void*":
                 at.append(ctypes.c_void_p)
             else:
@@ -103,7 +103,7 @@ def _dtypes():
 
 def call(name, *args):
     """Invoke a C-ABI entry point. torch tensors are passed as device pointers (checked: CUDA, contiguous,
-    dtype); None -> NULL; 3-sequences -> float[3]; the trailing `stream` argument is filled in automatically
+    dtype); None -> NULL; n-sequences -> float[n]; the trailing `stream` argument is filled in automatically
     with torch's current stream when omitted."""
     import torch
     lib = load_library()
@@ -134,8 +134,9 @@ def call(name, *args):
                 conv.append(a.data_ptr())
             else:
                 conv.append(int(a))
-        elif kind == "float3":
-            conv.append((ctypes.c_float * 3)(float(a[0]), float(a[1]), float(a[2])))
+        elif kind.startswith("float["):
+            n = int(kind[6:-1])
+            conv.append((ctypes.c_float * n)(*[float(a[i]) for i in range(n)]))
         elif kind == "void*":
             conv.append(a)
         elif kind == "float":
@@ -178,6 +179,7 @@ _KERNELS_PER_CALL = {"psdf_packed_compact_scan": 2, "psdf_vr_combine_uniform_sam
 _KERNELS_FN = {}        # entry point -> launches as a function of its arguments (none at present)
 _UNITS_FN = {"psdf_sdf_fused_forward_multi": lambda a: int(a[10]) + int(a[15]),
              "psdf_sdf_fused_forward_dim": lambda a: int(a[1]),
+             "psdf_sdf_sphere_trace_dim": lambda a: int(a[4]),
              "psdf_sdf_fused_backward_multi": lambda a: int(a[10]) + int(a[15]) + int(a[20]),
              "psdf_sdf_fused_backward_multi_dim": lambda a: int(a[11]) + int(a[16]) + int(a[21])}
 _STATS = None

@@ -433,6 +433,10 @@ k_sdf_fused_dual(FusedParams P, FwdSegs G, const float2* __restrict__ lattice, c
 // iteration is encoder -> 4 tensor-core layers -> step / occupancy advance, the weights stay resident, and a tile stops as soon
 // as its 128 rays have converged. Per ray the arithmetic is the one of the loop (same network evaluation, p + (d * sdf) * mult in
 // separate roundings, same DDA), so the traced points are bit-identical to it.
+// Template on the network's input width D and the boundary primitive. D = 4 is the space-time SDF traced at one time value
+// (train_4d_sdf.py:268, vis_4d_sdf.py:105: the loop concatenates a column filled with time_val before every model call); positions,
+// directions, the step and the boundary test stay 3-D and only the encoder sees the fourth coordinate. BOX replaces the bounding-sphere
+// test with AABB.check_point_inside_primitive (aabb.py:28-43). <3, false> is the original kernel.
 struct TraceParams {
     int nr_iters;
     float sdf_mult, conv_thresh;
@@ -440,11 +444,18 @@ struct TraceParams {
     psdf::GridGeom grid;
     float sph_radius, sph_cx, sph_cy, sph_cz;
 };
+// what the original kernel does not read: the time value (D = 4) and the box (BOX), as the fp32 values the reference compares against
+// (p - t < max, p - t > min, min = -max). A separate, last kernel argument: the original kernel's arguments keep their offsets.
+struct TraceExt {
+    float time_val;
+    float box_max[3], box_min[3], box_t[3];
+};
+template <int D, bool BOX>
 __global__ void __launch_bounds__(kValueThreads, 2)
 k_sdf_sphere_trace(FusedParams P, TraceParams Q, const float* __restrict__ pos_in, const float* __restrict__ dirs,
                    const float2* __restrict__ lattice, const float* __restrict__ scale, const float* __restrict__ shift,
                    const float* __restrict__ window, const uint8_t* __restrict__ blob, const uint8_t* __restrict__ occ,
-                   float* __restrict__ pos_out, uint8_t* __restrict__ converged_out, int* __restrict__ queue) {
+                   float* __restrict__ pos_out, uint8_t* __restrict__ converged_out, int* __restrict__ queue, TraceExt X) {
     // Persistent CTAs over a global ray queue: a CTA owns 128 ray SLOTS; a slot whose ray has finished (converged, left the occupied
     // region, or used its nr_iters evaluations) writes its result and is refilled with the next unclaimed ray (one warp-aggregated
     // atomicAdd per warp and iteration), so every network evaluation runs on a full tile until the frame is drained. Per ray the
@@ -471,7 +482,7 @@ k_sdf_sphere_trace(FusedParams P, TraceParams Q, const float* __restrict__ pos_i
         umma::mbar_fence_init();
         s_flag[0] = 0;
     }
-    load_level_consts(lc, P.L, scale, shift, window, tid, kValueThreads);
+    load_level_consts<D>(lc, P.L, scale, shift, window, tid, kValueThreads);
     __syncthreads();
     if (tid == 0) {
         umma::mbar_expect_tx(&bars[0], (uint32_t)P.g.total);
@@ -508,7 +519,10 @@ k_sdf_sphere_trace(FusedParams P, TraceParams Q, const float* __restrict__ pos_i
         if (__syncthreads_count(occupied) == 0) break;       // no ray left in this tile (and the queue is drained)
         const int nact = __syncthreads_count(active);
         evaluations += nact / kGroups;
-        float x[3] = {s_pos[row * 3], s_pos[row * 3 + 1], s_pos[row * 3 + 2]};
+        float x[D];
+#pragma unroll
+        for (int i = 0; i < 3; i++) x[i] = s_pos[row * 3 + i];
+        if constexpr (D == 4) x[3] = X.time_val;
         const bool run_net = nact > 0 && Q.nr_iters > 0;      // uniform
         rounds++;
         net_rounds += run_net ? 1 : 0;
@@ -518,13 +532,13 @@ k_sdf_sphere_trace(FusedParams P, TraceParams Q, const float* __restrict__ pos_i
                 if (kc < level_cores) {
 #pragma unroll
                     for (int q = 0; q < 4; q++) {
-                        Simplex3 s;
-                        float2 v[4];
-                        const float2 a = level_features(x, lc, kc * 4 + q, lattice, P.T, P.cap_mask, s, v);
+                        Simplex<D> s;
+                        float2 v[D + 1];
+                        const float2 a = level_features<D>(x, lc, kc * 4 + q, lattice, P.T, P.cap_mask, s, v);
                         fv[2 * q] = a.x; fv[2 * q + 1] = a.y;
                     }
                 } else {
-                    concat_core<0>(P, kc, x, nullptr, fv, nullptr);
+                    concat_core<0, D>(P, kc, x, nullptr, fv, nullptr);
                 }
                 store8(s_a, s_a + kATileBytes, row, kc, fv);
             }
@@ -575,6 +589,11 @@ k_sdf_sphere_trace(FusedParams P, TraceParams Q, const float* __restrict__ pos_i
                             if (active) { s_pos[row * 3] = px; s_pos[row * 3 + 1] = py; s_pos[row * 3 + 2] = pz; }
                             s_mt[row] = t; s_ms[row] = steps; s_new[row] = newly ? 1 : 0;
                         } else within = (st == 1);
+                    } else if constexpr (BOX) {
+                        const float q[3] = {__fsub_rn(px, X.box_t[0]), __fsub_rn(py, X.box_t[1]), __fsub_rn(pz, X.box_t[2])};
+                        within = true;
+#pragma unroll
+                        for (int i = 0; i < 3; i++) within = within && q[i] < X.box_max[i] && q[i] > X.box_min[i];
                     } else {
                         const float qx = __fsub_rn(px, Q.sph_cx), qy = __fsub_rn(py, Q.sph_cy), qz = __fsub_rn(pz, Q.sph_cz);
                         within = sqrtf(__fadd_rn(__fadd_rn(__fmul_rn(qx, qx), __fmul_rn(qy, qy)), __fmul_rn(qz, qz))) < Q.sph_radius;
@@ -630,13 +649,13 @@ k_sdf_sphere_trace(FusedParams P, TraceParams Q, const float* __restrict__ pos_i
 #define ST ((cudaStream_t)stream)
 }  // namespace
 
-extern "C" {
-
-int psdf_sdf_sphere_trace(int N, int L, int T, const float* pos, const float* dirs, const float* lattice, const float* scale_factor,
-                          const float* shift, const float* window, float points_scaling, int hidden, int out_dim, const uint8_t* blob,
-                          int nr_iters, float sdf_multiplier, float sdf_converged_tresh, const uint8_t* occupancy, int V, float extent,
-                          const float trans[3], float sphere_radius, const float sphere_center[3], float* pos_out, uint8_t* converged,
-                          int* queue_counter, void* stream) {
+// the launch of k_sdf_sphere_trace<D, BOX> (psdf_sdf_sphere_trace, psdf_sdf_sphere_trace_dim)
+template <int D, bool BOX>
+static int launch_trace(const TraceExt& X, int N, int L, int T, const float* pos, const float* dirs, const float* lattice,
+                        const float* scale_factor, const float* shift, const float* window, float points_scaling, int hidden, int out_dim,
+                        const uint8_t* blob, int nr_iters, float sdf_multiplier, float sdf_converged_tresh, const uint8_t* occupancy, int V,
+                        float extent, const float trans[3], float sphere_radius, const float sphere_center[3], float* pos_out,
+                        uint8_t* converged, int* queue_counter, void* stream) {
     if (!queue_counter) return PSDF_ERR_ARG;
     if (N < 0 || L < 1 || L > kMaxLevels || (L % 4) != 0 || hidden > 64 || hidden % 16 != 0 || out_dim > 64 || nr_iters < 0)
         return PSDF_ERR_UNSUPPORTED;
@@ -658,12 +677,47 @@ int psdf_sdf_sphere_trace(int N, int L, int T, const float* pos, const float* di
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     const size_t smem = (size_t)P.g.total + 2 * kATileBytes + sizeof(LevelC) + kTile * 12 * sizeof(float) + 80;
-    { static bool optin_[64]; psdf::psdf_optin_smem(k_sdf_sphere_trace, 227 * 1024, optin_); }
+    { static bool optin_[64]; psdf::psdf_optin_smem(k_sdf_sphere_trace<D, BOX>, 227 * 1024, optin_); }
     const int ntiles = div_up(N, kTile);
-    k_sdf_sphere_trace<<<min(min(ntiles, 2 * sms), 2 * kAccCtas), kValueThreads, smem, ST>>>(P, Q, pos, dirs, reinterpret_cast<const float2*>(lattice), scale_factor,
-                                                                     shift, window, blob, occupancy, pos_out, converged, queue_counter);
+    k_sdf_sphere_trace<D, BOX><<<min(min(ntiles, 2 * sms), 2 * kAccCtas), kValueThreads, smem, ST>>>(P, Q, pos, dirs, reinterpret_cast<const float2*>(lattice), scale_factor,
+                                                                     shift, window, blob, occupancy, pos_out, converged, queue_counter, X);
     PSDF_CHECK_LAUNCH();
     return PSDF_OK;
+}
+
+extern "C" {
+
+int psdf_sdf_sphere_trace(int N, int L, int T, const float* pos, const float* dirs, const float* lattice, const float* scale_factor,
+                          const float* shift, const float* window, float points_scaling, int hidden, int out_dim, const uint8_t* blob,
+                          int nr_iters, float sdf_multiplier, float sdf_converged_tresh, const uint8_t* occupancy, int V, float extent,
+                          const float trans[3], float sphere_radius, const float sphere_center[3], float* pos_out, uint8_t* converged,
+                          int* queue_counter, void* stream) {
+    TraceExt X = {};
+    return launch_trace<3, false>(X, N, L, T, pos, dirs, lattice, scale_factor, shift, window, points_scaling, hidden, out_dim, blob, nr_iters,
+                                  sdf_multiplier, sdf_converged_tresh, occupancy, V, extent, trans, sphere_radius, sphere_center, pos_out,
+                                  converged, queue_counter, stream);
+}
+
+int psdf_sdf_sphere_trace_dim(int pos_dim, float time_val, int boundary_kind, const float boundary[6], int N, int L, int T, const float* pos,
+                              const float* dirs, const float* lattice, const float* scale_factor, const float* shift, const float* window,
+                              float points_scaling, int hidden, int out_dim, const uint8_t* blob, int nr_iters, float sdf_multiplier,
+                              float sdf_converged_tresh, const uint8_t* occupancy, int V, float extent, const float trans[3],
+                              float* pos_out, uint8_t* converged, int* queue_counter, void* stream) {
+    if ((pos_dim != 3 && pos_dim != 4) || (boundary_kind != 0 && boundary_kind != 1)) return PSDF_ERR_UNSUPPORTED;
+    if (!boundary) return PSDF_ERR_ARG;
+    TraceExt X = {};
+    X.time_val = time_val;
+    float radius = 0.f, center[3] = {0.f, 0.f, 0.f};
+    if (boundary_kind == 0) {
+        radius = boundary[0];
+        for (int i = 0; i < 3; i++) center[i] = boundary[1 + i];
+    } else {
+        for (int i = 0; i < 3; i++) { X.box_max[i] = boundary[i]; X.box_min[i] = -boundary[i]; X.box_t[i] = boundary[3 + i]; }
+    }
+    auto launch = pos_dim == 3 ? (boundary_kind ? launch_trace<3, true> : launch_trace<3, false>)
+                               : (boundary_kind ? launch_trace<4, true> : launch_trace<4, false>);
+    return launch(X, N, L, T, pos, dirs, lattice, scale_factor, shift, window, points_scaling, hidden, out_dim, blob, nr_iters, sdf_multiplier,
+                  sdf_converged_tresh, occupancy, V, extent, trans, radius, center, pos_out, converged, queue_counter, stream);
 }
 
 

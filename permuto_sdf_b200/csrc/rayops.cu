@@ -50,6 +50,49 @@ __global__ void __launch_bounds__(kThreads) k_sphere_ray_intersection(int n, flo
     tx[i] = t1;
     hit[i] = miss ? 0 : 1;
 }
+// ------------------------------------------------------------------------------------------------ AABB
+// AABB.ray_intersection, permuto_sdf_py/utils/aabb.py:47-100 (torch ops there, one rounding per op here, in the same order). The box
+// bounds are the reference's fp32 tensors: bb_min = -size / 2 + t, bb_max = (size - size / 2) + t. Per axis the slab distances use IEEE
+// division (an axis-parallel ray gives +-inf, 0 / 0 gives NaN) and every torch.where is an explicit compare-and-select, so that a NaN
+// comparison picks the same operand as there (fminf / fmaxf would not). Misses get lo = hi = 0 (invalid_depth_val), then lo is clamped
+// at 0 as torch.clamp does it (NaN and -0 pass through).
+struct Box3 { float size[3], trans[3]; };
+__global__ void __launch_bounds__(kThreads) k_aabb_ray_intersection(int n, Box3 box, const float* __restrict__ origins,
+                                                                    const float* __restrict__ dirs, float* __restrict__ pe,
+                                                                    float* __restrict__ te, float* __restrict__ px,
+                                                                    float* __restrict__ tx, uint8_t* __restrict__ hit) {
+    int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const float o[3] = {origins[3 * i], origins[3 * i + 1], origins[3 * i + 2]};
+    const float d[3] = {dirs[3 * i], dirs[3 * i + 1], dirs[3 * i + 2]};
+    float lo = -1e10f, hi = 1e10f;            // -ones * HUGE_NUMBER, ones * HUGE_NUMBER
+    bool invalid = false;
+#pragma unroll
+    for (int k = 0; k < 3; k++) {
+        const float s = box.size[k], half = __fdiv_rn(s, 2.0f);
+        const float bmin = __fadd_rn(__fdiv_rn(-s, 2.0f), box.trans[k]);
+        const float bmax = __fadd_rn(__fsub_rn(s, half), box.trans[k]);
+        float dlo = __fdiv_rn(__fsub_rn(bmin, o[k]), d[k]);
+        float dhi = __fdiv_rn(__fsub_rn(bmax, o[k]), d[k]);
+        const bool swap = dlo > dhi;
+        const float dlo0 = dlo;
+        dlo = swap ? dhi : dlo;
+        dhi = swap ? dlo0 : dhi;
+        invalid = invalid || (dhi < lo) || (dlo > hi);
+        lo = (dlo > lo) ? dlo : lo;
+        hi = (dhi < hi) ? dhi : hi;
+    }
+    if (invalid) { lo = 0.0f; hi = 0.0f; }
+    lo = (lo < 0.0f) ? 0.0f : lo;
+#pragma unroll
+    for (int k = 0; k < 3; k++) {
+        pe[3 * i + k] = __fadd_rn(o[k], __fmul_rn(lo, d[k]));
+        px[3 * i + k] = __fadd_rn(o[k], __fmul_rn(hi, d[k]));
+    }
+    te[i] = lo;
+    tx[i] = hi;
+    hit[i] = invalid ? 0 : 1;
+}
 // SphereGPU.cuh:96-130 (the centre is not added, like the reference)
 __global__ void __launch_bounds__(kThreads) k_sphere_rand_points(int n, float radius, const float* __restrict__ phi,
                                                                  const float* __restrict__ ct, const float* __restrict__ u,
@@ -709,6 +752,17 @@ int psdf_sphere_ray_intersection(int nr_rays, float radius, const float center[3
     k_sphere_ray_intersection<<<div_up(nr_rays, kThreads), kThreads, 0, ST>>>(nr_rays, radius, center[0], center[1], center[2],
                                                                              origins, dirs, pts_entry, t_entry, pts_exit,
                                                                              t_exit, hit);
+    PSDF_CHECK_LAUNCH();
+    return PSDF_OK;
+}
+int psdf_aabb_ray_intersection(int nr_rays, const float sizes[3], const float translation[3], const float* origins, const float* dirs,
+                               float* pts_entry, float* t_entry, float* pts_exit, float* t_exit, uint8_t* hit, void* stream) {
+    if (nr_rays < 0) return PSDF_ERR_ARG;
+    if (nr_rays == 0) return PSDF_OK;
+    Box3 box;
+    for (int k = 0; k < 3; k++) { box.size[k] = sizes[k]; box.trans[k] = translation[k]; }
+    k_aabb_ray_intersection<<<div_up(nr_rays, kThreads), kThreads, 0, ST>>>(nr_rays, box, origins, dirs, pts_entry, t_entry, pts_exit,
+                                                                           t_exit, hit);
     PSDF_CHECK_LAUNCH();
     return PSDF_OK;
 }

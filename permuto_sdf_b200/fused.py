@@ -124,13 +124,29 @@ class FusedSDF:
         return sdf, grad, geom
 
 
-def _fused_sdf_sphere_trace(self, points, dirs, iter_nr, nr_iters, sdf_multiplier, sdf_converged_tresh, occupancy_grid=None):
+def _trace_boundary(model):
+    """-> (boundary_kind, boundary[6]) of psdf_sdf_sphere_trace_dim for the model's boundary_primitive; RuntimeError for other primitives"""
+    from .permuto_sdf import AABB, Sphere
+    b = model.boundary_primitive
+    if isinstance(b, Sphere):
+        return 0, [b.m_radius] + list(b.m_center) + [0.0, 0.0]
+    if isinstance(b, AABB):
+        # the fp32 values check_point_inside_primitive compares against: max_bounds (s / 2 rounded once) and the translation
+        return 1, [float(v) for v in b.max_bounds] + list(b.bounding_box_translation)
+    raise RuntimeError("FusedSDF.sphere_trace: the model's boundary_primitive is a %s; the fused tracer tests against a Sphere or an AABB"
+                       % type(b).__name__)
+
+
+def _fused_sdf_sphere_trace(self, points, dirs, iter_nr, nr_iters, sdf_multiplier, sdf_converged_tresh, occupancy_grid=None, time_val=None):
     """sphere_trace's iteration loop (sdf_utils.py:150-200) in one kernel: -> (traced points [N,3], converged [N] bool).
-    With an occupancy grid every step is followed by advance_sample_to_next_occupied_voxel, otherwise rays stop when they leave
-    the model's bounding sphere. pos_dim 3 only."""
-    if self.pos_dim != 3:
-        raise RuntimeError("FusedSDF.sphere_trace: pos_dim %d; the fused sphere tracer evaluates 3-D positions (a space-time SDF "
-                           "would need the time value and an AABB boundary)" % self.pos_dim)
+    With an occupancy grid every step is followed by advance_sample_to_next_occupied_voxel, otherwise rays stop when they leave the
+    model's boundary_primitive (a Sphere or an AABB). A space-time SDF (pos_dim 4) is traced at `time_val`: the network sees
+    (x, y, z, time_val) as the reference's loop feeds it, the points and the steps stay 3-D."""
+    if self.pos_dim == 4 and time_val is None:
+        raise RuntimeError("FusedSDF.sphere_trace: pos_dim 4; a space-time SDF is traced at a time value (time_val=...)")
+    if self.pos_dim == 3 and time_val is not None:
+        raise RuntimeError("FusedSDF.sphere_trace: time_val given for a pos_dim 3 SDF, which has no time input")
+    kind, boundary = _trace_boundary(self.model)
     if self._versions != self._cur_versions():
         self.repack()
     m, enc = self.model, self.model.encoding
@@ -141,16 +157,20 @@ def _fused_sdf_sphere_trace(self, points, dirs, iter_nr, nr_iters, sdf_multiplie
     queue = torch.zeros(8, dtype=torch.int32, device=pts.device)        # [0] ray queue of the persistent CTAs, [1..4] statistics
     self.last_trace_stats = queue
     window = m.window(iter_nr).view(-1).contiguous()
-    sph = m.boundary_primitive
     if occupancy_grid is not None:
         V, e, t = occupancy_grid._geom()
         occ = occupancy_grid.m_grid_occupancy
     else:
         V, e, t, occ = 1, 1.0, [0.0, 0.0, 0.0], None
+    net = (N, enc.nr_levels, enc.capacity, pts, drs, enc.lattice_values.detach(), enc.scale_factor, enc.shift_tensor(), window,
+           enc.concat_points_scaling, self.hidden, self.out_dim, self.blob, int(nr_iters), float(sdf_multiplier), float(sdf_converged_tresh),
+           occ, V, e, t)
     with torch.no_grad():
-        call("psdf_sdf_sphere_trace", N, enc.nr_levels, enc.capacity, pts, drs, enc.lattice_values.detach(), enc.scale_factor, enc.shift_tensor(),
-             window, enc.concat_points_scaling, self.hidden, self.out_dim, self.blob, int(nr_iters), float(sdf_multiplier),
-             float(sdf_converged_tresh), occ, V, e, t, float(sph.m_radius), sph.m_center, out, conv, queue)
+        if self.pos_dim == 3 and kind == 0:         # the original entry point: the (3, sphere) case of psdf_sdf_sphere_trace_dim
+            call("psdf_sdf_sphere_trace", *net, boundary[0], boundary[1:4], out, conv, queue)
+        else:
+            call("psdf_sdf_sphere_trace_dim", self.pos_dim, 0.0 if time_val is None else float(time_val), kind, boundary, *net, out, conv,
+                 queue)
     return out, conv
 
 

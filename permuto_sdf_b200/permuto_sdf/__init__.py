@@ -267,8 +267,9 @@ class Sphere:
 
 # ======================================================================================================
 class AABB:
-    """permuto_sdf_py/utils/aabb.py:8-114: the axis-aligned bounding box of train_sdf_from_mesh.py, the SDF model's boundary_primitive
-    there (sizes and translation are 3-sequences). The sphere tracer and the samplers of this package take a bounding Sphere."""
+    """permuto_sdf_py/utils/aabb.py:8-114: the axis-aligned bounding box of train_sdf_from_mesh.py and train_4d_sdf.py, the SDF model's
+    boundary_primitive there (sizes and translation are 3-sequences). The sphere tracer (train.sphere_trace, FusedSDF.sphere_trace) takes
+    it or a bounding Sphere; the NeuS samplers of this package take a Sphere."""
 
     def __init__(self, bounding_box_sizes_xyz, bounding_box_translation):
         self.bounding_box_sizes_xyz = [float(v) for v in bounding_box_sizes_xyz]
@@ -278,6 +279,22 @@ class AABB:
         half = [s / 2 for s in self.bounding_box_sizes_xyz]
         self.max_bounds = torch.tensor(half)
         self.min_bounds = torch.tensor([-h for h in half])
+
+    def ray_intersection(self, ray_origins, ray_dirs):
+        """aabb.py:47-100 in one kernel (psdf_aabb_ray_intersection), bit-identical to the reference's torch ops -> (entry points [N,3],
+        t_entry [N,1], exit points [N,3], t_exit [N,1], hit [N,1] bool). Rays that miss get t = 0 at both ends; t_entry is clamped at 0
+        (an origin inside the box enters at the origin)."""
+        if ray_origins.dim() != 2 or ray_dirs.dim() != 2:
+            raise RuntimeError("ray_origins / ray_dirs should have dim 2 corresponding to nr_rays x 3")
+        o, dr = _f32(ray_origins, "ray_origins", 3), _f32(ray_dirs, "ray_dirs", 3)
+        if o.shape[0] != dr.shape[0]:
+            raise RuntimeError("AABB.ray_intersection: %d origins but %d directions" % (o.shape[0], dr.shape[0]))
+        n, d = o.shape[0], o.device
+        pe = torch.empty(n, 3, device=d); te = torch.empty(n, 1, device=d)
+        px = torch.empty(n, 3, device=d); tx = torch.empty(n, 1, device=d)
+        hit = torch.empty(n, 1, dtype=torch.bool, device=d)
+        call("psdf_aabb_ray_intersection", n, self.bounding_box_sizes_xyz, self.bounding_box_translation, o, dr, pe, te, px, tx, hit)
+        return pe, te, px, tx, hit
 
     def check_point_inside_primitive(self, points):
         """[N,3] -> [N,1] bool: every coordinate strictly inside the box (aabb.py:28-43)"""

@@ -311,6 +311,42 @@ class SurfaceFit:
         self.iter_nr += 1
         return loss
 
+    # ------------------------------------------------------------------------------------ traced normals
+    def trace_normals(self, ray_origins, ray_dirs, nr_sphere_traces=20, sdf_multiplier=0.9, sdf_converged_tresh=2e-4, iter_nr=None):
+        """What train_sdf_from_mesh.py:193-199 displays: sphere_trace of the rays through the fitted SDF (bounded by its AABB, on the
+        fused tracer), then filter_unconverged_points with its default threshold and F.normalize of the gradient.
+        ray_origins, ray_dirs: [N,3] float32 on the model's device. iter_nr: the coarse-to-fine window to trace with; None = the one of the
+        last step (the iteration the reference's loop displays after its step). -> (ray_end [N,3], normals [N,3], normals of the
+        converged rays and zero elsewhere [N,3], is_converged [N,1] float). Runs under no_grad with the model in eval(); touches no
+        parameter, gradient, optimizer state, generator or the device-resident iteration."""
+        return self._trace_normals(ray_origins, ray_dirs, None, nr_sphere_traces, sdf_multiplier, sdf_converged_tresh, iter_nr)
+
+    def _trace_normals(self, ray_origins, ray_dirs, time_val, nr_sphere_traces, sdf_multiplier, sdf_converged_tresh, iter_nr):
+        from .train import filter_unconverged_points, sphere_trace
+        who = type(self).__name__ + ".trace_normals"
+        for name, t in (("ray_origins", ray_origins), ("ray_dirs", ray_dirs)):
+            if not isinstance(t, torch.Tensor) or t.dim() != 2 or t.shape[1] != 3 or t.dtype != torch.float32:
+                raise RuntimeError("%s: %s must be a float32 tensor of shape [N,3]" % (who, name))
+            if t.device != self.points.device:
+                raise RuntimeError("%s: %s on %s, the model on %s" % (who, name, t.device, self.points.device))
+        if ray_origins.shape[0] != ray_dirs.shape[0]:
+            raise RuntimeError("%s: %d ray origins but %d directions" % (who, ray_origins.shape[0], ray_dirs.shape[0]))
+        m = self.model_sdf
+        was_training, last_iter_nr = m.training, m.last_iter_nr
+        if iter_nr is None:
+            iter_nr = self.iter_nr - 1 if self.iter_nr > 0 else last_iter_nr
+        m.eval()
+        try:
+            with torch.no_grad(), torch.cuda.device(self.points.device):
+                m.last_iter_nr = int(iter_nr)
+                ray_end, ray_end_sdf, ray_end_gradient, _, _ = sphere_trace(int(nr_sphere_traces), ray_origins.contiguous(), ray_dirs.contiguous(),
+                                                                            m, True, sdf_multiplier, sdf_converged_tresh, None, time_val)
+                _, ray_end_gradient_converged, is_converged = filter_unconverged_points(ray_end, ray_end_sdf, ray_end_gradient)
+                return (ray_end, F.normalize(ray_end_gradient, dim=1), F.normalize(ray_end_gradient_converged, dim=1), is_converged)
+        finally:
+            m.train(was_training)
+            m.last_iter_nr = last_iter_nr
+
     # ------------------------------------------------------------------------------------ CUDA-graph replay
     def enable_cuda_graph(self):
         """later steps of the direct sequence replay one captured CUDA graph per shape and stretch of the coarse-to-fine schedule: the
@@ -398,3 +434,11 @@ class SpaceTimeFit(SurfaceFit):
     def fit(self, nr_iters, nr_surface=3000, nr_offsurface=3000):
         """`nr_iters` iterations -> detached 0-d loss of the last one (None when nr_iters is 0)"""
         return super().fit(nr_iters, nr_surface, nr_offsurface)
+
+    def trace_normals(self, ray_origins, ray_dirs, time_val, nr_sphere_traces=20, sdf_multiplier=0.7, sdf_converged_tresh=2e-4, iter_nr=None):
+        """What train_4d_sdf.py:268-274 displays at `time_val`: sphere_trace with time_val through the fitted space-time SDF (the network
+        sees (x, y, z, time_val), the rays stay 3-D), filter_unconverged_points and F.normalize of the spatial gradient. Arguments,
+        results and guarantees as SurfaceFit.trace_normals."""
+        if time_val is None:
+            raise RuntimeError("SpaceTimeFit.trace_normals: a space-time SDF is traced at a time value (time_val=...)")
+        return self._trace_normals(ray_origins, ray_dirs, float(time_val), nr_sphere_traces, sdf_multiplier, sdf_converged_tresh, iter_nr)

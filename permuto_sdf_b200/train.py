@@ -218,8 +218,10 @@ def loss_sphere_init(nr_points, aabb, model, iter_nr_for_anneal, points=None, sp
 
 
 def sphere_trace(nr_sphere_traces, ray_origins, ray_dirs, model, return_gradients, sdf_multiplier, sdf_converged_tresh,
-                 occupancy_grid=None):
-    """sdf_utils.py:120-218 (boolean-mask gather/scatter loop, as in the reference)"""
+                 occupancy_grid=None, time_val=None):
+    """sdf_utils.py:120-218 (boolean-mask gather/scatter loop, as in the reference). model.boundary_primitive is a Sphere or an AABB.
+    time_val: a space-time SDF (SDF(4, ...)) is traced at that time, as train_4d_sdf.py:268 does: the network sees (x, y, z, time_val),
+    the traced points stay 3-D and the returned gradient is the spatial one ([:, 0:3] of the reference's [N,4] gradient)."""
     ray_points_entry, ray_t_entry, _, ray_t_exit, _ = model.boundary_primitive.ray_intersection(ray_origins, ray_dirs)
     has_occupancy = occupancy_grid is not None
     if has_occupancy:
@@ -233,17 +235,21 @@ def sphere_trace(nr_sphere_traces, ray_origins, ray_dirs, model, return_gradient
         pos, dirs = rsp.samples_pos, rsp.samples_dirs
     pts = pos.clone()
     converged = torch.zeros_like(pos)[:, 0:1].bool()
+
+    def with_time(p):                   # the reference's torch.cat([p, torch.empty(n, 1).fill_(time_val)], 1)
+        return p if time_val is None else torch.cat([p, torch.full((p.shape[0], 1), float(time_val), device=p.device)], 1)
+
     fused_tracer = FUSED_SPHERE_TRACE and getattr(model, "fused", None) is not None and 0 < pos.shape[0] <= FUSED_SPHERE_TRACE_MAX_RAYS
     if fused_tracer:
         # the whole loop below in one kernel (csrc/fused_sdf.cu k_sdf_sphere_trace): same per-ray arithmetic, no gather / scatter / sync
         pts, _ = model.fused.sphere_trace(pos, dirs, model.last_iter_nr, nr_sphere_traces, sdf_multiplier, sdf_converged_tresh,
-                                          occupancy_grid if has_occupancy else None)
+                                          occupancy_grid if has_occupancy else None, time_val)
     for _ in range(0 if fused_tracer else nr_sphere_traces):
         sel = torch.logical_not(converged).view(-1)
         pos_u, dirs_u = pts[sel].contiguous(), dirs[sel].contiguous()
         if pos_u.shape[0] == 0:
             break
-        sdf, _ = model(pos_u, model.last_iter_nr)
+        sdf, _ = model(with_time(pos_u), model.last_iter_nr)
         pos_u = (pos_u + dirs_u * sdf * sdf_multiplier).contiguous()
         newly = (sdf.abs() < sdf_converged_tresh).view(-1)
         if has_occupancy:
@@ -253,17 +259,27 @@ def sphere_trace(nr_sphere_traces, ray_origins, ray_dirs, model, return_gradient
         conv_u = torch.logical_or(newly, torch.logical_not(within.view(-1)))
         converged[sel] = torch.logical_or(converged[sel].view(-1), conv_u).view(-1, 1)
         pts[sel] = pos_u
+    pts_t = with_time(pts).contiguous()
     if return_gradients and getattr(model, "fused", None) is not None:
-        sdf, grads, geom = model.fused(pts, model.last_iter_nr, with_gradient=True)      # forward-mode normal, one kernel
+        sdf, grads, geom = model.fused(pts_t, model.last_iter_nr, with_gradient=True)      # forward-mode normal, one kernel
     elif return_gradients:
         with torch.enable_grad():
-            sdf, grads, geom = model.get_sdf_and_gradient(pts.detach().clone(), model.last_iter_nr)
+            sdf, grads, geom = model.get_sdf_and_gradient(pts_t.detach().clone(), model.last_iter_nr)
             grads = grads.detach()[:, 0:3]
     else:
-        sdf, geom = model(pts, model.last_iter_nr)
+        sdf, geom = model(pts_t, model.last_iter_nr)
         grads = None
     rsp.samples_pos = pts
     return pts, sdf, grads, geom, rsp
+
+
+def filter_unconverged_points(points, sdf, sdf_gradients, sdf_converged_tresh=0.01):
+    """sdf_utils.py:221-231, as written there: rows whose SIGNED sdf is below the threshold count as converged (a point far inside the
+    surface passes too) -> (points * c, sdf_gradients * c or None, c [N,1] float)"""
+    is_sdf_converged = (sdf < sdf_converged_tresh) * 1.0
+    points_converged = points * is_sdf_converged
+    sdf_gradients_converged = sdf_gradients * is_sdf_converged if sdf_gradients is not None else None
+    return points_converged, sdf_gradients_converged, is_sdf_converged
 
 
 def run_net_sphere_traced(ray_origins, ray_dirs, hyperparams, model_sdf, model_rgb, occupancy_grid, iter_nr_for_anneal, nr_sphere_traces,
