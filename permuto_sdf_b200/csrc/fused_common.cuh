@@ -357,6 +357,24 @@ __device__ __forceinline__ void streams_product(float* acc, const uint8_t* a, in
     umma::wgmma_commit();
     umma::wgmma_wait0();
 }
+// The reverse product of streams_product: columns [n0, n0 + N) of D_s = A_s W, s = 0 .. S-1, the reduction running over the Np rows of
+// the FORWARD weight tile [Np rows][Kp] read as an MN-major B operand (8-row groups sbo_w apart, 8-column cores kLBO apart), so no
+// transposed copy is needed. A operands and fragments as in streams_product. Issue only: the caller brackets it with wgmma_fence() and
+// wgmma_commit() + wgmma_wait0().
+template <int N, int S>
+__device__ __forceinline__ void streams_product_wt(float* acc, const uint8_t* a, int stream_bytes, int lo_bytes, uint32_t row_off,
+                                                   const uint8_t* w_hi, const uint8_t* w_lo, int Kp, int Np, int n0) {
+    static_assert(S == 1 || N <= 32, "a stream's fragment holds 16 floats");
+    const uint32_t sbo_w = (Kp / 8) * kLBO, wo = (uint32_t)(n0 / 8) * kLBO;
+    const uint64_t dwh = umma::make_desc(umma::smem_u32(w_hi) + wo, sbo_w, kLBO), dwl = umma::make_desc(umma::smem_u32(w_lo) + wo, sbo_w, kLBO);
+#pragma unroll
+    for (int s = 0; s < S; s++) {
+        const uint8_t* as = a + s * stream_bytes;
+        const uint64_t dah = umma::make_desc(umma::smem_u32(as) + row_off, kLBO, kSBO_A);
+        const uint64_t dal = umma::make_desc(umma::smem_u32(as + lo_bytes) + row_off, kLBO, kSBO_A);
+        umma::wg_mma_regs<N, 0, 1>(acc + 16 * s, dah, dal, dwh, dwl, (2 * kLBO) >> 4, (2 * sbo_w) >> 4, Np / 16, false);
+    }
+}
 
 
 // column halves of an N-column product in units of 16 columns (MMA N % 16 == 0); the second half may be empty

@@ -1,8 +1,8 @@
 // Training backward of the fused encoding + SDF MLP (sm_90a, wgmma): given d loss / d {sdf, d sdf/dx, geom}
 // per sample it produces the lattice gradient, the bias gradients and the weight gradients. Two kernels: the persistent
 // tensor-core kernel forms the weight-gradient products from the operand tiles while they are still in shared memory
-// (accumulated in the CTA's accumulator area, umma.cuh, over all tiles of the CTA) and hands abar_0 | tabar_0 to a
-// full-occupancy kernel that scatters them into the lattice gradient.
+// (summed over all tiles of the CTA) and hands abar_0 | tabar_0 to a full-occupancy kernel that scatters them into the lattice
+// gradient.
 //
 // What it replaces in the reference: `loss.backward()` through SDF.get_sdf_and_gradient
 // (permuto_sdf_py/models/models.py:199-259, create_graph=True) -- i.e. the double backward of the
@@ -20,29 +20,36 @@
 //     dW_l = zbar_{l+1} a_l^T + tzbar_{l+1} ta_l^T,   db_l = sum zbar_{l+1}
 //     lattice[lvl][idx_r] += window_lvl (B_r abar_0[lvl] + dB_r tabar_0[lvl])       (B barycentric weights, dB their tangent)
 //
-// Per 128-sample tile (512 threads: row = tid & 127, group g = tid >> 7 owns operand cores g, g+4, .. in the encoder phases
-// and the 16-column chunk g in the epilogues). Two 64 KB operand-tile buffers X, Y ([value hi | value lo | tangent hi | tangent lo]):
-//   1. encoder: a_0, ta_0 -> X; X leaves by ONE TMA store (64 KB / tile, re-read from L2 in step 4: the only spill left)
-//   2. forward recompute, layers 0..2: each warpgroup forms a row half x column half of both streams in its registers (value and tangent
-//      of one (row, column) in the same thread) and writes a_1 -> Y, a_2 -> X, a_3 -> Y straight from the fragments; the raw z_1, z_2
-//      (value + tangent) STAY in the accumulator area (4 x 64 columns), z_3 passes through the work columns to give gelu'(z_3),
-//      gelu''(z_3) tz_3 in registers (layer 3 is reversed right away)
+// Per 128-sample tile (512 threads: row = tid & 127, group g = tid >> 7 owns operand cores g, g+4, .. in the encoder and seed
+// phases). Every product lands in the registers of the warpgroup that issues it: warpgroup (mh, nh) = (wgi & 1, wgi >> 1) forms rows
+// 64 mh .. 64 mh + 63 x column half nh (split_n) of both streams, the value and the tangent of one (row, column) in the same thread, and
+// consumes them in place. Two 64 KB operand-tile buffers X, Y ([value hi | value lo | tangent hi | tangent lo]):
+//   1. encoder: a_0, ta_0 -> X; X leaves by ONE TMA store (64 KB / tile, re-read from L2 in step 4)
+//   2. forward recompute, layers 0..2: a_1 -> Y, a_2 -> X, a_3 -> Y straight from the fragments; the raw z_1, z_2 (value + tangent)
+//      go to this thread's slots of the CTA's stash (global, L2 resident) and come back to the same thread in the reverse sweep: the
+//      reverse step l splits its Kp_l = Np_{l-1} columns exactly as the forward layer l-1 split them, so it needs no barrier.
+//      gelu'(z_3), gelu''(z_3) tz_3 stay in registers (layer 3 is reversed right away)
 //   3. seed zbar_4 -> X
-//   4. reverse sweep l = 3..0:  abar_l = zbar_{l+1} W_l uses the FORWARD weight tile as an MN-major B operand (no transposed
-//      copy, weights resident for the CTA's lifetime); while it runs, a_l / ta_l are rebuilt into Y from the stored z_l
-//      (l = 2, 1) or come back by TMA (l = 0); then dW_l += zbar_{l+1}^T a_l: the sample axis is the MMA K dimension and a
-//      K-major operand tile IS an MN-major operand for that product, so X and Y are multiplied as they sit. The four dW
-//      accumulators (M = 64) share 2 x 64 columns: an M = 64 product is stored to lanes (m / 16) * 32 + m % 16, so a second
-//      accumulator lives at lane offset 16 of the same columns (tests/test_umma_probe_gpu.py).
+//   4. reverse sweep l = 3..0, one wgmma group per warpgroup:  abar_l | tabar_l = zbar_{l+1} | tzbar_{l+1} W_l uses the FORWARD
+//      weight tile as an MN-major B operand (no transposed copy, weights resident for the CTA's lifetime), and columns
+//      16 wgi .. 16 wgi + 15 of dW_l += zbar_{l+1}^T a_l + tzbar_{l+1}^T ta_l (M = 64) as one register chain over both streams: the sample
+//      axis is the MMA K dimension and a K-major operand tile IS an MN-major operand for that product, so X and Y are multiplied
+//      as they sit. The CTA's dW sums live in the stash between tiles (one read-modify-write per layer and tile, same thread).
+//      After a barrier the fragments become zbar_l | tzbar_l -> X, the bias gradient (column sums over each 32-row group: the odd
+//      warp's fragments through shared memory, then the thread's two rows, then shuffles, in exactly the order of colsum16 over the
+//      rows of one warp in the per-row layout, so the partial sums and their one fixed-point rounding per tile, column and 32 rows
+//      have the bits of the per-row sum),
+//      and a_{l-1} | ta_{l-1} are rebuilt into Y from the stashed z_{l-1} (l = 3, 2) or come back by TMA (l = 1).
 //      In the last step (l = 0) abar_0 | tabar_0 leave from the registers to the exchange region of the workspace, one float4
-//      (a0, a1, t0, t1) per level and sample, [level][sample slot]: a warp's 32 rows of one level are one contiguous 512-byte store.
+//      (a0, a1, t0, t1) per level and sample, [level][sample slot]: a thread's column pair is one level.
 // The encoder backward is its own launch, k_sdf_lattice_scatter: warp-aggregated red.global.add.v2.f32 into the lattice gradient.
 // Inside the persistent kernel it was the longest phase of a tile (one CTA of 16 warps per SM, tensor cores idle, long dependent chains
 // of simplex recompute, match_any, shuffle sums and reductions); on its own it runs with every warp slot of the SM occupied. Its warps
 // are the rows of the persistent kernel's warps, so the match_any groups and the float peer sums are the same.
 // Deterministic mode (common.cuh): every gradient (lattice, weights, biases) is summed in fixed point instead and added to the float
 // gradients by the flush that follows the two launches.
-// Accumulator map (512 columns): [0,256) z_1 | tz_1 | z_2 | tz_2, [256,384) work (value | tangent), [384,512) dW_0/dW_1, dW_2/dW_3.
+// Stash of a CTA (float4 slots, slot index * 512 + tid): [0,16) z_1 | tz_1, z_2 | tz_2 fragments (8 slots per layer), [16,24) dW_0..dW_3
+// (2 slots per layer).
 #include <cstdio>
 #include <cstdlib>
 #include "fused_common.cuh"
@@ -54,8 +61,8 @@ namespace {
 constexpr int kBwdThreads = 512;
 constexpr int kGroups = kBwdThreads / kTile;
 constexpr int kSetBytes = 4 * kATileBytes;         // one operand tile set [value hi | value lo | tangent hi | tangent lo]
-constexpr uint32_t kColWork = 256, kColDw = 384;
-__device__ float g_acc_bwd[(size_t)kAccCtas * kTile * 512];     // accumulator areas (umma.cuh)
+constexpr int kStashDw = 16, kStashSlots = 24;      // stash map (float4 slots per thread), see the header
+__device__ float4 g_stash_bwd[(size_t)kAccCtas * kStashSlots * kBwdThreads];     // per-CTA stashes, 192 KB each
 constexpr int kFxW = kDetSdfW, kFxB = 4 * kDetSdfW;    // weight / bias offsets in DetBufs::sdf_mlp
 
 struct BwdOut {
@@ -91,57 +98,47 @@ enum { kPhEncoder = 0, kPhForward = 1, kPhSeed = 2, kPhReverse3 = 3, kPhReverse2
         }                                                                                  \
     } while (0)
 
-// in place for 16 accumulator columns (zz = z + bias): z <- a = gelu(zz), tz <- ta = gelu'(zz) tz; g1 = gelu'(zz), g2t = gelu''(zz) tz
-__device__ __forceinline__ void activations16(float* z, float* tz, const float* bias, float* g1, float* g2t) {
-#pragma unroll
-    for (int i = 0; i < 16; i++) {
-        const float zz = z[i] + bias[i];
-        const GeluEval ge = gelu_eval(zz);
-        const float d1 = fmaf(zz, ge.pdf, ge.cdf);
-        g2t[i] = ge.pdf * (2.0f - zz * zz) * tz[i];
-        z[i] = zz * ge.cdf;
-        tz[i] = d1 * tz[i];
-        g1[i] = d1;
-    }
-}
-__device__ __forceinline__ void store_set16(uint8_t* set, int row, int c, const float* a, const float* ta) {
-    store8(set, set + kATileBytes, row, 2 * c, a);
-    store8(set, set + kATileBytes, row, 2 * c + 1, a + 8);
-    store8(set + 2 * kATileBytes, set + 3 * kATileBytes, row, 2 * c, ta);
-    store8(set + 2 * kATileBytes, set + 3 * kATileBytes, row, 2 * c + 1, ta + 8);
+// zz = z + bias: a = gelu(zz), ta = gelu'(zz) tz; g1 = gelu'(zz), g2t = gelu''(zz) tz
+__device__ __forceinline__ void activation(float z, float tz, float bias, float& a, float& ta, float& g1, float& g2t) {
+    const float zz = z + bias;
+    const GeluEval ge = gelu_eval(zz);
+    const float d1 = fmaf(zz, ge.pdf, ge.cdf);
+    g2t = ge.pdf * (2.0f - zz * zz) * tz;
+    a = zz * ge.cdf;
+    ta = d1 * tz;
+    g1 = d1;
 }
 
-// The wgmma sequences of a reverse step are issued by several warpgroups: warpgroups 0 / 1 issue the value / tangent stream of the
-// reverse GEMM, warpgroups 2 / 3 one half of the weight-gradient columns each. Every issuer owns its accumulator columns and
-// all its threads arrive on the phase's mbarrier (initialised with the issuers' thread count) once the results are stored.
-// one stream of  abar[128 x Kp] = zbar[128 x Np] W : A = zbar tiles K-major, B = the FORWARD weight tile [Np rows][Kp] read as an
-// MN-major operand (reduction over the rows: 8-row groups are sbo_w apart, the k cores kLBO); both row halves, one warpgroup
-__device__ __forceinline__ void issue_reverse(uint32_t tmem_d, const uint8_t* z_hi, const uint8_t* z_lo, const uint8_t* w_hi,
-                                              const uint8_t* w_lo, int Kp, int Np) {
-    const uint32_t sbo_w = (Kp / 8) * kLBO;
-    const uint64_t dwh = umma::make_desc(umma::smem_u32(w_hi), sbo_w, kLBO), dwl = umma::make_desc(umma::smem_u32(w_lo), sbo_w, kLBO);
-    for (int mh = 0; mh < 2; mh++) {
-        const uint32_t ao = (uint32_t)(mh * 8 * kSBO_A);
-        const uint64_t dzh = umma::make_desc(umma::smem_u32(z_hi) + ao, kLBO, kSBO_A), dzl = umma::make_desc(umma::smem_u32(z_lo) + ao, kLBO, kSBO_A);
-        umma::wg_gemm<0, 1>(tmem_d + ((uint32_t)(64 * mh) << 16), false, dzh, dzl, dwh, dwl, (2 * kLBO) >> 4, (2 * sbo_w) >> 4, (8 * kLBO) >> 4,
-                            Np / 16, Kp, false);
-    }
-}
-// columns [n0, n0 + nn) of  dW (+)= zbar^T a + tzbar^T ta : both tile sets consumed as MN-major operands, K = the 128 samples, M = 64
-// (one warpgroup)
-__device__ __forceinline__ void issue_dw_part(uint32_t tmem_d, const uint8_t* zset, const uint8_t* aset, int n0, int nn, bool clear) {
-    if (nn <= 0) return;
+// columns [n0, n0 + 16) of  dW (+)= zbar^T a + tzbar^T ta  into the issuing warpgroup's registers (M = 64, umma::wg_mma_regs fragments):
+// both tile sets consumed as MN-major operands, K = the 128 samples, the value stream then the tangent stream in one chain. Issue only.
+__device__ __forceinline__ void issue_dw16(float* d, const uint8_t* zset, const uint8_t* aset, int n0, bool accumulate) {
     const uint32_t aoff = (n0 / 8) * kLBO;
-#pragma unroll 1
+#pragma unroll
     for (int s = 0; s < 2; s++) {
         const uint64_t dzh = umma::make_desc(umma::smem_u32(zset + s * 2 * kATileBytes), kSBO_A, kLBO);
         const uint64_t dzl = umma::make_desc(umma::smem_u32(zset + s * 2 * kATileBytes + kATileBytes), kSBO_A, kLBO);
         const uint64_t dah = umma::make_desc(umma::smem_u32(aset + s * 2 * kATileBytes) + aoff, kSBO_A, kLBO);
         const uint64_t dal = umma::make_desc(umma::smem_u32(aset + s * 2 * kATileBytes + kATileBytes) + aoff, kSBO_A, kLBO);
         // 16 samples = two 8-sample groups per K step
-        umma::wg_gemm<1, 1>(tmem_d + n0, true, dzh, dzl, dah, dal, (2 * kSBO_A) >> 4, (2 * kSBO_A) >> 4, (8 * kLBO) >> 4, kTile / 16, nn,
-                            !(clear && s == 0));
+        umma::wg_mma_regs<16, 1, 1>(d, dzh, dzl, dah, dal, (2 * kSBO_A) >> 4, (2 * kSBO_A) >> 4, kTile / 16, accumulate || s > 0);
     }
+}
+
+// Column sums of a fragment block over the 8 lanes t / 4 = 0..7 of one warp (halving butterfly over lanes ^ 16, ^ 8, ^ 4, 7 shuffles): v[2 j + b]
+// is this thread's value of column 8 j + 2 (t % 4) + b. Afterwards every lane holds the sum of one column, `col` = 8 (2 bit4 + bit3) +
+// 2 (t % 4) + bit2.
+__device__ __forceinline__ float frag_colsum8(const float* v, int lane, int& col) {
+    float a[4], b[2], c;
+    bool up = lane & 16;
+#pragma unroll
+    for (int i = 0; i < 4; i++) { float send = up ? v[i] : v[i + 4], keep = up ? v[i + 4] : v[i]; a[i] = keep + __shfl_xor_sync(kFull, send, 16); }
+    up = lane & 8;
+#pragma unroll
+    for (int i = 0; i < 2; i++) { float send = up ? a[i] : a[i + 2], keep = up ? a[i + 2] : a[i]; b[i] = keep + __shfl_xor_sync(kFull, send, 8); }
+    up = lane & 4;
+    { float send = up ? b[0] : b[1], keep = up ? b[1] : b[0]; c = keep + __shfl_xor_sync(kFull, send, 4); }
+    col = 8 * (2 * ((lane >> 4) & 1) + ((lane >> 3) & 1)) + 2 * (lane & 3) + ((lane >> 2) & 1);
+    return c;
 }
 
 // D = 3: positions [N,3]; D = 4: space-time positions [N,4] with the tangent along (g_grad, 0) (g_grad holds spatial derivatives)
@@ -158,23 +155,22 @@ k_sdf_fused_backward(FusedParams P, Segments S, const float2* __restrict__ latti
     unsigned long long* s_gb = reinterpret_cast<unsigned long long*>(lc + 1);
     float* s_gbf = reinterpret_cast<float*>(s_gb);
     const bool det = out.fx_mlp != nullptr;
-    uint64_t* bars = reinterpret_cast<uint64_t*>(s_gb + kNL * 64);   // [0] TMA loads, [1] mma, [2] dW mma
+    uint64_t* bars = reinterpret_cast<uint64_t*>(s_gb + kNL * 64);   // [0] TMA loads
     float* s_seed = reinterpret_cast<float*>(bars + 5);   // [128][(out_dim - 1) | 1] upstream d loss / d geom of the tile (coalesced copy)
+    // the same bytes in the reverse sweep (s_seed is dead from the seed phase to the next tile): [8 warp pairs][16][32 lanes] the odd
+    // warp's zbar fragments for the bias column sums
+    float* s_bx = s_seed;
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int row = tid & 127, grp = tid >> 7;
     const int level_cores = P.L / 4;
     const int K0 = P.g.Kp[0];
-    const int wgi = warp >> 2;
-    const bool gemm_issuer = wgi < 2;                      // stream = warpgroup
-    const bool dw_issuer = wgi >= 2;                       // column half = warpgroup - 2
+    const int wgi = warp >> 2, mh = wgi & 1, nh = wgi >> 1;
+    float4* stash = g_stash_bwd + (size_t)blockIdx.x * kStashSlots * kBwdThreads + tid;     // this thread's slot 0
 
     if (tid == 0) {
         umma::mbar_init(&bars[0], 1);
-        umma::mbar_init(&bars[1], 2 * 128);
-        umma::mbar_init(&bars[2], 2 * 128);
         umma::mbar_fence_init();
-        umma::acc_attach(g_acc_bwd + (size_t)blockIdx.x * kTile * 512, 512);
     }
     load_level_consts<D>(lc, P.L, scale, shift, window, tid, kBwdThreads);
     for (int i = tid; i < kNL * 64; i += kBwdThreads) s_gb[i] = 0ull;     // also clears s_gbf
@@ -184,10 +180,8 @@ k_sdf_fused_backward(FusedParams P, Segments S, const float2* __restrict__ latti
         umma::bulk_g2s(s_w, blob, (uint32_t)P.g.total, &bars[0]);
     }
     __syncthreads();
-    const uint32_t tmem_base = 0;
-    const uint32_t tlane = tmem_base + ((uint32_t)((warp & 3) * 32) << 16);     // this warp's 32 accumulator lanes
     umma::mbar_wait(&bars[0], 0);
-    uint32_t ld_phase = 1, mma_phase = 0, dw_phase = 0;
+    uint32_t ld_phase = 1;
 
     const int ntiles = S.tile0[kMaxSeg];
     bool first_tile = true;
@@ -247,10 +241,10 @@ k_sdf_fused_backward(FusedParams P, Segments S, const float2* __restrict__ latti
         }
 
         PSDF_PHASE(kPhEncoder);
-        // ---------------- 2. forward recompute, layers 0..2. Warpgroup (mh, nh) = (wgi & 1, wgi >> 1) forms rows 64 mh .. 64 mh + 63 x column
-        // half nh of both streams in its registers and consumes them in place: a_{l+1} | ta_{l+1} -> the next operand set, and the raw
-        // z_{l+1} | tz_{l+1} -> accumulator columns l * 128 (l = 0, 1) or the work columns (l = 2) for the reverse sweep
-        float g1[16], g2t[16];                 // gelu'(z_3), gelu''(z_3) tz_3 of this thread's chunk: consumed by the first reverse step
+        // ---------------- 2. forward recompute, layers 0..2. Warpgroup (mh, nh) forms rows 64 mh .. 64 mh + 63 x column half nh of both
+        // streams in its registers and consumes them in place: a_{l+1} | ta_{l+1} -> the next operand set, and the raw z_{l+1} | tz_{l+1}
+        // -> this thread's stash slots (l = 0, 1) or the GELU' / GELU'' factors of the first reverse step (l = 2)
+        float g1[16], g2t[16];                 // gelu'(z_l), gelu''(z_l) tz_l of this thread's fragments, for the reverse step l
         float seed[2][8];                      // upstream gradient columns of this thread (prefetched before the layer-2 MMAs)
 #pragma unroll 1
         for (int l = 0; l < 3; l++) {
@@ -259,7 +253,6 @@ k_sdf_fused_backward(FusedParams P, Segments S, const float2* __restrict__ latti
             __syncthreads();
             const uint8_t* at = (l == 1) ? s_Y : s_X;
             uint8_t* dst = (l == 1) ? s_X : s_Y;
-            const uint32_t col = (l == 2) ? kColWork : (uint32_t)(l * 128);
             if (l == 0 && tid == 0) {          // a_0 | ta_0 leave as they are (needed again for dW_0 at the end of the reverse sweep)
                 umma::bulk_s2g(out.a0_spill + (size_t)tile * kSetBytes, s_X, kSetBytes);
                 umma::bulk_commit();
@@ -281,15 +274,22 @@ k_sdf_fused_backward(FusedParams P, Segments S, const float2* __restrict__ latti
                     }
                 }
             }
-            const int mh = wgi & 1;
             int n0, nn;
-            split_n(P.g.Np[l], wgi >> 1, n0, nn);
+            split_n(P.g.Np[l], nh, n0, nn);
             float acc[2][16];
 #pragma unroll
             for (int i = 0; i < 16; i++) { acc[0][i] = 0.f; acc[1][i] = 0.f; }
             const uint32_t ro = (uint32_t)(mh * 8 * kSBO_A);
             if (nn == 32) streams_product<32, 2>(acc[0], at, 2 * kATileBytes, kATileBytes, ro, s_w + P.g.w_hi[l], s_w + P.g.w_lo[l], P.g.Kp[l], n0);
             else if (nn == 16) streams_product<16, 2>(acc[0], at, 2 * kATileBytes, kATileBytes, ro, s_w + P.g.w_hi[l], s_w + P.g.w_lo[l], P.g.Kp[l], n0);
+            if (l < 2) {
+                // fragment block j of stream s -> slot 8 l + 4 s + j (thread-private: read back by this thread in the reverse step l + 1)
+#pragma unroll
+                for (int s = 0; s < 2; s++)
+#pragma unroll
+                    for (int j = 0; j < 4; j++)
+                        if (8 * j < nn) stash[(8 * l + 4 * s + j) * kBwdThreads] = make_float4(acc[s][4 * j], acc[s][4 * j + 1], acc[s][4 * j + 2], acc[s][4 * j + 3]);
+            }
             const float* bias = reinterpret_cast<const float*>(s_w + P.g.bias[l]);
 #pragma unroll
             for (int j = 0; j < 4; j++) {
@@ -297,17 +297,13 @@ k_sdf_fused_backward(FusedParams P, Segments S, const float2* __restrict__ latti
 #pragma unroll
                     for (int h = 0; h < 2; h++) {
                         const int r = frag_row(mh, h), c = n0 + frag_col(j);
-                        const float z[2] = {acc[0][4 * j + 2 * h], acc[0][4 * j + 2 * h + 1]}, tz[2] = {acc[1][4 * j + 2 * h], acc[1][4 * j + 2 * h + 1]};
-                        float* zp = umma::acc_ptr((uint32_t)r, col + (uint32_t)c);
-                        *reinterpret_cast<float2*>(zp) = make_float2(z[0], z[1]);
-                        *reinterpret_cast<float2*>(zp + 64) = make_float2(tz[0], tz[1]);
                         float a[2], ta[2];
 #pragma unroll
                         for (int b = 0; b < 2; b++) {
-                            const float zz = z[b] + bias[c + b];
-                            const GeluEval ge = gelu_eval(zz);
-                            a[b] = zz * ge.cdf;
-                            ta[b] = fmaf(zz, ge.pdf, ge.cdf) * tz[b];
+                            const int i = 4 * j + 2 * h + b;
+                            float d1, d2t;
+                            activation(acc[0][i], acc[1][i], bias[c + b], a[b], ta[b], d1, d2t);
+                            if (l == 2) { g1[i] = d1; g2t[i] = d2t; }
                         }
                         store_pair(dst, dst + kATileBytes, r, c, a[0], a[1]);
                         store_pair(dst + 2 * kATileBytes, dst + 3 * kATileBytes, r, c, ta[0], ta[1]);
@@ -315,15 +311,8 @@ k_sdf_fused_backward(FusedParams P, Segments S, const float2* __restrict__ latti
                 }
             }
         }
-        // every layer-2 product has completed (a_2 in X is dead) and z_3 | tz_3 are stored: the GELU' / GELU'' factors of the first
-        // reverse step, in the per-row layout of the reverse epilogues
+        // every layer-2 product has completed: a_2 in X is dead
         __syncthreads();
-        if (grp < P.g.Np[2] / 16) {
-            float z[16], tz[16];
-            umma::tmem_ld16(tlane + kColWork + grp * 16, z);
-            umma::tmem_ld16(tlane + kColWork + 64 + grp * 16, tz);
-            activations16(z, tz, reinterpret_cast<const float*>(s_w + P.g.bias[2]) + grp * 16, g1, g2t);
-        }
         PSDF_PHASE(kPhForward);
         // ---------------- 3. seed: zbar_4 = upstream gradient, tzbar_4 = e_0 -> X
         {
@@ -351,126 +340,177 @@ k_sdf_fused_backward(FusedParams P, Segments S, const float2* __restrict__ latti
         }
         PSDF_PHASE(kPhSeed);
         // ---------------- 4. reverse sweep, layers 3..0: X = zbar_{l+1} | tzbar_{l+1}, Y = a_l | ta_l
+        const int nbase = (tile - seg_tile0) * kTile;
+        const bool rvalid0 = nbase + frag_row(mh, 0) < seg_n, rvalid1 = nbase + frag_row(mh, 1) < seg_n;   // this thread's fragment rows
 #pragma unroll 1
         for (int l = 3; l >= 0; l--) {
-            const uint32_t dw_col = tmem_base + kColDw + (uint32_t)(l >> 1) * 64 + ((l & 1) ? (16u << 16) : 0u);
             umma::fence_async_smem();
             __syncthreads();
-            if (gemm_issuer) {
-                const int s = wgi;
-                issue_reverse(tmem_base + kColWork + s * 64, s_X + s * 2 * kATileBytes, s_X + s * 2 * kATileBytes + kATileBytes,
-                              s_w + P.g.w_hi[l], s_w + P.g.w_lo[l], P.g.Kp[l], P.g.Np[l]);
-                umma::mbar_arrive(&bars[1]);
-            }
-            if (dw_issuer && (l == 3 || l == 0)) {
-                // l = 3: a_3 | ta_3 are in Y since the forward epilogue; l = 0: a_0 | ta_0 come back by TMA (requested after the
-                // previous step released Y)
-                if (l == 0) umma::mbar_wait(&bars[0], ld_phase);
-                int n0, nn;
-                split_n(P.g.Kp[l], wgi - 2, n0, nn);
-                issue_dw_part(dw_col, s_X, s_Y, n0, nn, first_tile);
-                umma::mbar_arrive(&bars[2]);
-            }
-            if (l == 1 || l == 2) {
-                // beside the reverse MMAs: rebuild a_l | ta_l -> Y and the GELU' / GELU'' factors from the stored z_l, tz_l
-                const int c = grp;
-                if (c < P.g.Kp[l] / 16) {
-                    float z[16], tz[16];
-                    const uint32_t col = (uint32_t)((l - 1) * 128);
-                    umma::tmem_ld16(tlane + col + c * 16, z);
-                    umma::tmem_ld16(tlane + col + 64 + c * 16, tz);
-                    activations16(z, tz, reinterpret_cast<const float*>(s_w + P.g.bias[l - 1]) + c * 16, g1, g2t);
-                    store_set16(s_Y, row, c, z, tz);
-                }
-                umma::fence_async_smem();
-                __syncthreads();
-                if (dw_issuer) {
-                    int n0, nn;
-                    split_n(P.g.Kp[l], wgi - 2, n0, nn);
-                    issue_dw_part(dw_col, s_X, s_Y, n0, nn, first_tile);
-                    umma::mbar_arrive(&bars[2]);
-                }
-            }
-            umma::mbar_wait(&bars[1], mma_phase);
-            mma_phase ^= 1;
-            const int c = grp;
-            const bool have = c < P.g.Kp[l] / 16;
-            float ab[16], tab_[16];
-            if (have) {
-                umma::tmem_ld16(tlane + kColWork + c * 16, ab);
-                umma::tmem_ld16(tlane + kColWork + 64 + c * 16, tab_);
-                if (l > 0) {
+            if (l == 0) umma::mbar_wait(&bars[0], ld_phase);     // a_0 | ta_0 are back in Y
+            int n0, nn;
+            split_n(P.g.Kp[l], nh, n0, nn);
+            const bool dw = 16 * wgi < P.g.Kp[l];              // this warpgroup's 16 columns of dW_l
+            float4* dws = stash + (kStashDw + 2 * l) * kBwdThreads;
+            float acc[2][16], dwa[8];                          // acc[0] = abar_l, acc[1] = tabar_l; dwa: the CTA's sum of dW_l
 #pragma unroll
-                    for (int i = 0; i < 16; i++) {
-                        const float zb = g1[i] * ab[i] + g2t[i] * tab_[i];
-                        tab_[i] = g1[i] * tab_[i];
-                        ab[i] = zb;                  // ab = zbar_l, tab_ = tzbar_l
-                    }
-                }
+            for (int i = 0; i < 16; i++) { acc[0][i] = 0.f; acc[1][i] = 0.f; }
+#pragma unroll
+            for (int q = 0; q < 2; q++) {
+                const float4 v = (dw && !first_tile) ? dws[q * kBwdThreads] : make_float4(0.f, 0.f, 0.f, 0.f);
+                dwa[4 * q] = v.x; dwa[4 * q + 1] = v.y; dwa[4 * q + 2] = v.z; dwa[4 * q + 3] = v.w;
             }
-            // X and Y are still operands of the weight-gradient MMAs
-            umma::mbar_wait(&bars[2], dw_phase);
-            dw_phase ^= 1;
+            const uint32_t ro = (uint32_t)(mh * 8 * kSBO_A);
+            umma::wgmma_fence();
+            if (nn == 32) streams_product_wt<32, 2>(acc[0], s_X, 2 * kATileBytes, kATileBytes, ro, s_w + P.g.w_hi[l], s_w + P.g.w_lo[l], P.g.Kp[l], P.g.Np[l], n0);
+            else if (nn == 16) streams_product_wt<16, 2>(acc[0], s_X, 2 * kATileBytes, kATileBytes, ro, s_w + P.g.w_hi[l], s_w + P.g.w_lo[l], P.g.Kp[l], P.g.Np[l], n0);
+            if (dw) issue_dw16(dwa, s_X, s_Y, 16 * wgi, !first_tile);
+            umma::wgmma_commit();
+            umma::wgmma_wait0();
+            if (dw) {
+#pragma unroll
+                for (int q = 0; q < 2; q++) dws[q * kBwdThreads] = make_float4(dwa[4 * q], dwa[4 * q + 1], dwa[4 * q + 2], dwa[4 * q + 3]);
+            }
+            __syncthreads();                                   // every product of this step has read X and Y
             if (l == 1 && tid == 0) {          // Y is free: bring a_0 | ta_0 back for the last step (the store completed long ago)
                 umma::bulk_wait0();
                 umma::mbar_expect_tx(&bars[0], (uint32_t)kSetBytes);
                 umma::bulk_g2s(s_Y, out.a0_spill + (size_t)tile * kSetBytes, (uint32_t)kSetBytes, &bars[0]);
             }
             if (l > 0) {
-                if (have) {
-                    store_set16(s_X, row, c, ab, tab_);
-                    if (!valid) {
+                if (nn > 0) {
+                    // zbar_l = gelu'(z_l) abar_l + gelu''(z_l) tz_l tabar_l, tzbar_l = gelu'(z_l) tabar_l -> X; acc[0] keeps zbar_l of the
+                    // valid rows (0 elsewhere) for the bias gradient of layer l - 1
 #pragma unroll
-                        for (int i = 0; i < 16; i++) ab[i] = 0.f;
+                    for (int j = 0; j < 4; j++) {
+                        if (8 * j < nn) {
+#pragma unroll
+                            for (int h = 0; h < 2; h++) {
+                                const int r = frag_row(mh, h), c = n0 + frag_col(j);
+                                float zb[2], tzb[2];
+#pragma unroll
+                                for (int b = 0; b < 2; b++) {
+                                    const int i = 4 * j + 2 * h + b;
+                                    zb[b] = g1[i] * acc[0][i] + g2t[i] * acc[1][i];
+                                    tzb[b] = g1[i] * acc[1][i];
+                                }
+                                store_pair(s_X, s_X + kATileBytes, r, c, zb[0], zb[1]);
+                                store_pair(s_X + 2 * kATileBytes, s_X + 3 * kATileBytes, r, c, tzb[0], tzb[1]);
+                                const bool rv = h ? rvalid1 : rvalid0;
+                                acc[0][4 * j + 2 * h] = rv ? zb[0] : 0.f;
+                                acc[0][4 * j + 2 * h + 1] = rv ? zb[1] : 0.f;
+                            }
+                        }
                     }
-                    int colb;
-                    const float cs = colsum16(ab, lane, colb);       // bias gradient: column sums over the warp's 32 rows
-                    if (!(lane & 1)) {
-                        if (det) fx_add(&s_gb[(l - 1) * 64 + c * 16 + colb], cs);
-                        else atomicAdd(&s_gbf[(l - 1) * 64 + c * 16 + colb], cs);
+                    // Column sums over each 32-row group (warps 2p, 2p + 1 of the warpgroup), added up in the order of colsum16 over the
+                    // rows r = 0..31 of one warp in the per-row layout: pairs r, r ^ 16 first, then r ^ 8, r ^ 4, r ^ 2, r ^ 1. Here bit 4
+                    // of r is the warp of the pair, bit 3 the fragment half h and bits 2..0 the lane bits 4..2, so the odd warp's values
+                    // come through shared memory, then h, then frag_colsum8's butterfly over lanes ^ 16, ^ 8, ^ 4. Every partial sum and
+                    // the one fixed-point rounding per tile, column and 32 rows are those of the per-row sum.
+                    const int pair = 2 * wgi + ((warp & 3) >> 1);
+                    float* bx = s_bx + pair * 16 * 32 + lane;
+                    if (warp & 1) {
+#pragma unroll
+                        for (int i = 0; i < 16; i++) if (2 * i < nn) bx[i * 32] = acc[0][i];
+                    }
+                    umma::bar_sync(1 + pair, 64);
+                    if (!(warp & 1)) {
+                        float bs[8];
+#pragma unroll
+                        for (int j = 0; j < 4; j++)
+#pragma unroll
+                            for (int b = 0; b < 2; b++) {
+                                const int i0 = 4 * j + b, i1 = 4 * j + 2 + b;
+                                bs[2 * j + b] = (8 * j < nn) ? (acc[0][i0] + bx[i0 * 32]) + (acc[0][i1] + bx[i1 * 32]) : 0.f;
+                            }
+                        int col;
+                        const float cs = frag_colsum8(bs, lane, col);
+                        if (col < nn) {
+                            if (det) fx_add(&s_gb[(l - 1) * 64 + n0 + col], cs);
+                            else atomicAdd(&s_gbf[(l - 1) * 64 + n0 + col], cs);
+                        }
                     }
                 }
-            } else if (have) {
-                // abar_0 | tabar_0 of this row's levels (columns 2 l, 2 l + 1) -> the exchange region, for k_sdf_lattice_scatter
-                float4* dst = out.xch + (size_t)tile * kTile + row;
+                if (l >= 2) {
+                    // a_{l-1} | ta_{l-1} -> Y and the GELU' / GELU'' factors of the next step from this thread's stashed z_{l-1} | tz_{l-1}
+                    // (the forward layer l - 2 split its columns as the reverse step l - 1 does)
+                    int m0, mn;
+                    split_n(P.g.Kp[l - 1], nh, m0, mn);
+                    float z[2][16];
 #pragma unroll
-                for (int i = 0; i < 8; i++) {
-                    const int lv = c * 8 + i;
-                    if (lv < P.L) dst[(size_t)lv * out.xch_stride] = make_float4(ab[2 * i], ab[2 * i + 1], tab_[2 * i], tab_[2 * i + 1]);
+                    for (int s = 0; s < 2; s++)
+#pragma unroll
+                        for (int j = 0; j < 4; j++) {
+                            const float4 v = (8 * j < mn) ? stash[(8 * (l - 2) + 4 * s + j) * kBwdThreads] : make_float4(0.f, 0.f, 0.f, 0.f);
+                            z[s][4 * j] = v.x; z[s][4 * j + 1] = v.y; z[s][4 * j + 2] = v.z; z[s][4 * j + 3] = v.w;
+                        }
+                    const float* bias = reinterpret_cast<const float*>(s_w + P.g.bias[l - 2]);
+#pragma unroll
+                    for (int j = 0; j < 4; j++) {
+                        if (8 * j < mn) {
+#pragma unroll
+                            for (int h = 0; h < 2; h++) {
+                                const int r = frag_row(mh, h), c = m0 + frag_col(j);
+                                float a[2], ta[2];
+#pragma unroll
+                                for (int b = 0; b < 2; b++) {
+                                    const int i = 4 * j + 2 * h + b;
+                                    activation(z[0][i], z[1][i], bias[c + b], a[b], ta[b], g1[i], g2t[i]);
+                                }
+                                store_pair(s_Y, s_Y + kATileBytes, r, c, a[0], a[1]);
+                                store_pair(s_Y + 2 * kATileBytes, s_Y + 3 * kATileBytes, r, c, ta[0], ta[1]);
+                            }
+                        }
+                    }
+                }
+            } else if (nn > 0) {
+                // abar_0 | tabar_0 -> the exchange region, for k_sdf_lattice_scatter: a thread's column pair 8 j + 2 (t % 4) is one level
+                float4* dst = out.xch + (size_t)tile * kTile;
+#pragma unroll
+                for (int j = 0; j < 4; j++) {
+                    const int lv = (n0 + frag_col(j)) >> 1;
+                    if (8 * j < nn && lv < P.L) {
+#pragma unroll
+                        for (int h = 0; h < 2; h++) {
+                            const int i = 4 * j + 2 * h;
+                            dst[(size_t)lv * out.xch_stride + frag_row(mh, h)] = make_float4(acc[0][i], acc[0][i + 1], acc[1][i], acc[1][i + 1]);
+                        }
+                    }
                 }
             }
             PSDF_PHASE(kPhReverse3 + (3 - l));
         }
         ld_phase ^= 1;
-        // no barrier before the next tile: every thread has waited for this tile's last MMAs (bars[1], bars[2]), the only readers of
-        // X and Y, and the accumulator columns read above are rewritten only after the next tile's first __syncthreads
+        // no barrier before the next tile: X and Y were last read by this tile's step-0 products, complete before its second barrier;
+        // s_bx (= s_seed) was last read in step 1, before the step-0 barriers
         if (out.phase_cycles && tid == 0) atomicAdd(out.phase_cycles + kPhTiles, 1ull);
     }
-    // ---------------- weight gradients of this CTA: accumulators -> global (+=). Warp w reads lanes 32 (w & 3) .. +31 of column chunk w >> 2:
-    // lanes 0..15 hold rows 16 (w & 3) + lane of the even layer of the pair, lanes 16..31 the same rows of the odd layer
+    // ---------------- weight gradients of this CTA: this thread's stashed dW fragments -> global (+=). Element 4 j + 2 h + b of dW_l is
+    // row 16 (warp & 3) + lane / 4 + 8 h, column 16 wgi + 8 j + 2 (lane % 4) + b
     if (!first_tile) {
-        const int q = warp & 3, c = warp >> 2;
 #pragma unroll 1
-        for (int p = 0; p < 2; p++) {
-            float acc[16];
-            umma::tmem_ld16(tlane + kColDw + p * 64 + c * 16, acc);
-            const int l = 2 * p + (lane >> 4), m = q * 16 + (lane & 15);
-            if (m < P.g.N[l] && det) {
-                const int K = P.g.K[l];
-                unsigned long long* dst = out.fx_mlp + l * kFxW + m * K;
+        for (int l = 0; l < kNL; l++) {
+            if (16 * wgi >= P.g.Kp[l]) continue;
+            const int K = P.g.K[l];
+            const bool vec = (K & 1) == 0 && ((uintptr_t)out.gW[l] & 7) == 0;      // column pairs stay 8-byte aligned
 #pragma unroll
-                for (int i = 0; i < 16; i++) if (c * 16 + i < K) fx_add(dst + c * 16 + i, acc[i]);
-            } else if (m < P.g.N[l]) {
-                const int K = P.g.K[l];
-                float* dst = out.gW[l] + (size_t)m * K + c * 16;
-                const bool vec = (K & 3) == 0 && ((uintptr_t)out.gW[l] & 15) == 0;      // rows stay 16-byte aligned
+            for (int j = 0; j < 2; j++) {
+                const float4 v = stash[(kStashDw + 2 * l + j) * kBwdThreads];
 #pragma unroll
-                for (int i = 0; i < 16; i += 4) {
-                    const int k = c * 16 + i;
-                    if (vec && k + 3 < K) red_v4(dst + i, acc[i], acc[i + 1], acc[i + 2], acc[i + 3]);
-                    else {
-#pragma unroll
-                        for (int j = 0; j < 4; j++) if (k + j < K) atomicAdd(dst + i + j, acc[i + j]);
+                for (int h = 0; h < 2; h++) {
+                    const int m = 16 * (warp & 3) + lane / 4 + 8 * h, k = 16 * wgi + 8 * j + 2 * (lane & 3);
+                    const float v0 = h ? v.z : v.x, v1 = h ? v.w : v.y;
+                    if (m >= P.g.N[l]) continue;
+                    if (det) {
+                        unsigned long long* dst = out.fx_mlp + l * kFxW + m * K + k;
+                        if (k < K) fx_add(dst, v0);
+                        if (k + 1 < K) fx_add(dst + 1, v1);
+                    } else {
+                        float* dst = out.gW[l] + (size_t)m * K + k;
+                        if (vec && k + 1 < K) red_v2(dst, make_float2(v0, v1));
+                        else {
+                            if (k < K) atomicAdd(dst, v0);
+                            if (k + 1 < K) atomicAdd(dst + 1, v1);
+                        }
                     }
                 }
             }
@@ -592,7 +632,10 @@ static int launch_backward(int nseg, const int* Ns, const float* const* pos, con
     int dev = 0, sms = 132;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    const size_t smem = (size_t)P.g.total + 2 * kSetBytes + sizeof(LevelC) + kNL * 64 * sizeof(unsigned long long) + 64 + (size_t)kTile * (size_t)((out_dim - 1) | 1) * sizeof(float);
+    // the last region holds the upstream geometric-feature rows of a tile or, in the reverse sweep, the 8 x 16 x 32 fragments exchanged
+    // for the bias column sums
+    const size_t seed_bytes = std::max((size_t)kTile * (size_t)((out_dim - 1) | 1) * sizeof(float), (size_t)(8 * 16 * 32 * sizeof(float)));
+    const size_t smem = (size_t)P.g.total + 2 * kSetBytes + sizeof(LevelC) + kNL * 64 * sizeof(unsigned long long) + 64 + seed_bytes;
     if (smem > 227 * 1024) return PSDF_ERR_UNSUPPORTED;
     { static bool optin_[64]; psdf::psdf_optin_smem(k_sdf_fused_backward<D>, 227 * 1024, optin_); }
     k_sdf_fused_backward<D><<<min(min(tiles, sms), kAccCtas), kBwdThreads, smem, ST>>>(P, S, reinterpret_cast<const float2*>(lattice), scale_factor, shift, window,

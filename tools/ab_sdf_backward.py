@@ -1,0 +1,130 @@
+"""Compare the SDF training backward of two builds on one fixed, seeded problem at the shape of the C2 training step.
+
+    python tools/ab_sdf_backward.py run --root TREE --out a.npz     # run TREE's library (default: this tree), twice, save the gradients
+    python tools/ab_sdf_backward.py compare a.npz b.npz             # gradients of two builds
+
+`run` calls psdf_sdf_fused_backward_multi in deterministic mode with the three sample sets of one training iteration (main samples with
+sdf, gradient and geometric-feature upstreams, the curvature pass with gradient upstreams only, 1024 off-surface points with sdf
+upstreams only): 16 levels, T = 2^18, hidden 64, out_dim 33, 1030 tiles. It checks that two runs give the same bits, times the call with
+CUDA events and saves the lattice, weight and bias gradients.
+
+`compare` requires every gradient (lattice, weights, biases) to be bit-identical and prints the largest difference of every tensor."""
+import argparse
+import os
+import sys
+
+import numpy as np
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+L, T, HIDDEN, OUT_DIM = 16, 2 ** 18, 64, 33
+N_MAIN, N_OFF = 65300, 1024           # 511 + 511 + 8 = 1030 tiles of 128 samples
+
+
+def tiles():
+    return 2 * ((N_MAIN + 127) // 128) + (N_OFF + 127) // 128
+
+
+def problem(torch):
+    g = torch.Generator().manual_seed(1234)
+    dims = [2 * L + 4, HIDDEN, HIDDEN, HIDDEN, OUT_DIM]
+    p = dict(
+        lat=(torch.rand(L, T, 2, generator=g) * 2 - 1) * 1e-2,
+        scale=torch.stack([torch.full((3,), 0.5 * 1.5 ** l) for l in range(L)]) * 10.0,
+        shift=torch.randn(L, 3, generator=g) * 10,
+        win=torch.ones(L),
+        W=[torch.randn(dims[i + 1], dims[i], generator=g) / dims[i] ** 0.5 for i in range(4)],
+        b=[torch.randn(dims[i + 1], generator=g) * 0.1 for i in range(4)],
+        pos=[(torch.rand(n, 3, generator=g) - 0.5) * 0.9 for n in (N_MAIN, N_MAIN, N_OFF)],
+        g_sdf=torch.randn(N_MAIN, generator=g) * 1e-3,
+        g_grad=torch.randn(N_MAIN, 3, generator=g) * 1e-3,
+        g_geom=torch.randn(N_MAIN, OUT_DIM - 1, generator=g) * 1e-3,
+        g_grad_s=torch.randn(N_MAIN, 3, generator=g) * 1e-3,
+        g_off=torch.randn(N_OFF, generator=g) * 1e-2,
+    )
+    return p
+
+
+def run(args):
+    sys.path.insert(0, os.path.abspath(args.root))
+    import torch
+    from permuto_sdf_b200._lib import call, load_library
+    lib = load_library()
+    assert lib.psdf_device_ok() == 1, "needs a CUDA device"
+    c = lambda t: t.float().contiguous().cuda()
+    p = problem(torch)
+    blob = torch.empty(int(lib.psdf_sdf_mlp_blob_bytes(2 * L + 4, HIDDEN, OUT_DIM)), dtype=torch.uint8, device="cuda")
+    call("psdf_sdf_mlp_pack", 2 * L + 4, HIDDEN, OUT_DIM, *[c(t) for l in range(4) for t in (p["W"][l], p["b"][l])], blob)
+    lat, scale, shift, win = c(p["lat"]), c(p["scale"]), c(p["shift"]), c(p["win"])
+    pos = [c(x) for x in p["pos"]]
+    segs = [N_MAIN, pos[0], c(p["g_sdf"]), c(p["g_grad"]), c(p["g_geom"]),
+            N_MAIN, pos[1], None, c(p["g_grad_s"]), None,
+            N_OFF, pos[2], c(p["g_off"]), None, None]
+    ws = torch.empty(int(lib.psdf_sdf_fused_backward_multi_workspace_bytes(N_MAIN, N_MAIN, N_OFF)), dtype=torch.uint8, device="cuda")
+    glat = torch.zeros(L, T, 2, device="cuda")
+    gW = [torch.zeros_like(c(w)) for w in p["W"]]
+    gb = [torch.zeros_like(c(x)) for x in p["b"]]
+
+    def once():
+        glat.zero_()
+        for x in gW + gb:
+            x.zero_()
+        call("psdf_sdf_fused_backward_multi", L, T, lat, scale, shift, win, 1e-3, HIDDEN, OUT_DIM, blob, *segs, glat, ws, *gW, *gb)
+
+    call("psdf_set_deterministic", 1, L * T * 2, 64 ** 3)
+    try:
+        results = []
+        for _ in range(2):
+            once()
+            torch.cuda.synchronize()
+            results.append({"lattice": glat.cpu().numpy(), **{"W%d" % l: gW[l].cpu().numpy() for l in range(4)},
+                            **{"b%d" % l: gb[l].cpu().numpy() for l in range(4)}})
+        same = all(np.array_equal(results[0][k], results[1][k]) for k in results[0])
+        for _ in range(5):
+            once()
+        reps = 50
+        s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        torch.cuda.synchronize()
+        s.record()
+        for _ in range(reps):
+            once()
+        e.record()
+        torch.cuda.synchronize()
+        ms = s.elapsed_time(e) / reps
+    finally:
+        call("psdf_set_deterministic", 0, 0, 0)
+    name = torch.cuda.get_device_name(0)
+    print("%s: two runs bit-identical: %s | %.3f ms per call (zeroing + backward, deterministic, %d tiles) on %s"
+          % (args.root, same, ms, tiles(), name))
+    np.savez(args.out, **results[0])
+    return 0 if same else 1
+
+
+def compare(args):
+    a, b = np.load(args.a), np.load(args.b)
+    ok = True
+    for k in sorted(a.files):
+        x, y = a[k].astype(np.float64), b[k].astype(np.float64)
+        d = float(np.abs(x - y).max())
+        good = np.array_equal(a[k], b[k])
+        what = "bit-identical"
+        ok &= good
+        print("%-8s max |diff| %.3e  max |value| %.3e  %s: %s" % (k, d, float(np.abs(x).max()), what, good))
+    print("PASS" if ok else "FAIL")
+    return 0 if ok else 1
+
+
+def main():
+    ap = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
+    sub = ap.add_subparsers(dest="cmd", required=True)
+    r = sub.add_parser("run")
+    r.add_argument("--root", default=ROOT, help="tree whose permuto_sdf_b200 package (and built library) runs")
+    r.add_argument("--out", required=True)
+    c = sub.add_parser("compare")
+    c.add_argument("a")
+    c.add_argument("b")
+    args = ap.parse_args()
+    return run(args) if args.cmd == "run" else compare(args)
+
+
+if __name__ == "__main__":
+    sys.exit(main())
