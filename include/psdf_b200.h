@@ -523,6 +523,28 @@ int psdf_surface_fit_loss(int Ns, int No, const float* sdf, const float* grad, c
                           float w_off, float scale, float* g_sdf, float* g_grad, float* acc, float* loss, float* terms, void* stream);
 /* Sphere.rand_points_inside (src/Sphere.cu) from ONE uniform draw u01 [3,n]: rows = phi / (2 pi), (cos(theta) + 1) / 2, u */
 int psdf_sphere_rand_points_inside_u01(int n, float radius, const float* u01, float* out, void* stream);
+
+/* ---------------------------------------------------------------- marching cubes (csrc/marching_cubes.cu)
+ * Replace skimage.measure.marching_cubes as extract_mesh_from_sdf_model calls it (permuto_sdf_py/utils/sdf_utils.py:280-283), on a volume
+ * [N0, N1, N2] (axis 0 = x) streamed in slabs along axis 0. A slab is S >= 1 cell slices: vol points at S + 1 slices [N1, N2] starting at
+ * global slice i0; last != 0 when its final slice is the volume's last. A corner is inside when value < threshold (NaN: outside). One vertex
+ * per crossing grid edge, at the corner plus t = (threshold - f_lo) / (f_hi - f_lo) along the edge (fp32, each operation rounded), and
+ * mapped to (x / div) * mul + off with affine_div_mul_off (a HOST array; {1, 1, 0} keeps index space). Vertices slice by slice (in-plane
+ * axis-1 edges, in-plane axis-2 edges, each row-major in (j, k), then the axis-0 edges to the next slice), faces cell by cell in row-major
+ * (i, j, k) order and in table order within a cell, so the output does not depend on the slab split. The triangle table is generated at
+ * load: face segments that cut off the inside corners of ambiguous faces, closed loops oriented inside -> outside (right-hand normal),
+ * fanned from their smallest edge (DESIGN.md §5a).
+ * Per slab: psdf_marching_cubes_count -> counts [3] (device int64) = {vertices the slab emits, triangles, crossing edges including the
+ * in-plane edges of its final slice}; the caller allocates verts [counts[0], 3] (float) and faces [counts[1], 3] (int32) and calls
+ * psdf_marching_cubes_emit with the same slab, workspace and vertex_base = vertices emitted by earlier slabs; face entries are global vertex
+ * ids, so vertex_base + counts[2] must stay below 2^31. The in-plane vertices of a slab's final slice are emitted by the next slab.
+ * workspace: psdf_marching_cubes_workspace_bytes(S, N1, N2) bytes, PSDF_ERR_UNSUPPORTED for a slab whose edges or triangles could exceed
+ * 2^31 - 1 (and for S < 1, N1 < 2 or N2 < 2). */
+long long psdf_marching_cubes_workspace_bytes(int S, int N1, int N2);
+int psdf_marching_cubes_count(int S, int N1, int N2, int i0, int last, float threshold, const float* vol, uint8_t* workspace, long long* counts,
+                              void* stream);
+int psdf_marching_cubes_emit(int S, int N1, int N2, int i0, int last, float threshold, const float* vol, long long vertex_base,
+                             const float affine_div_mul_off[3], uint8_t* workspace, float* verts, int* faces, void* stream);
 /* psdf_adamw_step over up to 8 parameter groups in one launch: device-resident step count, per-group hyper_dev [2] = {lr, weight_decay};
  * gradients scaled by grad_scale and reset to zero. n_l % 4 == 0, 16-byte aligned pointers. n and the five tables of device addresses
  * (one entry per group) are HOST arrays. The step used is step_dev[0] + step_offset (step_offset = 1: the counter is advanced afterwards

@@ -1,0 +1,179 @@
+"""Meshes from a volume or a trained SDF on the GPU (extract_mesh_from_sdf_model, permuto_sdf_py/utils/sdf_utils.py:252-292).
+
+The reference evaluates the SDF in 64^3 chunks into a dense host array of N^3 floats and runs skimage's marching cubes on the CPU. Here
+the grid is evaluated a slab of slices at a time by the fused forward kernel (FusedSDF), and each slab goes straight to the marching-cubes
+kernels (csrc/marching_cubes.cu), which carry the vertex numbering from slab to slab. The N^3 volume never exists; memory is
+O(N^2 * slab) plus the mesh. The output is a fixed function of the volume (see the header), the same for any slab split and on every run.
+"""
+import math
+
+import numpy as np
+import torch
+import torch.nn.functional as F
+
+from ._lib import call, load_library
+
+# grid points per slab: the slab's evaluation, values and edge ids (about 30 B per point in all)
+_SLAB_POINTS = 1 << 24
+_INT_MAX = 2 ** 31 - 1
+
+
+def _slab_slices(N0, N1, N2):
+    return max(1, min(N0 - 1, _SLAB_POINTS // (N1 * N2)))
+
+
+class _SlabMarchingCubes:
+    """the slab sequence of one volume: workspace, running vertex count and the pieces of the output"""
+
+    def __init__(self, N0, S, N1, N2, threshold, device, affine=(1.0, 1.0, 0.0)):
+        nbytes = int(load_library().psdf_marching_cubes_workspace_bytes(S, N1, N2))
+        if nbytes < 0:
+            raise RuntimeError("marching_cubes: a slab of %d slices of %d x %d points is more than the kernels index in 32 bits" % (S, N1, N2))
+        self.N0, self.N1, self.N2, self.thr, self.affine = N0, N1, N2, float(threshold), affine
+        self.ws = torch.empty(nbytes, dtype=torch.uint8, device=device)
+        self.counts = torch.zeros(3, dtype=torch.int64, device=device)
+        self.vbase = 0
+        self.verts, self.faces = [], []
+
+    def run(self, vol, i0):
+        """vol [S + 1, N1, N2]: slices i0 .. i0 + S; `last` when they end the volume"""
+        S = vol.shape[0] - 1
+        last = int(i0 + S == self.N0 - 1)
+        args = (S, self.N1, self.N2, i0, last, self.thr, vol)
+        call("psdf_marching_cubes_count", *args, self.ws, self.counts)
+        nv, nf, nx = self.counts.tolist()
+        if self.vbase + nx > _INT_MAX:
+            raise RuntimeError("marching_cubes: more than 2^31 - 1 vertices, which int32 faces cannot index")
+        dev = vol.device
+        verts = torch.empty(nv, 3, dtype=torch.float32, device=dev)
+        faces = torch.empty(nf, 3, dtype=torch.int32, device=dev)
+        call("psdf_marching_cubes_emit", *args, self.vbase, self.affine, self.ws, verts, faces)
+        self.vbase += nv
+        self.verts.append(verts)
+        self.faces.append(faces)
+
+    def result(self):
+        return torch.cat(self.verts), torch.cat(self.faces)
+
+
+def _check_volume(volume, threshold):
+    if not isinstance(volume, torch.Tensor) or volume.dtype != torch.float32 or not volume.is_cuda:
+        raise RuntimeError("marching_cubes: volume must be a float32 CUDA tensor")
+    if volume.dim() != 3 or min(volume.shape) < 2:
+        raise RuntimeError("marching_cubes: volume must have shape [N0, N1, N2] with every dimension >= 2, got %s" % list(volume.shape))
+    if not math.isfinite(float(threshold)):
+        raise RuntimeError("marching_cubes: threshold must be finite, got %r" % threshold)
+
+
+def _marching_cubes(volume, threshold, slab):
+    _check_volume(volume, threshold)
+    vol = volume.contiguous()
+    N0, N1, N2 = vol.shape
+    S = min(slab, N0 - 1) if slab else _slab_slices(N0, N1, N2)
+    with torch.cuda.device(vol.device):
+        mc = _SlabMarchingCubes(N0, S, N1, N2, threshold, vol.device)
+        for i0 in range(0, N0 - 1, S):
+            mc.run(vol[i0:min(i0 + S, N0 - 1) + 1], i0)
+        return mc.result()
+
+
+def marching_cubes(volume, threshold=0.0):
+    """skimage.measure.marching_cubes(volume, threshold) for a dense float32 CUDA volume [N0, N1, N2] (each >= 2), axis 0 = x.
+    -> (verts float32 [V,3] in index space, faces int32 [F,3]). A corner is inside when value < threshold; faces wind counter-clockwise
+    seen from outside (the right-hand normal points from inside to outside). Vertices come slice by slice along axis 0 and faces cell by
+    cell, in an order that depends only on the volume."""
+    return _marching_cubes(volume, threshold, None)
+
+
+class Mesh:
+    """the fields of EasyPBR's Mesh that the reference's programs read from an extracted mesh: V [V,3], F [F,3] int32, NV [V,3] (device
+    tensors)"""
+
+    def __init__(self, V, F, NV=None):
+        self.V, self.F, self.NV = V, F, NV
+
+    def remove_marked_vertices(self, mask, keep):
+        """keep=True keeps the marked vertices (create_my_meshes.py:74 with check_point_inside_primitive), keep=False removes them. Faces
+        that touch a removed vertex go; the remaining vertices keep their order and are renumbered. mask: bool [V] or [V,1], a tensor or a
+        numpy array. -> self"""
+        m = torch.as_tensor(mask).to(device=self.V.device).reshape(-1).bool()
+        if m.shape[0] != self.V.shape[0]:
+            raise RuntimeError("Mesh.remove_marked_vertices: mask has %d entries for %d vertices" % (m.shape[0], self.V.shape[0]))
+        kept = m if keep else ~m
+        new_id = torch.cumsum(kept.to(torch.int64), 0) - 1
+        F_ = self.F.long()
+        face_kept = kept[F_].all(1)
+        self.F = new_id[F_[face_kept]].to(torch.int32).reshape(-1, 3)
+        self.V = self.V[kept]
+        if self.NV is not None:
+            self.NV = self.NV[kept]
+        return self
+
+    def save_to_file(self, path):
+        """binary little-endian PLY: x y z nx ny nz (float) per vertex (zero normals when there are none), uchar int vertex_indices per
+        face"""
+        V = self.V.detach().float().cpu().contiguous()
+        NV = self.NV.detach().float().cpu() if self.NV is not None else torch.zeros_like(V)
+        Fc = self.F.detach().to(torch.int32).cpu().contiguous()
+        header = ("ply\nformat binary_little_endian 1.0\nelement vertex %d\nproperty float x\nproperty float y\nproperty float z\n"
+                  "property float nx\nproperty float ny\nproperty float nz\nelement face %d\nproperty list uchar int vertex_indices\n"
+                  "end_header\n" % (V.shape[0], Fc.shape[0]))
+        vbytes = torch.cat([V, NV], 1).numpy().astype("<f4").tobytes()
+        frec = np.empty(Fc.shape[0], dtype=[("n", "u1"), ("idx", "<i4", (3,))])
+        frec["n"] = 3
+        frec["idx"] = Fc.numpy()
+        with open(path, "wb") as f:
+            f.write(header.encode("ascii"))
+            f.write(vbytes)
+            f.write(frec.tobytes())
+
+
+@torch.no_grad()
+def extract_mesh_from_sdf_model(model, nr_points_per_dim, min_val, max_val, threshold=0, iter_nr=9999999):
+    """sdf_utils.py:252-292 for an SDF with in_channels 3: the grid linspace(min_val, max_val, N)^3 (axis 0 = x), evaluated by the model's
+    FusedSDF (value only) a slab of slices at a time and meshed on the GPU as it comes; vertices rescaled as the reference does,
+    v / fp32(N - 1) * fp32(max_val - min_val) + min_val in fp32; normals F.normalize of the SDF gradient at the vertices (outward).
+    iter_nr selects the coarse-to-fine window (the reference's 9999999: all levels). Restores model.training and model.last_iter_nr and
+    attaches nothing to the model. -> Mesh"""
+    from .fused import FusedSDF
+    if getattr(model, "in_channels", None) != 3:
+        raise RuntimeError("extract_mesh_from_sdf_model: the model has in_channels %s; meshes are extracted from a 3-D SDF (in_channels 3), "
+                           "a space-time SDF (in_channels 4) has no single surface" % getattr(model, "in_channels", None))
+    N = int(nr_points_per_dim)
+    if N < 2:
+        raise RuntimeError("extract_mesh_from_sdf_model: nr_points_per_dim must be >= 2, got %d" % N)
+    if not all(math.isfinite(float(x)) for x in (min_val, max_val, threshold)):
+        raise RuntimeError("extract_mesh_from_sdf_model: min_val, max_val and threshold must be finite")
+    fused = getattr(model, "fused", None) or FusedSDF(model)
+    dev = model.encoding.lattice_values.device
+    was_training, last_iter_nr = model.training, model.last_iter_nr
+    model.eval()
+    try:
+        with torch.cuda.device(dev):
+            lin = torch.linspace(min_val, max_val, N, device=dev)
+            S = _slab_slices(N, N, N)
+            vals = torch.empty(S + 1, N, N, device=dev)
+            mc = _SlabMarchingCubes(N, S, N, N, threshold, dev, affine=(float(N - 1), float(max_val - min_val), float(min_val)))
+            for i0 in range(0, N - 1, S):
+                i1 = min(i0 + S, N - 1)
+                first = 0 if i0 == 0 else 1
+                if first:
+                    vals[0].copy_(vals[S])               # the shared slice of the previous slab
+                rows = lin[i0 + first:i1 + 1]
+                pts = torch.stack(torch.meshgrid(rows, lin, lin, indexing="ij"), -1).reshape(-1, 3)
+                sdf = fused(pts, iter_nr, with_gradient=False, with_geom=False)[0]
+                vals[first:i1 - i0 + 1].view(-1).copy_(sdf.view(-1))
+                del pts, sdf
+                mc.run(vals[:i1 - i0 + 1], i0)
+            V, Fc = mc.result()
+            NV = torch.empty_like(V)
+            for a in range(0, V.shape[0], _SLAB_POINTS):
+                g = fused(V[a:a + _SLAB_POINTS], iter_nr, with_gradient=True, with_geom=False)[1]
+                NV[a:a + _SLAB_POINTS] = F.normalize(g, dim=1)
+        return Mesh(V, Fc, NV)
+    finally:
+        model.train(was_training)
+        model.last_iter_nr = last_iter_nr
+
+
+__all__ = ["Mesh", "marching_cubes", "extract_mesh_from_sdf_model"]
