@@ -299,7 +299,9 @@ __device__ __forceinline__ void adamw_update(float& p, float& m, float& v, float
 // which is associative (and modular, so partial sums may wrap), so the totals are the same in every run; k_fx_flush then adds them to
 // the float gradients (+=) and clears the accumulators. The accumulators are allocated when the mode is switched on.
 constexpr double kFxScale = 17179869184.0;
-__device__ __forceinline__ unsigned long long fx_of(float v) { return (unsigned long long)__double2ll_rn((double)v * kFxScale); }
+// v * 2^34 is exact in fp32 (a power-of-two scale), so rounding it to the nearest int64 gives the integer of the fp64 product (out of
+// range and NaN saturate the same way) with one conversion instead of three fp64 operations
+__device__ __forceinline__ unsigned long long fx_of(float v) { return (unsigned long long)__float2ll_rn(v * (float)kFxScale); }
 __device__ __forceinline__ void fx_add(unsigned long long* acc, float v) { atomicAdd(acc, fx_of(v)); }
 constexpr int kDetImages = 1 << 16;                 // calibration images with fixed-point gradients (later images: float atomics)
 constexpr int kDetSdfW = 64 * 64, kDetRgbW = 128 * 128;

@@ -13,7 +13,7 @@
 // Backward (k_bg_fused_backward): recompute of layers 0..5 with the pre-activations kept in the accumulator area, then the reverse sweep
 // l = 6..0: abar_l = zbar^(l) W_l on the tensor cores (warpgroups 0 / 1) beside dW_l = zbar^(l)^T a_l (warpgroups 2 / 3, fixed-point sums
 // per CTA as in fused_rgb_bwd.cu), zbar^(l-1) = abar_l gelu'(z^(l-1)) (softplus' for the density column), a_(l-1) rebuilt from the stored
-// pre-activations (a_0 from the encoder). abar_0's lattice columns leave to the workspace; k_bg_lattice_scatter scatters them.
+// pre-activations (a_0 from the encoder). abar_0's lattice columns leave to the workspace; k_lattice_scatter scatters them.
 #include "fused_common.cuh"
 #include "fused_rgb_common.cuh"
 #include "../../include/psdf_b200.h"
@@ -329,7 +329,7 @@ k_bg_fused_backward(BgParams P, const float* __restrict__ pos, const float* __re
                     build_bg_input<D>(P, lc, lattice, pos, dirs, n, valid, row, grp, s_a, s_a + kWTileBytes, false);
                 }
             } else {
-                // abar_0's lattice columns -> the exchange rows of k_bg_lattice_scatter
+                // abar_0's lattice columns -> the exchange rows of k_lattice_scatter
                 const int slot = tile * kTile + row;
                 for (int c = grp; c < (2 * P.L + 15) / 16; c += kRgbGroups) {
                     float ab[16];
@@ -369,32 +369,6 @@ k_bg_fused_backward(BgParams P, const float* __restrict__ pos, const float* __re
         if (det) { if (s_gb[i] != 0ull) atomicAdd(out.fx_mlp + kFxB + l * kBgMaxCols + dst, s_gb[i]); }
         else if (s_gbf[i] != 0.0f) atomicAdd(out.gbias[l] + dst, s_gbf[i]);
     }
-}
-
-// Encoder backward: lattice[l][idx_r] += window_l B_r abar_0[l] from the exchange rows of k_bg_fused_backward. blockIdx.y = level,
-// warp = 32 consecutive sample slots. pos, scale and shift have D columns.
-constexpr int kScatterThreads = 256;
-template <int D>
-__global__ void __launch_bounds__(kScatterThreads, 8)
-k_bg_lattice_scatter(BgParams P, const float* __restrict__ pos, const float2* __restrict__ xch, int xch_stride, const float* __restrict__ scale,
-                     const float* __restrict__ shift, const float* __restrict__ window, float* __restrict__ grad_lattice,
-                     unsigned long long* __restrict__ fx_lattice) {
-    const int slot = blockIdx.x * kScatterThreads + threadIdx.x;
-    if (slot >= xch_stride) return;                                  // whole warps (xch_stride % 128 == 0)
-    const int l = blockIdx.y, lane = threadIdx.x & 31;
-    const bool valid = slot < P.N;
-    float x[D], sc[D], sh[D];
-#pragma unroll
-    for (int i = 0; i < D; i++) {
-        x[i] = valid ? pos[(size_t)slot * D + i] : 0.0f;
-        sc[i] = scale[l * D + i];
-        sh[i] = shift ? shift[l * D + i] : 0.0f;
-    }
-    const float w = window ? window[l] : 1.0f;
-    const float2 a = xch[(size_t)l * xch_stride + slot];
-    const bool aggregate = sc[0] < kAggregateBelowScale;             // warp-uniform (l is)
-    scatter_level<false, D>(x, nullptr, sc, sh, w, a.x, a.y, 0.f, 0.f, valid, aggregate, true, lane, P.cap_mask, (unsigned)P.T,
-                            grad_lattice + (size_t)l * P.T * 2, fx_lattice ? fx_lattice + (size_t)l * P.T * 2 : nullptr);
 }
 
 // ---------------------------------------------------------------------------------------------- NeRF compositing
@@ -724,8 +698,8 @@ int nerf_fused_backward(int N, int L, int T, const float* pos, const float* dirs
     k_bg_fused_backward<D><<<persistent_grid(ntiles), kRgbThreads, smem, ST>>>(P, pos, dirs, reinterpret_cast<const float2*>(lattice),
                                                                               scale_factor, shift, window, blob, g_rgb_raw, g_density, out);
     PSDF_CHECK_LAUNCH();
-    k_bg_lattice_scatter<D><<<dim3(div_up(out.xch_stride, kScatterThreads), L), kScatterThreads, 0, ST>>>(
-        P, pos, out.xch, out.xch_stride, scale_factor, shift, window, grad_lattice, dbuf ? dbuf->rgb_lattice : nullptr);
+    k_lattice_scatter<D><<<dim3(div_up(out.xch_stride, kScatterThreads), L), kScatterThreads, 0, ST>>>(
+        P.N, P.T, P.cap_mask, pos, out.xch, out.xch_stride, scale_factor, shift, window, grad_lattice, dbuf ? dbuf->rgb_lattice : nullptr);
     PSDF_CHECK_LAUNCH();
     if (dbuf) {      // deterministic mode: fixed-point totals -> the float gradients (+=), 15 segments in two flushes
         FxSegs F, Fb;

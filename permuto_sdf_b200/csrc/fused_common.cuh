@@ -325,11 +325,12 @@ __device__ __forceinline__ void store8(uint8_t* a_hi, uint8_t* a_lo, int row, in
     *reinterpret_cast<uint4*>(a_hi + off) = make_uint4(h[0], h[1], h[2], h[3]);
     *reinterpret_cast<uint4*>(a_lo + off) = make_uint4(l[0], l[1], l[2], l[3]);
 }
-// bf16 hi / lo pair of two adjacent columns of one row -> the two operand tiles (4-byte stores; a warp covers whole 128-byte cores)
-__device__ __forceinline__ void store_pair(uint8_t* t_hi, uint8_t* t_lo, int row, int col, float x0, float x1) {
+// bf16 hi / lo pair of two adjacent columns of one row -> the two operand tiles (4-byte stores; a warp covers whole 128-byte cores);
+// sbo: the tiles' 8-row-group stride
+__device__ __forceinline__ void store_pair(uint8_t* t_hi, uint8_t* t_lo, int row, int col, float x0, float x1, int sbo = kSBO_A) {
     uint32_t h, l;
     umma::split2_bf16(x0, x1, h, l);
-    const int off = (row >> 3) * kSBO_A + (col >> 3) * kLBO + (row & 7) * 16 + (col & 7) * 2;
+    const int off = (row >> 3) * sbo + (col >> 3) * kLBO + (row & 7) * 16 + (col & 7) * 2;
     *reinterpret_cast<uint32_t*>(t_hi + off) = h;
     *reinterpret_cast<uint32_t*>(t_lo + off) = l;
 }
@@ -339,10 +340,11 @@ __device__ __forceinline__ int frag_row(int mh, int h) { return 64 * mh + 16 * (
 __device__ __forceinline__ int frag_col(int j) { return 8 * j + 2 * (threadIdx.x & 3); }
 // Columns [n0, n0 + N) of D_s = A_s W^T, s = 0 .. S-1, for the 64 rows starting `row_off` bytes into the A tiles, into the issuing
 // warpgroup's registers (umma::wg_mma_regs fragments): stream s lands in acc + 16 s, so the values of all streams at one (row, column)
-// are in the same thread. Stream s's A tiles are a + s * stream_bytes (hi) and + lo_bytes (lo); the weight tile is [Np rows][Kp] K-major.
+// are in the same thread. Stream s's A tiles are a + s * stream_bytes (hi) and + lo_bytes (lo), with the 8-row-group stride a_sbo; the
+// weight tile is [Np rows][Kp] K-major.
 template <int N, int S>
 __device__ __forceinline__ void streams_product(float* acc, const uint8_t* a, int stream_bytes, int lo_bytes, uint32_t row_off,
-                                                const uint8_t* w_hi, const uint8_t* w_lo, int Kp, int n0) {
+                                                const uint8_t* w_hi, const uint8_t* w_lo, int Kp, int n0, int a_sbo = kSBO_A) {
     static_assert(S == 1 || N <= 32, "a stream's fragment holds 16 floats");
     const uint32_t sbo_w = (Kp / 8) * kLBO, wo = (uint32_t)(n0 / 8) * sbo_w;
     const uint64_t dwh = umma::make_desc(umma::smem_u32(w_hi) + wo, kLBO, sbo_w), dwl = umma::make_desc(umma::smem_u32(w_lo) + wo, kLBO, sbo_w);
@@ -350,8 +352,8 @@ __device__ __forceinline__ void streams_product(float* acc, const uint8_t* a, in
 #pragma unroll
     for (int s = 0; s < S; s++) {
         const uint8_t* as = a + s * stream_bytes;
-        const uint64_t dah = umma::make_desc(umma::smem_u32(as) + row_off, kLBO, kSBO_A);
-        const uint64_t dal = umma::make_desc(umma::smem_u32(as + lo_bytes) + row_off, kLBO, kSBO_A);
+        const uint64_t dah = umma::make_desc(umma::smem_u32(as) + row_off, kLBO, a_sbo);
+        const uint64_t dal = umma::make_desc(umma::smem_u32(as + lo_bytes) + row_off, kLBO, a_sbo);
         umma::wg_mma_regs<N, 0, 0>(acc + 16 * s, dah, dal, dwh, dwl, (2 * kLBO) >> 4, (2 * kLBO) >> 4, Kp / 16, false);
     }
     umma::wgmma_commit();
@@ -496,6 +498,49 @@ __device__ __forceinline__ float colsum16(const float* v, int lane, int& col) {
     d += __shfl_xor_sync(kFull, d, 1);
     col = ((lane >> 4) & 1) * 8 + ((lane >> 3) & 1) * 4 + ((lane >> 2) & 1) * 2 + ((lane >> 1) & 1);
     return d;
+}
+// Column sums of a fragment block over the 8 lanes t / 4 = 0..7 of one warp (halving butterfly over lanes ^ 16, ^ 8, ^ 4, 7 shuffles): v[2 j + b]
+// is this thread's value of column 8 j + 2 (t % 4) + b. Afterwards every lane holds the sum of one column, `col` = 8 (2 bit4 + bit3) +
+// 2 (t % 4) + bit2.
+__device__ __forceinline__ float frag_colsum8(const float* v, int lane, int& col) {
+    float a[4], b[2], c;
+    bool up = lane & 16;
+#pragma unroll
+    for (int i = 0; i < 4; i++) { float send = up ? v[i] : v[i + 4], keep = up ? v[i + 4] : v[i]; a[i] = keep + __shfl_xor_sync(kFull, send, 16); }
+    up = lane & 8;
+#pragma unroll
+    for (int i = 0; i < 2; i++) { float send = up ? a[i] : a[i + 2], keep = up ? a[i + 2] : a[i]; b[i] = keep + __shfl_xor_sync(kFull, send, 8); }
+    up = lane & 4;
+    { float send = up ? b[0] : b[1], keep = up ? b[1] : b[0]; c = keep + __shfl_xor_sync(kFull, send, 4); }
+    col = 8 * (2 * ((lane >> 4) & 1) + ((lane >> 3) & 1)) + 2 * (lane & 3) + ((lane >> 2) & 1);
+    return c;
+}
+// Bias-gradient column sums of an M = 64 fragment block over each 32-row group, i.e. over the warp pair 2p, 2p + 1 of a warpgroup.
+// v: this thread's 16 values (v[4 j + 2 h + b], umma::wg_mma_regs layout), columns 8 j + 2 (t % 4) + b of which the first nn count (rows
+// outside the problem hold 0). The rows r = 0..31 of the group are added in the order of colsum16 over one warp in the per-row layout:
+// pairs r, r ^ 16 first, then r ^ 8, r ^ 4, r ^ 2, r ^ 1. Here bit 4 of r is the warp of the pair, bit 3 the fragment half h and bits 2..0
+// the lane bits 4..2, so the odd warp's values come through shared memory (bx: the pair's [16][32] floats), then h, then
+// frag_colsum8's butterfly. Every partial sum, and so the one fixed-point rounding per tile, column and 32 rows, is that of the per-row
+// sum. Both warps of the pair call it (named barrier bar_id); true in the even warp's lanes that hold the sum `cs` of a column col < nn.
+__device__ __forceinline__ bool frag_pair_colsum(const float* v, int nn, float* bx, int bar_id, float& cs, int& col) {
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    bx += lane;
+    if (warp & 1) {
+#pragma unroll
+        for (int i = 0; i < 16; i++) if (2 * i < nn) bx[i * 32] = v[i];
+    }
+    umma::bar_sync(bar_id, 64);
+    if (warp & 1) return false;
+    float bs[8];
+#pragma unroll
+    for (int j = 0; j < 4; j++)
+#pragma unroll
+        for (int b = 0; b < 2; b++) {
+            const int i0 = 4 * j + b, i1 = 4 * j + 2 + b;
+            bs[2 * j + b] = (8 * j < nn) ? (v[i0] + bx[i0 * 32]) + (v[i1] + bx[i1 * 32]) : 0.f;
+        }
+    cs = frag_colsum8(bs, lane, col);
+    return col < nn;
 }
 
 

@@ -1,28 +1,36 @@
 // Training backward of the fused colour network (sm_90a, wgmma): d loss / d (linear rgb) per sample in ->
-// lattice gradient (scatter fused), d loss / d sdf-gradient (through the normalisation), d loss / d geom feature,
-// weight + bias gradients of the 4 linear layers. Replaces loss.backward() through RGB.forward
-// (permuto_sdf_py/models/models.py:395-414) -- encoding backward, 4 x (GELU backward, 2 GEMMs), normalize / cat backward.
+// lattice gradient, d loss / d sdf-gradient (through the normalisation), d loss / d geom feature, weight + bias gradients of the 4
+// linear layers. Replaces loss.backward() through RGB.forward (permuto_sdf_py/models/models.py:395-414) -- encoding backward,
+// 4 x (GELU backward, 2 GEMMs), normalize / cat backward. Three kernels: the persistent tensor-core kernel below, the cross-CTA sum of
+// its weight-gradient sums (k_rgb_dw_reduce) and the full-occupancy lattice scatter k_lattice_scatter (fused_rgb_common.cuh, shared
+// with the background backward).
 //
-// Per 128-sample tile (512 threads: row = tid & 127, group = tid >> 7):
-//   1. input tile a_0 (encoder gather + SH + normal + geom) as in the forward; a_0 leaves by ONE TMA store (64 KB / tile, re-read from
-//      L2 by the same CTA for dW_0: the only spill);
-//   2. forward recompute, layers 0..2 on the tensor cores; pre-activations z^(0), z^(1), z^(2) STAY in the accumulator area
-//      (128 + 128 + 64 columns);
-//   3. reverse sweep l = 3..0: zbar^(l) tile -> MMA with W_l^T -> abar_l -> zbar^(l-1) = abar_l gelu'(z^(l-1)); beside that GEMM the
-//      layer's input a_l is rebuilt from the stored z^(l-1) (a_0 returns by TMA) and the WEIGHT GRADIENT dW_l = zbar^(l)^T a_l is
-//      formed on the tensor cores from the two tiles as they sit in shared memory: the sample axis is the MMA K dimension and an
-//      operand tile in the K-major core-matrix layout is an MN-major operand for that product (see fused_sdf_bwd.cu). The issuing
-//      warpgroups add the product from their registers to the CTA's fixed-point sums (each slot owned by one thread: no atomics); the
-//      CTA flushes the four sums once, after its last tile -- 37 k reductions per CTA instead of per tile, with the same totals as a
-//      per-tile fixed-point flush;
-//      bias gradients = column sums (shuffles + shared atomics);
-//   4. abar_0 -> lattice scatter (scatter_level without the tangent term: warp-aggregated red.global.add.v2.f32), normal -> sdf-gradient,
-//      geom gradient.
+// Per 128-sample tile (512 threads). Every product lands in the registers of the warpgroup that issues it: warpgroup (mh, nh) =
+// (wgi & 1, wgi >> 1) forms rows 64 mh .. 64 mh + 63 x column half nh (split_n) and consumes them in place.
+//   1. input tile a_0 (encoder gather + SH + normal + geom, per-row layout: row = tid & 127, group = tid >> 7) as in the forward; a_0
+//      leaves by ONE TMA store (64 KB / tile, re-read from L2 by the same CTA for dW_0: the only spill);
+//   2. forward recompute, layers 0..2: a_{l+1} = gelu(z^(l) + b_l) -> s_a straight from the fragments; the raw z^(l) go to this thread's
+//      slots of the CTA's stash (global, L2 resident) and come back to the same thread in the reverse sweep: the reverse step l splits
+//      its Kp_l = Np_{l-1} columns exactly as the forward layer l-1 split them, so it needs no barrier;
+//   3. seed zbar^(3) = d loss / d linear rgb -> s_z;
+//   4. reverse sweep l = 3..0, s_z = zbar^(l), s_a = a_l: abar_l = zbar^(l) W_l (transposed weight block as the B operand) and a share
+//      of the WEIGHT GRADIENT dW_l = zbar^(l)^T a_l, formed on the tensor cores from the two tiles as they sit in shared memory (the
+//      sample axis is the MMA K dimension and an operand tile in the K-major core-matrix layout is an MN-major operand for that
+//      product, see fused_sdf_bwd.cu). Each warpgroup adds its dW pieces from its registers to the CTA's fixed-point sums (each slot
+//      owned by one thread: no atomics); k_rgb_dw_reduce adds up the CTAs' sums after the launch -- with the same totals as a per-tile
+//      fixed-point flush. After a barrier the fragments become zbar^(l-1) = abar_l gelu'(z^(l-1)) -> s_z, the bias gradient
+//      (frag_pair_colsum: the bits of the per-row colsum16), and a_{l-1} is rebuilt into s_a from the stashed z^(l-2) (l = 3, 2) or
+//      comes back by TMA (l = 1);
+//   5. l = 0: abar_0's lattice columns leave from the registers to the exchange rows of the workspace ([level][tile * 128 + row]
+//      float2, a thread's column pair is one level) for k_lattice_scatter; the normal and geom columns pass through a small fp32
+//      staging tile over s_z to the per-row tail: normal -> sdf-gradient (= or +=), geom gradient.
 // Deterministic mode (common.cuh): every gradient is summed in fixed point instead and added to the float gradients by the flush that
-// follows the launch.
+// follows the launches.
 // Weights stream per layer through one 64 KB buffer by TMA; the next block is requested as soon as the MMAs that read the
 // current one have retired, so the copy hides behind the epilogue.
-// Accumulator map (umma.cuh): [0,128) z^(0) | [128,256) z^(1) | [256,384) z^(2) | [384,512) work. Weight-gradient sums: g_dw_rgb_bwd.
+// Stash of a CTA (float4 slots, slot index * 512 + tid): z^(l) fragments of layer l at [8 l, 8 l + 8). Weight-gradient sums: g_dw_rgb_bwd.
+#include <cstdio>
+#include <cstdlib>
 #include "fused_common.cuh"
 #include "fused_rgb_common.cuh"
 #include "../../include/psdf_b200.h"
@@ -31,26 +39,57 @@ using namespace psdf_fused;
 using namespace psdf_rgb;
 
 namespace {
-__device__ float g_acc_rgb_bwd[(size_t)kAccCtas * kTile * 512];     // accumulator areas (umma.cuh)
+constexpr int kStashSlots = 24;
+__device__ float4 g_stash_rgb_bwd[(size_t)kAccCtas * kStashSlots * kRgbThreads];     // per-CTA stashes, 192 KB each
 // weight-gradient sums of each CTA in fixed point (common.cuh fx_of), [CTA][layer][128 rows][128 columns]
 constexpr int kDwSlots = kNL * 128 * 128;
 __device__ unsigned long long g_dw_rgb_bwd[(size_t)kAccCtas * kDwSlots];
 constexpr int kFxW = kDetRgbW, kFxB = 4 * kDetRgbW;    // weight / bias offsets in DetBufs::rgb_mlp
 constexpr int kRgbSpillBytes = 2 * kWTileBytes;      // [hi | lo] of one operand tile
+constexpr int kTailCols = 3 + kGeomDim;              // abar_0 columns of the normal and the geom feature
+constexpr int kTailLd = kTailCols + 1;               // row stride of their fp32 staging tile
+constexpr int kBxBytes = 8 * 16 * 32 * sizeof(float);   // odd warps' fragments of the bias column sums, [8 warp pairs][16][32 lanes]
 
 struct RgbSpill {
     uint8_t* a0;         // [ntiles][64 KB] input tiles a_0 (written and re-read by the same CTA)
+    float2* xch;         // [L][xch_stride] abar_0 of every level and sample slot (tile * 128 + row)
+    int xch_stride;      // sample slots = ntiles * 128
     float* gW[kNL];      // [N_l, K_l] (+=)
     float* gbias[kNL];   // (+=)
-    unsigned long long* fx_lattice;   // deterministic mode: fixed-point accumulators (DetBufs::rgb_lattice, ::rgb_mlp), else NULL
-    unsigned long long* fx_mlp;
+    unsigned long long* fx_mlp;         // deterministic mode: fixed-point accumulators (DetBufs::rgb_mlp), else NULL
+    unsigned long long* phase_cycles;   // [16] += clock64 deltas of thread 0 per phase (PSDF_PHASE_TIMING=1, diagnostics), else NULL
 };
+// phase ids of the diagnostic counters
+enum { kPhEncoder = 0, kPhForward0 = 1, kPhSeed = 4, kPhReverse3 = 5, kPhTail = 9, kPhFlush = 10, kPhTiles = 11 };
+#define PSDF_PHASE(id)                                                                     \
+    do {                                                                                   \
+        if (sp.phase_cycles && tid == 0) {                                                 \
+            const long long now_ = clock64();                                              \
+            atomicAdd(sp.phase_cycles + (id), (unsigned long long)(now_ - phase_t0));      \
+            phase_t0 = now_;                                                               \
+        }                                                                                  \
+    } while (0)
+
+// rows 64 mh .. 64 mh + 63 x columns [n0, n0 + nn) of [128 x K] x [Nw x K]^T into the issuing warpgroup's registers: streams_product on
+// the 128-column tiles (A = 128 rows with the 2048-byte row-group stride, weight block [Nw rows][K] K-major)
+__device__ __forceinline__ void tile_product(float* acc, int nn, int mh, const uint8_t* a, const uint8_t* w_hi, const uint8_t* w_lo, int K, int n0) {
+#pragma unroll
+    for (int i = 0; i < 32; i++) acc[i] = 0.f;
+    const uint32_t ro = (uint32_t)(mh * 8 * kWSBO);
+    switch (nn / 16) {
+        case 1: streams_product<16, 1>(acc, a, 0, kWTileBytes, ro, w_hi, w_lo, K, n0, kWSBO); break;
+        case 2: streams_product<32, 1>(acc, a, 0, kWTileBytes, ro, w_hi, w_lo, K, n0, kWSBO); break;
+        case 3: streams_product<48, 1>(acc, a, 0, kWTileBytes, ro, w_hi, w_lo, K, n0, kWSBO); break;
+        case 4: streams_product<64, 1>(acc, a, 0, kWTileBytes, ro, w_hi, w_lo, K, n0, kWSBO); break;
+        default: break;
+    }
+}
+
 __global__ void __launch_bounds__(kRgbThreads, 1)
 k_rgb_fused_backward(RgbParams P, const float* __restrict__ pos, const float* __restrict__ dirs, const float* __restrict__ sdf_grad,
                      const float* __restrict__ geom, const float2* __restrict__ lattice, const float* __restrict__ scale,
                      const float* __restrict__ shift, const float* __restrict__ window, const uint8_t* __restrict__ blob,
-                     const float* __restrict__ g_out, float* __restrict__ grad_lattice, float* __restrict__ g_sdf_grad,
-                     float* __restrict__ g_geom, RgbSpill sp) {
+                     const float* __restrict__ g_out, float* __restrict__ g_sdf_grad, float* __restrict__ g_geom, RgbSpill sp) {
     extern __shared__ __align__(128) uint8_t smem[];
     uint8_t* s_a = smem;                                   // activation tiles [hi | lo]
     uint8_t* s_z = s_a + 2 * kWTileBytes;                  // adjoint tiles [hi | lo]
@@ -61,25 +100,22 @@ k_rgb_fused_backward(RgbParams P, const float* __restrict__ pos, const float* __
     unsigned long long* s_gb = reinterpret_cast<unsigned long long*>(s_bias + kNL * 128);
     float* s_gbf = reinterpret_cast<float*>(s_gb);
     const bool det = sp.fx_mlp != nullptr;
-    uint64_t* bars = reinterpret_cast<uint64_t*>(s_gb + kNL * 128);   // [0] weights, [1] reverse MMAs, [2] dW MMAs, [3] a_0 reload
-    // exchange tile abar_0: [128][K0 + 1] fp32 over s_a and, for K0 = 128 (L >= 28), the start of s_z; written after the last reverse
-    // step's MMAs, the only readers of both, have completed
-    float* s_x = reinterpret_cast<float*>(s_a);
+    uint64_t* bars = reinterpret_cast<uint64_t*>(s_gb + kNL * 128);   // [0] weights, [1] a_0 reload
+    float* s_bx = reinterpret_cast<float*>(bars + 8);      // bias column sums: the odd warps' fragments (frag_pair_colsum)
+    // staging tile of abar_0's normal | geom columns, [128][kTailLd] fp32 over s_z: written after the last reverse step's products,
+    // the last readers of s_z in the tile, have completed
+    float* s_tail = reinterpret_cast<float*>(s_z);
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int row = tid & 127, grp = tid >> 7;
-    const int K0 = P.g.Kp[0];
+    const int wgi = warp >> 2, mh = wgi & 1, nh = wgi >> 1;
+    const int pair = 2 * wgi + ((warp & 3) >> 1);          // 32-row group of this warp's fragment rows
+    float4* stash = g_stash_rgb_bwd + (size_t)blockIdx.x * kStashSlots * kRgbThreads + tid;     // this thread's slot 0
     if (tid == 0) {
         umma::mbar_init(&bars[0], 1);
-        umma::mbar_init(&bars[1], 2 * 128);
-        umma::mbar_init(&bars[2], 2 * 128);
-        umma::mbar_init(&bars[3], 1);
+        umma::mbar_init(&bars[1], 1);
         umma::mbar_fence_init();
-        umma::acc_attach(g_acc_rgb_bwd + (size_t)blockIdx.x * kTile * 512, 512);
     }
-    // reverse sweep: warpgroups 0 / 1 issue the row halves of the GEMM chain, warpgroups 2 / 3 the weight-gradient products beside it
-    const int wgi = warp >> 2;
-    const bool dw_issuer = wgi >= 2;
     load_level_consts(lc, P.L, scale, shift, window, tid, kRgbThreads);
     for (int i = tid; i < kNL * 128; i += kRgbThreads) {
         int l = i >> 7, c = i & 127;
@@ -87,20 +123,18 @@ k_rgb_fused_backward(RgbParams P, const float* __restrict__ pos, const float* __
         s_gb[i] = 0ull;        // also clears s_gbf
     }
     __syncthreads();
-    const uint32_t tmem_base = 0;
-    const uint32_t tmem_z[3] = {tmem_base, tmem_base + 128, tmem_base + 256};
-    const uint32_t tmem_work = tmem_base + 384;
-    const uint32_t lane_off = (uint32_t)((warp & 3) * 32) << 16;
-    uint32_t w_phase = 0, mma_phase = 0, dw_phase = 0, a0_phase = 0;
+    uint32_t w_phase = 0, a0_phase = 0;
     unsigned long long* dw_cta = g_dw_rgb_bwd + (size_t)blockIdx.x * kDwSlots;    // this CTA's weight-gradient sums, layer l at l * 128 * 128
 
     const int ntiles = (P.N + kTile - 1) / kTile;
     if (tid == 0 && blockIdx.x < ntiles) load_layer_weights(s_w, blob, P.g, 0, false, &bars[0]);
+    long long phase_t0 = sp.phase_cycles ? clock64() : 0;
     for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
         const bool first_tile = tile == (int)blockIdx.x;
         const int n = tile * kTile + row;
         const bool valid = n < P.N;
         build_input_tile(P, lc, lattice, pos, dirs, sdf_grad, geom, n, valid, row, grp, s_a, s_a + kWTileBytes);
+        PSDF_PHASE(kPhEncoder);
 
         // ---------------- forward recompute, layers 0..2
 #pragma unroll 1
@@ -113,18 +147,34 @@ k_rgb_fused_backward(RgbParams P, const float* __restrict__ pos, const float* __
                 umma::bulk_s2g(sp.a0 + (size_t)tile * kRgbSpillBytes, s_a, kRgbSpillBytes);
                 umma::bulk_commit();
             }
-            issue_gemm_w(tmem_z[l], wgi, s_a, s_a + kWTileBytes, s_w, s_w + P.g.Np[l] * P.g.Kp[l] * 2, P.g.Kp[l], P.g.Np[l]);
+            int n0, nn;
+            split_n(P.g.Np[l], nh, n0, nn);
+            float acc[32];
+            tile_product(acc, nn, mh, s_a, s_w, s_w + P.g.Np[l] * P.g.Kp[l] * 2, P.g.Kp[l], n0);
             if (l == 0 && tid == 0) umma::bulk_wait_read0();      // s_a is overwritten by this layer's epilogue: the store must have read it
-            __syncthreads();
+            __syncthreads();                                       // every product has read s_a and s_w
             if (tid == 0) load_layer_weights(s_w, blob, P.g, l < 2 ? l + 1 : 3, l == 2, &bars[0]);   // W_{l+1}, then W_3^T
-            for (int c = grp; c < P.g.Np[l] / 16; c += kRgbGroups) {
-                float z[16];
-                umma::tmem_ld16(tmem_z[l] + lane_off + c * 16, z);
+            // raw z^(l) -> this thread's stash slots (read back by this thread in the reverse steps l + 1 and l + 2), a_{l+1} -> s_a
 #pragma unroll
-                for (int i = 0; i < 16; i++) { const float zz = z[i] + s_bias[l * 128 + c * 16 + i]; z[i] = zz * gelu_eval(zz).cdf; }
-                store8w(s_a, s_a + kWTileBytes, row, 2 * c, z);
-                store8w(s_a, s_a + kWTileBytes, row, 2 * c + 1, z + 8);
+            for (int j = 0; j < 8; j++)
+                if (8 * j < nn) stash[(8 * l + j) * kRgbThreads] = make_float4(acc[4 * j], acc[4 * j + 1], acc[4 * j + 2], acc[4 * j + 3]);
+#pragma unroll
+            for (int j = 0; j < 8; j++) {
+                if (8 * j < nn) {
+#pragma unroll
+                    for (int h = 0; h < 2; h++) {
+                        const int r = frag_row(mh, h), c = n0 + frag_col(j);
+                        float a[2];
+#pragma unroll
+                        for (int b = 0; b < 2; b++) {
+                            const float zz = acc[4 * j + 2 * h + b] + s_bias[l * 128 + c + b];
+                            a[b] = zz * gelu_eval(zz).cdf;
+                        }
+                        store_pair(s_a, s_a + kWTileBytes, r, c, a[0], a[1], kWSBO);
+                    }
+                }
             }
+            PSDF_PHASE(kPhForward0 + l);
         }
         // ---------------- seed: zbar^(3) = d loss / d linear rgb (3 of 16 padded columns)
         if (grp == 0) {
@@ -140,166 +190,180 @@ k_rgb_fused_backward(RgbParams P, const float* __restrict__ pos, const float* __
                 else atomicAdd(&s_gbf[3 * 128 + col], cs);
             }
         }
-        // ---------------- reverse sweep, layers 3..0: s_z = zbar^(l), s_a = a_l (l = 3: still there from the forward)
+        PSDF_PHASE(kPhSeed);
+        // ---------------- reverse sweep, layers 3..0: s_z = zbar^(l), s_a = a_l
+        const bool rvalid0 = tile * kTile + frag_row(mh, 0) < P.N, rvalid1 = tile * kTile + frag_row(mh, 1) < P.N;   // fragment rows
 #pragma unroll 1
         for (int l = 3; l >= 0; l--) {
             umma::mbar_wait(&bars[0], w_phase);
             w_phase ^= 1;
+            if (l == 0) umma::mbar_wait(&bars[1], a0_phase);      // a_0 is back in s_a
             umma::fence_async_smem();
             __syncthreads();
-            const int Mdw = P.g.Np[l] > 64 ? 128 : 64;
-            if (!dw_issuer) {
-                // abar_l [128 x Kp_l] = zbar^(l) [128 x Np_l] W_l : B operand = W_l^T stored [Kp_l rows][Np_l]; both column halves
-                for (int nh = 0; nh < 2; nh++)
-                    issue_gemm_w(tmem_work, wgi + 2 * nh, s_z, s_z + kWTileBytes, s_w, s_w + P.g.Np[l] * P.g.Kp[l] * 2, P.g.Np[l], P.g.Kp[l]);
-                umma::mbar_arrive(&bars[1]);
-            }
-            if (dw_issuer && l == 3) {                    // a_3 | zbar^(3) are both in place
-                issue_dw_w(dw_cta + 3 * 128 * 128, wgi - 2, s_z, s_a, Mdw, P.g.Kp[3], first_tile);
-                umma::mbar_arrive(&bars[2]);
-            }
-            // beside the MMAs: gelu'(z^(l-1)) of this thread's column chunks from the stored pre-activations, and the layer's
-            // input a_l = gelu(z^(l-1)) back into s_a (its previous content a_(l+1) was last read by dW_(l+1), complete since the
-            // previous step's epilogue waited for it)
-            const int Kp = P.g.Kp[l];
-            float g1a[16], g1b[16];                       // chunks grp and grp + 4 (Kp <= 128 -> at most two chunks per thread)
-            if (l > 0) {
-#pragma unroll
-                for (int j = 0; j < 2; j++) {
-                    const int c = grp + j * kRgbGroups;
-                    if (c < Kp / 16) {
-                        float z[16];
-                        umma::tmem_ld16(tmem_z[l - 1] + lane_off + c * 16, z);
-#pragma unroll
-                        for (int i = 0; i < 16; i++) {
-                            const float zz = z[i] + s_bias[(l - 1) * 128 + c * 16 + i];
-                            const GeluEval ge = gelu_eval(zz);
-                            (j == 0 ? g1a : g1b)[i] = fmaf(zz, ge.pdf, ge.cdf);
-                            z[i] = zz * ge.cdf;
-                        }
-                        if (l < 3) {
-                            store8w(s_a, s_a + kWTileBytes, row, 2 * c, z);
-                            store8w(s_a, s_a + kWTileBytes, row, 2 * c + 1, z + 8);
-                        }
-                    }
-                }
-            }
-            if (l < 3) {
-                if (l == 0 && tid == 0) {                 // a_0 returns by TMA (its store completed long ago)
-                    umma::bulk_wait0();
-                    umma::mbar_expect_tx(&bars[3], (uint32_t)kRgbSpillBytes);
-                    umma::bulk_g2s(s_a, sp.a0 + (size_t)tile * kRgbSpillBytes, (uint32_t)kRgbSpillBytes, &bars[3]);
-                }
-                umma::fence_async_smem();
-                __syncthreads();
-                if (dw_issuer) {
-                    if (l == 0) umma::mbar_wait(&bars[3], a0_phase);
-                    issue_dw_w(dw_cta + l * 128 * 128, wgi - 2, s_z, s_a, Mdw, Kp, first_tile);
-                    umma::mbar_arrive(&bars[2]);
-                }
-            }
-            umma::mbar_wait(&bars[1], mma_phase);
-            mma_phase ^= 1;
+            const int Np = P.g.Np[l], Kp = P.g.Kp[l];
+            if (!first_tile) prefetch_dw_w(dw_cta + l * 128 * 128, mh, Np > 64 ? 128 : 64, Kp, nh, 2);
+            int n0, nn;
+            split_n(Kp, nh, n0, nn);
+            float acc[32];
+            // abar_l [128 x Kp] = zbar^(l) [128 x Np] W_l: B operand = W_l^T stored [Kp rows][Np]
+            tile_product(acc, nn, mh, s_z, s_w, s_w + Np * Kp * 2, Np, n0);
+            // dW_l: the row half mh, every other 32-column piece of it
+            issue_dw_w(dw_cta + l * 128 * 128, mh, s_z, s_a, Np > 64 ? 128 : 64, Kp, first_tile, nh, 2);
+            __syncthreads();                                       // every product of this step has read s_z, s_a and s_w
             if (tid == 0) {
                 if (l > 0) load_layer_weights(s_w, blob, P.g, l - 1, true, &bars[0]);
                 else if (tile + (int)gridDim.x < ntiles) load_layer_weights(s_w, blob, P.g, 0, false, &bars[0]);
+                if (l == 1) {                  // s_a is free: a_0 returns by TMA for the last step (its store completed long ago)
+                    umma::bulk_wait0();
+                    umma::mbar_expect_tx(&bars[1], (uint32_t)kRgbSpillBytes);
+                    umma::bulk_g2s(s_a, sp.a0 + (size_t)tile * kRgbSpillBytes, (uint32_t)kRgbSpillBytes, &bars[1]);
+                }
             }
-            // s_z (and, for l = 0, the exchange tile over s_a) may only be written once the dW_l MMAs that read them have completed
-            umma::mbar_wait(&bars[2], dw_phase);
-            dw_phase ^= 1;
             if (l > 0) {
+                // zbar^(l-1) = abar_l gelu'(z^(l-1)) -> s_z from this thread's stashed z^(l-1); acc keeps it on the valid rows (0 elsewhere)
+                // for the bias gradient of layer l - 1
 #pragma unroll
-                for (int j = 0; j < 2; j++) {
-                    const int c = grp + j * kRgbGroups;
-                    if (c >= Kp / 16) continue;
-                    float ab[16];
-                    umma::tmem_ld16(tmem_work + lane_off + c * 16, ab);
+                for (int j = 0; j < 8; j++) {
+                    if (8 * j < nn) {
+                        const float4 z4 = stash[(8 * (l - 1) + j) * kRgbThreads];
+                        const float z[4] = {z4.x, z4.y, z4.z, z4.w};
 #pragma unroll
-                    for (int i = 0; i < 16; i++) ab[i] *= (j == 0 ? g1a : g1b)[i];
-                    store8w(s_z, s_z + kWTileBytes, row, 2 * c, ab);
-                    store8w(s_z, s_z + kWTileBytes, row, 2 * c + 1, ab + 8);
-                    if (!valid) {
+                        for (int h = 0; h < 2; h++) {
+                            const int r = frag_row(mh, h), c = n0 + frag_col(j);
+                            float zb[2];
 #pragma unroll
-                        for (int i = 0; i < 16; i++) ab[i] = 0.f;
+                            for (int b = 0; b < 2; b++) {
+                                const int i = 4 * j + 2 * h + b;
+                                const float zz = z[2 * h + b] + s_bias[(l - 1) * 128 + c + b];
+                                const GeluEval ge = gelu_eval(zz);
+                                zb[b] = acc[i] * fmaf(zz, ge.pdf, ge.cdf);
+                                acc[i] = (h ? rvalid1 : rvalid0) ? zb[b] : 0.f;
+                            }
+                            store_pair(s_z, s_z + kWTileBytes, r, c, zb[0], zb[1], kWSBO);
+                        }
                     }
-                    int col;
-                    const float cs = colsum16(ab, lane, col);
-                    if (!(lane & 1)) {
-                        if (det) fx_add(&s_gb[(l - 1) * 128 + c * 16 + col], cs);
-                        else atomicAdd(&s_gbf[(l - 1) * 128 + c * 16 + col], cs);
+                }
+                // bias gradient of layer l - 1: column sums over each 32-row group, 32 columns at a time
+#pragma unroll
+                for (int q = 0; q < 2; q++) {
+                    if (32 * q < nn) {
+                        if (q) umma::bar_sync(1 + pair, 64);       // the even warp has read the first block's exchange
+                        float cs;
+                        int col;
+                        if (frag_pair_colsum(acc + 16 * q, nn - 32 * q, s_bx + pair * 16 * 32, 1 + pair, cs, col)) {
+                            if (det) fx_add(&s_gb[(l - 1) * 128 + n0 + 32 * q + col], cs);
+                            else atomicAdd(&s_gbf[(l - 1) * 128 + n0 + 32 * q + col], cs);
+                        }
+                    }
+                }
+                if (l >= 2) {
+                    // a_{l-1} = gelu(z^(l-2)) -> s_a from this thread's stashed z^(l-2) (the forward layer l - 2 split its columns as the
+                    // reverse step l - 1 does)
+                    int m0, mn;
+                    split_n(P.g.Np[l - 2], nh, m0, mn);
+#pragma unroll
+                    for (int j = 0; j < 8; j++) {
+                        if (8 * j < mn) {
+                            const float4 z4 = stash[(8 * (l - 2) + j) * kRgbThreads];
+                            const float z[4] = {z4.x, z4.y, z4.z, z4.w};
+#pragma unroll
+                            for (int h = 0; h < 2; h++) {
+                                const int r = frag_row(mh, h), c = m0 + frag_col(j);
+                                float a[2];
+#pragma unroll
+                                for (int b = 0; b < 2; b++) {
+                                    const float zz = z[2 * h + b] + s_bias[(l - 2) * 128 + c + b];
+                                    a[b] = zz * gelu_eval(zz).cdf;
+                                }
+                                store_pair(s_a, s_a + kWTileBytes, r, c, a[0], a[1], kWSBO);
+                            }
+                        }
                     }
                 }
             } else {
-                for (int c = grp; c < Kp / 16; c += kRgbGroups) {
-                    float ab[16];
-                    umma::tmem_ld16(tmem_work + lane_off + c * 16, ab);
+                // abar_0: lattice columns -> the exchange rows (a thread's column pair is one level), normal | geom -> the staging tile
+                const int tail0 = P.enc_cols + kShCols;
 #pragma unroll
-                    for (int i = 0; i < 16; i++) s_x[row * (K0 + 1) + c * 16 + i] = ab[i];
+                for (int j = 0; j < 8; j++) {
+                    if (8 * j < nn) {
+#pragma unroll
+                        for (int h = 0; h < 2; h++) {
+                            const int r = frag_row(mh, h), c = n0 + frag_col(j), i = 4 * j + 2 * h;
+                            if (c < 2 * P.L) sp.xch[(size_t)(c >> 1) * sp.xch_stride + tile * kTile + r] = make_float2(acc[i], acc[i + 1]);
+#pragma unroll
+                            for (int b = 0; b < 2; b++)
+                                if (c + b >= tail0 && c + b < tail0 + kTailCols) s_tail[r * kTailLd + c + b - tail0] = acc[i + b];
+                        }
+                    }
                 }
             }
+            PSDF_PHASE(kPhReverse3 + (3 - l));
         }
         a0_phase ^= 1;
         __syncthreads();
-        // ---------------- encoder / tail backward from abar_0
-        {
-            const float* xr = s_x + row * (K0 + 1);
-            float x[3] = {0.f, 0.f, 0.f};
-            if (valid) { x[0] = pos[(size_t)n * 3]; x[1] = pos[(size_t)n * 3 + 1]; x[2] = pos[(size_t)n * 3 + 2]; }
-            for (int l = grp; l < P.L; l += kRgbGroups) {
-                const bool aggregate = lc->scale[l * 4] < kAggregateBelowScale;       // warp-uniform (l is)
-                scatter_level<false>(x, nullptr, lc->scale + l * 4, lc->shift + l * 4, lc->window[l], xr[2 * l], xr[2 * l + 1], 0.f, 0.f, valid,
-                                     aggregate, true, lane, P.cap_mask, (unsigned)P.T, grad_lattice + (size_t)l * P.T * 2,
-                                     det ? sp.fx_lattice + (size_t)l * P.T * 2 : nullptr);
-            }
-            if (valid) {
-                const int tail = P.enc_cols;          // SH at [tail, tail+25), normal at tail+25.., geom at tail+28..
-                if (g_geom) {
-                    float* gg = g_geom + (size_t)n * kGeomDim + grp * 8;
+        // ---------------- tail: normal -> sdf-gradient, geom gradient (per row)
+        if (valid) {
+            const float* xr = s_tail + row * kTailLd;
+            if (g_geom) {
+                float* gg = g_geom + (size_t)n * kGeomDim + grp * 8;
 #pragma unroll
-                    for (int i = 0; i < 8; i++) gg[i] = xr[tail + kShCols + 3 + grp * 8 + i];
+                for (int i = 0; i < 8; i++) gg[i] = xr[3 + grp * 8 + i];
+            }
+            if (grp == 3 && g_sdf_grad) {
+                const float gx = sdf_grad[(size_t)n * 3], gy = sdf_grad[(size_t)n * 3 + 1], gz = sdf_grad[(size_t)n * 3 + 2];
+                const float nrm = sqrtf(gx * gx + gy * gy + gz * gz);
+                const float inv = 1.0f / fmaxf(nrm, 1e-12f);
+                const float bx = xr[0], by = xr[1], bz = xr[2];
+                float ox = bx * inv, oy = by * inv, oz = bz * inv;
+                if (nrm > 1e-12f) {           // d (g / |g|) : (I - n n^T) / |g|
+                    const float nx = gx * inv, ny = gy * inv, nz = gz * inv;
+                    const float d = nx * bx + ny * by + nz * bz;
+                    ox -= nx * d * inv; oy -= ny * d * inv; oz -= nz * d * inv;
                 }
-                if (grp == 3 && g_sdf_grad) {
-                    const float gx = sdf_grad[(size_t)n * 3], gy = sdf_grad[(size_t)n * 3 + 1], gz = sdf_grad[(size_t)n * 3 + 2];
-                    const float nrm = sqrtf(gx * gx + gy * gy + gz * gz);
-                    const float inv = 1.0f / fmaxf(nrm, 1e-12f);
-                    const float bx = xr[tail + kShCols], by = xr[tail + kShCols + 1], bz = xr[tail + kShCols + 2];
-                    float ox = bx * inv, oy = by * inv, oz = bz * inv;
-                    if (nrm > 1e-12f) {           // d (g / |g|) : (I - n n^T) / |g|
-                        const float nx = gx * inv, ny = gy * inv, nz = gz * inv;
-                        const float d = nx * bx + ny * by + nz * bz;
-                        ox -= nx * d * inv; oy -= ny * d * inv; oz -= nz * d * inv;
-                    }
-                    float* o = g_sdf_grad + (size_t)n * 3;
-                    if (P.acc_sdf_grad) { o[0] += ox; o[1] += oy; o[2] += oz; }
-                    else { o[0] = ox; o[1] = oy; o[2] = oz; }
-                }
+                float* o = g_sdf_grad + (size_t)n * 3;
+                if (P.acc_sdf_grad) { o[0] += ox; o[1] += oy; o[2] += oz; }
+                else { o[0] = ox; o[1] = oy; o[2] = oz; }
             }
         }
-        __syncthreads();     // exchange tile / accumulators free for the next tile
+        // no barrier before the next tile: s_a was last read by this tile's step-0 products, s_tail (over s_z) is next written by the
+        // next tile's seed, several barriers later
+        PSDF_PHASE(kPhTail);
+        if (sp.phase_cycles && tid == 0) atomicAdd(sp.phase_cycles + kPhTiles, 1ull);
     }
     __syncthreads();
-    // ---- weight gradients of this CTA: fixed-point sums -> the deterministic accumulators (integer atomics, exact), or their float
-    // value -> the gradients (+=)
-    if ((int)blockIdx.x < ntiles) {
-#pragma unroll 1
-        for (int l = 0; l < kNL; l++) {
-            const int K = P.g.K[l];
-            const unsigned long long* src = dw_cta + l * 128 * 128;
-            for (int i = tid; i < P.g.N[l] * K; i += kRgbThreads) {
-                const int m = i / K, k = i - m * K;
-                const unsigned long long v = src[m * 128 + k];
-                if (v == 0ull) continue;
-                if (det) atomicAdd(sp.fx_mlp + l * kFxW + i, v);
-                else atomicAdd(sp.gW[l] + i, (float)((double)(long long)v / kFxScale));
-            }
-        }
-    }
+    // ---- bias gradients of this CTA (the weight-gradient sums are added up across CTAs by k_rgb_dw_reduce)
     for (int i = tid; i < kNL * 128; i += kRgbThreads) {
         int l = i >> 7, c = i & 127;
         if (det) { if (c < P.g.N[l] && s_gb[i] != 0ull) atomicAdd(sp.fx_mlp + kFxB + l * 128 + c, s_gb[i]); }
         else if (c < P.g.N[l] && s_gbf[i] != 0.0f) atomicAdd(sp.gbias[l] + c, s_gbf[i]);
     }
+    PSDF_PHASE(kPhFlush);
     if (tid == 0) umma::bulk_wait0();
+}
+
+// Weight gradients: the CTAs' fixed-point sums of one slot (layer blockIdx.y, row-major index i over the true [N_l, K_l]) added up in
+// integer arithmetic (exact, in any order) over the CTAs of chunk blockIdx.z, then one integer atomic into the deterministic
+// accumulators, or the float value of the partial sum added to the gradient (+=). Flushing every CTA's sums with atomics at the end of
+// the persistent kernel was bound by the L2 atomic throughput: 37 k reductions per CTA, 4.9 M per C2 call, all to the same 37 k
+// addresses; here the sums are read once with coalesced loads and 4 partial sums per slot are reduced.
+constexpr int kDwReduceThreads = 256, kDwReduceChunks = 4;
+__global__ void __launch_bounds__(kDwReduceThreads)
+k_rgb_dw_reduce(MlpGeom g, int ctas, RgbSpill sp) {
+    const int l = blockIdx.y;
+    // no dynamic indexing of the parameter struct (local-memory copy)
+    const int K = l == 0 ? g.K[0] : (l == 1 ? g.K[1] : (l == 2 ? g.K[2] : g.K[3]));
+    const int N = l == 0 ? g.N[0] : (l == 1 ? g.N[1] : (l == 2 ? g.N[2] : g.N[3]));
+    const int i = blockIdx.x * kDwReduceThreads + threadIdx.x;
+    if (i >= N * K) return;
+    const int m = i / K, k = i - m * K;
+    const int per = (ctas + kDwReduceChunks - 1) / kDwReduceChunks, c0 = blockIdx.z * per, c1 = min(ctas, c0 + per);
+    const unsigned long long* src = g_dw_rgb_bwd + (size_t)l * 128 * 128 + m * 128 + k;
+    unsigned long long v = 0ull;
+#pragma unroll 8
+    for (int c = c0; c < c1; c++) v += src[(size_t)c * kDwSlots];
+    if (v == 0ull) return;
+    if (sp.fx_mlp) atomicAdd(sp.fx_mlp + l * kFxW + i, v);
+    else atomicAdd((l == 0 ? sp.gW[0] : (l == 1 ? sp.gW[1] : (l == 2 ? sp.gW[2] : sp.gW[3]))) + i, (float)((double)(long long)v / kFxScale));
 }
 
 #define ST ((cudaStream_t)stream)
@@ -307,11 +371,12 @@ k_rgb_fused_backward(RgbParams P, const float* __restrict__ pos, const float* __
 
 extern "C" {
 
-// workspace: the input operand tiles a_0 (64 KB per 128-sample tile), written by TMA store in the forward recompute and read back by the
-// same CTA for the first layer's weight gradient
+// workspace per 128-sample tile: the input operand tile a_0 (64 KB), written by TMA store in the forward recompute and read back by the
+// same CTA for the first layer's weight gradient, and the exchange rows of abar_0 (8 bytes per sample and level, sized for kMaxLevels
+// so that the size depends on the sample count alone)
 long long psdf_rgb_fused_backward_workspace_bytes(int N) {
     const int ntiles = div_up(N > 0 ? N : 1, kTile);
-    return (long long)ntiles * kRgbSpillBytes;
+    return (long long)ntiles * (kRgbSpillBytes + (long long)kTile * kMaxLevels * sizeof(float2));
 }
 
 static int rgb_backward_impl(int N, int L, int T, const float* pos, const float* dirs, const float* sdf_grad, const float* geom, int geom_dim,
@@ -324,26 +389,52 @@ static int rgb_backward_impl(int N, int L, int T, const float* pos, const float*
     if (rc != PSDF_OK) return rc;
     P.acc_sdf_grad = accumulate_sdf_grad ? 1 : 0;
     if (N == 0) return PSDF_OK;
-    static_assert((size_t)kTile * (128 + 1) * 4 <= (size_t)4 * kWTileBytes, "the exchange tile of K0 = 128 fits in s_a | s_z");
+    static_assert((size_t)kTile * kTailLd * 4 <= (size_t)2 * kWTileBytes, "the tail staging tile fits in s_z");
     const DetBufs* dbuf = det_buffers();
     if (dbuf && (long long)L * T * 2 > dbuf->lattice_len) return PSDF_ERR_UNSUPPORTED;   // reserve more with psdf_set_deterministic
     RgbSpill sp;
     float* b[kNL] = {gb0, gb1, gb2, gb3};
     float* w[kNL] = {gW0, gW1, gW2, gW3};
     for (int l = 0; l < kNL; l++) { sp.gbias[l] = b[l]; sp.gW[l] = w[l]; }
-    sp.fx_lattice = dbuf ? dbuf->rgb_lattice : nullptr;
     sp.fx_mlp = dbuf ? dbuf->rgb_mlp : nullptr;
-    sp.a0 = workspace;
     const int ntiles = div_up(N, kTile);
+    sp.a0 = workspace;
+    sp.xch = reinterpret_cast<float2*>(workspace + (size_t)ntiles * kRgbSpillBytes);
+    sp.xch_stride = ntiles * kTile;
+    // diagnostics: PSDF_PHASE_TIMING=1 prints thread 0's clock64 breakdown per phase (average cycles per tile) after every launch
+    static const bool timing = getenv("PSDF_PHASE_TIMING") && atoi(getenv("PSDF_PHASE_TIMING")) != 0;
+    static unsigned long long* d_cycles = nullptr;
+    static cudaEvent_t ev[4];
+    sp.phase_cycles = nullptr;
+    if (timing) {
+        if (!d_cycles) {
+            cudaMalloc(&d_cycles, 16 * sizeof(unsigned long long));
+            for (auto& e : ev) cudaEventCreate(&e);
+        }
+        cudaMemsetAsync(d_cycles, 0, 16 * sizeof(unsigned long long), ST);
+        sp.phase_cycles = d_cycles;
+        cudaEventRecord(ev[0], ST);
+    }
     int dev = 0, sms = 132;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    const size_t smem = (size_t)6 * kWTileBytes + sizeof(LevelC) + kNL * 128 * (sizeof(float) + sizeof(unsigned long long)) + 64;
+    const size_t smem = (size_t)6 * kWTileBytes + sizeof(LevelC) + kNL * 128 * (sizeof(float) + sizeof(unsigned long long)) + 64 + kBxBytes;
     // per device: set on every call (a second GPU needs its own opt-in)
     { static bool optin_[64]; psdf::psdf_optin_smem(k_rgb_fused_backward, 227 * 1024, optin_); }
-    k_rgb_fused_backward<<<min(min(ntiles, sms), kAccCtas), kRgbThreads, smem, ST>>>(P, pos, dirs, sdf_grad, geom, reinterpret_cast<const float2*>(lattice),
-                                                                      scale_factor, shift, window, blob, g_out, grad_lattice, g_sdf_grad, g_geom, sp);
+    const int ctas = min(min(ntiles, sms), kAccCtas);
+    k_rgb_fused_backward<<<ctas, kRgbThreads, smem, ST>>>(P, pos, dirs, sdf_grad, geom, reinterpret_cast<const float2*>(lattice),
+                                                                      scale_factor, shift, window, blob, g_out, g_sdf_grad, g_geom, sp);
     PSDF_CHECK_LAUNCH();
+    if (timing) cudaEventRecord(ev[1], ST);
+    int max_nk = 0;
+    for (int l = 0; l < kNL; l++) max_nk = max(max_nk, P.g.N[l] * P.g.K[l]);
+    k_rgb_dw_reduce<<<dim3(div_up(max_nk, kDwReduceThreads), kNL, kDwReduceChunks), kDwReduceThreads, 0, ST>>>(P.g, ctas, sp);
+    PSDF_CHECK_LAUNCH();
+    if (timing) cudaEventRecord(ev[2], ST);
+    k_lattice_scatter<3><<<dim3(div_up(sp.xch_stride, kScatterThreads), L), kScatterThreads, 0, ST>>>(
+        N, T, P.cap_mask, pos, sp.xch, sp.xch_stride, scale_factor, shift, window, grad_lattice, dbuf ? dbuf->rgb_lattice : nullptr);
+    PSDF_CHECK_LAUNCH();
+    if (timing) cudaEventRecord(ev[3], ST);
     if (dbuf) {      // deterministic mode: fixed-point totals -> the float gradients (+=)
         FxSegs F;
         F.add(dbuf->rgb_lattice, grad_lattice, (long long)L * T * 2);
@@ -352,6 +443,19 @@ static int rgb_backward_impl(int N, int L, int T, const float* pos, const float*
             F.add(dbuf->rgb_mlp + kFxB + l * 128, b[l], P.g.N[l]);
         }
         if (fx_flush(F, ST) != 0) return PSDF_ERR_LAUNCH;
+    }
+    if (timing) {
+        unsigned long long h[16];
+        cudaMemcpyAsync(h, d_cycles, sizeof(h), cudaMemcpyDeviceToHost, ST);
+        cudaStreamSynchronize(ST);
+        const double t = h[kPhTiles] ? (double)h[kPhTiles] : 1.0;
+        float ms_fused = 0.f, ms_reduce = 0.f, ms_scatter = 0.f;
+        cudaEventElapsedTime(&ms_fused, ev[0], ev[1]);
+        cudaEventElapsedTime(&ms_reduce, ev[1], ev[2]);
+        cudaEventElapsedTime(&ms_scatter, ev[2], ev[3]);
+        fprintf(stderr, "[psdf_rgb_fused_backward N=%d tiles=%llu] cycles/tile: encoder %.0f forward %.0f %.0f %.0f seed %.0f rev3 %.0f rev2 %.0f rev1 %.0f "
+                        "rev0 %.0f tail %.0f | flush/CTA %.0f | fused kernel %.3f ms, weight-gradient reduction %.3f ms, lattice scatter %.3f ms\n", N, h[kPhTiles], h[0] / t, h[1] / t, h[2] / t, h[3] / t,
+                h[4] / t, h[5] / t, h[6] / t, h[7] / t, h[8] / t, h[9] / t, (double)h[kPhFlush] / ctas, ms_fused, ms_reduce, ms_scatter);
     }
     return PSDF_OK;
 }

@@ -108,21 +108,37 @@ __device__ __forceinline__ void dw_rows_fx(unsigned long long* dw, int m0, int c
 }
 // dW_l = zbar^(l)^T a_l over the 128 samples of the tile: both tiles consumed as MN-major operands (one warpgroup, `half` = 0 / 1).
 // M = 128: the two warpgroups take rows 0..63 / 64..127; M = 64: columns [0, na) / [na, N) of one M = 64 product. Added to the CTA's
-// fixed-point sums (dw_rows_fx, row stride LD) in pieces of at most 32 columns (register budget).
+// fixed-point sums (dw_rows_fx, row stride LD) in pieces of at most 32 columns (register budget); pieces `part`, part + parts, ... of
+// the half (parts warpgroups share it).
 template <int LD = 128>
-__device__ __forceinline__ void issue_dw_w(unsigned long long* dw, int half, const uint8_t* z_hi, const uint8_t* a_hi, int M, int N, bool first) {
+__device__ __forceinline__ void issue_dw_w(unsigned long long* dw, int half, const uint8_t* z_hi, const uint8_t* a_hi, int M, int N, bool first,
+                                           int part = 0, int parts = 1) {
     int m0 = 0, n0 = 0, nn = N;
     if (M == 128) m0 = 64 * half;
     else split_n(N, half, n0, nn);
     if (nn <= 0) return;
     const uint32_t zh = umma::smem_u32(z_hi) + (uint32_t)(m0 / 8) * kLBO;
     const uint64_t dzh = umma::make_desc(zh, kWSBO, kLBO), dzl = umma::make_desc(zh + kWTileBytes, kWSBO, kLBO);
-    for (int p0 = 0; p0 < nn; p0 += 32) {
+    for (int p0 = 32 * part; p0 < nn; p0 += 32 * parts) {
         const uint32_t ah = umma::smem_u32(a_hi) + (uint32_t)((n0 + p0) / 8) * kLBO;
         const uint64_t dah = umma::make_desc(ah, kWSBO, kLBO), dal = umma::make_desc(ah + kWTileBytes, kWSBO, kLBO);
         if (nn - p0 >= 32) dw_rows_fx<32, LD>(dw, m0, n0 + p0, dzh, dzl, dah, dal, first);
         else dw_rows_fx<16, LD>(dw, m0, n0 + p0, dzh, dzl, dah, dal, first);
     }
+}
+
+// The CTA's sums of the slots issue_dw_w (same arguments) reads and writes in this thread -> L2, ahead of the products
+__device__ __forceinline__ void prefetch_dw_w(const unsigned long long* dw, int half, int M, int N, int part, int parts) {
+    int m0 = 0, n0 = 0, nn = N;
+    if (M == 128) m0 = 64 * half;
+    else split_n(N, half, n0, nn);
+    for (int p0 = 32 * part; p0 < nn; p0 += 32 * parts)
+#pragma unroll
+        for (int h = 0; h < 2; h++)
+#pragma unroll
+            for (int j = 0; j < 4; j++)
+                if (p0 + 8 * j < nn)
+                    asm volatile("prefetch.global.L2 [%0];" ::"l"(dw + (size_t)(m0 + frag_row(0, h)) * 128 + n0 + p0 + frag_col(j)));
 }
 
 // Layer-0 operand tile of one sample row. Thread (row, grp) builds the 8-column cores grp, grp+4, ... of the lattice part and
@@ -185,6 +201,37 @@ __device__ __forceinline__ void build_input_tile(const RgbParams& P, const Level
         float z8[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
         store8w(a_hi, a_lo, row, kc, z8);
     }
+}
+
+// Encoder backward of the colour-network-shaped backwards (no tangent term): lattice[l][idx_r] += window_l B_r abar_0[l] from the
+// exchange rows their persistent kernels write, xch[l][tile * 128 + row] = abar_0's two columns of level l. blockIdx.y = level (blocks
+// of one level run together: its gradient table stays in L2 while they land), warp = 32 consecutive sample slots, i.e. the rows of one
+// warp of the per-row layout, so the match_any groups and the float peer sums are those of a scatter inside the persistent kernel. It runs
+// with every warp slot of the SM occupied, where the persistent kernel's 16 warps per SM would wait on its dependent chains of simplex
+// recompute, match_any, shuffle sums and reductions with the tensor cores idle. pos, scale and shift have D columns; fx_lattice:
+// deterministic mode's fixed-point accumulators, else NULL.
+constexpr int kScatterThreads = 256;
+template <int D>
+static __global__ void __launch_bounds__(kScatterThreads, 8)
+k_lattice_scatter(int N, int T, unsigned cap_mask, const float* __restrict__ pos, const float2* __restrict__ xch, int xch_stride,
+                  const float* __restrict__ scale, const float* __restrict__ shift, const float* __restrict__ window,
+                  float* __restrict__ grad_lattice, unsigned long long* __restrict__ fx_lattice) {
+    const int slot = blockIdx.x * kScatterThreads + threadIdx.x;
+    if (slot >= xch_stride) return;                                  // whole warps (xch_stride % 128 == 0)
+    const int l = blockIdx.y, lane = threadIdx.x & 31;
+    const bool valid = slot < N;
+    float x[D], sc[D], sh[D];
+#pragma unroll
+    for (int i = 0; i < D; i++) {
+        x[i] = valid ? pos[(size_t)slot * D + i] : 0.0f;
+        sc[i] = scale[l * D + i];
+        sh[i] = shift ? shift[l * D + i] : 0.0f;
+    }
+    const float w = window ? window[l] : 1.0f;
+    const float2 a = xch[(size_t)l * xch_stride + slot];
+    const bool aggregate = sc[0] < kAggregateBelowScale;             // warp-uniform (l is)
+    scatter_level<false, D>(x, nullptr, sc, sh, w, a.x, a.y, 0.f, 0.f, valid, aggregate, true, lane, cap_mask, (unsigned)T,
+                            grad_lattice + (size_t)l * T * 2, fx_lattice ? fx_lattice + (size_t)l * T * 2 : nullptr);
 }
 
 }  // namespace psdf_rgb

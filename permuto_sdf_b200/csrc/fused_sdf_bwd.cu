@@ -124,23 +124,6 @@ __device__ __forceinline__ void issue_dw16(float* d, const uint8_t* zset, const 
     }
 }
 
-// Column sums of a fragment block over the 8 lanes t / 4 = 0..7 of one warp (halving butterfly over lanes ^ 16, ^ 8, ^ 4, 7 shuffles): v[2 j + b]
-// is this thread's value of column 8 j + 2 (t % 4) + b. Afterwards every lane holds the sum of one column, `col` = 8 (2 bit4 + bit3) +
-// 2 (t % 4) + bit2.
-__device__ __forceinline__ float frag_colsum8(const float* v, int lane, int& col) {
-    float a[4], b[2], c;
-    bool up = lane & 16;
-#pragma unroll
-    for (int i = 0; i < 4; i++) { float send = up ? v[i] : v[i + 4], keep = up ? v[i + 4] : v[i]; a[i] = keep + __shfl_xor_sync(kFull, send, 16); }
-    up = lane & 8;
-#pragma unroll
-    for (int i = 0; i < 2; i++) { float send = up ? a[i] : a[i + 2], keep = up ? a[i + 2] : a[i]; b[i] = keep + __shfl_xor_sync(kFull, send, 8); }
-    up = lane & 4;
-    { float send = up ? b[0] : b[1], keep = up ? b[1] : b[0]; c = keep + __shfl_xor_sync(kFull, send, 4); }
-    col = 8 * (2 * ((lane >> 4) & 1) + ((lane >> 3) & 1)) + 2 * (lane & 3) + ((lane >> 2) & 1);
-    return c;
-}
-
 // D = 3: positions [N,3]; D = 4: space-time positions [N,4] with the tangent along (g_grad, 0) (g_grad holds spatial derivatives)
 template <int D>
 __global__ void __launch_bounds__(kBwdThreads, 1)
@@ -401,33 +384,14 @@ k_sdf_fused_backward(FusedParams P, Segments S, const float2* __restrict__ latti
                             }
                         }
                     }
-                    // Column sums over each 32-row group (warps 2p, 2p + 1 of the warpgroup), added up in the order of colsum16 over the
-                    // rows r = 0..31 of one warp in the per-row layout: pairs r, r ^ 16 first, then r ^ 8, r ^ 4, r ^ 2, r ^ 1. Here bit 4
-                    // of r is the warp of the pair, bit 3 the fragment half h and bits 2..0 the lane bits 4..2, so the odd warp's values
-                    // come through shared memory, then h, then frag_colsum8's butterfly over lanes ^ 16, ^ 8, ^ 4. Every partial sum and
-                    // the one fixed-point rounding per tile, column and 32 rows are those of the per-row sum.
+                    // bias gradient: column sums over each 32-row group (warps 2p, 2p + 1 of the warpgroup) in the order of the per-row
+                    // colsum16 (frag_pair_colsum)
                     const int pair = 2 * wgi + ((warp & 3) >> 1);
-                    float* bx = s_bx + pair * 16 * 32 + lane;
-                    if (warp & 1) {
-#pragma unroll
-                        for (int i = 0; i < 16; i++) if (2 * i < nn) bx[i * 32] = acc[0][i];
-                    }
-                    umma::bar_sync(1 + pair, 64);
-                    if (!(warp & 1)) {
-                        float bs[8];
-#pragma unroll
-                        for (int j = 0; j < 4; j++)
-#pragma unroll
-                            for (int b = 0; b < 2; b++) {
-                                const int i0 = 4 * j + b, i1 = 4 * j + 2 + b;
-                                bs[2 * j + b] = (8 * j < nn) ? (acc[0][i0] + bx[i0 * 32]) + (acc[0][i1] + bx[i1 * 32]) : 0.f;
-                            }
-                        int col;
-                        const float cs = frag_colsum8(bs, lane, col);
-                        if (col < nn) {
-                            if (det) fx_add(&s_gb[(l - 1) * 64 + n0 + col], cs);
-                            else atomicAdd(&s_gbf[(l - 1) * 64 + n0 + col], cs);
-                        }
+                    float cs;
+                    int col;
+                    if (frag_pair_colsum(acc[0], nn, s_bx + pair * 16 * 32, 1 + pair, cs, col)) {
+                        if (det) fx_add(&s_gb[(l - 1) * 64 + n0 + col], cs);
+                        else atomicAdd(&s_gbf[(l - 1) * 64 + n0 + col], cs);
                     }
                 }
                 if (l >= 2) {
