@@ -30,8 +30,9 @@ import torch
 import torch.nn.functional as F
 
 from ._lib import call, load_library
+from .graphs import graph_state, run, sampler_graph_mode
 from .models import Colorcal, DeviceIter, NerfHash, map_range_val
-from .permuto_sdf import OccupancyGrid, PermutoSDF, RaySampler, RaySamplesPacked, Sphere
+from .permuto_sdf import OccupancyGrid, PermutoSDF, RaySampler, Sphere
 
 _INT32_MAX = 2 ** 31 - 1
 MASK_WEIGHT = 0.1                                  # train_nerf.py:182
@@ -121,7 +122,7 @@ class NerfTrainer:
         self.last = {}
         self._ws = {}
         self._dev = None            # device-resident iteration and step count of the direct sequence
-        self._cg = None             # CUDA-graph state (enable_cuda_graph)
+        self._cg = None             # graphs.graph_state of the step and the occupancy refresh (enable_cuda_graph)
 
     # ------------------------------------------------------------------------------------ inputs
     def _check_rays(self, R, has_mask):
@@ -215,60 +216,28 @@ class NerfTrainer:
         opt.sync_hyper()
         opt.zero_grad(set_to_none=False)
 
-        def body(dit, args):
+        def body(dit, *args):
             out = self._direct_forward_backward(*self._rays(args, make_rays), dit)
             opt.step_groups_deferred([0], st["step_dev"])
             st["step_dev"].add_(1)
             st["it_dev"].add_(1.0)
-            return out
+            return out, self.last
 
         with torch.cuda.device(dev):
             if self._cg is None:
                 if it % OCC_EVERY == 0:
                     self.update_occupancy(DeviceIter(it, st["it_dev"]))
-                loss = body(DeviceIter(it, st["it_dev"]), inputs)
+                loss = body(DeviceIter(it, st["it_dev"]), *inputs)[0]
             else:
+                bufs = lambda: dict(self._ws)
                 if it % OCC_EVERY == 0:
-                    self._replay("occ", ("occ",), it, st, lambda dit, _: self.update_occupancy(dit), ())
+                    run(self._cg, self._cg["occ"], ("occ",), DeviceIter(it, st["it_dev"]), self.update_occupancy, keep=bufs)
                 key = ("step", make_rays is not None) + tuple(None if t is None else (tuple(t.shape), t.dtype) for t in inputs)
-                loss = self._replay("step", key, it, st, body, inputs)
+                loss, self.last = run(self._cg, self._cg["step"], key, DeviceIter(it, st["it_dev"]), body, inputs, keep=bufs)
         opt.step_count += 1
         opt._clean = True
         self.iter_nr += 1
         return loss
-
-    def _replay(self, name, key, it, st, fn, inputs):
-        """fn(DeviceIter, inputs) eagerly on the capture stream the first time a shape is seen, captured the next time, replayed while the
-        iteration stays inside the range over which the captured Python control flow holds (DeviceIter)"""
-        cg = self._cg
-        g = cg["graphs"].get(name)
-        if g is not None and g["key"] == key and g["lo"] <= it < g["hi"]:
-            for dst, src in zip(g["static"], inputs):
-                if dst is not None:
-                    dst.copy_(src, non_blocking=True)
-            g["graph"].replay()
-            self.last = g["last"]
-            return g["out"]
-        side, cur = cg["stream"], torch.cuda.current_stream()
-        dit = DeviceIter(it, st["it_dev"])
-        if cg["warm"].get(name) != key:
-            side.wait_stream(cur)
-            with torch.cuda.stream(side):
-                out = fn(dit, inputs)
-            cur.wait_stream(side)
-            cg["warm"][name] = key
-            return out
-        dev = st["it_dev"].device
-        static = [None if t is None else t.detach().to(dev).clone() for t in inputs]
-        torch.cuda.synchronize()
-        graph = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(graph, stream=side):
-            out = fn(dit, static)
-        # the buffers the graph writes stay referenced for as long as the graph lives
-        cg["graphs"][name] = dict(graph=graph, key=key, lo=dit.lo, hi=dit.hi, out=out, static=static, last=self.last, bufs=dict(self._ws))
-        cg["captures"] += 1
-        graph.replay()                     # the capture recorded the work, it did not run it
-        return out
 
     def _rays(self, inputs, make_rays):
         if make_rays is None:
@@ -438,18 +407,14 @@ class NerfTrainer:
         if not self.direct:
             raise RuntimeError("NerfTrainer.enable_cuda_graph: the autograd formulation is not captured (%s)" % self.execution["step"])
         if self._cg is None:
-            RaySamplesPacked.static_capacity = True
-            for r in (OccupancyGrid.m_rng, RaySampler.m_rng):
-                r.to_device()
-            self._cg = dict(stream=torch.cuda.Stream(device=self.optimizer.flat_param.device), captures=0, graphs={}, warm={})
+            sampler_graph_mode(True, (OccupancyGrid.m_rng, RaySampler.m_rng))
+            self._cg = graph_state(torch.cuda.Stream(device=self.optimizer.flat_param.device), "occ", "step")
             self.execution["step"] = "direct kernel sequence (nerf_train.py), CUDA-graph replay"
 
     def disable_cuda_graph(self):
         if self._cg is not None:
             self.execution["step"] = "direct kernel sequence (nerf_train.py)"
-            RaySamplesPacked.static_capacity = False
-            for r in (OccupancyGrid.m_rng, RaySampler.m_rng):
-                r.to_host()
+            sampler_graph_mode(False, (OccupancyGrid.m_rng, RaySampler.m_rng))
             self._cg = None
 
     # ------------------------------------------------------------------------------------ checkpoints

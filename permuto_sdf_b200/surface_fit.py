@@ -28,6 +28,7 @@ import torch
 import torch.nn.functional as F
 
 from ._lib import call
+from .graphs import graph_state, run
 from .models import SDF, DeviceIter
 from .permuto_sdf import AABB
 
@@ -147,8 +148,8 @@ class SurfaceFit:
         self.fixed_random = None        # tests: {"surface_fit_idx": [Ns] int64, "surface_fit_u01": [No,3]} replace the torch RNG draws
         self.last = {}
         self._ws = None                 # buffers of the direct sequence, sized by (Ns, No, P)
-        self._dev = None                # device-resident iteration, step count and captured graph
-        self._cg = None                 # CUDA-graph state (enable_cuda_graph)
+        self._dev = None                # device-resident iteration and step count
+        self._cg = None                 # graphs.graph_state of the step (enable_cuda_graph)
 
     # ------------------------------------------------------------------------------------ draws
     def draw(self, name, fn):
@@ -196,8 +197,7 @@ class SurfaceFit:
         dev = opt.flat_param.device
         st = self._dev
         if st is None:
-            st = self._dev = dict(it_dev=torch.zeros((), device=dev), step_dev=torch.zeros(1, dtype=torch.int32, device=dev), graph=None,
-                                  warm=None)
+            st = self._dev = dict(it_dev=torch.zeros((), device=dev), step_dev=torch.zeros(1, dtype=torch.int32, device=dev))
         # device-resident iteration and AdamW step count: the same sequence runs eagerly and from the captured graph
         st["it_dev"].fill_(float(self.iter_nr))
         st["step_dev"].fill_(opt.step_count)
@@ -210,37 +210,17 @@ class SurfaceFit:
             out = self._direct_forward_backward(dit, Ns, No)
             opt.step_groups_deferred([0], st["step_dev"])
             self.model_sdf.fused.repack(advance=(st["step_dev"], st["it_dev"]))
-            return out
+            return out, self.last
 
         with torch.cuda.device(dev):
             for _ in range(n):
                 dit = DeviceIter(self.iter_nr, st["it_dev"])
-                g = st["graph"]
                 if self._cg is None:
-                    loss = one(dit)
-                elif g is not None and g["key"] == key and g["lo"] <= self.iter_nr < g["hi"]:
-                    g["graph"].replay()
-                    loss = g["loss"]
-                elif st["warm"] != key:
-                    # first iteration of this shape: eager, on the capture stream (workspaces and lazy library state are created there)
-                    side, cur = self._cg["stream"], torch.cuda.current_stream()
-                    side.wait_stream(cur)
-                    with torch.cuda.stream(side):
-                        loss = one(dit)
-                    cur.wait_stream(side)
-                    st["warm"] = key
+                    loss = one(dit)[0]
                 else:
-                    torch.cuda.synchronize()
-                    graph = torch.cuda.CUDAGraph()
-                    with torch.cuda.graph(graph, stream=self._cg["stream"]):
-                        loss = one(dit)
-                    st["graph"] = dict(graph=graph, key=key, lo=dit.lo, hi=dit.hi, loss=loss, last=self.last)
-                    self._cg["captures"] += 1
-                    graph.replay()                    # the capture recorded the iteration, it did not run it
+                    loss, self.last = run(self._cg, self._cg["step"], key, dit, one, keep=lambda: self._ws)
                 opt.step_count += 1
                 self.iter_nr += 1
-        if st["graph"] is not None and self._cg is not None:
-            self.last = st["graph"]["last"]
         opt._clean = True
         return loss
 
@@ -353,12 +333,10 @@ class SurfaceFit:
         first step of a shape runs eagerly, the next one is captured; one more capture follows where the window's ramp ends (iteration
         nr_iters_for_c2f). The autograd formulation is not captured."""
         if self._cg is None:
-            self._cg = dict(stream=torch.cuda.Stream(device=self.points.device), captures=0)
+            self._cg = graph_state(torch.cuda.Stream(device=self.points.device), "step")
 
     def disable_cuda_graph(self):
         self._cg = None
-        if self._dev is not None:
-            self._dev["graph"], self._dev["warm"] = None, None
 
     # ------------------------------------------------------------------------------------ checkpoints
     def save(self, ckpt_folder, experiment_name, iter_nr=None, with_optimizer=True):

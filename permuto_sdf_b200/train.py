@@ -14,6 +14,7 @@ import math
 import torch
 import torch.nn.functional as F
 
+from .graphs import capture, on_stream, run, sampler_graph_mode
 from .models import RGB, SDF, Colorcal, DeviceIter, NerfHash, map_range_val
 from .permuto_sdf import OccupancyGrid, PermutoSDF, RaySampler, RaySamplesPacked, Sphere, VolumeRendering
 
@@ -433,7 +434,7 @@ class Trainer:
         self.execution["sphere_fit"] = None      # set by fit_sphere()
         self.iter_nr = 0
         self.sphere_fit_iter = 0        # sphere-fit iterations run so far (fit_sphere)
-        self._fit = None                # device counters and captured graph of the direct sphere fit
+        self._fit = None                # device counters and graph slot (graphs.run) of the direct sphere fit
         self._cg = None                 # CUDA-graph state (enable_cuda_graph)
         self._dp = None                 # data-parallel state (enable_data_parallel)
         self._render = None             # workspaces of render()
@@ -772,35 +773,16 @@ class Trainer:
             out = self._direct.sphere_fit(dit, *args)
             opt.step_groups_deferred(gi, step_dev)
             self.model_sdf.fused.repack(advance=(step_dev, fit["it_dev"]))
-            return out
+            return out, self.last
 
         for _ in range(n):
             dit = DeviceIter(self.sphere_fit_iter, fit["it_dev"])
-            g = fit["graph"]
             if self._cg is None:
-                loss = one(dit)
-            elif g is not None and g["key"] == key and g["lo"] <= self.sphere_fit_iter < g["hi"]:
-                g["graph"].replay()
-                loss = g["loss"]
-            elif fit["warm"] != key:
-                # first iteration of this shape: eager, on the capture stream (workspace and lazy library state are created there)
-                side, cur = self._cg["stream"], torch.cuda.current_stream()
-                side.wait_stream(cur)
-                with torch.cuda.stream(side):
-                    loss = one(dit)
-                cur.wait_stream(side)
-                fit["warm"] = key
+                loss = one(dit)[0]
             else:
-                torch.cuda.synchronize()
-                graph = torch.cuda.CUDAGraph()
-                with torch.cuda.graph(graph, stream=self._cg["stream"]):
-                    loss = one(dit)
-                fit["graph"] = dict(graph=graph, key=key, lo=dit.lo, hi=dit.hi, loss=loss, last=self.last)
-                graph.replay()                    # the capture recorded the iteration, it did not run it
+                loss, self.last = run(self._cg, fit, key, dit, one, keep=lambda: self._direct._fit_ws)
             opt.step_count += 1
             self.sphere_fit_iter += 1
-        if fit["graph"] is not None and self._cg is not None:
-            self.last = fit["graph"]["last"]
         opt._clean = True
         return loss
 
@@ -832,16 +814,14 @@ class Trainer:
         The first `warmup_steps` iterations run eagerly (on the capture stream) with the same static shapes."""
         if not hasattr(self.optimizer, "flat_grad"):
             raise RuntimeError("CUDA-graph mode needs the flat-buffer optimizer (optimizer='fused')")
-        RaySamplesPacked.static_capacity = True
-        for r in (OccupancyGrid.m_rng, RaySampler.m_rng, VolumeRendering.m_rng):
-            r.to_device()
+        sampler_graph_mode(True, (OccupancyGrid.m_rng, RaySampler.m_rng, VolumeRendering.m_rng))
         opt = self.optimizer
         opt.device_step = True
         dev = opt.flat_param.device
         opt.step_dev = torch.full((1,), opt.step_count, dtype=torch.int32, device=dev)
         opt.sync_hyper()
         self._cg = dict(warm=int(warmup_steps), fb=None, opt={}, occ=None, it_dev=torch.zeros((), device=dev), it_host=None,
-                        stream=torch.cuda.Stream(device=dev), launches=0,
+                        stream=torch.cuda.Stream(device=dev), launches=0, captures=0,      # captures: the sphere fit's (graphs.run)
                         # the parameter-free head of the iteration (ray generation + occupancy sampling) is a graph of its own on this stream:
                         # it runs beside the previous iteration's optimizer step (see _step_graphed)
                         stream_a=torch.cuda.Stream(device=dev), ev_fb=None, split=(self._direct is not None))
@@ -851,14 +831,11 @@ class Trainer:
         if self._cg is None:
             return
         torch.cuda.synchronize()
-        RaySamplesPacked.static_capacity = False
-        for r in (OccupancyGrid.m_rng, RaySampler.m_rng, VolumeRendering.m_rng):
-            r.to_host()
+        sampler_graph_mode(False, (OccupancyGrid.m_rng, RaySampler.m_rng, VolumeRendering.m_rng))
         self.optimizer.device_step = False
         self.optimizer.step_dev = None
         self._cg = None
-        if self._fit is not None:
-            self._fit["graph"], self._fit["warm"] = None, None      # the captured fit reads the step count just dropped
+        self._fit = None                # its graph slot reads the step count just dropped
 
     def _sync_device_iter(self):
         cg = self._cg
@@ -907,9 +884,8 @@ class Trainer:
         if not valid and cg["warm"] > 0:
             # eager iteration with the static shapes, on the capture stream (lazy library state initialises there)
             cg["warm"] -= 1
-            side = cg["stream"]
-            side.wait_stream(cur)
-            with torch.cuda.stream(side):
+
+            def eager():
                 args = inputs
                 if make_rays is not None:
                     with torch.no_grad():
@@ -917,7 +893,8 @@ class Trainer:
                 self.optimizer.zero_grad(set_to_none=False)
                 loss = self.forward_backward(*args, DeviceIter(it, cg["it_dev"]))
                 self._dp_join_backward()
-            cur.wait_stream(side)
+                return loss
+            loss = on_stream(cg["stream"], eager)
         else:
             if not valid:
                 fb = cg["fb"] = self._capture_forward_backward(inputs, shapes, it, make_rays)
@@ -985,25 +962,12 @@ class Trainer:
         (re-captured when the iteration leaves the range for which the captured branches hold)"""
         cg = self._cg
         og = cg.get("occ")
+        dit = DeviceIter(it, cg["it_dev"])
         if cg["fb"] is None:                     # warm-up iterations: eager, on the capture stream
-            side, cur = cg["stream"], torch.cuda.current_stream()
-            side.wait_stream(cur)
-            with torch.cuda.stream(side):
-                self.update_occupancy(DeviceIter(it, cg["it_dev"]))
-            cur.wait_stream(side)
+            on_stream(cg["stream"], self.update_occupancy, dit)
             return
         if og is None or not (og["lo"] <= it < og["hi"]):
-            dit = DeviceIter(it, cg["it_dev"])
-            from ._lib import stats_pause, stats_resume
-            torch.cuda.synchronize()
-            paused = stats_pause()
-            from ._lib import stats_begin, stats_end
-            stats_begin(with_events=False)
-            g = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(g, stream=cg["stream"]):
-                self.update_occupancy(dit)
-            _, launches, _ = stats_end()
-            stats_resume(paused)
+            g, _, launches = capture(cg["stream"], self.update_occupancy, dit, count_launches=True)
             og = cg["occ"] = dict(graph=g, lo=dit.lo, hi=dit.hi, launches=launches)
         og["graph"].replay()
         from ._lib import stats_add_launches
@@ -1014,32 +978,29 @@ class Trainer:
         static = [None if t is None else t.detach().to(cg["it_dev"].device).clone() for t in inputs]
         dit = DeviceIter(it, cg["it_dev"])
         self.optimizer.zero_grad(set_to_none=False)
-        torch.cuda.synchronize()
-        from ._lib import stats_begin, stats_end
-        stats_begin(with_events=False)
-        g = torch.cuda.CUDAGraph()
-        g_a = None
+
+        def rays():
+            if make_rays is None:
+                return static
+            with torch.no_grad():
+                return make_rays(*static)
+
+        def forward_backward(args, pre=None):
+            out = self.forward_backward(*args, dit, pre=pre)
+            self._dp_join_backward()
+            return out
+
         if cg.get("split") and self._direct is not None:
             # graph A: inputs -> rays -> occupancy samples (no network parameter read); graph B: the rest, sharing A's memory pool
-            g_a = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(g_a, stream=cg["stream_a"]):
-                args = static
-                if make_rays is not None:
-                    with torch.no_grad():
-                        args = make_rays(*static)
-                pre = self._direct.sample_uniform(args[0], args[1])
-            with torch.cuda.graph(g, stream=cg["stream"], pool=g_a.pool()):
-                out = self.forward_backward(*args, dit, pre=pre)
-                self._dp_join_backward()
+            def head():
+                args = rays()
+                return args, self._direct.sample_uniform(args[0], args[1])
+            g_a, (args, pre), launches_a = capture(cg["stream_a"], head, count_launches=True)
+            g, out, launches = capture(cg["stream"], forward_backward, args, pre, pool=g_a.pool(), count_launches=True)
+            launches += launches_a
         else:
-            with torch.cuda.graph(g, stream=cg["stream"]):
-                args = static
-                if make_rays is not None:
-                    with torch.no_grad():
-                        args = make_rays(*static)
-                out = self.forward_backward(*args, dit)
-                self._dp_join_backward()
-        _, launches, _ = stats_end()
+            g_a = None
+            g, out, launches = capture(cg["stream"], lambda: forward_backward(rays()), count_launches=True)
         dp_rgb = bool(self._dp.pop("rgb_reduced", False)) if getattr(self, "_dp", None) is not None else False
         cg["occ"] = None               # the refresh graph reads tensors of the iteration graph (last inv_s): capture it again
         cg["ev_fb"] = None             # the first replay waits for everything queued so far
@@ -1073,11 +1034,7 @@ class Trainer:
                 self.model_sdf.fused.repack(advance=(None, cg["it_dev"]))
 
         if cg["fb"] is None:            # still in the eager warm-up iterations
-            side, cur = cg["stream"], torch.cuda.current_stream()
-            side.wait_stream(cur)
-            with torch.cuda.stream(side):
-                work()
-            cur.wait_stream(side)
+            on_stream(cg["stream"], work)
         elif dp is not None and dp["mode"] == "peer":
             # the cross-rank barriers of the peer-memory step are launched eagerly, right behind the replayed iteration graph (a handful
             # of launches; the host is far ahead of the GPU)
@@ -1086,13 +1043,7 @@ class Trainer:
             key = (grad_scale, allreduce, dp is not None, rgb_done)
             og = cg["opt"].get(key)
             if og is None:
-                from ._lib import stats_begin, stats_end
-                torch.cuda.synchronize()
-                stats_begin(with_events=False)
-                g = torch.cuda.CUDAGraph()
-                with torch.cuda.graph(g, stream=cg["stream"]):
-                    work()
-                _, launches, _ = stats_end()
+                g, _, launches = capture(cg["stream"], work, count_launches=True)
                 self.optimizer.step_count -= 1          # capture records, it does not run
                 og = cg["opt"][key] = dict(graph=g, launches=launches)
             og["graph"].replay()

@@ -33,11 +33,12 @@ def card():
 
 
 def make(kind, with_mask):
+    from permuto_sdf_b200.graphs import graph_state
     from permuto_sdf_b200.nerf_train import NerfTrainer
     tr = NerfTrainer(8, with_mask, optimizer="adamw" if kind == "autograd" else "fused", deterministic=True, direct=(kind != "autograd"))
     if kind == "graph":
         graph_mode(True)
-        tr._cg = dict(stream=torch.cuda.Stream(), captures=0, graphs={}, warm={})     # enable_cuda_graph without the class-wide switch
+        tr._cg = graph_state(torch.cuda.Stream(), "occ", "step")       # enable_cuda_graph without the class-wide switch
     return tr
 
 
