@@ -99,7 +99,7 @@ k_neus_forward(int nr_rays, int max_nr_samples, const int* __restrict__ start_en
         const int im = ext.img_idx[ray];
         if (im != ext.fixed_img) {
 #pragma unroll
-            for (int ch = 0; ch < 3; ch++) { hw[ch] = 1.0f + ext.weight_delta[3 * im + ch]; hb[ch] = ext.bias[3 * im + ch]; }
+            for (int ch = 0; ch < 3; ch++) { hw[ch] = 1.0f + ext.weight_delta[3 * im + ch]; hb[ch] = ext.bias ? ext.bias[3 * im + ch] : 0.0f; }
         }
     }
     float T = 1.0f, ax = 0.f, ay = 0.f, az = 0.f, ws = 0.f, eik = 0.f;
@@ -206,7 +206,7 @@ k_neus_backward(int nr_rays, int max_nr_samples, const int* __restrict__ start_e
         him = ext.img_idx[ray];
         if (him != ext.fixed_img) {
 #pragma unroll
-            for (int ch = 0; ch < 3; ch++) { hw[ch] = 1.0f + ext.weight_delta[3 * him + ch]; hb[ch] = ext.bias[3 * him + ch]; }
+            for (int ch = 0; ch < 3; ch++) { hw[ch] = 1.0f + ext.weight_delta[3 * him + ch]; hb[ch] = ext.bias ? ext.bias[3 * him + ch] : 0.0f; }
         } else him = -1;
     }
     float hgw[3] = {0.f, 0.f, 0.f}, hgb[3] = {0.f, 0.f, 0.f};
@@ -320,14 +320,21 @@ k_neus_backward(int nr_rays, int max_nr_samples, const int* __restrict__ start_e
             g_rgb[3 * k] = q0; g_rgb[3 * k + 1] = q1; g_rgb[3 * k + 2] = q2;
         }
     }
-    if (ext.head && him >= 0 && ext.g_weight_delta) {
+    if (ext.head && him >= 0 && (ext.g_weight_delta || ext.g_bias)) {
+        // each of the two gradients only where its buffer is given: a fixed-point total without a destination would never be flushed
+        // (and cleared), and would reach the next launch's
 #pragma unroll
         for (int c = 0; c < 3; c++) {
             float sw = hgw[c], sb = hgb[c];
 #pragma unroll
             for (int o = 16; o > 0; o >>= 1) { sw += __shfl_xor_sync(kFull, sw, o); sb += __shfl_xor_sync(kFull, sb, o); }
-            if (lane == 0 && ext.fx && him < kDetImages) { fx_add(ext.fx + 3 * him + c, sw); fx_add(ext.fx + 3 * kDetImages + 3 * him + c, sb); }
-            else if (lane == 0) { atomicAdd(ext.g_weight_delta + 3 * him + c, sw); atomicAdd(ext.g_bias + 3 * him + c, sb); }
+            if (lane == 0 && ext.fx && him < kDetImages) {
+                if (ext.g_weight_delta) fx_add(ext.fx + 3 * him + c, sw);
+                if (ext.g_bias) fx_add(ext.fx + 3 * kDetImages + 3 * him + c, sb);
+            } else if (lane == 0) {
+                if (ext.g_weight_delta) atomicAdd(ext.g_weight_delta + 3 * him + c, sw);
+                if (ext.g_bias) atomicAdd(ext.g_bias + 3 * him + c, sb);
+            }
         }
     }
     if (g_inv_s) {
@@ -419,7 +426,7 @@ int psdf_neus_render_loss_backward(int nr_rays, int max_nr_samples, const int* r
 
 // The same pair for the direct (autograd-free) iteration: the colour head (calibration + sigmoid) and the curvature term are folded in and
 // the tail rows of the gradient buffers are zero-filled by the backward launch (see NeusExt). x_raw [N,3] is the colour network's linear
-// output; img_idx / weight_delta / bias may be NULL (no calibration). weights may be NULL.
+// output; img_idx / weight_delta may be NULL (no calibration), bias may be NULL (zero bias). weights may be NULL.
 int psdf_neus_head_loss_forward(int nr_rays, int max_nr_samples, const int* ray_start_end, int equal, int fixed_n, const float* sdf,
                                 const float* grad, const float* x_raw, const float* dirs, const float* dt, const float* inv_s_dev,
                                 float cos_anneal_ratio, const float* cos_anneal_dev, const float* gt_rgb, const float* gt_mask, const uint8_t* hit,
@@ -434,7 +441,7 @@ int psdf_neus_head_loss_forward(int nr_rays, int max_nr_samples, const int* ray_
 }
 // -> g_sdf [n_rows], g_grad [n_rows,3] (compositing + eikonal + curvature terms), g_x [n_rows,3] (d loss / d raw colour output),
 // g_grad_shifted [n_rows,3] (curvature term wrt the shifted-point gradients; grad_shifted may be NULL: no curvature term), per-image
-// calibration gradients (+=, may be NULL). curv_scale multiplies the curvature MEAN over nr_samples_dev[0] (or max_nr_samples) rows.
+// calibration gradients (+=, each may be NULL). curv_scale multiplies the curvature MEAN over nr_samples_dev[0] (or max_nr_samples) rows.
 // nr_valid_dev [1] (static-capacity containers): rows [nr_valid_dev[0], n_rows) of the four gradient buffers are zero-filled.
 int psdf_neus_head_loss_backward(int nr_rays, int max_nr_samples, const int* ray_start_end, int equal, int fixed_n, const float* sdf,
                                  const float* grad, const float* x_raw, const float* dirs, const float* dt, const float* inv_s_dev,
@@ -490,7 +497,7 @@ int psdf_neus_head_bg_loss_backward(int nr_rays, int max_nr_samples, const int* 
                               nullptr, scale_rgb, scale_mask, scale_eik, nr_samples_dev, g_sdf, g_grad, g_x, g_bg_rgb, nullptr, e, stream);
 }
 // Forward-only compositing of a rendered frame (Trainer.render): the render mode of k_neus_forward, colour head on, no loss terms, nothing
-// stored per sample. x_raw [N,3] is the colour network's linear output; img_idx / weight_delta / bias may be NULL (no calibration),
+// stored per sample. x_raw [N,3] is the colour network's linear output; img_idx / weight_delta may be NULL (no calibration), bias NULL is zero,
 // bg_rgb [R,3] may be NULL (no background). pred_rgb_bg is written only with bg_rgb.
 int psdf_neus_render_forward(int nr_rays, int max_nr_samples, const int* ray_start_end, int equal, int fixed_n, const float* sdf, const float* grad,
                              const float* x_raw, const float* dirs, const float* dt, const float* inv_s_dev, float cos_anneal_ratio, const int* img_idx,
