@@ -109,6 +109,11 @@ __device__ __forceinline__ void activation(float z, float tz, float bias, float&
     g1 = d1;
 }
 
+// v broadcast from lane 0. For values that are the same in every lane of a warp but that ptxas cannot prove so: the warp index, and
+// the per-layer geometry P.g.*[l] under a runtime l (read per thread with a register index). Branches and wgmma k-loops bounded by
+// such values count as divergent for ptxas, which then spills more and reports C7520 for this kernel.
+__device__ __forceinline__ int warp_uniform(int v) { return __shfl_sync(0xffffffffu, v, 0); }
+
 // columns [n0, n0 + 16) of  dW (+)= zbar^T a + tzbar^T ta  into the issuing warpgroup's registers (M = 64, umma::wg_mma_regs fragments):
 // both tile sets consumed as MN-major operands, K = the 128 samples, the value stream then the tangent stream in one chain. Issue only.
 __device__ __forceinline__ void issue_dw16(float* d, const uint8_t* zset, const uint8_t* aset, int n0, bool accumulate) {
@@ -144,7 +149,7 @@ k_sdf_fused_backward(FusedParams P, Segments S, const float2* __restrict__ latti
     // warp's zbar fragments for the bias column sums
     float* s_bx = s_seed;
 
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const int tid = threadIdx.x, warp = warp_uniform(tid >> 5), lane = tid & 31;
     const int row = tid & 127, grp = tid >> 7;
     const int level_cores = P.L / 4;
     const int K0 = P.g.Kp[0];
@@ -258,13 +263,13 @@ k_sdf_fused_backward(FusedParams P, Segments S, const float2* __restrict__ latti
                 }
             }
             int n0, nn;
-            split_n(P.g.Np[l], nh, n0, nn);
+            split_n(warp_uniform(P.g.Np[l]), nh, n0, nn);
             float acc[2][16];
 #pragma unroll
             for (int i = 0; i < 16; i++) { acc[0][i] = 0.f; acc[1][i] = 0.f; }
             const uint32_t ro = (uint32_t)(mh * 8 * kSBO_A);
-            if (nn == 32) streams_product<32, 2>(acc[0], at, 2 * kATileBytes, kATileBytes, ro, s_w + P.g.w_hi[l], s_w + P.g.w_lo[l], P.g.Kp[l], n0);
-            else if (nn == 16) streams_product<16, 2>(acc[0], at, 2 * kATileBytes, kATileBytes, ro, s_w + P.g.w_hi[l], s_w + P.g.w_lo[l], P.g.Kp[l], n0);
+            if (nn == 32) streams_product<32, 2>(acc[0], at, 2 * kATileBytes, kATileBytes, ro, s_w + warp_uniform(P.g.w_hi[l]), s_w + warp_uniform(P.g.w_lo[l]), warp_uniform(P.g.Kp[l]), n0);
+            else if (nn == 16) streams_product<16, 2>(acc[0], at, 2 * kATileBytes, kATileBytes, ro, s_w + warp_uniform(P.g.w_hi[l]), s_w + warp_uniform(P.g.w_lo[l]), warp_uniform(P.g.Kp[l]), n0);
             if (l < 2) {
                 // fragment block j of stream s -> slot 8 l + 4 s + j (thread-private: read back by this thread in the reverse step l + 1)
 #pragma unroll
@@ -273,7 +278,7 @@ k_sdf_fused_backward(FusedParams P, Segments S, const float2* __restrict__ latti
                     for (int j = 0; j < 4; j++)
                         if (8 * j < nn) stash[(8 * l + 4 * s + j) * kBwdThreads] = make_float4(acc[s][4 * j], acc[s][4 * j + 1], acc[s][4 * j + 2], acc[s][4 * j + 3]);
             }
-            const float* bias = reinterpret_cast<const float*>(s_w + P.g.bias[l]);
+            const float* bias = reinterpret_cast<const float*>(s_w + warp_uniform(P.g.bias[l]));
 #pragma unroll
             for (int j = 0; j < 4; j++) {
                 if (8 * j < nn) {
@@ -331,8 +336,8 @@ k_sdf_fused_backward(FusedParams P, Segments S, const float2* __restrict__ latti
             __syncthreads();
             if (l == 0) umma::mbar_wait(&bars[0], ld_phase);     // a_0 | ta_0 are back in Y
             int n0, nn;
-            split_n(P.g.Kp[l], nh, n0, nn);
-            const bool dw = 16 * wgi < P.g.Kp[l];              // this warpgroup's 16 columns of dW_l
+            split_n(warp_uniform(P.g.Kp[l]), nh, n0, nn);
+            const bool dw = 16 * wgi < warp_uniform(P.g.Kp[l]);              // this warpgroup's 16 columns of dW_l
             float4* dws = stash + (kStashDw + 2 * l) * kBwdThreads;
             float acc[2][16], dwa[8];                          // acc[0] = abar_l, acc[1] = tabar_l; dwa: the CTA's sum of dW_l
 #pragma unroll
@@ -344,8 +349,8 @@ k_sdf_fused_backward(FusedParams P, Segments S, const float2* __restrict__ latti
             }
             const uint32_t ro = (uint32_t)(mh * 8 * kSBO_A);
             umma::wgmma_fence();
-            if (nn == 32) streams_product_wt<32, 2>(acc[0], s_X, 2 * kATileBytes, kATileBytes, ro, s_w + P.g.w_hi[l], s_w + P.g.w_lo[l], P.g.Kp[l], P.g.Np[l], n0);
-            else if (nn == 16) streams_product_wt<16, 2>(acc[0], s_X, 2 * kATileBytes, kATileBytes, ro, s_w + P.g.w_hi[l], s_w + P.g.w_lo[l], P.g.Kp[l], P.g.Np[l], n0);
+            if (nn == 32) streams_product_wt<32, 2>(acc[0], s_X, 2 * kATileBytes, kATileBytes, ro, s_w + warp_uniform(P.g.w_hi[l]), s_w + warp_uniform(P.g.w_lo[l]), warp_uniform(P.g.Kp[l]), warp_uniform(P.g.Np[l]), n0);
+            else if (nn == 16) streams_product_wt<16, 2>(acc[0], s_X, 2 * kATileBytes, kATileBytes, ro, s_w + warp_uniform(P.g.w_hi[l]), s_w + warp_uniform(P.g.w_lo[l]), warp_uniform(P.g.Kp[l]), warp_uniform(P.g.Np[l]), n0);
             if (dw) issue_dw16(dwa, s_X, s_Y, 16 * wgi, !first_tile);
             umma::wgmma_commit();
             umma::wgmma_wait0();
@@ -398,7 +403,7 @@ k_sdf_fused_backward(FusedParams P, Segments S, const float2* __restrict__ latti
                     // a_{l-1} | ta_{l-1} -> Y and the GELU' / GELU'' factors of the next step from this thread's stashed z_{l-1} | tz_{l-1}
                     // (the forward layer l - 2 split its columns as the reverse step l - 1 does)
                     int m0, mn;
-                    split_n(P.g.Kp[l - 1], nh, m0, mn);
+                    split_n(warp_uniform(P.g.Kp[l - 1]), nh, m0, mn);
                     float z[2][16];
 #pragma unroll
                     for (int s = 0; s < 2; s++)
@@ -407,7 +412,7 @@ k_sdf_fused_backward(FusedParams P, Segments S, const float2* __restrict__ latti
                             const float4 v = (8 * j < mn) ? stash[(8 * (l - 2) + 4 * s + j) * kBwdThreads] : make_float4(0.f, 0.f, 0.f, 0.f);
                             z[s][4 * j] = v.x; z[s][4 * j + 1] = v.y; z[s][4 * j + 2] = v.z; z[s][4 * j + 3] = v.w;
                         }
-                    const float* bias = reinterpret_cast<const float*>(s_w + P.g.bias[l - 2]);
+                    const float* bias = reinterpret_cast<const float*>(s_w + warp_uniform(P.g.bias[l - 2]));
 #pragma unroll
                     for (int j = 0; j < 4; j++) {
                         if (8 * j < mn) {
