@@ -348,14 +348,15 @@ __device__ __forceinline__ void streams_product(float* acc, const uint8_t* a, in
     static_assert(S == 1 || N <= 32, "a stream's fragment holds 16 floats");
     const uint32_t sbo_w = (Kp / 8) * kLBO, wo = (uint32_t)(n0 / 8) * sbo_w;
     const uint64_t dwh = umma::make_desc(umma::smem_u32(w_hi) + wo, kLBO, sbo_w), dwl = umma::make_desc(umma::smem_u32(w_lo) + wo, kLBO, sbo_w);
-    umma::wgmma_fence();
+    uint64_t dah[S], dal[S];
 #pragma unroll
     for (int s = 0; s < S; s++) {
         const uint8_t* as = a + s * stream_bytes;
-        const uint64_t dah = umma::make_desc(umma::smem_u32(as) + row_off, kLBO, a_sbo);
-        const uint64_t dal = umma::make_desc(umma::smem_u32(as + lo_bytes) + row_off, kLBO, a_sbo);
-        umma::wg_mma_regs<N, 0, 0>(acc + 16 * s, dah, dal, dwh, dwl, (2 * kLBO) >> 4, (2 * kLBO) >> 4, Kp / 16, false);
+        dah[s] = umma::make_desc(umma::smem_u32(as) + row_off, kLBO, a_sbo);
+        dal[s] = umma::make_desc(umma::smem_u32(as + lo_bytes) + row_off, kLBO, a_sbo);
     }
+    umma::wgmma_fence();
+    umma::wg_mma_streams<N, 0, 0, S>(acc, dah, dal, dwh, dwl, (2 * kLBO) >> 4, (2 * kLBO) >> 4, Kp / 16, false);
     umma::wgmma_commit();
     umma::wgmma_wait0();
 }
@@ -369,13 +370,14 @@ __device__ __forceinline__ void streams_product_wt(float* acc, const uint8_t* a,
     static_assert(S == 1 || N <= 32, "a stream's fragment holds 16 floats");
     const uint32_t sbo_w = (Kp / 8) * kLBO, wo = (uint32_t)(n0 / 8) * kLBO;
     const uint64_t dwh = umma::make_desc(umma::smem_u32(w_hi) + wo, sbo_w, kLBO), dwl = umma::make_desc(umma::smem_u32(w_lo) + wo, sbo_w, kLBO);
+    uint64_t dah[S], dal[S];
 #pragma unroll
     for (int s = 0; s < S; s++) {
         const uint8_t* as = a + s * stream_bytes;
-        const uint64_t dah = umma::make_desc(umma::smem_u32(as) + row_off, kLBO, kSBO_A);
-        const uint64_t dal = umma::make_desc(umma::smem_u32(as + lo_bytes) + row_off, kLBO, kSBO_A);
-        umma::wg_mma_regs<N, 0, 1>(acc + 16 * s, dah, dal, dwh, dwl, (2 * kLBO) >> 4, (2 * sbo_w) >> 4, Np / 16, false);
+        dah[s] = umma::make_desc(umma::smem_u32(as) + row_off, kLBO, kSBO_A);
+        dal[s] = umma::make_desc(umma::smem_u32(as + lo_bytes) + row_off, kLBO, kSBO_A);
     }
+    umma::wg_mma_streams<N, 0, 1, S>(acc, dah, dal, dwh, dwl, (2 * kLBO) >> 4, (2 * sbo_w) >> 4, Np / 16, false);
 }
 
 
@@ -399,6 +401,11 @@ __device__ __forceinline__ void issue_gemm(uint32_t tmem_d, int mh, const uint8_
     umma::wg_gemm<0, 0>(tmem_d + ((uint32_t)(64 * mh) << 16), false, dah, dal, dwh, dwl, (2 * kLBO) >> 4, (2 * kLBO) >> 4, (8 * sbo_w) >> 4,
                         Kp / 16, Np, false);
 }
+
+// v broadcast from lane 0. For values that are the same in every lane of a warp but that ptxas cannot prove so: the warp index, and
+// the per-layer geometry P.g.*[l] under a runtime l (read per thread with a register index). Branches and wgmma k-loops bounded by
+// such values count as divergent for ptxas, which then serializes the wgmma chains behind them (C7520: a wait after every HGMMA).
+__device__ __forceinline__ int warp_uniform(int v) { return __shfl_sync(0xffffffffu, v, 0); }
 
 // ---------------------------------------------------------------------------------------------- backward helpers
 constexpr unsigned kFull = 0xffffffffu;

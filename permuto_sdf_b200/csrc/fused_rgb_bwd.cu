@@ -106,7 +106,7 @@ k_rgb_fused_backward(RgbParams P, const float* __restrict__ pos, const float* __
     // the last readers of s_z in the tile, have completed
     float* s_tail = reinterpret_cast<float*>(s_z);
 
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const int tid = threadIdx.x, warp = warp_uniform(tid >> 5), lane = tid & 31;
     const int row = tid & 127, grp = tid >> 7;
     const int wgi = warp >> 2, mh = wgi & 1, nh = wgi >> 1;
     const int pair = 2 * wgi + ((warp & 3) >> 1);          // 32-row group of this warp's fragment rows
@@ -147,10 +147,11 @@ k_rgb_fused_backward(RgbParams P, const float* __restrict__ pos, const float* __
                 umma::bulk_s2g(sp.a0 + (size_t)tile * kRgbSpillBytes, s_a, kRgbSpillBytes);
                 umma::bulk_commit();
             }
+            const int Np = warp_uniform(P.g.Np[l]), Kp = warp_uniform(P.g.Kp[l]);
             int n0, nn;
-            split_n(P.g.Np[l], nh, n0, nn);
+            split_n(Np, nh, n0, nn);
             float acc[32];
-            tile_product(acc, nn, mh, s_a, s_w, s_w + P.g.Np[l] * P.g.Kp[l] * 2, P.g.Kp[l], n0);
+            tile_product(acc, nn, mh, s_a, s_w, s_w + Np * Kp * 2, Kp, n0);
             if (l == 0 && tid == 0) umma::bulk_wait_read0();      // s_a is overwritten by this layer's epilogue: the store must have read it
             __syncthreads();                                       // every product has read s_a and s_w
             if (tid == 0) load_layer_weights(s_w, blob, P.g, l < 2 ? l + 1 : 3, l == 2, &bars[0]);   // W_{l+1}, then W_3^T
@@ -200,7 +201,7 @@ k_rgb_fused_backward(RgbParams P, const float* __restrict__ pos, const float* __
             if (l == 0) umma::mbar_wait(&bars[1], a0_phase);      // a_0 is back in s_a
             umma::fence_async_smem();
             __syncthreads();
-            const int Np = P.g.Np[l], Kp = P.g.Kp[l];
+            const int Np = warp_uniform(P.g.Np[l]), Kp = warp_uniform(P.g.Kp[l]);
             if (!first_tile) prefetch_dw_w(dw_cta + l * 128 * 128, mh, Np > 64 ? 128 : 64, Kp, nh, 2);
             int n0, nn;
             split_n(Kp, nh, n0, nn);

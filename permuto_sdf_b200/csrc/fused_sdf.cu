@@ -267,12 +267,13 @@ k_sdf_fused_dual(FusedParams P, FwdSegs G, const float2* __restrict__ lattice, c
     constexpr int S = 4;
     extern __shared__ __align__(128) uint8_t smem[];
     uint8_t* s_blob = smem;
-    const int tid = threadIdx.x, grp2 = tid >> 8, t = tid & 255;            // group of the CTA, thread inside the group
+    const int tid = threadIdx.x, warp = warp_uniform(tid >> 5), t = tid & 255;
+    const int grp2 = warp >> 3;                                              // group of the CTA; t: thread inside the group
     uint8_t* s_a = smem + P.g.total + grp2 * (S * 2 * kSubTileBytes);       // this group's S streams x {hi, lo} x 8 KB
     LevelC* lc = reinterpret_cast<LevelC*>(smem + P.g.total + 2 * S * 2 * kSubTileBytes);
     uint64_t* bars = reinterpret_cast<uint64_t*>(lc + 1);                    // [0] weights, [3] start skew
     const int lane = tid & 31;
-    const int wg = t >> 5;                                                   // warp inside the group, 0..7
+    const int wg = warp & 7;                                                 // warp inside the group, 0..7
     const int row = t & (kSub - 1), eg = t >> 6;                             // encoder: 4 threads per sample row
     constexpr int kEnc = kGroupThreads / kSub;
 
@@ -517,7 +518,9 @@ k_sdf_sphere_trace(FusedParams P, TraceParams Q, const float* __restrict__ pos_i
         const bool occupied = s_ray[row] >= 0;
         const bool active = occupied && s_ms[row] < 0;       // evaluates the network in this round
         if (__syncthreads_count(occupied) == 0) break;       // no ray left in this tile (and the queue is drained)
-        const int nact = __syncthreads_count(active);
+        // the count is the same in every thread, but ptxas cannot prove so: the network evaluation below would be a divergent path
+        // and its wgmma chains serialized (C7520)
+        const int nact = warp_uniform(__syncthreads_count(active));
         evaluations += nact / kGroups;
         float x[D];
 #pragma unroll

@@ -52,6 +52,7 @@
 // (2 slots per layer).
 #include <cstdio>
 #include <cstdlib>
+#include <type_traits>
 #include "fused_common.cuh"
 #include "../../include/psdf_b200.h"
 
@@ -108,11 +109,6 @@ __device__ __forceinline__ void activation(float z, float tz, float bias, float&
     ta = d1 * tz;
     g1 = d1;
 }
-
-// v broadcast from lane 0. For values that are the same in every lane of a warp but that ptxas cannot prove so: the warp index, and
-// the per-layer geometry P.g.*[l] under a runtime l (read per thread with a register index). Branches and wgmma k-loops bounded by
-// such values count as divergent for ptxas, which then spills more and reports C7520 for this kernel.
-__device__ __forceinline__ int warp_uniform(int v) { return __shfl_sync(0xffffffffu, v, 0); }
 
 // columns [n0, n0 + 16) of  dW (+)= zbar^T a + tzbar^T ta  into the issuing warpgroup's registers (M = 64, umma::wg_mma_regs fragments):
 // both tile sets consumed as MN-major operands, K = the 128 samples, the value stream then the tangent stream in one chain. Issue only.
@@ -348,12 +344,21 @@ k_sdf_fused_backward(FusedParams P, Segments S, const float2* __restrict__ latti
                 dwa[4 * q] = v.x; dwa[4 * q + 1] = v.y; dwa[4 * q + 2] = v.z; dwa[4 * q + 3] = v.w;
             }
             const uint32_t ro = (uint32_t)(mh * 8 * kSBO_A);
-            umma::wgmma_fence();
-            if (nn == 32) streams_product_wt<32, 2>(acc[0], s_X, 2 * kATileBytes, kATileBytes, ro, s_w + warp_uniform(P.g.w_hi[l]), s_w + warp_uniform(P.g.w_lo[l]), warp_uniform(P.g.Kp[l]), warp_uniform(P.g.Np[l]), n0);
-            else if (nn == 16) streams_product_wt<16, 2>(acc[0], s_X, 2 * kATileBytes, kATileBytes, ro, s_w + warp_uniform(P.g.w_hi[l]), s_w + warp_uniform(P.g.w_lo[l]), warp_uniform(P.g.Kp[l]), warp_uniform(P.g.Np[l]), n0);
-            if (dw) issue_dw16(dwa, s_X, s_Y, 16 * wgi, !first_tile);
-            umma::wgmma_commit();
-            umma::wgmma_wait0();
+            // the reverse product (NC columns, none for NC = 0) and the dW chain as one wgmma group. Each column count is a whole group
+            // of its own: a branch between the fence and the wait joins the fragments of the two paths inside the group, and those
+            // register moves make ptxas serialize every wgmma chain of the kernel (C7515)
+            auto products = [&](auto nc) {
+                constexpr int NC = decltype(nc)::value;
+                umma::wgmma_fence();
+                if constexpr (NC > 0)
+                    streams_product_wt<NC, 2>(acc[0], s_X, 2 * kATileBytes, kATileBytes, ro, s_w + warp_uniform(P.g.w_hi[l]), s_w + warp_uniform(P.g.w_lo[l]), warp_uniform(P.g.Kp[l]), warp_uniform(P.g.Np[l]), n0);
+                if (dw) issue_dw16(dwa, s_X, s_Y, 16 * wgi, !first_tile);
+                umma::wgmma_commit();
+                umma::wgmma_wait0();
+            };
+            if (nn == 32) products(std::integral_constant<int, 32>());
+            else if (nn == 16) products(std::integral_constant<int, 16>());
+            else products(std::integral_constant<int, 0>());
             if (dw) {
 #pragma unroll
                 for (int q = 0; q < 2; q++) dws[q * kBwdThreads] = make_float4(dwa[4 * q], dwa[4 * q + 1], dwa[4 * q + 2], dwa[4 * q + 3]);

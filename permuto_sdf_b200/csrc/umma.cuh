@@ -142,6 +142,28 @@ __device__ __forceinline__ void wg_mma_regs(float* d, uint64_t ah, uint64_t al, 
     }
 }
 
+// S independent chains of wg_mma_regs sharing the B operand (stream s: A descriptors ah[s] / al[s], D = d + 16 s), in ONE k-step loop:
+// k-step kk issues the three split products of every stream. Each stream's products accumulate in the order wg_mma_regs gives them.
+// One loop rather than S loops one after the other: ptxas serializes the chains of S guarded loops (a wait after every HGMMA).
+template <int N, int TA, int TB, int S>
+__device__ __forceinline__ void wg_mma_streams(float* d, const uint64_t* ah, const uint64_t* al, uint64_t bh, uint64_t bl, uint32_t a_step,
+                                               uint32_t b_step, int ksteps, bool accumulate) {
+    if constexpr (S == 1) {
+        wg_mma_regs<N, TA, TB>(d, ah[0], al[0], bh, bl, a_step, b_step, ksteps, accumulate);
+    } else {
+#pragma unroll 1
+        for (int kk = 0; kk < ksteps; kk++) {
+            const uint64_t oa = (uint64_t)kk * a_step, ob = (uint64_t)kk * b_step;
+#pragma unroll
+            for (int s = 0; s < S; s++) {
+                wgmma_n<N, TA, TB>(d + 16 * s, ah[s] + oa, bh + ob, (kk > 0 || accumulate) ? 1u : 0u);
+                wgmma_n<N, TA, TB>(d + 16 * s, ah[s] + oa, bl + ob, 1u);
+                wgmma_n<N, TA, TB>(d + 16 * s, al[s] + oa, bh + ob, 1u);
+            }
+        }
+    }
+}
+
 template <int N, int TA, int TB>
 __device__ __forceinline__ void wg_gemm_n(uint32_t tdst, bool m64, uint64_t ah, uint64_t al, uint64_t bh, uint64_t bl, uint32_t a_step,
                                           uint32_t b_step, int ksteps, bool accumulate) {

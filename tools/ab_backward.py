@@ -1,4 +1,4 @@
-"""Compare a training backward of two builds on one fixed, seeded problem at the shape of the C2 training step.
+"""Compare a training backward (or the SDF forward) of two builds on one fixed, seeded problem at the shape of the C2 training step.
 
     python tools/ab_backward.py run --kernel sdf --root TREE --out a.npz   # run TREE's library (default: this tree), twice, save the gradients
     python tools/ab_backward.py compare a.npz b.npz                        # gradients of two builds
@@ -10,6 +10,10 @@ sdf upstreams only): 16 levels, T = 2^18, hidden 64, out_dim 33, 1030 tiles. It 
 `--kernel rgb` calls psdf_rgb_fused_backward_acc (the colour backward of the training step) in deterministic mode: 65 536 samples, 16
 levels, T = 2^18, hidden 128 / 128 / 64, 512 tiles. It saves the lattice, weight and bias gradients, g_sdf_grad (accumulated onto a
 seeded buffer) and g_geom.
+
+`--kernel sdf_fwd` runs the value + tangent SDF forward of the training step on the same network and sample sets: `--dim 3` calls
+psdf_sdf_fused_forward_multi with the main samples (sdf, gradient, geometric features) and the off-surface points (sdf), `--dim 4`
+psdf_sdf_fused_forward_dim with space-time positions (the main samples with a seeded time column). It saves every output.
 
 `run` checks that two runs give the same bits and times the call with CUDA events. `compare` requires every saved tensor to be
 bit-identical and prints the largest difference of every tensor."""
@@ -97,6 +101,36 @@ def sdf_setup(torch, lib, call, c):
     return once, result
 
 
+def sdf_fwd_setup(torch, lib, call, c, dim):
+    p = sdf_problem(torch)
+    blob = torch.empty(int(lib.psdf_sdf_mlp_blob_bytes(2 * L + 4, HIDDEN, OUT_DIM)), dtype=torch.uint8, device="cuda")
+    call("psdf_sdf_mlp_pack", 2 * L + 4, HIDDEN, OUT_DIM, *[c(t) for l in range(4) for t in (p["W"][l], p["b"][l])], blob)
+    lat, win = c(p["lat"]), c(p["win"])
+    sdf, grad, geom = (torch.zeros(N_MAIN, k, device="cuda") for k in (1, 3, OUT_DIM - 1))
+    if dim == 3:
+        scale, shift, pos, pos_off = c(p["scale"]), c(p["shift"]), c(p["pos"][0]), c(p["pos"][2])
+        sdf_off = torch.zeros(N_OFF, 1, device="cuda")
+    else:
+        g = torch.Generator().manual_seed(99)
+        scale = c(torch.cat([p["scale"], torch.rand(L, 1, generator=g) * 20], 1))
+        shift = c(torch.cat([p["shift"], torch.randn(L, 1, generator=g)], 1))
+        pos = c(torch.cat([p["pos"][0], torch.rand(N_MAIN, 1, generator=g)], 1))
+
+    def once():
+        if dim == 3:
+            call("psdf_sdf_fused_forward_multi", L, T, lat, scale, shift, win, 1e-3, HIDDEN, OUT_DIM, blob, N_MAIN, pos, sdf, grad, geom,
+                 N_OFF, pos_off, sdf_off, None, None)
+        else:
+            call("psdf_sdf_fused_forward_dim", 4, N_MAIN, L, T, pos, lat, scale, shift, win, 1e-3, HIDDEN, OUT_DIM, blob, sdf, grad, geom)
+
+    def result():
+        r = {"sdf": sdf.cpu().numpy(), "grad": grad.cpu().numpy(), "geom": geom.cpu().numpy()}
+        if dim == 3:
+            r["sdf_off"] = sdf_off.cpu().numpy()
+        return r
+    return once, result
+
+
 def rgb_setup(torch, lib, call, c):
     p = rgb_problem(torch)
     in_dim = 2 * L + 64
@@ -132,8 +166,13 @@ def run(args):
     lib = load_library()
     assert lib.psdf_device_ok() == 1, "needs a CUDA device"
     c = lambda t: t.float().contiguous().cuda()
-    once, result = (rgb_setup if args.kernel == "rgb" else sdf_setup)(torch, lib, call, c)
-    call("psdf_set_deterministic", 1, L * T * 2, 64 ** 3)
+    if args.kernel == "sdf_fwd":
+        once, result = sdf_fwd_setup(torch, lib, call, c, args.dim)
+    else:
+        once, result = (rgb_setup if args.kernel == "rgb" else sdf_setup)(torch, lib, call, c)
+    det = args.kernel != "sdf_fwd"               # the forward has no reductions
+    if det:
+        call("psdf_set_deterministic", 1, L * T * 2, 64 ** 3)
     try:
         results = []
         for _ in range(2):
@@ -153,10 +192,11 @@ def run(args):
         torch.cuda.synchronize()
         ms = s.elapsed_time(e) / reps
     finally:
-        call("psdf_set_deterministic", 0, 0, 0)
+        if det:
+            call("psdf_set_deterministic", 0, 0, 0)
     name = torch.cuda.get_device_name(0)
-    print("%s [%s]: two runs bit-identical: %s | %.3f ms per call (zeroing + backward, deterministic, %d tiles) on %s"
-          % (args.root, args.kernel, same, ms, tiles(args.kernel), name))
+    what = "forward, D = %d" % args.dim if args.kernel == "sdf_fwd" else "zeroing + backward, deterministic, %d tiles" % tiles(args.kernel)
+    print("%s [%s]: two runs bit-identical: %s | %.3f ms per call (%s) on %s" % (args.root, args.kernel, same, ms, what, name))
     np.savez(args.out, **results[0])
     return 0 if same else 1
 
@@ -178,7 +218,8 @@ def main():
     ap = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
     sub = ap.add_subparsers(dest="cmd", required=True)
     r = sub.add_parser("run")
-    r.add_argument("--kernel", choices=["sdf", "rgb"], default="sdf", help="which training backward runs")
+    r.add_argument("--kernel", choices=["sdf", "rgb", "sdf_fwd"], default="sdf", help="which training backward (or the SDF forward) runs")
+    r.add_argument("--dim", type=int, choices=[3, 4], default=3, help="input width of the SDF forward (--kernel sdf_fwd)")
     r.add_argument("--root", default=ROOT, help="tree whose permuto_sdf_b200 package (and built library) runs")
     r.add_argument("--out", required=True)
     c = sub.add_parser("compare")
