@@ -3,6 +3,7 @@
 // one level and its lattice scatter, GELU and its derivatives, operand tile stores (bf16 hi/lo split in the core-matrix operand
 // layout) and the split-product GEMM issue.
 #pragma once
+#include <type_traits>
 #include "common.cuh"
 #include "umma.cuh"
 
@@ -548,6 +549,40 @@ __device__ __forceinline__ bool frag_pair_colsum(const float* v, int nn, float* 
         }
     cs = frag_colsum8(bs, lane, col);
     return col < nn;
+}
+
+// Weight gradients of a persistent backward kernel whose CTAs each leave their sum of every weight in a slab of their own, with plain
+// stores: slot (l, m, k) of CTA c at (c * kNL + l) * LD * LD + m * LD + k. The CTAs' values of one slot (layer blockIdx.y, row-major
+// index i over the true [N_l, K_l]; Slab::get() is the slab array's device address) are added up over the CTAs of chunk blockIdx.z, then one atomic adds the partial sum. T = unsigned
+// long long: fixed-point sums (fx_of), added in integer arithmetic (exact, in any order) and then into the deterministic accumulators,
+// or as their float value into the gradient; T = float: float sums, added into the gradient. Flushing every CTA's sums with atomics at
+// the end of the persistent kernel is bound by the L2 atomic throughput on the same few thousand addresses (one reduction per weight
+// and CTA); here the sums are read once with coalesced loads and kDwReduceChunks partial sums per slot are reduced.
+constexpr int kDwReduceThreads = 256, kDwReduceChunks = 4;
+struct DwSums {
+    float* gW[kNL];                 // [N_l, K_l] (+=)
+    unsigned long long* fx_mlp;     // deterministic mode (T = unsigned long long): fixed-point accumulators, layer l at l * fx_w; else NULL
+    int fx_w;
+};
+template <int LD, typename T, typename Slab>
+static __global__ void __launch_bounds__(kDwReduceThreads) k_dw_reduce(MlpGeom g, int ctas, DwSums s) {
+    const int l = blockIdx.y;
+    // no dynamic indexing of the parameter struct (local-memory copy)
+    const int K = l == 0 ? g.K[0] : (l == 1 ? g.K[1] : (l == 2 ? g.K[2] : g.K[3]));
+    const int N = l == 0 ? g.N[0] : (l == 1 ? g.N[1] : (l == 2 ? g.N[2] : g.N[3]));
+    const int i = blockIdx.x * kDwReduceThreads + threadIdx.x;
+    if (i >= N * K) return;
+    const int m = i / K, k = i - m * K;
+    const int per = (ctas + kDwReduceChunks - 1) / kDwReduceChunks, c0 = blockIdx.z * per, c1 = min(ctas, c0 + per);
+    const T* src = reinterpret_cast<const T*>(Slab::get()) + (size_t)l * LD * LD + m * LD + k;
+    T v = T(0);
+#pragma unroll 8
+    for (int c = c0; c < c1; c++) v += src[(size_t)c * kNL * LD * LD];
+    if (v == T(0)) return;
+    float* gw = l == 0 ? s.gW[0] : (l == 1 ? s.gW[1] : (l == 2 ? s.gW[2] : s.gW[3]));
+    if constexpr (std::is_same<T, float>::value) atomicAdd(gw + i, v);
+    else if (s.fx_mlp) atomicAdd(s.fx_mlp + l * s.fx_w + i, v);
+    else atomicAdd(gw + i, (float)((double)(long long)v / kFxScale));
 }
 
 

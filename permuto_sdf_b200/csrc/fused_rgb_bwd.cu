@@ -1,14 +1,14 @@
 // Training backward of the fused colour network (sm_90a, wgmma): d loss / d (linear rgb) per sample in ->
 // lattice gradient, d loss / d sdf-gradient (through the normalisation), d loss / d geom feature, weight + bias gradients of the 4
 // linear layers. Replaces loss.backward() through RGB.forward (permuto_sdf_py/models/models.py:395-414) -- encoding backward,
-// 4 x (GELU backward, 2 GEMMs), normalize / cat backward. Three kernels: the persistent tensor-core kernel below, the cross-CTA sum of
-// its weight-gradient sums (k_rgb_dw_reduce) and the full-occupancy lattice scatter k_lattice_scatter (fused_rgb_common.cuh, shared
-// with the background backward).
+// 4 x (GELU backward, 2 GEMMs), normalize / cat backward. Four kernels: the input-tile kernel k_rgb_input_tiles (48 warps per SM), the
+// persistent tensor-core kernel below, the cross-CTA sum of its weight-gradient sums (k_dw_reduce, fused_common.cuh) and the
+// full-occupancy lattice scatter k_lattice_scatter (fused_rgb_common.cuh, shared with the background backward).
 //
 // Per 128-sample tile (512 threads). Every product lands in the registers of the warpgroup that issues it: warpgroup (mh, nh) =
 // (wgi & 1, wgi >> 1) forms rows 64 mh .. 64 mh + 63 x column half nh (split_n) and consumes them in place.
-//   1. input tile a_0 (encoder gather + SH + normal + geom, per-row layout: row = tid & 127, group = tid >> 7) as in the forward; a_0
-//      leaves by ONE TMA store (64 KB / tile, re-read from L2 by the same CTA for dW_0: the only spill);
+//   1. input tile a_0 (encoder gather + SH + normal + geom, built by k_rgb_input_tiles into the workspace) -> s_a by ONE TMA load
+//      (64 KB / tile, loaded again for dW_0). The next tile's load is issued as soon as the step-0 products have read s_a;
 //   2. forward recompute, layers 0..2: a_{l+1} = gelu(z^(l) + b_l) -> s_a straight from the fragments; the raw z^(l) go to this thread's
 //      slots of the CTA's stash (global, L2 resident) and come back to the same thread in the reverse sweep: the reverse step l splits
 //      its Kp_l = Np_{l-1} columns exactly as the forward layer l-1 split them, so it needs no barrier;
@@ -17,7 +17,7 @@
 //      of the WEIGHT GRADIENT dW_l = zbar^(l)^T a_l, formed on the tensor cores from the two tiles as they sit in shared memory (the
 //      sample axis is the MMA K dimension and an operand tile in the K-major core-matrix layout is an MN-major operand for that
 //      product, see fused_sdf_bwd.cu). Each warpgroup adds its dW pieces from its registers to the CTA's fixed-point sums (each slot
-//      owned by one thread: no atomics); k_rgb_dw_reduce adds up the CTAs' sums after the launch -- with the same totals as a per-tile
+//      owned by one thread: no atomics); k_dw_reduce adds up the CTAs' sums after the launch -- with the same totals as a per-tile
 //      fixed-point flush. After a barrier the fragments become zbar^(l-1) = abar_l gelu'(z^(l-1)) -> s_z, the bias gradient
 //      (frag_pair_colsum: the bits of the per-row colsum16), and a_{l-1} is rebuilt into s_a from the stashed z^(l-2) (l = 3, 2) or
 //      comes back by TMA (l = 1);
@@ -44,6 +44,7 @@ __device__ float4 g_stash_rgb_bwd[(size_t)kAccCtas * kStashSlots * kRgbThreads];
 // weight-gradient sums of each CTA in fixed point (common.cuh fx_of), [CTA][layer][128 rows][128 columns]
 constexpr int kDwSlots = kNL * 128 * 128;
 __device__ unsigned long long g_dw_rgb_bwd[(size_t)kAccCtas * kDwSlots];
+struct RgbDwSlab { static __device__ const void* get() { return g_dw_rgb_bwd; } };
 constexpr int kFxW = kDetRgbW, kFxB = 4 * kDetRgbW;    // weight / bias offsets in DetBufs::rgb_mlp
 constexpr int kRgbSpillBytes = 2 * kWTileBytes;      // [hi | lo] of one operand tile
 constexpr int kTailCols = 3 + kGeomDim;              // abar_0 columns of the normal and the geom feature
@@ -51,16 +52,15 @@ constexpr int kTailLd = kTailCols + 1;               // row stride of their fp32
 constexpr int kBxBytes = 8 * 16 * 32 * sizeof(float);   // odd warps' fragments of the bias column sums, [8 warp pairs][16][32 lanes]
 
 struct RgbSpill {
-    uint8_t* a0;         // [ntiles][64 KB] input tiles a_0 (written and re-read by the same CTA)
+    const uint8_t* a0;   // [ntiles][64 KB] input tiles a_0 (k_rgb_input_tiles)
     float2* xch;         // [L][xch_stride] abar_0 of every level and sample slot (tile * 128 + row)
     int xch_stride;      // sample slots = ntiles * 128
-    float* gW[kNL];      // [N_l, K_l] (+=)
     float* gbias[kNL];   // (+=)
     unsigned long long* fx_mlp;         // deterministic mode: fixed-point accumulators (DetBufs::rgb_mlp), else NULL
     unsigned long long* phase_cycles;   // [16] += clock64 deltas of thread 0 per phase (PSDF_PHASE_TIMING=1, diagnostics), else NULL
 };
 // phase ids of the diagnostic counters
-enum { kPhEncoder = 0, kPhForward0 = 1, kPhSeed = 4, kPhReverse3 = 5, kPhTail = 9, kPhFlush = 10, kPhTiles = 11 };
+enum { kPhTileLoad = 0, kPhForward0 = 1, kPhSeed = 4, kPhReverse3 = 5, kPhTail = 9, kPhFlush = 10, kPhTiles = 11 };
 #define PSDF_PHASE(id)                                                                     \
     do {                                                                                   \
         if (sp.phase_cycles && tid == 0) {                                                 \
@@ -85,22 +85,36 @@ __device__ __forceinline__ void tile_product(float* acc, int nn, int mh, const u
     }
 }
 
+// Layer-0 input tiles of every tile of the launch -> a0 ([tile][64 KB], the bytes build_input_tile writes into s_a in the forward):
+// block = (tile, group) with one thread per row, so a warp is 32 consecutive rows of one group, as in the per-row layout of the persistent
+// kernels. Cores past Kp[0] are not written.
+constexpr int kInputTileThreads = kTile;
+__global__ void __launch_bounds__(kInputTileThreads)
+k_rgb_input_tiles(RgbParams P, const float* __restrict__ pos, const float* __restrict__ dirs, const float* __restrict__ sdf_grad,
+                  const float* __restrict__ geom, const float2* __restrict__ lattice, const float* __restrict__ scale,
+                  const float* __restrict__ shift, const float* __restrict__ window, uint8_t* __restrict__ a0) {
+    __shared__ LevelC lc;
+    load_level_consts(&lc, P.L, scale, shift, window, threadIdx.x, kInputTileThreads);
+    __syncthreads();
+    const int tile = blockIdx.x / kRgbGroups, grp = blockIdx.x % kRgbGroups, row = threadIdx.x;
+    const int n = tile * kTile + row;
+    uint8_t* t = a0 + (size_t)tile * kRgbSpillBytes;
+    build_input_tile(P, &lc, lattice, pos, dirs, sdf_grad, geom, n, n < P.N, row, grp, t, t + kWTileBytes);
+}
+
 __global__ void __launch_bounds__(kRgbThreads, 1)
-k_rgb_fused_backward(RgbParams P, const float* __restrict__ pos, const float* __restrict__ dirs, const float* __restrict__ sdf_grad,
-                     const float* __restrict__ geom, const float2* __restrict__ lattice, const float* __restrict__ scale,
-                     const float* __restrict__ shift, const float* __restrict__ window, const uint8_t* __restrict__ blob,
-                     const float* __restrict__ g_out, float* __restrict__ g_sdf_grad, float* __restrict__ g_geom, RgbSpill sp) {
+k_rgb_fused_backward(RgbParams P, const float* __restrict__ sdf_grad, const uint8_t* __restrict__ blob, const float* __restrict__ g_out,
+                     float* __restrict__ g_sdf_grad, float* __restrict__ g_geom, RgbSpill sp) {
     extern __shared__ __align__(128) uint8_t smem[];
     uint8_t* s_a = smem;                                   // activation tiles [hi | lo]
     uint8_t* s_z = s_a + 2 * kWTileBytes;                  // adjoint tiles [hi | lo]
     uint8_t* s_w = s_z + 2 * kWTileBytes;                  // weights of the current GEMM [hi | lo]
-    LevelC* lc = reinterpret_cast<LevelC*>(s_w + 2 * kWTileBytes);
-    float* s_bias = reinterpret_cast<float*>(lc + 1);      // 4 x 128
+    float* s_bias = reinterpret_cast<float*>(s_w + 2 * kWTileBytes);      // 4 x 128
     // 4 x 128 bias-gradient accumulators of this CTA: float (s_gbf), or fixed point (s_gb) in deterministic mode
     unsigned long long* s_gb = reinterpret_cast<unsigned long long*>(s_bias + kNL * 128);
     float* s_gbf = reinterpret_cast<float*>(s_gb);
     const bool det = sp.fx_mlp != nullptr;
-    uint64_t* bars = reinterpret_cast<uint64_t*>(s_gb + kNL * 128);   // [0] weights, [1] a_0 reload
+    uint64_t* bars = reinterpret_cast<uint64_t*>(s_gb + kNL * 128);   // [0] weights, [1] a_0 reload for dW_0, [2] tile loads
     float* s_bx = reinterpret_cast<float*>(bars + 8);      // bias column sums: the odd warps' fragments (frag_pair_colsum)
     // staging tile of abar_0's normal | geom columns, [128][kTailLd] fp32 over s_z: written after the last reverse step's products,
     // the last readers of s_z in the tile, have completed
@@ -114,27 +128,33 @@ k_rgb_fused_backward(RgbParams P, const float* __restrict__ pos, const float* __
     if (tid == 0) {
         umma::mbar_init(&bars[0], 1);
         umma::mbar_init(&bars[1], 1);
+        umma::mbar_init(&bars[2], 1);
         umma::mbar_fence_init();
     }
-    load_level_consts(lc, P.L, scale, shift, window, tid, kRgbThreads);
     for (int i = tid; i < kNL * 128; i += kRgbThreads) {
         int l = i >> 7, c = i & 127;
         s_bias[i] = (c < P.g.Np[l]) ? reinterpret_cast<const float*>(blob + P.g.bias[l])[c] : 0.0f;
         s_gb[i] = 0ull;        // also clears s_gbf
     }
     __syncthreads();
-    uint32_t w_phase = 0, a0_phase = 0;
+    uint32_t w_phase = 0, a0_phase = 0, tl_phase = 0;
     unsigned long long* dw_cta = g_dw_rgb_bwd + (size_t)blockIdx.x * kDwSlots;    // this CTA's weight-gradient sums, layer l at l * 128 * 128
 
     const int ntiles = (P.N + kTile - 1) / kTile;
-    if (tid == 0 && blockIdx.x < ntiles) load_layer_weights(s_w, blob, P.g, 0, false, &bars[0]);
+    if (tid == 0 && blockIdx.x < ntiles) {
+        load_layer_weights(s_w, blob, P.g, 0, false, &bars[0]);
+        umma::mbar_expect_tx(&bars[2], (uint32_t)kRgbSpillBytes);
+        umma::bulk_g2s(s_a, sp.a0 + (size_t)blockIdx.x * kRgbSpillBytes, (uint32_t)kRgbSpillBytes, &bars[2]);
+    }
     long long phase_t0 = sp.phase_cycles ? clock64() : 0;
     for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
         const bool first_tile = tile == (int)blockIdx.x;
         const int n = tile * kTile + row;
         const bool valid = n < P.N;
-        build_input_tile(P, lc, lattice, pos, dirs, sdf_grad, geom, n, valid, row, grp, s_a, s_a + kWTileBytes);
-        PSDF_PHASE(kPhEncoder);
+        // a_0 of this tile -> s_a (TMA load issued next to the first weight load or after the previous tile's step 0)
+        umma::mbar_wait(&bars[2], tl_phase);
+        tl_phase ^= 1;
+        PSDF_PHASE(kPhTileLoad);
 
         // ---------------- forward recompute, layers 0..2
 #pragma unroll 1
@@ -143,16 +163,11 @@ k_rgb_fused_backward(RgbParams P, const float* __restrict__ pos, const float* __
             w_phase ^= 1;
             umma::fence_async_smem();
             __syncthreads();
-            if (l == 0 && tid == 0) {        // a_0 leaves as it is (needed again for dW_0 at the end of the reverse sweep)
-                umma::bulk_s2g(sp.a0 + (size_t)tile * kRgbSpillBytes, s_a, kRgbSpillBytes);
-                umma::bulk_commit();
-            }
             const int Np = warp_uniform(P.g.Np[l]), Kp = warp_uniform(P.g.Kp[l]);
             int n0, nn;
             split_n(Np, nh, n0, nn);
             float acc[32];
             tile_product(acc, nn, mh, s_a, s_w, s_w + Np * Kp * 2, Kp, n0);
-            if (l == 0 && tid == 0) umma::bulk_wait_read0();      // s_a is overwritten by this layer's epilogue: the store must have read it
             __syncthreads();                                       // every product has read s_a and s_w
             if (tid == 0) load_layer_weights(s_w, blob, P.g, l < 2 ? l + 1 : 3, l == 2, &bars[0]);   // W_{l+1}, then W_3^T
             // raw z^(l) -> this thread's stash slots (read back by this thread in the reverse steps l + 1 and l + 2), a_{l+1} -> s_a
@@ -213,9 +228,12 @@ k_rgb_fused_backward(RgbParams P, const float* __restrict__ pos, const float* __
             __syncthreads();                                       // every product of this step has read s_z, s_a and s_w
             if (tid == 0) {
                 if (l > 0) load_layer_weights(s_w, blob, P.g, l - 1, true, &bars[0]);
-                else if (tile + (int)gridDim.x < ntiles) load_layer_weights(s_w, blob, P.g, 0, false, &bars[0]);
-                if (l == 1) {                  // s_a is free: a_0 returns by TMA for the last step (its store completed long ago)
-                    umma::bulk_wait0();
+                else if (tile + (int)gridDim.x < ntiles) {       // the next tile's W_0 and, s_a being free, its a_0
+                    load_layer_weights(s_w, blob, P.g, 0, false, &bars[0]);
+                    umma::mbar_expect_tx(&bars[2], (uint32_t)kRgbSpillBytes);
+                    umma::bulk_g2s(s_a, sp.a0 + (size_t)(tile + gridDim.x) * kRgbSpillBytes, (uint32_t)kRgbSpillBytes, &bars[2]);
+                }
+                if (l == 1) {                  // s_a is free: a_0 returns by TMA for the last step
                     umma::mbar_expect_tx(&bars[1], (uint32_t)kRgbSpillBytes);
                     umma::bulk_g2s(s_a, sp.a0 + (size_t)tile * kRgbSpillBytes, (uint32_t)kRgbSpillBytes, &bars[1]);
                 }
@@ -326,45 +344,19 @@ k_rgb_fused_backward(RgbParams P, const float* __restrict__ pos, const float* __
                 else { o[0] = ox; o[1] = oy; o[2] = oz; }
             }
         }
-        // no barrier before the next tile: s_a was last read by this tile's step-0 products, s_tail (over s_z) is next written by the
-        // next tile's seed, several barriers later
+        // no barrier before the next tile: s_a was last read by this tile's step-0 products (the next tile's a_0 arrives by TMA, behind
+        // the mbarrier), s_tail (over s_z) is next written by the next tile's seed, several barriers later
         PSDF_PHASE(kPhTail);
         if (sp.phase_cycles && tid == 0) atomicAdd(sp.phase_cycles + kPhTiles, 1ull);
     }
     __syncthreads();
-    // ---- bias gradients of this CTA (the weight-gradient sums are added up across CTAs by k_rgb_dw_reduce)
+    // ---- bias gradients of this CTA (the weight-gradient sums are added up across CTAs by k_dw_reduce)
     for (int i = tid; i < kNL * 128; i += kRgbThreads) {
         int l = i >> 7, c = i & 127;
         if (det) { if (c < P.g.N[l] && s_gb[i] != 0ull) atomicAdd(sp.fx_mlp + kFxB + l * 128 + c, s_gb[i]); }
         else if (c < P.g.N[l] && s_gbf[i] != 0.0f) atomicAdd(sp.gbias[l] + c, s_gbf[i]);
     }
     PSDF_PHASE(kPhFlush);
-    if (tid == 0) umma::bulk_wait0();
-}
-
-// Weight gradients: the CTAs' fixed-point sums of one slot (layer blockIdx.y, row-major index i over the true [N_l, K_l]) added up in
-// integer arithmetic (exact, in any order) over the CTAs of chunk blockIdx.z, then one integer atomic into the deterministic
-// accumulators, or the float value of the partial sum added to the gradient (+=). Flushing every CTA's sums with atomics at the end of
-// the persistent kernel was bound by the L2 atomic throughput: 37 k reductions per CTA, 4.9 M per C2 call, all to the same 37 k
-// addresses; here the sums are read once with coalesced loads and 4 partial sums per slot are reduced.
-constexpr int kDwReduceThreads = 256, kDwReduceChunks = 4;
-__global__ void __launch_bounds__(kDwReduceThreads)
-k_rgb_dw_reduce(MlpGeom g, int ctas, RgbSpill sp) {
-    const int l = blockIdx.y;
-    // no dynamic indexing of the parameter struct (local-memory copy)
-    const int K = l == 0 ? g.K[0] : (l == 1 ? g.K[1] : (l == 2 ? g.K[2] : g.K[3]));
-    const int N = l == 0 ? g.N[0] : (l == 1 ? g.N[1] : (l == 2 ? g.N[2] : g.N[3]));
-    const int i = blockIdx.x * kDwReduceThreads + threadIdx.x;
-    if (i >= N * K) return;
-    const int m = i / K, k = i - m * K;
-    const int per = (ctas + kDwReduceChunks - 1) / kDwReduceChunks, c0 = blockIdx.z * per, c1 = min(ctas, c0 + per);
-    const unsigned long long* src = g_dw_rgb_bwd + (size_t)l * 128 * 128 + m * 128 + k;
-    unsigned long long v = 0ull;
-#pragma unroll 8
-    for (int c = c0; c < c1; c++) v += src[(size_t)c * kDwSlots];
-    if (v == 0ull) return;
-    if (sp.fx_mlp) atomicAdd(sp.fx_mlp + l * kFxW + i, v);
-    else atomicAdd((l == 0 ? sp.gW[0] : (l == 1 ? sp.gW[1] : (l == 2 ? sp.gW[2] : sp.gW[3]))) + i, (float)((double)(long long)v / kFxScale));
 }
 
 #define ST ((cudaStream_t)stream)
@@ -372,8 +364,8 @@ k_rgb_dw_reduce(MlpGeom g, int ctas, RgbSpill sp) {
 
 extern "C" {
 
-// workspace per 128-sample tile: the input operand tile a_0 (64 KB), written by TMA store in the forward recompute and read back by the
-// same CTA for the first layer's weight gradient, and the exchange rows of abar_0 (8 bytes per sample and level, sized for kMaxLevels
+// workspace per 128-sample tile: the input operand tile a_0 (64 KB), written by k_rgb_input_tiles and loaded by TMA into the persistent
+// kernel twice (forward recompute and the first layer's weight gradient), and the exchange rows of abar_0 (8 bytes per sample and level, sized for kMaxLevels
 // so that the size depends on the sample count alone)
 long long psdf_rgb_fused_backward_workspace_bytes(int N) {
     const int ntiles = div_up(N > 0 ? N : 1, kTile);
@@ -396,16 +388,17 @@ static int rgb_backward_impl(int N, int L, int T, const float* pos, const float*
     RgbSpill sp;
     float* b[kNL] = {gb0, gb1, gb2, gb3};
     float* w[kNL] = {gW0, gW1, gW2, gW3};
-    for (int l = 0; l < kNL; l++) { sp.gbias[l] = b[l]; sp.gW[l] = w[l]; }
+    for (int l = 0; l < kNL; l++) sp.gbias[l] = b[l];
     sp.fx_mlp = dbuf ? dbuf->rgb_mlp : nullptr;
     const int ntiles = div_up(N, kTile);
-    sp.a0 = workspace;
+    uint8_t* a0 = workspace;
+    sp.a0 = a0;
     sp.xch = reinterpret_cast<float2*>(workspace + (size_t)ntiles * kRgbSpillBytes);
     sp.xch_stride = ntiles * kTile;
     // diagnostics: PSDF_PHASE_TIMING=1 prints thread 0's clock64 breakdown per phase (average cycles per tile) after every launch
     static const bool timing = getenv("PSDF_PHASE_TIMING") && atoi(getenv("PSDF_PHASE_TIMING")) != 0;
     static unsigned long long* d_cycles = nullptr;
-    static cudaEvent_t ev[4];
+    static cudaEvent_t ev[5];
     sp.phase_cycles = nullptr;
     if (timing) {
         if (!d_cycles) {
@@ -419,23 +412,31 @@ static int rgb_backward_impl(int N, int L, int T, const float* pos, const float*
     int dev = 0, sms = 132;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    const size_t smem = (size_t)6 * kWTileBytes + sizeof(LevelC) + kNL * 128 * (sizeof(float) + sizeof(unsigned long long)) + 64 + kBxBytes;
+    const size_t smem = (size_t)6 * kWTileBytes + kNL * 128 * (sizeof(float) + sizeof(unsigned long long)) + 64 + kBxBytes;
     // per device: set on every call (a second GPU needs its own opt-in)
     { static bool optin_[64]; psdf::psdf_optin_smem(k_rgb_fused_backward, 227 * 1024, optin_); }
     const int ctas = min(min(ntiles, sms), kAccCtas);
-    k_rgb_fused_backward<<<ctas, kRgbThreads, smem, ST>>>(P, pos, dirs, sdf_grad, geom, reinterpret_cast<const float2*>(lattice),
-                                                                      scale_factor, shift, window, blob, g_out, g_sdf_grad, g_geom, sp);
+    k_rgb_input_tiles<<<ntiles * kRgbGroups, kInputTileThreads, 0, ST>>>(P, pos, dirs, sdf_grad, geom, reinterpret_cast<const float2*>(lattice),
+                                                                         scale_factor, shift, window, a0);
     PSDF_CHECK_LAUNCH();
     if (timing) cudaEventRecord(ev[1], ST);
-    int max_nk = 0;
-    for (int l = 0; l < kNL; l++) max_nk = max(max_nk, P.g.N[l] * P.g.K[l]);
-    k_rgb_dw_reduce<<<dim3(div_up(max_nk, kDwReduceThreads), kNL, kDwReduceChunks), kDwReduceThreads, 0, ST>>>(P.g, ctas, sp);
+    k_rgb_fused_backward<<<ctas, kRgbThreads, smem, ST>>>(P, sdf_grad, blob, g_out, g_sdf_grad, g_geom, sp);
     PSDF_CHECK_LAUNCH();
     if (timing) cudaEventRecord(ev[2], ST);
+    DwSums ds;
+    for (int l = 0; l < kNL; l++) ds.gW[l] = w[l];
+    ds.fx_mlp = sp.fx_mlp;
+    ds.fx_w = kFxW;
+    int max_nk = 0;
+    for (int l = 0; l < kNL; l++) max_nk = max(max_nk, P.g.N[l] * P.g.K[l]);
+    k_dw_reduce<128, unsigned long long, RgbDwSlab><<<dim3(div_up(max_nk, kDwReduceThreads), kNL, kDwReduceChunks), kDwReduceThreads, 0, ST>>>(
+        P.g, ctas, ds);
+    PSDF_CHECK_LAUNCH();
+    if (timing) cudaEventRecord(ev[3], ST);
     k_lattice_scatter<3><<<dim3(div_up(sp.xch_stride, kScatterThreads), L), kScatterThreads, 0, ST>>>(
         N, T, P.cap_mask, pos, sp.xch, sp.xch_stride, scale_factor, shift, window, grad_lattice, dbuf ? dbuf->rgb_lattice : nullptr);
     PSDF_CHECK_LAUNCH();
-    if (timing) cudaEventRecord(ev[3], ST);
+    if (timing) cudaEventRecord(ev[4], ST);
     if (dbuf) {      // deterministic mode: fixed-point totals -> the float gradients (+=)
         FxSegs F;
         F.add(dbuf->rgb_lattice, grad_lattice, (long long)L * T * 2);
@@ -450,13 +451,12 @@ static int rgb_backward_impl(int N, int L, int T, const float* pos, const float*
         cudaMemcpyAsync(h, d_cycles, sizeof(h), cudaMemcpyDeviceToHost, ST);
         cudaStreamSynchronize(ST);
         const double t = h[kPhTiles] ? (double)h[kPhTiles] : 1.0;
-        float ms_fused = 0.f, ms_reduce = 0.f, ms_scatter = 0.f;
-        cudaEventElapsedTime(&ms_fused, ev[0], ev[1]);
-        cudaEventElapsedTime(&ms_reduce, ev[1], ev[2]);
-        cudaEventElapsedTime(&ms_scatter, ev[2], ev[3]);
-        fprintf(stderr, "[psdf_rgb_fused_backward N=%d tiles=%llu] cycles/tile: encoder %.0f forward %.0f %.0f %.0f seed %.0f rev3 %.0f rev2 %.0f rev1 %.0f "
-                        "rev0 %.0f tail %.0f | flush/CTA %.0f | fused kernel %.3f ms, weight-gradient reduction %.3f ms, lattice scatter %.3f ms\n", N, h[kPhTiles], h[0] / t, h[1] / t, h[2] / t, h[3] / t,
-                h[4] / t, h[5] / t, h[6] / t, h[7] / t, h[8] / t, h[9] / t, (double)h[kPhFlush] / ctas, ms_fused, ms_reduce, ms_scatter);
+        float ms[4] = {0.f, 0.f, 0.f, 0.f};
+        for (int i = 0; i < 4; i++) cudaEventElapsedTime(&ms[i], ev[i], ev[i + 1]);
+        fprintf(stderr, "[psdf_rgb_fused_backward N=%d tiles=%llu] cycles/tile: tile load wait %.0f forward %.0f %.0f %.0f seed %.0f rev3 %.0f rev2 %.0f rev1 %.0f "
+                        "rev0 %.0f tail %.0f | flush/CTA %.0f | input tiles %.3f ms, fused kernel %.3f ms, weight-gradient reduction %.3f ms, "
+                        "lattice scatter %.3f ms\n", N, h[kPhTiles], h[0] / t, h[1] / t, h[2] / t, h[3] / t, h[4] / t, h[5] / t, h[6] / t,
+                h[7] / t, h[8] / t, h[9] / t, (double)h[kPhFlush] / ctas, ms[0], ms[1], ms[2], ms[3]);
     }
     return PSDF_OK;
 }

@@ -1,8 +1,9 @@
 // Training backward of the fused encoding + SDF MLP (sm_90a, wgmma): given d loss / d {sdf, d sdf/dx, geom}
-// per sample it produces the lattice gradient, the bias gradients and the weight gradients. Two kernels: the persistent
-// tensor-core kernel forms the weight-gradient products from the operand tiles while they are still in shared memory
-// (summed over all tiles of the CTA) and hands abar_0 | tabar_0 to a full-occupancy kernel that scatters them into the lattice
-// gradient.
+// per sample it produces the lattice gradient, the bias gradients and the weight gradients. Four kernels: a kernel with many warps per SM
+// builds the layer-0 operand tiles a_0 | ta_0 of every tile (k_sdf_input_tiles); the persistent tensor-core kernel loads them by TMA,
+// forms the weight-gradient products from the operand tiles while they are still in shared memory (summed over all tiles of the CTA,
+// left in a slab per CTA that k_dw_reduce adds up) and hands abar_0 | tabar_0 to a full-occupancy kernel that scatters them into the
+// lattice gradient.
 //
 // What it replaces in the reference: `loss.backward()` through SDF.get_sdf_and_gradient
 // (permuto_sdf_py/models/models.py:199-259, create_graph=True) -- i.e. the double backward of the
@@ -20,11 +21,12 @@
 //     dW_l = zbar_{l+1} a_l^T + tzbar_{l+1} ta_l^T,   db_l = sum zbar_{l+1}
 //     lattice[lvl][idx_r] += window_lvl (B_r abar_0[lvl] + dB_r tabar_0[lvl])       (B barycentric weights, dB their tangent)
 //
-// Per 128-sample tile (512 threads: row = tid & 127, group g = tid >> 7 owns operand cores g, g+4, .. in the encoder and seed
-// phases). Every product lands in the registers of the warpgroup that issues it: warpgroup (mh, nh) = (wgi & 1, wgi >> 1) forms rows
+// Per 128-sample tile (512 threads: row = tid & 127, group g = tid >> 7 owns operand cores g, g+4, .. in the seed phase). Every
+// product lands in the registers of the warpgroup that issues it: warpgroup (mh, nh) = (wgi & 1, wgi >> 1) forms rows
 // 64 mh .. 64 mh + 63 x column half nh (split_n) of both streams, the value and the tangent of one (row, column) in the same thread, and
 // consumes them in place. Two 64 KB operand-tile buffers X, Y ([value hi | value lo | tangent hi | tangent lo]):
-//   1. encoder: a_0, ta_0 -> X; X leaves by ONE TMA store (64 KB / tile, re-read from L2 in step 4)
+//   1. tile load: a_0 | ta_0 -> X by ONE TMA load (64 KB / tile, written by k_sdf_input_tiles and re-read from L2 in step 4). The next
+//      tile's load is issued as soon as the step-0 products have read X, so it lands behind the exchange stores and the loop turnaround
 //   2. forward recompute, layers 0..2: a_1 -> Y, a_2 -> X, a_3 -> Y straight from the fragments; the raw z_1, z_2 (value + tangent)
 //      go to this thread's slots of the CTA's stash (global, L2 resident) and come back to the same thread in the reverse sweep: the
 //      reverse step l splits its Kp_l = Np_{l-1} columns exactly as the forward layer l-1 split them, so it needs no barrier.
@@ -42,14 +44,17 @@
 //      and a_{l-1} | ta_{l-1} are rebuilt into Y from the stashed z_{l-1} (l = 3, 2) or come back by TMA (l = 1).
 //      In the last step (l = 0) abar_0 | tabar_0 leave from the registers to the exchange region of the workspace, one float4
 //      (a0, a1, t0, t1) per level and sample, [level][sample slot]: a thread's column pair is one level.
+// The encoder forward is its own launch, k_sdf_input_tiles: inside the persistent kernel its dependent lattice gathers ran on 16 warps
+// per SM with the tensor cores idle; on its own it runs with 40 (D = 3) or 32 (D = 4) warps per SM.
 // The encoder backward is its own launch, k_sdf_lattice_scatter: warp-aggregated red.global.add.v2.f32 into the lattice gradient.
 // Inside the persistent kernel it was the longest phase of a tile (one CTA of 16 warps per SM, tensor cores idle, long dependent chains
 // of simplex recompute, match_any, shuffle sums and reductions); on its own it runs with every warp slot of the SM occupied. Its warps
 // are the rows of the persistent kernel's warps, so the match_any groups and the float peer sums are the same.
 // Deterministic mode (common.cuh): every gradient (lattice, weights, biases) is summed in fixed point instead and added to the float
-// gradients by the flush that follows the two launches.
+// gradients by the flush that follows the launches.
 // Stash of a CTA (float4 slots, slot index * 512 + tid): [0,16) z_1 | tz_1, z_2 | tz_2 fragments (8 slots per layer), [16,24) dW_0..dW_3
-// (2 slots per layer).
+// (2 slots per layer). At the end of the kernel the dW sums go to the CTA's slab of g_dw_sdf_bwd: fx_of of the fp32 sum in
+// deterministic mode (the value the per-CTA atomics added), the fp32 sum otherwise.
 #include <cstdio>
 #include <cstdlib>
 #include <type_traits>
@@ -65,12 +70,16 @@ constexpr int kSetBytes = 4 * kATileBytes;         // one operand tile set [valu
 constexpr int kStashDw = 16, kStashSlots = 24;      // stash map (float4 slots per thread), see the header
 __device__ float4 g_stash_bwd[(size_t)kAccCtas * kStashSlots * kBwdThreads];     // per-CTA stashes, 192 KB each
 constexpr int kFxW = kDetSdfW, kFxB = 4 * kDetSdfW;    // weight / bias offsets in DetBufs::sdf_mlp
+// weight-gradient sums of each CTA, [CTA][layer][64 rows][64 columns] (k_dw_reduce): fixed point (fx_of) in deterministic mode, else
+// float (the same slot indices in the float view)
+constexpr int kDwLd = 64, kDwSlots = kNL * kDwLd * kDwLd;
+__device__ unsigned long long g_dw_sdf_bwd[(size_t)kAccCtas * kDwSlots];
+struct SdfDwSlab { static __device__ const void* get() { return g_dw_sdf_bwd; } };
 
 struct BwdOut {
-    uint8_t* a0_spill;  // [ntiles][64 KB] encoder operand tiles, written and re-read by the same CTA
+    const uint8_t* a0_spill;  // [ntiles][64 KB] layer-0 operand tiles a_0 | ta_0 (k_sdf_input_tiles)
     float4* xch;        // [L][xch_stride] abar_0 | tabar_0 (a0, a1, t0, t1) per level and sample slot (tile * 128 + row)
     int xch_stride;     // sample slots = ntiles * 128
-    float* gW[kNL];     // [N_l, K_l] (+=)
     float* gbias[kNL];  // [N_l]      (+=)
     unsigned long long* fx_mlp;       // deterministic mode: fixed-point accumulators (DetBufs::sdf_mlp), else NULL
     unsigned long long* phase_cycles;   // [16] += clock64 deltas of thread 0 per phase (PSDF_PHASE_TIMING=1, diagnostics), else NULL
@@ -88,7 +97,7 @@ struct Segments {
     const float* g_geom[kMaxSeg];
 };
 // phase ids of the diagnostic counters
-enum { kPhEncoder = 0, kPhForward = 1, kPhSeed = 2, kPhReverse3 = 3, kPhReverse2 = 4, kPhReverse1 = 5, kPhReverse0 = 6, kPhFlush = 7,
+enum { kPhTileLoad = 0, kPhForward = 1, kPhSeed = 2, kPhReverse3 = 3, kPhReverse2 = 4, kPhReverse1 = 5, kPhReverse0 = 6, kPhFlush = 7,
        kPhTiles = 8 };
 #define PSDF_PHASE(id)                                                                     \
     do {                                                                                   \
@@ -125,21 +134,76 @@ __device__ __forceinline__ void issue_dw16(float* d, const uint8_t* zset, const 
     }
 }
 
+// Layer-0 operand tiles a_0 | ta_0 of every tile of the launch -> a0_spill ([tile][64 KB], the bytes of X in the persistent kernel):
+// the window-weighted features of each level and their directional tangent along v (the barycentric weights' tangent dB_r applied to
+// the same vertex values), then the concatenated points. Thread (tile, operand core kc, row): a warp is 32 consecutive rows of one
+// core (4 levels = 8 features = one 16-byte core row), as in the persistent kernel's encoder phase that this replaces, so its gathers
+// are the same. Invalid rows (past the end of their sample set) are built from x = v = 0. Cores past Kp[0] are not written.
 // D = 3: positions [N,3]; D = 4: space-time positions [N,4] with the tangent along (g_grad, 0) (g_grad holds spatial derivatives)
+constexpr int kInputTileThreads = 256;
+template <int D>
+__global__ void __launch_bounds__(kInputTileThreads)
+k_sdf_input_tiles(FusedParams P, Segments S, const float2* __restrict__ lattice, const float* __restrict__ scale,
+                  const float* __restrict__ shift, const float* __restrict__ window, uint8_t* __restrict__ a0_spill) {
+    __shared__ LevelC lc;
+    load_level_consts<D>(&lc, P.L, scale, shift, window, threadIdx.x, kInputTileThreads);
+    __syncthreads();
+    const int cores = P.g.Kp[0] / 8, level_cores = P.L / 4;
+    const int u = blockIdx.x * kInputTileThreads + threadIdx.x;          // (tile * cores + kc) * 128 + row
+    const int row = u % kTile, kc = (u / kTile) % cores, tile = u / (kTile * cores);
+    if (tile >= S.tile0[kMaxSeg]) return;
+    const int seg = tile >= S.tile0[2] ? 2 : (tile >= S.tile0[1] ? 1 : 0);
+#define PSDF_SEG(f) (seg == 2 ? S.f[2] : (seg == 1 ? S.f[1] : S.f[0]))     // no dynamic indexing of the parameter struct (local-memory copy)
+    const int n = (tile - PSDF_SEG(tile0)) * kTile + row;              // row inside its sample set
+    const bool valid = n < PSDF_SEG(n);
+    const float* __restrict__ pos = PSDF_SEG(pos);
+    const float* __restrict__ g_grad = PSDF_SEG(g_grad);
+#undef PSDF_SEG
+    float x[D], v[3];
+#pragma unroll
+    for (int i = 0; i < D; i++) {
+        x[i] = valid ? pos[(size_t)n * D + i] : 0.0f;
+        if (i < 3) v[i] = (valid && g_grad) ? g_grad[(size_t)n * 3 + i] : 0.0f;
+    }
+    float fv[8], ft[1][8];
+    if (kc < level_cores) {
+#pragma unroll
+        for (int q = 0; q < 4; q++) {
+            const int l = kc * 4 + q;
+            float dcf[D], db[D + 2];
+#pragma unroll
+            for (int i = 0; i < D; i++) dcf[i] = i < 3 ? v[i] * lc.scale[l * 4 + i] : 0.0f;
+            Simplex<D> s;
+            float2 val[D + 1];
+            const float2 a = level_features<D>(x, &lc, l, lattice, P.T, P.cap_mask, s, val);
+            bary_tangent<D>(dcf, s, db);
+            const float w = lc.window[l];
+            float t0 = 0.f, t1 = 0.f;
+#pragma unroll
+            for (int r = 0; r <= D; r++) { const float cr = db[r] * w; t0 = fmaf(val[r].x, cr, t0); t1 = fmaf(val[r].y, cr, t1); }
+            fv[2 * q] = a.x; fv[2 * q + 1] = a.y; ft[0][2 * q] = t0; ft[0][2 * q + 1] = t1;
+        }
+    } else {
+        concat_core<1, D>(P, kc, x, &v, fv, ft);
+    }
+    uint8_t* t = a0_spill + (size_t)tile * kSetBytes;
+    store8(t, t + kATileBytes, row, kc, fv);
+    store8(t + 2 * kATileBytes, t + 3 * kATileBytes, row, kc, ft[0]);
+}
+
+// The same code at D = 3 and 4 (the input width only matters to k_sdf_input_tiles and the scatter); one instantiation per width
 template <int D>
 __global__ void __launch_bounds__(kBwdThreads, 1)
-k_sdf_fused_backward(FusedParams P, Segments S, const float2* __restrict__ lattice, const float* __restrict__ scale,
-                     const float* __restrict__ shift, const float* __restrict__ window, const uint8_t* __restrict__ blob, BwdOut out) {
+k_sdf_fused_backward(FusedParams P, Segments S, const uint8_t* __restrict__ blob, BwdOut out) {
     extern __shared__ __align__(128) uint8_t smem[];
     uint8_t* s_w = smem;                                   // forward operand blob (weights hi/lo + biases), resident
     uint8_t* s_X = smem + P.g.total;
     uint8_t* s_Y = s_X + kSetBytes;
-    LevelC* lc = reinterpret_cast<LevelC*>(s_Y + kSetBytes);
     // 4 x 64 bias-gradient accumulators of this CTA: float (s_gbf), or fixed point (s_gb) in deterministic mode
-    unsigned long long* s_gb = reinterpret_cast<unsigned long long*>(lc + 1);
+    unsigned long long* s_gb = reinterpret_cast<unsigned long long*>(s_Y + kSetBytes);
     float* s_gbf = reinterpret_cast<float*>(s_gb);
     const bool det = out.fx_mlp != nullptr;
-    uint64_t* bars = reinterpret_cast<uint64_t*>(s_gb + kNL * 64);   // [0] TMA loads
+    uint64_t* bars = reinterpret_cast<uint64_t*>(s_gb + kNL * 64);   // [0] weights, a_0 | ta_0 reload into Y; [1] tile loads into X
     float* s_seed = reinterpret_cast<float*>(bars + 5);   // [128][(out_dim - 1) | 1] upstream d loss / d geom of the tile (coalesced copy)
     // the same bytes in the reverse sweep (s_seed is dead from the seed phase to the next tile): [8 warp pairs][16][32 lanes] the odd
     // warp's zbar fragments for the bias column sums
@@ -147,27 +211,27 @@ k_sdf_fused_backward(FusedParams P, Segments S, const float2* __restrict__ latti
 
     const int tid = threadIdx.x, warp = warp_uniform(tid >> 5), lane = tid & 31;
     const int row = tid & 127, grp = tid >> 7;
-    const int level_cores = P.L / 4;
-    const int K0 = P.g.Kp[0];
     const int wgi = warp >> 2, mh = wgi & 1, nh = wgi >> 1;
     float4* stash = g_stash_bwd + (size_t)blockIdx.x * kStashSlots * kBwdThreads + tid;     // this thread's slot 0
 
     if (tid == 0) {
         umma::mbar_init(&bars[0], 1);
+        umma::mbar_init(&bars[1], 1);
         umma::mbar_fence_init();
     }
-    load_level_consts<D>(lc, P.L, scale, shift, window, tid, kBwdThreads);
     for (int i = tid; i < kNL * 64; i += kBwdThreads) s_gb[i] = 0ull;     // also clears s_gbf
     __syncthreads();
-    if (tid == 0) {
+    const int ntiles = S.tile0[kMaxSeg];
+    if (tid == 0) {          // the weights and the first tile (the grid has no more CTAs than tiles)
         umma::mbar_expect_tx(&bars[0], (uint32_t)P.g.total);
         umma::bulk_g2s(s_w, blob, (uint32_t)P.g.total, &bars[0]);
+        umma::mbar_expect_tx(&bars[1], (uint32_t)kSetBytes);
+        umma::bulk_g2s(s_X, out.a0_spill + (size_t)blockIdx.x * kSetBytes, (uint32_t)kSetBytes, &bars[1]);
     }
     __syncthreads();
     umma::mbar_wait(&bars[0], 0);
-    uint32_t ld_phase = 1;
+    uint32_t ld_phase = 1;      // parity of bars[0]'s a_0 | ta_0 reload; bars[1] (one tile load per tile) runs at ld_phase ^ 1
 
-    const int ntiles = S.tile0[kMaxSeg];
     bool first_tile = true;
     long long phase_t0 = out.phase_cycles ? clock64() : 0;
     for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, first_tile = false) {
@@ -176,17 +240,9 @@ k_sdf_fused_backward(FusedParams P, Segments S, const float2* __restrict__ latti
         const int seg_tile0 = PSDF_SEG(tile0), seg_n = PSDF_SEG(n);
         const int n = (tile - seg_tile0) * kTile + row;              // row inside its sample set
         const bool valid = n < seg_n;
-        const float* __restrict__ pos = PSDF_SEG(pos);
         const float* __restrict__ g_sdf = PSDF_SEG(g_sdf);
-        const float* __restrict__ g_grad = PSDF_SEG(g_grad);
         const float* __restrict__ g_geom = PSDF_SEG(g_geom);
 #undef PSDF_SEG
-        float x[D], v[3];
-#pragma unroll
-        for (int i = 0; i < D; i++) {
-            x[i] = valid ? pos[(size_t)n * D + i] : 0.0f;
-            if (i < 3) v[i] = (valid && g_grad) ? g_grad[(size_t)n * 3 + i] : 0.0f;
-        }
         if (g_geom) {
             // the tile's rows of the upstream geometric-feature gradient are contiguous: copy them with coalesced loads now (consumed by
             // the seed phase, several barriers later) instead of 16 scalar loads per thread 128 bytes apart (5 % of the stall samples)
@@ -196,35 +252,9 @@ k_sdf_fused_backward(FusedParams P, Segments S, const float2* __restrict__ latti
             const float* __restrict__ src = g_geom + (size_t)row0 * gw;
             for (int i = tid; i < cnt; i += kBwdThreads) s_seed[(i / gw) * (gw | 1) + (i % gw)] = src[i];
         }
-        // ---------------- 1. encoder -> X: operand cores grp, grp+4, ... (4 levels = 8 features = one 16-byte core row)
-        for (int kc = grp; kc < K0 / 8; kc += kGroups) {
-            float fv[8], ft[1][8];
-            if (kc < level_cores) {
-#pragma unroll
-                for (int q = 0; q < 4; q++) {
-                    const int l = kc * 4 + q;
-                    // directional tangent along v: the barycentric weights' tangent dB_r applied to the same vertex values
-                    float dcf[D], db[D + 2];
-#pragma unroll
-                    for (int i = 0; i < D; i++) dcf[i] = i < 3 ? v[i] * lc->scale[l * 4 + i] : 0.0f;
-                    Simplex<D> s;
-                    float2 val[D + 1];
-                    const float2 a = level_features<D>(x, lc, l, lattice, P.T, P.cap_mask, s, val);
-                    bary_tangent<D>(dcf, s, db);
-                    const float w = lc->window[l];
-                    float t0 = 0.f, t1 = 0.f;
-#pragma unroll
-                    for (int r = 0; r <= D; r++) { const float cr = db[r] * w; t0 = fmaf(val[r].x, cr, t0); t1 = fmaf(val[r].y, cr, t1); }
-                    fv[2 * q] = a.x; fv[2 * q + 1] = a.y; ft[0][2 * q] = t0; ft[0][2 * q + 1] = t1;
-                }
-            } else {
-                concat_core<1, D>(P, kc, x, &v, fv, ft);
-            }
-            store8(s_X, s_X + kATileBytes, row, kc, fv);
-            store8(s_X + 2 * kATileBytes, s_X + 3 * kATileBytes, row, kc, ft[0]);
-        }
-
-        PSDF_PHASE(kPhEncoder);
+        // ---------------- 1. a_0 | ta_0 of this tile -> X (TMA load issued next to the weight load or after the previous tile's step 0)
+        umma::mbar_wait(&bars[1], ld_phase ^ 1);
+        PSDF_PHASE(kPhTileLoad);
         // ---------------- 2. forward recompute, layers 0..2. Warpgroup (mh, nh) forms rows 64 mh .. 64 mh + 63 x column half nh of both
         // streams in its registers and consumes them in place: a_{l+1} | ta_{l+1} -> the next operand set, and the raw z_{l+1} | tz_{l+1}
         // -> this thread's stash slots (l = 0, 1) or the GELU' / GELU'' factors of the first reverse step (l = 2)
@@ -232,15 +262,10 @@ k_sdf_fused_backward(FusedParams P, Segments S, const float2* __restrict__ latti
         float seed[2][8];                      // upstream gradient columns of this thread (prefetched before the layer-2 MMAs)
 #pragma unroll 1
         for (int l = 0; l < 3; l++) {
-            if (l == 1 && tid == 0) umma::bulk_wait_read0();   // X is overwritten by this layer's epilogue: the store must have read it
             umma::fence_async_smem();
             __syncthreads();
             const uint8_t* at = (l == 1) ? s_Y : s_X;
             uint8_t* dst = (l == 1) ? s_X : s_Y;
-            if (l == 0 && tid == 0) {          // a_0 | ta_0 leave as they are (needed again for dW_0 at the end of the reverse sweep)
-                umma::bulk_s2g(out.a0_spill + (size_t)tile * kSetBytes, s_X, kSetBytes);
-                umma::bulk_commit();
-            }
             if (l == 2) {                      // zbar_4 = [g_sdf, g_geom...] columns of this thread, loaded while the MMAs run
                 const int Np = P.g.Np[3], nout = P.g.N[3];
 #pragma unroll
@@ -364,10 +389,13 @@ k_sdf_fused_backward(FusedParams P, Segments S, const float2* __restrict__ latti
                 for (int q = 0; q < 2; q++) dws[q * kBwdThreads] = make_float4(dwa[4 * q], dwa[4 * q + 1], dwa[4 * q + 2], dwa[4 * q + 3]);
             }
             __syncthreads();                                   // every product of this step has read X and Y
-            if (l == 1 && tid == 0) {          // Y is free: bring a_0 | ta_0 back for the last step (the store completed long ago)
-                umma::bulk_wait0();
+            if (l == 1 && tid == 0) {          // Y is free: bring a_0 | ta_0 back for the last step
                 umma::mbar_expect_tx(&bars[0], (uint32_t)kSetBytes);
                 umma::bulk_g2s(s_Y, out.a0_spill + (size_t)tile * kSetBytes, (uint32_t)kSetBytes, &bars[0]);
+            }
+            if (l == 0 && tid == 0 && tile + (int)gridDim.x < ntiles) {     // X is free: the next tile's a_0 | ta_0
+                umma::mbar_expect_tx(&bars[1], (uint32_t)kSetBytes);
+                umma::bulk_g2s(s_X, out.a0_spill + (size_t)(tile + gridDim.x) * kSetBytes, (uint32_t)kSetBytes, &bars[1]);
             }
             if (l > 0) {
                 if (nn > 0) {
@@ -454,18 +482,19 @@ k_sdf_fused_backward(FusedParams P, Segments S, const float2* __restrict__ latti
             PSDF_PHASE(kPhReverse3 + (3 - l));
         }
         ld_phase ^= 1;
-        // no barrier before the next tile: X and Y were last read by this tile's step-0 products, complete before its second barrier;
-        // s_bx (= s_seed) was last read in step 1, before the step-0 barriers
+        // no barrier before the next tile: X and Y were last read by this tile's step-0 products, complete before its second barrier
+        // (the next tile's X arrives by TMA, behind the mbarrier); s_bx (= s_seed) was last read in step 1, before the step-0 barriers
         if (out.phase_cycles && tid == 0) atomicAdd(out.phase_cycles + kPhTiles, 1ull);
     }
-    // ---------------- weight gradients of this CTA: this thread's stashed dW fragments -> global (+=). Element 4 j + 2 h + b of dW_l is
-    // row 16 (warp & 3) + lane / 4 + 8 h, column 16 wgi + 8 j + 2 (lane % 4) + b
+    // ---------------- weight gradients of this CTA: this thread's stashed dW fragments -> the CTA's slab (plain stores; k_dw_reduce adds
+    // up the CTAs' slabs). Element 4 j + 2 h + b of dW_l is row 16 (warp & 3) + lane / 4 + 8 h, column 16 wgi + 8 j + 2 (lane % 4) + b; the
+    // thread's columns past K_l (up to Kp_l) are written too and never read
     if (!first_tile) {
+        unsigned long long* dw = g_dw_sdf_bwd + (size_t)blockIdx.x * kDwSlots;          // deterministic mode
+        float* dwf = reinterpret_cast<float*>(g_dw_sdf_bwd) + (size_t)blockIdx.x * kDwSlots;   // float mode
 #pragma unroll 1
         for (int l = 0; l < kNL; l++) {
             if (16 * wgi >= P.g.Kp[l]) continue;
-            const int K = P.g.K[l];
-            const bool vec = (K & 1) == 0 && ((uintptr_t)out.gW[l] & 7) == 0;      // column pairs stay 8-byte aligned
 #pragma unroll
             for (int j = 0; j < 2; j++) {
                 const float4 v = stash[(kStashDw + 2 * l + j) * kBwdThreads];
@@ -473,19 +502,9 @@ k_sdf_fused_backward(FusedParams P, Segments S, const float2* __restrict__ latti
                 for (int h = 0; h < 2; h++) {
                     const int m = 16 * (warp & 3) + lane / 4 + 8 * h, k = 16 * wgi + 8 * j + 2 * (lane & 3);
                     const float v0 = h ? v.z : v.x, v1 = h ? v.w : v.y;
-                    if (m >= P.g.N[l]) continue;
-                    if (det) {
-                        unsigned long long* dst = out.fx_mlp + l * kFxW + m * K + k;
-                        if (k < K) fx_add(dst, v0);
-                        if (k + 1 < K) fx_add(dst + 1, v1);
-                    } else {
-                        float* dst = out.gW[l] + (size_t)m * K + k;
-                        if (vec && k + 1 < K) red_v2(dst, make_float2(v0, v1));
-                        else {
-                            if (k < K) atomicAdd(dst, v0);
-                            if (k + 1 < K) atomicAdd(dst + 1, v1);
-                        }
-                    }
+                    const int slot = l * kDwLd * kDwLd + m * kDwLd + k;
+                    if (det) *reinterpret_cast<ulonglong2*>(dw + slot) = make_ulonglong2(fx_of(v0), fx_of(v1));
+                    else *reinterpret_cast<float2*>(dwf + slot) = make_float2(v0, v1);
                 }
             }
         }
@@ -496,7 +515,6 @@ k_sdf_fused_backward(FusedParams P, Segments S, const float2* __restrict__ latti
         else if (c < P.g.N[l] && s_gbf[i] != 0.0f) atomicAdd(out.gbias[l] + c, s_gbf[i]);
     }
     PSDF_PHASE(kPhFlush);
-    if (tid == 0) umma::bulk_wait0();      // spill stores complete before the CTA retires
 }
 
 // Encoder backward: lattice[l][idx_r] += window_l (B_r abar_0[l] + dB_r tabar_0[l]) from the exchange rows of k_sdf_fused_backward.
@@ -535,8 +553,8 @@ k_sdf_lattice_scatter(FusedParams P, Segments S, const float4* __restrict__ xch,
                   grad_lattice + (size_t)l * P.T * 2, fx_lattice ? fx_lattice + (size_t)l * P.T * 2 : nullptr);
 }
 
-// workspace per 128-sample tile: the encoder operand tiles (a_0 | ta_0, 64 KB), written by TMA store in the forward recompute and read
-// back by the same CTA for the first layer's weight gradient, and the exchange rows abar_0 | tabar_0 (16 bytes per sample and level,
+// workspace per 128-sample tile: the layer-0 operand tiles (a_0 | ta_0, 64 KB), written by k_sdf_input_tiles and read by TMA into the
+// persistent kernel twice (forward recompute and the first layer's weight gradient), and the exchange rows abar_0 | tabar_0 (16 bytes per sample and level,
 // sized for kMaxLevels so that the size depends on the sample count alone)
 constexpr long long kWsTileBytes = kSetBytes + (long long)kTile * kMaxLevels * sizeof(float4);
 
@@ -584,15 +602,16 @@ static int launch_backward(int nseg, const int* Ns, const float* const* pos, con
     const DetBufs* dbuf = det_buffers();
     if (dbuf && (long long)L * T * 2 > dbuf->lattice_len) return PSDF_ERR_UNSUPPORTED;   // reserve more with psdf_set_deterministic
     BwdOut out;
-    for (int l = 0; l < kNL; l++) { out.gW[l] = gW[l]; out.gbias[l] = gb[l]; }
+    for (int l = 0; l < kNL; l++) out.gbias[l] = gb[l];
     out.fx_mlp = dbuf ? dbuf->sdf_mlp : nullptr;
-    out.a0_spill = workspace;
+    uint8_t* a0_spill = workspace;
+    out.a0_spill = a0_spill;
     out.xch = reinterpret_cast<float4*>(workspace + (size_t)tiles * kSetBytes);
     out.xch_stride = tiles * kTile;
     // diagnostics: PSDF_PHASE_TIMING=1 prints thread 0's clock64 breakdown per phase (average cycles per tile) after every launch
     static const bool timing = getenv("PSDF_PHASE_TIMING") && atoi(getenv("PSDF_PHASE_TIMING")) != 0;
     static unsigned long long* d_cycles = nullptr;
-    static cudaEvent_t ev[3];
+    static cudaEvent_t ev[5];
     out.phase_cycles = nullptr;
     if (timing) {
         if (!d_cycles) {
@@ -609,17 +628,35 @@ static int launch_backward(int nseg, const int* Ns, const float* const* pos, con
     // the last region holds the upstream geometric-feature rows of a tile or, in the reverse sweep, the 8 x 16 x 32 fragments exchanged
     // for the bias column sums
     const size_t seed_bytes = std::max((size_t)kTile * (size_t)((out_dim - 1) | 1) * sizeof(float), (size_t)(8 * 16 * 32 * sizeof(float)));
-    const size_t smem = (size_t)P.g.total + 2 * kSetBytes + sizeof(LevelC) + kNL * 64 * sizeof(unsigned long long) + 64 + seed_bytes;
+    const size_t smem = (size_t)P.g.total + 2 * kSetBytes + kNL * 64 * sizeof(unsigned long long) + 64 + seed_bytes;
     if (smem > 227 * 1024) return PSDF_ERR_UNSUPPORTED;
-    { static bool optin_[64]; psdf::psdf_optin_smem(k_sdf_fused_backward<D>, 227 * 1024, optin_); }
-    k_sdf_fused_backward<D><<<min(min(tiles, sms), kAccCtas), kBwdThreads, smem, ST>>>(P, S, reinterpret_cast<const float2*>(lattice), scale_factor, shift, window,
-                                                                    blob, out);
+    const long long tile_threads = (long long)tiles * (P.g.Kp[0] / 8) * kTile;
+    k_sdf_input_tiles<D><<<(unsigned)div_up(tile_threads, (long long)kInputTileThreads), kInputTileThreads, 0, ST>>>(
+        P, S, reinterpret_cast<const float2*>(lattice), scale_factor, shift, window, a0_spill);
     PSDF_CHECK_LAUNCH();
     if (timing) cudaEventRecord(ev[1], ST);
+    { static bool optin_[64]; psdf::psdf_optin_smem(k_sdf_fused_backward<D>, 227 * 1024, optin_); }
+    const int ctas = min(min(tiles, sms), kAccCtas);
+    k_sdf_fused_backward<D><<<ctas, kBwdThreads, smem, ST>>>(P, S, blob, out);
+    PSDF_CHECK_LAUNCH();
+    if (timing) cudaEventRecord(ev[2], ST);
+    {
+        DwSums ds;
+        for (int l = 0; l < kNL; l++) ds.gW[l] = gW[l];
+        ds.fx_mlp = out.fx_mlp;
+        ds.fx_w = kFxW;
+        int max_nk = 0;
+        for (int l = 0; l < kNL; l++) max_nk = max(max_nk, P.g.N[l] * P.g.K[l]);
+        const dim3 grid(div_up(max_nk, kDwReduceThreads), kNL, kDwReduceChunks);
+        if (dbuf) k_dw_reduce<kDwLd, unsigned long long, SdfDwSlab><<<grid, kDwReduceThreads, 0, ST>>>(P.g, ctas, ds);
+        else k_dw_reduce<kDwLd, float, SdfDwSlab><<<grid, kDwReduceThreads, 0, ST>>>(P.g, ctas, ds);
+        PSDF_CHECK_LAUNCH();
+    }
+    if (timing) cudaEventRecord(ev[3], ST);
     k_sdf_lattice_scatter<D><<<dim3(div_up(out.xch_stride, kScatterThreads), L), kScatterThreads, 0, ST>>>(
         P, S, out.xch, out.xch_stride, scale_factor, shift, window, grad_lattice, dbuf ? dbuf->sdf_lattice : nullptr);
     PSDF_CHECK_LAUNCH();
-    if (timing) cudaEventRecord(ev[2], ST);
+    if (timing) cudaEventRecord(ev[4], ST);
     if (dbuf) {      // deterministic mode: fixed-point totals -> the float gradients (+=)
         FxSegs F;
         F.add(dbuf->sdf_lattice, grad_lattice, (long long)L * T * 2);
@@ -634,12 +671,12 @@ static int launch_backward(int nseg, const int* Ns, const float* const* pos, con
         cudaMemcpyAsync(h, d_cycles, sizeof(h), cudaMemcpyDeviceToHost, ST);
         cudaStreamSynchronize(ST);
         const double t = h[kPhTiles] ? (double)h[kPhTiles] : 1.0;
-        float ms_fused = 0.f, ms_scatter = 0.f;
-        cudaEventElapsedTime(&ms_fused, ev[0], ev[1]);
-        cudaEventElapsedTime(&ms_scatter, ev[1], ev[2]);
-        fprintf(stderr, "[psdf_sdf_fused_backward N=%d tiles=%llu] cycles/tile: encoder %.0f forward %.0f seed %.0f rev3 %.0f rev2 %.0f rev1 %.0f rev0 %.0f "
-                        "| flush/CTA %.0f | fused kernel %.3f ms, lattice scatter %.3f ms\n", total, h[kPhTiles], h[0] / t, h[1] / t, h[2] / t, h[3] / t,
-                h[4] / t, h[5] / t, h[6] / t, (double)h[kPhFlush] / min(tiles, sms), ms_fused, ms_scatter);
+        float ms[4] = {0.f, 0.f, 0.f, 0.f};
+        for (int i = 0; i < 4; i++) cudaEventElapsedTime(&ms[i], ev[i], ev[i + 1]);
+        fprintf(stderr, "[psdf_sdf_fused_backward N=%d tiles=%llu] cycles/tile: tile load wait %.0f forward %.0f seed %.0f rev3 %.0f rev2 %.0f rev1 %.0f "
+                        "rev0 %.0f | flush/CTA %.0f | input tiles %.3f ms, fused kernel %.3f ms, weight-gradient reduction %.3f ms, lattice "
+                        "scatter %.3f ms\n", total, h[kPhTiles], h[0] / t, h[1] / t, h[2] / t, h[3] / t, h[4] / t, h[5] / t, h[6] / t,
+                (double)h[kPhFlush] / ctas, ms[0], ms[1], ms[2], ms[3]);
     }
     return PSDF_OK;
 }
