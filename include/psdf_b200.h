@@ -353,6 +353,12 @@ int psdf_bg_fused_forward(int N, int L, int T, const float* pos, const float* di
 int psdf_nerf_fused_forward(int pos_dim, int N, int L, int T, const float* pos, const float* dirs, const float* lattice,
                             const float* scale_factor, const float* shift, const float* window, float points_scaling, const uint8_t* blob,
                             float* rgb_raw, float* density, void* stream);
+/* NerfHash.get_only_density (permuto_sdf_py/models/models.py:528-550) of the foreground NerfHash(3): encoding(pos [N,3]) -> trunk ->
+ * density [N] = softplus(z[:,0]), no colour head and no view directions. The blob of psdf_bg_mlp_pack (the head's blocks are not read);
+ * the density equals psdf_nerf_fused_forward(3, ...)'s bit for bit. Row limits and PSDF_ERR_UNSUPPORTED cases of
+ * psdf_nerf_fused_forward at pos_dim 3; N == 0 is a no-op; rows >= N are not written. */
+int psdf_nerf_density_forward(int N, int L, int T, const float* pos, const float* lattice, const float* scale_factor, const float* shift,
+                              const float* window, float points_scaling, const uint8_t* blob, float* density, void* stream);
 /* backward of psdf_bg_fused_forward (loss.backward() through NerfHash.forward, first order): g_rgb_raw [N,3], g_density [N] ->
  * grad_lattice (+=), weight gradients gW_l [N_l,K_l] (+=) and bias gradients gb_l (+=). workspace:
  * psdf_bg_fused_backward_workspace_bytes(N) bytes of scratch. Launches the tensor-core kernel, then the lattice-scatter kernel. */

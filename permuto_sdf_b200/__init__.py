@@ -10,6 +10,7 @@ sphere-tracing hot path behind the reference's own Python operator API.
     permuto_sdf_b200.SpaceTimeFit             space-time SDF from a point sequence (train_4d_sdf.py) on the fused kernels
     permuto_sdf_b200.NerfTrainer              NeRF training (train_nerf.py) on the fused kernels
     permuto_sdf_b200.extract_mesh_from_sdf_model / marching_cubes / Mesh   meshes from a trained SDF or a volume on the GPU
+    permuto_sdf_b200.extract_mesh_from_density_model   meshes from a trained NeRF's density (NerfTrainer.model) on the GPU
 
 All device work goes through the C ABI in include/psdf_b200.h (libpsdf_b200.so, hand-written CUDA).
 There is no CPU or PyTorch fallback: importing is cheap, but any op raises if the library is missing
@@ -32,7 +33,7 @@ def __getattr__(name):
     if name == "NerfTrainer":
         from .nerf_train import NerfTrainer
         return NerfTrainer
-    if name in ("Mesh", "marching_cubes", "extract_mesh_from_sdf_model"):
+    if name in ("Mesh", "marching_cubes", "extract_mesh_from_sdf_model", "extract_mesh_from_density_model"):
         from . import mesh
         return getattr(mesh, name)
     if name == "AABB":

@@ -14,6 +14,9 @@
 // l = 6..0: abar_l = zbar^(l) W_l on the tensor cores (warpgroups 0 / 1) beside dW_l = zbar^(l)^T a_l (warpgroups 2 / 3, fixed-point sums
 // per CTA as in fused_rgb_bwd.cu), zbar^(l-1) = abar_l gelu'(z^(l-1)) (softplus' for the density column), a_(l-1) rebuilt from the stored
 // pre-activations (a_0 from the encoder). abar_0's lattice columns leave to the workspace; k_lattice_scatter scatters them.
+//
+// Density only (k_bg_fused<D, true>, NerfHash.get_only_density): the same code for encoder and layers 0..3, without the SH columns, the
+// GELU of layer 3's feature columns and the colour head. Its density is the full forward's, bit for bit.
 #include "fused_common.cuh"
 #include "fused_rgb_common.cuh"
 #include "../../include/psdf_b200.h"
@@ -131,7 +134,7 @@ __device__ __forceinline__ void gelu_chunk_to_tile(uint32_t taddr, const float* 
 // chunks of layer l's output that feed the next layer (the trunk output's density chunk does not)
 __device__ __forceinline__ int act_chunks(const BgGeom& g, int l) { return l == 3 ? kBgFeat / 16 : g.Np[l] / 16; }
 
-template <int D>
+template <int D, bool kDensityOnly>
 __global__ void __launch_bounds__(kRgbThreads, 1)
 k_bg_fused(BgParams P, const float* __restrict__ pos, const float* __restrict__ dirs, const float2* __restrict__ lattice,
            const float* __restrict__ scale, const float* __restrict__ shift, const float* __restrict__ window, const uint8_t* __restrict__ blob,
@@ -158,13 +161,14 @@ k_bg_fused(BgParams P, const float* __restrict__ pos, const float* __restrict__ 
     __syncthreads();
     uint32_t w_phase = 0;
     const int ntiles = (P.N + kTile - 1) / kTile;
+    constexpr int kLayers = kDensityOnly ? 4 : kBgNL;      // density only: the trunk, whose last layer holds the density column
     if (tid == 0 && blockIdx.x < ntiles) load_layer_weights(s_w, blob, P.g, 0, false, &bars[0]);
     for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
         const int n = tile * kTile + row;
         const bool valid = n < P.N;
-        build_bg_input<D>(P, lc, lattice, pos, dirs, n, valid, row, grp, s_a, s_a + kWTileBytes, true);
+        build_bg_input<D>(P, lc, lattice, pos, dirs, n, valid, row, grp, s_a, s_a + kWTileBytes, !kDensityOnly);
 #pragma unroll 1
-        for (int l = 0; l < kBgNL; l++) {
+        for (int l = 0; l < kLayers; l++) {
             umma::mbar_wait(&bars[0], w_phase);
             w_phase ^= 1;
             umma::fence_async_smem();
@@ -172,12 +176,13 @@ k_bg_fused(BgParams P, const float* __restrict__ pos, const float* __restrict__ 
             issue_gemm_w(0, warp >> 2, s_a, s_a + kWTileBytes, s_w, s_w + P.g.Np[l] * P.g.Kp[l] * 2, P.g.Kp[l], P.g.Np[l]);
             __syncthreads();
             if (tid == 0) {
-                if (l + 1 < kBgNL) load_layer_weights(s_w, blob, P.g, l + 1, false, &bars[0]);
+                if (l + 1 < kLayers) load_layer_weights(s_w, blob, P.g, l + 1, false, &bars[0]);
                 else if (tile + (int)gridDim.x < ntiles) load_layer_weights(s_w, blob, P.g, 0, false, &bars[0]);
             }
             const uint32_t trow = (uint32_t)((warp & 3) * 32) << 16;
             if (l < kBgNL - 1) {
-                for (int c = grp; c < act_chunks(P.g, l); c += kRgbGroups) gelu_chunk_to_tile(trow + c * 16, s_bias + l * 128 + c * 16, s_a, row, c);
+                if (!kDensityOnly || l < kLayers - 1)      // layer 3's feature columns feed the colour head only
+                    for (int c = grp; c < act_chunks(P.g, l); c += kRgbGroups) gelu_chunk_to_tile(trow + c * 16, s_bias + l * 128 + c * 16, s_a, row, c);
                 if (l == 3 && grp == 0 && valid) {
                     float z[16];
                     umma::tmem_ld16(trow + kBgDensityCol, z);
@@ -661,7 +666,8 @@ int persistent_grid(int ntiles) {
 
 #define ST ((cudaStream_t)stream)
 
-template <int D>
+// kDensityOnly: density alone (dirs and rgb_raw unused)
+template <int D, bool kDensityOnly = false>
 int nerf_fused_forward(int N, int L, int T, const float* pos, const float* dirs, const float* lattice, const float* scale_factor,
                        const float* shift, const float* window, float points_scaling, const uint8_t* blob, float* rgb_raw, float* density,
                        void* stream) {
@@ -670,9 +676,9 @@ int nerf_fused_forward(int N, int L, int T, const float* pos, const float* dirs,
     if (rc != PSDF_OK) return rc;
     if (N == 0) return PSDF_OK;
     const size_t smem = (size_t)2 * kWTileBytes + kBgWBytes + sizeof(LevelC) + kBgNL * 128 * sizeof(float) + 64;
-    { static bool optin_[64]; psdf::psdf_optin_smem(k_bg_fused<D>, 227 * 1024, optin_); }
-    k_bg_fused<D><<<persistent_grid(div_up(N, kTile)), kRgbThreads, smem, ST>>>(P, pos, dirs, reinterpret_cast<const float2*>(lattice),
-                                                                               scale_factor, shift, window, blob, rgb_raw, density);
+    { static bool optin_[64]; psdf::psdf_optin_smem(k_bg_fused<D, kDensityOnly>, 227 * 1024, optin_); }
+    k_bg_fused<D, kDensityOnly><<<persistent_grid(div_up(N, kTile)), kRgbThreads, smem, ST>>>(
+        P, pos, dirs, reinterpret_cast<const float2*>(lattice), scale_factor, shift, window, blob, rgb_raw, density);
     PSDF_CHECK_LAUNCH();
     return PSDF_OK;
 }
@@ -762,6 +768,13 @@ int psdf_nerf_fused_forward(int pos_dim, int N, int L, int T, const float* pos, 
     if (N < 0 || !nerf_rows_ok(pos_dim, N)) return PSDF_ERR_UNSUPPORTED;
     return pos_dim == 3 ? nerf_fused_forward<3>(N, L, T, pos, dirs, lattice, scale_factor, shift, window, points_scaling, blob, rgb_raw, density, stream)
                         : nerf_fused_forward<4>(N, L, T, pos, dirs, lattice, scale_factor, shift, window, points_scaling, blob, rgb_raw, density, stream);
+}
+
+int psdf_nerf_density_forward(int N, int L, int T, const float* pos, const float* lattice, const float* scale_factor, const float* shift,
+                              const float* window, float points_scaling, const uint8_t* blob, float* density, void* stream) {
+    if (N < 0 || !nerf_rows_ok(3, N)) return PSDF_ERR_UNSUPPORTED;
+    return nerf_fused_forward<3, true>(N, L, T, pos, nullptr, lattice, scale_factor, shift, window, points_scaling, blob, nullptr, density,
+                                       stream);
 }
 
 // workspace: abar_0 of every level and sample slot (8 bytes each), sized for kMaxLevels so that the size depends on the sample count alone

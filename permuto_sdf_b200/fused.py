@@ -537,10 +537,11 @@ class FusedNerfHash:
         call("psdf_bg_mlp_pack", self.in_dim, *[p.detach() for p in params], self.blob)
         self.packed_versions = tuple(p._version for p in params)
 
-    def _window(self, iter_nr):
+    def _window(self, iter_nr, record=True):
         from .models import map_range_val
         m = self.model
-        m.last_iter_nr = int(iter_nr)
+        if record:
+            m.last_iter_nr = int(iter_nr)
         return m.c2f(map_range_val(iter_nr, 0.0, m.nr_iters_for_c2f, 0.3, 1.0)).view(-1).contiguous()
 
     def _forward(self, pos, dirs, lattice, window):
@@ -558,6 +559,22 @@ class FusedNerfHash:
         self.pack(self.params())
         return self._forward(samples_pos.detach().contiguous(), samples_dirs.detach().contiguous(), self.model.encoding.lattice_values,
                              self._window(iter_nr))
+
+    @torch.no_grad()
+    def density(self, pos, iter_nr):
+        """NerfHash.get_only_density (models.py:528-550) of a foreground NerfHash(3): density [N,1] at pos [N,3], no autograd, from the
+        density-only kernel (encoder and trunk; the colour head is not run). Bit-identical to the density of __call__. Leaves
+        model.last_iter_nr as it is, as the reference's get_only_density does."""
+        if self.pos_dim != 3:
+            raise RuntimeError("FusedNerfHash.density: the density-only kernel serves the 3-D NerfHash (pos_dim 3), got pos_dim %d"
+                               % self.pos_dim)
+        self.pack(self.params())
+        enc = self.model.encoding
+        pos = pos.detach().contiguous()
+        density = torch.empty(pos.shape[0], 1, device=pos.device)
+        call("psdf_nerf_density_forward", pos.shape[0], enc.nr_levels, enc.capacity, pos, enc.lattice_values.detach(), enc.scale_factor,
+             enc.shift_tensor(), self._window(iter_nr, record=False), enc.concat_points_scaling, self.blob, density)
+        return density
 
     def train_forward(self, samples_pos, samples_dirs, iter_nr):
         """differentiable (wrt the hash table, weights and biases) linear colour [N,3] and density [N,1]"""

@@ -1,9 +1,10 @@
-"""Meshes from a volume or a trained SDF on the GPU (extract_mesh_from_sdf_model, permuto_sdf_py/utils/sdf_utils.py:252-292).
+"""Meshes from a volume, a trained SDF or a trained NeRF density on the GPU (extract_mesh_from_sdf_model and
+extract_mesh_from_density_model, permuto_sdf_py/utils/sdf_utils.py:252-292 and :339-380).
 
 The reference evaluates the SDF in 64^3 chunks into a dense host array of N^3 floats and runs skimage's marching cubes on the CPU. Here
-the grid is evaluated a slab of slices at a time by the fused forward kernel (FusedSDF), and each slab goes straight to the marching-cubes
-kernels (csrc/marching_cubes.cu), which carry the vertex numbering from slab to slab. The N^3 volume never exists; memory is
-O(N^2 * slab) plus the mesh. The output is a fixed function of the volume (see the header), the same for any slab split and on every run.
+the grid is evaluated a slab of slices at a time by a fused forward kernel (FusedSDF, or the density-only FusedNerfHash.density), and
+each slab goes straight to the marching-cubes kernels (csrc/marching_cubes.cu), which carry the vertex numbering from slab to slab.
+The N^3 volume never exists; memory is O(N^2 * slab) plus the mesh. The output is a fixed function of the volume (see the header), the same for any slab split and on every run.
 """
 import math
 
@@ -128,6 +129,40 @@ class Mesh:
             f.write(frec.tobytes())
 
 
+def _mesh_grid(N, min_val, max_val, threshold, dev, values):
+    """the grid linspace(min_val, max_val, N)^3 (axis 0 = x) a slab of slices at a time: values(pts [n,3], out [n]) writes the volume's
+    values at the slab's points into out (a view of the slab buffer), and each slab goes through the marching-cubes kernels with
+    `threshold` as it comes. Vertices rescaled as the reference does, v / fp32(N - 1) * fp32(max_val - min_val) + min_val in fp32.
+    -> (V [V,3], F [F,3] int32)"""
+    lin = torch.linspace(min_val, max_val, N, device=dev)
+    S = _slab_slices(N, N, N)
+    vals = torch.empty(S + 1, N, N, device=dev)
+    mc = _SlabMarchingCubes(N, S, N, N, threshold, dev, affine=(float(N - 1), float(max_val - min_val), float(min_val)))
+    for i0 in range(0, N - 1, S):
+        i1 = min(i0 + S, N - 1)
+        first = 0 if i0 == 0 else 1
+        if first:
+            vals[0].copy_(vals[S])               # the shared slice of the previous slab
+        rows = lin[i0 + first:i1 + 1]
+        pts = torch.stack(torch.meshgrid(rows, lin, lin, indexing="ij"), -1).reshape(-1, 3)
+        values(pts, vals[first:i1 - i0 + 1].view(-1))
+        del pts
+        mc.run(vals[:i1 - i0 + 1], i0)
+    return mc.result()
+
+
+def _check_extraction_args(fn, model, kind, nr_points_per_dim, min_val, max_val, threshold):
+    if getattr(model, "in_channels", None) != 3:
+        raise RuntimeError("%s: the model has in_channels %s; meshes are extracted from a 3-D %s (in_channels 3), %s" % (
+            fn, getattr(model, "in_channels", None), kind[0], kind[1]))
+    N = int(nr_points_per_dim)
+    if N < 2:
+        raise RuntimeError("%s: nr_points_per_dim must be >= 2, got %d" % (fn, N))
+    if not all(math.isfinite(float(x)) for x in (min_val, max_val, threshold)):
+        raise RuntimeError("%s: min_val, max_val and threshold must be finite" % fn)
+    return N
+
+
 @torch.no_grad()
 def extract_mesh_from_sdf_model(model, nr_points_per_dim, min_val, max_val, threshold=0, iter_nr=9999999):
     """sdf_utils.py:252-292 for an SDF with in_channels 3: the grid linspace(min_val, max_val, N)^3 (axis 0 = x), evaluated by the model's
@@ -136,36 +171,17 @@ def extract_mesh_from_sdf_model(model, nr_points_per_dim, min_val, max_val, thre
     iter_nr selects the coarse-to-fine window (the reference's 9999999: all levels). Restores model.training and model.last_iter_nr and
     attaches nothing to the model. -> Mesh"""
     from .fused import FusedSDF
-    if getattr(model, "in_channels", None) != 3:
-        raise RuntimeError("extract_mesh_from_sdf_model: the model has in_channels %s; meshes are extracted from a 3-D SDF (in_channels 3), "
-                           "a space-time SDF (in_channels 4) has no single surface" % getattr(model, "in_channels", None))
-    N = int(nr_points_per_dim)
-    if N < 2:
-        raise RuntimeError("extract_mesh_from_sdf_model: nr_points_per_dim must be >= 2, got %d" % N)
-    if not all(math.isfinite(float(x)) for x in (min_val, max_val, threshold)):
-        raise RuntimeError("extract_mesh_from_sdf_model: min_val, max_val and threshold must be finite")
+    N = _check_extraction_args("extract_mesh_from_sdf_model", model, ("SDF", "a space-time SDF (in_channels 4) has no single surface"),
+                               nr_points_per_dim, min_val, max_val, threshold)
     fused = getattr(model, "fused", None) or FusedSDF(model)
     dev = model.encoding.lattice_values.device
     was_training, last_iter_nr = model.training, model.last_iter_nr
     model.eval()
     try:
         with torch.cuda.device(dev):
-            lin = torch.linspace(min_val, max_val, N, device=dev)
-            S = _slab_slices(N, N, N)
-            vals = torch.empty(S + 1, N, N, device=dev)
-            mc = _SlabMarchingCubes(N, S, N, N, threshold, dev, affine=(float(N - 1), float(max_val - min_val), float(min_val)))
-            for i0 in range(0, N - 1, S):
-                i1 = min(i0 + S, N - 1)
-                first = 0 if i0 == 0 else 1
-                if first:
-                    vals[0].copy_(vals[S])               # the shared slice of the previous slab
-                rows = lin[i0 + first:i1 + 1]
-                pts = torch.stack(torch.meshgrid(rows, lin, lin, indexing="ij"), -1).reshape(-1, 3)
-                sdf = fused(pts, iter_nr, with_gradient=False, with_geom=False)[0]
-                vals[first:i1 - i0 + 1].view(-1).copy_(sdf.view(-1))
-                del pts, sdf
-                mc.run(vals[:i1 - i0 + 1], i0)
-            V, Fc = mc.result()
+            def sdf(pts, out):
+                out.copy_(fused(pts, iter_nr, with_gradient=False, with_geom=False)[0].view(-1))
+            V, Fc = _mesh_grid(N, min_val, max_val, threshold, dev, sdf)
             NV = torch.empty_like(V)
             for a in range(0, V.shape[0], _SLAB_POINTS):
                 g = fused(V[a:a + _SLAB_POINTS], iter_nr, with_gradient=True, with_geom=False)[1]
@@ -176,4 +192,41 @@ def extract_mesh_from_sdf_model(model, nr_points_per_dim, min_val, max_val, thre
         model.last_iter_nr = last_iter_nr
 
 
-__all__ = ["Mesh", "marching_cubes", "extract_mesh_from_sdf_model"]
+@torch.no_grad()
+def extract_mesh_from_density_model(model, nr_points_per_dim, min_val, max_val, threshold=0, iter_nr=9999999):
+    """sdf_utils.py:339-380 for a NeRF density model (NerfHash with in_channels 3, e.g. NerfTrainer.model): the grid
+    linspace(min_val, max_val, N)^3 (axis 0 = x), evaluated by the density-only fused kernel (FusedNerfHash.density) a slab of slices
+    at a time and meshed on the GPU as it comes. Inside is density > threshold: the marching-cubes kernels see -density against
+    -threshold (negation is exact, so the vertices are those of the density at threshold, and faces wind counter-clockwise seen from
+    outside the dense region). Vertices rescaled as extract_mesh_from_sdf_model does. Normals: F.normalize of the central difference
+    density(v - h e_i) - density(v + h e_i), i = x, y, z, with h = fp32(max_val - min_val) / fp32(N - 1) (one grid spacing); they point
+    out of the dense region. The reference's unused `lattice` argument is dropped. iter_nr selects the coarse-to-fine window (the
+    reference's 9999999: all levels). Restores model.training and model.last_iter_nr and attaches nothing to the model. -> Mesh"""
+    from .fused import FusedNerfHash
+    N = _check_extraction_args("extract_mesh_from_density_model", model,
+                               ("NeRF density model", "a background NerfHash (in_channels 4) has no single surface"),
+                               nr_points_per_dim, min_val, max_val, threshold)
+    fused = getattr(model, "fused", None) or FusedNerfHash(model)
+    dev = model.encoding.lattice_values.device
+    was_training, last_iter_nr = model.training, model.last_iter_nr
+    model.eval()
+    try:
+        with torch.cuda.device(dev):
+            def neg_density(pts, out):
+                torch.neg(fused.density(pts, iter_nr).view(-1), out=out)
+            V, Fc = _mesh_grid(N, min_val, max_val, -float(threshold), dev, neg_density)
+            h = float(np.float32(max_val - min_val) / np.float32(N - 1))
+            offs = h * torch.eye(3, device=dev)
+            NV = torch.empty_like(V)
+            step = _SLAB_POINTS // 6
+            for a in range(0, V.shape[0], step):
+                v = V[a:a + step]
+                d = fused.density(torch.cat([v - offs[i] for i in range(3)] + [v + offs[i] for i in range(3)]), iter_nr).view(6, -1)
+                NV[a:a + step] = F.normalize((d[:3] - d[3:]).t().contiguous(), dim=1)
+        return Mesh(V, Fc, NV)
+    finally:
+        model.train(was_training)
+        model.last_iter_nr = last_iter_nr
+
+
+__all__ = ["Mesh", "marching_cubes", "extract_mesh_from_sdf_model", "extract_mesh_from_density_model"]

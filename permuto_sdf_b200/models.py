@@ -405,6 +405,17 @@ class NerfHash(torch.nn.Module, _Checkpointed):
             rgb = model_colorcal.calib_RGB_samples_packed(rgb, img_indices, ray_start_end_idx)
         return torch.sigmoid(rgb), density
 
+    def get_only_density(self, ray_samples, iter_nr):
+        """models.py:528-550: density [N,1] = softplus of the trunk's first output at ray_samples (reshaped to [-1, in_channels]), no
+        colour head. A fused 3-D model on CUDA input runs the density-only kernel (FusedNerfHash.density, no autograd); otherwise the
+        per-op encoder and trunk. Sets no last_iter_nr, as the reference does not."""
+        points = ray_samples.reshape(-1, self.in_channels)
+        if getattr(self, "fused", None) is not None and points.is_cuda and self.in_channels == 3:
+            return self.fused.density(points, iter_nr)
+        window = self.c2f(map_range_val(iter_nr, 0.0, self.nr_iters_for_c2f, 0.3, 1.0))
+        fd = self.mlp_feat_and_density(self.encoding(points, window.view(-1)))
+        return F.softplus(fd[:, 0:1])
+
 
 class Colorcal(torch.nn.Module, _Checkpointed):
     """models.py:677-741: per-image affine colour calibration, image `idx_with_fixed_calib` stays identity"""
