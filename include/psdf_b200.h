@@ -30,7 +30,7 @@ extern "C" {
 #endif
 
 /* changes when an existing entry point changes its signature or behaviour; entry points that are only added leave it as it is */
-#define PSDF_ABI_VERSION 1
+#define PSDF_ABI_VERSION 2
 #define PSDF_ERR_ARG_ -1
 #define PSDF_ERR_LAUNCH_ -2
 #define PSDF_ERR_UNSUPPORTED_ -3
@@ -314,8 +314,7 @@ int psdf_sdf_fused_backward_multi(int L, int T, const float* lattice, const floa
  * column 2L + 3 holds t * points_scaling), so the blob of psdf_sdf_mlp_pack serves both. grad / g_grad are [N,3] for both: the SPATIAL
  * derivatives d sdf / d (x, y, z), which is all train_4d_sdf.py:212-217 reads of model.get_sdf_and_gradient (it keeps [:, 0:3] of the
  * [N,4] gradient); the time derivative is not formed. The backward's tangent direction is (g_grad, 0). The workspace does not depend on
- * pos_dim (psdf_sdf_fused_backward_multi_workspace_bytes). A pos_dim = 4 forward with grad always runs the two-group kernel (the
- * lock-step variant of psdf_sdf_forward_variant is D = 3). Any other pos_dim: PSDF_ERR_UNSUPPORTED. Replaces
+ * pos_dim (psdf_sdf_fused_backward_multi_workspace_bytes). Any other pos_dim: PSDF_ERR_UNSUPPORTED. Replaces
  * model.get_sdf_and_gradient(points_time, iter_nr) (models.py:199-259) and loss.backward() through it (train_4d_sdf.py:212, 237). */
 int psdf_sdf_fused_forward_dim(int pos_dim, int N, int L, int T, const float* pos, const float* lattice, const float* scale_factor,
                                const float* shift, const float* window, float points_scaling, int hidden, int out_dim, const uint8_t* blob,
@@ -410,9 +409,6 @@ int psdf_nerf_loss_backward(PSDF_RSP, const float* x_raw, const float* density, 
  * The reference's iteration (permuto_sdf_py/train_permuto_sdf.py:311-422) spends ~70 one-block PyTorch launches between its big kernels
  * (schedule ramps, Lipschitz normalisation, calibration, loss reductions, zero-fills, gradient adds). These entry points fold them into
  * the neighbouring kernels; permuto_sdf_b200/train.py Trainer._iteration_direct strings them together. */
-/* kernel variant of the value + tangent forward (A/B measurements): 1 = two independent 64-sample groups per CTA (default),
- * 0 = lock-step 128-sample tiles; any other value only queries. Returns the variant in use. Same results to the last bit. */
-int psdf_sdf_forward_variant(int variant);
 /* two independent sample sets in one psdf_sdf_fused_forward launch (N1 = 0: unused); grad / geom may be NULL per set */
 int psdf_sdf_fused_forward_multi(int L, int T, const float* lattice, const float* scale_factor, const float* shift, const float* window,
                                  float points_scaling, int hidden, int out_dim, const uint8_t* blob, int N0, const float* pos0, float* sdf0,

@@ -60,7 +60,7 @@ def declared_symbols():
 
 
 _lib = None
-_NON_STATUS = ("psdf_abi_version", "psdf_device_ok", "psdf_sdf_forward_variant")
+_NON_STATUS = ("psdf_abi_version", "psdf_device_ok")
 
 
 def load_library(path=LIB_PATH):

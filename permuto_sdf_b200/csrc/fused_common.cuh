@@ -217,8 +217,6 @@ struct FusedParams {
     unsigned cap_mask;   // t_magic(T): multiplier of the division-free h mod T (any capacity, not only powers of two)
     float points_scaling;
     int in_dim;          // (L + E) * 2 feature columns
-    int knockout = 0;    // diagnostics only (PSDF_EXPERIMENT_KNOCKOUT, k_sdf_lattice_scatter): bit 0 issue no reduction, bit 1 no warp
-                         // aggregation -- "what would this cost if it were free" timings (results are garbage); 0 in production
     MlpGeom g;
 };
 
@@ -389,20 +387,6 @@ __device__ __forceinline__ void split_n(int N, int half, int& n0, int& nn) {
     nn = half ? N - na : na;
 }
 
-// rows [64 mh, 64 mh + 64) of one stream of D[128 x Np] = A[128 x Kp] W^T as the three split products (one warpgroup, see
-// umma::wg_gemm). A tiles have the 8-row-group stride a_sbo; the weight tile is [Np rows][Kp] K-major. Descriptor convention
-// checked by tests/test_fused_gpu.py::test_umma_gemm_self_test: the first offset field (LBO) is the stride between core
-// matrices adjacent along K, the second (SBO) between 8-row groups.
-__device__ __forceinline__ void issue_gemm(uint32_t tmem_d, int mh, const uint8_t* a_hi, const uint8_t* a_lo, const uint8_t* w_hi,
-                                           const uint8_t* w_lo, int Kp, int Np, int a_sbo = kSBO_A) {
-    const uint32_t sbo_w = (Kp / 8) * kLBO;
-    const uint32_t ao = (uint32_t)(mh * 8 * a_sbo);
-    const uint64_t dah = umma::make_desc(umma::smem_u32(a_hi) + ao, kLBO, a_sbo), dal = umma::make_desc(umma::smem_u32(a_lo) + ao, kLBO, a_sbo);
-    const uint64_t dwh = umma::make_desc(umma::smem_u32(w_hi), kLBO, sbo_w), dwl = umma::make_desc(umma::smem_u32(w_lo), kLBO, sbo_w);
-    umma::wg_gemm<0, 0>(tmem_d + ((uint32_t)(64 * mh) << 16), false, dah, dal, dwh, dwl, (2 * kLBO) >> 4, (2 * kLBO) >> 4, (8 * sbo_w) >> 4,
-                        Kp / 16, Np, false);
-}
-
 // v broadcast from lane 0. For values that are the same in every lane of a warp but that ptxas cannot prove so: the warp index, and
 // the per-layer geometry P.g.*[l] under a runtime l (read per thread with a register index). Branches and wgmma k-loops bounded by
 // such values count as divergent for ptxas, which then serializes the wgmma chains behind them (C7520: a wait after every HGMMA).
@@ -438,9 +422,6 @@ __device__ __forceinline__ float2 add_peers2(unsigned peers, float2 x, int lane)
 __device__ __forceinline__ void red_v2(float* addr, float2 v) {
     asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(addr), "f"(v.x), "f"(v.y) : "memory");
 }
-__device__ __forceinline__ void red_v4(float* addr, float a, float b, float c, float d) {     // 16-byte aligned address
-    asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(addr), "f"(a), "f"(b), "f"(c), "f"(d) : "memory");
-}
 // one lattice-gradient contribution: float atomics, or fixed point (deterministic mode, ftab != NULL)
 __device__ __forceinline__ void scatter2(float* gtab, unsigned long long* ftab, unsigned idx, float2 cv) {
     if (ftab) { fx_add(ftab + (size_t)idx * 2, cv.x); fx_add(ftab + (size_t)idx * 2 + 1, cv.y); }
@@ -450,11 +431,10 @@ __device__ __forceinline__ void scatter2(float* gtab, unsigned long long* ftab, 
 //     lattice[idx_r] += w (B_r abar + dB_r tabar),  r = 0..D,   abar = (a0, a1), tabar = (t0, t1) of the level's two features
 // x, v: position and tangent direction (D coordinates); scale3 / shift3: the level's scale and shift; gtab / ftab: the level's float /
 // fixed-point gradient table (scatter2). TAN = false: no tangent term (v, t0, t1 unused), lattice[idx_r] += w B_r abar. Invalid lanes add
-// nothing. aggregate: warp-uniform, sum the lanes that share a vertex first (match_any + add_peers2, one reduction per distinct vertex);
-// do_red = false issues no reduction (diagnostics, PSDF_EXPERIMENT_KNOCKOUT).
+// nothing. aggregate: warp-uniform, sum the lanes that share a vertex first (match_any + add_peers2, one reduction per distinct vertex).
 template <bool TAN, int D = 3>
 __device__ __forceinline__ void scatter_level(const float* x, const float* v, const float* scale3, const float* shift3, float w, float a0,
-                                              float a1, float t0, float t1, bool valid, bool aggregate, bool do_red, int lane,
+                                              float a1, float t0, float t1, bool valid, bool aggregate, int lane,
                                               unsigned cap_mask, unsigned T, float* gtab, unsigned long long* ftab) {
     float cf[D], dcf[D], e[D + 1];
 #pragma unroll
@@ -482,8 +462,8 @@ __device__ __forceinline__ void scatter_level(const float* x, const float* v, co
             unsigned key = valid ? idx : 0xffffffffu;
             unsigned peers = __match_any_sync(kFull, key);
             cv = add_peers2(peers, cv, lane);
-            if (valid && lane == __ffs(peers) - 1 && do_red) scatter2(gtab, ftab, idx, cv);
-        } else if (valid && (do_red || cv.x == 123.456f)) {
+            if (valid && lane == __ffs(peers) - 1) scatter2(gtab, ftab, idx, cv);
+        } else if (valid) {
             scatter2(gtab, ftab, idx, cv);
         }
     }

@@ -230,7 +230,7 @@ k_lattice_scatter(int N, int T, unsigned cap_mask, const float* __restrict__ pos
     const float w = window ? window[l] : 1.0f;
     const float2 a = xch[(size_t)l * xch_stride + slot];
     const bool aggregate = sc[0] < kAggregateBelowScale;             // warp-uniform (l is)
-    scatter_level<false, D>(x, nullptr, sc, sh, w, a.x, a.y, 0.f, 0.f, valid, aggregate, true, lane, cap_mask, (unsigned)T,
+    scatter_level<false, D>(x, nullptr, sc, sh, w, a.x, a.y, 0.f, 0.f, valid, aggregate, lane, cap_mask, (unsigned)T,
                             grad_lattice + (size_t)l * T * 2, fx_lattice ? fx_lattice + (size_t)l * T * 2 : nullptr);
 }
 

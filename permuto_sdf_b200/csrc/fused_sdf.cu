@@ -13,26 +13,22 @@
 // the same weights ( tz_l = W_l ta_{l-1}, ta_l = gelu'(z_l) * tz_l ), their level-0 input being d feat / d x_j,
 // which is exact because barycentric weights are piecewise linear in x.
 //
-// Work mapping: one CTA = one 128-sample tile = the M of the MMA, 512 threads = 4 groups x 128 rows.
-//   encoder : thread (row, g) computes the 16-byte operand cores g, g+4, ... (4 lattice levels = 8 features each)
-//             of its sample for all streams -> 16 gathers per thread in flight at L = 16, 16 warps per SM;
-//   MMA     : warpgroup s issues stream s, (K/16) x 3 wgmma per 64 rows, into the CTA's accumulator area;
-//   epilogue: thread (row, g) owns accumulator columns [16g, 16g+16) of row `row` (accumulator lane row) of every stream:
-//             bias, GELU / GELU', bf16 hi/lo split, 16-byte core stores for the next layer.
-// The value-only kernels (256 threads) and the two-group value + tangent kernel keep their products in registers instead (see
-// value_rows and k_sdf_fused_dual).
+// Work mapping: the encoder threads of a sample row each compute some of its 16-byte operand cores (4 lattice levels = 8 features
+// each) for all streams; wgmma products stay in the registers of the warpgroup that issues them, whose epilogue (bias, GELU / GELU',
+// bf16 hi/lo split) writes the next layer's operand tiles from the fragments. Value only (k_sdf_fused, the sphere tracer): 128-sample
+// tiles, 256 threads, two CTAs per SM (see value_rows). Value + tangents: two groups of 256 threads per CTA on 64-sample sub-tiles
+// (k_sdf_fused_dual).
 // Weights (hi+lo, pre-packed in the core-matrix operand layout by k_pack_mlp) are fetched once per CTA with one
-// cp.async.bulk (TMA) and stay resident; CTAs are persistent over tiles (one CTA per SM).
+// cp.async.bulk (TMA) and stay resident; CTAs are persistent over tiles.
 #include "fused_common.cuh"
 #include "../../include/psdf_b200.h"
 
 using namespace psdf_fused;
 
 namespace {
-// Threads per CTA. The value + tangent kernel needs 186 KB of shared memory (one CTA per SM, 512 threads = 4 per sample row). The
-// value-only kernels (inference forward, sphere tracer) need 93 KB: with 256 threads (2 per row, <= 128 registers) TWO CTAs share an
-// SM, each on its own tile with its own barriers, so that one CTA's MMA / barrier / gather waits are filled by the other's work.
-constexpr int kFusedThreads = 512;
+// Threads per CTA of the value-only kernels (inference forward, sphere tracer). They need 93 KB of shared memory: with 256 threads (2 per
+// row, <= 128 registers) TWO CTAs share an SM, each on its own tile with its own barriers, so that one CTA's MMA / barrier / gather waits
+// are filled by the other's work.
 constexpr int kValueThreads = 256;
 // Up to two independent sample sets per launch (the main samples and the off-surface points of a training iteration): each set starts on
 // a tile boundary and has its own outputs (grad / geom may be NULL per set).
@@ -44,11 +40,8 @@ struct FwdSegs {
     float* grad[2];
     float* geom[2];
 };
-template <bool TAN> struct FwdCfg { static constexpr int kThreads = TAN ? kFusedThreads : kValueThreads; static constexpr int kCtasPerSm = TAN ? 1 : 2; };
 // directions of the three spatial tangents d / d x_j (concat_core)
 __device__ constexpr float kUnit3[3][3] = {{1.f, 0.f, 0.f}, {0.f, 1.f, 0.f}, {0.f, 0.f, 1.f}};
-// accumulator areas (umma.cuh) of the kernels of this file
-__device__ float g_acc_tan[(size_t)kAccCtas * kTile * 256];
 
 // ---------------------------------------------------------------------------------------------- value-only layers in registers
 // Layer l of a value-only 128-row tile (inference forward, sphere tracer): warpgroup mh forms rows 64 mh .. 64 mh + 63 of D = A W^T in
@@ -82,17 +75,16 @@ __device__ __forceinline__ void gelu_to_tiles(const float* acc, const float* bia
     }
 }
 
-// D = 3: positions [N,3]; D = 4: space-time positions [N,4] (x, y, z, t), value only (the tangent variants are D = 3)
-template <bool TAN, int D = 3>
-__global__ void __launch_bounds__(FwdCfg<TAN>::kThreads, FwdCfg<TAN>::kCtasPerSm)
+// Value only (sdf and geometric feature, no tangents). D = 3: positions [N,3]; D = 4: space-time positions [N,4] (x, y, z, t)
+template <int D>
+__global__ void __launch_bounds__(kValueThreads, 2)
 k_sdf_fused(FusedParams P, FwdSegs G, const float2* __restrict__ lattice, const float* __restrict__ scale,
             const float* __restrict__ shift, const float* __restrict__ window, const uint8_t* __restrict__ blob) {
-    constexpr int S = TAN ? 4 : 1;
-    constexpr int kThreads = FwdCfg<TAN>::kThreads, kGroups = kThreads / kTile;
+    constexpr int kGroups = kValueThreads / kTile;
     extern __shared__ __align__(128) uint8_t smem[];
     uint8_t* s_blob = smem;
-    uint8_t* s_a = smem + P.g.total;                       // S streams x {hi, lo} x 16 KB
-    LevelC* lc = reinterpret_cast<LevelC*>(s_a + S * 2 * kATileBytes);
+    uint8_t* s_a = smem + P.g.total;                       // {hi, lo} x 16 KB
+    LevelC* lc = reinterpret_cast<LevelC*>(s_a + 2 * kATileBytes);
     uint64_t* bars = reinterpret_cast<uint64_t*>(lc + 1);  // [0] weights
     const int tid = threadIdx.x, warp = tid >> 5;
     const int row = tid & (kTile - 1), grp = tid >> 7;
@@ -100,15 +92,13 @@ k_sdf_fused(FusedParams P, FwdSegs G, const float2* __restrict__ lattice, const 
     if (tid == 0) {
         umma::mbar_init(&bars[0], 1);
         umma::mbar_fence_init();
-        if (TAN) umma::acc_attach(g_acc_tan + (size_t)blockIdx.x * kTile * (S * 64), S * 64);
     }
-    load_level_consts<D>(lc, P.L, scale, shift, window, tid, kThreads);
+    load_level_consts<D>(lc, P.L, scale, shift, window, tid, kValueThreads);
     __syncthreads();
     if (tid == 0) {
         umma::mbar_expect_tx(&bars[0], (uint32_t)P.g.total);
         umma::bulk_g2s(s_blob, blob, (uint32_t)P.g.total, &bars[0]);
     }
-    const uint32_t tmem_base = 0;
     umma::mbar_wait(&bars[0], 0);
     const int level_cores = P.L / 4;                        // 4 levels x 2 features = one 16-byte core row
     const int all_cores = P.g.Kp[0] / 8;
@@ -120,38 +110,26 @@ k_sdf_fused(FusedParams P, FwdSegs G, const float2* __restrict__ lattice, const 
         const bool valid = n < (seg1 ? G.n[1] : G.n[0]);
         const float* __restrict__ pos = seg1 ? G.pos[1] : G.pos[0];
         float* __restrict__ sdf_out = seg1 ? G.sdf[1] : G.sdf[0];
-        float* __restrict__ grad_out = seg1 ? G.grad[1] : G.grad[0];
         float* __restrict__ geom_out = seg1 ? G.geom[1] : G.geom[0];
         float x[D];
 #pragma unroll
         for (int i = 0; i < D; i++) x[i] = valid ? pos[(size_t)n * D + i] : 0.0f;
 
-        // ---------------- encoder: operand cores grp, grp+4, ... of this row
+        // ---------------- encoder: operand cores grp, grp + 2, ... of this row
         for (int kc = grp; kc < all_cores; kc += kGroups) {
-            float fv[8], ft[3][8];
+            float fv[8];
             if (kc < level_cores) {
 #pragma unroll
                 for (int q = 0; q < 4; q++) {
-                    const int l = kc * 4 + q;
                     Simplex<D> s;
                     float2 v[D + 1];
-                    const float2 a = level_features<D>(x, lc, l, lattice, P.T, P.cap_mask, s, v);
+                    const float2 a = level_features<D>(x, lc, kc * 4 + q, lattice, P.T, P.cap_mask, s, v);
                     fv[2 * q] = a.x; fv[2 * q + 1] = a.y;
-                    if (TAN) {
-                        float2 t[3];
-                        spatial_tangents<D>(s, v, lc->window[l], lc->scale + l * 4, t);
-#pragma unroll
-                        for (int j = 0; j < 3; j++) { ft[j][2 * q] = t[j].x; ft[j][2 * q + 1] = t[j].y; }
-                    }
                 }
             } else {
-                concat_core<TAN ? 3 : 0, D>(P, kc, x, kUnit3, fv, ft);
+                concat_core<0, D>(P, kc, x, nullptr, fv, nullptr);
             }
             store8(s_a, s_a + kATileBytes, row, kc, fv);
-            if (TAN) {
-#pragma unroll
-                for (int j = 0; j < 3; j++) store8(s_a + (1 + j) * 2 * kATileBytes, s_a + (1 + j) * 2 * kATileBytes + kATileBytes, row, kc, ft[j]);
-            }
         }
 
         // ---------------- MLP: 4 dense layers on the tensor cores
@@ -159,98 +137,41 @@ k_sdf_fused(FusedParams P, FwdSegs G, const float2* __restrict__ lattice, const 
         for (int l = 0; l < kNL; l++) {
             umma::fence_async_smem();
             __syncthreads();
-            if constexpr (!TAN) {
-                // value only: warpgroup mh owns rows 64 mh .. 64 mh + 63 from the product to the outputs (see value_rows)
-                const int mh = warp >> 2;
-                float acc[32];
-                value_rows(acc, P.g, l, mh, s_a, s_blob);
-                const float* bias = reinterpret_cast<const float*>(s_blob + P.g.bias[l]);
-                if (l < kNL - 1) {
-                    gelu_to_tiles(acc, bias, P.g.Np[l], mh, s_a);
-                } else {
-                    const int nout = P.g.N[l], n0 = n - row, cnt = seg1 ? G.n[1] : G.n[0];
-#pragma unroll
-                    for (int j = 0; j < 8; j++) {
-#pragma unroll
-                        for (int h = 0; h < 2; h++) {
-#pragma unroll
-                            for (int b = 0; b < 2; b++) {
-                                const int c = frag_col(j) + b, nr = n0 + frag_row(mh, h);
-                                if (c >= nout || nr >= cnt) continue;
-                                const float v = acc[4 * j + 2 * h + b] + bias[c];
-                                if (c == 0) sdf_out[nr] = v;
-                                else if (geom_out) geom_out[(size_t)nr * (nout - 1) + c - 1] = v;
-                            }
-                        }
-                    }
-                }
-                continue;
-            }
-            // value + tangents: warpgroup s issues stream s (both row halves)
-            const int wgi = warp >> 2;
-            for (int mh = 0; mh < 2; mh++)
-                issue_gemm(tmem_base + wgi * 64, mh, s_a + wgi * 2 * kATileBytes, s_a + wgi * 2 * kATileBytes + kATileBytes,
-                           s_blob + P.g.w_hi[l], s_blob + P.g.w_lo[l], P.g.Kp[l], P.g.Np[l]);
-            __syncthreads();
+            // warpgroup mh owns rows 64 mh .. 64 mh + 63 from the product to the outputs (see value_rows)
+            const int mh = warp >> 2;
+            float acc[32];
+            value_rows(acc, P.g, l, mh, s_a, s_blob);
             const float* bias = reinterpret_cast<const float*>(s_blob + P.g.bias[l]);
-            const uint32_t trow = tmem_base + ((uint32_t)((warp & 3) * 32) << 16);
-            const bool last = (l == kNL - 1);
-            for (int c = grp; c < P.g.Np[l] / 16; c += kGroups) {     // this thread's 16-column chunks
-                float z[16], tz[3][16];
-                umma::tmem_ld16(trow + c * 16, z);
-                if (TAN) {
+            if (l < kNL - 1) {
+                gelu_to_tiles(acc, bias, P.g.Np[l], mh, s_a);
+            } else {
+                const int nout = P.g.N[l], n0 = n - row, cnt = seg1 ? G.n[1] : G.n[0];
 #pragma unroll
-                    for (int j = 0; j < 3; j++) umma::tmem_ld16(trow + (1 + j) * 64 + c * 16, tz[j]);
-                }
+                for (int j = 0; j < 8; j++) {
 #pragma unroll
-                for (int i = 0; i < 16; i++) z[i] += bias[c * 16 + i];
-                if (!last) {
+                    for (int h = 0; h < 2; h++) {
 #pragma unroll
-                    for (int i = 0; i < 16; i++) {
-                        const GeluEval ge = gelu_eval(z[i]);
-                        if (TAN) {
-                            const float g1 = fmaf(z[i], ge.pdf, ge.cdf);
-#pragma unroll
-                            for (int j = 0; j < 3; j++) tz[j][i] *= g1;
-                        }
-                        z[i] *= ge.cdf;
-                    }
-                    store8(s_a, s_a + kATileBytes, row, 2 * c, z);
-                    store8(s_a, s_a + kATileBytes, row, 2 * c + 1, z + 8);
-                    if (TAN) {
-#pragma unroll
-                        for (int j = 0; j < 3; j++) {
-                            uint8_t* hi = s_a + (1 + j) * 2 * kATileBytes;
-                            store8(hi, hi + kATileBytes, row, 2 * c, tz[j]);
-                            store8(hi, hi + kATileBytes, row, 2 * c + 1, tz[j] + 8);
-                        }
-                    }
-                } else if (valid) {
-                    const int nout = P.g.N[l];
-                    if (c == 0) {
-                        sdf_out[n] = z[0];
-                        if (TAN && grad_out) { grad_out[(size_t)n * 3] = tz[0][0]; grad_out[(size_t)n * 3 + 1] = tz[1][0]; grad_out[(size_t)n * 3 + 2] = tz[2][0]; }
-                    }
-                    if (geom_out) {
-#pragma unroll
-                        for (int i = 0; i < 16; i++) {
-                            int col = c * 16 + i;
-                            if (col >= 1 && col < nout) geom_out[(size_t)n * (nout - 1) + col - 1] = z[i];
+                        for (int b = 0; b < 2; b++) {
+                            const int c = frag_col(j) + b, nr = n0 + frag_row(mh, h);
+                            if (c >= nout || nr >= cnt) continue;
+                            const float v = acc[4 * j + 2 * h + b] + bias[c];
+                            if (c == 0) sdf_out[nr] = v;
+                            else if (geom_out) geom_out[(size_t)nr * (nout - 1) + c - 1] = v;
                         }
                     }
                 }
             }
         }
-        __syncthreads();   // all accumulator reads of this tile done before the next tile's MMAs overwrite them
+        __syncthreads();   // all reads of this tile's operand tiles done before the next tile's encoder overwrites them
     }
 }
 
 // ---------------------------------------------------------------------------------------------- value + tangents, two groups per CTA
-// The kernel above runs its phases in lock step: all 16 warps gather, then all wait for the tensor core, then all run the epilogue
-// Two CTAs per SM would let one CTA's waits be filled by the other's work, but the operand tiles of four streams (128 KB) + the weight
-// blob (57 KB) allow one. Here ONE CTA holds TWO independent groups of 256 threads, each working on its own 64-sample sub-tile
-// (M = 64 MMAs, 64 KB of operand tiles, its own named barrier and 256 accumulator columns) and sharing the resident weights: the
-// groups drift apart and each one's MMA / barrier / gather waits overlap the other's encoder and epilogue work.
+// A single CTA of 512 threads on 128-sample tiles would run its phases in lock step: all 16 warps gather, then all wait for the tensor
+// core, then all run the epilogue. Two CTAs per SM would let one CTA's waits be filled by the other's work, but the operand tiles of
+// four streams (128 KB) + the weight blob (57 KB) allow one. Here ONE CTA holds TWO independent groups of 256 threads, each working on
+// its own 64-sample sub-tile (M = 64 MMAs, 64 KB of operand tiles, its own named barrier and 256 accumulator columns) and sharing the
+// resident weights: the groups drift apart and each one's MMA / barrier / gather waits overlap the other's encoder and epilogue work.
 // Warpgroup hc of a group forms columns 32 hc .. 32 hc + 31 of all four streams (M = 64, N = 32) and keeps them in registers: the
 // m16n8 fragments are exactly what its epilogue consumes (every thread holds useful values), so these products never leave the SM;
 // the next layer's operand cores are written as 4-byte bf16 pairs.
@@ -752,14 +673,6 @@ int psdf_sdf_mlp_pack_advance(int in_dim, int hidden, int out_dim, const float* 
     return PSDF_OK;
 }
 
-// kernel choice of the value + tangent forward: 1 = two 64-sample groups per CTA (default), 0 = lock-step 128-sample tiles; switchable at
-// run time for tests and A/B measurements (psdf_sdf_forward_variant)
-static int forward_dual_mode = 1;
-int psdf_sdf_forward_variant(int variant) {
-    if (variant == 0 || variant == 1) forward_dual_mode = variant;
-    return forward_dual_mode;
-}
-
 }  // extern "C"
 
 template <int D>
@@ -794,10 +707,8 @@ static int launch_forward(int L, int T, const float* lattice, const float* scale
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     const float2* lat = reinterpret_cast<const float2*>(lattice);
-    // value + tangents: two independent 64-sample groups per CTA (k_sdf_fused_dual) unless psdf_sdf_forward_variant(0) chose the lock-step
-    // kernel, which exists for D = 3 only
-    const bool dual = forward_dual_mode != 0 || D != 3;
-    if (tangents && dual) {
+    if (tangents) {
+        // value + tangents: two independent 64-sample groups per CTA
         FwdSegs H = G;
         int subs = 0;
         for (int i = 0; i < 2; i++) { H.tile0[i] = subs; subs += div_up(G.n[i], kSub); }
@@ -805,16 +716,10 @@ static int launch_forward(int L, int T, const float* lattice, const float* scale
         size_t smem = (size_t)P.g.total + 2 * 4 * 2 * kSubTileBytes + sizeof(LevelC) + 64;
         { static bool optin_[64]; psdf::psdf_optin_smem(k_sdf_fused_dual<D>, 227 * 1024, optin_); }
         k_sdf_fused_dual<D><<<min(min(div_up(subs, 2), sms), kAccCtas), 2 * kGroupThreads, smem, ST>>>(P, H, lat, scale_factor, shift, window, blob);
-    } else if (tangents) {
-        if constexpr (D == 3) {
-            size_t smem = (size_t)P.g.total + 4 * 2 * kATileBytes + sizeof(LevelC) + 64;
-            { static bool optin_[64]; psdf::psdf_optin_smem(k_sdf_fused<true>, 227 * 1024, optin_); }
-            k_sdf_fused<true><<<min(min(tiles, sms), kAccCtas), kFusedThreads, smem, ST>>>(P, G, lat, scale_factor, shift, window, blob);
-        }
     } else {
         size_t smem = (size_t)P.g.total + 2 * kATileBytes + sizeof(LevelC) + 64;
-        { static bool optin_[64]; psdf::psdf_optin_smem(k_sdf_fused<false, D>, 113 * 1024, optin_); }
-        k_sdf_fused<false, D><<<min(min(tiles, 2 * sms), 2 * kAccCtas), kValueThreads, smem, ST>>>(P, G, lat, scale_factor, shift, window, blob);
+        { static bool optin_[64]; psdf::psdf_optin_smem(k_sdf_fused<D>, 113 * 1024, optin_); }
+        k_sdf_fused<D><<<min(min(tiles, 2 * sms), 2 * kAccCtas), kValueThreads, smem, ST>>>(P, G, lat, scale_factor, shift, window, blob);
     }
     PSDF_CHECK_LAUNCH();
     return PSDF_OK;
@@ -843,7 +748,7 @@ int psdf_sdf_fused_forward_multi(int L, int T, const float* lattice, const float
 }
 
 // psdf_sdf_fused_forward at either input width: pos [N, pos_dim], pos_dim 3 (psdf_sdf_fused_forward) or 4 (space-time positions; grad holds
-// the three spatial derivatives). A pos_dim = 4 launch with grad runs the two-group kernel whatever psdf_sdf_forward_variant chose.
+// the three spatial derivatives).
 int psdf_sdf_fused_forward_dim(int pos_dim, int N, int L, int T, const float* pos, const float* lattice, const float* scale_factor,
                                const float* shift, const float* window, float points_scaling, int hidden, int out_dim, const uint8_t* blob,
                                float* sdf, float* grad, float* geom, void* stream) {

@@ -547,9 +547,8 @@ k_sdf_lattice_scatter(FusedParams P, Segments S, const float4* __restrict__ xch,
     }
     const float w = window ? window[l] : 1.0f;
     const float4 a = xch[(size_t)l * xch_stride + slot];
-    const bool aggregate = sc[0] < kAggregateBelowScale && !(P.knockout & 2);      // warp-uniform (l is)
-    const bool do_red = !(P.knockout & 1);            // diagnostics (PSDF_EXPERIMENT_KNOCKOUT): bit 0 no atomics, bit 1 no aggregation
-    scatter_level<true, D>(x, v, sc, sh, w, a.x, a.y, a.z, a.w, valid, aggregate, do_red, lane, P.cap_mask, (unsigned)P.T,
+    const bool aggregate = sc[0] < kAggregateBelowScale;      // warp-uniform (l is)
+    scatter_level<true, D>(x, v, sc, sh, w, a.x, a.y, a.z, a.w, valid, aggregate, lane, P.cap_mask, (unsigned)P.T,
                   grad_lattice + (size_t)l * P.T * 2, fx_lattice ? fx_lattice + (size_t)l * P.T * 2 : nullptr);
 }
 
@@ -583,8 +582,6 @@ static int launch_backward(int nseg, const int* Ns, const float* const* pos, con
     P.in_dim = (L + 2) * 2;
     if (P.in_dim > 64) return PSDF_ERR_UNSUPPORTED;
     P.g = make_geom(P.in_dim, hidden, out_dim);
-    static const int knockout = getenv("PSDF_EXPERIMENT_KNOCKOUT") ? atoi(getenv("PSDF_EXPERIMENT_KNOCKOUT")) : 0;
-    P.knockout = knockout;
     Segments S;
     int tiles = 0, total = 0;
     for (int i = 0; i < kMaxSeg; i++) {

@@ -10,7 +10,6 @@
 //                       the seeds d loss / d {sdf, grad}                                                                             1 for ~15
 //   k_rand_points_u01   Sphere.rand_points_inside from one uniform draw [3,n]                                                          1 for 3
 //   k_adamw_multi       AdamW over several parameter groups in one launch (optim.cu k_adamw per group otherwise)
-#include <cstdlib>
 #include "fused_rgb_common.cuh"
 #include "../../include/psdf_b200.h"
 
@@ -526,15 +525,10 @@ int psdf_adamw_multi_step(int n_groups, const long long* n, const uint64_t* para
     // Persistent grid-stride blocks. leave_room = 0: 8 blocks of 256 threads per SM, 2 float4 quadruples in flight per thread (the
     // fastest sweep on its own). leave_room != 0: 2 blocks per SM with 4 quadruples in flight -- most of the register file stays free, so
     // that the next iteration's ray generation / occupancy sampling kernels, replayed on another stream while this sweep runs
-    // (Trainer._step_graphed), are co-resident instead of waiting for the sweep to drain. PSDF_ADAMW_BLOCKS_PER_SM / PSDF_ADAMW_UNROLL
-    // override both for measurements.
-    static const int per_sm_env = getenv("PSDF_ADAMW_BLOCKS_PER_SM") ? atoi(getenv("PSDF_ADAMW_BLOCKS_PER_SM")) : 0;
-    static const int unroll_env = getenv("PSDF_ADAMW_UNROLL") ? atoi(getenv("PSDF_ADAMW_UNROLL")) : 0;
-    const int per_sm = per_sm_env > 0 ? per_sm_env : (leave_room ? 2 : 8);
-    const int unroll = unroll_env > 0 ? unroll_env : (leave_room ? 4 : 2);
-    const long long blocks = (off + 255) / 256, cap = (long long)sms * per_sm;
+    // (Trainer._step_graphed), are co-resident instead of waiting for the sweep to drain.
+    const long long blocks = (off + 255) / 256, cap = (long long)sms * (leave_room ? 2 : 8);
     const unsigned grid = (unsigned)(blocks < cap ? blocks : cap);
-    if (unroll >= 4) k_adamw_multi<4><<<grid, 256, 0, ST>>>(A, beta1, beta2, eps, step_dev, step_offset, grad_scale);
+    if (leave_room) k_adamw_multi<4><<<grid, 256, 0, ST>>>(A, beta1, beta2, eps, step_dev, step_offset, grad_scale);
     else k_adamw_multi<2><<<grid, 256, 0, ST>>>(A, beta1, beta2, eps, step_dev, step_offset, grad_scale);
     PSDF_CHECK_LAUNCH();
     return PSDF_OK;

@@ -47,19 +47,6 @@ __device__ __forceinline__ void tmem_ld16(uint32_t taddr, float* v) {
 #pragma unroll
     for (int i = 0; i < 4; i++) { const float4 q = p[i]; v[4 * i] = q.x; v[4 * i + 1] = q.y; v[4 * i + 2] = q.z; v[4 * i + 3] = q.w; }
 }
-// 16 lanes x 32 consecutive columns in the layout of an M = 64 accumulator quadrant (rows 16q .. 16q+15 live in lanes
-// 32q .. 32q+15): thread t of the warp gets, for j = 0..3, h = 0..1, b = 0..1,
-//     v[4 j + 2 h + b] = lane (base_lane + t / 4 + 8 h), column (base_col + 8 j + 2 (t % 4) + b)
-// i.e. the m16n8 accumulator fragment repeated over four 8-column blocks
-__device__ __forceinline__ void tmem_ld16x32(uint32_t taddr, float* v) {
-    const int t = threadIdx.x & 31;
-#pragma unroll
-    for (int h = 0; h < 2; h++) {
-        const float* p = acc_ptr((taddr >> 16) + t / 4 + 8 * h, (taddr & 0xffff) + 2 * (t % 4));
-#pragma unroll
-        for (int j = 0; j < 4; j++) { const float2 q = *reinterpret_cast<const float2*>(p + 8 * j); v[4 * j + 2 * h] = q.x; v[4 * j + 2 * h + 1] = q.y; }
-    }
-}
 // store counterpart of tmem_ld16
 __device__ __forceinline__ void tmem_st16(uint32_t taddr, const float* v) {
     float4* p = reinterpret_cast<float4*>(acc_ptr((taddr >> 16) + (threadIdx.x & 31), taddr & 0xffff));
@@ -128,8 +115,9 @@ __device__ __forceinline__ void wgmma_n(float* d, uint64_t a, uint64_t b, uint32
 __device__ __forceinline__ uint32_t frag_lane(int r, bool m64) { return m64 ? (uint32_t)(32 * (r >> 4) + (r & 15)) : (uint32_t)r; }
 
 // The three split products D (+)= A_hi B_hi + A_hi B_lo + A_lo B_hi of one warpgroup's M = 64 x N block, D in its registers in the
-// m16n8 fragment layout (warp w of the warpgroup, lane t: d[4 j + 2 h + b] = row 16 w + t / 4 + 8 h, column 8 j + 2 (t % 4) + b, the
-// layout tmem_ld16x32 returns). Issue only: the caller brackets a batch with wgmma_fence() and wgmma_commit() + wgmma_wait0().
+// m16n8 fragment layout (warp w of the warpgroup, lane t: d[4 j + 2 h + b] = row 16 w + t / 4 + 8 h, column 8 j + 2 (t % 4) + b, i.e.
+// the m16n8 accumulator fragment repeated over the 8-column blocks). Issue only: the caller brackets a batch with wgmma_fence() and
+// wgmma_commit() + wgmma_wait0().
 template <int N, int TA, int TB>
 __device__ __forceinline__ void wg_mma_regs(float* d, uint64_t ah, uint64_t al, uint64_t bh, uint64_t bl, uint32_t a_step, uint32_t b_step,
                                             int ksteps, bool accumulate) {
@@ -241,15 +229,6 @@ __device__ __forceinline__ void bulk_g2s(void* smem_dst, const void* gmem_src, u
                  : "memory");
 }
 
-// 1-D bulk copy shared -> global (TMA store). Bulk groups are per thread: the issuing thread commits and waits.
-__device__ __forceinline__ void bulk_s2g(void* gmem_dst, const void* smem_src, uint32_t bytes) {
-    asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(gmem_dst), "r"(smem_u32(smem_src)), "r"(bytes)
-                 : "memory");
-}
-__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
-__device__ __forceinline__ void bulk_wait_read0() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }   // smem reusable
-__device__ __forceinline__ void bulk_wait0() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }             // writes done
-
 // split a float into bf16 hi + bf16 lo (x ~= hi + lo with ~2^-17 relative error)
 __device__ __forceinline__ void split_bf16(float x, __nv_bfloat16& hi, __nv_bfloat16& lo) {
     hi = __float2bfloat16_rn(x);
@@ -260,9 +239,6 @@ __device__ __forceinline__ void split2_bf16(float x0, float x1, uint32_t& hi, ui
     asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(hi) : "f"(x1), "f"(x0));
     float h0 = __uint_as_float(hi << 16), h1 = __uint_as_float(hi & 0xffff0000u);
     asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(lo) : "f"(x1 - h1), "f"(x0 - h0));
-}
-__device__ __forceinline__ uint32_t pack2(__nv_bfloat16 a, __nv_bfloat16 b) {
-    return (uint32_t)__bfloat16_as_ushort(a) | ((uint32_t)__bfloat16_as_ushort(b) << 16);
 }
 
 }  // namespace umma

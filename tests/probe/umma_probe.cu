@@ -5,7 +5,7 @@
 //   mode 1: D[128 x Kp] = A[128 x Np] * W[Np x Kp] with A K-major and B = the FORWARD weight tile ([Np rows][Kp] K-major along k)
 //           consumed as an MN-major operand (reduction over the rows): the reverse GEMM without a transposed weight copy.
 //   umma_probe_gemm / umma_probe_gemm_tn: self-tests of the descriptor conventions (K-major forward GEMM with the kernels' own split /
-//           pack / issue / load helpers; weight-gradient product with the sample axis as the MMA K dimension, MN-major operands).
+//           pack / load helpers; weight-gradient product with the sample axis as the MMA K dimension, MN-major operands).
 #include "../../permuto_sdf_b200/csrc/fused_common.cuh"
 
 using namespace psdf_fused;
@@ -82,7 +82,20 @@ __global__ void __launch_bounds__(kTile) k_probe(int mode, const float* __restri
     dump_all(dump, 64);
 }
 // ---------------------------------------------------------------------------------------------- debug GEMM (descriptor check)
-// D[128 x N] = A[128 x K] * B[N x K]^T with the same split/pack/issue/load helpers as the fused kernel.
+// rows [64 mh, 64 mh + 64) of D[128 x Np] = A[128 x Kp] W^T as the three split products (one warpgroup, see umma::wg_gemm). A tiles
+// have the 8-row-group stride kSBO_A; the weight tile is [Np rows][Kp] K-major. Descriptor convention checked by
+// tests/test_fused_gpu.py::test_umma_gemm_self_test: the first offset field (LBO) is the stride between core matrices adjacent along K,
+// the second (SBO) between 8-row groups.
+__device__ __forceinline__ void issue_gemm(uint32_t tmem_d, int mh, const uint8_t* a_hi, const uint8_t* a_lo, const uint8_t* w_hi,
+                                           const uint8_t* w_lo, int Kp, int Np) {
+    const uint32_t sbo_w = (Kp / 8) * kLBO;
+    const uint32_t ao = (uint32_t)(mh * 8 * kSBO_A);
+    const uint64_t dah = umma::make_desc(umma::smem_u32(a_hi) + ao, kLBO, kSBO_A), dal = umma::make_desc(umma::smem_u32(a_lo) + ao, kLBO, kSBO_A);
+    const uint64_t dwh = umma::make_desc(umma::smem_u32(w_hi), kLBO, sbo_w), dwl = umma::make_desc(umma::smem_u32(w_lo), kLBO, sbo_w);
+    umma::wg_gemm<0, 0>(tmem_d + ((uint32_t)(64 * mh) << 16), false, dah, dal, dwh, dwl, (2 * kLBO) >> 4, (2 * kLBO) >> 4, (8 * sbo_w) >> 4,
+                        Kp / 16, Np, false);
+}
+// D[128 x N] = A[128 x K] * B[N x K]^T with the same split/pack/load helpers as the fused kernels.
 __global__ void __launch_bounds__(kTile) k_debug_gemm(int N, int K, const float* __restrict__ A, const float* __restrict__ B,
                                                       float* __restrict__ D) {
     extern __shared__ __align__(128) uint8_t smem[];

@@ -25,7 +25,7 @@ def test_header_parses_and_library_exports_every_symbol():
 
 def test_library_identifies_itself():
     lib = _lib.load_library()
-    assert lib.psdf_abi_version() == 1
+    assert lib.psdf_abi_version() == 2
     if not torch.cuda.is_available():
         assert lib.psdf_device_ok() == 0
 

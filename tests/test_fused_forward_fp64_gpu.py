@@ -1,7 +1,6 @@
 """The fused forward kernels against the fp64 reference of the same operations (oracle/backward_fp64.py: *_forward_reference), element
-by element, at the shape limits of every variant: the SDF value + tangent kernels (two-group k_sdf_fused_dual and lock-step
-k_sdf_fused<true>), the value-only kernel (grad NULL, with and without geom), two sample sets in one launch, the sphere tracer, the
-colour network (operand blob packed from normalised matrices and by psdf_lipschitz_pack4) and the background network. The C ABI is
+by element, at the shape limits of every variant: the SDF value + tangent kernel (two-group k_sdf_fused_dual), the value-only
+kernel (grad NULL, with and without geom), two sample sets in one launch, the sphere tracer, the colour network (operand blob packed from normalised matrices and by psdf_lipschitz_pack4) and the background network. The C ABI is
 driven directly, so kernel variants, NULL outputs and sample sets are under the test's control.
 
 Bounds, per output tensor:
@@ -11,8 +10,6 @@ Bounds, per output tensor:
     tests/test_forward_fp64_reference_cpu.py);
   * every output buffer carries guard rows past N filled with a NaN sentinel: they must be unchanged, and rows [0, N) finite.
 `pytest -s` prints the observed per-tensor error and the worst per-element ratio err / (EPS A) of every case."""
-import contextlib
-
 import pytest
 import torch
 
@@ -96,17 +93,6 @@ def check(case, kernel, name, got, ref, A):
                               torch.nonzero(bad.any(0)).reshape(-1).tolist()[:16]))
 
 
-@contextlib.contextmanager
-def lock_step():
-    """the lock-step value + tangent kernel (k_sdf_fused<true>) instead of the two-group one"""
-    from permuto_sdf_b200._lib import call
-    assert call("psdf_sdf_forward_variant", 0) == 0
-    try:
-        yield
-    finally:
-        call("psdf_sdf_forward_variant", 1)
-
-
 # ------------------------------------------------------------------------------------------------ SDF
 def sdf_blob(L, hidden, out_dim, W, b):
     from permuto_sdf_b200._lib import call, load_library
@@ -149,7 +135,7 @@ SDF_CASES = sdf_cases()
 
 @pytest.mark.parametrize("shape,T,N,layout,win", SDF_CASES, ids=["L%d-h%d-o%d-T%d-N%s-%s-%s" % (c[0] + c[1:]) for c in SDF_CASES])
 def test_sdf_forward_matches_fp64(cuda, shape, T, N, layout, win):
-    """value + tangent kernels (two-group and lock-step) and the value-only kernel with and without geom, against one reference"""
+    """value + tangent kernel (two-group) and the value-only kernel with and without geom, against one reference"""
     L, hidden, out_dim = shape
     n = n_spec(N)
     g, lat, shift, W, b = sdf_problem(L, hidden, out_dim, T, seed=L * 1000 + hidden + n % 997)
@@ -159,10 +145,9 @@ def test_sdf_forward_matches_fp64(cuda, shape, T, N, layout, win):
     net = (lat.cuda(), scale.cuda(), shift.cuda(), w.cuda())
     blob = sdf_blob(L, hidden, out_dim, W, b)
     case = "sdf L%d h%d o%d T%d N%d %s %s" % (L, hidden, out_dim, T, n, layout, win)
-    for kernel in ("dual", "lock-step", "value+geom", "value"):
-        tangents, with_geom = kernel in ("dual", "lock-step"), kernel != "value"
-        with lock_step() if kernel == "lock-step" else contextlib.nullcontext():
-            sdf, grad, geom = run_sdf(L, T, net, [(n, pos, tangents, with_geom)], hidden, out_dim, blob)[0]
+    for kernel in ("dual", "value+geom", "value"):
+        tangents, with_geom = kernel == "dual", kernel != "value"
+        sdf, grad, geom = run_sdf(L, T, net, [(n, pos, tangents, with_geom)], hidden, out_dim, blob)[0]
         check(case, kernel, "sdf", sdf, ref["sdf"], ref["A_sdf"])
         if tangents:
             check(case, kernel, "grad", grad, ref["grad"], ref["A_grad"])

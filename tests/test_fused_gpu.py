@@ -286,28 +286,3 @@ def test_fused_kernels_tile_boundaries(cuda, N):
         assert rel(res[True][i], res[False][i]) < 1e-3, i
     for a, b in zip(res[True][4], res[False][4]):
         assert rel(a, b) < 1e-3
-
-
-@pytest.mark.parametrize("n", [1000, 128 * 37 + 5, 65536])
-def test_dual_group_forward_equals_lock_step_forward(cuda, n):
-    """k_sdf_fused_dual (two independent 64-sample groups per CTA, M = 64 MMAs, fragment-layout accumulator loads) against k_sdf_fused<true> (one
-    128-sample tile per CTA): same arithmetic per sample -> identical sdf, gradient and geometric feature"""
-    from permuto_sdf import Sphere
-    from permuto_sdf_b200 import call
-    from permuto_sdf_b200.models import SDF
-    torch.manual_seed(3)
-    m = SDF(3, Sphere(0.5, [0, 0, 0]), 32, 10000, nr_levels=16, capacity=2 ** 18, hidden=64).to("cuda")
-    with torch.no_grad():
-        m.encoding.lattice_values.mul_(1e4)          # default init is 1e-5: make the lattice matter
-    f = m.enable_fused_inference()
-    pos = ((torch.rand(n, 3) - 0.5) * 0.9).cuda()
-    res = {}
-    try:
-        for variant in (0, 1):
-            assert call("psdf_sdf_forward_variant", variant) == variant
-            res[variant] = f(pos, 4000, with_gradient=True)
-    finally:
-        call("psdf_sdf_forward_variant", 1)
-    for a, b in zip(res[0], res[1]):
-        assert torch.isfinite(b).all()
-        assert float((a - b).abs().max()) <= 1e-6 * float(a.abs().max()), float((a - b).abs().max())

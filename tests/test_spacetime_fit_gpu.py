@@ -70,7 +70,7 @@ FWD_CASES = [((24, 32, 1), 2 ** 18, "1", "uniform", "open"), ((4, 16, 1), 5003, 
 
 @pytest.mark.parametrize("shape,T,N,layout,win", FWD_CASES, ids=["L%d-h%d-o%d-T%d-N%s-%s-%s" % (c[0] + c[1:]) for c in FWD_CASES])
 def test_forward_d4_matches_fp64(cuda, shape, T, N, layout, win):
-    """value + spatial tangents (two-group kernel, also when the lock-step variant is selected), value + geom and value only"""
+    """value + spatial tangents (two-group kernel), value + geom and value only"""
     from permuto_sdf_b200._lib import call
     L, hidden, out_dim = shape
     n = n_spec(N)
@@ -81,17 +81,12 @@ def test_forward_d4_matches_fp64(cuda, shape, T, N, layout, win):
     ref_grad, A_grad = ref["grad"][:, :3], ref["A_grad"][:, :3]          # the spatial derivatives
     blob = blob_of(L, hidden, out_dim, W, b)
     case = "sdf4 L%d h%d o%d T%d N%d %s %s" % (L, hidden, out_dim, T, n, layout, win)
-    for kernel in ("dual", "dual (variant 0)", "value+geom", "value"):
-        tangents, with_geom = kernel.startswith("dual"), kernel != "value"
+    for kernel in ("dual", "value+geom", "value"):
+        tangents, with_geom = kernel == "dual", kernel != "value"
         sdf, grad, geom = guarded(n, 0), guarded(n, 3) if tangents else None, guarded(n, out_dim - 1) if with_geom and out_dim > 1 else None
-        if kernel == "dual (variant 0)":
-            assert call("psdf_sdf_forward_variant", 0) == 0
-        try:
-            call("psdf_sdf_fused_forward_dim", 4, n, L, T, cu(pos), lat.cuda(), scale.cuda(), shift.cuda(), w.cuda(), 1e-3, hidden, out_dim,
-                 blob, sdf, grad, geom)
-            torch.cuda.synchronize()
-        finally:
-            call("psdf_sdf_forward_variant", 1)
+        call("psdf_sdf_fused_forward_dim", 4, n, L, T, cu(pos), lat.cuda(), scale.cuda(), shift.cuda(), w.cuda(), 1e-3, hidden, out_dim,
+             blob, sdf, grad, geom)
+        torch.cuda.synchronize()
         fwd_check(case, kernel, "sdf", rows(sdf, n, "sdf"), ref["sdf"], ref["A_sdf"])
         if tangents:
             fwd_check(case, kernel, "grad", rows(grad, n, "grad"), ref_grad, A_grad)

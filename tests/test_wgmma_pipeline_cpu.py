@@ -17,7 +17,7 @@ SERIALIZED = ("C7514", "C7515", "C7520")
 PIPELINED = ["k_sdf_fused_dual<3>", "k_sdf_fused_dual<4>", "k_sdf_fused_backward<3>", "k_sdf_fused_backward<4>", "k_rgb_fused_backward",
              "k_sdf_sphere_trace<3, false>", "k_sdf_sphere_trace<3, true>", "k_sdf_sphere_trace<4, false>", "k_sdf_sphere_trace<4, true>"]
 # value-only and colour-forward kernels that were batched before the kernels above
-ALREADY_BATCHED = ["k_sdf_fused<false, 3>", "k_sdf_fused<false, 4>", "k_sdf_fused<true, 3>", "k_rgb_fused"]
+ALREADY_BATCHED = ["k_sdf_fused<3>", "k_sdf_fused<4>", "k_rgb_fused"]
 
 
 @pytest.fixture(scope="module")
