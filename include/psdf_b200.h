@@ -221,7 +221,10 @@ int psdf_random_rays_from_reel(int nr_rays, int nr_images, int H, int W, const f
 /* ---------------------------------------------------------------- permutohedral_encoding (external package; call sites
  * permuto_sdf_py/models/models.py:149,186; semantics SURVEY.md Appendix B)
  * pos [N,D] fp32, lattice [L,T,F] fp32, scale_factor [L,D], shift [L,D], window [L];
- * out [N,(L+E)*F] with E=ceil(D/F) concat columns when concat_points. D in {3,4}, F == 2. */
+ * out [N,(L+E)*F] with E=ceil(D/F) concat columns (the D coordinates * points_scaling, then zeros) when concat_points.
+ * Supported: D in {2, 3, 4, 5, 6}, F in {1, 2, 4, 8}, 1 <= L <= 32, T >= 1; any other shape returns PSDF_ERR_UNSUPPORTED before the
+ * device is touched. lattice (and grad_lattice) must be F*4-byte aligned, 16-byte for F >= 4 (else PSDF_ERR_ARG). The three entry
+ * points share this contract. */
 int psdf_enc_forward(int N, int D, int L, int F, int T, const float* pos, const float* lattice, const float* scale_factor,
                      const float* shift, const float* window, int concat_points, float points_scaling, float* out, void* stream);
 /* grad wrt lattice (+=, caller zeroes) and/or positions (=) from grad_out [N,(L+E)*F]; either output may be NULL */

@@ -9,15 +9,22 @@
 // residuals, barycentric weights by rank, hash the D-int key of each of the D+1 simplex vertices
 // (h = (h + key_i) * 2531011 over i, mod capacity), blend F features, multiply by the level window.
 //
+// Every kernel is a template on the input width D in {2..6} and the features per level F in {1, 2, 4, 8}; the
+// library instantiates all 20 pairs (with_dim_feat below is the one list of them).
+//
 // Mapping. One thread per sample, all levels in that thread; a warp is 32 consecutive samples,
-// i.e. neighbours on a ray, so on coarse levels the 32 lanes hit the same few 8-byte table rows (L1
-// broadcast) and on fine levels each lane has 4*UNROLL independent gathers in flight against the
-// L2-resident table (L*T*F*4 B = 33.5 MB at L=16 < 50 MB L2). Outputs are staged in shared memory
-// and written as one contiguous [32, C] block per warp. The backward reduces duplicates inside the warp
-// (match_any + segmented shuffle tree) before issuing one red.global.add.v2.f32 per distinct vertex.
+// i.e. neighbours on a ray, so on coarse levels the 32 lanes hit the same few F*4-byte table rows (L1
+// broadcast) and on fine levels each lane has (D+1)*UNROLL independent gathers in flight against the
+// L2-resident table (L*T*F*4 B = 33.5 MB at L=16, F=2 < 50 MB L2). A row is one ld.global.nc of f32, v2 or v4
+// (two v4 at F=8). Outputs are staged in shared memory and written as one contiguous [32, C] block per warp.
+// The backward reduces duplicates inside the warp (match_any + segmented shuffle tree over the F lanes of
+// values) before issuing one red.global.add.{f32,v2.f32,v4.f32} (two v4 at F=8) per distinct vertex.
 // Position gradients need no atomics because a thread owns all levels of its sample.
 #include "common.cuh"
 #include "../../include/psdf_b200.h"
+
+#include <type_traits>
+#include <utility>
 
 using namespace psdf;
 
@@ -33,6 +40,13 @@ struct EncParams {
     float points_scaling;
     unsigned cap_mask;       // floor(2^32 / T): multiplier of the division-free h mod T (see vertex_index)
 };
+
+// Levels in flight per thread (unroll of the level loop): 4 in the forward, 2 in both backward kernels, as at F = 2, except where ptxas
+// spills at that unroll (CUDA 12.9, sm_90a; chosen from its -v report, checked by tests/test_encoding_dims_cpu.py): the forward at
+// (4, 8) and (5, 8), the backward at (6, 2), the double backward at F = 8.
+template <int D, int F> constexpr int kFwdUnroll = (F == 8 && (D == 4 || D == 5)) ? 2 : 4;
+template <int D, int F> constexpr int kBwdUnroll = (D == 6 && F == 2) ? 1 : 2;
+template <int D, int F> constexpr int kDblUnroll = F == 8 ? 1 : 2;
 
 template <int D>
 struct Simplex {
@@ -157,48 +171,106 @@ __device__ __forceinline__ void bary_grad_to_cf(float* dB /* size D+2, dB[D+1] m
     }
 }
 
+// one table row of F floats: its vector type, and one ld.global.nc per 16 bytes (F = 8: two v4)
+struct float8 { float4 lo, hi; };
+template <int F> struct RowOf;
+template <> struct RowOf<1> { using T = float; };
+template <> struct RowOf<2> { using T = float2; };
+template <> struct RowOf<4> { using T = float4; };
+template <> struct RowOf<8> { using T = float8; };
+template <int F> using Row = typename RowOf<F>::T;
+
+template <int F>
+__device__ __forceinline__ void load_row(const Row<F>* p, float (&v)[F]) {
+    if constexpr (F == 1) {
+        v[0] = __ldg(p);
+    } else if constexpr (F == 2) {
+        float2 t = __ldg(p);
+        v[0] = t.x; v[1] = t.y;
+    } else {
+        const float4* q = reinterpret_cast<const float4*>(p);
+#pragma unroll
+        for (int k = 0; k < F / 4; k++) {
+            float4 t = __ldg(q + k);
+            v[4 * k] = t.x; v[4 * k + 1] = t.y; v[4 * k + 2] = t.z; v[4 * k + 3] = t.w;
+        }
+    }
+}
+
+// F floats held in registers, passed by value like the float2 of the F = 2 kernels
+template <int F>
+struct Feat {
+    float v[F];
+};
+// op(0), ..., op(F - 1) as straight-line code (no loop for the optimizer to rotate or unroll late)
+template <typename Op, int... K>
+__device__ __forceinline__ void each_feat(Op&& op, std::integer_sequence<int, K...>) {
+    (op(K), ...);
+}
+template <int F, typename Op>
+__device__ __forceinline__ void each_feat(Op&& op) {
+    each_feat(op, std::make_integer_sequence<int, F>{});
+}
+
 // segmented sum over lanes that share a key (peers mask from __match_any_sync); result valid in the first peer
-__device__ __forceinline__ float2 add_peers(unsigned peers, float2 x, int lane) {
+template <int F>
+__device__ __forceinline__ Feat<F> add_peers(unsigned peers, Feat<F> x, int lane) {
     int rel = __popc(peers << (31 - lane) << 1);  // peers below me
     peers &= (0xfffffffeu << lane);
     while (__any_sync(kFull, peers)) {
         int next = __ffs(peers);
-        float tx = __shfl_sync(kFull, x.x, (next - 1) & 31);
-        float ty = __shfl_sync(kFull, x.y, (next - 1) & 31);
-        if (next) { x.x += tx; x.y += ty; }
+        Feat<F> t;
+        each_feat<F>([&](int k) { t.v[k] = __shfl_sync(kFull, x.v[k], (next - 1) & 31); });
+        if (next) each_feat<F>([&](int k) { x.v[k] += t.v[k]; });
         int done = rel & 1;
         peers &= __ballot_sync(kFull, !done);
         rel >>= 1;
     }
     return x;
 }
-__device__ __forceinline__ void red_add_v2(float* addr, float2 v) {
-    asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(addr), "f"(v.x), "f"(v.y) : "memory");
+// one vector reduction per 16 bytes of the row (F * 4 bytes, 16-byte aligned for F >= 4)
+template <int F>
+__device__ __forceinline__ void red_add(float* addr, Feat<F> x) {
+    if constexpr (F == 1) {
+        asm volatile("red.global.add.f32 [%0], %1;" ::"l"(addr), "f"(x.v[0]) : "memory");
+    } else if constexpr (F == 2) {
+        asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(addr), "f"(x.v[0]), "f"(x.v[1]) : "memory");
+    } else {
+#pragma unroll
+        for (int k = 0; k < F; k += 4)
+            asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(addr + k), "f"(x.v[k]), "f"(x.v[k + 1]), "f"(x.v[k + 2]),
+                         "f"(x.v[k + 3]) : "memory");
+    }
 }
 
+// per-level scale / shift with a fixed stride per level: 4 floats up to D = 4, 8 for D = 5, 6
+template <int D>
 struct LevelConsts {
-    float scale[kMaxLevels * 4];
-    float shift[kMaxLevels * 4];
+    static constexpr int S = D <= 4 ? 4 : 8;
+    float scale[kMaxLevels * S];
+    float shift[kMaxLevels * S];
     float window[kMaxLevels];
 };
 template <int D>
-__device__ __forceinline__ void load_level_consts(LevelConsts& lc, const float* __restrict__ scale,
+__device__ __forceinline__ void load_level_consts(LevelConsts<D>& lc, const float* __restrict__ scale,
                                                   const float* __restrict__ shift, const float* __restrict__ window, int L) {
+    constexpr int S = LevelConsts<D>::S;
     for (int i = threadIdx.x; i < L * D; i += blockDim.x) {
-        lc.scale[(i / D) * 4 + (i % D)] = scale[i];
-        lc.shift[(i / D) * 4 + (i % D)] = shift ? shift[i] : 0.0f;
+        lc.scale[(i / D) * S + (i % D)] = scale[i];
+        lc.shift[(i / D) * S + (i % D)] = shift ? shift[i] : 0.0f;
     }
     for (int i = threadIdx.x; i < L; i += blockDim.x) lc.window[i] = window ? window[i] : 1.0f;
 }
 
 // ------------------------------------------------------------------------------------------------ forward
-template <int D>
+template <int D, int F>
 __global__ void __launch_bounds__(kEncThreads)
-k_enc_forward(EncParams p, const float* __restrict__ pos, const float2* __restrict__ lattice, const float* __restrict__ scale,
+k_enc_forward(EncParams p, const float* __restrict__ pos, const Row<F>* __restrict__ lattice, const float* __restrict__ scale,
               const float* __restrict__ shift, const float* __restrict__ window, float* __restrict__ out) {
     // block = 32 consecutive samples x 4 level groups: warp g handles levels g, g+4, ... of the same 32 samples
+    constexpr int S = LevelConsts<D>::S;
     extern __shared__ float smem_dyn[];
-    __shared__ LevelConsts lc;
+    __shared__ LevelConsts<D> lc;
     load_level_consts<D>(lc, scale, shift, window, p.L);
     __syncthreads();
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -210,31 +282,33 @@ k_enc_forward(EncParams p, const float* __restrict__ pos, const float2* __restri
 #pragma unroll
     for (int i = 0; i < D; i++) x[i] = valid ? pos[(size_t)n * D + i] : 0.0f;
 
-#pragma unroll 4
+#pragma unroll kFwdUnroll<D, F>
     for (int l = warp; l < p.L; l += kGroups) {
         float cf[D], elevated[D + 1];
 #pragma unroll
-        for (int i = 0; i < D; i++) cf[i] = __fmul_rn(__fadd_rn(x[i], lc.shift[l * 4 + i]), lc.scale[l * 4 + i]);
+        for (int i = 0; i < D; i++) cf[i] = __fmul_rn(__fadd_rn(x[i], lc.shift[l * S + i]), lc.scale[l * S + i]);
         elevate<D>(cf, elevated);
         Simplex<D> s;
         locate<D>(elevated, s);
-        const float2* tab = lattice + (size_t)l * p.T;
-        float2 v[D + 1];
+        const Row<F>* tab = lattice + (size_t)l * p.T;
+        float v[D + 1][F];
 #pragma unroll
-        for (int r = 0; r <= D; r++) v[r] = __ldg(tab + vertex_index<D>(s, r, p));
+        for (int r = 0; r <= D; r++) load_row<F>(tab + vertex_index<D>(s, r, p), v[r]);
         float w = lc.window[l];
-        float a0 = 0.0f, a1 = 0.0f;
+        float a[F];
+#pragma unroll
+        for (int k = 0; k < F; k++) a[k] = 0.0f;
 #pragma unroll
         for (int r = 0; r <= D; r++) {
             float wr = s.bary[r] * w;
-            a0 = fmaf(v[r].x, wr, a0);
-            a1 = fmaf(v[r].y, wr, a1);
+#pragma unroll
+            for (int k = 0; k < F; k++) a[k] = fmaf(v[r][k], wr, a[k]);
         }
-        tile[lane * stride + 2 * l] = a0;
-        tile[lane * stride + 2 * l + 1] = a1;
+#pragma unroll
+        for (int k = 0; k < F; k++) tile[lane * stride + F * l + k] = a[k];
     }
     if (p.concat && warp == kGroups - 1) {
-        const int base = 2 * p.L;
+        const int base = F * p.L;
         for (int c = base; c < p.C; c++) {
             int d = c - base;
             float val = 0.0f;
@@ -256,16 +330,17 @@ k_enc_forward(EncParams p, const float* __restrict__ pos, const float2* __restri
 }
 
 // ------------------------------------------------------------------------------------------------ backward
-// grad_lattice[l][idx][:] += window_l * bary_r * g[n][l][:]         (warp aggregated red.v2)
+// grad_lattice[l][idx][:] += window_l * bary_r * g[n][l][:]         (warp aggregated vector red)
 // grad_pos[n][j]          = sum_l window_l * sum_r (val_r . g_l) dB_r/dx_j  (+ concat columns)
-template <int D, bool LATTICE, bool POS>
+template <int D, int F, bool LATTICE, bool POS>
 __global__ void __launch_bounds__(kEncThreads)
-k_enc_backward(EncParams p, const float* __restrict__ pos, const float2* __restrict__ lattice, const float* __restrict__ scale,
+k_enc_backward(EncParams p, const float* __restrict__ pos, const Row<F>* __restrict__ lattice, const float* __restrict__ scale,
                const float* __restrict__ shift, const float* __restrict__ window, const float* __restrict__ grad_out,
                float* __restrict__ grad_lattice, float* __restrict__ grad_pos) {
+    constexpr int S = LevelConsts<D>::S;
     extern __shared__ float smem_dyn[];
-    __shared__ LevelConsts lc;
-    __shared__ float red[kGroups][32][4];
+    __shared__ LevelConsts<D> lc;
+    __shared__ float red[kGroups][32][S];
     load_level_consts<D>(lc, scale, shift, window, p.L);
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int stride = p.C + 1;
@@ -287,43 +362,49 @@ k_enc_backward(EncParams p, const float* __restrict__ pos, const float2* __restr
     for (int i = 0; i < D; i++) { x[i] = valid ? pos[(size_t)n * D + i] : 0.0f; gp[i] = 0.0f; }
     const float* g_row = gtile + lane * stride;
 
-#pragma unroll 2
+#pragma unroll kBwdUnroll<D, F>
     for (int l = warp; l < p.L; l += kGroups) {
         float cf[D], elevated[D + 1];
 #pragma unroll
-        for (int i = 0; i < D; i++) cf[i] = __fmul_rn(__fadd_rn(x[i], lc.shift[l * 4 + i]), lc.scale[l * 4 + i]);
+        for (int i = 0; i < D; i++) cf[i] = __fmul_rn(__fadd_rn(x[i], lc.shift[l * S + i]), lc.scale[l * S + i]);
         elevate<D>(cf, elevated);
         Simplex<D> s;
         locate<D>(elevated, s);
-        float2 g = make_float2(g_row[2 * l], g_row[2 * l + 1]);
+        float g[F];
+        each_feat<F>([&](int k) { g[k] = g_row[F * l + k]; });
         float w = lc.window[l];
         unsigned idx[D + 1];
 #pragma unroll
         for (int r = 0; r <= D; r++) idx[r] = vertex_index<D>(s, r, p);
         if (POS) {
-            const float2* tab = lattice + (size_t)l * p.T;
+            const Row<F>* tab = lattice + (size_t)l * p.T;
             float dB[D + 2];
 #pragma unroll
             for (int r = 0; r <= D; r++) {
-                float2 v = __ldg(tab + idx[r]);
-                dB[r] = w * (v.x * g.x + v.y * g.y);
+                float v[F];
+                load_row<F>(tab + idx[r], v);
+                float dot = v[0] * g[0];
+                each_feat<F - 1>([&](int k) { dot = dot + v[k + 1] * g[k + 1]; });
+                dB[r] = w * dot;
             }
             dB[D + 1] = 0.0f;
             float dcf[D];
             bary_grad_to_cf<D>(dB, s, dcf);
 #pragma unroll
-            for (int i = 0; i < D; i++) gp[i] = fmaf(dcf[i], lc.scale[l * 4 + i], gp[i]);
+            for (int i = 0; i < D; i++) gp[i] = fmaf(dcf[i], lc.scale[l * S + i], gp[i]);
         }
         if (LATTICE) {
-            float* gtab = grad_lattice + (size_t)l * p.T * 2;
+            float* gtab = grad_lattice + (size_t)l * p.T * F;
 #pragma unroll
             for (int r = 0; r <= D; r++) {
                 float wr = s.bary[r] * w;
-                float2 c = make_float2(g.x * wr, g.y * wr);
+                Feat<F> c;
+#pragma unroll
+                for (int k = 0; k < F; k++) c.v[k] = g[k] * wr;
                 unsigned key = valid ? idx[r] : 0xffffffffu;
                 unsigned peers = __match_any_sync(kFull, key);
-                c = add_peers(peers, c, lane);
-                if (valid && lane == __ffs(peers) - 1) red_add_v2(gtab + (size_t)idx[r] * 2, c);
+                c = add_peers<F>(peers, c, lane);
+                if (valid && lane == __ffs(peers) - 1) red_add<F>(gtab + (size_t)idx[r] * F, c);
             }
         }
     }
@@ -338,7 +419,7 @@ k_enc_backward(EncParams p, const float* __restrict__ pos, const float2* __restr
                 float acc = red[0][lane][i];
 #pragma unroll
                 for (int w2 = 1; w2 < kGroups; w2++) acc += red[w2][lane][i];
-                if (p.concat && 2 * p.L + i < p.C) acc = fmaf(g_row[2 * p.L + i], p.points_scaling, acc);
+                if (p.concat && F * p.L + i < p.C) acc = fmaf(g_row[F * p.L + i], p.points_scaling, acc);
                 grad_pos[(size_t)n * D + i] = acc;
             }
         }
@@ -349,14 +430,15 @@ k_enc_backward(EncParams p, const float* __restrict__ pos, const float2* __restr
 // Upstream gradient gg[n][j] flows into grad_pos. With dB_r = sum_j gg_j dB_r/dx_j (tangent of the weights):
 //   grad_lattice[l][idx_r][:] += window_l * dB_r * g[n][l][:]
 //   grad_grad_out[n][l][:]     = window_l * sum_r dB_r * val_r[:]      (concat columns: gg_j * scaling)
-template <int D, bool LATTICE, bool GOUT>
+template <int D, int F, bool LATTICE, bool GOUT>
 __global__ void __launch_bounds__(kEncThreads)
-k_enc_double_backward(EncParams p, const float* __restrict__ pos, const float2* __restrict__ lattice,
+k_enc_double_backward(EncParams p, const float* __restrict__ pos, const Row<F>* __restrict__ lattice,
                       const float* __restrict__ scale, const float* __restrict__ shift, const float* __restrict__ window,
                       const float* __restrict__ gg_pos, const float* __restrict__ grad_out, float* __restrict__ grad_lattice,
                       float* __restrict__ grad_grad_out) {
+    constexpr int S = LevelConsts<D>::S;
     extern __shared__ float smem_dyn[];
-    __shared__ LevelConsts lc;
+    __shared__ LevelConsts<D> lc;
     load_level_consts<D>(lc, scale, shift, window, p.L);
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int stride = p.C + 1;
@@ -380,13 +462,13 @@ k_enc_double_backward(EncParams p, const float* __restrict__ pos, const float2* 
         x[i] = valid ? pos[(size_t)n * D + i] : 0.0f;
         u[i] = valid ? gg_pos[(size_t)n * D + i] : 0.0f;
     }
-#pragma unroll 2
+#pragma unroll kDblUnroll<D, F>
     for (int l = warp; l < p.L; l += kGroups) {
         float cf[D], dcf[D], elevated[D + 1], d_elev[D + 1];
 #pragma unroll
         for (int i = 0; i < D; i++) {
-            cf[i] = __fmul_rn(__fadd_rn(x[i], lc.shift[l * 4 + i]), lc.scale[l * 4 + i]);
-            dcf[i] = u[i] * lc.scale[l * 4 + i];
+            cf[i] = __fmul_rn(__fadd_rn(x[i], lc.shift[l * S + i]), lc.scale[l * S + i]);
+            dcf[i] = u[i] * lc.scale[l * S + i];
         }
         elevate<D>(cf, elevated);
         Simplex<D> s;
@@ -404,35 +486,38 @@ k_enc_double_backward(EncParams p, const float* __restrict__ pos, const float2* 
 #pragma unroll
         for (int r = 0; r <= D; r++) idx[r] = vertex_index<D>(s, r, p);
         if (GOUT) {
-            const float2* tab = lattice + (size_t)l * p.T;
-            float a0 = 0.0f, a1 = 0.0f;
+            const Row<F>* tab = lattice + (size_t)l * p.T;
+            float a[F];
+            each_feat<F>([&](int k) { a[k] = 0.0f; });
 #pragma unroll
             for (int r = 0; r <= D; r++) {
-                float2 v = __ldg(tab + idx[r]);
+                float v[F];
+                load_row<F>(tab + idx[r], v);
                 float c = db[r] * w;
-                a0 = fmaf(v.x, c, a0);
-                a1 = fmaf(v.y, c, a1);
+                each_feat<F>([&](int k) { a[k] = fmaf(v[k], c, a[k]); });
             }
-            otile[lane * stride + 2 * l] = a0;
-            otile[lane * stride + 2 * l + 1] = a1;
+            each_feat<F>([&](int k) { otile[lane * stride + F * l + k] = a[k]; });
         }
         if (LATTICE) {
-            float2 g = make_float2(gtile[lane * stride + 2 * l], gtile[lane * stride + 2 * l + 1]);
-            float* gtab = grad_lattice + (size_t)l * p.T * 2;
+            float g[F];
+            each_feat<F>([&](int k) { g[k] = gtile[lane * stride + F * l + k]; });
+            float* gtab = grad_lattice + (size_t)l * p.T * F;
 #pragma unroll
             for (int r = 0; r <= D; r++) {
                 float c = db[r] * w;
-                float2 cv = make_float2(g.x * c, g.y * c);
+                Feat<F> cv;
+#pragma unroll
+                for (int k = 0; k < F; k++) cv.v[k] = g[k] * c;
                 unsigned key = valid ? idx[r] : 0xffffffffu;
                 unsigned peers = __match_any_sync(kFull, key);
-                cv = add_peers(peers, cv, lane);
-                if (valid && lane == __ffs(peers) - 1) red_add_v2(gtab + (size_t)idx[r] * 2, cv);
+                cv = add_peers<F>(peers, cv, lane);
+                if (valid && lane == __ffs(peers) - 1) red_add<F>(gtab + (size_t)idx[r] * F, cv);
             }
         }
     }
     if (GOUT) {
         if (p.concat && warp == kGroups - 1) {
-            const int base = 2 * p.L;
+            const int base = F * p.L;
             for (int c = base; c < p.C; c++) {
                 int d = c - base;
                 float val = 0.0f;
@@ -451,8 +536,33 @@ k_enc_double_backward(EncParams p, const float* __restrict__ pos, const float2* 
     }
 }
 
+// The (D, F) pairs the library is built for: fn(integral_constant D, integral_constant F) runs for one of them and the call returns
+// true; any other pair returns false without calling fn. This switch is the only list of the supported pairs.
+template <int D, typename Fn>
+inline bool with_feat(int F, Fn&& fn) {
+    using std::integral_constant;
+    switch (F) {
+        case 1: fn(integral_constant<int, D>{}, integral_constant<int, 1>{}); return true;
+        case 2: fn(integral_constant<int, D>{}, integral_constant<int, 2>{}); return true;
+        case 4: fn(integral_constant<int, D>{}, integral_constant<int, 4>{}); return true;
+        case 8: fn(integral_constant<int, D>{}, integral_constant<int, 8>{}); return true;
+        default: return false;
+    }
+}
+template <typename Fn>
+inline bool with_dim_feat(int D, int F, Fn&& fn) {
+    switch (D) {
+        case 2: return with_feat<2>(F, fn);
+        case 3: return with_feat<3>(F, fn);
+        case 4: return with_feat<4>(F, fn);
+        case 5: return with_feat<5>(F, fn);
+        case 6: return with_feat<6>(F, fn);
+        default: return false;
+    }
+}
+
 inline int make_params(EncParams& p, int N, int D, int L, int F, int T, int concat, float points_scaling) {
-    if (F != 2 || (D != 3 && D != 4) || L < 1 || L > kMaxLevels || T < 1) return PSDF_ERR_UNSUPPORTED;
+    if (!with_dim_feat(D, F, [](auto, auto) {}) || L < 1 || L > kMaxLevels || T < 1) return PSDF_ERR_UNSUPPORTED;
     p.N = N; p.L = L; p.T = T;
     int E = concat ? (D + F - 1) / F : 0;
     p.C = (L + E) * F;
@@ -460,6 +570,19 @@ inline int make_params(EncParams& p, int N, int D, int L, int F, int T, int conc
     p.points_scaling = points_scaling;
     p.cap_mask = T <= 1 ? 0xffffffffu : (unsigned)(0x100000000ull / (unsigned long long)(unsigned)T);
     return PSDF_OK;
+}
+// table rows are read and reduced as F * 4-byte vectors (16-byte pieces for F >= 4)
+inline bool rows_aligned(const void* a, int F) { return ((uintptr_t)a % (size_t)(F < 4 ? F * 4 : 16)) == 0; }
+
+// Dynamic shared memory is 32 * (C + 1) floats per staged tile, C = (L + E) * F; at F = 8 and L = 32 the double backward's two tiles
+// take 66 KB. A kernel asked for more than this opts in (once per device) to as much as the device allows beside its static shared
+// memory; smaller launches (every F <= 4 call) leave the kernel's attributes as they are.
+constexpr size_t kSmemOptInAbove = 32 * 1024;
+template <auto Kernel, typename... Args>
+inline void launch(int blocks, size_t smem, cudaStream_t stream, Args... args) {
+    static bool slot[64];
+    if (smem > kSmemOptInAbove) psdf_optin_smem(Kernel, 227 * 1024, slot);
+    Kernel<<<blocks, kEncThreads, smem, stream>>>(args...);
 }
 #define ST ((cudaStream_t)stream)
 }  // namespace
@@ -472,11 +595,13 @@ int psdf_enc_forward(int N, int D, int L, int F, int T, const float* pos, const 
     int rc = make_params(p, N, D, L, F, T, concat_points, points_scaling);
     if (rc) return rc;
     if (N == 0) return PSDF_OK;
+    if (!rows_aligned(lattice, F)) return PSDF_ERR_ARG;
     int blocks = div_up(N, 32);
     size_t smem = (size_t)32 * (p.C + 1) * sizeof(float);
-    const float2* lat = reinterpret_cast<const float2*>(lattice);
-    if (D == 3) k_enc_forward<3><<<blocks, kEncThreads, smem, ST>>>(p, pos, lat, scale_factor, shift, window, out);
-    else k_enc_forward<4><<<blocks, kEncThreads, smem, ST>>>(p, pos, lat, scale_factor, shift, window, out);
+    with_dim_feat(D, F, [&](auto d, auto f) {
+        constexpr int DD = decltype(d)::value, FF = decltype(f)::value;
+        launch<k_enc_forward<DD, FF>>(blocks, smem, ST, p, pos, reinterpret_cast<const Row<FF>*>(lattice), scale_factor, shift, window, out);
+    });
     PSDF_CHECK_LAUNCH();
     return PSDF_OK;
 }
@@ -488,20 +613,19 @@ int psdf_enc_backward(int N, int D, int L, int F, int T, const float* pos, const
     int rc = make_params(p, N, D, L, F, T, concat_points, points_scaling);
     if (rc) return rc;
     if (N == 0 || (!grad_lattice && !grad_pos)) return PSDF_OK;
+    if (!rows_aligned(lattice, F) || !rows_aligned(grad_lattice, F)) return PSDF_ERR_ARG;
     int blocks = div_up(N, 32);
     size_t smem = (size_t)32 * (p.C + 1) * sizeof(float);
-    const float2* lat = reinterpret_cast<const float2*>(lattice);
-#define LAUNCH_BWD(DD, LA, PO) \
-    k_enc_backward<DD, LA, PO><<<blocks, kEncThreads, smem, ST>>>(p, pos, lat, scale_factor, shift, window, grad_out, grad_lattice, grad_pos)
-    if (D == 3) {
-        if (grad_lattice && grad_pos) LAUNCH_BWD(3, true, true);
-        else if (grad_lattice) LAUNCH_BWD(3, true, false);
-        else LAUNCH_BWD(3, false, true);
-    } else {
-        if (grad_lattice && grad_pos) LAUNCH_BWD(4, true, true);
-        else if (grad_lattice) LAUNCH_BWD(4, true, false);
-        else LAUNCH_BWD(4, false, true);
-    }
+    with_dim_feat(D, F, [&](auto d, auto f) {
+        constexpr int DD = decltype(d)::value, FF = decltype(f)::value;
+        const Row<FF>* lat = reinterpret_cast<const Row<FF>*>(lattice);
+#define LAUNCH_BWD(LA, PO) \
+    launch<k_enc_backward<DD, FF, LA, PO>>(blocks, smem, ST, p, pos, lat, scale_factor, shift, window, grad_out, grad_lattice, grad_pos)
+        if (grad_lattice && grad_pos) LAUNCH_BWD(true, true);
+        else if (grad_lattice) LAUNCH_BWD(true, false);
+        else LAUNCH_BWD(false, true);
+#undef LAUNCH_BWD
+    });
     PSDF_CHECK_LAUNCH();
     return PSDF_OK;
 }
@@ -513,21 +637,20 @@ int psdf_enc_double_backward(int N, int D, int L, int F, int T, const float* pos
     int rc = make_params(p, N, D, L, F, T, concat_points, points_scaling);
     if (rc) return rc;
     if (N == 0 || (!grad_lattice && !grad_grad_out)) return PSDF_OK;
+    if (!rows_aligned(lattice, F) || !rows_aligned(grad_lattice, F)) return PSDF_ERR_ARG;
     int blocks = div_up(N, 32);
     size_t smem = (size_t)2 * 32 * (p.C + 1) * sizeof(float);
-    const float2* lat = reinterpret_cast<const float2*>(lattice);
-#define LAUNCH_DBL(DD, LA, GO)                                                                                                  \
-    k_enc_double_backward<DD, LA, GO><<<blocks, kEncThreads, smem, ST>>>(p, pos, lat, scale_factor, shift, window, gg_pos, grad_out, \
-                                                                     grad_lattice, grad_grad_out)
-    if (D == 3) {
-        if (grad_lattice && grad_grad_out) LAUNCH_DBL(3, true, true);
-        else if (grad_lattice) LAUNCH_DBL(3, true, false);
-        else LAUNCH_DBL(3, false, true);
-    } else {
-        if (grad_lattice && grad_grad_out) LAUNCH_DBL(4, true, true);
-        else if (grad_lattice) LAUNCH_DBL(4, true, false);
-        else LAUNCH_DBL(4, false, true);
-    }
+    with_dim_feat(D, F, [&](auto d, auto f) {
+        constexpr int DD = decltype(d)::value, FF = decltype(f)::value;
+        const Row<FF>* lat = reinterpret_cast<const Row<FF>*>(lattice);
+#define LAUNCH_DBL(LA, GO)                                                                                                         \
+    launch<k_enc_double_backward<DD, FF, LA, GO>>(blocks, smem, ST, p, pos, lat, scale_factor, shift, window, gg_pos, grad_out, grad_lattice, \
+                                                  grad_grad_out)
+        if (grad_lattice && grad_grad_out) LAUNCH_DBL(true, true);
+        else if (grad_lattice) LAUNCH_DBL(true, false);
+        else LAUNCH_DBL(false, true);
+#undef LAUNCH_DBL
+    });
     PSDF_CHECK_LAUNCH();
     return PSDF_OK;
 }

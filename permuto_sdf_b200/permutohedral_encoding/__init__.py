@@ -19,13 +19,23 @@ def _enc_consts(mod):
     return (mod.pos_dim, mod.nr_levels, mod.nr_feat_per_level, mod.capacity)
 
 
+def _enc_call(name, mod, *args):
+    """one encoding entry point of the library; its refusal (e.g. a (pos_dim, nr_feat_per_level) pair it has no kernel for) is raised
+    with the module's shape, so the supported set is stated in one place only: the library"""
+    try:
+        return call(name, *args)
+    except RuntimeError as e:
+        raise RuntimeError("PermutoEncoding(pos_dim=%d, nr_feat_per_level=%d, nr_levels=%d, capacity=%d): %s" %
+                           (mod.pos_dim, mod.nr_feat_per_level, mod.nr_levels, mod.capacity, e)) from e
+
+
 class _EncodeFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, lattice, positions, window, mod):
         D, L, F, T = _enc_consts(mod)
         N = positions.shape[0]
         out = torch.empty(N, mod.output_dims(), device=positions.device, dtype=torch.float32)
-        call("psdf_enc_forward", N, D, L, F, T, positions, lattice, mod.scale_factor, mod.shift_tensor(), window,
+        _enc_call("psdf_enc_forward", mod, N, D, L, F, T, positions, lattice, mod.scale_factor, mod.shift_tensor(), window,
              1 if mod.concat_points else 0, mod.concat_points_scaling, out)
         ctx.mod = mod
         ctx.save_for_backward(lattice, positions, window)
@@ -55,7 +65,7 @@ class _EncodeBackFn(torch.autograd.Function):
             lattice.grad.is_contiguous()
         g_l = (lattice.grad if in_place else torch.zeros_like(lattice)) if need_l else None
         g_p = torch.empty_like(positions) if need_p else None
-        call("psdf_enc_backward", N, D, L, F, T, positions, lattice, mod.scale_factor, mod.shift_tensor(), window,
+        _enc_call("psdf_enc_backward", mod, N, D, L, F, T, positions, lattice, mod.scale_factor, mod.shift_tensor(), window,
              1 if mod.concat_points else 0, mod.concat_points_scaling, grad_out, g_l, g_p)
         ctx.mod = mod
         ctx.save_for_backward(lattice, positions, window, grad_out)
@@ -79,7 +89,7 @@ class _EncodeBackFn(torch.autograd.Function):
         if gg_pos is not None and (need_l or need_go):
             g_l = torch.zeros_like(lattice) if need_l else None
             g_go = torch.empty_like(grad_out) if need_go else None
-            call("psdf_enc_double_backward", N, D, L, F, T, positions, lattice, mod.scale_factor, mod.shift_tensor(), window,
+            _enc_call("psdf_enc_double_backward", mod, N, D, L, F, T, positions, lattice, mod.scale_factor, mod.shift_tensor(), window,
                  1 if mod.concat_points else 0, mod.concat_points_scaling, gg_pos.contiguous(), grad_out, g_l, g_go)
         return g_l, None, None, g_go, None, None, None, None
 
