@@ -223,8 +223,8 @@ int psdf_random_rays_from_reel(int nr_rays, int nr_images, int H, int W, const f
  * pos [N,D] fp32, lattice [L,T,F] fp32, scale_factor [L,D], shift [L,D], window [L];
  * out [N,(L+E)*F] with E=ceil(D/F) concat columns (the D coordinates * points_scaling, then zeros) when concat_points.
  * Supported: D in {2, 3, 4, 5, 6}, F in {1, 2, 4, 8}, 1 <= L <= 32, T >= 1; any other shape returns PSDF_ERR_UNSUPPORTED before the
- * device is touched. lattice (and grad_lattice) must be F*4-byte aligned, 16-byte for F >= 4 (else PSDF_ERR_ARG). The three entry
- * points share this contract. */
+ * device is touched. lattice (and grad_lattice) must be F*4-byte aligned, 16-byte for F >= 4 (else PSDF_ERR_ARG). The five entry
+ * points below share this contract. */
 int psdf_enc_forward(int N, int D, int L, int F, int T, const float* pos, const float* lattice, const float* scale_factor,
                      const float* shift, const float* window, int concat_points, float points_scaling, float* out, void* stream);
 /* grad wrt lattice (+=, caller zeroes) and/or positions (=) from grad_out [N,(L+E)*F]; either output may be NULL */
@@ -236,6 +236,19 @@ int psdf_enc_backward(int N, int D, int L, int F, int T, const float* pos, const
 int psdf_enc_double_backward(int N, int D, int L, int F, int T, const float* pos, const float* lattice, const float* scale_factor,
                              const float* shift, const float* window, int concat_points, float points_scaling,
                              const float* gg_pos, const float* grad_out, float* grad_lattice, float* grad_grad_out, void* stream);
+/* Deterministic twins of psdf_enc_backward and psdf_enc_double_backward: the same outputs, except that the lattice gradient is
+ * reduced in 64-bit fixed point (2^-34 grid, the unit of psdf_set_deterministic). Every contribution is rounded to the grid before
+ * anything is added to it, so grad_lattice depends only on the multiset of (pos, grad_out[, gg_pos]) rows, not on their order or the
+ * run. grad_pos and grad_grad_out are bit-identical to the float entry points'. fx_lattice: caller-owned [L,T,F] accumulators, 8-byte
+ * aligned, zero on entry and zero again on return (the totals are added to grad_lattice, +=, and cleared); the library never
+ * allocates. grad_lattice NULL: exactly the float entry point, fx_lattice ignored. grad_lattice without fx_lattice: PSDF_ERR_ARG. */
+int psdf_enc_backward_fx(int N, int D, int L, int F, int T, const float* pos, const float* lattice, const float* scale_factor,
+                         const float* shift, const float* window, int concat_points, float points_scaling, const float* grad_out,
+                         float* grad_lattice, float* grad_pos, uint64_t* fx_lattice, void* stream);
+int psdf_enc_double_backward_fx(int N, int D, int L, int F, int T, const float* pos, const float* lattice, const float* scale_factor,
+                                const float* shift, const float* window, int concat_points, float points_scaling,
+                                const float* gg_pos, const float* grad_out, float* grad_lattice, float* grad_grad_out,
+                                uint64_t* fx_lattice, void* stream);
 
 /* ---------------------------------------------------------------- fused encoding + SDF MLP (wgmma)
  * Replaces SDF.forward / SDF.get_sdf_and_gradient of permuto_sdf_py/models/models.py:176-259 for evaluations that

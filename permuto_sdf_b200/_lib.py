@@ -176,7 +176,10 @@ _KERNELS_PER_CALL = {"psdf_packed_compact_scan": 2, "psdf_vr_combine_uniform_sam
                      "psdf_bg_fused_backward": 2, "psdf_nerf_fused_backward": 2}
 
 
-_KERNELS_FN = {}        # entry point -> launches as a function of its arguments (none at present)
+# entry point -> launches as a function of its arguments: the deterministic encoding backward adds the fixed-point flush when it has a
+# lattice output
+_KERNELS_FN = {"psdf_enc_backward_fx": lambda a: 2 if a[13] is not None else 1,
+               "psdf_enc_double_backward_fx": lambda a: 2 if a[14] is not None else 1}
 _UNITS_FN = {"psdf_sdf_fused_forward_multi": lambda a: int(a[10]) + int(a[15]),
              "psdf_sdf_fused_forward_dim": lambda a: int(a[1]),
              "psdf_sdf_sphere_trace_dim": lambda a: int(a[4]),

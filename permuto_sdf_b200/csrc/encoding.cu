@@ -20,6 +20,13 @@
 // The backward reduces duplicates inside the warp (match_any + segmented shuffle tree over the F lanes of
 // values) before issuing one red.global.add.{f32,v2.f32,v4.f32} (two v4 at F=8) per distinct vertex.
 // Position gradients need no atomics because a thread owns all levels of its sample.
+//
+// Deterministic variants (k_fx_enc_backward, k_fx_enc_double_backward): the same kernels with the lattice scatter in 64-bit fixed
+// point. Each contribution is rounded to the 2^-34 grid (fx_of) before anything is added to it; the peers' integers are summed with
+// 64-bit shuffles and one red.global.add.u64 per feature and distinct vertex adds them to caller-owned accumulators, which k_fx_flush
+// adds to the float table and clears. Integer addition is associative, so the lattice gradient depends only on the multiset of
+// (position, upstream gradient) rows, not on their order, the warp layout or the run. The float kernels are left as they are: these are
+// separate kernels rather than a template parameter of them, so the float kernels keep their names and their SASS.
 #include "common.cuh"
 #include "../../include/psdf_b200.h"
 
@@ -47,6 +54,10 @@ struct EncParams {
 template <int D, int F> constexpr int kFwdUnroll = (F == 8 && (D == 4 || D == 5)) ? 2 : 4;
 template <int D, int F> constexpr int kBwdUnroll = (D == 6 && F == 2) ? 1 : 2;
 template <int D, int F> constexpr int kDblUnroll = F == 8 ? 1 : 2;
+// The fixed-point variants hold F 64-bit partial sums per vertex in the peer reduction; lowered from 2 to 1 where ptxas spills at 2: the
+// backward at (3, 1), (3, 2), (4, 2) and (6, 2), the double backward at F >= 4 and at (5, 2).
+template <int D, int F> constexpr int kFxBwdUnroll = ((D == 3 && F <= 2) || (D == 4 && F == 2) || (D == 6 && F == 2)) ? 1 : 2;
+template <int D, int F> constexpr int kFxDblUnroll = (F >= 4 || (D == 5 && F == 2)) ? 1 : 2;
 
 template <int D>
 struct Simplex {
@@ -227,6 +238,41 @@ __device__ __forceinline__ Feat<F> add_peers(unsigned peers, Feat<F> x, int lane
         rel >>= 1;
     }
     return x;
+}
+// F fixed-point values (fx_of) held in registers
+template <int F>
+struct FeatFx {
+    unsigned long long v[F];
+};
+// add_peers on integers: wrap-around addition is exact and associative, so the sums do not depend on the order of the peers
+template <int F>
+__device__ __forceinline__ FeatFx<F> add_peers(unsigned peers, FeatFx<F> x, int lane) {
+    int rel = __popc(peers << (31 - lane) << 1);
+    peers &= (0xfffffffeu << lane);
+    while (__any_sync(kFull, peers)) {
+        int next = __ffs(peers);
+        FeatFx<F> t;
+        each_feat<F>([&](int k) { t.v[k] = __shfl_sync(kFull, x.v[k], (next - 1) & 31); });
+        if (next) each_feat<F>([&](int k) { x.v[k] += t.v[k]; });
+        int done = rel & 1;
+        peers &= __ballot_sync(kFull, !done);
+        rel >>= 1;
+    }
+    return x;
+}
+// the contributions c of this lane's sample (valid) to row idx of one level's accumulators: rounded to fixed point, summed over the
+// lanes that share the row, added by the first of them with F scalar reductions (PTX has no vector u64 red)
+template <int F>
+__device__ __forceinline__ void scatter_row_fx(unsigned long long* acc, unsigned idx, bool valid, const Feat<F>& c, int lane) {
+    FeatFx<F> q;
+    each_feat<F>([&](int k) { q.v[k] = fx_of(c.v[k]); });
+    unsigned key = valid ? idx : 0xffffffffu;
+    unsigned peers = __match_any_sync(kFull, key);
+    q = add_peers<F>(peers, q, lane);
+    if (valid && lane == __ffs(peers) - 1) {
+        unsigned long long* row = acc + (size_t)idx * F;
+        each_feat<F>([&](int k) { asm volatile("red.global.add.u64 [%0], %1;" ::"l"(row + k), "l"(q.v[k]) : "memory"); });
+    }
 }
 // one vector reduction per 16 bytes of the row (F * 4 bytes, 16-byte aligned for F >= 4)
 template <int F>
@@ -426,6 +472,96 @@ k_enc_backward(EncParams p, const float* __restrict__ pos, const Row<F>* __restr
     }
 }
 
+// the backward with the lattice gradient in fixed point: k_enc_backward<D, F, true, POS> with the scatter into the accumulators fx
+// [L, T, F] (scatter_row_fx); grad_pos is formed by the same operations, so it is the float kernel's bit for bit
+template <int D, int F, bool POS>
+__global__ void __launch_bounds__(kEncThreads)
+k_fx_enc_backward(EncParams p, const float* __restrict__ pos, const Row<F>* __restrict__ lattice, const float* __restrict__ scale,
+                  const float* __restrict__ shift, const float* __restrict__ window, const float* __restrict__ grad_out,
+                  unsigned long long* __restrict__ fx, float* __restrict__ grad_pos) {
+    constexpr int S = LevelConsts<D>::S;
+    extern __shared__ float smem_dyn[];
+    __shared__ LevelConsts<D> lc;
+    __shared__ float red[kGroups][32][S];
+    load_level_consts<D>(lc, scale, shift, window, p.L);
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int stride = p.C + 1;
+    float* gtile = smem_dyn;
+    const int row0 = blockIdx.x * 32;
+    {
+        const int rows = min(32, p.N - row0);
+        const float* src = grad_out + (size_t)row0 * p.C;
+        for (int e = threadIdx.x; e < 32 * p.C; e += kEncThreads) {
+            int r = e / p.C, c = e - r * p.C;
+            gtile[r * stride + c] = (r < rows) ? src[e] : 0.0f;
+        }
+    }
+    __syncthreads();
+    const int n = row0 + lane;
+    const bool valid = n < p.N;
+    float x[D], gp[D];
+#pragma unroll
+    for (int i = 0; i < D; i++) { x[i] = valid ? pos[(size_t)n * D + i] : 0.0f; gp[i] = 0.0f; }
+    const float* g_row = gtile + lane * stride;
+
+#pragma unroll kFxBwdUnroll<D, F>
+    for (int l = warp; l < p.L; l += kGroups) {
+        float cf[D], elevated[D + 1];
+#pragma unroll
+        for (int i = 0; i < D; i++) cf[i] = __fmul_rn(__fadd_rn(x[i], lc.shift[l * S + i]), lc.scale[l * S + i]);
+        elevate<D>(cf, elevated);
+        Simplex<D> s;
+        locate<D>(elevated, s);
+        float g[F];
+        each_feat<F>([&](int k) { g[k] = g_row[F * l + k]; });
+        float w = lc.window[l];
+        unsigned idx[D + 1];
+#pragma unroll
+        for (int r = 0; r <= D; r++) idx[r] = vertex_index<D>(s, r, p);
+        if (POS) {
+            const Row<F>* tab = lattice + (size_t)l * p.T;
+            float dB[D + 2];
+#pragma unroll
+            for (int r = 0; r <= D; r++) {
+                float v[F];
+                load_row<F>(tab + idx[r], v);
+                float dot = v[0] * g[0];
+                each_feat<F - 1>([&](int k) { dot = dot + v[k + 1] * g[k + 1]; });
+                dB[r] = w * dot;
+            }
+            dB[D + 1] = 0.0f;
+            float dcf[D];
+            bary_grad_to_cf<D>(dB, s, dcf);
+#pragma unroll
+            for (int i = 0; i < D; i++) gp[i] = fmaf(dcf[i], lc.scale[l * S + i], gp[i]);
+        }
+        unsigned long long* acc = fx + (size_t)l * p.T * F;
+#pragma unroll
+        for (int r = 0; r <= D; r++) {
+            float wr = s.bary[r] * w;
+            Feat<F> c;
+#pragma unroll
+            for (int k = 0; k < F; k++) c.v[k] = g[k] * wr;
+            scatter_row_fx<F>(acc, idx[r], valid, c, lane);
+        }
+    }
+    if (POS) {
+#pragma unroll
+        for (int i = 0; i < D; i++) red[warp][lane][i] = gp[i];
+        __syncthreads();
+        if (warp == 0 && valid) {
+#pragma unroll
+            for (int i = 0; i < D; i++) {
+                float acc = red[0][lane][i];
+#pragma unroll
+                for (int w2 = 1; w2 < kGroups; w2++) acc += red[w2][lane][i];
+                if (p.concat && F * p.L + i < p.C) acc = fmaf(g_row[F * p.L + i], p.points_scaling, acc);
+                grad_pos[(size_t)n * D + i] = acc;
+            }
+        }
+    }
+}
+
 // ------------------------------------------------------------------------------------------------ double backward
 // Upstream gradient gg[n][j] flows into grad_pos. With dB_r = sum_j gg_j dB_r/dx_j (tangent of the weights):
 //   grad_lattice[l][idx_r][:] += window_l * dB_r * g[n][l][:]
@@ -513,6 +649,109 @@ k_enc_double_backward(EncParams p, const float* __restrict__ pos, const Row<F>* 
                 cv = add_peers<F>(peers, cv, lane);
                 if (valid && lane == __ffs(peers) - 1) red_add<F>(gtab + (size_t)idx[r] * F, cv);
             }
+        }
+    }
+    if (GOUT) {
+        if (p.concat && warp == kGroups - 1) {
+            const int base = F * p.L;
+            for (int c = base; c < p.C; c++) {
+                int d = c - base;
+                float val = 0.0f;
+#pragma unroll
+                for (int i = 0; i < D; i++) if (i == d) val = u[i] * p.points_scaling;
+                otile[lane * stride + c] = val;
+            }
+        }
+        __syncthreads();
+        float* dst = grad_grad_out + (size_t)row0 * p.C;
+        const int total = rows * p.C;
+        for (int e = threadIdx.x; e < total; e += kEncThreads) {
+            int r = e / p.C, c = e - r * p.C;
+            dst[e] = otile[r * stride + c];
+        }
+    }
+}
+
+// the double backward with the lattice term in fixed point: k_enc_double_backward<D, F, true, GOUT> with the scatter into the
+// accumulators fx [L, T, F]; grad_grad_out is formed by the same operations, so it is the float kernel's bit for bit
+template <int D, int F, bool GOUT>
+__global__ void __launch_bounds__(kEncThreads)
+k_fx_enc_double_backward(EncParams p, const float* __restrict__ pos, const Row<F>* __restrict__ lattice,
+                         const float* __restrict__ scale, const float* __restrict__ shift, const float* __restrict__ window,
+                         const float* __restrict__ gg_pos, const float* __restrict__ grad_out, unsigned long long* __restrict__ fx,
+                         float* __restrict__ grad_grad_out) {
+    constexpr int S = LevelConsts<D>::S;
+    extern __shared__ float smem_dyn[];
+    __shared__ LevelConsts<D> lc;
+    load_level_consts<D>(lc, scale, shift, window, p.L);
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int stride = p.C + 1;
+    float* gtile = smem_dyn;
+    float* otile = smem_dyn + 32 * stride;
+    const int row0 = blockIdx.x * 32;
+    const int rows = min(32, p.N - row0);
+    {
+        const float* src = grad_out + (size_t)row0 * p.C;
+        for (int e = threadIdx.x; e < 32 * p.C; e += kEncThreads) {
+            int r = e / p.C, c = e - r * p.C;
+            gtile[r * stride + c] = (r < rows) ? src[e] : 0.0f;
+        }
+    }
+    __syncthreads();
+    const int n = row0 + lane;
+    const bool valid = n < p.N;
+    float x[D], u[D];
+#pragma unroll
+    for (int i = 0; i < D; i++) {
+        x[i] = valid ? pos[(size_t)n * D + i] : 0.0f;
+        u[i] = valid ? gg_pos[(size_t)n * D + i] : 0.0f;
+    }
+#pragma unroll kFxDblUnroll<D, F>
+    for (int l = warp; l < p.L; l += kGroups) {
+        float cf[D], dcf[D], elevated[D + 1], d_elev[D + 1];
+#pragma unroll
+        for (int i = 0; i < D; i++) {
+            cf[i] = __fmul_rn(__fadd_rn(x[i], lc.shift[l * S + i]), lc.scale[l * S + i]);
+            dcf[i] = u[i] * lc.scale[l * S + i];
+        }
+        elevate<D>(cf, elevated);
+        Simplex<D> s;
+        locate<D>(elevated, s);
+        {
+            float sm = 0.0f;
+#pragma unroll
+            for (int i = D; i > 0; i--) { d_elev[i] = sm - (float)i * dcf[i - 1]; sm += dcf[i - 1]; }
+            d_elev[0] = sm;
+        }
+        float db[D + 2];
+        bary_tangent<D>(d_elev, s, db);
+        float w = lc.window[l];
+        unsigned idx[D + 1];
+#pragma unroll
+        for (int r = 0; r <= D; r++) idx[r] = vertex_index<D>(s, r, p);
+        if (GOUT) {
+            const Row<F>* tab = lattice + (size_t)l * p.T;
+            float a[F];
+            each_feat<F>([&](int k) { a[k] = 0.0f; });
+#pragma unroll
+            for (int r = 0; r <= D; r++) {
+                float v[F];
+                load_row<F>(tab + idx[r], v);
+                float c = db[r] * w;
+                each_feat<F>([&](int k) { a[k] = fmaf(v[k], c, a[k]); });
+            }
+            each_feat<F>([&](int k) { otile[lane * stride + F * l + k] = a[k]; });
+        }
+        float g[F];
+        each_feat<F>([&](int k) { g[k] = gtile[lane * stride + F * l + k]; });
+        unsigned long long* acc = fx + (size_t)l * p.T * F;
+#pragma unroll
+        for (int r = 0; r <= D; r++) {
+            float c = db[r] * w;
+            Feat<F> cv;
+#pragma unroll
+            for (int k = 0; k < F; k++) cv.v[k] = g[k] * c;
+            scatter_row_fx<F>(acc, idx[r], valid, cv, lane);
         }
     }
     if (GOUT) {
@@ -653,6 +892,71 @@ int psdf_enc_double_backward(int N, int D, int L, int F, int T, const float* pos
     });
     PSDF_CHECK_LAUNCH();
     return PSDF_OK;
+}
+
+// The deterministic twins: the lattice gradient is summed in the caller's zeroed fixed-point accumulators fx_lattice [L, T, F], then
+// k_fx_flush adds the totals to grad_lattice and clears the accumulators again. Without grad_lattice they are the float entry points.
+static int fx_flush_lattice(unsigned long long* fx, float* grad_lattice, const EncParams& p, int F, cudaStream_t stream) {
+    FxSegs S;
+    S.add(fx, grad_lattice, (long long)p.L * p.T * F);
+    return fx_flush(S, stream) ? PSDF_ERR_LAUNCH : PSDF_OK;
+}
+
+int psdf_enc_backward_fx(int N, int D, int L, int F, int T, const float* pos, const float* lattice, const float* scale_factor,
+                         const float* shift, const float* window, int concat_points, float points_scaling, const float* grad_out,
+                         float* grad_lattice, float* grad_pos, uint64_t* fx_lattice, void* stream) {
+    if (!grad_lattice)
+        return psdf_enc_backward(N, D, L, F, T, pos, lattice, scale_factor, shift, window, concat_points, points_scaling, grad_out,
+                                 nullptr, grad_pos, stream);
+    EncParams p;
+    int rc = make_params(p, N, D, L, F, T, concat_points, points_scaling);
+    if (rc) return rc;
+    if (!fx_lattice || (uintptr_t)fx_lattice % 8) return PSDF_ERR_ARG;
+    if (N == 0) return PSDF_OK;
+    if (!rows_aligned(lattice, F) || !rows_aligned(grad_lattice, F)) return PSDF_ERR_ARG;
+    unsigned long long* fx = reinterpret_cast<unsigned long long*>(fx_lattice);
+    int blocks = div_up(N, 32);
+    size_t smem = (size_t)32 * (p.C + 1) * sizeof(float);
+    with_dim_feat(D, F, [&](auto d, auto f) {
+        constexpr int DD = decltype(d)::value, FF = decltype(f)::value;
+        const Row<FF>* lat = reinterpret_cast<const Row<FF>*>(lattice);
+#define LAUNCH_FX_BWD(PO) \
+    launch<k_fx_enc_backward<DD, FF, PO>>(blocks, smem, ST, p, pos, lat, scale_factor, shift, window, grad_out, fx, grad_pos)
+        if (grad_pos) LAUNCH_FX_BWD(true);
+        else LAUNCH_FX_BWD(false);
+#undef LAUNCH_FX_BWD
+    });
+    PSDF_CHECK_LAUNCH();
+    return fx_flush_lattice(fx, grad_lattice, p, F, ST);
+}
+
+int psdf_enc_double_backward_fx(int N, int D, int L, int F, int T, const float* pos, const float* lattice, const float* scale_factor,
+                                const float* shift, const float* window, int concat_points, float points_scaling,
+                                const float* gg_pos, const float* grad_out, float* grad_lattice, float* grad_grad_out,
+                                uint64_t* fx_lattice, void* stream) {
+    if (!grad_lattice)
+        return psdf_enc_double_backward(N, D, L, F, T, pos, lattice, scale_factor, shift, window, concat_points, points_scaling, gg_pos,
+                                        grad_out, nullptr, grad_grad_out, stream);
+    EncParams p;
+    int rc = make_params(p, N, D, L, F, T, concat_points, points_scaling);
+    if (rc) return rc;
+    if (!fx_lattice || (uintptr_t)fx_lattice % 8) return PSDF_ERR_ARG;
+    if (N == 0) return PSDF_OK;
+    if (!rows_aligned(lattice, F) || !rows_aligned(grad_lattice, F)) return PSDF_ERR_ARG;
+    unsigned long long* fx = reinterpret_cast<unsigned long long*>(fx_lattice);
+    int blocks = div_up(N, 32);
+    size_t smem = (size_t)2 * 32 * (p.C + 1) * sizeof(float);
+    with_dim_feat(D, F, [&](auto d, auto f) {
+        constexpr int DD = decltype(d)::value, FF = decltype(f)::value;
+        const Row<FF>* lat = reinterpret_cast<const Row<FF>*>(lattice);
+#define LAUNCH_FX_DBL(GO) \
+    launch<k_fx_enc_double_backward<DD, FF, GO>>(blocks, smem, ST, p, pos, lat, scale_factor, shift, window, gg_pos, grad_out, fx, grad_grad_out)
+        if (grad_grad_out) LAUNCH_FX_DBL(true);
+        else LAUNCH_FX_DBL(false);
+#undef LAUNCH_FX_DBL
+    });
+    PSDF_CHECK_LAUNCH();
+    return fx_flush_lattice(fx, grad_lattice, p, F, ST);
 }
 
 int psdf_abi_version(void) { return PSDF_ABI_VERSION; }

@@ -1,7 +1,8 @@
 """Drop-in replacement of the external `permutohedral_encoding` package the reference imports
 (permuto_sdf_py/models/models.py:20; constructor call :149, forward :186, `.output_dims()` :154,
 `Coarse2Fine` :172,183). Semantics: SURVEY.md Appendix B. The device work is done by the sm_90a kernels in
-csrc/encoding.cu through the C ABI (psdf_enc_forward / psdf_enc_backward / psdf_enc_double_backward).
+csrc/encoding.cu through the C ABI (psdf_enc_forward / psdf_enc_backward / psdf_enc_double_backward, and the fixed-point
+psdf_enc_backward_fx / psdf_enc_double_backward_fx of PermutoEncoding(deterministic=True)).
 
 Differentiability contract (SURVEY.md F7): out is differentiable wrt `lattice_values` and wrt `positions`;
 the positions gradient itself is differentiable again wrt `lattice_values` and wrt the upstream gradient
@@ -65,8 +66,12 @@ class _EncodeBackFn(torch.autograd.Function):
             lattice.grad.is_contiguous()
         g_l = (lattice.grad if in_place else torch.zeros_like(lattice)) if need_l else None
         g_p = torch.empty_like(positions) if need_p else None
-        _enc_call("psdf_enc_backward", mod, N, D, L, F, T, positions, lattice, mod.scale_factor, mod.shift_tensor(), window,
-             1 if mod.concat_points else 0, mod.concat_points_scaling, grad_out, g_l, g_p)
+        args = (N, D, L, F, T, positions, lattice, mod.scale_factor, mod.shift_tensor(), window, 1 if mod.concat_points else 0,
+                mod.concat_points_scaling, grad_out, g_l, g_p)
+        if getattr(mod, "deterministic", False) and g_l is not None:
+            _enc_call("psdf_enc_backward_fx", mod, *args, mod.fx_workspace(lattice.device))
+        else:
+            _enc_call("psdf_enc_backward", mod, *args)
         ctx.mod = mod
         ctx.save_for_backward(lattice, positions, window, grad_out)
         if g_l is None or in_place:
@@ -89,18 +94,29 @@ class _EncodeBackFn(torch.autograd.Function):
         if gg_pos is not None and (need_l or need_go):
             g_l = torch.zeros_like(lattice) if need_l else None
             g_go = torch.empty_like(grad_out) if need_go else None
-            _enc_call("psdf_enc_double_backward", mod, N, D, L, F, T, positions, lattice, mod.scale_factor, mod.shift_tensor(), window,
-                 1 if mod.concat_points else 0, mod.concat_points_scaling, gg_pos.contiguous(), grad_out, g_l, g_go)
+            args = (N, D, L, F, T, positions, lattice, mod.scale_factor, mod.shift_tensor(), window, 1 if mod.concat_points else 0,
+                    mod.concat_points_scaling, gg_pos.contiguous(), grad_out, g_l, g_go)
+            if getattr(mod, "deterministic", False) and g_l is not None:
+                _enc_call("psdf_enc_double_backward_fx", mod, *args, mod.fx_workspace(lattice.device))
+            else:
+                _enc_call("psdf_enc_double_backward", mod, *args)
         return g_l, None, None, g_go, None, None, None, None
 
 
 class PermutoEncoding(torch.nn.Module):
     """PermutoEncoding(pos_dim, capacity, nr_levels, nr_feat_per_level, scale_per_level,
                        appply_random_shift_per_level=True, concat_points=False, concat_points_scaling=1.0)
-    (the triple-p spelling is the upstream one, models.py:149)."""
+    (the triple-p spelling is the upstream one, models.py:149).
+
+    deterministic=True (or setting the `deterministic` attribute) reduces the lattice gradient of the backward and of the double
+    backward in 64-bit fixed point (psdf_enc_backward_fx / psdf_enc_double_backward_fx): every contribution is rounded to the 2^-34
+    grid before it is added, so lattice_values.grad depends on the set of (position, upstream gradient) rows only, not on their order
+    or the run. It costs a workspace of 8 L T F bytes per module and device (100 MB at L = 24, T = 2^18, F = 2), allocated zeroed at
+    the first deterministic backward and kept out of state_dict. The workspace is shared by the module's calls, so they must run on
+    one stream. The positions gradient and the double backward's grad_out gradient are the same bits in both modes."""
 
     def __init__(self, pos_dim, capacity, nr_levels, nr_feat_per_level, scale_per_level, appply_random_shift_per_level=True,
-                 concat_points=False, concat_points_scaling=1.0, dtype=torch.float32, init_scale=1e-5):
+                 concat_points=False, concat_points_scaling=1.0, dtype=torch.float32, init_scale=1e-5, deterministic=False):
         super().__init__()
         if dtype != torch.float32:
             raise RuntimeError("only float32 lattice values are supported")
@@ -125,6 +141,16 @@ class PermutoEncoding(torch.nn.Module):
         self.register_buffer("scale_factor", self.compute_scale_factor(self.scale_per_level, self.pos_dim).to(dev), persistent=False)
         self._ones = None
         self.grad_in_place = False      # True: backward scatters into lattice_values.grad directly (set by the flat-buffer optimizer path)
+        self.deterministic = bool(deterministic)
+        self._fx = {}                   # device -> int64 [L, T, F] fixed-point accumulators of the deterministic backward (all zero between calls)
+
+    def fx_workspace(self, device):
+        """the zeroed fixed-point accumulators of the deterministic lattice gradient on `device`, allocated at the first request (an eager
+        call, before any CUDA-graph capture replays it); every deterministic call leaves them zero again"""
+        ws = self._fx.get(device)
+        if ws is None:
+            ws = self._fx[device] = torch.zeros(self.nr_levels, self.capacity, self.nr_feat_per_level, dtype=torch.int64, device=device)
+        return ws
 
     @staticmethod
     def compute_scale_factor(sigmas, pos_dim):
