@@ -563,6 +563,26 @@ int psdf_marching_cubes_count(int S, int N1, int N2, int i0, int last, float thr
                               void* stream);
 int psdf_marching_cubes_emit(int S, int N1, int N2, int i0, int last, float threshold, const float* vol, long long vertex_base,
                              const float affine_div_mul_off[3], uint8_t* workspace, float* verts, int* faces, void* stream);
+
+/* ---------------------------------------------------------------- mesh connected components (csrc/mesh_components.cu)
+ * Connected components of the vertex graph of an indexed triangle mesh: V vertices, faces [F,3] int32, each face joining its three
+ * vertices. The label of a vertex is the smallest vertex index of its component, so the labels depend only on the partition and the
+ * vertex numbering: the same bits for any face order and on every run (lock-free union-find that links the larger root under the smaller,
+ * integer atomics for every count). A vertex that no face references is a component of its own, with 0 faces.
+ * workspace: psdf_mesh_components_workspace_bytes(V, F) = 256 + 8 V bytes; PSDF_ERR_UNSUPPORTED when V or F is 2^31 or more,
+ * PSDF_ERR_ARG when negative. psdf_mesh_components fills it, and the caller may read it once the stream reaches that point:
+ *   int64 info[4] at byte 0 = {number of components, faces with an index outside [0, V), largest key, 0},
+ *   int32 labels [V] at byte 256, int32 face_counts [V] at byte 256 + 4 V (faces per component, indexed by label; each face counts
+ *   for the component of its first vertex, entries of non-root vertices are 0).
+ * The largest component is the one with the most faces, ties broken by the smallest label: largest key = (face count << 32) |
+ * (2^32 - 1 - label), 0 for V = 0. A face with an index outside [0, V) is neither linked nor counted and nothing out of range is touched;
+ * info[1] reports such faces, and the result is then not that of the mesh: callers check info[1] and refuse it. */
+long long psdf_mesh_components_workspace_bytes(long long nr_vertices, long long nr_faces);
+int psdf_mesh_components(int V, int F, const int* faces, uint8_t* workspace, void* stream);
+/* keep [V] (uint8 / bool) from a workspace psdf_mesh_components filled for the same mesh: largest != 0 keeps the vertices of the largest
+ * component (min_faces ignored), else those of components with at least min_faces faces (min_faces < 0: PSDF_ERR_ARG; 0 keeps every
+ * vertex). */
+int psdf_mesh_components_keep(int V, int largest, long long min_faces, const uint8_t* workspace, uint8_t* keep, void* stream);
 /* psdf_adamw_step over up to 8 parameter groups in one launch: device-resident step count, per-group hyper_dev [2] = {lr, weight_decay};
  * gradients scaled by grad_scale and reset to zero. n_l % 4 == 0, 16-byte aligned pointers. n and the five tables of device addresses
  * (one entry per group) are HOST arrays. The step used is step_dev[0] + step_offset (step_offset = 1: the counter is advanced afterwards

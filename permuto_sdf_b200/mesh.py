@@ -5,6 +5,8 @@ The reference evaluates the SDF in 64^3 chunks into a dense host array of N^3 fl
 the grid is evaluated a slab of slices at a time by a fused forward kernel (FusedSDF, or the density-only FusedNerfHash.density), and
 each slab goes straight to the marching-cubes kernels (csrc/marching_cubes.cu), which carry the vertex numbering from slab to slab.
 The N^3 volume never exists; memory is O(N^2 * slab) plus the mesh. The output is a fixed function of the volume (see the header), the same for any slab split and on every run.
+Mesh.connected_components, remove_small_components and keep_largest_component clean an extracted mesh of floaters and bubbles on the GPU
+(csrc/mesh_components.cu): labels, counts and the kept vertices are a fixed function of the mesh as well.
 """
 import math
 
@@ -17,6 +19,8 @@ from ._lib import call, load_library
 # grid points per slab: the slab's evaluation, values and edge ids (about 30 B per point in all)
 _SLAB_POINTS = 1 << 24
 _INT_MAX = 2 ** 31 - 1
+# workspace of psdf_mesh_components: int64 info[4] in the first 256 bytes, then int32 labels [V], then int32 face counts [V]
+_CC_HEADER = 256
 
 
 def _slab_slices(N0, N1, N2):
@@ -109,6 +113,62 @@ class Mesh:
         if self.NV is not None:
             self.NV = self.NV[kept]
         return self
+
+    def _components(self, fn):
+        """psdf_mesh_components of F -> (workspace, number of components); raises on faces that index outside [0, V)"""
+        Fc, V = self.F, self.V
+        if not isinstance(Fc, torch.Tensor) or Fc.dtype != torch.int32:
+            raise RuntimeError("%s: F must be an int32 tensor of shape [F,3], got %s" % (fn, getattr(Fc, "dtype", type(Fc).__name__)))
+        if Fc.dim() != 2 or Fc.shape[1] != 3:
+            raise RuntimeError("%s: F must have shape [F,3], got %s" % (fn, list(Fc.shape)))
+        if not Fc.is_cuda:
+            raise RuntimeError("%s: F must be a CUDA tensor (there is no CPU path)" % fn)
+        if not isinstance(V, torch.Tensor) or V.device != Fc.device:
+            raise RuntimeError("%s: V must be a tensor on F's device %s" % (fn, Fc.device))
+        nv, nf = V.shape[0], Fc.shape[0]
+        if nv > _INT_MAX or nf > _INT_MAX:
+            raise RuntimeError("%s: %d vertices and %d faces; both must be below 2^31" % (fn, nv, nf))
+        with torch.cuda.device(Fc.device):
+            ws = torch.empty(int(load_library().psdf_mesh_components_workspace_bytes(nv, nf)), dtype=torch.uint8, device=Fc.device)
+            call("psdf_mesh_components", nv, nf, Fc.contiguous(), ws)
+            nr, bad = ws[:16].view(torch.int64).tolist()
+        if bad:
+            raise RuntimeError("%s: %d faces have a vertex index outside [0, %d)" % (fn, bad, nv))
+        return ws, nr
+
+    def connected_components(self, with_face_counts=False):
+        """connected components of the vertex graph (each face joins its three vertices) on the GPU -> (labels int32 [V], number of
+        components). The label of a vertex is the smallest vertex index of its component, so the labels are the same bits for any face
+        order and on every run; a vertex no face references is a component of its own. with_face_counts: also the faces of each
+        component, int32 [V] indexed by label (0 at non-root vertices), a face counting for the component of its first vertex. F must be
+        an int32 CUDA tensor [F,3] with indices in [0, V) (checked on the device), V and F below 2^31; there is no CPU path."""
+        ws, nr = self._components("Mesh.connected_components")
+        nv = self.V.shape[0]
+        labels = ws[_CC_HEADER:_CC_HEADER + 4 * nv].view(torch.int32)
+        if with_face_counts:
+            return labels, nr, ws[_CC_HEADER + 4 * nv:_CC_HEADER + 8 * nv].view(torch.int32)
+        return labels, nr
+
+    def _keep_components(self, fn, largest, min_faces):
+        ws, _ = self._components(fn)
+        keep = torch.empty(self.V.shape[0], dtype=torch.bool, device=self.F.device)
+        with torch.cuda.device(self.F.device):
+            call("psdf_mesh_components_keep", self.V.shape[0], int(largest), min_faces, ws, keep)
+        return self.remove_marked_vertices(keep, True)
+
+    def remove_small_components(self, min_faces):
+        """keeps the vertices of the components (connected_components) with at least min_faces faces and compacts the mesh as
+        remove_marked_vertices(mask, keep=True) does: faces that touch a removed vertex go, V, NV and the vertex ids of F keep their
+        order. min_faces = 0 keeps everything; 1 drops vertices no face uses. -> self"""
+        if isinstance(min_faces, bool) or not isinstance(min_faces, (int, np.integer)) or min_faces < 0:
+            raise RuntimeError("Mesh.remove_small_components: min_faces must be a non-negative integer, got %r" % (min_faces,))
+        return self._keep_components("Mesh.remove_small_components", False, int(min_faces))
+
+    def keep_largest_component(self):
+        """keeps only the component with the most faces, ties broken by the smallest label, and compacts the mesh as
+        remove_small_components does. A mesh without faces keeps its vertex 0 (a component of 0 faces with the smallest label); an empty
+        mesh stays empty. -> self"""
+        return self._keep_components("Mesh.keep_largest_component", True, 0)
 
     def save_to_file(self, path):
         """binary little-endian PLY: x y z nx ny nz (float) per vertex (zero normals when there are none), uchar int vertex_indices per
