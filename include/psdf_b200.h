@@ -583,6 +583,55 @@ int psdf_mesh_components(int V, int F, const int* faces, uint8_t* workspace, voi
  * component (min_faces ignored), else those of components with at least min_faces faces (min_faces < 0: PSDF_ERR_ARG; 0 keeps every
  * vertex). */
 int psdf_mesh_components_keep(int V, int largest, long long min_faces, const uint8_t* workspace, uint8_t* keep, void* stream);
+
+/* ---------------------------------------------------------------- mesh decimation and vertex normals (csrc/mesh_decimate.cu)
+ * Garland-Heckbert edge collapse in parallel rounds of independent collapses, on verts [V,3] (float) and faces [F,3] (int32), V and F
+ * below 2^31. Built with -fmad=false: each fp64 / fp32 operation below is rounded as written, in the order written (oracle/decimate.py
+ * restates it and matches bit for bit). Positions enter fp64 exactly (p = double(fp32)). The output is the same bits on every run; it
+ * depends on the face order (edge ids are face corners).
+ * CSR: the faces of each vertex. Faces with an index outside [0, V) or a repeated vertex are counted (info[0], info[1]) and left out.
+ * Quadrics (begin): face t = (i0, i1, i2): N = (p1 - p0) x (p2 - p0), l = sqrt((Nx Nx + Ny Ny) + Nz Nz); l = 0 adds nothing; n = N / l,
+ *   d = -((nx p0x + ny p0y) + nz p0z), w = l * 0.5, q = w * (x y) for the pairs {xx, xy, xz, xd, yy, yz, yd, zz, zd, dd} of (nx, ny, nz, d).
+ *   Q[v] = sum of q over v's faces in ascending face order from 0. Collapsing b into a sets Q[a] = Q[a] + Q[b].
+ * Locks (begin): half-edge (u, v) of a face (v the corner after u) locks u and v unless exactly one face of u holds u -> v and exactly one
+ *   holds v -> u (boundary, an edge of three or more faces, inconsistent orientation).
+ * Candidates: half-edge (u, v) at corner k of face f with u < v, id c = 3 f + k; it needs exactly one u -> v and one v -> u (face g) among
+ *   u's faces, not both ends locked, and neither end in more than 64 faces (which bounds a candidate's work to 64^2 face reads). Survivor a = the locked end, else u; b = the other. Opposite vertices w (of f) != x (of g), each in
+ *   more than 3 faces. Link: exactly 2 neighbours of b (the corners that follow b in its faces), other than a, lie in a face of a.
+ * Position: Q = Q[a] + Q[b]. A locked a stays. Else with the cofactors c00 = Q4 Q7 - Q5 Q5, c01 = Q2 Q5 - Q1 Q7, c02 = Q1 Q5 - Q4 Q2,
+ *   c11 = Q0 Q7 - Q2 Q2, c12 = Q1 Q2 - Q0 Q5, c22 = Q0 Q4 - Q1 Q1, det = (Q0 c00 + Q1 c01) + Q2 c02, tr = (Q0 + Q4) + Q7: when
+ *   |det| > 1e-12 ((tr tr) tr), x = -(((c00 Q3 + c01 Q6) + c02 Q8) / det) and likewise with (c01, c11, c12) and (c02, c12, c22); x is taken,
+ *   rounded to fp32, when |x - m|^2 <= |pb - pa|^2 with m = (pa + pb) * 0.5 (fp64, dot = (xx + yy) + zz). Otherwise the least error of
+ *   pa, pb, then the fp32 midpoint (pa + pb) * 0.5f, a later one only when strictly smaller.
+ * Error: r_i = ((Q row i . (x, y, z)) + Q row i's 4th entry) left to right, err = ((x r0 + y r1) + z r2) + r3, at double(fp32 position).
+ * Validity: every face of a and of b except f and g keeps dot(N_before, N_after) > 0 (fp64, N as for the quadrics) with a or b moved.
+ * Key = (fp32 bits of float(err > 0 ? err : 0)) << 33 | c, UINT64_MAX when any check fails. best[v] = min key of v's candidates,
+ *   best2[v] = min best over v and the vertices of its faces; a candidate is chosen when its key == best2[u] == best2[v], so chosen
+ *   collapses neither share nor neighbour a vertex. When more than `allowed` are chosen, those with the `allowed` smallest keys are applied.
+ * Apply: position and Q to a, b -> a in b's faces, f and g dropped, removed[b] = 1, faces compacted in order; the caller's F shrinks by
+ *   2 * applied.
+ * Workspace: psdf_mesh_decimate_workspace_bytes(V, F) ~ 113 B per vertex + 37 B per face (sections each padded to 256 B):
+ *   int64 info[8] at byte 0 = {faces with an index outside [0, V), faces that repeat a vertex, collapses chosen in the last round, collapses
+ *   applied in it, threshold key, 0, 0, 0}, then int64 CSR offsets [V + 1], int32 counts [V], int32 CSR faces [3F], int64 scan tile sums,
+ *   fp64 quadrics [V][10], uint64 best [V], best2 [V], uint8 locks [V], uint64 chosen keys [V / 2 + 1], uint64 keys [3F] + 8 B (the
+ *   compaction's int64 prefix [F + 1] and int32 faces [3F] in the same bytes), uint8 dropped [F]. The normals' workspace
+ *   (psdf_mesh_normals_workspace_bytes ~ 12 B per vertex + 12 B per face) is the first five sections.
+ *   Both return PSDF_ERR_UNSUPPORTED when V or F is 2^31 or more and PSDF_ERR_ARG when negative.
+ * psdf_mesh_decimate_begin: clears removed [V] (uint8), counts bad faces into info, builds the sorted CSR, the locks and the quadrics. Bad
+ *   faces are left out, so nothing out of range is touched; the caller checks info[0] and info[1] and stops.
+ * psdf_mesh_decimate_round: one round on the current faces [F] (F <= F0, the count given to begin, which sized the workspace); at most
+ *   `allowed` collapses; verts, faces and removed are updated in place; info[2], info[3] tell what it did (info[3] = 0: no edge passes).
+ * psdf_mesh_normals: normals [V,3] (float) = n / sqrtf((nx nx + ny ny) + nz nz) of n = the fp32 sum, in ascending face order from 0, of
+ *   (p1 - p0) x (p2 - p0) (fp32, x = ay bz - az by) over v's faces; 0 when that length is 0. info[0] and info[1] count the bad faces as
+ *   begin does (they are left out; the caller refuses them).
+ * Cost: begin sorts each vertex's faces by heap sort (O(d log d) at valence d); twins are looked up in the list of the end with fewer
+ *   faces; every other step reads each vertex's faces a bounded number of times, so a round is linear in the mesh. */
+long long psdf_mesh_decimate_workspace_bytes(long long nr_vertices, long long nr_faces);
+long long psdf_mesh_normals_workspace_bytes(long long nr_vertices, long long nr_faces);
+int psdf_mesh_decimate_begin(int V, int F, const float* verts, const int* faces, uint8_t* workspace, uint8_t* removed, void* stream);
+int psdf_mesh_decimate_round(int V, int F0, int F, long long allowed, float* verts, int* faces, uint8_t* workspace, uint8_t* removed,
+                             void* stream);
+int psdf_mesh_normals(int V, int F, const float* verts, const int* faces, uint8_t* workspace, float* normals, void* stream);
 /* psdf_adamw_step over up to 8 parameter groups in one launch: device-resident step count, per-group hyper_dev [2] = {lr, weight_decay};
  * gradients scaled by grad_scale and reset to zero. n_l % 4 == 0, 16-byte aligned pointers. n and the five tables of device addresses
  * (one entry per group) are HOST arrays. The step used is step_dev[0] + step_offset (step_offset = 1: the counter is advanced afterwards

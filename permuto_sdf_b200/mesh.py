@@ -7,6 +7,8 @@ each slab goes straight to the marching-cubes kernels (csrc/marching_cubes.cu), 
 The N^3 volume never exists; memory is O(N^2 * slab) plus the mesh. The output is a fixed function of the volume (see the header), the same for any slab split and on every run.
 Mesh.connected_components, remove_small_components and keep_largest_component clean an extracted mesh of floaters and bubbles on the GPU
 (csrc/mesh_components.cu): labels, counts and the kept vertices are a fixed function of the mesh as well.
+Mesh.decimate reduces a mesh to a target face count by quadric edge collapse, in parallel rounds of independent collapses on the GPU
+(csrc/mesh_decimate.cu), and Mesh.recalculate_normals sets NV from the faces; both give the same bits on every run.
 """
 import math
 
@@ -169,6 +171,102 @@ class Mesh:
         remove_small_components does. A mesh without faces keeps its vertex 0 (a component of 0 faces with the smallest label); an empty
         mesh stays empty. -> self"""
         return self._keep_components("Mesh.keep_largest_component", True, 0)
+
+    def _check_vf(self, fn):
+        """V float32 CUDA [V,3] with finite values, F int32 [F,3] on V's device, both below 2^31 -> (V, F) contiguous"""
+        V, Fc = self.V, self.F
+        if not isinstance(V, torch.Tensor) or V.dtype != torch.float32:
+            raise RuntimeError("%s: V must be a float32 tensor of shape [V,3], got %s" % (fn, getattr(V, "dtype", type(V).__name__)))
+        if V.dim() != 2 or V.shape[1] != 3:
+            raise RuntimeError("%s: V must have shape [V,3], got %s" % (fn, list(V.shape)))
+        if not isinstance(Fc, torch.Tensor) or Fc.dtype != torch.int32:
+            raise RuntimeError("%s: F must be an int32 tensor of shape [F,3], got %s" % (fn, getattr(Fc, "dtype", type(Fc).__name__)))
+        if Fc.dim() != 2 or Fc.shape[1] != 3:
+            raise RuntimeError("%s: F must have shape [F,3], got %s" % (fn, list(Fc.shape)))
+        if not V.is_cuda:
+            raise RuntimeError("%s: V must be a CUDA tensor (there is no CPU path)" % fn)
+        if Fc.device != V.device:
+            raise RuntimeError("%s: F must be on V's device %s, got %s" % (fn, V.device, Fc.device))
+        nv, nf = V.shape[0], Fc.shape[0]
+        if nv > _INT_MAX or nf > _INT_MAX:
+            raise RuntimeError("%s: %d vertices and %d faces; both must be below 2^31" % (fn, nv, nf))
+        if not bool(torch.isfinite(V).all()):
+            raise RuntimeError("%s: V has values that are not finite" % fn)
+        return V.contiguous(), Fc.contiguous()
+
+    def _decimate(self, nr_target_faces):
+        """the rounds of decimate before the final compaction -> (V, F, removed [V] bool, rounds); None when the target is at or above
+        the face count"""
+        fn = "Mesh.decimate"
+        if isinstance(nr_target_faces, bool) or not isinstance(nr_target_faces, (int, np.integer)) or nr_target_faces < 0:
+            raise RuntimeError("%s: nr_target_faces must be a non-negative integer, got %r" % (fn, nr_target_faces))
+        target = int(nr_target_faces)
+        V, Fc = self._check_vf(fn)
+        nv, nf = V.shape[0], Fc.shape[0]
+        if target >= nf:
+            return None
+        dev = V.device
+        with torch.cuda.device(dev):
+            V, Fc = V.clone(), Fc.clone()
+            ws = torch.empty(int(load_library().psdf_mesh_decimate_workspace_bytes(nv, nf)), dtype=torch.uint8, device=dev)
+            removed = torch.empty(nv, dtype=torch.bool, device=dev)
+            call("psdf_mesh_decimate_begin", nv, nf, V, Fc, ws, removed)
+            bad, rep = ws[:16].view(torch.int64).tolist()
+            if bad:
+                raise RuntimeError("%s: %d faces have a vertex index outside [0, %d)" % (fn, bad, nv))
+            if rep:
+                raise RuntimeError("%s: %d faces repeat a vertex" % (fn, rep))
+            cur, rounds = nf, 0
+            while True:
+                allowed = (cur - target + 1) // 2
+                if allowed <= 0:
+                    break
+                call("psdf_mesh_decimate_round", nv, nf, cur, allowed, V, Fc, ws, removed)
+                applied = int(ws[24:32].view(torch.int64).item())
+                rounds += 1
+                if applied == 0:
+                    break
+                cur -= 2 * applied
+        return V, Fc[:cur], removed, rounds
+
+    def decimate(self, nr_target_faces):
+        """quadric edge-collapse decimation on the GPU (Garland-Heckbert, in parallel rounds of collapses that share no vertex or
+        neighbour; the rules are in include/psdf_b200.h). Interior edges collapse in order of quadric error until the mesh has
+        nr_target_faces or nr_target_faces - 1 faces (each collapse removes two), or fewer when no edge passes the checks (link
+        condition, no face flips or degenerates, no opposite vertex in 3 faces or fewer, no end in more than 64 faces); 0 decimates as far as
+        they allow. Boundary,
+        non-manifold and inconsistently oriented edges lock their vertices, which never move, so such edges stay exactly as they are.
+        Removed vertices go and the rest keep their order, as remove_marked_vertices does; vertices no face uses stay. NV, when present,
+        is recalculated (recalculate_normals). The same bits on every run. A target at or above the face count returns the mesh as it
+        is. V must be float32 CUDA [V,3] with finite values and F int32 [F,3] on its device, both below 2^31; faces with an index outside
+        [0, V) or a repeated vertex are refused (checked on the device). There is no CPU path. -> self"""
+        out = self._decimate(nr_target_faces)
+        if out is None:
+            return self
+        self.V, self.F, removed, _ = out
+        self.remove_marked_vertices(removed, False)
+        if self.NV is not None:
+            self.recalculate_normals()
+        return self
+
+    def recalculate_normals(self):
+        """NV = the normalised sum of the cross products (p1 - p0) x (p2 - p0) of each vertex's faces, summed in fp32 in ascending face
+        order; zero for a vertex without faces. On the GPU, with the checks of decimate: faces with an index outside [0, V) or a
+        repeated vertex are refused. -> self"""
+        fn = "Mesh.recalculate_normals"
+        V, Fc = self._check_vf(fn)
+        nv, nf = V.shape[0], Fc.shape[0]
+        with torch.cuda.device(V.device):
+            ws = torch.empty(int(load_library().psdf_mesh_normals_workspace_bytes(nv, nf)), dtype=torch.uint8, device=V.device)
+            NV = torch.empty_like(V)
+            call("psdf_mesh_normals", nv, nf, V, Fc, ws, NV)
+            bad, rep = ws[:16].view(torch.int64).tolist()
+        if bad:
+            raise RuntimeError("%s: %d faces have a vertex index outside [0, %d)" % (fn, bad, nv))
+        if rep:
+            raise RuntimeError("%s: %d faces repeat a vertex" % (fn, rep))
+        self.NV = NV
+        return self
 
     def save_to_file(self, path):
         """binary little-endian PLY: x y z nx ny nz (float) per vertex (zero normals when there are none), uchar int vertex_indices per
