@@ -632,6 +632,43 @@ int psdf_mesh_decimate_begin(int V, int F, const float* verts, const int* faces,
 int psdf_mesh_decimate_round(int V, int F0, int F, long long allowed, float* verts, int* faces, uint8_t* workspace, uint8_t* removed,
                              void* stream);
 int psdf_mesh_normals(int V, int F, const float* verts, const int* faces, uint8_t* workspace, float* normals, void* stream);
+
+/* ---------------------------------------------------------------- mesh subdivision (csrc/mesh_subdivide.cu)
+ * One round of midpoint (smooth = 0) or Loop (smooth != 0) subdivision of verts [V,3] (float) and faces [F,3] (int32): every face becomes
+ * four. Built with -fmad=false: each fp32 operation below is rounded as written, in the order written (oracle/subdivide.py restates it and
+ * matches bit for bit). The output depends only on V's bits and F, the same bits on every run.
+ * Input: faces with an index outside [0, V) or a repeated vertex are counted (info[0], info[1]) and left out; the caller refuses them.
+ *   Vertices without faces are carried over unchanged.
+ * Edges: corner k of face f is the half-edge F[f][k] -> F[f][(k + 1) % 3], id 3 f + k. The faces of an undirected edge {u, v} are those
+ *   that hold u and v; the edge is interior when there are exactly two, a crease otherwise (one, or three and more). Each edge gets one new
+ *   vertex; they are numbered V + j in ascending order of the edge's smallest corner id, so the order depends on F alone.
+ * Faces: face f = (v0, v1, v2) with edge vertices e01, e12, e20 (of its corners 0, 1, 2) becomes faces 4f .. 4f + 3 = (v0, e01, e20),
+ *   (e01, v1, e12), (e20, e12, v2), (e01, e12, e20): the winding is kept, so a closed, oriented mesh stays closed and oriented.
+ * Midpoint: edge vertex = 0.5f * (pu + pv); old vertices do not move.
+ * Loop, edge vertices: interior edge of corner (u -> v) of face f with w the third vertex of f and x that of the other face:
+ *   0.375f * (pu + pv) + 0.125f * (pw + px); crease edge: the midpoint. Sums of two points are commutative in fp32, so the order of u, v
+ *   and of w, x does not matter.
+ * Loop, old vertices: n = v's distinct neighbours, k = those joined to v by a crease edge.
+ *   k = 0: beta = 0.1875f (n = 3), else 3.0f / float(8 n); w = 1.0f - float(n) * beta; p = w * pv + beta * s, where s = the fp32 sum of
+ *     the neighbours' positions from 0.0f in ascending vertex index (s = s + pn).
+ *   k = 2: p = 0.75f * pv + 0.125f * (pa + pb) with a < b the two crease neighbours.
+ *   Otherwise (corners, non-manifold vertices) v does not move.
+ *   beta is Warren's simplification, which libigl's loop uses as far as we recall; its source is not at hand, so this is unverified.
+ *   Every product above is per coordinate: s * (x, y, z) = (s x, s y, s z).
+ * Workspace: psdf_mesh_subdivide_workspace_bytes(V, F) ~ 12 B per vertex + 72 B per face (sections each padded to 256 B): int64 info[4]
+ *   at byte 0 = {faces with an index outside [0, V), faces that repeat a vertex, edges E, 0}, then int64 CSR offsets [V + 1], int32 counts
+ *   [V], int32 CSR faces [3F], int32 CSR neighbours [6F] (the two other corners of each of those faces), int64 scan tile sums, int32 edge
+ *   owners [3F] (the smallest corner id of each corner's edge), int64 edge ids [3F + 1] (exclusive prefix of the corners that own their
+ *   edge). PSDF_ERR_UNSUPPORTED when V or 4 F is 2^31 or more (the output faces are int32 rows), PSDF_ERR_ARG when negative.
+ * psdf_mesh_subdivide_count: builds the CSR, counts bad faces into info[0], info[1] and the edges into info[2]. The caller reads info once,
+ *   refuses bad faces, checks that V + E stays below 2^31 and allocates verts_out [V + E, 3] and faces_out [4F, 3].
+ * psdf_mesh_subdivide_emit: with the workspace count filled for the same faces, writes verts_out and faces_out.
+ * Cost: the Loop rule sorts each vertex's neighbour list by heap sort (O(d log d) at valence d); an edge's faces are looked up in the list
+ *   of the end with fewer faces; every other step is one pass, so a round is linear in the mesh. */
+long long psdf_mesh_subdivide_workspace_bytes(long long nr_vertices, long long nr_faces);
+int psdf_mesh_subdivide_count(int V, int F, const int* faces, uint8_t* workspace, void* stream);
+int psdf_mesh_subdivide_emit(int V, int F, int smooth, const float* verts, const int* faces, uint8_t* workspace, float* verts_out,
+                             int* faces_out, void* stream);
 /* psdf_adamw_step over up to 8 parameter groups in one launch: device-resident step count, per-group hyper_dev [2] = {lr, weight_decay};
  * gradients scaled by grad_scale and reset to zero. n_l % 4 == 0, 16-byte aligned pointers. n and the five tables of device addresses
  * (one entry per group) are HOST arrays. The step used is step_dev[0] + step_offset (step_offset = 1: the counter is advanced afterwards

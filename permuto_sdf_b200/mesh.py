@@ -9,6 +9,8 @@ Mesh.connected_components, remove_small_components and keep_largest_component cl
 (csrc/mesh_components.cu): labels, counts and the kept vertices are a fixed function of the mesh as well.
 Mesh.decimate reduces a mesh to a target face count by quadric edge collapse, in parallel rounds of independent collapses on the GPU
 (csrc/mesh_decimate.cu), and Mesh.recalculate_normals sets NV from the faces; both give the same bits on every run.
+Mesh.load reads PLY, OBJ and STL files on the host, the torch ops below weld, compact and place a mesh as train_sdf_from_mesh.py does,
+and Mesh.upsample runs midpoint or Loop subdivision on the GPU (csrc/mesh_subdivide.cu), the same bits on every run.
 """
 import math
 
@@ -268,6 +270,156 @@ class Mesh:
         self.NV = NV
         return self
 
+    def upsample(self, nr_subdivisions, smooth):
+        """nr_subdivisions rounds of subdivision on the GPU, each splitting every face into four: smooth=False is midpoint subdivision
+        (libigl's upsample), smooth=True Loop subdivision (libigl's loop). New vertices follow the old ones; the rules, the numbering and
+        the fp32 arithmetic are in include/psdf_b200.h, and the result is the same bits on every run. Boundary and non-manifold edges are
+        creases: their vertices are midpoints and their ends follow the boundary rule or stay. NV, when present, is recalculated
+        (recalculate_normals). The checks of decimate apply; a result with 2^31 or more faces (4^rounds F) is refused before anything
+        runs, and one with 2^31 or more vertices before its round. -> self"""
+        fn = "Mesh.upsample"
+        if isinstance(nr_subdivisions, bool) or not isinstance(nr_subdivisions, (int, np.integer)) or nr_subdivisions < 0:
+            raise RuntimeError("%s: nr_subdivisions must be a non-negative integer, got %r" % (fn, nr_subdivisions))
+        rounds = int(nr_subdivisions)
+        if isinstance(self.F, torch.Tensor) and self.F.dim() == 2 and self.F.shape[0] * 4 ** rounds > _INT_MAX:
+            raise RuntimeError("%s: %d faces become %d after %d rounds; int32 faces hold fewer than 2^31" % (
+                fn, self.F.shape[0], self.F.shape[0] * 4 ** rounds, rounds))
+        V, Fc = self._check_vf(fn)
+        if rounds == 0:
+            return self
+        with torch.cuda.device(V.device):
+            for _ in range(rounds):
+                nv, nf = V.shape[0], Fc.shape[0]
+                ws = torch.empty(int(load_library().psdf_mesh_subdivide_workspace_bytes(nv, nf)), dtype=torch.uint8, device=V.device)
+                call("psdf_mesh_subdivide_count", nv, nf, Fc, ws)
+                bad, rep, E = ws[:24].view(torch.int64).tolist()
+                if bad:
+                    raise RuntimeError("%s: %d faces have a vertex index outside [0, %d)" % (fn, bad, nv))
+                if rep:
+                    raise RuntimeError("%s: %d faces repeat a vertex" % (fn, rep))
+                if nv + E > _INT_MAX:
+                    raise RuntimeError("%s: %d vertices and %d edges make %d vertices; V must stay below 2^31" % (fn, nv, E, nv + E))
+                Vn = torch.empty(nv + E, 3, dtype=torch.float32, device=V.device)
+                Fn = torch.empty(4 * nf, 3, dtype=torch.int32, device=V.device)
+                call("psdf_mesh_subdivide_emit", nv, nf, int(bool(smooth)), V, Fc, ws, Vn, Fn)
+                V, Fc = Vn, Fn
+                del ws
+        self.V, self.F = V, Fc
+        if self.NV is not None:
+            self.recalculate_normals()
+        return self
+
+    # ------------------------------------------------------------------ reading, welding and placing a mesh
+    @staticmethod
+    def load(path, device="cuda", weld=None):
+        """reads a PLY (ascii, binary little or big endian), OBJ or STL (binary or ASCII) file -> Mesh with V float32 [V,3], F int32 [F,3]
+        and NV on `device` (device="cpu" reads without a GPU; the GPU operations still need CUDA tensors). The format is told by the
+        content (PLY magic, a binary STL's size of 84 + 50 n bytes, a leading "solid"), else by the extension. Polygons are fan-triangulated
+        in file order, (p0, pj, pj+1).
+        PLY: vertex x y z (float or double) and nx ny nz when all three are there (NV); other fixed-size properties and elements are
+        skipped; the face list is vertex_indices or vertex_index with any integer count and index types; other list elements are refused.
+        Mesh.save_to_file followed by load gives back V, F and NV bit for bit.
+        OBJ: v x y z [w] and f with a, a/b, a//c or a/b/c, 1-based or negative (relative to the vertices read so far); vn is per corner in
+        OBJ, so NV is None; other keywords are ignored.
+        STL: three vertices per facet, NV None. weld=None welds STL only, through remove_duplicate_vertices, which the connectivity of
+        components, decimation, normals and subdivision needs; weld=True welds any format, weld=False keeps the triangle soup.
+        Truncated data, indices outside [0, V), unsupported property types and unreadable files raise RuntimeError naming the path; V and
+        F must stay below 2^31."""
+        path = str(path)
+        try:
+            with open(path, "rb") as f:
+                data = f.read()
+        except OSError as e:
+            raise RuntimeError("Mesh.load: %s: %s" % (path, e.strerror)) from None
+        ext = path.lower().rsplit(".", 1)[-1] if "." in path else ""
+        if data.startswith(b"ply\n") or data.startswith(b"ply\r\n"):
+            kind, (V, Fc, NV) = "ply", _load_ply(path, data)
+        elif _is_binary_stl(data) or data.lstrip().startswith(b"solid") or ext == "stl":
+            kind, (V, Fc, NV) = "stl", _load_stl(path, data)
+        elif ext == "obj":
+            kind, (V, Fc, NV) = "obj", _load_obj(path, data)
+        elif ext == "ply":
+            raise RuntimeError("Mesh.load: %s: not a PLY file (no 'ply' magic)" % path)
+        else:
+            raise RuntimeError("Mesh.load: %s: cannot tell the format (PLY, OBJ or STL) from the content or the extension" % path)
+        if V.shape[0] > _INT_MAX or Fc.shape[0] > _INT_MAX:
+            raise RuntimeError("Mesh.load: %s: %d vertices and %d faces; both must be below 2^31" % (path, V.shape[0], Fc.shape[0]))
+        if Fc.size and (Fc.min() < 0 or Fc.max() >= V.shape[0]):
+            raise RuntimeError("Mesh.load: %s: %d faces have a vertex index outside [0, %d)" % (
+                path, int(((Fc < 0) | (Fc >= V.shape[0])).any(1).sum()), V.shape[0]))
+        t = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(device)
+        m = Mesh(t(V), t(Fc.astype(np.int32)), None if NV is None else t(NV))
+        if weld or (weld is None and kind == "stl"):
+            m.remove_duplicate_vertices()
+        return m
+
+    def remove_duplicate_vertices(self):
+        """merges vertices with equal fp32 positions (-0.0 equal to +0.0; exact, no tolerance): each group keeps the vertex with the
+        smallest index, the survivors keep their order (and their NV), F is remapped, and faces that then repeat a vertex are dropped.
+        V must be finite. CPU or CUDA tensors. -> self"""
+        if not bool(torch.isfinite(self.V).all()):
+            raise RuntimeError("Mesh.remove_duplicate_vertices: V has values that are not finite")
+        nv = self.V.shape[0]
+        if nv == 0:
+            return self
+        key = (self.V.float() + 0.0).view(torch.int32).long()          # + 0.0 turns -0.0 into +0.0
+        _, group = torch.unique(key, dim=0, return_inverse=True)
+        idx = torch.arange(nv, device=self.V.device)
+        first = torch.full((int(group.max()) + 1,), nv, dtype=torch.int64, device=self.V.device).scatter_reduce(0, group, idx, "amin")
+        rep = first[group]
+        kept = rep == idx
+        new_id = torch.cumsum(kept.to(torch.int64), 0) - 1
+        Fn = new_id[rep[self.F.long()]]
+        Fn = Fn[(Fn[:, 0] != Fn[:, 1]) & (Fn[:, 1] != Fn[:, 2]) & (Fn[:, 2] != Fn[:, 0])]
+        self.F = Fn.to(torch.int32).reshape(-1, 3)
+        self.V = self.V[kept]
+        if self.NV is not None:
+            self.NV = self.NV[kept]
+        return self
+
+    def remove_unreferenced_verts(self):
+        """drops the vertices no face uses and compacts the mesh as remove_marked_vertices does. -> self"""
+        used = torch.zeros(self.V.shape[0], dtype=torch.bool, device=self.V.device)
+        used[self.F.long().reshape(-1)] = True
+        return self.remove_marked_vertices(used, True)
+
+    def _bounds(self, fn):
+        if self.V.shape[0] == 0:
+            raise RuntimeError("%s: the mesh has no vertices" % fn)
+        return self.V.min(0).values, self.V.max(0).values
+
+    def normalize_position(self):
+        """translates V by minus the centre of its bounding box, c = (min + max) / 2 (fp32, over all vertices), and returns c (float32
+        tensor [3]); translate(c) undoes it. EasyPBR's definition is not in the reference's checkout, so this formula is ours, not pinned
+        to it."""
+        lo, hi = self._bounds("Mesh.normalize_position")
+        c = (lo + hi) / 2
+        self.translate(-c)
+        return c
+
+    def normalize_size(self):
+        """scales V by s = 1 / d with d = |max - min| the bounding-box diagonal, d = sqrt((dx dx + dy dy) + dz dz) in fp32 and s = 1.0 / d
+        in fp64, applied as scale_mesh(s); returns s (a float), so scale_mesh(1.0 / s) undoes it. EasyPBR's definition is not in the
+        reference's checkout, so this formula is ours, not pinned to it."""
+        lo, hi = self._bounds("Mesh.normalize_size")
+        e = hi - lo
+        d = float(torch.sqrt((e[0] * e[0] + e[1] * e[1]) + e[2] * e[2]))
+        if not d > 0:
+            raise RuntimeError("Mesh.normalize_size: the bounding box has zero size")
+        s = 1.0 / d
+        self.scale_mesh(s)
+        return s
+
+    def scale_mesh(self, s):
+        """V = V * s (fp32). -> self"""
+        self.V = self.V * s
+        return self
+
+    def translate(self, t):
+        """V = V + t (fp32), t a 3-vector. -> self"""
+        self.V = self.V + torch.as_tensor(t, dtype=self.V.dtype, device=self.V.device)
+        return self
+
     def save_to_file(self, path):
         """binary little-endian PLY: x y z nx ny nz (float) per vertex (zero normals when there are none), uchar int vertex_indices per
         face"""
@@ -285,6 +437,183 @@ class Mesh:
             f.write(header.encode("ascii"))
             f.write(vbytes)
             f.write(frec.tobytes())
+
+
+# ---------------------------------------------------------------- reading meshes (host side)
+_PLY_TYPES = {"char": "i1", "int8": "i1", "uchar": "u1", "uint8": "u1", "short": "i2", "int16": "i2", "ushort": "u2", "uint16": "u2",
+              "int": "i4", "int32": "i4", "uint": "u4", "uint32": "u4", "float": "f4", "float32": "f4", "double": "f8", "float64": "f8"}
+
+
+def _fan(polys):
+    """[n, c] polygons -> [n (c - 2), 3] triangles (p0, pj, pj+1), j = 1 .. c - 2, polygon by polygon"""
+    n, c = polys.shape
+    if c < 3:
+        return np.zeros((0, 3), dtype=np.int64)
+    j = np.arange(1, c - 1)
+    return np.stack([np.broadcast_to(polys[:, :1], (n, c - 2)), polys[:, j], polys[:, j + 1]], 2).reshape(-1, 3)
+
+
+def _ply_type(path, t):
+    if t not in _PLY_TYPES:
+        raise RuntimeError("Mesh.load: %s: unsupported PLY property type %r" % (path, t))
+    return _PLY_TYPES[t]
+
+
+def _ply_header(path, data):
+    """-> (format, [(element, count, [(name, type) or (name, count type, item type)])], body offset)"""
+    end = data.find(b"end_header")
+    if end < 0:
+        raise RuntimeError("Mesh.load: %s: PLY header without end_header" % path)
+    nl = data.find(b"\n", end)
+    body = len(data) if nl < 0 else nl + 1
+    fmt, elements = None, []
+    for line in data[:end].decode("ascii", "replace").splitlines()[1:]:
+        w = line.split()
+        if not w or w[0] in ("comment", "obj_info"):
+            continue
+        if w[0] == "format" and len(w) >= 2:
+            fmt = w[1]
+        elif w[0] == "element" and len(w) == 3:
+            elements.append((w[1], int(w[2]), []))
+        elif w[0] == "property" and elements and len(w) == 5 and w[1] == "list":
+            elements[-1][2].append((w[4], _ply_type(path, w[2]), _ply_type(path, w[3])))
+        elif w[0] == "property" and elements and len(w) == 3:
+            elements[-1][2].append((w[2], _ply_type(path, w[1])))
+        else:
+            raise RuntimeError("Mesh.load: %s: cannot read the PLY header line %r" % (path, line))
+    if fmt not in ("ascii", "binary_little_endian", "binary_big_endian"):
+        raise RuntimeError("Mesh.load: %s: unsupported PLY format %r" % (path, fmt))
+    return fmt, elements, body
+
+
+def _ply_lists(path, buf, off, n, pre, post, cdt, idt):
+    """n records of (pre bytes, count cdt, count x idt, post bytes) from buf at off, read a run of equal counts at a time ->
+    (triangles [m, 3] int64, in file order, the offset after the records)"""
+    cs, isz = cdt.itemsize, idt.itemsize
+    tris, i = [], 0
+    while i < n:
+        if off + pre + cs > len(buf):
+            raise RuntimeError("Mesh.load: %s: truncated PLY face data (%d of %d faces)" % (path, i, n))
+        c0 = np.frombuffer(buf, cdt, 1, off + pre)[0]
+        c = int(c0)
+        if c < 0 or c != c0:
+            raise RuntimeError("Mesh.load: %s: a PLY face with %d vertices" % (path, c))
+        rec = pre + cs + c * isz + post
+        j, w = 1, 64
+        while i + j < n:
+            k = min(w, n - i - j, max((len(buf) - off - j * rec - pre - cs) // rec + 1, 0))
+            if k <= 0:
+                break
+            counts = np.ndarray((k,), cdt, buf, off + j * rec + pre, (rec,))
+            bad = np.flatnonzero(counts != c)
+            if bad.size:
+                j += int(bad[0])
+                break
+            j += k
+            w *= 2
+        if off + j * rec > len(buf):
+            raise RuntimeError("Mesh.load: %s: truncated PLY face data (%d of %d faces)" % (path, i, n))
+        idx = np.ndarray((j, c), idt, buf, off + pre + cs, (rec, isz))
+        if idx.dtype.kind == "f" and not (idx == np.floor(idx)).all():
+            raise RuntimeError("Mesh.load: %s: a PLY face index that is not an integer" % path)
+        tris.append(_fan(idx.astype(np.int64)))
+        off += j * rec
+        i += j
+    return (np.concatenate(tris) if tris else np.zeros((0, 3), dtype=np.int64)), off
+
+
+def _load_ply(path, data):
+    fmt, elements, off = _ply_header(path, data)
+    if fmt == "ascii":
+        # every value becomes an fp64 token, and the binary reader runs over them with every type 8 bytes wide
+        try:
+            buf = np.array(data[off:].split(), dtype=np.float64).tobytes()
+        except ValueError:
+            raise RuntimeError("Mesh.load: %s: a PLY value that is not a number" % path) from None
+        to = lambda t: np.dtype("f8")
+        off = 0
+    else:
+        buf, bo = data, "<" if fmt == "binary_little_endian" else ">"
+        to = lambda t: np.dtype(bo + t)
+    V = NV = Fc = None
+    for name, n, props in elements:
+        lists = [p for p in props if len(p) == 3]
+        if not lists:
+            dt = np.dtype([(p[0], to(p[1])) for p in props])
+            if off + n * dt.itemsize > len(buf):
+                raise RuntimeError("Mesh.load: %s: truncated PLY %s data (%d records expected)" % (path, name, n))
+            rec = np.frombuffer(buf, dt, n, off)
+            off += n * dt.itemsize
+            if name == "vertex":
+                names = dt.names or ()
+                for a in ("x", "y", "z", "nx", "ny", "nz"):
+                    if a in names and dt[a].kind != "f":
+                        raise RuntimeError("Mesh.load: %s: unsupported type of vertex property %s (float or double)" % (path, a))
+                if not all(a in names for a in "xyz"):
+                    raise RuntimeError("Mesh.load: %s: the PLY vertices have no x y z" % path)
+                V = np.stack([rec[a] for a in "xyz"], 1).astype(np.float32)
+                if all(a in names for a in ("nx", "ny", "nz")):
+                    NV = np.stack([rec[a] for a in ("nx", "ny", "nz")], 1).astype(np.float32)
+            continue
+        if name != "face" or len(lists) != 1 or lists[0][0] not in ("vertex_indices", "vertex_index"):
+            raise RuntimeError("Mesh.load: %s: unsupported PLY list element %r (%s)" % (path, name, ", ".join(p[0] for p in lists)))
+        _, ct, it = lists[0]
+        if np.dtype(ct).kind not in "iu" or np.dtype(it).kind not in "iu":
+            raise RuntimeError("Mesh.load: %s: unsupported PLY face list type (%s %s): integers expected" % (path, ct, it))
+        k = props.index(lists[0])
+        size = lambda ps: sum(to(p[1]).itemsize for p in ps)
+        tri, off = _ply_lists(path, buf, off, n, size(props[:k]), size(props[k + 1:]), to(ct), to(it))
+        Fc = tri
+    if V is None:
+        raise RuntimeError("Mesh.load: %s: the PLY file has no vertex element" % path)
+    return V, (np.zeros((0, 3), dtype=np.int64) if Fc is None else Fc), NV
+
+
+def _load_obj(path, data):
+    vs, faces = [], []
+    for ln, line in enumerate(data.decode("utf-8", "replace").splitlines(), 1):
+        w = line.split()
+        if not w:
+            continue
+        try:
+            if w[0] == "v":
+                vs.append([float(x) for x in w[1:4]] if len(w) >= 4 else None)
+                if vs[-1] is None:
+                    raise ValueError
+            elif w[0] == "f":
+                idx = [int(x.split("/")[0]) for x in w[1:]]
+                faces.append([i - 1 if i > 0 else len(vs) + i if i < 0 else -(2 ** 40) for i in idx])
+        except ValueError:
+            raise RuntimeError("Mesh.load: %s: cannot read OBJ line %d: %r" % (path, ln, line)) from None
+    tris = [(f[0], f[j], f[j + 1]) for f in faces for j in range(1, len(f) - 1)]
+    V = np.array(vs, dtype=np.float64).reshape(-1, 3).astype(np.float32)
+    return V, np.array(tris, dtype=np.int64).reshape(-1, 3), None
+
+
+_STL_REC = np.dtype([("n", "<f4", (3,)), ("v", "<f4", (3, 3)), ("attr", "<u2")])
+
+
+def _is_binary_stl(data):
+    return len(data) >= 84 and 84 + 50 * int(np.frombuffer(data, "<u4", 1, 80)[0]) == len(data)
+
+
+def _load_stl(path, data):
+    if _is_binary_stl(data):
+        n = int(np.frombuffer(data, "<u4", 1, 80)[0])
+        V = np.frombuffer(data, _STL_REC, n, 84)["v"].reshape(-1, 3).astype(np.float32)
+    else:
+        import re
+        text = data.decode("ascii", "replace")
+        if not text.lstrip().startswith("solid"):
+            raise RuntimeError("Mesh.load: %s: neither a binary STL (84 + 50 n bytes for n facets) nor an ASCII STL" % path)
+        try:
+            V = np.array(re.findall(r"\bvertex\s+(\S+)\s+(\S+)\s+(\S+)", text), dtype=np.float64).reshape(-1, 3).astype(np.float32)
+        except ValueError:
+            raise RuntimeError("Mesh.load: %s: an STL vertex that is not a number" % path) from None
+        if V.shape[0] % 3 or V.shape[0] // 3 != len(re.findall(r"\bendfacet\b", text)):
+            raise RuntimeError("Mesh.load: %s: truncated ASCII STL: %d vertices in %d complete facets" % (
+                path, V.shape[0], len(re.findall(r"\bendfacet\b", text))))
+    return V, np.arange(V.shape[0], dtype=np.int64).reshape(-1, 3), None
 
 
 def _mesh_grid(N, min_val, max_val, threshold, dev, values):

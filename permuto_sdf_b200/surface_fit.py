@@ -106,6 +106,14 @@ class SurfaceFit:
     # not form)
     MODEL_ON_FUSED_PAIR = True
 
+    @classmethod
+    def from_mesh(cls, mesh, **kwargs):
+        """cls(mesh.V, mesh.NV, **kwargs): a fit to the vertices of a Mesh and their normals (train_sdf_from_mesh.py:93 takes
+        gt_points, gt_normals = mesh.V, mesh.NV). A mesh without NV is refused; Mesh.recalculate_normals gives it one."""
+        if getattr(mesh, "NV", None) is None:
+            raise RuntimeError("%s.from_mesh: the mesh has no vertex normals (NV); call mesh.recalculate_normals() first" % cls.__name__)
+        return cls(mesh.V, mesh.NV, **kwargs)
+
     def __init__(self, points, normals, nr_levels=24, capacity=2 ** 18, hidden=32, box_size=(1, 1, 1), box_translation=(0, 0, 0),
                  nr_iters_for_c2f=5000, lr=1e-3, optimizer="fused", deterministic=False, direct=None, seed=0, fused_training=True):
         who = type(self).__name__
