@@ -2,14 +2,11 @@
 // every fp64 and fp32 operation is rounded as written, so oracle/decimate.py reproduces the output bit for bit. The rules (quadrics,
 // candidates, locks, cost, validity, selection, apply) are stated in include/psdf_b200.h; this file only adds how they are computed.
 //
-// Vertex -> face CSR: k_dc_degree counts the faces of each vertex, a three-kernel exclusive scan (k_dc_scan_tiles, k_dc_scan_top,
-// k_dc_scan_out) turns the counts into int64 offsets, k_dc_fill places the faces with atomics and k_dc_sort puts each vertex's list in
-// ascending face order (only begin and the normals need the order; a round's CSR is left as filled, every use of it there is
-// order-free). Faces with an index outside [0, V) or a repeated vertex are counted in begin and never enter the CSR.
+// Vertex -> face CSR (mesh_csr.cuh): k_mesh_degree counts the faces of each vertex, the scan k_mesh_scan_* turns the counts into int64
+// offsets, k_dc_fill places the faces with atomics and k_dc_sort puts each vertex's list in ascending face order (only begin and the
+// normals need the order; a round's CSR is left as filled, every use of it there is order-free). Faces with an index outside [0, V) or a
+// repeated vertex are counted by k_mesh_check in begin and never enter the CSR. The compaction scans the faces kept with the same kernels.
 //
-//   k_dc_check     counts faces outside [0, V) and faces that repeat a vertex                    thread per face
-//   k_dc_degree    deg[v] += 1 for the three corners of every valid face                         thread per face
-//   k_dc_scan_*    exclusive prefix of deg (CSR offsets) or of the faces kept (compaction)       tile / one block / tile
 //   k_dc_fill      adj[off[v] + cursor] = f                                                      thread per face
 //   k_dc_sort      heap sort of each vertex's face list                                          thread per vertex
 //   k_dc_lock      a half-edge whose direction is not there once or whose twin is not there once locks both ends   thread per half-edge
@@ -22,26 +19,15 @@
 //   k_dc_compact   faces that no collapse dropped, in order, into the scratch                    thread per face
 //   k_dc_copy      the kept faces from the scratch back into the caller's faces                  thread per face
 //   k_dc_normals   NV[v] = normalised sum of the cross products of v's faces, ascending           thread per vertex
-#include "common.cuh"
+#include "mesh_csr.cuh"
 #include "../../include/psdf_b200.h"
 
 using namespace psdf;
 
 namespace {
-constexpr unsigned kFullMask = 0xffffffffu;
-constexpr int kThreads = 256;
-constexpr int kTileItems = 8;                                 // scan: elements per thread in a tile
-constexpr long long kTile = (long long)kThreads * kTileItems;
-constexpr int kTopThreads = 1024;
-constexpr long long kHeaderBytes = 256;
-constexpr long long kIntMax = 0x7fffffffLL;
 constexpr unsigned long long kNoKey = ~0ull;
 // an edge with an end in more faces is no candidate; it bounds the work of a candidate (link condition, flip test) to kMaxFaces^2
 constexpr long long kMaxFaces = 64;
-#define ST ((cudaStream_t)stream)
-
-long long align256(long long n) { return (n + 255) & ~255LL; }
-long long scan_len(long long V, long long F) { return V + 1 > F ? V + 1 : F; }
 
 // workspace sections in order; the normals use the first five
 struct Ws {
@@ -60,42 +46,25 @@ struct Ws {
 };
 
 long long carve(void* ws, long long V, long long F, bool decimate, Ws* W) {
-    char* base = static_cast<char*>(ws);
-    long long o = 0;
-    auto take = [&](long long bytes) { char* p = base ? base + o : nullptr; o += align256(bytes); return p; };
-    const long long ntiles = (scan_len(V, F) + kTile - 1) / kTile + 1;
+    Sections s{static_cast<char*>(ws)};
     Ws w;
-    w.info = reinterpret_cast<long long*>(take(kHeaderBytes));
-    w.off = reinterpret_cast<long long*>(take(8 * (V + 1)));
-    w.deg = reinterpret_cast<int*>(take(4 * V));
-    w.adj = reinterpret_cast<int*>(take(12 * F));
-    w.tiles = reinterpret_cast<long long*>(take(8 * ntiles));
+    s.take(w.info, kHeaderBytes);
+    s.take(w.off, 8 * (V + 1));
+    s.take(w.deg, 4 * V);
+    s.take(w.adj, 12 * F);
+    s.take(w.tiles, 8 * tile_sums(V + 1 > F ? V + 1 : F));
     if (decimate) {
-        w.Q = reinterpret_cast<double*>(take(80 * V));
-        w.best = reinterpret_cast<unsigned long long*>(take(8 * V));
-        w.best2 = reinterpret_cast<unsigned long long*>(take(8 * V));
-        w.lock = reinterpret_cast<uint8_t*>(take(V));
-        w.list = reinterpret_cast<unsigned long long*>(take(8 * (V / 2 + 1)));
-        w.keys = reinterpret_cast<unsigned long long*>(take(24 * F + 8));
-        w.drop = reinterpret_cast<uint8_t*>(take(F));
+        s.take(w.Q, 80 * V);
+        s.take(w.best, 8 * V);
+        s.take(w.best2, 8 * V);
+        s.take(w.lock, V);
+        s.take(w.list, 8 * (V / 2 + 1));
+        s.take(w.keys, 24 * F + 8);
+        s.take(w.drop, F);
     }
     if (W) *W = w;
-    return o;
+    return s.size;
 }
-
-__device__ __forceinline__ long long thread_index() { return (long long)blockIdx.x * kThreads + threadIdx.x; }
-
-__device__ __forceinline__ int3 load_face(const int* __restrict__ faces, long long f) {
-    const int* p = faces + 3 * f;
-    return make_int3(p[0], p[1], p[2]);
-}
-
-__device__ __forceinline__ int corner(int3 t, int k) { return k == 0 ? t.x : (k == 1 ? t.y : t.z); }
-
-__device__ __forceinline__ bool in_range(int3 t, int V) {
-    return (unsigned)t.x < (unsigned)V && (unsigned)t.y < (unsigned)V && (unsigned)t.z < (unsigned)V;
-}
-__device__ __forceinline__ bool distinct(int3 t) { return t.x != t.y && t.y != t.z && t.z != t.x; }
 
 // vertex-indexed addresses are formed in 64 bits: 3 v and 10 v overflow int32 long before v does
 __device__ __forceinline__ double3 pos64(const float* __restrict__ verts, long long v) {
@@ -108,187 +77,34 @@ __device__ __forceinline__ double3 cross3(double3 a, double3 b) {
 }
 __device__ __forceinline__ double dot3(double3 a, double3 b) { return (a.x * b.x + a.y * b.y) + a.z * b.z; }
 
-// ---------------------------------------------------------------- checks and the CSR
-__global__ void __launch_bounds__(kThreads) k_dc_check(int V, int F, const int* __restrict__ faces, Ws W) {
-    const long long f = thread_index();
-    bool out = false, rep = false;
-    if (f < F) {
-        const int3 t = load_face(faces, f);
-        out = !in_range(t, V);
-        rep = !out && !distinct(t);
-    }
-    const unsigned mo = __ballot_sync(kFullMask, out), mr = __ballot_sync(kFullMask, rep);
-    if ((threadIdx.x & 31) == 0) {
-        if (mo) atomicAdd(reinterpret_cast<unsigned long long*>(W.info), (unsigned long long)__popc(mo));
-        if (mr) atomicAdd(reinterpret_cast<unsigned long long*>(W.info + 1), (unsigned long long)__popc(mr));
-    }
-}
-
-__global__ void __launch_bounds__(kThreads) k_dc_degree(int V, int F, const int* __restrict__ faces, Ws W) {
-    const long long f = thread_index();
-    if (f >= F) return;
-    const int3 t = load_face(faces, f);
-    if (!in_range(t, V) || !distinct(t)) return;
-    atomicAdd(W.deg + t.x, 1);
-    atomicAdd(W.deg + t.y, 1);
-    atomicAdd(W.deg + t.z, 1);
-}
-
-__device__ __forceinline__ long long scan_value(const int* cnt, const uint8_t* drop, long long n, long long i) {
-    if (i >= n) return 0;
-    return cnt ? (long long)cnt[i] : (long long)(drop[i] == 0);
-}
-
-// inclusive block prefix of x over kThreads threads -> (inclusive value, block total)
-__device__ __forceinline__ long long block_inclusive(long long x, long long& total) {
-    __shared__ long long sh[kThreads / 32];
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    for (int o = 1; o < 32; o <<= 1) {
-        const long long y = __shfl_up_sync(kFullMask, x, o);
-        if (lane >= o) x += y;
-    }
-    if (lane == 31) sh[warp] = x;
-    __syncthreads();
-    if (warp == 0) {
-        long long w = lane < kThreads / 32 ? sh[lane] : 0;
-        for (int o = 1; o < 32; o <<= 1) {
-            const long long y = __shfl_up_sync(kFullMask, w, o);
-            if (lane >= o) w += y;
-        }
-        if (lane < kThreads / 32) sh[lane] = w;
-    }
-    __syncthreads();
-    const long long r = x + (warp ? sh[warp - 1] : 0);
-    total = sh[kThreads / 32 - 1];
-    __syncthreads();
-    return r;
-}
-
-// tile sums: tiles[b] = sum of the tile's values (cnt[i], or 1 for a face not dropped)
-__global__ void __launch_bounds__(kThreads) k_dc_scan_tiles(const int* __restrict__ cnt, const uint8_t* __restrict__ drop, long long n,
-                                                            long long* __restrict__ tiles) {
-    const long long b0 = (long long)blockIdx.x * kTile + (long long)threadIdx.x * kTileItems;
-    long long s = 0;
-    for (int j = 0; j < kTileItems; j++) s += scan_value(cnt, drop, n, b0 + j);
-    long long total;
-    block_inclusive(s, total);
-    if (threadIdx.x == 0) tiles[blockIdx.x] = total;
-}
-
-// exclusive prefix of the tile sums in place, in chunks of kTopThreads; tiles[ntiles] = the total
-__global__ void __launch_bounds__(kTopThreads) k_dc_scan_top(long long* __restrict__ tiles, long long ntiles) {
-    __shared__ long long sh[kTopThreads / 32];
-    __shared__ long long carry;
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    if (threadIdx.x == 0) carry = 0;
-    __syncthreads();
-    for (long long c0 = 0; c0 < ntiles; c0 += kTopThreads) {
-        const long long i = c0 + threadIdx.x;
-        const long long v = i < ntiles ? tiles[i] : 0;
-        long long x = v;
-        for (int o = 1; o < 32; o <<= 1) {
-            const long long y = __shfl_up_sync(kFullMask, x, o);
-            if (lane >= o) x += y;
-        }
-        if (lane == 31) sh[warp] = x;
-        __syncthreads();
-        if (warp == 0) {
-            long long w = sh[lane];
-            for (int o = 1; o < 32; o <<= 1) {
-                const long long y = __shfl_up_sync(kFullMask, w, o);
-                if (lane >= o) w += y;
-            }
-            sh[lane] = w;
-        }
-        __syncthreads();
-        const long long base = carry;
-        if (i < ntiles) tiles[i] = base + x - v + (warp ? sh[warp - 1] : 0);
-        __syncthreads();
-        if (threadIdx.x == 0) carry = base + sh[kTopThreads / 32 - 1];
-        __syncthreads();
-    }
-    if (threadIdx.x == 0) tiles[ntiles] = carry;
-}
-
-// out[i] = exclusive prefix; out[n] = total when out_total
-__global__ void __launch_bounds__(kThreads) k_dc_scan_out(const int* __restrict__ cnt, const uint8_t* __restrict__ drop, long long n,
-                                                          const long long* __restrict__ tiles, long long ntiles, long long* __restrict__ out,
-                                                          int out_total) {
-    const long long b0 = (long long)blockIdx.x * kTile + (long long)threadIdx.x * kTileItems;
-    long long v[kTileItems], s = 0;
-    for (int j = 0; j < kTileItems; j++) {
-        v[j] = scan_value(cnt, drop, n, b0 + j);
-        s += v[j];
-    }
-    long long total;
-    long long run = block_inclusive(s, total) - s + tiles[blockIdx.x];
-    for (int j = 0; j < kTileItems; j++) {
-        if (b0 + j < n) out[b0 + j] = run;
-        run += v[j];
-    }
-    if (out_total && threadIdx.x == 0 && blockIdx.x == 0) out[n] = tiles[ntiles];
-}
-
-unsigned blocks(long long n) { return (unsigned)(n > 0 ? div_up(n, kThreads) : 1); }
-
-// exclusive scan of cnt [n] (or of the faces not dropped) into out; out[n] = total when out_total
-void scan(const int* cnt, const uint8_t* drop, long long n, long long* tiles, long long* out, int out_total, cudaStream_t s) {
-    const long long nt = (n + kTile - 1) / kTile;
-    if (nt > 0) k_dc_scan_tiles<<<(unsigned)nt, kThreads, 0, s>>>(cnt, drop, n, tiles);
-    k_dc_scan_top<<<1, kTopThreads, 0, s>>>(tiles, nt);
-    if (nt > 0) k_dc_scan_out<<<(unsigned)nt, kThreads, 0, s>>>(cnt, drop, n, tiles, nt, out, out_total);
-    else if (out_total) cudaMemsetAsync(out, 0, sizeof(long long), s);
-}
-
+// ---------------------------------------------------------------- the CSR
 __global__ void __launch_bounds__(kThreads) k_dc_fill(int V, int F, const int* __restrict__ faces, Ws W) {
     const long long f = thread_index();
     if (f >= F) return;
     const int3 t = load_face(faces, f);
-    if (!in_range(t, V) || !distinct(t)) return;
+    if (!valid(t, V)) return;
     W.adj[W.off[t.x] + atomicAdd(W.deg + t.x, 1)] = (int)f;
     W.adj[W.off[t.y] + atomicAdd(W.deg + t.y, 1)] = (int)f;
     W.adj[W.off[t.z] + atomicAdd(W.deg + t.z, 1)] = (int)f;
 }
 
-__device__ void sift_down(int* a, long long i, long long n) {
-    const int x = a[i];
-    for (long long c = 2 * i + 1; c < n; c = 2 * i + 1) {
-        if (c + 1 < n && a[c + 1] > a[c]) c++;
-        if (a[c] <= x) break;
-        a[i] = a[c];
-        i = c;
-    }
-    a[i] = x;
-}
-
-// heap sort, O(n log n) for a vertex of any valence (a fan of 10^5 faces sorts in about 2 * 10^6 steps)
 __global__ void __launch_bounds__(kThreads) k_dc_sort(int V, Ws W) {
     const long long v = thread_index();
     if (v >= V) return;
-    int* a = W.adj + W.off[v];
-    const long long n = W.off[v + 1] - W.off[v];
-    for (long long i = n / 2 - 1; i >= 0; i--) sift_down(a, i, n);
-    for (long long e = n - 1; e > 0; e--) {
-        const int x = a[0];
-        a[0] = a[e];
-        a[e] = x;
-        sift_down(a, 0, e);
-    }
+    heap_sort(W.adj + W.off[v], W.off[v + 1] - W.off[v]);
 }
 
 // the CSR of the valid faces (deg and off rebuilt)
 void build_csr(int V, int F, const int* faces, const Ws& W, bool sorted, cudaStream_t s) {
     cudaMemsetAsync(W.deg, 0, 4 * (size_t)V, s);
-    if (F > 0) k_dc_degree<<<blocks(F), kThreads, 0, s>>>(V, F, faces, W);
-    scan(W.deg, nullptr, V, W.tiles, W.off, 1, s);
+    if (F > 0) k_mesh_degree<<<blocks(F), kThreads, 0, s>>>(V, F, faces, W);
+    scan<Count>(W.deg, V, W.tiles, W.off, s);
     cudaMemsetAsync(W.deg, 0, 4 * (size_t)V, s);
     if (F > 0) k_dc_fill<<<blocks(F), kThreads, 0, s>>>(V, F, faces, W);
     if (sorted && V > 0) k_dc_sort<<<blocks(V), kThreads, 0, s>>>(V, W);
 }
 
 // ---------------------------------------------------------------- locks and quadrics
-__device__ __forceinline__ long long nr_faces(const Ws& W, int v) { return W.off[v + 1] - W.off[v]; }
-
 __device__ __forceinline__ bool follows(int3 t, int u, int v) {
     return (t.x == u && t.y == v) || (t.y == u && t.z == v) || (t.z == u && t.x == v);
 }
@@ -314,7 +130,7 @@ __global__ void __launch_bounds__(kThreads) k_dc_lock(int V, int F, const int* _
     const long long f = c / 3;
     const int k = (int)(c - 3 * f);
     const int3 t = load_face(faces, f);
-    if (!in_range(t, V) || !distinct(t)) return;
+    if (!valid(t, V)) return;
     const int u = corner(t, k), v = corner(t, k == 2 ? 0 : k + 1);
     const Twin tw = find_twin(W, faces, u, v);
     if (tw.nsame != 1 || tw.ntwin != 1) {
@@ -366,9 +182,6 @@ __device__ __forceinline__ double quadric_error(const double Q[10], double3 p) {
     return ((p.x * r0 + p.y * r1) + p.z * r2) + r3;
 }
 
-__device__ __forceinline__ float3 load3(const float* __restrict__ verts, long long v) {
-    return make_float3(verts[3 * v], verts[3 * v + 1], verts[3 * v + 2]);
-}
 __device__ __forceinline__ double3 to64(float3 p) { return make_double3((double)p.x, (double)p.y, (double)p.z); }
 
 // the position of the unlocked pair (a, b) with Q = Q_a + Q_b and its error
@@ -562,6 +375,11 @@ __global__ void __launch_bounds__(kThreads) k_dc_apply(int V, int* __restrict__ 
     atomicAdd(reinterpret_cast<unsigned long long*>(W.info + 3), 1ull);
 }
 
+// the scanned value of the compaction: 1 for a face no collapse dropped
+struct Kept {
+    __device__ __forceinline__ long long operator()(uint8_t drop, long long) const { return drop == 0; }
+};
+
 // faces no collapse dropped, in order: pos = exclusive prefix of the kept faces (int64 [F + 1]), the faces go to the scratch behind it
 __global__ void __launch_bounds__(kThreads) k_dc_compact(int F, const int* __restrict__ faces, Ws W) {
     const long long f = thread_index();
@@ -631,7 +449,7 @@ int psdf_mesh_decimate_begin(int V, int F, const float* verts, const int* faces,
         cudaMemsetAsync(removed, 0, (size_t)V, ST);
         cudaMemsetAsync(W.lock, 0, (size_t)V, ST);
     }
-    if (F > 0) k_dc_check<<<blocks(F), kThreads, 0, ST>>>(V, F, faces, W);
+    if (F > 0) k_mesh_check<<<blocks(F), kThreads, 0, ST>>>(V, F, faces, W);
     build_csr(V, F, faces, W, true, ST);
     if (F > 0) k_dc_lock<<<blocks(3LL * F), kThreads, 0, ST>>>(V, F, faces, W);
     if (V > 0) k_dc_quadric<<<blocks(V), kThreads, 0, ST>>>(V, faces, verts, W);
@@ -656,7 +474,7 @@ int psdf_mesh_decimate_round(int V, int F0, int F, long long allowed, float* ver
     k_dc_select<<<1, kTopThreads, 0, ST>>>(allowed, W);
     k_dc_apply<<<blocks(V / 2 + 1), kThreads, 0, ST>>>(V, faces, verts, W, removed);
     long long* pos = reinterpret_cast<long long*>(W.keys);
-    scan(nullptr, W.drop, F, W.tiles, pos, 1, ST);
+    scan<Kept>(W.drop, F, W.tiles, pos, ST);
     k_dc_compact<<<blocks(F), kThreads, 0, ST>>>(F, faces, W);
     k_dc_copy<<<blocks(F), kThreads, 0, ST>>>(F, faces, W);
     PSDF_CHECK_LAUNCH();
@@ -668,7 +486,7 @@ int psdf_mesh_normals(int V, int F, const float* verts, const int* faces, uint8_
     Ws W;
     carve(workspace, V, F, false, &W);
     cudaMemsetAsync(W.info, 0, kHeaderBytes, ST);
-    if (F > 0) k_dc_check<<<blocks(F), kThreads, 0, ST>>>(V, F, faces, W);
+    if (F > 0) k_mesh_check<<<blocks(F), kThreads, 0, ST>>>(V, F, faces, W);
     build_csr(V, F, faces, W, true, ST);
     if (V > 0) k_dc_normals<<<blocks(V), kThreads, 0, ST>>>(V, faces, verts, W, normals);
     PSDF_CHECK_LAUNCH();

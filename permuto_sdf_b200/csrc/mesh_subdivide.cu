@@ -2,39 +2,25 @@
 // so oracle/subdivide.py reproduces the output bit for bit. The rules (edges, their numbering, faces, positions) are stated in
 // include/psdf_b200.h; this file only adds how they are computed.
 //
-// Vertex -> face CSR as in mesh_decimate.cu: k_sd_degree counts the faces of each vertex, a three-kernel exclusive scan (k_sd_scan_tiles,
-// k_sd_scan_top, k_sd_scan_out) turns the counts into int64 offsets, and k_sd_fill places each face in its vertices' lists with atomics,
-// together with the two other corners of the face (the vertex's neighbours in it) at twice the offset. The face lists stay as filled
-// (every use of them is order-free); k_sd_sort sorts each vertex's neighbour list, so that the Loop rule sums the neighbours in ascending
-// index and a neighbour appears there once per face of the edge between them. The edge numbering is an exclusive scan of the corners that
-// own their edge. Faces with an index outside [0, V) or a repeated vertex are counted and never enter the CSR.
+// Vertex -> face CSR (mesh_csr.cuh): k_mesh_degree counts the faces of each vertex, the scan k_mesh_scan_* turns the counts into int64
+// offsets, and k_sd_fill places each face in its vertices' lists with atomics, together with the two other corners of the face (the
+// vertex's neighbours in it) at twice the offset. The face lists stay as filled (every use of them is order-free); k_sd_sort sorts each
+// vertex's neighbour list, so that the Loop rule sums the neighbours in ascending index and a neighbour appears there once per face of the
+// edge between them. The edge numbering is an exclusive scan of the corners that own their edge, with the same kernels. Faces with an
+// index outside [0, V) or a repeated vertex are counted by k_mesh_check and never enter the CSR.
 //
-//   k_sd_check     counts faces outside [0, V) and faces that repeat a vertex                    thread per face
-//   k_sd_degree    deg[v] += 1 for the three corners of every valid face                         thread per face
-//   k_sd_scan_*    exclusive prefix of deg (CSR offsets) or of the owning corners (edge ids)     tile / one block / tile
 //   k_sd_fill      adj[off[v] + cursor] = f, nb[2 (off[v] + cursor) ..] = the other two corners   thread per face
 //   k_sd_edge      own[c] = the smallest corner id of c's edge                                    thread per corner
 //   k_sd_sort      heap sort of each vertex's neighbour list (Loop only)                          thread per vertex
 //   k_sd_even      the old vertices: copied (midpoint) or moved by the Loop even rule              thread per vertex
 //   k_sd_odd       the edge vertex of every owning corner                                          thread per corner
 //   k_sd_faces     the four faces of every face                                                    thread per face
-#include "common.cuh"
+#include "mesh_csr.cuh"
 #include "../../include/psdf_b200.h"
 
 using namespace psdf;
 
 namespace {
-constexpr unsigned kFullMask = 0xffffffffu;
-constexpr int kThreads = 256;
-constexpr int kTileItems = 8;                                 // scan: elements per thread in a tile
-constexpr long long kTile = (long long)kThreads * kTileItems;
-constexpr int kTopThreads = 1024;
-constexpr long long kHeaderBytes = 256;
-constexpr long long kIntMax = 0x7fffffffLL;
-#define ST ((cudaStream_t)stream)
-
-long long align256(long long n) { return (n + 255) & ~255LL; }
-
 // workspace sections in order
 struct Ws {
     long long* info;          // {faces outside [0, V), faces repeating a vertex, edges, 0}
@@ -48,179 +34,31 @@ struct Ws {
 };
 
 long long carve(void* ws, long long V, long long F, Ws* W) {
-    char* base = static_cast<char*>(ws);
-    long long o = 0;
-    auto take = [&](long long bytes) { char* p = base ? base + o : nullptr; o += align256(bytes); return p; };
-    const long long n = V + 1 > 3 * F ? V + 1 : 3 * F;
-    const long long ntiles = (n + kTile - 1) / kTile + 1;
+    Sections s{static_cast<char*>(ws)};
     Ws w;
-    w.info = reinterpret_cast<long long*>(take(kHeaderBytes));
-    w.off = reinterpret_cast<long long*>(take(8 * (V + 1)));
-    w.deg = reinterpret_cast<int*>(take(4 * V));
-    w.adj = reinterpret_cast<int*>(take(12 * F));
-    w.nb = reinterpret_cast<int*>(take(24 * F));
-    w.tiles = reinterpret_cast<long long*>(take(8 * ntiles));
-    w.own = reinterpret_cast<int*>(take(12 * F));
-    w.pos = reinterpret_cast<long long*>(take(8 * (3 * F + 1)));
+    s.take(w.info, kHeaderBytes);
+    s.take(w.off, 8 * (V + 1));
+    s.take(w.deg, 4 * V);
+    s.take(w.adj, 12 * F);
+    s.take(w.nb, 24 * F);
+    s.take(w.tiles, 8 * tile_sums(V + 1 > 3 * F ? V + 1 : 3 * F));
+    s.take(w.own, 12 * F);
+    s.take(w.pos, 8 * (3 * F + 1));
     if (W) *W = w;
-    return o;
+    return s.size;
 }
 
-__device__ __forceinline__ long long thread_index() { return (long long)blockIdx.x * kThreads + threadIdx.x; }
-
-__device__ __forceinline__ int3 load_face(const int* __restrict__ faces, long long f) {
-    const int* p = faces + 3 * f;
-    return make_int3(p[0], p[1], p[2]);
-}
-
-__device__ __forceinline__ int corner(int3 t, int k) { return k == 0 ? t.x : (k == 1 ? t.y : t.z); }
-
-__device__ __forceinline__ bool in_range(int3 t, int V) {
-    return (unsigned)t.x < (unsigned)V && (unsigned)t.y < (unsigned)V && (unsigned)t.z < (unsigned)V;
-}
-__device__ __forceinline__ bool distinct(int3 t) { return t.x != t.y && t.y != t.z && t.z != t.x; }
-__device__ __forceinline__ bool valid(int3 t, int V) { return in_range(t, V) && distinct(t); }
-
-// vertex-indexed addresses are formed in 64 bits: 3 v overflows int32 long before v does
-__device__ __forceinline__ float3 load3(const float* __restrict__ verts, long long v) {
-    return make_float3(verts[3 * v], verts[3 * v + 1], verts[3 * v + 2]);
-}
 __device__ __forceinline__ void store3(float* __restrict__ verts, long long v, float3 p) {
     verts[3 * v] = p.x;
     verts[3 * v + 1] = p.y;
     verts[3 * v + 2] = p.z;
 }
 
-// ---------------------------------------------------------------- checks and the CSR
-__global__ void __launch_bounds__(kThreads) k_sd_check(int V, int F, const int* __restrict__ faces, Ws W) {
-    const long long f = thread_index();
-    bool out = false, rep = false;
-    if (f < F) {
-        const int3 t = load_face(faces, f);
-        out = !in_range(t, V);
-        rep = !out && !distinct(t);
-    }
-    const unsigned mo = __ballot_sync(kFullMask, out), mr = __ballot_sync(kFullMask, rep);
-    if ((threadIdx.x & 31) == 0) {
-        if (mo) atomicAdd(reinterpret_cast<unsigned long long*>(W.info), (unsigned long long)__popc(mo));
-        if (mr) atomicAdd(reinterpret_cast<unsigned long long*>(W.info + 1), (unsigned long long)__popc(mr));
-    }
-}
-
-__global__ void __launch_bounds__(kThreads) k_sd_degree(int V, int F, const int* __restrict__ faces, Ws W) {
-    const long long f = thread_index();
-    if (f >= F) return;
-    const int3 t = load_face(faces, f);
-    if (!valid(t, V)) return;
-    atomicAdd(W.deg + t.x, 1);
-    atomicAdd(W.deg + t.y, 1);
-    atomicAdd(W.deg + t.z, 1);
-}
-
-// the scanned value: cnt[i], or 1 for a corner that owns its edge
-__device__ __forceinline__ long long scan_value(const int* cnt, const int* own, long long n, long long i) {
-    if (i >= n) return 0;
-    return cnt ? (long long)cnt[i] : (long long)(own[i] == i);
-}
-
-// inclusive block prefix of x over kThreads threads -> (inclusive value, block total)
-__device__ __forceinline__ long long block_inclusive(long long x, long long& total) {
-    __shared__ long long sh[kThreads / 32];
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    for (int o = 1; o < 32; o <<= 1) {
-        const long long y = __shfl_up_sync(kFullMask, x, o);
-        if (lane >= o) x += y;
-    }
-    if (lane == 31) sh[warp] = x;
-    __syncthreads();
-    if (warp == 0) {
-        long long w = lane < kThreads / 32 ? sh[lane] : 0;
-        for (int o = 1; o < 32; o <<= 1) {
-            const long long y = __shfl_up_sync(kFullMask, w, o);
-            if (lane >= o) w += y;
-        }
-        if (lane < kThreads / 32) sh[lane] = w;
-    }
-    __syncthreads();
-    const long long r = x + (warp ? sh[warp - 1] : 0);
-    total = sh[kThreads / 32 - 1];
-    __syncthreads();
-    return r;
-}
-
-__global__ void __launch_bounds__(kThreads) k_sd_scan_tiles(const int* __restrict__ cnt, const int* __restrict__ own, long long n,
-                                                            long long* __restrict__ tiles) {
-    const long long b0 = (long long)blockIdx.x * kTile + (long long)threadIdx.x * kTileItems;
-    long long s = 0;
-    for (int j = 0; j < kTileItems; j++) s += scan_value(cnt, own, n, b0 + j);
-    long long total;
-    block_inclusive(s, total);
-    if (threadIdx.x == 0) tiles[blockIdx.x] = total;
-}
-
-// exclusive prefix of the tile sums in place, in chunks of kTopThreads; tiles[ntiles] = the total
-__global__ void __launch_bounds__(kTopThreads) k_sd_scan_top(long long* __restrict__ tiles, long long ntiles) {
-    __shared__ long long sh[kTopThreads / 32];
-    __shared__ long long carry;
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    if (threadIdx.x == 0) carry = 0;
-    __syncthreads();
-    for (long long c0 = 0; c0 < ntiles; c0 += kTopThreads) {
-        const long long i = c0 + threadIdx.x;
-        const long long v = i < ntiles ? tiles[i] : 0;
-        long long x = v;
-        for (int o = 1; o < 32; o <<= 1) {
-            const long long y = __shfl_up_sync(kFullMask, x, o);
-            if (lane >= o) x += y;
-        }
-        if (lane == 31) sh[warp] = x;
-        __syncthreads();
-        if (warp == 0) {
-            long long w = sh[lane];
-            for (int o = 1; o < 32; o <<= 1) {
-                const long long y = __shfl_up_sync(kFullMask, w, o);
-                if (lane >= o) w += y;
-            }
-            sh[lane] = w;
-        }
-        __syncthreads();
-        const long long base = carry;
-        if (i < ntiles) tiles[i] = base + x - v + (warp ? sh[warp - 1] : 0);
-        __syncthreads();
-        if (threadIdx.x == 0) carry = base + sh[kTopThreads / 32 - 1];
-        __syncthreads();
-    }
-    if (threadIdx.x == 0) tiles[ntiles] = carry;
-}
-
-// out[i] = exclusive prefix, out[n] = total
-__global__ void __launch_bounds__(kThreads) k_sd_scan_out(const int* __restrict__ cnt, const int* __restrict__ own, long long n,
-                                                          const long long* __restrict__ tiles, long long ntiles, long long* __restrict__ out) {
-    const long long b0 = (long long)blockIdx.x * kTile + (long long)threadIdx.x * kTileItems;
-    long long v[kTileItems], s = 0;
-    for (int j = 0; j < kTileItems; j++) {
-        v[j] = scan_value(cnt, own, n, b0 + j);
-        s += v[j];
-    }
-    long long total;
-    long long run = block_inclusive(s, total) - s + tiles[blockIdx.x];
-    for (int j = 0; j < kTileItems; j++) {
-        if (b0 + j < n) out[b0 + j] = run;
-        run += v[j];
-    }
-    if (threadIdx.x == 0 && blockIdx.x == 0) out[n] = tiles[ntiles];
-}
-
-unsigned blocks(long long n) { return (unsigned)(n > 0 ? div_up(n, kThreads) : 1); }
-
-// exclusive scan of cnt [n] (or of the owning corners of own [n]) into out [n + 1]
-void scan(const int* cnt, const int* own, long long n, long long* tiles, long long* out, cudaStream_t s) {
-    const long long nt = (n + kTile - 1) / kTile;
-    if (nt > 0) k_sd_scan_tiles<<<(unsigned)nt, kThreads, 0, s>>>(cnt, own, n, tiles);
-    k_sd_scan_top<<<1, kTopThreads, 0, s>>>(tiles, nt);
-    if (nt > 0) k_sd_scan_out<<<(unsigned)nt, kThreads, 0, s>>>(cnt, own, n, tiles, nt, out);
-    else cudaMemsetAsync(out, 0, sizeof(long long), s);
-}
+// ---------------------------------------------------------------- the CSR and the edges
+// the scanned value of the edge numbering: 1 for a corner that owns its edge
+struct Owns {
+    __device__ __forceinline__ long long operator()(int own, long long i) const { return own == i; }
+};
 
 __global__ void __launch_bounds__(kThreads) k_sd_fill(int V, int F, const int* __restrict__ faces, Ws W) {
     const long long f = thread_index();
@@ -235,8 +73,6 @@ __global__ void __launch_bounds__(kThreads) k_sd_fill(int V, int F, const int* _
         W.nb[2 * i + 1] = corner(t, k == 0 ? 2 : k - 1);
     }
 }
-
-__device__ __forceinline__ long long nr_faces(const Ws& W, int v) { return W.off[v + 1] - W.off[v]; }
 
 // the faces that hold the undirected edge {u, v} (both orders; a valid face holds it at one corner at most): their number, the smallest
 // of those corner ids, and the opposite vertex of the last such face other than f. The list of the end with fewer faces is scanned.
@@ -269,30 +105,10 @@ __global__ void __launch_bounds__(kThreads) k_sd_edge(int V, int F, const int* _
     W.own[c] = find_edge(W, faces, corner(t, k), corner(t, k == 2 ? 0 : k + 1), f).min_corner;
 }
 
-__device__ void sift_down(int* a, long long i, long long n) {
-    const int x = a[i];
-    for (long long c = 2 * i + 1; c < n; c = 2 * i + 1) {
-        if (c + 1 < n && a[c + 1] > a[c]) c++;
-        if (a[c] <= x) break;
-        a[i] = a[c];
-        i = c;
-    }
-    a[i] = x;
-}
-
-// heap sort, O(n log n) for a vertex of any valence
 __global__ void __launch_bounds__(kThreads) k_sd_sort(int V, Ws W) {
     const long long v = thread_index();
     if (v >= V) return;
-    int* a = W.nb + 2 * W.off[v];
-    const long long n = 2 * (W.off[v + 1] - W.off[v]);
-    for (long long i = n / 2 - 1; i >= 0; i--) sift_down(a, i, n);
-    for (long long e = n - 1; e > 0; e--) {
-        const int x = a[0];
-        a[0] = a[e];
-        a[e] = x;
-        sift_down(a, 0, e);
-    }
+    heap_sort(W.nb + 2 * W.off[v], 2 * (W.off[v + 1] - W.off[v]));
 }
 
 // ---------------------------------------------------------------- the new vertices and faces
@@ -383,16 +199,16 @@ int psdf_mesh_subdivide_count(int V, int F, const int* faces, uint8_t* workspace
     cudaMemsetAsync(W.info, 0, kHeaderBytes, ST);
     cudaMemsetAsync(W.deg, 0, 4 * (size_t)V, ST);
     if (F > 0) {
-        k_sd_check<<<blocks(F), kThreads, 0, ST>>>(V, F, faces, W);
-        k_sd_degree<<<blocks(F), kThreads, 0, ST>>>(V, F, faces, W);
+        k_mesh_check<<<blocks(F), kThreads, 0, ST>>>(V, F, faces, W);
+        k_mesh_degree<<<blocks(F), kThreads, 0, ST>>>(V, F, faces, W);
     }
-    scan(W.deg, nullptr, V, W.tiles, W.off, ST);
+    scan<Count>(W.deg, V, W.tiles, W.off, ST);
     cudaMemsetAsync(W.deg, 0, 4 * (size_t)V, ST);
     if (F > 0) {
         k_sd_fill<<<blocks(F), kThreads, 0, ST>>>(V, F, faces, W);
         k_sd_edge<<<blocks(3LL * F), kThreads, 0, ST>>>(V, F, faces, W);
     }
-    scan(nullptr, W.own, 3LL * F, W.tiles, W.pos, ST);
+    scan<Owns>(W.own, 3LL * F, W.tiles, W.pos, ST);
     cudaMemcpyAsync(W.info + 2, W.pos + 3LL * F, sizeof(long long), cudaMemcpyDeviceToDevice, ST);
     PSDF_CHECK_LAUNCH();
     return PSDF_OK;

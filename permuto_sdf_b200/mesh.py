@@ -27,6 +27,31 @@ _INT_MAX = 2 ** 31 - 1
 _CC_HEADER = 256
 
 
+def _check_f(fn, Fc):
+    if not isinstance(Fc, torch.Tensor) or Fc.dtype != torch.int32:
+        raise RuntimeError("%s: F must be an int32 tensor of shape [F,3], got %s" % (fn, getattr(Fc, "dtype", type(Fc).__name__)))
+    if Fc.dim() != 2 or Fc.shape[1] != 3:
+        raise RuntimeError("%s: F must have shape [F,3], got %s" % (fn, list(Fc.shape)))
+
+
+def _check_sizes(fn, nv, nf):
+    if nv > _INT_MAX or nf > _INT_MAX:
+        raise RuntimeError("%s: %d vertices and %d faces; both must be below 2^31" % (fn, nv, nf))
+
+
+def _checked_call(fn, workspace_bytes, entry, nv, nf, args, out=()):
+    """entry(nv, nf, *args, workspace, *out) on a new workspace of workspace_bytes(nv, nf) bytes on the device of args[-1]; raises on the
+    faces with an index outside [0, nv) or a repeated vertex that it counted into info[0], info[1] -> (workspace, info[2])"""
+    ws = torch.empty(int(workspace_bytes(nv, nf)), dtype=torch.uint8, device=args[-1].device)
+    call(entry, nv, nf, *args, ws, *out)
+    bad, rep, info2 = ws[:24].view(torch.int64).tolist()
+    if bad:
+        raise RuntimeError("%s: %d faces have a vertex index outside [0, %d)" % (fn, bad, nv))
+    if rep:
+        raise RuntimeError("%s: %d faces repeat a vertex" % (fn, rep))
+    return ws, info2
+
+
 def _slab_slices(N0, N1, N2):
     return max(1, min(N0 - 1, _SLAB_POINTS // (N1 * N2)))
 
@@ -121,17 +146,13 @@ class Mesh:
     def _components(self, fn):
         """psdf_mesh_components of F -> (workspace, number of components); raises on faces that index outside [0, V)"""
         Fc, V = self.F, self.V
-        if not isinstance(Fc, torch.Tensor) or Fc.dtype != torch.int32:
-            raise RuntimeError("%s: F must be an int32 tensor of shape [F,3], got %s" % (fn, getattr(Fc, "dtype", type(Fc).__name__)))
-        if Fc.dim() != 2 or Fc.shape[1] != 3:
-            raise RuntimeError("%s: F must have shape [F,3], got %s" % (fn, list(Fc.shape)))
+        _check_f(fn, Fc)
         if not Fc.is_cuda:
             raise RuntimeError("%s: F must be a CUDA tensor (there is no CPU path)" % fn)
         if not isinstance(V, torch.Tensor) or V.device != Fc.device:
             raise RuntimeError("%s: V must be a tensor on F's device %s" % (fn, Fc.device))
         nv, nf = V.shape[0], Fc.shape[0]
-        if nv > _INT_MAX or nf > _INT_MAX:
-            raise RuntimeError("%s: %d vertices and %d faces; both must be below 2^31" % (fn, nv, nf))
+        _check_sizes(fn, nv, nf)
         with torch.cuda.device(Fc.device):
             ws = torch.empty(int(load_library().psdf_mesh_components_workspace_bytes(nv, nf)), dtype=torch.uint8, device=Fc.device)
             call("psdf_mesh_components", nv, nf, Fc.contiguous(), ws)
@@ -181,17 +202,12 @@ class Mesh:
             raise RuntimeError("%s: V must be a float32 tensor of shape [V,3], got %s" % (fn, getattr(V, "dtype", type(V).__name__)))
         if V.dim() != 2 or V.shape[1] != 3:
             raise RuntimeError("%s: V must have shape [V,3], got %s" % (fn, list(V.shape)))
-        if not isinstance(Fc, torch.Tensor) or Fc.dtype != torch.int32:
-            raise RuntimeError("%s: F must be an int32 tensor of shape [F,3], got %s" % (fn, getattr(Fc, "dtype", type(Fc).__name__)))
-        if Fc.dim() != 2 or Fc.shape[1] != 3:
-            raise RuntimeError("%s: F must have shape [F,3], got %s" % (fn, list(Fc.shape)))
+        _check_f(fn, Fc)
         if not V.is_cuda:
             raise RuntimeError("%s: V must be a CUDA tensor (there is no CPU path)" % fn)
         if Fc.device != V.device:
             raise RuntimeError("%s: F must be on V's device %s, got %s" % (fn, V.device, Fc.device))
-        nv, nf = V.shape[0], Fc.shape[0]
-        if nv > _INT_MAX or nf > _INT_MAX:
-            raise RuntimeError("%s: %d vertices and %d faces; both must be below 2^31" % (fn, nv, nf))
+        _check_sizes(fn, V.shape[0], Fc.shape[0])
         if not bool(torch.isfinite(V).all()):
             raise RuntimeError("%s: V has values that are not finite" % fn)
         return V.contiguous(), Fc.contiguous()
@@ -210,14 +226,9 @@ class Mesh:
         dev = V.device
         with torch.cuda.device(dev):
             V, Fc = V.clone(), Fc.clone()
-            ws = torch.empty(int(load_library().psdf_mesh_decimate_workspace_bytes(nv, nf)), dtype=torch.uint8, device=dev)
             removed = torch.empty(nv, dtype=torch.bool, device=dev)
-            call("psdf_mesh_decimate_begin", nv, nf, V, Fc, ws, removed)
-            bad, rep = ws[:16].view(torch.int64).tolist()
-            if bad:
-                raise RuntimeError("%s: %d faces have a vertex index outside [0, %d)" % (fn, bad, nv))
-            if rep:
-                raise RuntimeError("%s: %d faces repeat a vertex" % (fn, rep))
+            ws, _ = _checked_call(fn, load_library().psdf_mesh_decimate_workspace_bytes, "psdf_mesh_decimate_begin", nv, nf, (V, Fc),
+                                  (removed,))
             cur, rounds = nf, 0
             while True:
                 allowed = (cur - target + 1) // 2
@@ -259,14 +270,8 @@ class Mesh:
         V, Fc = self._check_vf(fn)
         nv, nf = V.shape[0], Fc.shape[0]
         with torch.cuda.device(V.device):
-            ws = torch.empty(int(load_library().psdf_mesh_normals_workspace_bytes(nv, nf)), dtype=torch.uint8, device=V.device)
             NV = torch.empty_like(V)
-            call("psdf_mesh_normals", nv, nf, V, Fc, ws, NV)
-            bad, rep = ws[:16].view(torch.int64).tolist()
-        if bad:
-            raise RuntimeError("%s: %d faces have a vertex index outside [0, %d)" % (fn, bad, nv))
-        if rep:
-            raise RuntimeError("%s: %d faces repeat a vertex" % (fn, rep))
+            _checked_call(fn, load_library().psdf_mesh_normals_workspace_bytes, "psdf_mesh_normals", nv, nf, (V, Fc), (NV,))
         self.NV = NV
         return self
 
@@ -290,13 +295,7 @@ class Mesh:
         with torch.cuda.device(V.device):
             for _ in range(rounds):
                 nv, nf = V.shape[0], Fc.shape[0]
-                ws = torch.empty(int(load_library().psdf_mesh_subdivide_workspace_bytes(nv, nf)), dtype=torch.uint8, device=V.device)
-                call("psdf_mesh_subdivide_count", nv, nf, Fc, ws)
-                bad, rep, E = ws[:24].view(torch.int64).tolist()
-                if bad:
-                    raise RuntimeError("%s: %d faces have a vertex index outside [0, %d)" % (fn, bad, nv))
-                if rep:
-                    raise RuntimeError("%s: %d faces repeat a vertex" % (fn, rep))
+                ws, E = _checked_call(fn, load_library().psdf_mesh_subdivide_workspace_bytes, "psdf_mesh_subdivide_count", nv, nf, (Fc,))
                 if nv + E > _INT_MAX:
                     raise RuntimeError("%s: %d vertices and %d edges make %d vertices; V must stay below 2^31" % (fn, nv, E, nv + E))
                 Vn = torch.empty(nv + E, 3, dtype=torch.float32, device=V.device)

@@ -1,6 +1,6 @@
 """Mesh decimation and vertex normals without a GPU: the argument checks of Mesh.decimate and Mesh.recalculate_normals, the C ABI's
-entry points and their limits, a compile check that the kernels of csrc/mesh_decimate.cu exist and do not spill, and the properties of
-oracle/decimate.py on small marching-cubes meshes."""
+entry points and their limits, a compile check that the kernels of csrc/mesh_decimate.cu (its own and those of csrc/mesh_csr.cuh it
+launches) exist and do not spill, and the properties of oracle/decimate.py on small marching-cubes meshes."""
 import ctypes
 import os
 import shutil
@@ -20,7 +20,8 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 NVCC = shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
 ENTRY_POINTS = ("psdf_mesh_decimate_workspace_bytes", "psdf_mesh_normals_workspace_bytes", "psdf_mesh_decimate_begin",
                 "psdf_mesh_decimate_round", "psdf_mesh_normals")
-KERNELS = ("k_dc_check", "k_dc_degree", "k_dc_scan_tiles", "k_dc_scan_top", "k_dc_scan_out", "k_dc_fill", "k_dc_sort", "k_dc_lock",
+KERNELS = ("k_mesh_check<Ws>", "k_mesh_degree<Ws>", "k_mesh_scan_tiles<Count, int>", "k_mesh_scan_tiles<Kept, unsigned char>",
+           "k_mesh_scan_top", "k_mesh_scan_out<Count, int>", "k_mesh_scan_out<Kept, unsigned char>", "k_dc_fill", "k_dc_sort", "k_dc_lock",
            "k_dc_quadric", "k_dc_key", "k_dc_best2", "k_dc_choose", "k_dc_select", "k_dc_apply", "k_dc_compact", "k_dc_copy", "k_dc_normals")
 
 
@@ -129,7 +130,7 @@ def kernels():
 
 
 def test_kernels_are_built_and_do_not_spill(kernels):
-    dc = {k: r for k, r in kernels.items() if k.startswith("k_dc_")}
+    dc = {k: r for k, r in kernels.items() if k.startswith(("k_dc_", "k_mesh_"))}
     assert set(dc) == set(KERNELS)
     spilling = {k: (r["spill_st"], r["spill_ld"]) for k, r in dc.items() if r["spill_st"] or r["spill_ld"]}
     assert not spilling, spilling

@@ -1,6 +1,7 @@
 """Mesh subdivision without a GPU: the argument checks of Mesh.upsample, the C ABI's entry points and their limits, a compile check that
-the kernels of csrc/mesh_subdivide.cu exist and do not spill, and the properties of oracle/subdivide.py: counts, Euler characteristic,
-closed and oriented meshes, exact midpoints, a tetrahedron computed by hand in both modes, a flat open grid and a non-manifold fan."""
+the kernels of csrc/mesh_subdivide.cu (its own and those of csrc/mesh_csr.cuh it launches) exist and do not spill, and the properties of
+oracle/subdivide.py: counts, Euler characteristic, closed and oriented meshes, exact midpoints, a tetrahedron computed by hand in both
+modes, a flat open grid and a non-manifold fan."""
 import ctypes
 import os
 import shutil
@@ -19,8 +20,9 @@ from permuto_sdf_b200.mesh import Mesh
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 NVCC = shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
 ENTRY_POINTS = ("psdf_mesh_subdivide_workspace_bytes", "psdf_mesh_subdivide_count", "psdf_mesh_subdivide_emit")
-KERNELS = ("k_sd_check", "k_sd_degree", "k_sd_scan_tiles", "k_sd_scan_top", "k_sd_scan_out", "k_sd_fill", "k_sd_edge", "k_sd_sort",
-           "k_sd_even", "k_sd_odd", "k_sd_faces")
+KERNELS = ("k_mesh_check<Ws>", "k_mesh_degree<Ws>", "k_mesh_scan_tiles<Count, int>", "k_mesh_scan_tiles<Owns, int>", "k_mesh_scan_top",
+           "k_mesh_scan_out<Count, int>", "k_mesh_scan_out<Owns, int>", "k_sd_fill", "k_sd_edge", "k_sd_sort", "k_sd_even", "k_sd_odd",
+           "k_sd_faces")
 
 
 def tri_mesh(V=None, F=None):
@@ -97,7 +99,7 @@ def kernels():
 
 
 def test_kernels_are_built_and_do_not_spill(kernels):
-    sd = {k: r for k, r in kernels.items() if k.startswith("k_sd_")}
+    sd = {k: r for k, r in kernels.items() if k.startswith(("k_sd_", "k_mesh_"))}
     assert set(sd) == set(KERNELS)
     spilling = {k: (r["spill_st"], r["spill_ld"]) for k, r in sd.items() if r["spill_st"] or r["spill_ld"]}
     assert not spilling, spilling
