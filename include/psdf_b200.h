@@ -669,6 +669,29 @@ long long psdf_mesh_subdivide_workspace_bytes(long long nr_vertices, long long n
 int psdf_mesh_subdivide_count(int V, int F, const int* faces, uint8_t* workspace, void* stream);
 int psdf_mesh_subdivide_emit(int V, int F, int smooth, const float* verts, const int* faces, uint8_t* workspace, float* verts_out,
                              int* faces_out, void* stream);
+
+/* ---------------------------------------------------------------- image metrics (csrc/image_metrics.cu)
+ * Per-image PSNR and SSIM of the reference's experiments/evaluation/evaluate_psnr.py, which scores each frame with piq.psnr and piq.ssim
+ * (data_range = 1; kernel 11, sigma 1.5, k1 0.01, k2 0.03, downsampling on). x (the prediction) and y (the ground truth) are float images of
+ * B x C x H x W values, each stored as [B,C,H,W] (nhwc = 0) or [B,H,W,C] (nhwc = 1); mask [B,H,W] or NULL. Offsets are 64-bit.
+ * Before anything else, in this order:
+ *   quantize_x != 0: x = min(255, max(0, rne(x * 255))) / 255 in fp32, create_my_images.py's 8-bit PNG round trip;
+ *   mask: x = x m, y = y m (masked-out pixels stay in the means as exact matches, as in evaluate_psnr.py).
+ * Everything after that is fp64:
+ *   psdf_image_psnr: out[b] = -10 log10(mse + 1e-8), mse = the mean of (x - y)^2 over C, H, W at full resolution (piq.psnr);
+ *   psdf_image_ssim: f = max(1, round(min(H, W) / 256)) (round half to even); f > 1 average-pools both images by f x f with stride f,
+ *     dropping the remainder (F.avg_pool2d); H / f and W / f below 11: PSDF_ERR_ARG. Valid-mode sums with the normalised 11 x 11 Gaussian
+ *     window give mu_x, mu_y, s_xx = W(x^2) - mu_x^2, s_yy, s_xy = W(xy) - mu_x mu_y; cs = (2 s_xy + c2) / (s_xx + s_yy + c2),
+ *     ss = (2 mu_x mu_y + c1) / (mu_x^2 + mu_y^2 + c1) cs with c1 = 0.01^2, c2 = 0.03^2; out[b] = the mean of ss over C and the
+ *     (H/f - 10)(W/f - 10) positions (piq.ssim's _ssim_per_channel, then the mean over channels).
+ * out [B] (double). Partial sums go to the workspace, psdf_image_metrics_workspace_bytes(B, C, H, W) bytes (PSDF_ERR_ARG for a size below
+ * 1, PSDF_ERR_UNSUPPORTED for B > 65535 or a size of 2^31 or more); their number depends only on the image size and they are added in a
+ * fixed order, so a call gives the same bits on every run. Invalid arguments: PSDF_ERR_ARG before anything is launched. */
+long long psdf_image_metrics_workspace_bytes(long long B, long long C, long long H, long long W);
+int psdf_image_psnr(int B, int C, int H, int W, const float* x, int x_nhwc, const float* y, int y_nhwc, const float* mask, int quantize_x,
+                    double* out, uint8_t* workspace, void* stream);
+int psdf_image_ssim(int B, int C, int H, int W, const float* x, int x_nhwc, const float* y, int y_nhwc, const float* mask, int quantize_x,
+                    double* out, uint8_t* workspace, void* stream);
 /* psdf_adamw_step over up to 8 parameter groups in one launch: device-resident step count, per-group hyper_dev [2] = {lr, weight_decay};
  * gradients scaled by grad_scale and reset to zero. n_l % 4 == 0, 16-byte aligned pointers. n and the five tables of device addresses
  * (one entry per group) are HOST arrays. The step used is step_dev[0] + step_offset (step_offset = 1: the counter is advanced afterwards

@@ -11,6 +11,7 @@ sphere-tracing hot path behind the reference's own Python operator API.
     permuto_sdf_b200.NerfTrainer              NeRF training (train_nerf.py) on the fused kernels
     permuto_sdf_b200.extract_mesh_from_sdf_model / marching_cubes / Mesh   meshes from a trained SDF or a volume on the GPU
     permuto_sdf_b200.extract_mesh_from_density_model   meshes from a trained NeRF's density (NerfTrainer.model) on the GPU
+    permuto_sdf_b200.psnr / ssim              image metrics of evaluate_psnr.py on the GPU (metrics.py; Trainer.evaluate scores frames)
 
 All device work goes through the C ABI in include/psdf_b200.h (libpsdf_b200.so, hand-written CUDA).
 There is no CPU or PyTorch fallback: importing is cheap, but any op raises if the library is missing
@@ -36,6 +37,9 @@ def __getattr__(name):
     if name in ("Mesh", "marching_cubes", "extract_mesh_from_sdf_model", "extract_mesh_from_density_model"):
         from . import mesh
         return getattr(mesh, name)
+    if name in ("psnr", "ssim"):
+        from . import metrics
+        return getattr(metrics, name)
     if name == "AABB":
         from .permuto_sdf import AABB
         return AABB

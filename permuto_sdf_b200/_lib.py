@@ -97,7 +97,7 @@ def _dtypes():
     if _DT is None:
         import torch
         _DT = {"float": (torch.float32,), "int": (torch.int32,), "uint8_t": (torch.uint8, torch.bool), "uint64_t": (torch.int64, torch.uint64),
-               "long long": (torch.int64,)}
+               "long long": (torch.int64,), "double": (torch.float64,)}
     return _DT
 
 

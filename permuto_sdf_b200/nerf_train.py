@@ -390,6 +390,31 @@ class NerfTrainer:
                  None, 0.0, out[0][a:b], out[2][a:b], torch.empty(b - a, 1, device=o.device), pbg, None, None, None)
         return tuple(out)
 
+    def _frame_models(self):
+        return (*self.models, self.model_colorcal)
+
+    def _frame_render(self, chunk_size):
+        return (lambda o, d: self.render(o, d)) if chunk_size is None else (lambda o, d: self.render(o, d, chunk_size))
+
+    def render_frame(self, tensor_reel, img_idx, chunk_size=None):
+        """Every pixel of image img_idx of a TensorReel (the rays of PermutoSDF.rays_from_reel_indices) through render() with the models in
+        eval mode (train flags restored afterwards). Changes no parameter, .grad, grid, counter or generator.
+        -> (rgb [1,3,H,W], weights sum [1,1,H,W]), channels-last views of the rendered rows"""
+        from . import metrics
+        (rgb, _, wsum), H, W = metrics.render_frame("NerfTrainer.render_frame", tensor_reel, img_idx, self._frame_models(),
+                                                    self._frame_render(chunk_size))
+        return metrics.image(rgb, H, W), metrics.image(wsum, H, W)
+
+    def evaluate(self, tensor_reel, image_indices=None, chunk_size=None, quantize=True):
+        """PSNR and SSIM of rendered frames (render_frame), scored as evaluate_psnr.py scores them: the colour 8-bit quantized when
+        `quantize`, prediction and the reel's rgb multiplied by the reel's mask when it has one, then metrics.psnr and metrics.ssim.
+        image_indices None: every image of the reel.
+        -> {"image_indices", "psnr", "ssim" (fp64 per image, on the host), "psnr_mean", "ssim_mean"}"""
+        from .metrics import evaluate_frames
+        render = self._frame_render(chunk_size)
+        return evaluate_frames("NerfTrainer.evaluate", tensor_reel, image_indices, quantize, self._frame_models(),
+                               lambda o, d: render(o, d)[0])
+
     def train(self):
         for m in self.models:
             m.train()

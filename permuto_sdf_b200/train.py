@@ -703,6 +703,37 @@ class Trainer:
         return self._render.render(ray_origins, ray_dirs, DEFAULT_CHUNK if chunk_size is None else chunk_size,
                                    self.iter_nr if iter_nr_for_anneal is None else iter_nr_for_anneal, cos_anneal_ratio, forced_variance)
 
+    def _frame_models(self):
+        return (self.model_sdf, self.model_rgb, self.model_bg, self.model_colorcal)
+
+    def _frame_render(self, chunk_size):
+        """render() with the settings of create_my_images.py: iteration 9999999, cos_anneal_ratio 1, hp.forced_variance_finish"""
+        from .metrics import FRAME_ITER
+        return lambda o, d: self.render(o, d, chunk_size, FRAME_ITER, 1.0, self.hp.forced_variance_finish)
+
+    def render_frame(self, tensor_reel, img_idx, chunk_size=None):
+        """Every pixel of image img_idx of a TensorReel, rendered as create_my_images.py renders a frame: the rays of
+        PermutoSDF.rays_from_reel_indices, the models in eval mode (train flags restored afterwards), iteration 9999999, cos_anneal_ratio 1,
+        hp.forced_variance_finish. Changes no parameter, .grad, occupancy grid, iteration counter or generator; raises as render() does.
+        -> (rgb [1,3,H,W], unit normals in camera coordinates [1,3,H,W], weights sum [1,1,H,W]), channels-last views of the rendered rows.
+        The normals are F.normalize(R n) with R the rotation of tf_cam_world = tf_world_cam^-1, so a zero normal stays zero."""
+        from . import metrics
+        (rgb, _, normals, wsum), H, W = metrics.render_frame("Trainer.render_frame", tensor_reel, img_idx, self._frame_models(),
+                                                             self._frame_render(chunk_size))
+        tf = tensor_reel.tf_world_cam_reel[int(img_idx)]
+        R = torch.linalg.inv(tf.cpu())[0:3, 0:3].to(normals.device)
+        normals = F.normalize(torch.matmul(R, normals.t()).t(), dim=1)
+        return metrics.image(rgb, H, W), metrics.image(normals, H, W), metrics.image(wsum, H, W)
+
+    def evaluate(self, tensor_reel, image_indices=None, chunk_size=None, quantize=True):
+        """PSNR and SSIM of rendered frames, as create_my_images.py renders them (render_frame) and evaluate_psnr.py scores them: the
+        colour 8-bit quantized when `quantize` (the PNG round trip), prediction and the reel's rgb multiplied by the reel's mask when it
+        has one, then metrics.psnr and metrics.ssim. image_indices None: every image of the reel.
+        -> {"image_indices", "psnr", "ssim" (fp64 per image, on the host), "psnr_mean", "ssim_mean"}"""
+        from .metrics import evaluate_frames
+        render = self._frame_render(chunk_size)
+        return evaluate_frames("Trainer.evaluate", tensor_reel, image_indices, quantize, self._frame_models(), lambda o, d: render(o, d)[0])
+
     def step(self, ray_origins, ray_dirs, gt_rgb, gt_mask, img_indices, update_occupancy=None, optimizer_step=True):
         """forward + losses + backward (+ optimizer). Returns the detached loss tensor (no host sync)."""
         self.model_sdf.train(); self.model_rgb.train()
