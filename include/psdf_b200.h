@@ -670,6 +670,52 @@ int psdf_mesh_subdivide_count(int V, int F, const int* faces, uint8_t* workspace
 int psdf_mesh_subdivide_emit(int V, int F, int smooth, const float* verts, const int* faces, uint8_t* workspace, float* verts_out,
                              int* faces_out, void* stream);
 
+/* ---------------------------------------------------------------- mesh ray casting (csrc/mesh_raycast.cu)
+ * Any-hit queries of rays against the triangles of verts [V,3] (float) and faces [F,3] (int32) through a linear BVH, and per-vertex
+ * ambient occlusion. Built with -fmad=false; oracle/raycast.py restates the triangle test and checks every answer by brute force.
+ * Ray-triangle test (two-sided Moller-Trumbore, fp32, each operation rounded as written; dot(a, b) = (ax bx + ay by) + az bz, cross(a, b) =
+ *   (ay bz - az by, az bx - ax bz, ax by - ay bx)): e1 = p1 - p0, e2 = p2 - p0, pv = cross(d, e2), det = dot(e1, pv); det == 0 or NaN
+ *   misses. inv = 1.0f / det, tv = o - p0, u = dot(tv, pv) * inv, miss unless 0 <= u <= 1; qv = cross(tv, e1), v = dot(d, qv) * inv, miss
+ *   unless v >= 0 and u + v <= 1; t = dot(e2, qv) * inv, hit iff tnear < t < tfar. A face that repeats a vertex has det == 0: never hit.
+ * A ray is occluded exactly when some triangle passes the test; the tree only chooses which triangles are tested, so it changes no answer
+ *   as long as its box test passes every box that holds a passing triangle:
+ *   - Boxes are the exact fp32 min / max of their triangles' corners, grown at query time by pad = 2^-12 (s + max |o_k|), s the largest
+ *     |coordinate| of the mesh. A passing (u, v, t) puts o + t d within |r| of the triangle, |r| <= c eps |tv| |d| |e1| |e2| / |det|
+ *     (c ~ 10, eps = 2^-24, |tv| <= sqrt(3) (s + max |o_k|)); that is below pad unless the ray lies within about 1 degree of the triangle's
+ *     plane (|det| < 2^-6 |d| |e1| |e2|). A ray that close to a far triangle's plane can pass the test by rounding alone, anywhere in that
+ *     plane; such far passes are the one case where the answer can differ from the brute-force one. Zero-thickness boxes (axis-aligned
+ *     triangles) are thickened by the pad, so origins on their planes lie inside.
+ *   - Slab test: per axis, d_k == 0 requires lo_k - pad <= o_k <= hi_k + pad exactly (no 1/0, no 0 * inf); a d_k whose reciprocal is not
+ *     finite leaves that axis out (conservative); otherwise the slab interval of (bound - o_k) * (1 / d_k). The box passes when
+ *     max(tnear, slab starts) <= t1 + |t1| 2^-20 with t1 = min(tfar, slab ends): 2^-20 exceeds the 2 gamma_3 that covers the rounding of
+ *     the slab arithmetic (Ize, Robust BVH ray traversal, 2013).
+ *   - Traversal stack: 64 entries. Keys are the 30-bit Morton code of each centroid (within the centroids' bounds) with the sorted position
+ *     breaking ties, so every internal node's common prefix length lies in [2, 63] and grows strictly from parent to child: at most 62
+ *     internal nodes lie on a path, and only internal nodes are pushed, at most one per level.
+ * Build: the faces are sorted by Morton code (four stable 8-bit radix passes), Karras' radix tree (2012) gives the F - 1 internal nodes
+ *   (root 0), and the boxes are refit bottom-up. Faces with an index outside [0, V) are counted into info[0] (faces that repeat a vertex
+ *   into info[1]; they are allowed) and get an empty box and NaN corners, so nothing out of range is read; the caller refuses them. F = 0
+ *   (nothing is hit), F = 1, equal centroids and all faces at one point build a valid tree.
+ * Workspace: psdf_mesh_bvh_workspace_bytes(V, F) ~ 152 B per face + 4 B per vertex (sections each padded to 256 B): int64 info[4] at byte
+ *   0 = {faces with an index outside [0, V), faces that repeat a vertex, 0, 0}, uint32 bounds [8] (ordered keys of the centroid bounds, the
+ *   bits of s), uint32 keys [2][F], int32 face ids [2][F], int32 radix histogram [256 ceil(F / 256)], int64 its prefix [+ 1], int64 scan
+ *   tile sums, nodes [F - 1] of 64 B (both children's boxes, then the children; child >= F - 1 is leaf child - (F - 1)), int32 parents
+ *   [2F - 1], int32 refit flags [F - 1], the sorted triangles [F] of 48 B (p0, p1, p2), int32 hit counts [V]. PSDF_ERR_UNSUPPORTED when V
+ *   or F is 2^31 or more, PSDF_ERR_ARG when negative.
+ * psdf_mesh_bvh_build: fills the workspace; queries pass the same V and F and read it.
+ * psdf_mesh_occluded: hit_out[r] (uint8) = 1 when ray r (origins [R,3], dirs [R,3], any length) is occluded within (tnear, tfar); R is
+ *   64-bit (PSDF_ERR_UNSUPPORTED above 256 (2^31 - 1)).
+ * psdf_mesh_ambient_occlusion: V S rays, one per (vertex i, direction s), 64-bit ray ids: origin verts[i], direction dirs[s] [S,3], negated
+ *   when dot(dirs[s], normals[i]) < 0 (fp32 as above), tnear = 1e-4f, tfar = +inf; vis_out[i] = float(S - hits) / float(S). Hits are
+ *   integer counts, so the result is the same bits on every run.
+ * Cost: build O(F) (sort, tree and refit are one pass each); a query visits the nodes whose padded boxes the ray meets. */
+long long psdf_mesh_bvh_workspace_bytes(long long nr_vertices, long long nr_faces);
+int psdf_mesh_bvh_build(int V, int F, const float* verts, const int* faces, uint8_t* workspace, void* stream);
+int psdf_mesh_occluded(int V, int F, long long R, const float* origins, const float* dirs, float tnear, float tfar, const uint8_t* workspace,
+                       uint8_t* hit_out, void* stream);
+int psdf_mesh_ambient_occlusion(int V, int F, int S, const float* verts, const float* normals, const float* dirs, uint8_t* workspace,
+                                float* vis_out, void* stream);
+
 /* ---------------------------------------------------------------- image metrics (csrc/image_metrics.cu)
  * Per-image PSNR and SSIM of the reference's experiments/evaluation/evaluate_psnr.py, which scores each frame with piq.psnr and piq.ssim
  * (data_range = 1; kernel 11, sigma 1.5, k1 0.01, k2 0.03, downsampling on). x (the prediction) and y (the ground truth) are float images of

@@ -11,8 +11,12 @@ Mesh.decimate reduces a mesh to a target face count by quadric edge collapse, in
 (csrc/mesh_decimate.cu), and Mesh.recalculate_normals sets NV from the faces; both give the same bits on every run.
 Mesh.load reads PLY, OBJ and STL files on the host, the torch ops below weld, compact and place a mesh as train_sdf_from_mesh.py does,
 and Mesh.upsample runs midpoint or Loop subdivision on the GPU (csrc/mesh_subdivide.cu), the same bits on every run.
+Mesh.occluded and Mesh.ambient_occlusion cast rays against the faces through a linear BVH on the GPU (csrc/mesh_raycast.cu), and
+load_mesh_sequence assembles the point sequence of train_4d_sdf.py from a folder of meshes.
 """
 import math
+import os
+import re
 
 import numpy as np
 import torch
@@ -308,6 +312,69 @@ class Mesh:
             self.recalculate_normals()
         return self
 
+    # ------------------------------------------------------------------ ray casting
+    def _bvh(self, fn):
+        """the BVH of the faces (psdf_mesh_bvh_build) -> (V, F, workspace); raises on faces with an index outside [0, V)"""
+        V, Fc = self._check_vf(fn)
+        nv, nf = V.shape[0], Fc.shape[0]
+        ws = torch.empty(int(load_library().psdf_mesh_bvh_workspace_bytes(nv, nf)), dtype=torch.uint8, device=V.device)
+        call("psdf_mesh_bvh_build", nv, nf, V, Fc, ws)
+        bad = int(ws[:8].view(torch.int64).item())
+        if bad:
+            raise RuntimeError("%s: %d faces have a vertex index outside [0, %d)" % (fn, bad, nv))
+        return V, Fc, ws
+
+    def occluded(self, origins, dirs, tnear=1e-4, tfar=math.inf):
+        """any-hit ray casting on the GPU: bool [R], True where ray r (origins [R,3], dirs [R,3], float32 CUDA tensors on V's device with
+        finite values; dirs need not be unit) passes the two-sided fp32 ray-triangle test of include/psdf_b200.h against some face at a
+        parameter t with tnear < t < tfar (both rounded to fp32). The answer is that of testing every face; a BVH built on each call only
+        chooses which faces are tested. Faces that repeat a vertex are never hit. V and F are checked as decimate checks them, except that
+        faces repeating a vertex are allowed."""
+        fn = "Mesh.occluded"
+        o, d = _check_rays(fn, origins, dirs, self.V)
+        if not (math.isfinite(float(tnear)) and not math.isnan(float(tfar))):
+            raise RuntimeError("%s: tnear must be finite and tfar a number, got %r, %r" % (fn, tnear, tfar))
+        with torch.cuda.device(o.device):
+            V, Fc, ws = self._bvh(fn)
+            hit = torch.empty(o.shape[0], dtype=torch.uint8, device=o.device)
+            call("psdf_mesh_occluded", V.shape[0], Fc.shape[0], o.shape[0], o, d, float(tnear), float(tfar), ws, hit)
+        return hit.bool()
+
+    def ambient_occlusion(self, nr_samples=100):
+        """the visible fraction of every vertex, float32 [V]: of the nr_samples rays from V[i] along the fixed Fibonacci directions
+        (fibonacci_directions: the same for every vertex), each negated when it points against NV[i] (fp32 dot < 0), the share that
+        hits no face at 1e-4 < t < inf, float(S - hits) / float(S). The same bits on every run. NV is required (recalculate_normals).
+        This is what the reference reads as compute_embree_ao(n) then C[:, 0]. EasyPBR's compute_embree_ao is not in the reference's
+        checkout; as far as we recall it wraps libigl's embree ambient_occlusion with random directions and stores 1 - the hit fraction,
+        so the directions here are ours and the values agree with it only up to its sampling noise."""
+        fn = "Mesh.ambient_occlusion"
+        if isinstance(nr_samples, bool) or not isinstance(nr_samples, (int, np.integer)) or not 1 <= nr_samples <= _INT_MAX:
+            raise RuntimeError("%s: nr_samples must be a positive integer, got %r" % (fn, nr_samples))
+        if self.NV is None:
+            raise RuntimeError("%s: the mesh has no vertex normals (NV); call mesh.recalculate_normals() first" % fn)
+        S = int(nr_samples)
+        NV = self.NV
+        if not isinstance(NV, torch.Tensor) or NV.dtype != torch.float32 or not isinstance(self.V, torch.Tensor) or \
+                NV.shape != self.V.shape or NV.device != self.V.device:
+            raise RuntimeError("%s: NV must be a float32 tensor shaped and placed like V" % fn)
+        with torch.cuda.device(self.V.device):
+            V, Fc, ws = self._bvh(fn)
+            dirs = torch.from_numpy(fibonacci_directions(S)).to(V.device)
+            vis = torch.empty(V.shape[0], dtype=torch.float32, device=V.device)
+            call("psdf_mesh_ambient_occlusion", V.shape[0], Fc.shape[0], S, V, NV.contiguous(), dirs, ws, vis)
+        return vis
+
+    def interpolate(self, other, t):
+        """Mesh(torch.lerp(V, other.V, t), F.clone(), None): the in-between mesh of two frames of one topology (EasyPBR's interpolate as
+        train_4d_sdf.py uses it); the caller recalculates normals. Refused unless F equals other.F and V has other.V's shape."""
+        if not isinstance(other, Mesh):
+            raise RuntimeError("Mesh.interpolate: other must be a Mesh, got %s" % type(other).__name__)
+        if self.V.shape != other.V.shape:
+            raise RuntimeError("Mesh.interpolate: V has shape %s and other.V %s" % (list(self.V.shape), list(other.V.shape)))
+        if self.F.shape != other.F.shape or not torch.equal(self.F, other.F.to(self.F.device)):
+            raise RuntimeError("Mesh.interpolate: the meshes have different faces; only frames of one topology are interpolated")
+        return Mesh(torch.lerp(self.V, other.V, float(t)), self.F.clone(), None)
+
     # ------------------------------------------------------------------ reading, welding and placing a mesh
     @staticmethod
     def load(path, device="cuda", weld=None):
@@ -436,6 +503,104 @@ class Mesh:
             f.write(header.encode("ascii"))
             f.write(vbytes)
             f.write(frec.tobytes())
+
+
+def _check_rays(fn, origins, dirs, V):
+    if not isinstance(V, torch.Tensor) or not V.is_cuda:
+        raise RuntimeError("%s: V must be a CUDA tensor (there is no CPU path)" % fn)
+    out = []
+    for name, x in (("origins", origins), ("dirs", dirs)):
+        if not isinstance(x, torch.Tensor) or x.dtype != torch.float32 or x.dim() != 2 or x.shape[1] != 3:
+            raise RuntimeError("%s: %s must be a float32 tensor of shape [R,3]" % (fn, name))
+        if x.device != V.device:
+            raise RuntimeError("%s: %s must be on V's device %s, got %s" % (fn, name, V.device, x.device))
+        if not bool(torch.isfinite(x).all()):
+            raise RuntimeError("%s: %s has values that are not finite" % (fn, name))
+        out.append(x.contiguous())
+    if out[0].shape[0] != out[1].shape[0]:
+        raise RuntimeError("%s: %d origins and %d dirs" % (fn, out[0].shape[0], out[1].shape[0]))
+    return out
+
+
+def fibonacci_directions(S):
+    """the S directions of Mesh.ambient_occlusion, float32 [S,3] on the host: z = 1 - (2s + 1) / S, phi = s pi (3 - sqrt 5),
+    (sqrt(1 - z^2) cos phi, sqrt(1 - z^2) sin phi, z), computed in fp64 and rounded to fp32"""
+    s = np.arange(S, dtype=np.float64)
+    z = 1.0 - (2.0 * s + 1.0) / S
+    phi = s * (math.pi * (3.0 - math.sqrt(5.0)))
+    r = np.sqrt(np.maximum(0.0, 1.0 - z * z))
+    return np.stack([r * np.cos(phi), r * np.sin(phi), z], 1).astype(np.float32)
+
+
+# ---------------------------------------------------------------- mesh sequences (train_4d_sdf.py:47-141)
+_SEQ_MAX_INDEX = 12          # the reference reads files while i <= min(12, n): at most 13
+_SEQ_MULTIPLICITY = 20       # in-between meshes per pair of frames
+_SEQ_AO_SAMPLES = 100
+_SEQ_AO_MIN = 0.01
+
+
+def natural_key(name):
+    """sort key that orders the digit runs of a name by value: f_2.obj < f_10.obj (natsort's default for such names)"""
+    return [int(t) if i % 2 else t for i, t in enumerate(re.split(r"(\d+)", name))]
+
+
+def sequence_files(names):
+    """the frames load_mesh_sequence reads of a folder's file names: those ending in .obj or .ply, natural-sorted, at most the first 13.
+    The reference matches ".obj" or ".py"; ".py" is read as a typo for ".ply"."""
+    files = sorted((n for n in names if n.endswith(".obj") or n.endswith(".ply")), key=natural_key)
+    return files[:min(_SEQ_MAX_INDEX, len(files)) + 1]
+
+
+def load_mesh_sequence(folder, device="cuda"):
+    """train_4d_sdf.py's load_mesh_sequence -> (points_time float32 [P,4], normals float32 [P,3]) on `device`, step by step:
+    - the frames are sequence_files(os.listdir(folder)), loaded with Mesh.load; fewer than 2 are refused, and so is a frame whose faces
+      differ from frame 0's (named);
+    - frame 0: s = normalize_size(), c = normalize_position(); every other frame: scale_mesh(s), translate(-c). The reference's EasyPBR
+      calls are scale_mesh(1.0 / scale) and translate_model_matrix(pos): its normalize_size returns the inverse of the factor it applies
+      and normalize_position the translation, while ours return the factor and the centre, hence s and -c here;
+    - every frame: recalculate_normals(), upsample(2, True) (Loop, normals recalculated);
+    - frame 0's ambient_occlusion(100) < 0.01 marks the vertices removed from every frame: remove_marked_vertices(mask, False), then
+      remove_unreferenced_verts();
+    - each consecutive pair (a, b) gives 20 meshes a.interpolate(b, j / 20), j = 0 .. 19, each with recalculate_normals(); the last frame is
+      never an endpoint itself;
+    - the K = 20 (n - 1) meshes are concatenated in order, mesh k with the time column fp32(k / (K - 1)).
+    The viewer colouring of the reference is left out."""
+    fn = "load_mesh_sequence"
+    folder = str(folder)
+    files = sequence_files(os.listdir(folder))
+    if len(files) < 2:
+        raise RuntimeError("%s: %s: %d mesh files (.obj or .ply); a sequence needs at least 2" % (fn, folder, len(files)))
+    frames, mask, F0 = [], None, None
+    for i, name in enumerate(files):
+        path = os.path.join(folder, name)
+        m = Mesh.load(path, device=device)
+        if i == 0:
+            F0, nv0 = m.F, m.V.shape[0]
+            s = m.normalize_size()
+            c = m.normalize_position()
+        else:
+            if m.F.shape != F0.shape or not torch.equal(m.F, F0) or m.V.shape[0] != nv0:
+                raise RuntimeError("%s: %s: its faces (or vertex count) differ from those of %s; every frame must have one topology" % (
+                    fn, path, files[0]))
+            m.scale_mesh(s)
+            m.translate(-c)
+        m.recalculate_normals()
+        m.upsample(2, True)
+        if i == 0:
+            mask = m.ambient_occlusion(_SEQ_AO_SAMPLES) < _SEQ_AO_MIN
+        m.remove_marked_vertices(mask, False)
+        m.remove_unreferenced_verts()
+        frames.append(m)
+    meshes = []
+    for a, b in zip(frames[:-1], frames[1:]):
+        for j in range(_SEQ_MULTIPLICITY):
+            meshes.append(a.interpolate(b, j / _SEQ_MULTIPLICITY).recalculate_normals())
+    K = len(meshes)
+    pts, nrm = [], []
+    for k, m in enumerate(meshes):
+        pts.append(torch.cat([m.V, torch.full((m.V.shape[0], 1), k / (K - 1), dtype=torch.float32, device=m.V.device)], 1))
+        nrm.append(m.NV)
+    return torch.cat(pts), torch.cat(nrm)
 
 
 # ---------------------------------------------------------------- reading meshes (host side)
@@ -715,4 +880,5 @@ def extract_mesh_from_density_model(model, nr_points_per_dim, min_val, max_val, 
         model.last_iter_nr = last_iter_nr
 
 
-__all__ = ["Mesh", "marching_cubes", "extract_mesh_from_sdf_model", "extract_mesh_from_density_model"]
+__all__ = ["Mesh", "marching_cubes", "extract_mesh_from_sdf_model", "extract_mesh_from_density_model", "load_mesh_sequence",
+           "fibonacci_directions"]

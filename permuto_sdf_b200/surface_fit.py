@@ -395,6 +395,13 @@ class SpaceTimeFit(SurfaceFit):
         # the model's own get_sdf_and_gradient stays on the per-op kernels (MODEL_ON_FUSED_PAIR); only the direct sequence is fused
         self.execution["sdf_training"] = "fused wgmma (direct sequence)" if self.direct else "per-op kernels + autograd"
 
+    @classmethod
+    def from_mesh_sequence(cls, folder, device="cuda", **kwargs):
+        """cls(*load_mesh_sequence(folder, device), **kwargs): a fit to the mesh sequence in `folder`, assembled as train_4d_sdf.py's
+        load_mesh_sequence does (mesh.load_mesh_sequence)"""
+        from .mesh import load_mesh_sequence
+        return cls(*load_mesh_sequence(folder, device), **kwargs)
+
     def _draws(self, Ns, No):
         """-> (sequence row indices [Ns], box draw [No,3], time draw [No,1]) in the reference's order (train_4d_sdf.py:202-206)"""
         idx, u01 = super()._draws(Ns, No)
