@@ -126,6 +126,10 @@ int psdf_packed_per_sample_ray_idx(int nr_rays, int nr_samples, const int* ray_s
 
 /* ---------------------------------------------------------------- VolumeRendering (include/permuto_sdf/VolumeRendering.cuh:22-38) */
 #define PSDF_RSP int nr_rays, int max_nr_samples, const int* ray_start_end, int equal, int fixed_n
+/* A ray is skipped when it is empty or its end > max_nr_samples. Of a skipped ray's outputs only these rows are written:
+ * bg_transmittance = 1 (cumprod), out = 0 (integrate), sum_ray = 0 (sum), pred_rgb = 0, pred_depth = 0, bg_transmittance = 1 (NeRF
+ * render) and its importance samples (pos = dirs = 0, z = -1). The NeRF render and its backward stop a ray once T < 1e-4: the
+ * per-sample rows after that point are not written. */
 int psdf_vr_cumprod_alpha2transmittance(PSDF_RSP, const float* one_minus_alpha, float* transmittance, float* bg_transmittance, void* stream);
 int psdf_vr_integrate_with_weights(PSDF_RSP, const float* vals, const float* weights, float* out, void* stream);
 int psdf_vr_sdf2alpha(PSDF_RSP, const float* ray_fixed_dt, const float* samples_dt, const float* sdf, float inv_s, int dynamic_inv_s,
@@ -136,6 +140,8 @@ int psdf_vr_compute_cdf(PSDF_RSP, const float* weights, float* cdf, void* stream
 int psdf_vr_importance_sample(PSDF_RSP, const float* origins, const float* dirs, const float* ray_fixed_dt, const float* samples_z,
                               const float* cdf, int nr_imp, uint64_t rng_state, uint64_t rng_inc, int jitter, float* o_pos,
                               float* o_dirs, float* o_z, void* stream);
+/* (importance_sample / importance_round) a ray with a single sample has no cdf interval to draw from: its importance samples are
+ * those of a skipped ray. Every other output of a ray depends on that ray's rows only. */
 long long psdf_vr_combine_workspace_bytes(int nr_rays);
 /* one round of importance_sampling_sdf_model (permuto_sdf_py/utils/sdf_utils.py): sdf2alpha -> clip -> cumprod(1 - alpha + 1e-7) ->
  * weights -> per-ray normalisation (clamp 1e-6) -> cdf -> importance_sample, one launch, bit-identical to the separate calls.
@@ -144,6 +150,8 @@ int psdf_vr_importance_round(PSDF_RSP, const float* origins, const float* dirs, 
                              const float* samples_z, const float* sdf, float inv_s, int dynamic_inv_s, float inv_s_multiplier, int nr_imp,
                              uint64_t rng_state, uint64_t rng_inc, int jitter, float* cdf, float* o_pos, float* o_dirs, float* o_z,
                              void* stream);
+/* merge of each ray's uniform and importance samples by z (the uniform one first only if strictly smaller), into slots scanned in
+ * ray order; rays with at most one uniform sample get start_end (0, 0) and fixed_dt 0. Any merged length is supported. */
 int psdf_vr_combine_uniform_samples_with_imp(PSDF_RSP, const float* origins, const float* dirs, const float* t_exit,
                                              const float* u_fixed_dt, const float* u_z, const float* u_sdf, int u_has_sdf,
                                              int imp_n, const float* i_z, const float* i_sdf, int i_has_sdf, int c_max,

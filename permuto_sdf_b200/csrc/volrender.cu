@@ -174,7 +174,8 @@ __device__ __forceinline__ int cdf_search(const float* __restrict__ cdf, float v
     }
     return imax;
 }
-// VolumeRenderingGPU.cuh:793-946 ; lane i produces importance sample i (loops if nr_imp > 32)
+// VolumeRenderingGPU.cuh:793-946 ; lane i produces importance sample i (loops if nr_imp > 32). A ray with one sample has no
+// cdf interval to draw from (the search would pair its sample with the previous ray's): it gets the samples of a skipped ray.
 __global__ void __launch_bounds__(kThreads)
 k_importance_sample(int nr_rays, const float* __restrict__ origins, const float* __restrict__ dirs, int max_nr_samples,
                     const int* __restrict__ start_end, const float* __restrict__ ray_fixed_dt, bool equal, int fixed_n,
@@ -188,7 +189,7 @@ k_importance_sample(int nr_rays, const float* __restrict__ origins, const float*
     float fixed_dt = ray_fixed_dt[ray];
     for (int i = lane; i < nr_imp; i += 32) {
         int s = ist + i;
-        if (skip) {
+        if (skip || rr.n == 1) {
             o_pos[3 * s] = 0; o_pos[3 * s + 1] = 0; o_pos[3 * s + 2] = 0;
             o_dirs[3 * s] = 0; o_dirs[3 * s + 1] = 0; o_dirs[3 * s + 2] = 0;
             o_z[s] = -1.0f;
@@ -288,14 +289,14 @@ k_importance_round(int nr_rays, const float* __restrict__ origins, const float* 
         }
         __syncwarp();
     }
-    // importance samples from the cdf (same body as k_importance_sample)
+    // importance samples from the cdf (same body as k_importance_sample, one-sample rays included)
     const int ist = ray * nr_imp;
     const float ox = origins[3 * ray], oy = origins[3 * ray + 1], oz = origins[3 * ray + 2];
     const float dx = dirs[3 * ray], dy = dirs[3 * ray + 1], dz = dirs[3 * ray + 2];
     const float fixed_dt = ray_fixed_dt[ray];
     for (int i = lane; i < nr_imp; i += 32) {
         const int s = ist + i;
-        if (skip) {
+        if (skip || rr.n == 1) {
             o_pos[3 * s] = 0; o_pos[3 * s + 1] = 0; o_pos[3 * s + 2] = 0;
             o_dirs[3 * s] = 0; o_dirs[3 * s + 1] = 0; o_dirs[3 * s + 2] = 0;
             o_z[s] = -1.0f;
@@ -328,7 +329,8 @@ k_importance_round(int nr_rays, const float* __restrict__ origins, const float* 
 // VolumeRenderingGPU.cuh:950-1131. Two-pointer merge of the uniform and importance samples of one ray.
 // Lane 0 replays the reference's merge decisions into shared memory (source index per output slot), then
 // the whole warp materialises positions / dirs / z / sdf / dt with coalesced stores. Output slots come from
-// an exclusive scan (offsets) instead of an atomic counter.
+// an exclusive scan (offsets) instead of an atomic counter. A ray longer than the shared-memory stage is merged
+// by lane 0 alone, straight from and to global memory, with the same decisions and arithmetic.
 constexpr int kMergeCap = 1024;  // max merged samples per ray handled in shared memory
 __global__ void __launch_bounds__(128)
 k_combine(int nr_rays, const float* __restrict__ origins, const float* __restrict__ dirs, const float* __restrict__ t_exit_,
@@ -352,10 +354,33 @@ k_combine(int nr_rays, const float* __restrict__ origins, const float* __restric
     int cn = ur.n + imp_n;
     int cs = offsets[ray] + block_sums[ray / scan_block];
     if (lane == 0) reinterpret_cast<int2*>(c_start_end)[ray] = make_int2(cs, cs + cn);
-    if (cs + cn > c_max || cn > kMergeCap) return;
+    if (cs + cn > c_max) return;
     float fixed_dt = u_fixed_dt[ray];
     if (lane == 0) c_fixed_dt[ray] = fixed_dt;
     int ist = ray * imp_n;
+    if (cn > kMergeCap) {
+        if (lane != 0) return;
+        float ox = origins[3 * ray], oy = origins[3 * ray + 1], oz = origins[3 * ray + 2];
+        float dx = dirs[3 * ray], dy = dirs[3 * ray + 1], dz = dirs[3 * ray + 2];
+        int iu = 0, ii = 0;
+        float prev = 0.0f;
+        for (int i = 0; i < cn; i++) {
+            float zu = (iu < ur.n) ? u_z[ur.start + iu] : 1e10f;
+            float zi = (ii < imp_n) ? i_z[ist + ii] : 1e10f;
+            bool take_u = zu < zi;
+            float zz = take_u ? zu : zi;
+            int s = cs + i;
+            c_pos[3 * s] = __fmaf_rn(zz, dx, ox); c_pos[3 * s + 1] = __fmaf_rn(zz, dy, oy); c_pos[3 * s + 2] = __fmaf_rn(zz, dz, oz);
+            c_dirs[3 * s] = dx; c_dirs[3 * s + 1] = dy; c_dirs[3 * s + 2] = dz;
+            c_z[s] = zz;
+            if (take_u) { if (u_has_sdf) c_sdf[s] = u_sdf[ur.start + iu]; iu++; }
+            else { if (i_has_sdf) c_sdf[s] = i_sdf[ist + ii]; ii++; }
+            if (i > 0) c_dt[s - 1] = fminf(__fsub_rn(zz, prev), fixed_dt);
+            prev = zz;
+        }
+        c_dt[cs + cn - 1] = clampf(__fsub_rn(t_exit_[ray], prev), 0.0f, fixed_dt);
+        return;
+    }
     // stage both z lists: uniform at [0,n), importance at [n, n+imp)
     for (int i = lane; i < ur.n; i += 32) zs[wib][i] = u_z[ur.start + i];
     for (int i = lane; i < imp_n; i += 32) zs[wib][ur.n + i] = i_z[ist + i];
