@@ -724,6 +724,74 @@ int psdf_mesh_occluded(int V, int F, long long R, const float* origins, const fl
 int psdf_mesh_ambient_occlusion(int V, int F, int S, const float* verts, const float* normals, const float* dirs, uint8_t* workspace,
                                 float* vis_out, void* stream);
 
+/* ---------------------------------------------------------------- mesh distances (csrc/mesh_distance.cu)
+ * Closest points on the faces of verts [V,3] (float) and faces [F,3] (int32) through the BVH of psdf_mesh_bvh_build, pseudonormals,
+ * signed distances and surface samples. Built with -fmad=false; oracle/mesh_distance.py restates the closest-point formula and checks
+ * dist2, face and bary bit for bit by brute force. fp32 as in the ray casting section: dot(a, b) = (ax bx + ay by) + az bz, cross as there,
+ * x + t e per coordinate, dist2(p, q) = dot(p - q, p - q).
+ * Closest point of p on face (a, b, c) (Ericson, Real-Time Collision Detection 5.1.5, each division guarded), -> (dist2, bary):
+ *   ab = b - a, ac = c - a, n = cross(ab, ac); n == (0, 0, 0) (zero fp32 area, e.g. collinear corners): the nearest edge, below. Else
+ *   ap = p - a, d1 = dot(ab, ap), d2 = dot(ac, ap); d1 <= 0 and d2 <= 0: a, (1, 0, 0).
+ *   bp = p - b, d3 = dot(ab, bp), d4 = dot(ac, bp); d3 >= 0 and d4 <= d3: b, (0, 1, 0).
+ *   vc = dot(n, cross(ap, bp)); vc <= 0, d1 >= 0, d3 <= 0 and d1 - d3 > 0: v = d1 / (d1 - d3), a + v ab, (1 - v, v, 0).
+ *   cp = p - c, d5 = dot(ab, cp), d6 = dot(ac, cp); d6 >= 0 and d5 <= d6: c, (0, 0, 1).
+ *   vb = dot(n, cross(cp, ap)); vb <= 0, d2 >= 0, d6 <= 0 and d2 - d6 > 0: w = d2 / (d2 - d6), a + w ac, (1 - w, 0, w).
+ *   va = dot(n, cross(bp, cp)), e43 = d4 - d3, e56 = d5 - d6; va <= 0, e43 >= 0, e56 >= 0 and e43 + e56 > 0: w = e43 / (e43 + e56),
+ *     b + w (c - b), (0, 1 - w, w).
+ *   den = (va + vb) + vc; den > 0, v = vb / den, w = vc / den, v >= 0, w >= 0, v + w <= 1: (a + v ab) + w ac, ((1 - v) - w, v, w),
+ *     unless the nearest edge (below) has a strictly smaller dist2, which then replaces it: on a sliver the weights carry a relative
+ *     error of about eps |ab| / h (h its width) and can put q farther from p than the sliver's edges are.
+ *   Otherwise (a sliver whose interior weights round out of range): the nearest edge. The signed areas va, vb, vc are the book's triple
+ *   products, not its Lagrange-identity form (vc = d1 d4 - d3 d2, ...): that form cancels on slivers, whose |n|^2 falls below the rounding
+ *   of |ab|^2 |ap|^2, and puts points inside them on an edge or a corner up to the sliver's width away.
+ *   Nearest edge: for (x, y) = (a, b), (b, c), (c, a) in that order, e = y - x, ee = dot(e, e), t = dot(p - x, e) / ee (0 when ee is 0),
+ *   clamped by min(max(t, 0), 1), q = x + t e; the first with the smallest dist2 (strictly smaller replaces); bary (1 - t, t, 0),
+ *   (0, 1 - t, t), (t, 0, 1 - t). No denominator is ever zero.
+ * Answer: among the faces with three distinct indices, the smallest dist2, ties to the smallest face index; faces that repeat a vertex are
+ *   skipped (occluded never hits them). No such face: dist2 = +inf, face = -1, bary = 0.
+ * The tree only prunes: a node is skipped when its bound is strictly above the best dist2 so far, so ties are visited. The bound is the
+ *   fp32 dist2 from p to the box grown by pad = 2^-12 s (s as for the rays): per axis max((lo - pad) - p, p - (hi + pad), 0), then
+ *   (ex ex + ey ey) + ez ez. Every closest point above is x + t e with 0 <= t <= 1 or (a + v ab) + w ac with v, w >= 0 and v + w <= 1,
+ *   so it lies within a few ulps of s (far below pad) of its face's exact box; then |p_k - q_k| rounded is at least the box gap per axis,
+ *   and rounding is monotone, so the bound never exceeds the face's computed dist2. Nearer child first (child 0 on a tie), 64-entry stack
+ *   as for the rays, one query per thread, 64-bit query ids.
+ * psdf_mesh_closest_points: dist2_out [P] (float), face_out [P] (int32, the original face index), bary_out [P,3] (float) of points [P,3];
+ *   workspace is a psdf_mesh_bvh_build workspace of the same V and F (read only; verts is not read). P is 64-bit (PSDF_ERR_UNSUPPORTED
+ *   above 256 (2^31 - 1)); P = 0 launches nothing.
+ * Pseudonormals (Baerentzen and Aanaes 2005), in fp32, every sum in ascending face order over the vertex -> face CSR of mesh_csr.cuh (each
+ *   list heap-sorted after the fill), so the bits are the same on every run:
+ *   face_n [F,3]: n / sqrtf(dot(n, n)) of n = cross(b - a, c - a); 0 when that length is 0 and for faces that repeat a vertex.
+ *   vert_n [V,3]: sum over v's faces of angle * face_n, angle = atan2f(|e1 x e2|, dot(e1, e2)) of the two edges e1, e2 leaving v in the face
+ *     (its next, then its previous corner); not normalised.
+ *   edge_n [F,3,3]: row 3 f + k, the edge from corner k to corner (k + 1) % 3 of f: the sum of face_n over every face holding both ends
+ *     (f itself included), read from the list of the end with fewer faces; not normalised. A non-manifold edge sums more faces.
+ *   Topology is not validated: the sign below is right for closed, consistently oriented, edge-manifold meshes only. Faces with an index
+ *   outside [0, V) or a repeated vertex are counted into info[0], info[1] and left out (the caller refuses the former).
+ *   Workspace: psdf_mesh_pseudonormals_workspace_bytes(V, F) ~ 12 B per vertex + 12 B per face (sections each padded to 256 B): int64
+ *   info[4] at byte 0, int64 CSR offsets [V + 1], int32 counts [V], int32 CSR faces [3F], int64 scan tile sums. PSDF_ERR_UNSUPPORTED when
+ *   V or F is 2^31 or more, PSDF_ERR_ARG when negative.
+ * psdf_mesh_signed_distance: psdf_mesh_closest_points into dist2_out, face_out, bary_out, then sdf_out [P] (float) =
+ *   sign(dot(p - q, n)) sqrtf(dist2) with q = (b0 a + b1 b) + b2 c per coordinate and n the pseudonormal of the closest feature, read off
+ *   the weights: two exact zeros, the vertex of the third; one, the edge of the other two; none, the face. The vertex and edge cases of
+ *   the formula write exact zeros, so this is the region it took, or a vertex where an edge weight came out 0 or 1. A zero dot gives +0;
+ *   no face gives +inf.
+ * psdf_mesh_sample_surface: N area-weighted samples, 64-bit sample ids. cdf [F] (double) is a non-decreasing inclusive sum of face
+ *   weights (the areas; Mesh sums them as int64 fixed point, exactly), its last entry positive; a face of weight 0 is never drawn. x_n = output n of SplitMix64 seeded with seed (z = seed + (n + 1) 0x9E3779B97F4A7C15, then
+ *   the SplitMix64 finaliser). Sample k: u0 = double(x_3k >> 11) 2^-53 * total, the face is the first with cdf > u0 (with cdf >= total
+ *   when u0 rounds to the total); r1 = float(x_3k+1 >> 40) 2^-24, r2 = float(x_3k+2 >> 40) 2^-24, s = sqrtf(r1), weights (1 - s,
+ *   s (1 - r2), s r2), point = (b0 a + b1 b) + b2 c per coordinate (fp32). Sample k depends only on (seed, k): the same bits for any N and
+ *   launch shape. F = 0 with N > 0: PSDF_ERR_ARG. */
+int psdf_mesh_closest_points(int V, int F, long long P, const float* points, const float* verts, const int* faces, const uint8_t* workspace,
+                             float* dist2_out, int* face_out, float* bary_out, void* stream);
+long long psdf_mesh_pseudonormals_workspace_bytes(long long nr_vertices, long long nr_faces);
+int psdf_mesh_pseudonormals(int V, int F, const float* verts, const int* faces, uint8_t* workspace, float* face_n, float* vert_n,
+                            float* edge_n, void* stream);
+int psdf_mesh_signed_distance(int V, int F, long long P, const float* points, const float* verts, const int* faces, const uint8_t* workspace,
+                              const float* face_n, const float* vert_n, const float* edge_n, float* dist2_out, int* face_out,
+                              float* bary_out, float* sdf_out, void* stream);
+int psdf_mesh_sample_surface(int V, int F, const float* verts, const int* faces, const double* cdf, long long N, uint64_t seed,
+                             float* points_out, int* face_out, void* stream);
+
 /* ---------------------------------------------------------------- image metrics (csrc/image_metrics.cu)
  * Per-image PSNR and SSIM of the reference's experiments/evaluation/evaluate_psnr.py, which scores each frame with piq.psnr and piq.ssim
  * (data_range = 1; kernel 11, sigma 1.5, k1 0.01, k2 0.03, downsampling on). x (the prediction) and y (the ground truth) are float images of

@@ -12,6 +12,7 @@ sphere-tracing hot path behind the reference's own Python operator API.
     permuto_sdf_b200.extract_mesh_from_sdf_model / marching_cubes / Mesh   meshes from a trained SDF or a volume on the GPU
     permuto_sdf_b200.extract_mesh_from_density_model   meshes from a trained NeRF's density (NerfTrainer.model) on the GPU
     permuto_sdf_b200.load_mesh_sequence       the [P,4] point sequence of train_4d_sdf.py from a folder of meshes (ray-cast AO on the GPU)
+    permuto_sdf_b200.mesh_distance            accuracy, completeness, chamfer and Hausdorff distance of two meshes (BVH queries on the GPU)
     permuto_sdf_b200.psnr / ssim              image metrics of evaluate_psnr.py on the GPU (metrics.py; Trainer.evaluate scores frames)
 
 All device work goes through the C ABI in include/psdf_b200.h (libpsdf_b200.so, hand-written CUDA).
@@ -35,7 +36,8 @@ def __getattr__(name):
     if name == "NerfTrainer":
         from .nerf_train import NerfTrainer
         return NerfTrainer
-    if name in ("Mesh", "marching_cubes", "extract_mesh_from_sdf_model", "extract_mesh_from_density_model", "load_mesh_sequence"):
+    if name in ("Mesh", "marching_cubes", "extract_mesh_from_sdf_model", "extract_mesh_from_density_model", "load_mesh_sequence",
+                "mesh_distance"):
         from . import mesh
         return getattr(mesh, name)
     if name in ("psnr", "ssim"):

@@ -12,7 +12,9 @@ Mesh.decimate reduces a mesh to a target face count by quadric edge collapse, in
 Mesh.load reads PLY, OBJ and STL files on the host, the torch ops below weld, compact and place a mesh as train_sdf_from_mesh.py does,
 and Mesh.upsample runs midpoint or Loop subdivision on the GPU (csrc/mesh_subdivide.cu), the same bits on every run.
 Mesh.occluded and Mesh.ambient_occlusion cast rays against the faces through a linear BVH on the GPU (csrc/mesh_raycast.cu), and
-load_mesh_sequence assembles the point sequence of train_4d_sdf.py from a folder of meshes.
+load_mesh_sequence assembles the point sequence of train_4d_sdf.py from a folder of meshes. Mesh.closest_points and
+Mesh.signed_distance query the nearest point of the faces through the same BVH (csrc/mesh_distance.cu), and mesh_distance measures how
+far apart two meshes are from surface samples of each.
 """
 import math
 import os
@@ -364,6 +366,103 @@ class Mesh:
             call("psdf_mesh_ambient_occlusion", V.shape[0], Fc.shape[0], S, V, NV.contiguous(), dirs, ws, vis)
         return vis
 
+    # ------------------------------------------------------------------ distances
+    def _closest(self, fn, p):
+        """psdf_mesh_closest_points of the checked points p -> (V, F, BVH workspace, dist2 [P], face [P], bary [P,3])"""
+        V, Fc, ws = self._bvh(fn)
+        P = p.shape[0]
+        dist2 = torch.empty(P, dtype=torch.float32, device=V.device)
+        face = torch.empty(P, dtype=torch.int32, device=V.device)
+        bary = torch.empty(P, 3, dtype=torch.float32, device=V.device)
+        call("psdf_mesh_closest_points", V.shape[0], Fc.shape[0], P, p, V, Fc, ws, dist2, face, bary)
+        return V, Fc, ws, dist2, face, bary
+
+    def closest_points(self, points):
+        """the nearest point of the faces to each of points [P,3] (float32 CUDA on V's device, finite), on the GPU ->
+        (dist float32 [P], face int32 [P], closest float32 [P,3]): dist = sqrt of the fp32 squared distance, face the original face index,
+        closest = (b0 a + b1 b) + b2 c of its barycentrics. The answer is that of testing every face with the fp32 closest-point formula
+        of include/psdf_b200.h: the smallest squared distance, ties to the smallest face index; a BVH built on each call only prunes.
+        Faces that repeat a vertex are skipped; zero-area faces count as their edges. Without such faces: (+inf, -1, NaN). V and F are
+        checked as occluded checks them."""
+        fn = "Mesh.closest_points"
+        p = _check_points(fn, points, self.V)
+        with torch.cuda.device(p.device):
+            V, Fc, _, dist2, face, bary = self._closest(fn, p)
+            corners = V[Fc[face.clamp(min=0).long()].long()] if Fc.shape[0] else torch.full((face.shape[0], 3, 3), math.nan,
+                                                                                               device=V.device)
+            closest = (bary[:, 0:1] * corners[:, 0] + bary[:, 1:2] * corners[:, 1]) + bary[:, 2:3] * corners[:, 2]
+            closest[face < 0] = math.nan
+            return torch.sqrt(dist2), face, closest
+
+    def _pseudonormals(self, fn):
+        """angle-weighted pseudonormals (Baerentzen and Aanaes 2005) on the GPU -> (face_n float32 [F,3] unit, vert_n float32 [V,3],
+        edge_n float32 [F,3,3]): vertex and edge sums in ascending face order, the same bits on every run (include/psdf_b200.h). Not
+        normalised except face_n; only their directions are used."""
+        V, Fc = self._check_vf(fn)
+        nv, nf = V.shape[0], Fc.shape[0]
+        with torch.cuda.device(V.device):
+            face_n = torch.empty(nf, 3, dtype=torch.float32, device=V.device)
+            vert_n = torch.empty(nv, 3, dtype=torch.float32, device=V.device)
+            edge_n = torch.empty(nf, 3, 3, dtype=torch.float32, device=V.device)
+            ws = torch.empty(int(load_library().psdf_mesh_pseudonormals_workspace_bytes(nv, nf)), dtype=torch.uint8, device=V.device)
+            call("psdf_mesh_pseudonormals", nv, nf, V, Fc, ws, face_n, vert_n, edge_n)
+            bad = int(ws[:8].view(torch.int64).item())
+        if bad:
+            raise RuntimeError("%s: %d faces have a vertex index outside [0, %d)" % (fn, bad, nv))
+        return face_n, vert_n, edge_n
+
+    def signed_distance(self, points):
+        """signed distance from the faces to each of points [P,3] (float32 CUDA on V's device, finite), on the GPU -> float32 [P],
+        negative inside: sqrt of closest_points' squared distance, with the sign of dot(p - q, n), n the angle-weighted pseudonormal of the
+        vertex, edge or face holding the closest point q (include/psdf_b200.h); a zero dot gives +0, a mesh without faces +inf. The sign
+        is right only for a closed, consistently oriented (outward), edge-manifold mesh, such as marching_cubes gives; topology is not
+        checked. For other meshes the magnitude is still the unsigned distance."""
+        fn = "Mesh.signed_distance"
+        p = _check_points(fn, points, self.V)
+        with torch.cuda.device(p.device):
+            face_n, vert_n, edge_n = self._pseudonormals(fn)
+            V, Fc, ws = self._bvh(fn)
+            P = p.shape[0]
+            dist2 = torch.empty(P, dtype=torch.float32, device=p.device)
+            face = torch.empty(P, dtype=torch.int32, device=p.device)
+            bary = torch.empty(P, 3, dtype=torch.float32, device=p.device)
+            sdf = torch.empty(P, dtype=torch.float32, device=p.device)
+            call("psdf_mesh_signed_distance", V.shape[0], Fc.shape[0], P, p, V, Fc, ws, face_n, vert_n, edge_n, dist2, face, bary, sdf)
+        return sdf
+
+    def _area_cdf(self, fn):
+        """the cdf psdf_mesh_sample_surface draws faces from -> (V, F, cdf fp64 [F]): the face areas |(b - a) x (c - a)| / 2 in fp64 (0 for
+        faces that repeat a vertex), as int64 fixed point floor(area * 2^62 / (F * max area)), summed by an int64 cumsum on the device
+        (integer sums are exact, so the bits are the same on every call; torch's CUDA cumsum of floats is not deterministic) and
+        converted to fp64. A face below 2^-62 F of the largest area gets no samples. Faces with an index outside [0, V) and a mesh of
+        zero area are refused."""
+        V, Fc = self._check_vf(fn)
+        nv, nf = V.shape[0], Fc.shape[0]
+        with torch.cuda.device(V.device):
+            out = ((Fc < 0) | (Fc >= nv)).any(1)
+            if bool(out.any()):
+                raise RuntimeError("%s: %d faces have a vertex index outside [0, %d)" % (fn, int(out.sum()), nv))
+            p = V.double()[Fc.long()]
+            area = torch.linalg.vector_norm(torch.cross(p[:, 1] - p[:, 0], p[:, 2] - p[:, 0], dim=1), dim=1) * 0.5
+            area[(Fc[:, 0] == Fc[:, 1]) | (Fc[:, 1] == Fc[:, 2]) | (Fc[:, 2] == Fc[:, 0])] = 0
+            amax = float(area.max()) if nf else 0.0
+            if not amax > 0:
+                raise RuntimeError("%s: the mesh has no face of positive area" % fn)
+            q = torch.floor(area * (2.0 ** 62 / (amax * nf))).to(torch.int64)
+            return V, Fc, torch.cumsum(q, 0).double()
+
+    def _sample_surface(self, fn, nr_samples, seed):
+        """nr_samples points drawn by area on the GPU -> (points float32 [N,3], face int32 [N]): sample k depends only on (seed, k)
+        (psdf_mesh_sample_surface: SplitMix64, the face by the area cdf of _area_cdf, the sqrt(u) barycentric map), so a larger N extends
+        a smaller one, and the result is the same bits on every call."""
+        V, Fc, cdf = self._area_cdf(fn)
+        with torch.cuda.device(V.device):
+            N = int(nr_samples)
+            pts = torch.empty(N, 3, dtype=torch.float32, device=V.device)
+            face = torch.empty(N, dtype=torch.int32, device=V.device)
+            call("psdf_mesh_sample_surface", V.shape[0], Fc.shape[0], V, Fc, cdf, N, int(seed), pts, face)
+        return pts, face
+
     def interpolate(self, other, t):
         """Mesh(torch.lerp(V, other.V, t), F.clone(), None): the in-between mesh of two frames of one topology (EasyPBR's interpolate as
         train_4d_sdf.py uses it); the caller recalculates normals. Refused unless F equals other.F and V has other.V's shape."""
@@ -520,6 +619,55 @@ def _check_rays(fn, origins, dirs, V):
     if out[0].shape[0] != out[1].shape[0]:
         raise RuntimeError("%s: %d origins and %d dirs" % (fn, out[0].shape[0], out[1].shape[0]))
     return out
+
+
+def _check_points(fn, points, V):
+    if not isinstance(V, torch.Tensor) or not V.is_cuda:
+        raise RuntimeError("%s: V must be a CUDA tensor (there is no CPU path)" % fn)
+    if not isinstance(points, torch.Tensor) or points.dtype != torch.float32 or points.dim() != 2 or points.shape[1] != 3:
+        raise RuntimeError("%s: points must be a float32 tensor of shape [P,3]" % fn)
+    if points.device != V.device:
+        raise RuntimeError("%s: points must be on V's device %s, got %s" % (fn, V.device, points.device))
+    if not bool(torch.isfinite(points).all()):
+        raise RuntimeError("%s: points has values that are not finite" % fn)
+    return points.contiguous()
+
+
+def mesh_distance(a, b, nr_samples=1_000_000, seed=0):
+    """how far apart two meshes are, on the GPU: nr_samples area-weighted samples of each surface (the same seed for both, so swapping a
+    and b swaps the two directions exactly), each queried against the other mesh with Mesh.closest_points. -> dict:
+      accuracy      mean distance from the samples of a to b
+      completeness  mean distance from the samples of b to a
+      chamfer       (accuracy + completeness) / 2
+      hausdorff     the larger of the two maximum distances
+      dist_a_to_b, dist_b_to_a   the per-sample distances, float32 [nr_samples] on the device
+    The means are fp64 sums of the fp32 distances, the same bits on every call. Sample k of a mesh depends only on (seed, k): SplitMix64
+    picks a face by its share of the area (fixed point, summed exactly) and a point by the sqrt(u) barycentric map (psdf_mesh_sample_surface). Both meshes are
+    checked as Mesh.occluded checks them (V float32 CUDA and finite, F int32 on its device with indices in [0, V)) and need a face of
+    positive area; each mesh's BVH is built once, for the queries against it. Thresholded precision, recall or F-score follow from the
+    returned distances."""
+    fn = "mesh_distance"
+    for name, m in (("a", a), ("b", b)):
+        if not isinstance(m, Mesh):
+            raise RuntimeError("%s: %s must be a Mesh, got %s" % (fn, name, type(m).__name__))
+    if isinstance(nr_samples, bool) or not isinstance(nr_samples, (int, np.integer)) or not 1 <= nr_samples <= 256 * _INT_MAX:
+        raise RuntimeError("%s: nr_samples must be a positive integer, got %r" % (fn, nr_samples))
+    if isinstance(seed, bool) or not isinstance(seed, (int, np.integer)) or not 0 <= seed < 2 ** 64:
+        raise RuntimeError("%s: seed must be an integer in [0, 2^64), got %r" % (fn, seed))
+    a._check_vf(fn)
+    b._check_vf(fn)
+    if b.V.device != a.V.device:
+        raise RuntimeError("%s: the meshes are on %s and %s; both must be on one device" % (fn, a.V.device, b.V.device))
+    with torch.cuda.device(a.V.device):
+        sa, _ = a._sample_surface(fn, int(nr_samples), int(seed))
+        sb, _ = b._sample_surface(fn, int(nr_samples), int(seed))
+        d_ab = b.closest_points(sa)[0]
+        d_ba = a.closest_points(sb)[0]
+        acc, comp = d_ab.double().mean(), d_ba.double().mean()
+        hd = torch.maximum(d_ab.max(), d_ba.max())
+        acc, comp, hd = torch.stack([acc, comp, hd.double()]).tolist()
+    return {"accuracy": acc, "completeness": comp, "chamfer": (acc + comp) / 2, "hausdorff": hd, "dist_a_to_b": d_ab,
+            "dist_b_to_a": d_ba}
 
 
 def fibonacci_directions(S):
@@ -881,4 +1029,4 @@ def extract_mesh_from_density_model(model, nr_points_per_dim, min_val, max_val, 
 
 
 __all__ = ["Mesh", "marching_cubes", "extract_mesh_from_sdf_model", "extract_mesh_from_density_model", "load_mesh_sequence",
-           "fibonacci_directions"]
+           "fibonacci_directions", "mesh_distance"]
