@@ -679,8 +679,9 @@ int psdf_mesh_subdivide_emit(int V, int F, int smooth, const float* verts, const
                              int* faces_out, void* stream);
 
 /* ---------------------------------------------------------------- mesh ray casting (csrc/mesh_raycast.cu)
- * Any-hit queries of rays against the triangles of verts [V,3] (float) and faces [F,3] (int32) through a linear BVH, and per-vertex
- * ambient occlusion. Built with -fmad=false; oracle/raycast.py restates the triangle test and checks every answer by brute force.
+ * Any-hit and first-hit queries of rays against the triangles of verts [V,3] (float) and faces [F,3] (int32) through a linear BVH, per-vertex
+ * ambient occlusion and rendering from reel cameras. Built with -fmad=false; oracle/raycast.py restates the triangle test and checks every
+ * any-hit answer by brute force, tests/first_hit_oracle.py every first hit and rendered pixel.
  * Ray-triangle test (two-sided Moller-Trumbore, fp32, each operation rounded as written; dot(a, b) = (ax bx + ay by) + az bz, cross(a, b) =
  *   (ay bz - az by, az bx - ax bz, ax by - ay bx)): e1 = p1 - p0, e2 = p2 - p0, pv = cross(d, e2), det = dot(e1, pv); det == 0 or NaN
  *   misses. inv = 1.0f / det, tv = o - p0, u = dot(tv, pv) * inv, miss unless 0 <= u <= 1; qv = cross(tv, e1), v = dot(d, qv) * inv, miss
@@ -716,11 +717,35 @@ int psdf_mesh_subdivide_emit(int V, int F, int smooth, const float* verts, const
  * psdf_mesh_ambient_occlusion: V S rays, one per (vertex i, direction s), 64-bit ray ids: origin verts[i], direction dirs[s] [S,3], negated
  *   when dot(dirs[s], normals[i]) < 0 (fp32 as above), tnear = 1e-4f, tfar = +inf; vis_out[i] = float(S - hits) / float(S). Hits are
  *   integer counts, so the result is the same bits on every run.
+ * psdf_mesh_first_hit: of the faces that pass the test for ray r within (tnear, tfar), the one with the smallest fp32 t, ties to the
+ *   smallest original face index -> t_out [R] (float) = that t, face_out [R] (int32) = the face, bary_out [R,3] (float) = ((1 - u) - v, u,
+ *   v) with the test's u and v, rounded as written; no such face (F = 0 included): (+inf, -1, 0). The answer is that of testing every face;
+ *   the tree only prunes. Nearer child first by the slab entry max(tnear, slab starts) (child 0 on equal entries); a box is skipped when
+ *   the slab test above fails against (tnear, min(tfar, best t)); it is non-strict, so boxes holding a tie are still visited. Leaves use
+ *   the test with the caller's tfar. Far passes (see above) can make a first hit differ from the brute-force one in the same way: a ray
+ *   within about 1 degree of a far triangle's plane can pass the test by rounding outside that triangle's padded box. Same workspace
+ *   (read only), ray ids and limits as psdf_mesh_occluded; no atomics, so the bits are the same on every run and for any launch shape.
+ * psdf_mesh_render: I images of H x W pixels (H W < 2^31), one thread per (image, pixel), 64-bit ids. The ray of pixel (x, y) of image i
+ *   is that of psdf_random_rays_from_reel for pix = y W + x, img = i, bit for bit: centre (x + 0.5, y + 0.5), K [I,3,3] (row-major, reads
+ *   K[0], K[2], K[4], K[5]), tf_world_cam [I,4,4] (row-major), normalised with rsqrtf. Its first hit (psdf_mesh_first_hit under tnear,
+ *   tfar) on face (a, b, c) of faces with weights (b0, b1, b2) gives: n = (b0 N_a + b1 N_b) + b2 N_c per coordinate with normals [V,3],
+ *   or without (NULL) the geometric cross(p_b - p_a, p_c - p_a); l = sqrtf(dot(n, n)), n = n / l per component, n = 0 when l == 0 (not
+ *   flipped toward the camera); rgb = (b0 C_a + b1 C_b) + b2 C_c with colors [V,3], or without (NULL) 0.5f + 0.5f n; mask 1, depth t,
+ *   normal n (world), face the original index. A miss: rgb 0, mask 0, depth 0, normal 0, face -1 (the rgb of a reel is already multiplied
+ *   by its mask). Outputs NCHW: rgb_out [I,3,H,W], mask_out and depth_out [I,1,H,W] (float), normal_out [I,3,H,W] (float), face_out
+ *   [I,1,H,W] (int32); a NULL output is not written. Each warp takes an 8 x 4 pixel tile, so its rays stay coherent; every pixel is
+ *   computed on its own, so the mapping changes no bit, and the result is the same bits on every run. workspace is the psdf_mesh_bvh_build
+ *   workspace of verts and faces (read only). PSDF_ERR_UNSUPPORTED when H W >= 2^31 or the threads exceed 256 (2^31 - 1).
  * Cost: build O(F) (sort, tree and refit are one pass each); a query visits the nodes whose padded boxes the ray meets. */
 long long psdf_mesh_bvh_workspace_bytes(long long nr_vertices, long long nr_faces);
 int psdf_mesh_bvh_build(int V, int F, const float* verts, const int* faces, uint8_t* workspace, void* stream);
 int psdf_mesh_occluded(int V, int F, long long R, const float* origins, const float* dirs, float tnear, float tfar, const uint8_t* workspace,
                        uint8_t* hit_out, void* stream);
+int psdf_mesh_first_hit(int V, int F, long long R, const float* origins, const float* dirs, float tnear, float tfar, const uint8_t* workspace,
+                        float* t_out, int* face_out, float* bary_out, void* stream);
+int psdf_mesh_render(int V, int F, const float* verts, const int* faces, const float* normals, const float* colors, int I, int H, int W,
+                     const float* K, const float* tf_world_cam, float tnear, float tfar, const uint8_t* workspace, float* rgb_out,
+                     float* mask_out, float* depth_out, float* normal_out, int* face_out, void* stream);
 int psdf_mesh_ambient_occlusion(int V, int F, int S, const float* verts, const float* normals, const float* dirs, uint8_t* workspace,
                                 float* vis_out, void* stream);
 

@@ -13,6 +13,8 @@ sphere-tracing hot path behind the reference's own Python operator API.
     permuto_sdf_b200.extract_mesh_from_density_model   meshes from a trained NeRF's density (NerfTrainer.model) on the GPU
     permuto_sdf_b200.load_mesh_sequence       the [P,4] point sequence of train_4d_sdf.py from a folder of meshes (ray-cast AO on the GPU)
     permuto_sdf_b200.mesh_distance            accuracy, completeness, chamfer and Hausdorff distance of two meshes (BVH queries on the GPU)
+    permuto_sdf_b200.look_at / sphere_cameras / orbit_cameras / TensorReel   camera rigs and an in-memory reel; with Mesh.render
+                                              (first hits on the GPU BVH) any mesh becomes a training scene
     permuto_sdf_b200.psnr / ssim              image metrics of evaluate_psnr.py on the GPU (metrics.py; Trainer.evaluate scores frames)
 
 All device work goes through the C ABI in include/psdf_b200.h (libpsdf_b200.so, hand-written CUDA).
@@ -40,6 +42,9 @@ def __getattr__(name):
                 "mesh_distance"):
         from . import mesh
         return getattr(mesh, name)
+    if name in ("look_at", "sphere_cameras", "orbit_cameras", "TensorReel"):
+        from . import cameras
+        return getattr(cameras, name)
     if name in ("psnr", "ssim"):
         from . import metrics
         return getattr(metrics, name)

@@ -1,6 +1,8 @@
-// Any-hit ray casting against an indexed triangle mesh through a linear BVH, and per-vertex ambient occlusion, sm_90a. Built with
-// -fmad=false: the ray-triangle test is rounded operation by operation as include/psdf_b200.h states it, so oracle/raycast.py (brute force
-// over all triangles) reproduces every answer. The tree only decides which triangles are tested; the answer is "some triangle passes".
+// Any-hit and first-hit ray casting against an indexed triangle mesh through a linear BVH, per-vertex ambient occlusion and rendering from
+// reel cameras, sm_90a. Built with -fmad=false: the ray-triangle test is rounded operation by operation as include/psdf_b200.h states it,
+// so oracle/raycast.py and, for first hits, tests/first_hit_oracle.py (brute force over all triangles) reproduce every answer. The tree
+// only decides which triangles are tested; the answer is "some triangle passes", or for first hits the passing triangle of smallest t,
+// ties to the smallest original face index.
 //
 // Build (psdf_mesh_bvh_build): the centroids' bounds and the largest |coordinate| are reduced with ordered-key atomics (k_rc_bounds);
 // each face gets the 30-bit Morton code of its centroid within those bounds (k_rc_morton); four stable 8-bit LSD radix passes
@@ -15,9 +17,12 @@
 //   k_rc_internal   children and parents of internal node i (Karras 2012)                            thread per internal node
 //   k_rc_leaves     leaf triangles and the bottom-up box refit                                       thread per leaf
 //   k_rc_occluded   hit_out[r] = any hit of ray r                                                    thread per ray
+//   k_fh_rays       t, face, bary of the first hit of ray r, nearer child first                      thread per ray
+//   k_fh_render     first hit of the reel ray of each pixel, shaded into NCHW images                 thread per (image, pixel), warp per 8 x 4 tile
 //   k_rc_ao         hits[i] += any hit of (V[i], dirs[s] flipped to NV[i]'s side)                    thread per (vertex, direction)
 //   k_rc_vis        vis[i] = float(S - hits[i]) / float(S)                                           thread per vertex
 #include "mesh_bvh.cuh"
+#include "reel_ray.cuh"
 #include "../../include/psdf_b200.h"
 
 using namespace psdf;
@@ -26,20 +31,21 @@ namespace {
 constexpr int kWarps = kThreads / 32;
 constexpr float kSlabRel = 1.0f / 1048576.0f;   // relative slack of the slab test's far end: above 2 gamma_3 of fp32 (Ize 2013)
 
-// two-sided Moller-Trumbore as include/psdf_b200.h states it
-__device__ __forceinline__ bool hit_triangle(float3 p0, float3 p1, float3 p2, float3 o, float3 d, float tnear, float tfar) {
+// two-sided Moller-Trumbore as include/psdf_b200.h states it; on a pass, t, u and v as computed
+__device__ __forceinline__ bool hit_triangle(float3 p0, float3 p1, float3 p2, float3 o, float3 d, float tnear, float tfar, float& t, float& u,
+                                             float& v) {
     const float3 e1 = sub3(p1, p0), e2 = sub3(p2, p0);
     const float3 pv = cross3(d, e2);
     const float det = dot3(e1, pv);
     if (det == 0.0f || det != det) return false;
     const float inv = 1.0f / det;
     const float3 tv = sub3(o, p0);
-    const float u = dot3(tv, pv) * inv;
+    u = dot3(tv, pv) * inv;
     if (!(u >= 0.0f && u <= 1.0f)) return false;
     const float3 qv = cross3(tv, e1);
-    const float v = dot3(d, qv) * inv;
+    v = dot3(d, qv) * inv;
     if (!(v >= 0.0f && u + v <= 1.0f)) return false;
-    const float t = dot3(e2, qv) * inv;
+    t = dot3(e2, qv) * inv;
     return t > tnear && t < tfar;
 }
 
@@ -237,9 +243,10 @@ __global__ void __launch_bounds__(kThreads) k_rc_leaves(int V, int F, const floa
 // ---------------------------------------------------------------- traversal
 __device__ __forceinline__ float axis(float3 v, int k) { return k == 0 ? v.x : (k == 1 ? v.y : v.z); }
 
-// the ray's parameter interval in the padded box meets [tnear, tfar]; conservative (see the header)
-__device__ __forceinline__ bool box_hit(const float* b, float3 o, float3 d, float3 inv, float tnear, float tfar, float pad) {
-    float t0 = tnear, t1 = tfar;
+// the ray's parameter interval in the padded box meets [tnear, tfar]; conservative (see the header). t0: the entry, max(tnear, slab starts)
+__device__ __forceinline__ bool box_hit(const float* b, float3 o, float3 d, float3 inv, float tnear, float tfar, float pad, float& t0) {
+    t0 = tnear;
+    float t1 = tfar;
     for (int k = 0; k < 3; k++) {
         const float lo = b[k] - pad, hi = b[3 + k] + pad, ok = axis(o, k), dk = axis(d, k), ik = axis(inv, k);
         if (dk == 0.0f) {
@@ -256,13 +263,16 @@ __device__ __forceinline__ bool box_hit(const float* b, float3 o, float3 d, floa
 __device__ __forceinline__ bool leaf_hit(const Ws& W, long long i, float3 o, float3 d, float tnear, float tfar) {
     float3 p0, p1, p2;
     leaf_corners(W, i, p0, p1, p2);
-    return hit_triangle(p0, p1, p2, o, d, tnear, tfar);
+    float t, u, v;
+    return hit_triangle(p0, p1, p2, o, d, tnear, tfar, t, u, v);
 }
+
+__device__ __forceinline__ float box_pad(float3 o, float scale) { return kPad * (scale + fmaxf(fmaxf(fabsf(o.x), fabsf(o.y)), fabsf(o.z))); }
 
 __device__ bool any_hit(const Ws& W, int F, float3 o, float3 d, float tnear, float tfar, float scale) {
     if (F == 0) return false;
     if (F == 1) return leaf_hit(W, 0, o, d, tnear, tfar);
-    const float pad = kPad * (scale + fmaxf(fmaxf(fabsf(o.x), fabsf(o.y)), fabsf(o.z)));
+    const float pad = box_pad(o, scale);
     const float3 inv = make_float3(1.0f / d.x, 1.0f / d.y, 1.0f / d.z);
     const int nl = F - 1;                                     // children at or above nl are leaves
     int stack[kStack];
@@ -272,7 +282,8 @@ __device__ bool any_hit(const Ws& W, int F, float3 o, float3 d, float tnear, flo
         const float4 a = __ldg(&nd->a), b = __ldg(&nd->b), c = __ldg(&nd->c);
         const int4 ch = __ldg(&nd->d);
         const float b0[6] = {a.x, a.y, a.z, a.w, b.x, b.y}, b1[6] = {b.z, b.w, c.x, c.y, c.z, c.w};
-        bool h0 = box_hit(b0, o, d, inv, tnear, tfar, pad), h1 = box_hit(b1, o, d, inv, tnear, tfar, pad);
+        float e0, e1;
+        bool h0 = box_hit(b0, o, d, inv, tnear, tfar, pad, e0), h1 = box_hit(b1, o, d, inv, tnear, tfar, pad, e1);
         if (h0 && ch.x >= nl) {
             if (leaf_hit(W, ch.x - nl, o, d, tnear, tfar)) return true;
             h0 = false;
@@ -298,6 +309,173 @@ __global__ void __launch_bounds__(kThreads) k_rc_occluded(int F, long long R, co
     const long long r = thread_index();
     if (r >= R) return;
     hit[r] = any_hit(W, F, load3(origins, r), load3(dirs, r), tnear, tfar, mesh_scale(W)) ? 1 : 0;
+}
+
+// ---------------------------------------------------------------- first hits
+struct Hit {
+    float t;
+    int face;                                                 // original index; -1: no hit
+    float u, v;
+};
+
+// sorted leaf i under the caller's (tnear, tfar): taken when its t is smaller, or equal with a smaller original face
+__device__ __forceinline__ void visit_first(const Ws& W, long long i, float3 o, float3 d, float tnear, float tfar, Hit& best) {
+    float3 p0, p1, p2;
+    leaf_corners(W, i, p0, p1, p2);
+    float t, u, v;
+    if (!hit_triangle(p0, p1, p2, o, d, tnear, tfar, t, u, v) || t > best.t) return;
+    const int f = __ldg(W.vals0 + i);
+    if (t == best.t && f > best.face) return;
+    best = Hit{t, f, u, v};
+}
+
+// the smallest passing t, ties to the smallest face: that of testing every face. Nearer child first by the slab entry (child 0 on a tie);
+// a box is skipped when the slab test fails against (tnear, min(tfar, best t)), which is non-strict, so boxes holding a tie are visited.
+// A popped node is skipped when its stored entry fails that test's bound against the best t of now (x + |x| 2^-20 is monotone in x).
+__device__ Hit first_hit(const Ws& W, int F, float3 o, float3 d, float tnear, float tfar, float scale) {
+    Hit best{INFINITY, -1, 0.0f, 0.0f};
+    if (F == 0) return best;
+    if (F == 1) {
+        visit_first(W, 0, o, d, tnear, tfar, best);
+        return best;
+    }
+    const float pad = box_pad(o, scale);
+    const float3 inv = make_float3(1.0f / d.x, 1.0f / d.y, 1.0f / d.z);
+    const int nl = F - 1;
+    int stack[kStack];
+    float tstack[kStack];
+    int sp = 0, node = 0;
+    while (true) {
+        const Node* nd = W.nodes + node;
+        const float4 a = __ldg(&nd->a), b = __ldg(&nd->b), c = __ldg(&nd->c);
+        const int4 ch = __ldg(&nd->d);
+        const float b0[6] = {a.x, a.y, a.z, a.w, b.x, b.y}, b1[6] = {b.z, b.w, c.x, c.y, c.z, c.w};
+        const float cap = fminf(tfar, best.t);
+        float e0, e1;
+        const bool g0 = box_hit(b0, o, d, inv, tnear, cap, pad, e0), g1 = box_hit(b1, o, d, inv, tnear, cap, pad, e1);
+        const bool swap = g0 && g1 ? e1 < e0 : false;
+        const int n0 = swap ? ch.y : ch.x, n1 = swap ? ch.x : ch.y;
+        bool h0 = swap ? g1 : g0, h1 = swap ? g0 : g1;
+        const float f1 = swap ? e0 : e1;
+        if (h0 && n0 >= nl) {
+            visit_first(W, n0 - nl, o, d, tnear, tfar, best);
+            h0 = false;
+        }
+        if (h1 && n1 >= nl) {
+            visit_first(W, n1 - nl, o, d, tnear, tfar, best);
+            h1 = false;
+        }
+        if (h0 && h1) {
+            stack[sp] = n1;
+            tstack[sp++] = f1;
+            node = n0;
+        } else if (h0 || h1) {
+            node = h0 ? n0 : n1;
+        } else {
+            float bound;
+            do {
+                if (sp == 0) return best;
+                --sp;
+                const float cp = fminf(tfar, best.t);
+                bound = cp + fabsf(cp) * kSlabRel;
+            } while (tstack[sp] > bound);
+            node = stack[sp];
+        }
+    }
+}
+
+__global__ void __launch_bounds__(kThreads) k_fh_rays(int F, long long R, const float* __restrict__ origins, const float* __restrict__ dirs,
+                                                           float tnear, float tfar, Ws W, float* __restrict__ t_out, int* __restrict__ face_out,
+                                                           float* __restrict__ bary_out) {
+    const long long r = thread_index();
+    if (r >= R) return;
+    const Hit h = first_hit(W, F, load3(origins, r), load3(dirs, r), tnear, tfar, mesh_scale(W));
+    const bool hit = h.face >= 0;
+    t_out[r] = h.t;
+    face_out[r] = h.face;
+    bary_out[3 * r] = hit ? (1.0f - h.u) - h.v : 0.0f;
+    bary_out[3 * r + 1] = hit ? h.u : 0.0f;
+    bary_out[3 * r + 2] = hit ? h.v : 0.0f;
+}
+
+// ---------------------------------------------------------------- rendering
+#ifndef PSDF_RENDER_ROWS
+constexpr bool kRenderTiles = true;
+#else
+constexpr bool kRenderTiles = false;                          // row order: built only by tools/bench_mesh_render.py, to measure against
+#endif
+constexpr int kTileW = 8, kTileH = 4;                         // the pixels of one warp
+
+struct RenderOut {
+    float* rgb;                                               // [I,3,H,W]
+    float* mask;                                              // [I,1,H,W]
+    float* depth;                                             // [I,1,H,W]
+    float* normal;                                            // [I,3,H,W]
+    int* face;                                                // [I,1,H,W]
+};
+
+__device__ __forceinline__ float3 blend(const float* __restrict__ a, int3 t, float b0, float b1, float b2) {
+    const float3 x = load3(a, t.x), y = load3(a, t.y), z = load3(a, t.z);
+    return make_float3((b0 * x.x + b1 * y.x) + b2 * z.x, (b0 * x.y + b1 * y.y) + b2 * z.y, (b0 * x.z + b1 * y.z) + b2 * z.z);
+}
+
+// thread g -> (image, x, y): a warp takes one 8 x 4 tile (tiles row by row, image by image), or in row order 32 consecutive pixels
+// (at least 4 blocks per SM: without that minimum ptxas keeps it to 48 registers and spills; with it, 56 and no spills)
+template <bool kTiles>
+__global__ void __launch_bounds__(kThreads, 4) k_fh_render(int F, int I, int H, int Wd, const float* __restrict__ verts,
+                                                        const int* __restrict__ faces, const float* __restrict__ normals,
+                                                        const float* __restrict__ colors, const float* __restrict__ K,
+                                                        const float* __restrict__ tf, float tnear, float tfar, Ws W, RenderOut out) {
+    const long long g = thread_index();
+    long long im;
+    int x, y;
+    if (kTiles) {
+        const long long tx = (Wd + kTileW - 1) / kTileW, per = tx * ((H + kTileH - 1) / kTileH) * 32;
+        im = g / per;
+        const long long q = g - im * per, tile = q >> 5;
+        const int lane = (int)(q & 31);
+        x = (int)(tile % tx) * kTileW + (lane & (kTileW - 1));
+        y = (int)(tile / tx) * kTileH + (lane >> 3);
+        if (im >= I || x >= Wd || y >= H) return;
+    } else {
+        const long long plane = (long long)H * Wd;
+        im = g / plane;
+        if (im >= I) return;
+        const int p = (int)(g - im * plane);
+        x = p % Wd;
+        y = p / Wd;
+    }
+    float3 o, d;
+    reel_ray((float)x + 0.5f, (float)y + 0.5f, K + 9 * im, tf + 16 * im, o, d);
+    const Hit h = first_hit(W, F, o, d, tnear, tfar, mesh_scale(W));
+    float3 n = make_float3(0.0f, 0.0f, 0.0f), rgb = n;
+    float depth = 0.0f;
+    if (h.face >= 0) {
+        const int3 t = load_face(faces, h.face);
+        const float b0 = (1.0f - h.u) - h.v, b1 = h.u, b2 = h.v;
+        if (normals) {
+            n = blend(normals, t, b0, b1, b2);
+        } else {
+            const float3 a = load3(verts, t.x);
+            n = cross3(sub3(load3(verts, t.y), a), sub3(load3(verts, t.z), a));
+        }
+        const float l = sqrtf(dot3(n, n));
+        n = l == 0.0f ? make_float3(0.0f, 0.0f, 0.0f) : make_float3(n.x / l, n.y / l, n.z / l);
+        rgb = colors ? blend(colors, t, b0, b1, b2) : make_float3(0.5f + 0.5f * n.x, 0.5f + 0.5f * n.y, 0.5f + 0.5f * n.z);
+        depth = h.t;
+    }
+    const long long plane = (long long)H * Wd, p = (long long)y * Wd + x;
+    if (out.rgb) {
+        float* q = out.rgb + 3 * im * plane + p;
+        q[0] = rgb.x; q[plane] = rgb.y; q[2 * plane] = rgb.z;
+    }
+    if (out.normal) {
+        float* q = out.normal + 3 * im * plane + p;
+        q[0] = n.x; q[plane] = n.y; q[2 * plane] = n.z;
+    }
+    if (out.mask) out.mask[im * plane + p] = h.face >= 0 ? 1.0f : 0.0f;
+    if (out.depth) out.depth[im * plane + p] = depth;
+    if (out.face) out.face[im * plane + p] = h.face;
 }
 
 __global__ void __launch_bounds__(kThreads) k_rc_ao(int V, int F, int S, const float* __restrict__ verts, const float* __restrict__ normals,
@@ -362,6 +540,37 @@ int psdf_mesh_occluded(int V, int F, long long R, const float* origins, const fl
     Ws W;
     carve(const_cast<uint8_t*>(workspace), V, F, &W);
     k_rc_occluded<<<blocks(R), kThreads, 0, ST>>>(F, R, origins, dirs, tnear, tfar, W, hit_out);
+    PSDF_CHECK_LAUNCH();
+    return PSDF_OK;
+}
+
+int psdf_mesh_first_hit(int V, int F, long long R, const float* origins, const float* dirs, float tnear, float tfar, const uint8_t* workspace,
+                        float* t_out, int* face_out, float* bary_out, void* stream) {
+    if (V < 0 || F < 0 || R < 0 || !workspace || (R > 0 && (!origins || !dirs || !t_out || !face_out || !bary_out))) return PSDF_ERR_ARG;
+    if (R > (long long)kThreads * kIntMax) return PSDF_ERR_UNSUPPORTED;
+    if (R == 0) return PSDF_OK;
+    Ws W;
+    carve(const_cast<uint8_t*>(workspace), V, F, &W);
+    k_fh_rays<<<blocks(R), kThreads, 0, ST>>>(F, R, origins, dirs, tnear, tfar, W, t_out, face_out, bary_out);
+    PSDF_CHECK_LAUNCH();
+    return PSDF_OK;
+}
+
+int psdf_mesh_render(int V, int F, const float* verts, const int* faces, const float* normals, const float* colors, int I, int H, int W_,
+                     const float* K, const float* tf_world_cam, float tnear, float tfar, const uint8_t* workspace, float* rgb_out,
+                     float* mask_out, float* depth_out, float* normal_out, int* face_out, void* stream) {
+    if (V < 0 || F < 0 || I < 0 || H < 0 || W_ < 0 || !workspace) return PSDF_ERR_ARG;
+    if ((F > 0 && (!verts || !faces)) || (I > 0 && (!K || !tf_world_cam))) return PSDF_ERR_ARG;
+    const long long plane = (long long)H * W_;
+    if (plane > kIntMax) return PSDF_ERR_UNSUPPORTED;
+    const long long n = kRenderTiles ? (long long)I * psdf::div_up(W_, kTileW) * psdf::div_up(H, kTileH) * 32 : (long long)I * plane;
+    if (n > (long long)kThreads * kIntMax) return PSDF_ERR_UNSUPPORTED;
+    if (I == 0 || plane == 0) return PSDF_OK;
+    Ws W;
+    carve(const_cast<uint8_t*>(workspace), V, F, &W);
+    const RenderOut out{rgb_out, mask_out, depth_out, normal_out, face_out};
+    k_fh_render<kRenderTiles><<<blocks(n), kThreads, 0, ST>>>(F, I, H, W_, verts, faces, normals, colors, K, tf_world_cam, tnear, tfar, W,
+                                                               out);
     PSDF_CHECK_LAUNCH();
     return PSDF_OK;
 }

@@ -11,6 +11,7 @@
 // by a global atomic (SURVEY.md F8), with the reference's atomic order available as slot_mode=0.
 #include "common.cuh"
 #include "sh.cuh"
+#include "reel_ray.cuh"
 #include "../../include/psdf_b200.h"
 
 using namespace psdf;
@@ -709,19 +710,12 @@ k_random_rays_from_reel(int nr_rays, int H, int W, const float* __restrict__ rgb
     if (i >= nr_rays) return;
     int im = img[i], p = pix[i];
     float sx = (float)(p % W) + 0.5f, sy = (float)(p / W) + 0.5f;
-    const float* Ki = K + 9 * im;
-    const float* T = tf + 16 * im;
-    float cxp = (sx - Ki[2]) / Ki[0], cyp = (sy - Ki[5]) / Ki[4];
-    float tx = T[3], ty = T[7], tz = T[11];
-    float wx = T[0] * cxp + T[1] * cyp + T[2] + tx;
-    float wy = T[4] * cxp + T[5] * cyp + T[6] + ty;
-    float wz = T[8] * cxp + T[9] * cyp + T[10] + tz;
-    float vx = wx - tx, vy = wy - ty, vz = wz - tz;
-    float inv = rsqrtf(vx * vx + vy * vy + vz * vz);
+    float3 o, d;
+    reel_ray(sx, sy, K + 9 * im, tf + 16 * im, o, d);
     int x = (int)floorf(sx), y = (int)floorf(sy);
     float m = has_mask ? mask_reel[((size_t)im * H + y) * W + x] : 1.0f;
-    o_out[3 * i] = tx; o_out[3 * i + 1] = ty; o_out[3 * i + 2] = tz;
-    d_out[3 * i] = vx * inv; d_out[3 * i + 1] = vy * inv; d_out[3 * i + 2] = vz * inv;
+    o_out[3 * i] = o.x; o_out[3 * i + 1] = o.y; o_out[3 * i + 2] = o.z;
+    d_out[3 * i] = d.x; d_out[3 * i + 1] = d.y; d_out[3 * i + 2] = d.z;
     size_t plane = (size_t)H * W;
     size_t base = (size_t)im * 3 * plane + (size_t)y * W + x;
     gt_rgb[3 * i] = rgb_reel[base] * m;

@@ -14,7 +14,8 @@ and Mesh.upsample runs midpoint or Loop subdivision on the GPU (csrc/mesh_subdiv
 Mesh.occluded and Mesh.ambient_occlusion cast rays against the faces through a linear BVH on the GPU (csrc/mesh_raycast.cu), and
 load_mesh_sequence assembles the point sequence of train_4d_sdf.py from a folder of meshes. Mesh.closest_points and
 Mesh.signed_distance query the nearest point of the faces through the same BVH (csrc/mesh_distance.cu), and mesh_distance measures how
-far apart two meshes are from surface samples of each.
+far apart two meshes are from surface samples of each. Mesh.first_hit finds the first face each ray meets through that BVH, and
+Mesh.render shades the first hits of the rays of reel cameras (cameras.py), so a mesh becomes a training scene with a known answer.
 """
 import math
 import os
@@ -31,6 +32,8 @@ _SLAB_POINTS = 1 << 24
 _INT_MAX = 2 ** 31 - 1
 # workspace of psdf_mesh_components: int64 info[4] in the first 256 bytes, then int32 labels [V], then int32 face counts [V]
 _CC_HEADER = 256
+# the images Mesh.render can produce, in the order of psdf_mesh_render's outputs
+RENDER_OUTPUTS = ("rgb", "mask", "depth", "normal", "face")
 
 
 def _check_f(fn, Fc):
@@ -334,8 +337,7 @@ class Mesh:
         faces repeating a vertex are allowed."""
         fn = "Mesh.occluded"
         o, d = _check_rays(fn, origins, dirs, self.V)
-        if not (math.isfinite(float(tnear)) and not math.isnan(float(tfar))):
-            raise RuntimeError("%s: tnear must be finite and tfar a number, got %r, %r" % (fn, tnear, tfar))
+        _check_window(fn, tnear, tfar)
         with torch.cuda.device(o.device):
             V, Fc, ws = self._bvh(fn)
             hit = torch.empty(o.shape[0], dtype=torch.uint8, device=o.device)
@@ -365,6 +367,67 @@ class Mesh:
             vis = torch.empty(V.shape[0], dtype=torch.float32, device=V.device)
             call("psdf_mesh_ambient_occlusion", V.shape[0], Fc.shape[0], S, V, NV.contiguous(), dirs, ws, vis)
         return vis
+
+    def first_hit(self, origins, dirs, tnear=0.0, tfar=math.inf):
+        """first-hit ray casting on the GPU -> (t float32 [R], face int32 [R], bary float32 [R,3]): of the faces that pass occluded's
+        ray-triangle test for ray r with tnear < t < tfar, the one with the smallest fp32 t, ties to the smallest face index; bary =
+        ((1 - u) - v, u, v) of the test's u and v, so the hit point is (b0 a + b1 b) + b2 c. A miss is (+inf, -1, 0). The answer is that
+        of testing every face (a BVH built on each call only prunes) and the same bits on every run. Rays, V and F are checked as occluded
+        checks them."""
+        fn = "Mesh.first_hit"
+        o, d = _check_rays(fn, origins, dirs, self.V)
+        _check_window(fn, tnear, tfar)
+        with torch.cuda.device(o.device):
+            V, Fc, ws = self._bvh(fn)
+            R = o.shape[0]
+            t = torch.empty(R, dtype=torch.float32, device=o.device)
+            face = torch.empty(R, dtype=torch.int32, device=o.device)
+            bary = torch.empty(R, 3, dtype=torch.float32, device=o.device)
+            call("psdf_mesh_first_hit", V.shape[0], Fc.shape[0], R, o, d, float(tnear), float(tfar), ws, t, face, bary)
+        return t, face, bary
+
+    def render(self, K, tf_world_cam, H, W, colors=None, tnear=0.0, tfar=math.inf, outputs=RENDER_OUTPUTS):
+        """renders the mesh from I reel cameras on the GPU, one ray per pixel: the ray of pixel (x, y) of image i is the one
+        PermutoSDF.rays_from_reel_indices forms for pix = y W + x, img = i, bit for bit (a trainer drawing that pixel casts the ray that
+        rendered it), and its first_hit within (tnear, tfar) is shaded:
+          normal  (b0 N_a + b1 N_b) + b2 N_c of NV when the mesh has it, else the face's cross(p_b - p_a, p_c - p_a), normalised (0 when its
+                  length is 0); in world coordinates and not flipped toward the camera
+          rgb     (b0 C_a + b1 C_b) + b2 C_c of colors [V,3] when given, else 0.5 + 0.5 normal (bench.analytic_reel's shading)
+          mask 1, depth t, face the face index; a missed pixel is 0 everywhere and face -1 (a reel's rgb is already multiplied by its mask)
+        K float32 [I,3,3] and tf_world_cam float32 [I,4,4] (camera to world), finite, on V's device; H, W positive with H W < 2^31.
+        -> dict of the names in `outputs` (any of "rgb", "mask", "depth", "normal", "face"): rgb and normal float32 [I,3,H,W], mask and depth
+        float32 [I,1,H,W], face int32 [I,1,H,W]; other outputs are not computed. The same bits on every run. V and F are checked as
+        occluded checks them."""
+        fn = "Mesh.render"
+        V = self.V
+        if not isinstance(V, torch.Tensor) or not V.is_cuda:
+            raise RuntimeError("%s: V must be a CUDA tensor (there is no CPU path)" % fn)
+        for name, v in (("H", H), ("W", W)):
+            if isinstance(v, bool) or not isinstance(v, (int, np.integer)) or v < 1:
+                raise RuntimeError("%s: %s must be a positive integer, got %r" % (fn, name, v))
+        H, W = int(H), int(W)
+        if H * W > _INT_MAX:
+            raise RuntimeError("%s: a %d x %d image has 2^31 or more pixels" % (fn, H, W))
+        K = _check_camera(fn, "K", K, (3, 3), V.device)
+        tf = _check_camera(fn, "tf_world_cam", tf_world_cam, (4, 4), V.device)
+        if K.shape[0] != tf.shape[0]:
+            raise RuntimeError("%s: %d K and %d tf_world_cam" % (fn, K.shape[0], tf.shape[0]))
+        outputs = tuple(outputs)
+        bad = [o for o in outputs if o not in RENDER_OUTPUTS]
+        if bad:
+            raise RuntimeError("%s: unknown output %r; the outputs are %s" % (fn, bad[0], ", ".join(RENDER_OUTPUTS)))
+        _check_window(fn, tnear, tfar)
+        NV = _check_vertex_field(fn, "NV", self.NV, V)
+        C = _check_vertex_field(fn, "colors", colors, V)
+        I = K.shape[0]
+        with torch.cuda.device(V.device):
+            Vc, Fc, ws = self._bvh(fn)
+            shapes = {"rgb": (3, torch.float32), "mask": (1, torch.float32), "depth": (1, torch.float32), "normal": (3, torch.float32),
+                      "face": (1, torch.int32)}
+            out = {o: torch.empty(I, shapes[o][0], H, W, dtype=shapes[o][1], device=V.device) for o in outputs}
+            call("psdf_mesh_render", Vc.shape[0], Fc.shape[0], Vc, Fc, NV, C, I, H, W, K, tf, float(tnear), float(tfar), ws,
+                 *[out.get(o) for o in RENDER_OUTPUTS])
+        return out
 
     # ------------------------------------------------------------------ distances
     def _closest(self, fn, p):
@@ -619,6 +682,36 @@ def _check_rays(fn, origins, dirs, V):
     if out[0].shape[0] != out[1].shape[0]:
         raise RuntimeError("%s: %d origins and %d dirs" % (fn, out[0].shape[0], out[1].shape[0]))
     return out
+
+
+def _check_window(fn, tnear, tfar):
+    if not (math.isfinite(float(tnear)) and not math.isnan(float(tfar))):
+        raise RuntimeError("%s: tnear must be finite and tfar a number, got %r, %r" % (fn, tnear, tfar))
+
+
+def _check_camera(fn, name, x, shape, device):
+    """float32 [I, *shape] finite on device -> contiguous"""
+    if not isinstance(x, torch.Tensor) or x.dim() != 3 or tuple(x.shape[1:]) != shape:
+        raise RuntimeError("%s: %s must be a tensor of shape [I,%d,%d], got %s" % (
+            fn, name, shape[0], shape[1], list(x.shape) if isinstance(x, torch.Tensor) else type(x).__name__))
+    if x.dtype != torch.float32:
+        raise RuntimeError("%s: %s must be float32, got %s" % (fn, name, x.dtype))
+    if x.device != device:
+        raise RuntimeError("%s: %s must be on V's device %s, got %s" % (fn, name, device, x.device))
+    if not bool(torch.isfinite(x).all()):
+        raise RuntimeError("%s: %s has values that are not finite" % (fn, name))
+    return x.contiguous()
+
+
+def _check_vertex_field(fn, name, x, V):
+    """None, or float32 [V,3] on V's device -> contiguous"""
+    if x is None:
+        return None
+    if not isinstance(x, torch.Tensor) or x.dtype != torch.float32 or tuple(x.shape) != tuple(V.shape):
+        raise RuntimeError("%s: %s must be a float32 tensor of shape [V,3] = %s" % (fn, name, list(V.shape)))
+    if x.device != V.device:
+        raise RuntimeError("%s: %s must be on V's device %s, got %s" % (fn, name, V.device, x.device))
+    return x.contiguous()
 
 
 def _check_points(fn, points, V):
