@@ -817,6 +817,44 @@ int psdf_mesh_signed_distance(int V, int F, long long P, const float* points, co
 int psdf_mesh_sample_surface(int V, int F, const float* verts, const int* faces, const double* cdf, long long N, uint64_t seed,
                              float* points_out, int* face_out, void* stream);
 
+/* ---------------------------------------------------------------- mesh winding numbers (csrc/mesh_winding.cu)
+ * Generalized winding numbers (Jacobson et al. 2013) of points against the faces of verts [V,3] (float) and faces [F,3] (int32) through
+ * the BVH of psdf_mesh_bvh_build, with the far field of Barill et al. 2018 for triangle soups. Built with -fmad=false; oracle/winding.py
+ * sums every face in fp64 under the same rules. w(p) = (1/4 pi) sum_f Omega_f(p): 1 inside and 0 outside a closed, outward mesh, -1
+ * inside an inward one, k where k closed copies overlap, in between across holes; it depends on the triangles alone, not on
+ * connectivity, welding or manifoldness.
+ * Solid angle of face (p0, p1, p2) from p (Van Oosterom and Strackee 1983), fp32 as in the ray casting section: a = p0 - p, b = p1 - p,
+ *   c = p2 - p, det = dot(a, cross(b, c)); 0 when cross(p1 - p0, p2 - p0) == (0, 0, 0) (zero fp32 area: equal corners, which every face
+ *   that repeats a vertex has, or collinear ones) or det == 0 (p in the face's plane, p on a corner) or NaN, so no degenerate face gives
+ *   atan2(+-0, negative) = +-pi. Otherwise la = sqrtf(dot(a, a)),
+ *   lb, lc alike, den = (((la lb) lc + dot(a, b) lc) + dot(b, c) la) + dot(c, a) lb, Omega = 2 atan2f(det, den).
+ * Moments (psdf_mesh_winding_build), for every internal node of the tree, bottom-up as the box refit (the second child to arrive goes
+ *   on): A = the node's area; c = its area-weighted centroid (the centre of its box when A = 0), rounded to fp32; r = the distance from c
+ *   to the farthest corner of its box, rounded up to fp32; and, about c, M0 = sum A n, M1_ji = sum int (x - c)_j n_i dA and M2_jki = 1/2
+ *   sum int (x - c)_j (x - c)_k n_i dA (symmetric in j, k). A face's moments are integrated exactly (faces of zero fp32 area have
+ *   none); a node's are its children's, child 0 then child 1, shifted algebraically to its c; all in fp64, stored in fp32, so the bits
+ *   do not depend on which child arrives second.
+ * Query (psdf_mesh_winding_number): one point per thread, 64-bit point ids, 64-entry stack, depth first with child 0 first. An internal
+ *   node with fp32 dot(p - c, p - c) > (beta r)(beta r) contributes its order-2 expansion, in fp64 with R = c - p, s = |R|:
+ *   (M0 . R + tr M1) / s^3 - 3 R^T M1 R / s^5 - 3 (2 sum_ji M2_jii R_j + sum_ji M2_jji R_i) / s^5 + 15 sum_jki M2_jki R_j R_k R_i / s^7;
+ *   otherwise its children are visited; a leaf always contributes Omega. The terms are summed in fp64 in that order and w_out[p] (float)
+ *   = float(sum / 4 pi), rounded once. No atomics: the same bits on every run and for any launch shape. beta = +inf never takes the far
+ *   field and gives the exact sum over all faces in tree order; beta = 2 is the usual trade (DESIGN.md 5a has its measured error). F = 0
+ *   gives 0; F = 1 has no internal node.
+ * Workspace: psdf_mesh_winding_workspace_bytes(V, F) = 144 (F - 1) B of node moments (c, r, M0, A, M1, M2, a zero) + 4 (F - 1) B of
+ *   arrival flags (sections each padded to 256 B; 0 when F < 2, and then workspace may be NULL). The BVH workspace is read only and its
+ *   layout is unchanged. PSDF_ERR_UNSUPPORTED when V or F is 2^31 or more, PSDF_ERR_ARG when negative.
+ * psdf_mesh_winding_build: fills workspace from bvh_workspace, the psdf_mesh_bvh_build workspace of the same V and F; verts and faces
+ *   are not read (the BVH holds the sorted corners).
+ * psdf_mesh_winding_number: w_out [P] (float) of points [P,3]; bvh_workspace and workspace as built above (read only). PSDF_ERR_ARG when
+ *   beta is not positive (or NaN); P is 64-bit (PSDF_ERR_UNSUPPORTED above 256 (2^31 - 1)); P = 0 launches nothing.
+ * Cost: build O(F); a query visits the nodes it is not beyond beta r of, and the faces of the leaves below them. */
+long long psdf_mesh_winding_workspace_bytes(long long nr_vertices, long long nr_faces);
+int psdf_mesh_winding_build(int V, int F, const float* verts, const int* faces, const uint8_t* bvh_workspace, uint8_t* workspace,
+                            void* stream);
+int psdf_mesh_winding_number(int V, int F, long long P, const float* points, const uint8_t* bvh_workspace, const uint8_t* workspace,
+                             float beta, float* w_out, void* stream);
+
 /* ---------------------------------------------------------------- image metrics (csrc/image_metrics.cu)
  * Per-image PSNR and SSIM of the reference's experiments/evaluation/evaluate_psnr.py, which scores each frame with piq.psnr and piq.ssim
  * (data_range = 1; kernel 11, sigma 1.5, k1 0.01, k2 0.03, downsampling on). x (the prediction) and y (the ground truth) are float images of

@@ -16,6 +16,8 @@ load_mesh_sequence assembles the point sequence of train_4d_sdf.py from a folder
 Mesh.signed_distance query the nearest point of the faces through the same BVH (csrc/mesh_distance.cu), and mesh_distance measures how
 far apart two meshes are from surface samples of each. Mesh.first_hit finds the first face each ray meets through that BVH, and
 Mesh.render shades the first hits of the rays of reel cameras (cameras.py), so a mesh becomes a training scene with a known answer.
+Mesh.winding_number sums the faces' solid angles through the same BVH with a hierarchical far field (csrc/mesh_winding.cu), which gives
+an inside/outside for any triangle soup: Mesh.signed_distance(points, sign="winding").
 """
 import math
 import os
@@ -474,14 +476,25 @@ class Mesh:
             raise RuntimeError("%s: %d faces have a vertex index outside [0, %d)" % (fn, bad, nv))
         return face_n, vert_n, edge_n
 
-    def signed_distance(self, points):
+    def signed_distance(self, points, sign="pseudonormal"):
         """signed distance from the faces to each of points [P,3] (float32 CUDA on V's device, finite), on the GPU -> float32 [P],
-        negative inside: sqrt of closest_points' squared distance, with the sign of dot(p - q, n), n the angle-weighted pseudonormal of the
-        vertex, edge or face holding the closest point q (include/psdf_b200.h); a zero dot gives +0, a mesh without faces +inf. The sign
-        is right only for a closed, consistently oriented (outward), edge-manifold mesh, such as marching_cubes gives; topology is not
-        checked. For other meshes the magnitude is still the unsigned distance."""
+        negative inside: sqrt of closest_points' squared distance, with a sign by one of two definitions:
+          "pseudonormal" (the default)  the sign of dot(p - q, n), n the angle-weighted pseudonormal of the vertex, edge or face holding the
+                  closest point q (include/psdf_b200.h); a zero dot gives +0. Exact and one traversal, but right only for a closed,
+                  consistently oriented (outward), edge-manifold mesh, such as marching_cubes gives; topology is not checked.
+          "winding"  negative where winding_number(points) > 0.5, else +: defined for any triangle soup (holes, overlaps, unwelded or
+                  non-manifold faces), but approximate far from the faces (beta = 2); use it for meshes that are not closed manifolds.
+        In both, a zero distance is +0 and a mesh without faces gives +inf."""
         fn = "Mesh.signed_distance"
+        if sign not in ("pseudonormal", "winding"):
+            raise RuntimeError("%s: unknown sign %r; the signs are 'pseudonormal' and 'winding'" % (fn, sign))
         p = _check_points(fn, points, self.V)
+        if sign == "winding":
+            with torch.cuda.device(p.device):
+                V, Fc, ws, dist2, _, _ = self._closest(fn, p)
+                w = self._winding(fn, p, V, Fc, ws, 2.0)
+            dist = torch.sqrt(dist2)
+            return torch.where((w > 0.5) & (dist > 0), -dist, dist)
         with torch.cuda.device(p.device):
             face_n, vert_n, edge_n = self._pseudonormals(fn)
             V, Fc, ws = self._bvh(fn)
@@ -492,6 +505,31 @@ class Mesh:
             sdf = torch.empty(P, dtype=torch.float32, device=p.device)
             call("psdf_mesh_signed_distance", V.shape[0], Fc.shape[0], P, p, V, Fc, ws, face_n, vert_n, edge_n, dist2, face, bary, sdf)
         return sdf
+
+    def _winding(self, fn, p, V, Fc, bvh, beta):
+        """psdf_mesh_winding_build on the BVH workspace bvh of (V, Fc), then psdf_mesh_winding_number of the checked points p -> float32 [P]"""
+        nv, nf = V.shape[0], Fc.shape[0]
+        ws = torch.empty(int(load_library().psdf_mesh_winding_workspace_bytes(nv, nf)), dtype=torch.uint8, device=V.device)
+        call("psdf_mesh_winding_build", nv, nf, V, Fc, bvh, ws)
+        w = torch.empty(p.shape[0], dtype=torch.float32, device=p.device)
+        call("psdf_mesh_winding_number", nv, nf, p.shape[0], p, bvh, ws, float(beta), w)
+        return w
+
+    def winding_number(self, points, beta=2.0):
+        """generalized winding number of each of points [P,3] (float32 CUDA on V's device, finite) against the faces, on the GPU ->
+        float32 [P]: (1/4 pi) times the sum of the signed solid angles of the faces seen from the point (Jacobson et al. 2013). About 1
+        inside and 0 outside a closed, outward mesh, -1 inside an inward one, k where k closed copies overlap, and in between across holes;
+        it depends on the triangles alone, not on connectivity, welding or manifoldness. Faces with two equal corners (those repeating a
+        vertex included) and faces whose plane holds the point contribute 0. A BVH node whose centroid is farther than beta times its
+        radius contributes its order-2 moment expansion (Barill et al. 2018); beta = math.inf sums every face exactly (fp32 solid angles,
+        fp64 sum). The same bits on every run and for any order of the points. V and F are checked as occluded checks them."""
+        fn = "Mesh.winding_number"
+        if isinstance(beta, bool) or not isinstance(beta, (int, float, np.integer, np.floating)) or not float(beta) > 0:
+            raise RuntimeError("%s: beta must be a positive number (math.inf for the exact sum), got %r" % (fn, beta))
+        p = _check_points(fn, points, self.V)
+        with torch.cuda.device(p.device):
+            V, Fc, bvh = self._bvh(fn)
+            return self._winding(fn, p, V, Fc, bvh, beta)
 
     def _area_cdf(self, fn):
         """the cdf psdf_mesh_sample_surface draws faces from -> (V, F, cdf fp64 [F]): the face areas |(b - a) x (c - a)| / 2 in fp64 (0 for
