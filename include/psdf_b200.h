@@ -678,40 +678,53 @@ int psdf_mesh_subdivide_count(int V, int F, const int* faces, uint8_t* workspace
 int psdf_mesh_subdivide_emit(int V, int F, int smooth, const float* verts, const int* faces, uint8_t* workspace, float* verts_out,
                              int* faces_out, void* stream);
 
+/* ---------------------------------------------------------------- mesh BVH (csrc/mesh_bvh.cu)
+ * A linear BVH over the faces of verts [V,3] (float) and faces [F,3] (int32), built once and read by the ray casting, distance and winding
+ * queries below, which pass the same V and F. Built with -fmad=false.
+ * Build: the faces are sorted by Morton code (four stable 8-bit radix passes), Karras' radix tree (2012) gives the F - 1 internal nodes
+ *   (root 0), and the boxes are refit bottom-up. Faces with an index outside [0, V) are counted into info[0] (faces that repeat a vertex
+ *   into info[1]; they are allowed) and get an empty box and NaN corners, so nothing out of range is read; the caller refuses them. F = 0
+ *   (nothing is hit), F = 1, equal centroids and all faces at one point build a valid tree.
+ * Boxes are the exact fp32 min / max of their triangles' corners; a query grows them by a pad of 2^-12 times a scale that includes s, the
+ *   largest |coordinate| of the mesh (the ray and distance sections state their pads and why they are enough).
+ * Traversal (rays and closest points): depth first from the root; at each internal node both children's boxes are tested and the child
+ *   of smaller key (the slab entry for rays, the box distance for points) goes first when both pass, child 0 on a tie; after a first
+ *   child that is a leaf has been visited, the second is tested again against the query's bound as it now stands, and a popped node is
+ *   skipped when its key fails that bound. Stack: 64 entries. Sort keys are the 30-bit Morton code of each centroid (within the centroids'
+ *   bounds) with the sorted position breaking ties, so every internal node's common prefix length lies in [2, 63] and grows strictly from
+ *   parent to child: at most 62 internal nodes lie on a path, and only internal nodes are pushed, at most one per level.
+ * Workspace: psdf_mesh_bvh_workspace_bytes(V, F) ~ 152 B per face + 4 B per vertex (sections each padded to 256 B): int64 info[4] at byte
+ *   0 = {faces with an index outside [0, V), faces that repeat a vertex, 0, 0}, uint32 bounds [8] (ordered keys of the centroid bounds, the
+ *   bits of s), uint32 keys [2][F], int32 face ids [2][F], int32 radix histogram [256 ceil(F / 256)], int64 its prefix [+ 1], int64 scan
+ *   tile sums, nodes [F - 1] of 64 B (both children's boxes, then the children; child >= F - 1 is leaf child - (F - 1)), int32 parents
+ *   [2F - 1], int32 refit flags [F - 1], the sorted triangles [F] of 48 B (p0, p1, p2), int32 hit counts [V] (psdf_mesh_ambient_occlusion's).
+ *   PSDF_ERR_UNSUPPORTED when V or F is 2^31 or more, PSDF_ERR_ARG when negative.
+ * psdf_mesh_bvh_build: fills the workspace; queries pass the same V and F and read it.
+ * Cost: build O(F) (sort, tree and refit are one pass each). */
+long long psdf_mesh_bvh_workspace_bytes(long long nr_vertices, long long nr_faces);
+int psdf_mesh_bvh_build(int V, int F, const float* verts, const int* faces, uint8_t* workspace, void* stream);
+
 /* ---------------------------------------------------------------- mesh ray casting (csrc/mesh_raycast.cu)
- * Any-hit and first-hit queries of rays against the triangles of verts [V,3] (float) and faces [F,3] (int32) through a linear BVH, per-vertex
- * ambient occlusion and rendering from reel cameras. Built with -fmad=false; oracle/raycast.py restates the triangle test and checks every
- * any-hit answer by brute force, tests/first_hit_oracle.py every first hit and rendered pixel.
+ * Any-hit and first-hit queries of rays against the triangles of verts [V,3] (float) and faces [F,3] (int32) through the mesh BVH above,
+ * per-vertex ambient occlusion and rendering from reel cameras. Built with -fmad=false; oracle/raycast.py restates the triangle test and
+ * checks every any-hit answer by brute force, tests/first_hit_oracle.py every first hit and rendered pixel.
  * Ray-triangle test (two-sided Moller-Trumbore, fp32, each operation rounded as written; dot(a, b) = (ax bx + ay by) + az bz, cross(a, b) =
  *   (ay bz - az by, az bx - ax bz, ax by - ay bx)): e1 = p1 - p0, e2 = p2 - p0, pv = cross(d, e2), det = dot(e1, pv); det == 0 or NaN
  *   misses. inv = 1.0f / det, tv = o - p0, u = dot(tv, pv) * inv, miss unless 0 <= u <= 1; qv = cross(tv, e1), v = dot(d, qv) * inv, miss
  *   unless v >= 0 and u + v <= 1; t = dot(e2, qv) * inv, hit iff tnear < t < tfar. A face that repeats a vertex has det == 0: never hit.
  * A ray is occluded exactly when some triangle passes the test; the tree only chooses which triangles are tested, so it changes no answer
  *   as long as its box test passes every box that holds a passing triangle:
- *   - Boxes are the exact fp32 min / max of their triangles' corners, grown at query time by pad = 2^-12 (s + max |o_k|), s the largest
- *     |coordinate| of the mesh. A passing (u, v, t) puts o + t d within |r| of the triangle, |r| <= c eps |tv| |d| |e1| |e2| / |det|
- *     (c ~ 10, eps = 2^-24, |tv| <= sqrt(3) (s + max |o_k|)); that is below pad unless the ray lies within about 1 degree of the triangle's
- *     plane (|det| < 2^-6 |d| |e1| |e2|). A ray that close to a far triangle's plane can pass the test by rounding alone, anywhere in that
- *     plane; such far passes are the one case where the answer can differ from the brute-force one. Zero-thickness boxes (axis-aligned
- *     triangles) are thickened by the pad, so origins on their planes lie inside.
+ *   - Boxes are grown at query time by pad = 2^-12 (s + max |o_k|). A passing (u, v, t) puts o + t d within |r| of the triangle,
+ *     |r| <= c eps |tv| |d| |e1| |e2| / |det| (c ~ 10, eps = 2^-24, |tv| <= sqrt(3) (s + max |o_k|)); that is below pad unless the ray lies
+ *     within about 1 degree of the triangle's plane (|det| < 2^-6 |d| |e1| |e2|). A ray that close to a far triangle's plane can pass the
+ *     test by rounding alone, anywhere in that plane; such far passes are the one case where the answer can differ from the brute-force
+ *     one. Zero-thickness boxes (axis-aligned triangles) are thickened by the pad, so origins on their planes lie inside.
  *   - Slab test: per axis, d_k == 0 requires lo_k - pad <= o_k <= hi_k + pad exactly (no 1/0, no 0 * inf); a d_k whose reciprocal is not
  *     finite leaves that axis out (conservative); otherwise the slab interval of (bound - o_k) * (1 / d_k). The box passes when
  *     max(tnear, slab starts) <= t1 + |t1| 2^-20 with t1 = min(tfar, slab ends): 2^-20 exceeds the 2 gamma_3 that covers the rounding of
  *     the slab arithmetic (Ize, Robust BVH ray traversal, 2013).
- *   - Traversal stack: 64 entries. Keys are the 30-bit Morton code of each centroid (within the centroids' bounds) with the sorted position
- *     breaking ties, so every internal node's common prefix length lies in [2, 63] and grows strictly from parent to child: at most 62
- *     internal nodes lie on a path, and only internal nodes are pushed, at most one per level.
- * Build: the faces are sorted by Morton code (four stable 8-bit radix passes), Karras' radix tree (2012) gives the F - 1 internal nodes
- *   (root 0), and the boxes are refit bottom-up. Faces with an index outside [0, V) are counted into info[0] (faces that repeat a vertex
- *   into info[1]; they are allowed) and get an empty box and NaN corners, so nothing out of range is read; the caller refuses them. F = 0
- *   (nothing is hit), F = 1, equal centroids and all faces at one point build a valid tree.
- * Workspace: psdf_mesh_bvh_workspace_bytes(V, F) ~ 152 B per face + 4 B per vertex (sections each padded to 256 B): int64 info[4] at byte
- *   0 = {faces with an index outside [0, V), faces that repeat a vertex, 0, 0}, uint32 bounds [8] (ordered keys of the centroid bounds, the
- *   bits of s), uint32 keys [2][F], int32 face ids [2][F], int32 radix histogram [256 ceil(F / 256)], int64 its prefix [+ 1], int64 scan
- *   tile sums, nodes [F - 1] of 64 B (both children's boxes, then the children; child >= F - 1 is leaf child - (F - 1)), int32 parents
- *   [2F - 1], int32 refit flags [F - 1], the sorted triangles [F] of 48 B (p0, p1, p2), int32 hit counts [V]. PSDF_ERR_UNSUPPORTED when V
- *   or F is 2^31 or more, PSDF_ERR_ARG when negative.
- * psdf_mesh_bvh_build: fills the workspace; queries pass the same V and F and read it.
+ *   - Any hit walks the tree as the BVH section states with every key equal (child 0 first) and no bound, and stops at the first passing
+ *     triangle.
  * psdf_mesh_occluded: hit_out[r] (uint8) = 1 when ray r (origins [R,3], dirs [R,3], any length) is occluded within (tnear, tfar); R is
  *   64-bit (PSDF_ERR_UNSUPPORTED above 256 (2^31 - 1)).
  * psdf_mesh_ambient_occlusion: V S rays, one per (vertex i, direction s), 64-bit ray ids: origin verts[i], direction dirs[s] [S,3], negated
@@ -721,10 +734,12 @@ int psdf_mesh_subdivide_emit(int V, int F, int smooth, const float* verts, const
  *   smallest original face index -> t_out [R] (float) = that t, face_out [R] (int32) = the face, bary_out [R,3] (float) = ((1 - u) - v, u,
  *   v) with the test's u and v, rounded as written; no such face (F = 0 included): (+inf, -1, 0). The answer is that of testing every face;
  *   the tree only prunes. Nearer child first by the slab entry max(tnear, slab starts) (child 0 on equal entries); a box is skipped when
- *   the slab test above fails against (tnear, min(tfar, best t)); it is non-strict, so boxes holding a tie are still visited. Leaves use
- *   the test with the caller's tfar. Far passes (see above) can make a first hit differ from the brute-force one in the same way: a ray
- *   within about 1 degree of a far triangle's plane can pass the test by rounding outside that triangle's padded box. Same workspace
- *   (read only), ray ids and limits as psdf_mesh_occluded; no atomics, so the bits are the same on every run and for any launch shape.
+ *   the slab test above fails against (tnear, min(tfar, best t)); it is non-strict, so boxes holding a tie are still visited. The second
+ *   child after a leaf, and a popped node, are skipped when their entry exceeds c + |c| 2^-20 with c = min(tfar, best t) of then: the
+ *   slab test's last comparison, which the full test would fail too. Leaves use the test with the caller's tfar. Far passes (see above)
+ *   can make a first hit differ from the brute-force one in the same way: a ray within about 1 degree of a far triangle's plane can pass
+ *   the test by rounding outside that triangle's padded box. Same workspace (read only), ray ids and limits as psdf_mesh_occluded; no
+ *   atomics, so the bits are the same on every run and for any launch shape.
  * psdf_mesh_render: I images of H x W pixels (H W < 2^31), one thread per (image, pixel), 64-bit ids. The ray of pixel (x, y) of image i
  *   is that of psdf_random_rays_from_reel for pix = y W + x, img = i, bit for bit: centre (x + 0.5, y + 0.5), K [I,3,3] (row-major, reads
  *   K[0], K[2], K[4], K[5]), tf_world_cam [I,4,4] (row-major), normalised with rsqrtf. Its first hit (psdf_mesh_first_hit under tnear,
@@ -736,9 +751,7 @@ int psdf_mesh_subdivide_emit(int V, int F, int smooth, const float* verts, const
  *   [I,1,H,W] (int32); a NULL output is not written. Each warp takes an 8 x 4 pixel tile, so its rays stay coherent; every pixel is
  *   computed on its own, so the mapping changes no bit, and the result is the same bits on every run. workspace is the psdf_mesh_bvh_build
  *   workspace of verts and faces (read only). PSDF_ERR_UNSUPPORTED when H W >= 2^31 or the threads exceed 256 (2^31 - 1).
- * Cost: build O(F) (sort, tree and refit are one pass each); a query visits the nodes whose padded boxes the ray meets. */
-long long psdf_mesh_bvh_workspace_bytes(long long nr_vertices, long long nr_faces);
-int psdf_mesh_bvh_build(int V, int F, const float* verts, const int* faces, uint8_t* workspace, void* stream);
+ * Cost: a query visits the nodes whose padded boxes the ray meets. */
 int psdf_mesh_occluded(int V, int F, long long R, const float* origins, const float* dirs, float tnear, float tfar, const uint8_t* workspace,
                        uint8_t* hit_out, void* stream);
 int psdf_mesh_first_hit(int V, int F, long long R, const float* origins, const float* dirs, float tnear, float tfar, const uint8_t* workspace,
@@ -775,11 +788,11 @@ int psdf_mesh_ambient_occlusion(int V, int F, int S, const float* verts, const f
  * Answer: among the faces with three distinct indices, the smallest dist2, ties to the smallest face index; faces that repeat a vertex are
  *   skipped (occluded never hits them). No such face: dist2 = +inf, face = -1, bary = 0.
  * The tree only prunes: a node is skipped when its bound is strictly above the best dist2 so far, so ties are visited. The bound is the
- *   fp32 dist2 from p to the box grown by pad = 2^-12 s (s as for the rays): per axis max((lo - pad) - p, p - (hi + pad), 0), then
+ *   fp32 dist2 from p to the box grown by pad = 2^-12 s (s as in the BVH section): per axis max((lo - pad) - p, p - (hi + pad), 0), then
  *   (ex ex + ey ey) + ez ez. Every closest point above is x + t e with 0 <= t <= 1 or (a + v ab) + w ac with v, w >= 0 and v + w <= 1,
  *   so it lies within a few ulps of s (far below pad) of its face's exact box; then |p_k - q_k| rounded is at least the box gap per axis,
- *   and rounding is monotone, so the bound never exceeds the face's computed dist2. Nearer child first (child 0 on a tie), 64-entry stack
- *   as for the rays, one query per thread, 64-bit query ids.
+ *   and rounding is monotone, so the bound never exceeds the face's computed dist2. The walk is the BVH section's with the bound as
+ *   key (nearer child first, child 0 on a tie), one query per thread, 64-bit query ids.
  * psdf_mesh_closest_points: dist2_out [P] (float), face_out [P] (int32, the original face index), bary_out [P,3] (float) of points [P,3];
  *   workspace is a psdf_mesh_bvh_build workspace of the same V and F (read only; verts is not read). P is 64-bit (PSDF_ERR_UNSUPPORTED
  *   above 256 (2^31 - 1)); P = 0 launches nothing.

@@ -1,6 +1,7 @@
 """Ray casting against a triangle mesh by brute force (numpy, fp32): the ray-triangle test of include/psdf_b200.h (two-sided
 Moller-Trumbore, each operation rounded as written), tested against every triangle, and occluded / ambient_occlusion restated on top of it.
-csrc/mesh_raycast.cu gives the same answers through its BVH."""
+intersect also returns the test's t, u and v, for the first hits of tests/first_hit_oracle.py. csrc/mesh_raycast.cu gives the same answers
+through its BVH."""
 import math
 
 import numpy as np
@@ -17,8 +18,9 @@ def cross(a, b):
                      a[..., 0] * b[..., 1] - a[..., 1] * b[..., 0]], -1)
 
 
-def hit(p0, p1, p2, o, d, tnear, tfar):
-    """the test of every pair of triangles (p0, p1, p2 [..., 3]) and rays (o, d [..., 3]), broadcast -> bool [...]"""
+def intersect(p0, p1, p2, o, d, tnear, tfar):
+    """the test of every pair of triangles (p0, p1, p2 [..., 3]) and rays (o, d [..., 3]), broadcast -> (pass bool [...], t, u, v float32
+    [...]); t, u and v are meaningful where the test passes"""
     p0, p1, p2, o, d = (np.asarray(x, f32) for x in (p0, p1, p2, o, d))
     tnear, tfar = f32(tnear), f32(tfar)
     with np.errstate(all="ignore"):
@@ -34,7 +36,12 @@ def hit(p0, p1, p2, o, d, tnear, tfar):
         v = dot(d, qv) * inv
         ok &= (v >= 0) & (u + v <= 1)
         t = dot(e2, qv) * inv
-        return ok & (t > tnear) & (t < tfar)
+        return ok & (t > tnear) & (t < tfar), t, u, v
+
+
+def hit(p0, p1, p2, o, d, tnear, tfar):
+    """the test of every pair of triangles (p0, p1, p2 [..., 3]) and rays (o, d [..., 3]), broadcast -> bool [...]"""
+    return intersect(p0, p1, p2, o, d, tnear, tfar)[0]
 
 
 def occluded(V, F, origins, dirs, tnear=1e-4, tfar=math.inf, chunk=1 << 22):

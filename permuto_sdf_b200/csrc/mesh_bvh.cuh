@@ -1,5 +1,7 @@
-// The linear BVH over the faces of an indexed triangle mesh, shared by mesh_raycast.cu (which builds it and casts rays) and
-// mesh_distance.cu (closest points). The workspace layout, the node format and the box padding are stated in include/psdf_b200.h.
+// The linear BVH over the faces of an indexed triangle mesh: its workspace, its node format, and the two walks over it. mesh_bvh.cu
+// builds the tree; mesh_raycast.cu (any and first hits), mesh_distance.cu (closest points) and mesh_winding.cu (winding numbers) read it.
+// traverse is the top-down walk of the ray and distance queries, climb the bottom-up one of the box refit and the winding moments. The
+// workspace layout, the node format, the box padding and the traversal rules are stated in include/psdf_b200.h.
 #pragma once
 #include "mesh_csr.cuh"
 
@@ -72,5 +74,95 @@ __device__ __forceinline__ void leaf_corners(const Ws& W, long long i, float3& p
     p0 = make_float3(x.x, x.y, x.z);
     p1 = make_float3(x.w, y.x, y.y);
     p2 = make_float3(y.z, y.w, z.x);
+}
+
+// ---------------------------------------------------------------- nodes
+struct Box {
+    float3 lo, hi;
+};
+
+// internal node i as a walk reads it: the boxes of both children and the children (>= F - 1: leaf child - (F - 1))
+struct NodeView {
+    Box box[2];
+    int child[2];
+};
+
+__device__ __forceinline__ NodeView load_node(const Ws& W, int i) {
+    const Node* nd = W.nodes + i;
+    const float4 a = __ldg(&nd->a), b = __ldg(&nd->b), c = __ldg(&nd->c);
+    const int4 d = __ldg(&nd->d);
+    return NodeView{{{make_float3(a.x, a.y, a.z), make_float3(a.w, b.x, b.y)}, {make_float3(b.z, b.w, c.x), make_float3(c.y, c.z, c.w)}},
+                    {d.x, d.y}};
+}
+
+// ---------------------------------------------------------------- top-down: one query, depth first
+// The walk of query q over the tree, the same rule for every query. q supplies
+//   enter(box, key)  whether to go into a child's box, and that child's order key;
+//   visit(i)         visits sorted leaf i; true ends the walk;
+//   keep(key)        whether a child entered with this key still passes the query's bound as it stands now.
+// At a node both children's boxes are tested; the one of smaller key goes first only when both enter (child 0 on a tie). A first child
+// that is a leaf is visited at once, and the second is then tested with keep again, since the visit may have tightened the bound. Of
+// two internal children the second is pushed with its key; a popped node is skipped while !keep(key). Only internal nodes are pushed,
+// at most one per level, so kStack entries hold any path (see the header).
+template <class Q> __device__ __forceinline__ void traverse(const Ws& W, int F, Q& q) {
+    if (F == 0) return;
+    if (F == 1) {                                             // the root is leaf 0
+        q.visit(0);
+        return;
+    }
+    const int nl = F - 1;                                     // children at or above nl are leaves
+    int stack[kStack];
+    float kstack[kStack];
+    int sp = 0, node = 0;
+    while (true) {
+        const NodeView nd = load_node(W, node);
+        float k0, k1;
+        const bool g0 = q.enter(nd.box[0], k0), g1 = q.enter(nd.box[1], k1);
+        const bool swap = g0 && g1 && k1 < k0;
+        const int n0 = swap ? nd.child[1] : nd.child[0], n1 = swap ? nd.child[0] : nd.child[1];
+        bool h0 = swap ? g1 : g0, h1 = swap ? g0 : g1;
+        const float f1 = swap ? k0 : k1;
+        if (h0 && n0 >= nl) {
+            if (q.visit(n0 - nl)) return;
+            h0 = false;
+            h1 = h1 && q.keep(f1);
+        }
+        if (h1 && n1 >= nl) {
+            if (q.visit(n1 - nl)) return;
+            h1 = false;
+        }
+        if (h0 && h1) {
+            stack[sp] = n1;
+            kstack[sp++] = f1;
+            node = n0;
+        } else if (h0 || h1) {
+            node = h0 ? n0 : n1;
+        } else {
+            do {
+                if (sp == 0) return;
+                --sp;
+            } while (!q.keep(kstack[sp]));
+            node = stack[sp];
+        }
+    }
+}
+
+// ---------------------------------------------------------------- bottom-up: one thread per leaf
+// The climb from sorted leaf i to the root, every internal node combined once, after both its children. At each parent p the child
+// first calls publish(p, slot), with slot its side of p, and fences what it and the nodes below it wrote; then it arrives on flags[p].
+// The first to arrive returns; the second calls combine(p), which reads both children's results with __ldcg (another thread of the
+// same launch may have written them), and goes on from p. flags [F - 1] must be zero before the launch.
+template <class Publish, class Combine>
+__device__ __forceinline__ void climb(const Ws& W, int F, long long i, int* flags, Publish publish, Combine combine) {
+    long long node = (F - 1) + i;
+    while (node != 0) {                                       // the root is internal node 0 (a single leaf when F = 1)
+        const int pp = W.parent[node];
+        const int p = pp >> 1;
+        publish(p, pp & 1);
+        __threadfence();
+        if (atomicAdd(flags + p, 1) == 0) return;            // the other child is not done yet; it goes on
+        combine(p);
+        node = p;
+    }
 }
 }  // namespace

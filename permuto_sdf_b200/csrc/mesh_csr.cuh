@@ -1,15 +1,22 @@
-// The vertex -> face CSR of an indexed triangle mesh and what builds it, shared by mesh_decimate.cu and mesh_subdivide.cu.
+// The vertex -> face CSR of an indexed triangle mesh and what builds it, shared by mesh_decimate.cu, mesh_distance.cu (pseudonormals)
+// and mesh_subdivide.cu.
 //
 // A unit lays out its own workspace Ws with Sections. Every such Ws holds at least
 //   long long* info;   int64 header: info[0] = faces with an index outside [0, V), info[1] = faces that repeat a vertex
 //   long long* off;    [V + 1] CSR offsets
 //   int* deg;          [V] face count, then the fill cursor
-// and the kernels here are templates on it; the unit fills the face lists itself. The offsets come from an exclusive int64 scan
-// (k_mesh_scan_tiles, k_mesh_scan_top, k_mesh_scan_out) of op(a[i], i) over an array a: Count here, and what a unit scans besides.
+// and the kernels here are templates on it. build_csr also needs
+//   int* adj;          [3F] faces of each vertex
+//   long long* tiles;  scan tile sums of at least tile_sums(V) entries
+// and fills the face lists; a unit that fills more than the lists (mesh_subdivide.cu) launches k_mesh_degree and the scan itself. The
+// offsets come from an exclusive int64 scan (k_mesh_scan_tiles, k_mesh_scan_top, k_mesh_scan_out) of op(a[i], i) over an array a: Count
+// here, and what a unit scans besides.
 //
 //   k_mesh_check      counts faces outside [0, V) and faces that repeat a vertex into info[0], info[1]   thread per face
 //   k_mesh_degree     deg[v] += 1 for the three corners of every valid face                             thread per face
 //   k_mesh_scan_*     exclusive prefix of op(a[i], i) over [0, n) and its total                          tile / one block / tile
+//   k_mesh_fill       adj[off[v] + cursor] = f for the three corners of every valid face                thread per face
+//   k_mesh_sort       heap sort of each vertex's face list                                              thread per vertex
 #pragma once
 #include "common.cuh"
 
@@ -221,5 +228,33 @@ __device__ __forceinline__ void heap_sort(int* a, long long n) {
         a[e] = x;
         sift_down(a, 0, e);
     }
+}
+
+// ---------------------------------------------------------------- the CSR
+template <class Ws>
+__global__ void __launch_bounds__(kThreads) k_mesh_fill(int V, int F, const int* __restrict__ faces, Ws W) {
+    const long long f = thread_index();
+    if (f >= F) return;
+    const int3 t = load_face(faces, f);
+    if (!valid(t, V)) return;
+    W.adj[W.off[t.x] + atomicAdd(W.deg + t.x, 1)] = (int)f;
+    W.adj[W.off[t.y] + atomicAdd(W.deg + t.y, 1)] = (int)f;
+    W.adj[W.off[t.z] + atomicAdd(W.deg + t.z, 1)] = (int)f;
+}
+
+template <class Ws> __global__ void __launch_bounds__(kThreads) k_mesh_sort(int V, Ws W) {
+    const long long v = thread_index();
+    if (v >= V) return;
+    heap_sort(W.adj + W.off[v], W.off[v + 1] - W.off[v]);
+}
+
+// the CSR of the valid faces (deg and off rebuilt); sorted: each vertex's list in ascending face order, else in fill order
+template <class Ws> void build_csr(int V, int F, const int* faces, const Ws& W, bool sorted, cudaStream_t s) {
+    cudaMemsetAsync(W.deg, 0, 4 * (size_t)V, s);
+    if (F > 0) k_mesh_degree<<<blocks(F), kThreads, 0, s>>>(V, F, faces, W);
+    scan<Count>(W.deg, V, W.tiles, W.off, s);
+    cudaMemsetAsync(W.deg, 0, 4 * (size_t)V, s);
+    if (F > 0) k_mesh_fill<<<blocks(F), kThreads, 0, s>>>(V, F, faces, W);
+    if (sorted && V > 0) k_mesh_sort<<<blocks(V), kThreads, 0, s>>>(V, W);
 }
 }  // namespace

@@ -3,12 +3,10 @@
 // candidates, locks, cost, validity, selection, apply) are stated in include/psdf_b200.h; this file only adds how they are computed.
 //
 // Vertex -> face CSR (mesh_csr.cuh): k_mesh_degree counts the faces of each vertex, the scan k_mesh_scan_* turns the counts into int64
-// offsets, k_dc_fill places the faces with atomics and k_dc_sort puts each vertex's list in ascending face order (only begin and the
+// offsets, k_mesh_fill places the faces with atomics and k_mesh_sort puts each vertex's list in ascending face order (only begin and the
 // normals need the order; a round's CSR is left as filled, every use of it there is order-free). Faces with an index outside [0, V) or a
 // repeated vertex are counted by k_mesh_check in begin and never enter the CSR. The compaction scans the faces kept with the same kernels.
 //
-//   k_dc_fill      adj[off[v] + cursor] = f                                                      thread per face
-//   k_dc_sort      heap sort of each vertex's face list                                          thread per vertex
 //   k_dc_lock      a half-edge whose direction is not there once or whose twin is not there once locks both ends   thread per half-edge
 //   k_dc_quadric   Q[v] = sum of the area-weighted plane quadrics of v's faces, ascending        thread per vertex
 //   k_dc_key       key of every candidate half-edge, best[v] = atomicMin over v's candidates    thread per half-edge
@@ -76,33 +74,6 @@ __device__ __forceinline__ double3 cross3(double3 a, double3 b) {
     return make_double3(a.y * b.z - a.z * b.y, a.z * b.x - a.x * b.z, a.x * b.y - a.y * b.x);
 }
 __device__ __forceinline__ double dot3(double3 a, double3 b) { return (a.x * b.x + a.y * b.y) + a.z * b.z; }
-
-// ---------------------------------------------------------------- the CSR
-__global__ void __launch_bounds__(kThreads) k_dc_fill(int V, int F, const int* __restrict__ faces, Ws W) {
-    const long long f = thread_index();
-    if (f >= F) return;
-    const int3 t = load_face(faces, f);
-    if (!valid(t, V)) return;
-    W.adj[W.off[t.x] + atomicAdd(W.deg + t.x, 1)] = (int)f;
-    W.adj[W.off[t.y] + atomicAdd(W.deg + t.y, 1)] = (int)f;
-    W.adj[W.off[t.z] + atomicAdd(W.deg + t.z, 1)] = (int)f;
-}
-
-__global__ void __launch_bounds__(kThreads) k_dc_sort(int V, Ws W) {
-    const long long v = thread_index();
-    if (v >= V) return;
-    heap_sort(W.adj + W.off[v], W.off[v + 1] - W.off[v]);
-}
-
-// the CSR of the valid faces (deg and off rebuilt)
-void build_csr(int V, int F, const int* faces, const Ws& W, bool sorted, cudaStream_t s) {
-    cudaMemsetAsync(W.deg, 0, 4 * (size_t)V, s);
-    if (F > 0) k_mesh_degree<<<blocks(F), kThreads, 0, s>>>(V, F, faces, W);
-    scan<Count>(W.deg, V, W.tiles, W.off, s);
-    cudaMemsetAsync(W.deg, 0, 4 * (size_t)V, s);
-    if (F > 0) k_dc_fill<<<blocks(F), kThreads, 0, s>>>(V, F, faces, W);
-    if (sorted && V > 0) k_dc_sort<<<blocks(V), kThreads, 0, s>>>(V, W);
-}
 
 // ---------------------------------------------------------------- locks and quadrics
 __device__ __forceinline__ bool follows(int3 t, int u, int v) {

@@ -1,13 +1,12 @@
-// Closest points on an indexed triangle mesh through the BVH of mesh_raycast.cu, angle-weighted pseudonormals, signed distances and
+// Closest points on an indexed triangle mesh through the BVH of mesh_bvh.cu, angle-weighted pseudonormals, signed distances and
 // area-weighted surface samples, sm_90a. Built with -fmad=false: the closest-point formula is rounded operation by operation as
 // include/psdf_b200.h states it, so oracle/mesh_distance.py (brute force over all faces) reproduces dist2, face and bary bit for bit.
 // The tree only prunes: a node is skipped when the fp32 distance to its padded box is strictly above the best squared distance so far,
-// and that bound never exceeds the computed distance of a face inside (see the header).
+// and that bound never exceeds the computed distance of a face inside (see the header). The pseudonormals sum over the vertex -> face
+// CSR of mesh_csr.cuh.
 //
-//   k_md_closest   dist2, face, bary of the nearest valid face, nearer child first, 64-entry stack   thread per point
+//   k_md_closest   dist2, face, bary of the nearest valid face, traverse of mesh_bvh.cuh             thread per point
 //   k_md_sign      sign of dot(p - q, pseudonormal of the closest feature) times sqrt(dist2)         thread per point
-//   k_md_fill      adj[off[v] + cursor] = f                                                          thread per face
-//   k_md_sort      heap sort of each vertex's face list (mesh_csr.cuh)                               thread per vertex
 //   k_md_face_n    unit face normal                                                                  thread per face
 //   k_md_vert_n    sum of angle * face normal over the vertex's faces, ascending                     thread per vertex
 //   k_md_edge_n    sum of the face normals of the faces holding both ends of a face edge, ascending  thread per (face, corner)
@@ -100,10 +99,10 @@ __device__ Closest closest_on_triangle(float3 p, float3 a, float3 b, float3 c) {
 
 // ---------------------------------------------------------------- traversal
 // squared fp32 distance from p to the box grown by pad: per axis max(lo - pad - p, p - (hi + pad), 0), summed as dot3
-__device__ __forceinline__ float box_d2(const float* b, float3 p, float pad) {
-    const float ex = fmaxf(fmaxf((b[0] - pad) - p.x, p.x - (b[3] + pad)), 0.0f);
-    const float ey = fmaxf(fmaxf((b[1] - pad) - p.y, p.y - (b[4] + pad)), 0.0f);
-    const float ez = fmaxf(fmaxf((b[2] - pad) - p.z, p.z - (b[5] + pad)), 0.0f);
+__device__ __forceinline__ float box_d2(const Box& b, float3 p, float pad) {
+    const float ex = fmaxf(fmaxf((b.lo.x - pad) - p.x, p.x - (b.hi.x + pad)), 0.0f);
+    const float ey = fmaxf(fmaxf((b.lo.y - pad) - p.y, p.y - (b.hi.y + pad)), 0.0f);
+    const float ez = fmaxf(fmaxf((b.lo.z - pad) - p.z, p.z - (b.hi.z + pad)), 0.0f);
     return (ex * ex + ey * ey) + ez * ez;
 }
 
@@ -125,50 +124,28 @@ __device__ __forceinline__ void visit_leaf(const Ws& W, const int* __restrict__ 
     best = Best{r.d2, f, r.b0, r.b1, r.b2};
 }
 
+// the nearest face (traverse): the key is the box bound, and a box is kept while its bound is not above the best dist2, so ties are visited
+struct Nearest {
+    const Ws& W;
+    const int* __restrict__ faces;
+    float3 p;
+    float pad;
+    Best best;
+    __device__ bool keep(float key) const { return key <= best.d2; }
+    __device__ bool enter(const Box& b, float& key) const {
+        key = box_d2(b, p, pad);
+        return keep(key);
+    }
+    __device__ bool visit(long long i) {
+        visit_leaf(W, faces, i, p, best);
+        return false;
+    }
+};
+
 __device__ Best nearest(const Ws& W, const int* __restrict__ faces, int F, float3 p, float pad) {
-    Best best{INFINITY, -1, 0.0f, 0.0f, 0.0f};
-    if (F == 0) return best;
-    if (F == 1) {
-        visit_leaf(W, faces, 0, p, best);
-        return best;
-    }
-    const int nl = F - 1;                                     // children at or above nl are leaves
-    int stack[kStack];
-    float dstack[kStack];
-    int sp = 0, node = 0;
-    while (true) {
-        const Node* nd = W.nodes + node;
-        const float4 a = __ldg(&nd->a), b = __ldg(&nd->b), c = __ldg(&nd->c);
-        const int4 ch = __ldg(&nd->d);
-        const float b0[6] = {a.x, a.y, a.z, a.w, b.x, b.y}, b1[6] = {b.z, b.w, c.x, c.y, c.z, c.w};
-        const float e0 = box_d2(b0, p, pad), e1 = box_d2(b1, p, pad);
-        const bool swap = e1 < e0;                            // the nearer child first; child 0 on a tie
-        const int n0 = swap ? ch.y : ch.x, n1 = swap ? ch.x : ch.y;
-        const float f0 = swap ? e1 : e0, f1 = swap ? e0 : e1;
-        bool h0 = f0 <= best.d2, h1 = f1 <= best.d2;
-        if (h0 && n0 >= nl) {
-            visit_leaf(W, faces, n0 - nl, p, best);
-            h0 = false;
-        }
-        h1 = h1 && f1 <= best.d2;
-        if (h1 && n1 >= nl) {
-            visit_leaf(W, faces, n1 - nl, p, best);
-            h1 = false;
-        }
-        if (h0 && h1) {
-            stack[sp] = n1;
-            dstack[sp++] = f1;
-            node = n0;
-        } else if (h0 || h1) {
-            node = h0 ? n0 : n1;
-        } else {
-            do {
-                if (sp == 0) return best;
-                --sp;
-            } while (dstack[sp] > best.d2);
-            node = stack[sp];
-        }
-    }
+    Nearest q{W, faces, p, pad, Best{INFINITY, -1, 0.0f, 0.0f, 0.0f}};
+    traverse(W, F, q);
+    return q.best;
 }
 
 __global__ void __launch_bounds__(kThreads) k_md_closest(int F, long long P, const float* __restrict__ points, const int* __restrict__ faces,
@@ -233,22 +210,6 @@ long long carve_pn(void* ws, long long V, long long F, PnWs* W) {
     s.take(w.tiles, 8 * tile_sums(V));
     if (W) *W = w;
     return s.size;
-}
-
-__global__ void __launch_bounds__(kThreads) k_md_fill(int V, int F, const int* __restrict__ faces, PnWs W) {
-    const long long f = thread_index();
-    if (f >= F) return;
-    const int3 t = load_face(faces, f);
-    if (!valid(t, V)) return;
-    W.adj[W.off[t.x] + atomicAdd(W.deg + t.x, 1)] = (int)f;
-    W.adj[W.off[t.y] + atomicAdd(W.deg + t.y, 1)] = (int)f;
-    W.adj[W.off[t.z] + atomicAdd(W.deg + t.z, 1)] = (int)f;
-}
-
-__global__ void __launch_bounds__(kThreads) k_md_sort(int V, PnWs W) {
-    const long long v = thread_index();
-    if (v >= V) return;
-    heap_sort(W.adj + W.off[v], W.off[v + 1] - W.off[v]);
 }
 
 __device__ __forceinline__ void store3(float* __restrict__ out, long long i, float3 v) {
@@ -377,18 +338,9 @@ int psdf_mesh_pseudonormals(int V, int F, const float* verts, const int* faces, 
     carve_pn(workspace, V, F, &W);
     cudaMemsetAsync(W.info, 0, kHeaderBytes, ST);
     if (F > 0) k_mesh_check<<<blocks(F), kThreads, 0, ST>>>(V, F, faces, W);
-    cudaMemsetAsync(W.deg, 0, 4 * (size_t)V, ST);
-    if (F > 0) k_mesh_degree<<<blocks(F), kThreads, 0, ST>>>(V, F, faces, W);
-    scan<Count>(W.deg, V, W.tiles, W.off, ST);
-    cudaMemsetAsync(W.deg, 0, 4 * (size_t)V, ST);
-    if (F > 0) {
-        k_md_fill<<<blocks(F), kThreads, 0, ST>>>(V, F, faces, W);
-        k_md_face_n<<<blocks(F), kThreads, 0, ST>>>(V, F, verts, faces, face_n);
-    }
-    if (V > 0) {
-        k_md_sort<<<blocks(V), kThreads, 0, ST>>>(V, W);
-        k_md_vert_n<<<blocks(V), kThreads, 0, ST>>>(V, verts, faces, face_n, W, vert_n);
-    }
+    build_csr(V, F, faces, W, true, ST);
+    if (F > 0) k_md_face_n<<<blocks(F), kThreads, 0, ST>>>(V, F, verts, faces, face_n);
+    if (V > 0) k_md_vert_n<<<blocks(V), kThreads, 0, ST>>>(V, verts, faces, face_n, W, vert_n);
     if (F > 0) k_md_edge_n<<<blocks(3LL * F), kThreads, 0, ST>>>(V, F, faces, face_n, W, edge_n);
     PSDF_CHECK_LAUNCH();
     return PSDF_OK;

@@ -1,9 +1,9 @@
-// Generalized winding numbers of an indexed triangle mesh (Jacobson et al. 2013) through the BVH of mesh_raycast.cu, with the
+// Generalized winding numbers of an indexed triangle mesh (Jacobson et al. 2013) through the BVH of mesh_bvh.cu, with the
 // hierarchical far field of Barill et al. 2018 for triangle soups, sm_90a. Built with -fmad=false: each face's solid angle is rounded
 // operation by operation as include/psdf_b200.h states it. w(p) = (1/4 pi) sum over faces of the signed solid angle of the face seen from
 // p; oracle/winding.py sums the same faces in fp64, so at beta = +inf (no far field) the only difference is the rounding of each term.
 //
-// Build (psdf_mesh_winding_build): bottom-up over the existing tree, as k_rc_leaves refits its boxes. Each internal node gets its
+// Build (psdf_mesh_winding_build): bottom-up over the existing tree, climb of mesh_bvh.cuh as the box refit. Each internal node gets its
 // area-weighted centroid c (fp32), the radius r of the sphere about c holding its box, and the moments of its faces about c up to order
 // 2: sum A n, sum int (x - c) n^T dA and 1/2 sum int (x - c)(x - c)^T n dA (symmetric in the first two indices, 6 pairs x 3). A leaf's
 // moments are integrated exactly; a node's are its children's, child 0 then child 1, shifted to its own c, all in fp64 and stored in
@@ -147,23 +147,20 @@ __device__ __forceinline__ void child_shape(const Ws& W, const WnWs& M, int ch, 
     }
 }
 
+// nothing is published before an arrival: the second child combines both children's records and writes its node's
 __global__ void __launch_bounds__(kThreads) k_wn_build(int F, Ws W, WnWs M) {
     const long long i = thread_index();
     if (i >= F) return;
     const int nl = F - 1;
-    long long node = (long long)nl + i;
-    while (node != 0) {                                       // the root is internal node 0 (a single leaf when F = 1)
-        const int p = W.parent[node] >> 1;
-        __threadfence();                                      // this node's moments before its arrival
-        if (atomicAdd(M.flags + p, 1) == 0) return;           // the other child is not done yet; it goes on
-        const int4 ch = __ldg(&W.nodes[p].d);
+    climb(W, F, i, M.flags, [](int, int) {}, [&](int p) {
+        const NodeView nd = load_node(W, p);
         double a0, a1;
         double3 c0, c1;
-        child_shape(W, M, ch.x, nl, a0, c0);
-        child_shape(W, M, ch.y, nl, a1, c1);
-        const float4 ba = __ldg(&W.nodes[p].a), bb = __ldg(&W.nodes[p].b), bc = __ldg(&W.nodes[p].c);
-        const double lo[3] = {fminf(ba.x, bb.z), fminf(ba.y, bb.w), fminf(ba.z, bc.x)};
-        const double hi[3] = {fmaxf(ba.w, bc.y), fmaxf(bb.x, bc.z), fmaxf(bb.y, bc.w)};
+        child_shape(W, M, nd.child[0], nl, a0, c0);
+        child_shape(W, M, nd.child[1], nl, a1, c1);
+        const Box &b0 = nd.box[0], &b1 = nd.box[1];
+        const double lo[3] = {fminf(b0.lo.x, b1.lo.x), fminf(b0.lo.y, b1.lo.y), fminf(b0.lo.z, b1.lo.z)};
+        const double hi[3] = {fmaxf(b0.hi.x, b1.hi.x), fmaxf(b0.hi.y, b1.hi.y), fmaxf(b0.hi.z, b1.hi.z)};
         const double area = a0 + a1;
         double cd[3];
         #pragma unroll
@@ -178,10 +175,11 @@ __global__ void __launch_bounds__(kThreads) k_wn_build(int F, Ws W, WnWs M) {
             r2 += e * e;
         }
         Moments m{};
-        if (ch.x >= nl) add_leaf(W, ch.x - nl, c, m);
-        else add_node(M.mom + (long long)kSlots * ch.x, c, m);
-        if (ch.y >= nl) add_leaf(W, ch.y - nl, c, m);
-        else add_node(M.mom + (long long)kSlots * ch.y, c, m);
+        for (int s = 0; s < 2; s++) {
+            const int ch = nd.child[s];
+            if (ch >= nl) add_leaf(W, ch - nl, c, m);
+            else add_node(M.mom + (long long)kSlots * ch, c, m);
+        }
         float4* q = M.mom + (long long)kSlots * p;
         q[0] = make_float4(cf.x, cf.y, cf.z, __double2float_ru(sqrt(r2)));
         q[1] = make_float4((float)m.m0[0], (float)m.m0[1], (float)m.m0[2], (float)area);
@@ -192,8 +190,7 @@ __global__ void __launch_bounds__(kThreads) k_wn_build(int F, Ws W, WnWs M) {
         x[27] = 0.0f;
         #pragma unroll
         for (int k = 0; k < 7; k++) q[2 + k] = make_float4(x[4 * k], x[4 * k + 1], x[4 * k + 2], x[4 * k + 3]);
-        node = p;
-    }
+    });
 }
 
 // ---------------------------------------------------------------- query

@@ -50,15 +50,16 @@ def _check_sizes(fn, nv, nf):
         raise RuntimeError("%s: %d vertices and %d faces; both must be below 2^31" % (fn, nv, nf))
 
 
-def _checked_call(fn, workspace_bytes, entry, nv, nf, args, out=()):
+def _checked_call(fn, workspace_bytes, entry, nv, nf, args, out=(), repeats_allowed=False):
     """entry(nv, nf, *args, workspace, *out) on a new workspace of workspace_bytes(nv, nf) bytes on the device of args[-1]; raises on the
-    faces with an index outside [0, nv) or a repeated vertex that it counted into info[0], info[1] -> (workspace, info[2])"""
+    faces with an index outside [0, nv) that it counted into info[0], and unless repeats_allowed on those with a repeated vertex that it
+    counted into info[1] -> (workspace, info[2])"""
     ws = torch.empty(int(workspace_bytes(nv, nf)), dtype=torch.uint8, device=args[-1].device)
     call(entry, nv, nf, *args, ws, *out)
     bad, rep, info2 = ws[:24].view(torch.int64).tolist()
     if bad:
         raise RuntimeError("%s: %d faces have a vertex index outside [0, %d)" % (fn, bad, nv))
-    if rep:
+    if rep and not repeats_allowed:
         raise RuntimeError("%s: %d faces repeat a vertex" % (fn, rep))
     return ws, info2
 
@@ -323,12 +324,8 @@ class Mesh:
     def _bvh(self, fn):
         """the BVH of the faces (psdf_mesh_bvh_build) -> (V, F, workspace); raises on faces with an index outside [0, V)"""
         V, Fc = self._check_vf(fn)
-        nv, nf = V.shape[0], Fc.shape[0]
-        ws = torch.empty(int(load_library().psdf_mesh_bvh_workspace_bytes(nv, nf)), dtype=torch.uint8, device=V.device)
-        call("psdf_mesh_bvh_build", nv, nf, V, Fc, ws)
-        bad = int(ws[:8].view(torch.int64).item())
-        if bad:
-            raise RuntimeError("%s: %d faces have a vertex index outside [0, %d)" % (fn, bad, nv))
+        ws, _ = _checked_call(fn, load_library().psdf_mesh_bvh_workspace_bytes, "psdf_mesh_bvh_build", V.shape[0], Fc.shape[0], (V, Fc),
+                              repeats_allowed=True)
         return V, Fc, ws
 
     def occluded(self, origins, dirs, tnear=1e-4, tfar=math.inf):
@@ -469,11 +466,8 @@ class Mesh:
             face_n = torch.empty(nf, 3, dtype=torch.float32, device=V.device)
             vert_n = torch.empty(nv, 3, dtype=torch.float32, device=V.device)
             edge_n = torch.empty(nf, 3, 3, dtype=torch.float32, device=V.device)
-            ws = torch.empty(int(load_library().psdf_mesh_pseudonormals_workspace_bytes(nv, nf)), dtype=torch.uint8, device=V.device)
-            call("psdf_mesh_pseudonormals", nv, nf, V, Fc, ws, face_n, vert_n, edge_n)
-            bad = int(ws[:8].view(torch.int64).item())
-        if bad:
-            raise RuntimeError("%s: %d faces have a vertex index outside [0, %d)" % (fn, bad, nv))
+            _checked_call(fn, load_library().psdf_mesh_pseudonormals_workspace_bytes, "psdf_mesh_pseudonormals", nv, nf, (V, Fc),
+                          (face_n, vert_n, edge_n), repeats_allowed=True)
         return face_n, vert_n, edge_n
 
     def signed_distance(self, points, sign="pseudonormal"):

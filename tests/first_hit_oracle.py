@@ -1,34 +1,13 @@
 """The first-hit answer of psdf_mesh_first_hit and the per-pixel shading of psdf_mesh_render, by brute force in numpy fp32 (test
-infrastructure): the ray-triangle test of include/psdf_b200.h (oracle/raycast.py's, each operation rounded as written) restated to also
-return its t, u and v, tested against every triangle. csrc/mesh_raycast.cu gives the same answers through its BVH."""
+infrastructure): the ray-triangle test of include/psdf_b200.h (oracle/raycast.py's intersect, each operation rounded as written, with its
+t, u and v) against every triangle. csrc/mesh_raycast.cu gives the same answers through its BVH."""
 import math
 
 import numpy as np
 
-from oracle.raycast import cross, dot
+from oracle.raycast import cross, dot, intersect
 
 f32 = np.float32
-
-
-def intersect(p0, p1, p2, o, d, tnear, tfar):
-    """the test of every pair of triangles (p0, p1, p2 [..., 3]) and rays (o, d [..., 3]), broadcast -> (pass bool [...], t, u, v float32
-    [...]); t, u and v are meaningful where the test passes"""
-    p0, p1, p2, o, d = (np.asarray(x, f32) for x in (p0, p1, p2, o, d))
-    tnear, tfar = f32(tnear), f32(tfar)
-    with np.errstate(all="ignore"):
-        e1, e2 = p1 - p0, p2 - p0
-        pv = cross(d, e2)
-        det = dot(e1, pv)
-        ok = (det != 0) & ~np.isnan(det)
-        inv = f32(1) / det
-        tv = o - p0
-        u = dot(tv, pv) * inv
-        ok &= (u >= 0) & (u <= 1)
-        qv = cross(tv, e1)
-        v = dot(d, qv) * inv
-        ok &= (v >= 0) & (u + v <= 1)
-        t = dot(e2, qv) * inv
-        return ok & (t > tnear) & (t < tfar), t, u, v
 
 
 def first_hit(V, F, origins, dirs, tnear=0.0, tfar=math.inf, chunk=1 << 22):

@@ -21,7 +21,8 @@ NVCC = shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
 ENTRY_POINTS = ("psdf_mesh_decimate_workspace_bytes", "psdf_mesh_normals_workspace_bytes", "psdf_mesh_decimate_begin",
                 "psdf_mesh_decimate_round", "psdf_mesh_normals")
 KERNELS = ("k_mesh_check<Ws>", "k_mesh_degree<Ws>", "k_mesh_scan_tiles<Count, int>", "k_mesh_scan_tiles<Kept, unsigned char>",
-           "k_mesh_scan_top", "k_mesh_scan_out<Count, int>", "k_mesh_scan_out<Kept, unsigned char>", "k_dc_fill", "k_dc_sort", "k_dc_lock",
+           "k_mesh_scan_top", "k_mesh_scan_out<Count, int>", "k_mesh_scan_out<Kept, unsigned char>", "k_mesh_fill<Ws>", "k_mesh_sort<Ws>",
+           "k_dc_lock",
            "k_dc_quadric", "k_dc_key", "k_dc_best2", "k_dc_choose", "k_dc_select", "k_dc_apply", "k_dc_compact", "k_dc_copy", "k_dc_normals")
 
 
@@ -129,7 +130,7 @@ def kernels():
     return {r["kernel"]: r for r in wgmma_report.report(("mesh_decimate.cu",))}
 
 
-def test_kernels_are_built_and_do_not_spill(kernels):
+def test_kernels_and_the_shared_csr_fill_are_built_and_do_not_spill(kernels):
     dc = {k: r for k, r in kernels.items() if k.startswith(("k_dc_", "k_mesh_"))}
     assert set(dc) == set(KERNELS)
     spilling = {k: (r["spill_st"], r["spill_ld"]) for k, r in dc.items() if r["spill_st"] or r["spill_ld"]}

@@ -1,5 +1,5 @@
 """Mesh distances without a GPU: the C ABI's entry points, workspace sizes and argument errors, a compile check that the kernels of
-csrc/mesh_distance.cu exist and do not spill, and the closest-point formula, pseudonormals and samples of oracle/mesh_distance.py on cases
+csrc/mesh_distance.cu (its own and those of csrc/mesh_csr.cuh it launches) exist and do not spill, and the closest-point formula, pseudonormals and samples of oracle/mesh_distance.py on cases
 worked by hand."""
 import ctypes
 import math
@@ -20,7 +20,7 @@ NVCC = shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
 ENTRY_POINTS = ("psdf_mesh_closest_points", "psdf_mesh_pseudonormals_workspace_bytes", "psdf_mesh_pseudonormals",
                 "psdf_mesh_signed_distance", "psdf_mesh_sample_surface")
 KERNELS = ("k_mesh_check<PnWs>", "k_mesh_degree<PnWs>", "k_mesh_scan_tiles<Count, int>", "k_mesh_scan_top", "k_mesh_scan_out<Count, int>",
-           "k_md_closest", "k_md_sign", "k_md_fill", "k_md_sort", "k_md_face_n", "k_md_vert_n", "k_md_edge_n", "k_md_sample")
+           "k_mesh_fill<PnWs>", "k_mesh_sort<PnWs>", "k_md_closest", "k_md_sign", "k_md_face_n", "k_md_vert_n", "k_md_edge_n", "k_md_sample")
 
 
 # ------------------------------------------------------------------------------------------------ C ABI
@@ -103,7 +103,7 @@ def kernels():
     return {r["kernel"]: r for r in wgmma_report.report(("mesh_distance.cu",))}
 
 
-def test_kernels_are_built_and_do_not_spill(kernels):
+def test_kernels_and_the_shared_csr_fill_are_built_and_do_not_spill(kernels):
     md = {k: r for k, r in kernels.items() if k.startswith(("k_md_", "k_mesh_"))}
     assert set(md) == set(KERNELS)
     spilling = {k: (r["spill_st"], r["spill_ld"]) for k, r in md.items() if r["spill_st"] or r["spill_ld"]}

@@ -1,6 +1,6 @@
-"""Mesh ray casting without a GPU: the C ABI's entry points, workspace sizes and argument errors, a compile check that the kernels of
-csrc/mesh_raycast.cu (its own and those of csrc/mesh_csr.cuh it launches) exist and do not spill, the ray-triangle test of oracle/raycast.py
-on cases worked by hand, and the file selection of load_mesh_sequence."""
+"""Mesh ray casting without a GPU: the C ABI's entry points, workspace sizes and argument errors, a compile check that the BVH build
+kernels of csrc/mesh_bvh.cu (its own and those of csrc/mesh_csr.cuh it launches) and the any-hit kernels of csrc/mesh_raycast.cu exist and
+do not spill, the ray-triangle test of oracle/raycast.py on cases worked by hand, and the file selection of load_mesh_sequence."""
 import ctypes
 import math
 import os
@@ -18,8 +18,10 @@ from permuto_sdf_b200.mesh import Mesh, fibonacci_directions, natural_key, seque
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 NVCC = shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
 ENTRY_POINTS = ("psdf_mesh_bvh_workspace_bytes", "psdf_mesh_bvh_build", "psdf_mesh_occluded", "psdf_mesh_ambient_occlusion")
-KERNELS = ("k_mesh_check<Ws>", "k_mesh_scan_tiles<Count, int>", "k_mesh_scan_top", "k_mesh_scan_out<Count, int>", "k_rc_bounds",
-           "k_rc_morton", "k_rc_hist", "k_rc_scatter", "k_rc_internal", "k_rc_leaves", "k_rc_occluded", "k_rc_ao", "k_rc_vis")
+# the build, compiled from csrc/mesh_bvh.cu, and the any-hit queries, compiled from csrc/mesh_raycast.cu
+BUILD_KERNELS = ("k_mesh_check<Ws>", "k_mesh_scan_tiles<Count, int>", "k_mesh_scan_top", "k_mesh_scan_out<Count, int>", "k_bvh_bounds",
+                 "k_bvh_morton", "k_bvh_hist", "k_bvh_scatter", "k_bvh_internal", "k_bvh_leaves")
+QUERY_KERNELS = ("k_rc_occluded", "k_rc_ao", "k_rc_vis")
 
 
 # ------------------------------------------------------------------------------------------------ C ABI
@@ -93,14 +95,17 @@ def kernels():
         pytest.skip("nvcc not available")
     sys.path.insert(0, os.path.join(ROOT, "tools"))
     import wgmma_report
-    return {r["kernel"]: r for r in wgmma_report.report(("mesh_raycast.cu",))}
+    return {(r["unit"], r["kernel"]): r for r in wgmma_report.report(("mesh_bvh.cu", "mesh_raycast.cu"))}
 
 
-def test_kernels_are_built_and_do_not_spill(kernels):
-    rc = {k: r for k, r in kernels.items() if k.startswith(("k_rc_", "k_mesh_"))}
-    assert set(rc) == set(KERNELS)
-    spilling = {k: (r["spill_st"], r["spill_ld"]) for k, r in rc.items() if r["spill_st"] or r["spill_ld"]}
-    assert not spilling, spilling
+def test_build_and_query_kernels_are_built_and_do_not_spill(kernels):
+    units = {"mesh_bvh.cu": (("k_bvh_", "k_rc_", "k_mesh_"), BUILD_KERNELS),
+             "mesh_raycast.cu": (("k_bvh_", "k_rc_"), QUERY_KERNELS)}       # it also emits mesh_csr.cuh's k_mesh_scan_top, never launched
+    for unit, (prefixes, expected) in units.items():
+        rc = {k: r for (u, k), r in kernels.items() if u == unit and k.startswith(prefixes)}
+        assert set(rc) == set(expected), unit
+        spilling = {k: (r["spill_st"], r["spill_ld"]) for k, r in rc.items() if r["spill_st"] or r["spill_ld"]}
+        assert not spilling, (unit, spilling)
 
 
 # ------------------------------------------------------------------------------------------------ the oracle's test by hand
